@@ -6,10 +6,12 @@ snapshot epoch (SURVEY.md §8d).  Reported on one JSON line:
   value     decisions/s with the batch already resident in HBM (CUDA events around the scoring kernel, max over ranks)
   e2e       the same batch through mmp_place_batch with pinned HOST buffers (H2D + kernel + D2H inside the timed region)
   roofline  algorithmic bytes (1312 B/decision + 80 B/instance, SURVEY.md §8d) / measured kernel time vs the measured
-            HBM copy peak in MEASURED_PEAKS.json
+            HBM copy peak in MEASURED_PEAKS.json when present, else the H100 SXM data sheet's 3.35 TB/s
   cpu_baseline  the oracle (C++ restatement of the reference's Java path; the JVM cannot run here) on the host cores
-`--impl reference` times only that CPU path.  N > 1 (torchrun): the registry is sharded by model across ranks (each rank
-places its slice against a replicated instance table; no data-path collective), so total work is fixed: "strong".
+`--impl reference` times only that CPU path.  `--dump-outputs DIR` writes what the timed path returned in its last step as
+DIR/<name>.npy (float64), so that two builds can be compared output for output on the same seeded inputs.
+N > 1 (torchrun): the registry is sharded by model across ranks (each rank places its slice against a replicated instance
+table; no data-path collective), so total work is fixed: "strong".
 """
 from __future__ import annotations
 
@@ -42,7 +44,7 @@ def bytes_per_decision(row_words: int) -> int:
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu_index: int):
         super().__init__(daemon=True)
@@ -132,7 +134,7 @@ def measured_hbm_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy kernel)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 def scoring_kernel() -> str:
@@ -140,22 +142,6 @@ def scoring_kernel() -> str:
     MMP_KERNEL selects the streaming kernel (lanes) or the cooperative tiles (tile)."""
     k = os.environ.get("MMP_KERNEL", "direct")
     return {"lanes": "k_place_lanes", "tile": "k_place"}.get(k, "k_place_direct")
-
-
-def captured_traffic(batch: int):
-    """dram__bytes_read + dram__bytes_write of one launch of the scoring kernel from the committed `ncu --set full` capture of
-    this configuration (profiles/r02_ncu_<kernel>_<config>.json, written by tools/ncu_summary.py), scaled per decision when
-    the capture was taken on another batch size (the traffic is proportional to the number of decisions)."""
-    for name in (f"r02_ncu_{scoring_kernel()}_{CONFIG.lower()}.json",):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                d = json.load(f)
-            nd = int(d.get("n_decisions") or 0)
-            if nd > 0:
-                return float(d["dram_bytes_per_launch"]) * batch / nd, f"profiles/{name.replace('.json', '.txt')}"
-        except Exception:
-            pass
-    return None, None
 
 
 def build_oracle(fl):
@@ -202,10 +188,12 @@ def run_reference(args, rank: int, world: int):
     times, dense_times = [], []
     for step in range(args.warmup + args.steps):
         t0 = time.perf_counter()
-        oracle.get_next_batch(od, fl.type_names, off, idx, fl.now_ms, SEED, threads=threads)
+        res = oracle.get_next_batch(od, fl.type_names, off, idx, fl.now_ms, SEED, threads=threads)
         dt = time.perf_counter() - t0
         if step >= args.warmup:
             times.append(dt)
+    if args.dump_outputs:  # the same files as the GPU path's, from the same decisions
+        dump_outputs(args.dump_outputs, res, ("target", "n_candidates"))
     for step in range(min(3, args.steps)):
         t0 = time.perf_counter()
         oracle.get_next_batch(od, fl.type_names, off, idx, fl.now_ms, SEED, threads=threads, dense=True)
@@ -282,9 +270,11 @@ def run_reference_churn(args):
         ev = w.events(ep, CHURN_EVENTS, SEED)
         now0 = fl.now_ms + ep * w.window_ms
         t0 = time.perf_counter()
-        sim.step(ev, now0, now0 + w.window_ms, 400 + ep)
+        dec, evi, rows, _, _ = sim.step(ev, now0, now0 + w.window_ms, 400 + ep)
         if ep >= args.warmup:
             times.append(time.perf_counter() - t0)
+    if args.dump_outputs:
+        dump_churn_outputs(args.dump_outputs, dec, evi, rows)
     value = CHURN_EVENTS * len(times) / sum(times)
     print(json.dumps({
         "impl": "reference", "metric": CHURN_METRIC, "value": value, "unit": "events/s", "n_gpus": args.gpus, "steps": args.steps,
@@ -354,6 +344,8 @@ def run_churn(args, rank: int, world: int, local_rank: int):
             dev_ms.append(rep.ms_total); wall_ms.append(1000.0 * dt)
             phases.append([rep.ms_classify, rep.ms_place, rep.ms_route, rep.ms_apply, rep.ms_registry, rep.ms_commit])
             n_dec += len(dec); n_evict += len(evi); n_lru += rep.n_lru_events; n_pub += rep.n_published
+        if args.dump_outputs and ep == args.warmup + args.steps - 1:
+            dump_churn_outputs(args.dump_outputs, dec, evi, rows)
     clocks = sampler.finish()
     launches = s.kernel_launches() - launches0
     ph = np.asarray(phases)
@@ -416,6 +408,20 @@ def run_churn(args, rank: int, world: int, local_rank: int):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir: str, rec: np.ndarray, fields, prefix: str = ""):
+    """Each field of a result record array as out_dir/<prefix><field>.npy in float64 (exact for these integers: all < 2**53)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for k in fields:
+        np.save(os.path.join(out_dir, f"{prefix}{k}.npy"), np.ascontiguousarray(rec[k], dtype=np.float64))
+
+
+def dump_churn_outputs(out_dir: str, dec: np.ndarray, evi: np.ndarray, rows: np.ndarray):
+    """One closed-loop window's decisions, evictions in listener order and republished instance rows."""
+    dump_outputs(out_dir, dec, ("model", "self", "target", "n_candidates", "status", "event"), prefix="decisions_")
+    dump_outputs(out_dir, evi, ("instance", "model", "last_used", "weight", "order", "reload"), prefix="evictions_")
+    dump_outputs(out_dir, rows, ("lru_time", "used", "count", "capacity"), prefix="rows_")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -425,6 +431,7 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-instance-shards", action="store_true", help="N > 1: skip the instance-sharded leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's results to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank = int(os.environ.get("RANK", 0))
@@ -497,6 +504,8 @@ def main():
     dev_ms = float(np.sum(kernel_ms))
     out_dev = np.zeros(B, dtype=DECISION_OUT)
     solver._ck(lib.mmp_device_download(solver.h, out_dev.ctypes.data_as(C.c_void_p), d_out, out_dev.nbytes))
+    if args.dump_outputs:  # this rank's slice of the sweep: 16 B per decision, 16 MB at 1 M decisions
+        dump_outputs(args.dump_outputs, out_dev, ("target", "n_candidates"), prefix=f"rank{rank}_" if world > 1 else "")
 
     # ---- end to end through the C ABI with pinned host buffers ----
     e2e_ms = []
@@ -699,14 +708,11 @@ def main():
         alg_bytes = B * bytes_per_decision(row_words) + 80 * fl.n_instances
         k_avg_s = float(np.mean(kernel_ms)) / 1000.0
         achieved = alg_bytes / k_avg_s / 1e9
-        traffic, traffic_src = captured_traffic(B)
         roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "traffic": traffic, "peak_source": peak_src, "kernel": scoring_kernel(),
-                    "traffic_GBps": (traffic / k_avg_s / 1e9) if traffic else None,
+                    "peak_source": peak_src, "kernel": scoring_kernel(),
                     "note": ("achieved = ALGORITHMIC bytes (whole bitmap row + model row + result per decision, SURVEY.md 8d) / kernel time. "
-                             "k_place_direct reads only the row words a decision looks at, so its DRAM traffic (`traffic`, ncu) is far below "
-                             "the algorithmic bytes and `frac` can exceed 1; traffic_GBps = traffic / kernel time is the physical HBM rate"),
-                    "traffic_source": (traffic_src + " (ncu --set full, one launch; scaled per decision to this batch)") if traffic_src else None,
+                             "k_place_direct reads only the row words a decision looks at, so its DRAM traffic is far below "
+                             "the algorithmic bytes and `frac` can exceed 1"),
                     "algorithmic_bytes_per_launch": int(alg_bytes), "kernel_ms_avg": 1000.0 * k_avg_s}
         cpu = None
         if not args.no_cpu:

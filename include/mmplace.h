@@ -1,5 +1,5 @@
 /*
- * mmplace.h — C ABI of libmmplace: a B200-native (sm_100a CUDA) placement / LRU-eviction solver that drops in
+ * mmplace.h — C ABI of libmmplace: an H100-native (sm_90a CUDA) placement / LRU-eviction solver that drops in
  * behind ModelMesh's decision API.  Plain pointers and sizes only; no CUDA/torch types.  This is the boundary a
  * JNI shim binds (see INTEGRATION.md for the Java side).  Reference = kserve/modelmesh @ ea13cdc5;
  * MM = src/main/java/com/ibm/watson/modelmesh/ModelMesh.java, IR = InstanceRecord.java, MR = ModelRecord.java,

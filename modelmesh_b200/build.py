@@ -1,4 +1,4 @@
-"""Build libmmplace.so in-tree with nvcc for sm_100a (B200).  `python -m modelmesh_b200.build`."""
+"""Build libmmplace.so in-tree with nvcc for sm_90a (H100).  `python -m modelmesh_b200.build`."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,8 @@ CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(CSRC, "libmmplace.so")
 SOURCES = ["mmplace.cu"]
 DEPS = ["mmplace.cu", "place_core.cuh", "host_state.hpp", "scan_kernels.cuh", "commit_kernels.cuh", "churn_kernels.cuh",
-        "registry_kernels.cuh", os.path.join("..", "..", "include", "mmplace.h")]
+        "registry_kernels.cuh", os.path.join("..", "..", "include", "mmplace.h"),
+        os.path.join("..", "build.py")]  # the compiler flags below: a library built with other flags is rebuilt
 
 
 def nvcc_path() -> str:
@@ -31,7 +32,7 @@ def up_to_date() -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and up_to_date():
         return SO
-    cmd = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "-Xcompiler", "-fPIC", "-Xlinker", "-Bsymbolic", "-shared", "-ldl", "-o", SO] + [os.path.join(CSRC, s) for s in SOURCES]
     if verbose:
         cmd.insert(1, "-Xptxas")

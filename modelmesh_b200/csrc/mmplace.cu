@@ -1,4 +1,4 @@
-// mmplace.cu — libmmplace: the sm_100a CUDA implementation behind include/mmplace.h.
+// mmplace.cu — libmmplace: the sm_90a CUDA implementation behind include/mmplace.h.
 //
 // Data layout in HBM (DESIGN.md §4), per snapshot epoch (double-buffered, flipped atomically at commit):
 //   excl      [n_models][row_words] u32   model x instance exclusion bitmap (loaded ∪ failed, MR:69,73), bit = RANK of
@@ -1157,7 +1157,7 @@ struct PlaceCtx {
 struct mmp_fleet {
   HostState hs;
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;           // (H100 SXM; replaced by the device's own count in mmp_fleet_create)
   std::mutex ingest_mu;         // single-writer ingest, but do not corrupt state if violated
   std::shared_mutex snap_mu;    // readers: place/stats; writer: the epoch flip in commit
   DeviceSnapshot snaps[2];
@@ -1201,9 +1201,8 @@ struct mmp_fleet {
   std::atomic<int64_t> launches{0};
   int tile = 16;                // lanes per decision in k_place (MMP_TILE = 8 | 16 | 32)
   int ring_k = 4;               // ring depth for rows <= 2 KiB (MMP_RING_K = 2 | 4)
-  int lane_stages = 4;          // MMP_LANE_STAGES caps the landing stages per SM (0: as many as fit).  Measured on B200 at 10k
-                                // instances: 3 stages 3.5, 4 stages 4.1-4.3, 5 stages 3.8 G decisions/s (the fifth stage costs the L1
-                                // its 196 -> 228 KB carve-out step and the lane tables no longer stay resident)
+  int lane_stages = 4;          // MMP_LANE_STAGES caps the landing stages per SM (0: as many as fit).  A fifth stage takes the
+                                // shared-memory carve-out from 196 to 228 KB and leaves too little L1 for the lane tables to stay resident
   int shard_chunks = 1;         // MMP_SHARD_CHUNKS (see place_sharded)
   int one_mode = 3;             // MMP_ONE = lanes | small | graph | server: how tiny batches are launched (0: the streaming kernel, 1: k_place_small
                                 // as a stream launch, 2: k_place_small as a replayed CUDA graph, 3: a request to the resident k_place_server)
@@ -1395,8 +1394,6 @@ static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
   // production path: one decision per lane (any row width of which at least two 32-row landing stages fit: ~3 KiB rows)
   if (!(a.tr || a.cand) && f->lanes) {
     int ns = 0;
-    // warps per block: 12 per SM measured best at 10k instances (8: 3.7-3.8, 12: 4.1-4.3, 16: 3.6-3.9 G decisions/s); picking
-    // the width with the fewest rounds of steps for small launches was measured too and made no difference
     const int lw = f->lane_warps ? f->lane_warps : 12;
     if (lw == 8 && lanes_geometry(a.s.excl_stride, 8, ns)) return launch_place_lanes<8>(f, a, st, ns);
     if (lw == 10 && lanes_geometry(a.s.excl_stride, 10, ns)) return launch_place_lanes<10>(f, a, st, ns);
@@ -1502,8 +1499,8 @@ static int32_t place_sharded(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds
   CK(cudaMemsetAsync(c->d_n_open.p, 0, sizeof(int), st));
   // 1-3. per-shard keys (the scoring kernel), the min-loc combine over NVLink, keys -> results.  MMP_SHARD_CHUNKS = 2..4
   // splits a large batch so that the all-reduce and decode of chunk k run on a second stream while the scoring kernel
-  // works on chunk k + 1; measured on 2 x B200 at 1 M decisions it is SLOWER than one all-reduce (0.316 vs 0.267 ms per
-  // step: four short launches and four collectives cost more than the 8 MB exchange they hide), so the default is 1.
+  // works on chunk k + 1.  Four short launches and four collectives can cost more than the 8 MB exchange of a 1 M-decision
+  // batch they hide, so the default is 1.
   const int K = (n >= (1 << 18) && f->shard_chunks > 1) ? std::min(f->shard_chunks, (int)PlaceCtx::NSHARD_CHUNKS) : 1;
   const int32_t chunk = ((n + K - 1) / K + 31) / 32 * 32;
   cudaStream_t side = c->pipe[0];
@@ -2530,7 +2527,7 @@ int32_t mmp_host_free(mmp_fleet *f, void *p) { NEED(f); int32_t rc = set_device(
 int32_t mmp_flush_l2(mmp_fleet *f) {
   NEED(f);
   int32_t rc = set_device(f); if (rc < 0) return rc;
-  const size_t bytes = 256u << 20;  // > 126 MB L2
+  const size_t bytes = 128u << 20;  // > 2 x the 50 MB L2 of an H100
   CK(f->d_flush.ensure(bytes));
   CK(cudaMemsetAsync(f->d_flush.p, (int)(f->launches.load() & 0xff), bytes, 0));
   CK(cudaStreamSynchronize(0));

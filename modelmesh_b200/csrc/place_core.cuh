@@ -1,5 +1,5 @@
 // place_core.cuh — the placement decision in rank space, written once for two cooperative shapes:
-//   * Coop32: one 32-lane warp per decision on sm_100a.  The decision's exclusion-bitmap row has been staged in shared
+//   * Coop32: one 32-lane warp per decision on sm_90a.  The decision's exclusion-bitmap row has been staged in shared
 //     memory by a TMA bulk copy; the row is visited in windows of 32 consecutive words, one word per lane (1 024 ranks
 //     per step), reductions are REDUX / SHFL / VOTE.
 //   * Coop1: a single "lane", window = one word; compiled by g++ into the CPU-only test harness (tests/emul) so the
