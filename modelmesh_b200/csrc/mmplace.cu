@@ -3,6 +3,8 @@
 // Data layout in HBM (DESIGN.md §4), per snapshot epoch (double-buffered, flipped atomically at commit):
 //   excl      [n_models][row_words] u32   model x instance exclusion bitmap (loaded ∪ failed, MR:69,73), bit = RANK of
 //                                         the instance under PLACEMENT_ORDER; row stride is a multiple of 128 B
+//   excl_ranks [n_models] int4            the ranks of a model's <= 4 inline edges (-1: none), r[0] = -2: overflow ids,
+//                                         read the row (unsharded fleets)
 //   cand/pref [n_slots][row_words]  u32   per type-constraint slot: allowed ∧ active / preferred instances (TCM:242-251)
 //   candx     [n_slots][row_words]  u32   cand minus likely-replaced replicaset members (MM:4769-4770)
 //   full      [row_words]           u32   isFull instances (MM:4640)
@@ -12,7 +14,7 @@
 //   nzw/nz_n  [n_slots][row_words] u16    compressed word lists: the row words that hold any candidate of the slot (walks beyond the window)
 //   front     [n_models][16] u32          instance-sharded fleets: the first row words, replicated on every shard
 // Kernels (DESIGN.md §5, §7):
-//   k_place_direct<4, MINB>  the scoring kernel (default): one decision per lane, the row's window read straight from memory,
+//   k_place_direct<4, MINB>  the scoring kernel (default): one decision per lane, the row rebuilt from the model's excl_ranks,
 //                            longer walks through the word lists; optional slot-sorted batches (k_slot_keys + cub radix sort)
 //   k_place_lanes<WARPS>     round 1's streaming kernel (whole rows through TMA landing stages): MMP_KERNEL=lanes and the
 //                            collective instance-shard path
@@ -64,29 +66,35 @@ static thread_local std::string g_err;
 // ---------------------------------------------------------------------------------------------------------------
 // One thread per model scatters its (<= 4) inline edges into its own bitmap row: no atomics needed.
 // (instance-sharded: a stored row holds row words [word_lo, word_hi) at a stride of `stride` words)
+// ranks (optional, SnapshotView::excl_ranks): the rank of every bit set here, -1 for an edge that sets none.
 __global__ void k_build_bitmap(uint32_t *__restrict__ excl, const int4 *__restrict__ edge_inl,
-                               const int32_t *__restrict__ rank_of, int n_models, int stride, int word_lo, int word_hi) {
+                               const int32_t *__restrict__ rank_of, int n_models, int stride, int word_lo, int word_hi,
+                               int4 *__restrict__ ranks) {
   int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= n_models) return;
   int4 e = edge_inl[m];
   uint32_t *row = excl + (size_t)m * stride;
   int es[4] = {e.x, e.y, e.z, e.w};
+  int rs[4] = {-1, -1, -1, -1};
 #pragma unroll
   for (int i = 0; i < 4; i++) {
     if (es[i] >= 0) {
       int r = rank_of[es[i]];
-      if (r >= 0 && (r >> 5) >= word_lo && (r >> 5) < word_hi) row[(r >> 5) - word_lo] |= 1u << (r & 31);
+      if (r >= 0 && (r >> 5) >= word_lo && (r >> 5) < word_hi) { row[(r >> 5) - word_lo] |= 1u << (r & 31); rs[i] = r; }
     }
   }
+  if (ranks) ranks[m] = make_int4(rs[0], rs[1], rs[2], rs[3]);
 }
+// (launched after k_build_bitmap: a model with overflow pairs gets the EXCL_RANKS_OVF marker in its rank entry)
 __global__ void k_build_bitmap_ovf(uint32_t *__restrict__ excl, const int2 *__restrict__ pairs, int n_pairs,
-                                   const int32_t *__restrict__ rank_of, int stride, int word_lo, int word_hi) {
+                                   const int32_t *__restrict__ rank_of, int stride, int word_lo, int word_hi, int4 *__restrict__ ranks) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pairs) return;
   int2 p = pairs[i];
   int r = rank_of[p.y];
   if (r >= 0 && (r >> 5) >= word_lo && (r >> 5) < word_hi)
     atomicOr(&excl[(size_t)p.x * stride + ((r >> 5) - word_lo)], 1u << (r & 31));
+  if (ranks) ranks[p.x].x = EXCL_RANKS_OVF;
 }
 
 // ---- TMA 1-D bulk copy + mbarrier helpers (cp.async.bulk: SASS UBLKCP) ----
@@ -625,12 +633,14 @@ __global__ void __launch_bounds__(32) k_place_small(const SnapshotView s_arg, co
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// k_place_direct -- one decision per lane WITHOUT landing stages: a lane reads the first MMP_LANE_WIN words of its
-// decision's exclusion row straight from global memory (three 16-byte loads: two 32-byte sectors of the row) into its
-// warp's window buffer, and whatever a walk needs beyond them word by word through the compressed list (decide_stream's
-// second loop).  A decision costs the sectors it looks at (~170 B at 10 k instances: record, model row, window, self's
-// word, result) instead of the whole 1 280-byte row, and without the 41 KB stages an SM holds 16-32 warps instead of 12.
-// One warp per batch of 32 decisions, no per-warp software pipeline: the other resident warps hide the gathers.
+// k_place_direct -- one decision per lane WITHOUT landing stages and without reading the bitmap: a lane loads its
+// model's 16-byte entry of excl_ranks (the ranks of its <= 4 inline edges) and rebuilds from it, in registers, the first
+// MMP_LANE_WIN words of its exclusion row into its warp's window buffer, self's row word, and whatever word a walk needs
+// beyond the window (RowRanks in decide_stream's second loop).  A plain decision reads 80 B, all of it sequential in a
+// sweep: 32 B record, 24 B model row, 16 B ranks, 8 B result -- instead of scattered sectors of its 1 280-byte row.
+// A model with overflow ids (more than 4: rare) is marked in its entry and resolved from its row by the warp
+// (decide_warp).  Without the 41 KB stages an SM holds 16-32 warps instead of 12.  One warp per batch of 32 decisions,
+// no per-warp software pipeline: the other resident warps hide the gathers.
 // ---------------------------------------------------------------------------------------------------------------
 // how many type slots have fewer than `few` candidates among the first `win` row words (one thread per slot)
 __global__ void k_sparse_slots(const uint32_t *__restrict__ cx, int row_words, int n_slots, int word_lo, int win, int few, int *__restrict__ out) {
@@ -680,31 +690,32 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
     d.flags = (uint32_t)c.x; d.fresh = c.y; d.extra_off = c.z; d.extra_n = c.w;
   }
   const int m = (valid && d.model >= 0 && d.model < s.n_models) ? d.model : 0;
-  const uint32_t *row = s.excl + (size_t)m * RW;
-  // the window's loads go out first: they depend on the record only
-  const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
-  uint4 q[LANE_WIN / 4];
-#pragma unroll
-  for (int j = 0; j < LANE_WIN / 4; j++) {
-    q[j] = make_uint4(0u, 0u, 0u, 0u);
-    if (valid && (uint32_t)(j * 4) < win_words)
-      asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(q[j].x), "=r"(q[j].y), "=r"(q[j].z), "=r"(q[j].w) : "l"(row + j * 4));
-  }
+  // the model's excluded ranks go out first: they depend on the record only
+  RowRanks row;
+  row.r[0] = row.r[1] = row.r[2] = row.r[3] = -1;
+  if (valid) row = load_ranks(s.excl_ranks + (size_t)m * 4);
   DecisionCtx c;
   c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
   if (valid) prepare_ctx(s, d, fresh, n_fresh, extra, c);
-  uint32_t self_eword = 0;
-  if (valid && c.self_rank >= 0) self_eword = __ldg(row + (c.self_rank >> 5) - s.word_lo);
+  // a model with overflow ids is resolved from its bitmap row by the warp (decide_warp)
+  const bool ovf = valid && row.overflow();
+  const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
+  const uint32_t self_eword = c.self_rank >= 0 ? row.word((uint32_t)c.self_rank >> 5) : 0u;
   uint32_t *w = win_s[warp] + lane * LANE_STRIDE;
 #pragma unroll
-  for (int j = 0; j < LANE_WIN / 4; j++) { w[j * 4] = q[j].x; w[j * 4 + 1] = q[j].y; w[j * 4 + 2] = q[j].z; w[j * 4 + 3] = q[j].w; }
+  for (int j = 0; j < LANE_WIN; j++) w[j] = 0u;
+#pragma unroll
+  for (int j = 0; j < 4; j++) {  // (a negative rank is no word of the window)
+    const uint32_t wi = (uint32_t)row.r[j] >> 5;
+    if (wi < (uint32_t)LANE_WIN) w[wi] |= 1u << (row.r[j] & 31);
+  }
   __syncwarp();
   const LaneTables T = lane_tables_global(s, c.slot >= 0 ? ctx_slot(c) : 0);
   DecideOut o;
   const uint64_t my_id = pick_id(d, id_base + (uint64_t)i);
-  const bool handled = decide_stream(s, T, T, c, valid, w, win_words, RowPtr{row, (uint32_t)s.word_lo}, self_eword, now, seed, my_id, WarpVote(), o, budget,
+  const bool handled = decide_stream(s, T, T, c, valid && !ovf, w, win_words, row, self_eword, now, seed, my_id, WarpVote(), o, budget,
                                      chunk_s[warp] + lane * MMP_CHUNK_WORDS);
-  uint32_t pending = __ballot_sync(0xffffffffu, valid && !handled);
+  uint32_t pending = __ballot_sync(0xffffffffu, valid && (ovf || !handled));
   while (pending) {
     const int l = __ffs((int)pending) - 1;
     pending &= pending - 1;
@@ -1115,7 +1126,7 @@ struct DevBuf {
 #include "commit_kernels.cuh"
 
 struct DeviceSnapshot {
-  DevBuf excl, cand, candx, pref, has_pref, type_slot, full, rows, rank_of, csum, lsum, models;
+  DevBuf excl, excl_ranks, cand, candx, pref, has_pref, type_slot, full, rows, rank_of, csum, lsum, models;
   DevBuf cap_col, lthreads_col, linprog_col, part_of_rank, count_col, cand_before, nzw, nz_n;
   DevBuf front, nzw_full, nz_n_full;  // instance-sharded fleets: replicated first words of every row; word lists over the whole row
   SnapshotView view{};
@@ -1125,7 +1136,7 @@ struct DeviceSnapshot {
   bool host_stale = false;  // built on the device: the rank-space vectors of `host` are downloaded on first use (host_mirror)
   int32_t n_models = 0;
   void release() {
-    for (DevBuf *b : {&excl, &cand, &candx, &pref, &has_pref, &type_slot, &full, &rows, &rank_of, &csum, &lsum, &models,
+    for (DevBuf *b : {&excl, &excl_ranks, &cand, &candx, &pref, &has_pref, &type_slot, &full, &rows, &rank_of, &csum, &lsum, &models,
                       &cap_col, &lthreads_col, &linprog_col, &part_of_rank, &count_col, &cand_before, &nzw, &nz_n, &front, &nzw_full, &nz_n_full})
       b->release();
   }
@@ -1359,8 +1370,9 @@ static cudaError_t launch_place_lanes(mmp_fleet *f, const PlaceArgs &a, cudaStre
 
 static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st) {
   const int rw = a.s.row_words;
-  // the direct kernel: rows are read straight from memory, only the words a decision looks at (MMP_KERNEL=direct | lanes)
-  if (!(a.tr || a.cand) && !a.emit_keys && !a.orig_id && f->direct && a.n > f->small_max && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words) {
+  // the direct kernel: rows rebuilt from the snapshot's excl_ranks (whole-row fleets), no landing stages (MMP_KERNEL=direct | lanes)
+  if (!(a.tr || a.cand) && !a.emit_keys && !a.orig_id && f->direct && a.n > f->small_max && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words &&
+      a.s.excl_ranks) {
     const int blocks = (a.n + 127) / 128;
     const int32_t *perm = a.perm;
     if (!perm && a.ctx && a.n >= 8192 && (f->sort_slots == 1 || (f->sort_slots == 2 && f->snaps[f->cur].sparse_slots))) {
@@ -1551,7 +1563,7 @@ static int32_t place_sharded(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds
   CK(cudaGetLastError());
   f->launches += 2;
   SnapshotView whole = vw;
-  whole.excl = c->d_rows.as<uint32_t>();
+  whole.excl = c->d_rows.as<uint32_t>(); whole.excl_ranks = nullptr;
   whole.excl_stride = NW; whole.word_lo = 0; whole.word_hi = NW;
   if (G > 1) { whole.nzw = ds.nzw_full.as<uint16_t>(); whole.nz_n = ds.nz_n_full.as<int32_t>(); }  // word lists over the whole row, not this shard's block
   PlaceArgs b{whole, c->d_in_open.as<mmp_decision_in>(), n_open, d_fresh, n_fresh, d_extra, c->d_out_open.as<mmp_decision_out>(),
@@ -2080,15 +2092,19 @@ static int32_t commit_locked(mmp_fleet *f) {
   // (instance-sharded: sized for max_models rows from the first commit on, so that the block keeps the address its peers mapped)
   CK(ds.excl.ensure(f->hs.cfg.shard_count > 1 ? std::max(mmp_fleet::Peers::IPC_MIN_BYTES, (size_t)std::max(nm, f->hs.cfg.max_models) * ST * 4)
                                               : (size_t)std::max(nm, 1) * ST * 4));
+  // the excluded ranks of every model beside its row (k_place_direct reads them instead of the row): whole rows only
+  const bool whole_rows = h.word_lo == 0 && h.word_hi == RW;
+  if (whole_rows) CK(ds.excl_ranks.ensure((size_t)std::max(nm, 1) * 16));
+  int4 *ranks = whole_rows ? ds.excl_ranks.as<int4>() : nullptr;
   if (nm) {
     CK(cudaMemsetAsync(ds.excl.p, 0, (size_t)nm * ST * 4, st));
     k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, ST,
-                                                     h.word_lo, h.word_hi);
+                                                     h.word_lo, h.word_hi, ranks);
     f->launches++;
     CK(cudaGetLastError());
     if (lv.n_ovf) {
       k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.ovf_pairs.as<int2>(), lv.n_ovf,
-                                                                 ds.rank_of.as<int32_t>(), ST, h.word_lo, h.word_hi);
+                                                                 ds.rank_of.as<int32_t>(), ST, h.word_lo, h.word_hi, ranks);
       f->launches++;
       CK(cudaGetLastError());
     }
@@ -2097,8 +2113,8 @@ static int32_t commit_locked(mmp_fleet *f) {
     const int F = std::min(SHARD_FRONT_WORDS, RW);
     CK(ds.front.ensure((size_t)nm * F * 4));
     CK(cudaMemsetAsync(ds.front.p, 0, (size_t)nm * F * 4, st));
-    k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, F, 0, F);
-    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf_pairs.as<int2>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F);
+    k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, F, 0, F, nullptr);
+    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf_pairs.as<int2>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F, nullptr);
     f->launches += 2;
     CK(cudaGetLastError());
   }
@@ -2118,7 +2134,8 @@ static int32_t commit_locked(mmp_fleet *f) {
   v.word_lo = h.word_lo; v.word_hi = h.word_hi; v.excl_stride = ST; v.n_slots = h.n_slots; v.n_extra = 0;
   v.count_col = ds.count_col.as<int32_t>(); v.cand_before = ds.cand_before.as<int32_t>();
   v.nzw = ds.nzw.as<uint16_t>(); v.nz_n = ds.nz_n.as<int32_t>();
-  v.excl = ds.excl.as<uint32_t>(); v.cand = ds.cand.as<uint32_t>(); v.pref = ds.pref.as<uint32_t>();
+  v.excl = ds.excl.as<uint32_t>(); v.excl_ranks = ranks ? ds.excl_ranks.as<int32_t>() : nullptr;
+  v.cand = ds.cand.as<uint32_t>(); v.pref = ds.pref.as<uint32_t>();
   v.has_pref = ds.has_pref.as<uint8_t>(); v.type_slot = ds.type_slot.as<uint16_t>(); v.candx = ds.candx.as<uint32_t>();
   v.full = ds.full.as<uint32_t>(); v.rows = ds.rows.as<RankRow>(); v.rank_of = ds.rank_of.as<int32_t>();
   v.csum = ds.csum.as<WordSumI>(); v.lsum = ds.lsum.as<WordSumL>(); v.models = ds.models.as<mmp_model_row>();

@@ -80,6 +80,7 @@ struct SnapshotView {  // pointers into HBM (or host vectors in the CPU harness)
   int32_t n_extra, pad_;       // PER CALL (set by the entry point, not by commit): number of entries in the call's extra[] table
   int64_t min_space;
   const uint32_t *excl;        // [n_models][excl_stride] loaded ∪ failed, bit = rank (word 0 of a stored row = row word word_lo)
+  const int32_t *excl_ranks;   // [n_models][4] the ranks whose bits excl's row holds (see RowRanks); unsharded fleets only, else null
   const uint32_t *cand;        // [n_slots][row_words]  allowed(type) ∧ active
   const uint32_t *candx;       // [n_slots][row_words]  cand ∧ ¬(likely-replaced replicaset members)  (MM:4769-4770)
   const uint32_t *pref;        // [n_slots][row_words]
@@ -839,6 +840,27 @@ struct RowPtr {
   MMP_HD bool ok() const { return p != nullptr; }
   MMP_HD uint32_t word(uint32_t wi) const { return ldro(p + (wi - ws)); }
 };
+// RowRanks (unsharded fleets): the row rebuilt in registers from the model's entry of excl_ranks -- the epoch ranks of its
+// (at most 4) inline edges, -1 for no edge or an instance that is not live.  A model with overflow ids (more than the inline
+// edges hold) has EXCL_RANKS_OVF in r[0] and must be read from its bitmap row instead.  16 bytes per decision, read in
+// sweep order, where the row's words sit one 1 280-byte stride apart.
+static constexpr int32_t EXCL_RANKS_OVF = -2;
+MMP_HD uint32_t rank_bit_in(int32_t r, uint32_t wi) { return ((uint32_t)r >> 5) == wi ? 1u << (r & 31) : 0u; }  // (r < 0: no word)
+struct RowRanks {
+  int32_t r[4];
+  MMP_HD bool ok() const { return true; }
+  MMP_HD bool overflow() const { return r[0] == EXCL_RANKS_OVF; }
+  MMP_HD uint32_t word(uint32_t wi) const { return rank_bit_in(r[0], wi) | rank_bit_in(r[1], wi) | rank_bit_in(r[2], wi) | rank_bit_in(r[3], wi); }
+};
+MMP_HD RowRanks load_ranks(const int32_t *p) {  // read once per decision: kept out of L1 like the decision record
+  RowRanks k;
+#if defined(__CUDA_ARCH__)
+  asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(k.r[0]), "=r"(k.r[1]), "=r"(k.r[2]), "=r"(k.r[3]) : "l"(p));
+#else
+  for (int j = 0; j < 4; j++) k.r[j] = p[j];
+#endif
+  return k;
+}
 // RowDealt (instance-sharded fleets with peer access, SURVEY.md §8e): row words [0, front_words) are replicated on every
 // shard, word wi beyond them lives in the column block of shard wi / block_words -- this GPU's HBM or a peer's, read through
 // its NVLink-mapped pointer.
