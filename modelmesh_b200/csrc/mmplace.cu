@@ -2044,8 +2044,13 @@ static int32_t commit_locked(mmp_fleet *f) {
   const int32_t nm = f->hs.n_models_used;
   ds.n_models = nm;
   // ---- registry: model rows + edges live on the device; a commit sends only what changed on the host ----
+  // A fresh allocation starts as the host holds a model that was never upserted: a zero row, no edges (-1).  A device-path
+  // commit scatters only the dirty models, so an upsert past n_models_used leaves the rows in between to this initial state.
+  const size_t models_cap0 = lv.models.cap, edges_cap0 = lv.edges.cap;
   CK(lv.models.ensure((size_t)std::max(f->hs.cfg.max_models, 1) * sizeof(mmp_model_row)));
   CK(lv.edges.ensure((size_t)std::max(f->hs.cfg.max_models, 1) * HostState::EDGE_INL * 4));
+  if (lv.models.cap != models_cap0) CK(cudaMemsetAsync(lv.models.p, 0, lv.models.cap, st));
+  if (lv.edges.cap != edges_cap0) CK(cudaMemsetAsync(lv.edges.p, 0xff, lv.edges.cap, st));
   if (!f->device_ahead) {
     if (structural || f->hs.all_models_dirty) {
       if (nm) {
