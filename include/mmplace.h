@@ -38,8 +38,10 @@ enum {
   MMP_TARGET_SELF = -2,   /* getNext returned ABORT_REQUEST (MM:4894,4932,4990)    */
   MMP_TARGET_INVALID = -3 /* malformed decision, nothing was decided: model / self index out of range, self not live and no
                              fresh row given, or an extra[] slice outside the table passed with the call (extra_off < 0,
-                             extra_n outside [0, MMP_MAX_EXTRA], extra_off + extra_n > n_extra).  The reference has no
-                             counterpart (a Java caller cannot form such a call); the batch itself still succeeds. */
+                             extra_n outside [0, MMP_MAX_EXTRA], extra_off + extra_n > n_extra); with MMP_DF_REQUEST_MODEL
+                             also a type id outside [0, 65535), the flag combined with MMP_DF_MODEL_LAST_USED, or an
+                             instance-sharded fleet.  The reference has no counterpart (a Java caller cannot form such a
+                             call); the batch itself still succeeds. */
 };
 #define MMP_MAX_EXTRA 16  /* per-decision additional excludes (tried-this-request ∪ explicit, MM:4706-4715) */
 
@@ -86,14 +88,22 @@ typedef struct {
 } mmp_model_row;
 
 /* One call of CacheMissForwardingLB.getNext (MM:4776-5004): 32 bytes.
- * The model's exclusion set (loaded ∪ failed, MM:4735-4743) and type come from the model table. */
+ * The model's exclusion set (loaded ∪ failed, MM:4735-4743) and type come from the model table of the last committed
+ * snapshot -- or, with MMP_DF_REQUEST_MODEL, from the decision itself. */
 #define MMP_DF_FAVOUR_SELF 1u        /* CacheMissExcludeSet.favourSelf (MM:4721) */
 #define MMP_DF_MODEL_LAST_USED 2u    /* take last_used from the model row instead of this struct */
 #define MMP_DF_OWN_ID 4u             /* bits 8..31 of flags carry the decision's own id for the hash-indexed pick (N4, MM:4981)
                                         instead of its position in the batch: the result of a decision then does not depend on
                                         which batch it travelled in (mmp_place_submit coalesces callers this way) */
+#define MMP_DF_REQUEST_MODEL 8u      /* the model record this request read (MM:3537, refreshed after a failed load MM:4088-4097)
+                                        instead of the committed one: `model` holds the model's TYPE ID (mmp_type_id; an id the
+                                        snapshot does not know resolves like type 0, as a model row holding it would), and its
+                                        loaded ∪ failed instance indices (MR:69,73) travel in the extra[] slice together with the
+                                        request's own excludes -- at most MMP_MAX_EXTRA in all.  No registry state of the snapshot
+                                        is read, so a model registered or changed since the last commit is placed on its current
+                                        record.  Not with MMP_DF_MODEL_LAST_USED; unsharded fleets only (else MMP_TARGET_INVALID) */
 typedef struct {
-  int32_t model;        /* model index */
+  int32_t model;        /* model index, or the type id with MMP_DF_REQUEST_MODEL */
   int32_t self;         /* instance index of the calling pod ("instanceId", MM:4780,4808) */
   int64_t last_used;    /* CacheMissExcludeSet.lastUsedTime (MM:4730, 4949) */
   uint32_t flags;       /* MMP_DF_* */

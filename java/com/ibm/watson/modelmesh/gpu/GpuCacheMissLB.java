@@ -17,6 +17,9 @@ public abstract class GpuCacheMissLB implements LoadBalancer {
     public interface Host {
         String instanceId();
         String requestModelId();                                   // the model the current request is about
+        String requestModelType();                                 // CacheMissExcludeSet.modelType: the record's type (MM:3782)
+        java.util.Set<String> requestLoadedAndFailed();            // its loaded / failed key sets: the record read for this request
+                                                                   // (MM:3537, 3785 -> 4735-4743; refreshed after a failed load MM:4088-4097)
         java.util.Set<String> requestExcludes();                   // CacheMissExcludeSet's own members ∪ explicit (MM:4706-4715)
         long requestLastUsedTime();                                // CacheMissExcludeSet.lastUsedTime (MM:4730)
         boolean requestFavourSelf();                               // CacheMissExcludeSet.favourSelf (MM:4721)
@@ -36,9 +39,9 @@ public abstract class GpuCacheMissLB implements LoadBalancer {
     public <T> T getNext(Object[] sis, String method, Object[] args) {
         final String chosen;
         try {
-            chosen = gpu.placeOne(host.requestModelId(), host.instanceId(), host.requestLastUsedTime(), host.requestFavourSelf(),
-                    host.freshInstanceRecord(), host.requestExcludes().toArray(new String[0]), System.currentTimeMillis());
-        } catch (RuntimeException e) {
+            chosen = gpu.placeOne(host.requestModelType(), host.requestLoadedAndFailed(), host.instanceId(), host.requestLastUsedTime(),
+                    host.requestFavourSelf(), host.freshInstanceRecord(), host.requestExcludes(), System.currentTimeMillis());
+        } catch (RuntimeException e) {  // library error, or more than MMP_MAX_EXTRA ids to exclude
             return host.fallback(sis, method, args);
         }
         if (chosen == null) return null;                                      // MM:4796, 4941: "Nowhere available to load" upstream

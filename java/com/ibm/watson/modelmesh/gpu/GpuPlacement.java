@@ -27,6 +27,8 @@ public final class GpuPlacement implements AutoCloseable {
     final long h;
     private final int maxInstances, maxModels;
     private final Map<String, Integer> instanceIdx = new HashMap<>(), modelIdx = new ConcurrentHashMap<>();
+    /** model-type name -> MmPlace.typeId (interned by the library, stable for the fleet's life) */
+    private final Map<String, Integer> typeIdOf = new ConcurrentHashMap<>();
     private final ArrayDeque<Integer> freeInstanceIdx = new ArrayDeque<>();
     private final String[] instanceIdOf;
     private int nextModelIdx;
@@ -90,24 +92,36 @@ public final class GpuPlacement implements AutoCloseable {
     // ---- plug point 1: one getNext on the request thread (GpuCacheMissLB) ----
     /** @return instance id, null (getNext returned null) or SELF for LoadBalancer.ABORT_REQUEST */
     public static final String SELF = new String("<self>");
-    public String placeOne(String modelId, String selfId, long lastUsedTime, boolean favourSelf, InstanceRecord fresh, String[] extraExcluded,
-                           long nowMs) {
-        Integer m = modelIdx.get(modelId);
+    /**
+     * The model travels as the record this request read (MMP_DF_REQUEST_MODEL): its type and its loaded ∪ failed instances,
+     * as the reference builds the CacheMissExcludeSet from the record (MM:3537, 3782-3785), so a model registered or changed
+     * since the last commit is placed on its current record.  Instance ids the dictionary does not know are dropped (they
+     * name no live instance); more than MMP_MAX_EXTRA ids in all throws, and GpuCacheMissLB falls back to the Java LB.
+     */
+    public String placeOne(String modelType, java.util.Set<String> loadedAndFailed, String selfId, long lastUsedTime, boolean favourSelf,
+                           InstanceRecord fresh, java.util.Set<String> requestExcludes, long nowMs) {
+        // (ModelRecord's DEFAULT_TYPE for a record without one, MR:117-130, as the library reads a JSON record)
+        int type = typeIdOf.computeIfAbsent(modelType == null ? "NLCLASSIFIER" : modelType, t -> check(MmPlace.typeId(h, t)));
         Integer self;
-        int[] extra;
+        int[] extra = new int[MmPlace.MAX_EXTRA];
+        int n = 0;
         synchronized (this) {
             self = instanceIdx.get(selfId);
-            extra = new int[extraExcluded.length];
-            int n = 0;
-            for (String e : extraExcluded) { Integer i = instanceIdx.get(e); if (i != null) extra[n++] = i; }
-            if (n != extra.length) extra = java.util.Arrays.copyOf(extra, n);
+            for (java.util.Set<String> set : java.util.Arrays.asList(loadedAndFailed, requestExcludes))
+                for (String e : set) {
+                    Integer i = instanceIdx.get(e);
+                    if (i == null) continue;
+                    if (n == extra.length) throw new IllegalStateException("more than " + MmPlace.MAX_EXTRA + " instances to exclude");
+                    extra[n++] = i;
+                }
         }
-        if (m == null || self == null) return null;
+        if (self == null) return null;
         ByteBuffer[] s = scratch.get();
         ByteBuffer in = s[0], fr = s[1], out = s[2];
         in.clear();
-        in.putInt(m).putInt(self).putLong(lastUsedTime).putInt(favourSelf ? MmPlace.DF_FAVOUR_SELF : 0).putInt(fresh != null ? 0 : -1)
-          .putInt(0).putInt(extra.length);
+        in.putInt(type).putInt(self).putLong(lastUsedTime).putInt(MmPlace.DF_REQUEST_MODEL | (favourSelf ? MmPlace.DF_FAVOUR_SELF : 0))
+          .putInt(fresh != null ? 0 : -1).putInt(0).putInt(n);
+        extra = java.util.Arrays.copyOf(extra, n);
         if (fresh != null) encode(fresh, true, fr);
         int rc = MmPlace.placeOne(h, in, fresh != null ? fr : null, extra.length > 0 ? extra : null, out, nowMs, pickSeed.incrementAndGet());
         if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h));  // the caller falls back to the Java load balancer

@@ -15,7 +15,8 @@ final class MmPlace {
     private MmPlace() {}
 
     static final int TARGET_NONE = -1, TARGET_SELF = -2, TARGET_INVALID = -3;     // mmp_decision_out.target
-    static final int DF_FAVOUR_SELF = 1, DF_MODEL_LAST_USED = 2;                   // mmp_decision_in.flags
+    static final int DF_FAVOUR_SELF = 1, DF_MODEL_LAST_USED = 2, DF_REQUEST_MODEL = 8;  // mmp_decision_in.flags
+    static final int MAX_EXTRA = 16;                                               // MMP_MAX_EXTRA
     static final int INSTANCE_ROW_BYTES = 64, MODEL_ROW_BYTES = 24, DECISION_IN_BYTES = 32, DECISION_OUT_BYTES = 8;
 
     // lifecycle

@@ -71,6 +71,8 @@ class ChurnReport(C.Structure):
 DF_FAVOUR_SELF = 1
 DF_MODEL_LAST_USED = 2
 DF_OWN_ID = 4
+DF_REQUEST_MODEL = 8  # model = type id, the model's loaded ∪ failed instances in extra[] (MMP_DF_REQUEST_MODEL)
+MAX_EXTRA = 16
 TARGET_NONE = -1
 TARGET_SELF = -2
 TARGET_INVALID = -3

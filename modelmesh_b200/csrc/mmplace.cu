@@ -5,6 +5,7 @@
 //                                         the instance under PLACEMENT_ORDER; row stride is a multiple of 128 B
 //   excl_ranks [n_models] int4            the ranks of a model's <= 4 inline edges (-1: none), r[0] = -2: overflow ids,
 //                                         read the row (unsharded fleets)
+//   zero_row  [row_words]           u32   all zero, one per fleet: the row of every MMP_DF_REQUEST_MODEL decision (unsharded fleets)
 //   cand/pref [n_slots][row_words]  u32   per type-constraint slot: allowed ∧ active / preferred instances (TCM:242-251)
 //   candx     [n_slots][row_words]  u32   cand minus likely-replaced replicaset members (MM:4769-4770)
 //   full      [row_words]           u32   isFull instances (MM:4640)
@@ -184,7 +185,7 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place(const SnapshotView s
     const int i = batch * 32 + lane;
     DecisionCtx cn;
     cn.slot = -2;  // absent
-    cn.d.model = 0;
+    cn.d.model = 0; cn.d.flags = 0;
     if (batch < nb && i < n) {
       const int4 *dp = reinterpret_cast<const int4 *>(in + i);
       int4 a = __ldg(dp), b = __ldg(dp + 1);
@@ -195,11 +196,10 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place(const SnapshotView s
     }
     dst[lane] = cn;
   };
-  auto issue = [&](int model, uint32_t pos) {  // lane 0 only
-    const int m = (model >= 0 && model < s.n_models) ? model : 0;
+  auto issue = [&](int row_id, uint32_t pos) {  // lane 0 only; row_id from excl_row_id
     const uint32_t sl = pos % (uint32_t)K;
     mbar_expect_tx(&bars[sl], row_bytes);
-    bulk_g2s(rows_s + (size_t)sl * RW, s.excl + (size_t)m * RW, row_bytes, &bars[sl]);
+    bulk_g2s(rows_s + (size_t)sl * RW, excl_row(s, row_id), row_bytes, &bars[sl]);
   };
   int b = gw;
   prep(b, ctx_s);
@@ -207,17 +207,17 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place(const SnapshotView s
   if (b < nb) {
     const int count = min(32, n - b * 32);
     if (lane == 0)
-      for (int t = 0; t < K && t < count; t++) issue(ctx_s[t].d.model, (uint32_t)t);
+      for (int t = 0; t < K && t < count; t++) issue(excl_row_id(s, ctx_s[t].d.model, ctx_s[t].d.flags), (uint32_t)t);
   }
   while (b < nb) {
     const int bn = b + nw;
     const DecisionCtx *cc = ctx_s;
-    // the next batch's contexts are staged when this batch is done (one buffer); only its model indices are fetched
-    // now, because the ring must start loading its first rows K positions before the batch boundary
+    // the next batch's contexts are staged when this batch is done (one buffer); only its row ids are fetched now,
+    // because the ring must start loading its first rows K positions before the batch boundary
     int next_model = -1;
     {
       const int i = bn * 32 + lane;
-      if (bn < nb && i < n) next_model = __ldg(&in[i].model);
+      if (bn < nb && i < n) next_model = excl_row_id(s, __ldg(&in[i].model), __ldg(&in[i].flags));
     }
     const int count = min(32, n - b * 32);
     mmp_decision_out mine{MMP_TARGET_NONE, 0};
@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place(const SnapshotView s
       const int t = jdone + K;
       int nm = 0;
       bool have = false;
-      if (t < count) { nm = cc[t].d.model; have = true; }
+      if (t < count) { nm = excl_row_id(s, cc[t].d.model, cc[t].d.flags); have = true; }
       else if (t - count < K && nm_next[t - count] != -1) { nm = nm_next[t - count]; have = true; }
       if (have) {
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -477,7 +477,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
     unsigned char *stage = smem_raw + (size_t)st * lay.stage_bytes;
     const uint32_t *my_row = reinterpret_cast<const uint32_t *>(stage + (size_t)lane * lay.stride);
     // row of this decision: its model's, or row i of a gathered row set (orig_id != nullptr: the instance-shard gather pass)
-    const int m = orig_id ? (valid ? b * 32 + lane : 0) : ((valid && d.model >= 0 && d.model < s.n_models) ? d.model : 0);
+    const int m = orig_id ? (valid ? b * 32 + lane : 0) : (valid ? excl_row_id(s, d.model, d.flags) : 0);
     DecisionCtx c;
     c.slot = -2; c.d.model = 0; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
     bool skip = false;  // instance-sharded, not the first shard: an entry in a lower shard wins, the row is not even read
@@ -487,7 +487,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
     if (valid && !skip) {
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the previous owner's reads precede this async write
       mbar_expect_tx(&bars[st], lay.row_bytes);
-      bulk_g2s(const_cast<uint32_t *>(my_row), s.excl + (size_t)m * RW, lay.row_bytes, &bars[st]);
+      bulk_g2s(const_cast<uint32_t *>(my_row), excl_row(s, m), lay.row_bytes, &bars[st]);
     } else mbar_arrive(&bars[st]);
     LANE_T(1);
     // ---- the rest of this batch's context while its rows are in flight ----
@@ -535,7 +535,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
       Tw.full = f_full - WS; Tw.csum = f_csum - WS; Tw.count_col = f_count - WS * 32; Tw.rows = f_rows - WS * 32;
     }
     if ((mode & 1) == 0)
-      handled = decide_stream(s, Tw, T, c, valid && !skip, win + lane * LANE_STRIDE, win_words, RowPtr{s.excl + (size_t)m * RW, (uint32_t)s.word_lo}, self_eword,
+      handled = decide_stream(s, Tw, T, c, valid && !skip, win + lane * LANE_STRIDE, win_words, RowPtr{excl_row(s, m), (uint32_t)s.word_lo}, self_eword,
                               now, seed, my_id, WarpVote(), o, budget);
     else { o.target = (int32_t)(self_eword & 1u) - 1; o.n_candidates = 0; }  // MMP_LANE_MODE=1: stream-only probe (no decisions)
     // ---- what the lane routine declined: the whole warp redoes it, reading the row from global memory (L2) ----
@@ -549,7 +549,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
       const uint64_t idl = __shfl_sync(0xffffffffu, my_id, l);
       __syncwarp();
       int32_t t2, c2, f2, g2;
-      decide_warp(s, *ctx_one, s.excl + (size_t)ml * RW, extra, now, seed, idl, &t2, &c2, &f2, &g2);
+      decide_warp(s, *ctx_one, excl_row(s, ml), extra, now, seed, idl, &t2, &c2, &f2, &g2);
       if (lane == l) { o.target = t2; o.n_candidates = c2; o.first_rank = f2; o.flags = g2; }
       __syncwarp();
     }
@@ -589,15 +589,14 @@ __device__ __forceinline__ void place_small_block(const SnapshotView &s, const m
   const int lane = threadIdx.x;
   const int i = blk * 32 + lane;
   const bool valid = i < n;
-  const int RW = s.excl_stride;
   mmp_decision_in d;
   d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
   if (valid) d = in[i];
   DecisionCtx c;
   c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
   if (valid) prepare_ctx(s, d, fresh, n_fresh, extra, c);
-  const int m = (valid && d.model >= 0 && d.model < s.n_models) ? d.model : 0;
-  const uint32_t *row = s.excl + (size_t)m * RW;
+  const int m = excl_row_id(s, d.model, d.flags);
+  const uint32_t *row = excl_row(s, m);
   const LaneTables T = lane_tables_global(s, c.slot >= 0 ? ctx_slot(c) : 0);
   uint32_t self_eword = 0;
   if (valid && c.self_rank >= 0) self_eword = __ldg(row + (c.self_rank >> 5));
@@ -615,7 +614,7 @@ __device__ __forceinline__ void place_small_block(const SnapshotView &s, const m
     const uint64_t idl = __shfl_sync(0xffffffffu, my_id, l);
     __syncwarp();
     int32_t t2, c2, f2, g2;
-    decide_warp(s, *ctx_one, s.excl + (size_t)ml * RW, extra, now, seed, idl, &t2, &c2, &f2, &g2);
+    decide_warp(s, *ctx_one, excl_row(s, ml), extra, now, seed, idl, &t2, &c2, &f2, &g2);
     if (lane == l) { o.target = t2; o.n_candidates = c2; }
     __syncwarp();
   }
@@ -654,10 +653,10 @@ __global__ void k_sparse_slots(const uint32_t *__restrict__ cx, int row_words, i
 __global__ void k_slot_keys(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n, uint16_t *__restrict__ keys, int32_t *__restrict__ idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const int m = in[i].model;
+  const mmp_decision_in d = in[i];
   uint32_t k = 0xffffu;
-  if (m >= 0 && m < s.n_models) {
-    const int ty = s.models[m].type_id;
+  if (request_model(d) ? (d.model >= 0 && d.model < 65535) : (d.model >= 0 && d.model < s.n_models)) {
+    const int ty = request_model(d) ? d.model : s.models[d.model].type_id;
     k = (uint32_t)s.type_slot[(ty >= 0 && ty < s.n_type_ids) ? ty : 0] & 0x7fffu;  // (as prepare_ctx_b resolves it)
   }
   keys[i] = (uint16_t)k;
@@ -678,7 +677,6 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
   // perm (optional): the batch in type-slot order -- decisions of one slot walk the same masks, so the 32 lanes of a warp
   // finish their walks together instead of waiting for the longest (fleets with sparse candidate sets: C5)
   const int i = valid ? (perm ? perm[j_] : j_) : 0;
-  const int RW = s.excl_stride;
   mmp_decision_in d;
   d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
   if (valid) {
@@ -689,11 +687,12 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
     d.model = a.x; d.self = a.y; d.last_used = (int64_t)(((uint64_t)(uint32_t)a.w << 32) | (uint32_t)a.z);
     d.flags = (uint32_t)c.x; d.fresh = c.y; d.extra_off = c.z; d.extra_n = c.w;
   }
-  const int m = (valid && d.model >= 0 && d.model < s.n_models) ? d.model : 0;
-  // the model's excluded ranks go out first: they depend on the record only
+  const int m = excl_row_id(s, d.model, d.flags);
+  // the model's excluded ranks go out first: they depend on the record only (a request-model decision has none: its
+  // model's instances are among its extras)
   RowRanks row;
   row.r[0] = row.r[1] = row.r[2] = row.r[3] = -1;
-  if (valid) row = load_ranks(s.excl_ranks + (size_t)m * 4);
+  if (valid && m != ZERO_ROW) row = load_ranks(s.excl_ranks + (size_t)m * 4);
   DecisionCtx c;
   c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
   if (valid) prepare_ctx(s, d, fresh, n_fresh, extra, c);
@@ -724,7 +723,7 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
     const uint64_t idl = __shfl_sync(0xffffffffu, my_id, l);
     __syncwarp();
     int32_t t2, c2, f2, g2;
-    decide_warp(s, ctx_w[warp], s.excl + (size_t)ml * RW, extra, now, seed, idl, &t2, &c2, &f2, &g2);
+    decide_warp(s, ctx_w[warp], excl_row(s, ml), extra, now, seed, idl, &t2, &c2, &f2, &g2);
     if (lane == l) { o.target = t2; o.n_candidates = c2; }
     __syncwarp();
   }
@@ -740,10 +739,11 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
 // device to drain (cudaFree inside a commit) waits at most life_ns, and a crashed host leaves no kernel behind.
 // ---------------------------------------------------------------------------------------------------------------
 // request line 0 (one 64-byte line = one PCIe read per poll): everything a single decision without side tables needs.
-// seq: low 56 bits = request counter, top 8 bits = kind (1: one decision, its fresh row -- if any -- in line 1;
-// 2: a batch of up to 32 laid out like the graph path's buffer, sizes in line 1; 0xff: leave)
+// seq: low 56 bits = request counter, top 8 bits = kind (1: one decision, its fresh row and up to SRV_INLINE_EXTRA extra
+// excludes -- if any -- in line 1; 2: a batch of up to 32 laid out like the graph path's buffer, sizes in line 1; 0xff: leave)
+static constexpr int SRV_INLINE_EXTRA = 4;  // a request-thread getNext carries its model's copies and failures (< 5 and < 3 at a cache miss)
 struct SrvLine0 { unsigned long long seq; long long now; unsigned long long seed, id_base; mmp_decision_in d; };
-struct SrvLine1 { int n, n_fresh, n_extra, pad; FreshRow fr; unsigned long long pad2[3]; };
+struct SrvLine1 { int n, n_fresh, n_extra, pad; FreshRow fr; int32_t extra[SRV_INLINE_EXTRA]; unsigned long long pad2; };
 struct ServerResp { unsigned long long done_seq; int alive, served; mmp_decision_out out0; unsigned long long pad[5]; };
 static_assert(sizeof(SrvLine0) == 64 && sizeof(SrvLine1) == 64 && sizeof(ServerResp) == 64, "one line each");
 struct SrvTabs {
@@ -757,6 +757,7 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
                                                      mmp_decision_out *out_tab, unsigned long long life_ns, unsigned long long idle_ns, int budget) {
   __shared__ DecisionCtx ctx_one;
   __shared__ __align__(16) uint32_t line_s[16];
+  __shared__ __align__(16) uint32_t line1_s[16];  // kind 1's line 1: fresh row and inline extras (extra[] of the decision)
   __shared__ FreshRow fresh_s;
   __shared__ uint32_t win_s[32 * LANE_STRIDE];
   __shared__ uint32_t chunk_v[32 * MMP_CHUNK_WORDS];
@@ -824,15 +825,18 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
       if (valid) d = *reinterpret_cast<const mmp_decision_in *>(line_s + 8);
       int n_fresh = 0;
       s.n_extra = 0;
-      if (__shfl_sync(0xffffffffu, d.fresh, 0) >= 0 || __shfl_sync(0xffffffffu, d.extra_n, 0) > 0) {  // side tables: a second read
-        if (lane == 0) { n_fresh = l1->n_fresh; s.n_extra = l1->n_extra; fresh_s.lru = l1->fr.lru; fresh_s.rem = l1->fr.rem; fresh_s.count = l1->fr.count; fresh_s.rpm = l1->fr.rpm; }
-        n_fresh = __shfl_sync(0xffffffffu, n_fresh, 0);
-        s.n_extra = __shfl_sync(0xffffffffu, s.n_extra, 0);
+      // the decision's extra[] is line 1's inline part (extra_off = 0, at most SRV_INLINE_EXTRA entries: place_server)
+      const int32_t *extra1 = reinterpret_cast<const int32_t *>(line1_s + offsetof(SrvLine1, extra) / 4);
+      if (__shfl_sync(0xffffffffu, d.fresh, 0) >= 0 || __shfl_sync(0xffffffffu, d.extra_n, 0) > 0) {  // side tables: a second read, one line
+        if (lane < 16) line1_s[lane] = reinterpret_cast<volatile uint32_t *>(l1)[lane];
+        __syncwarp();
+        n_fresh = (int)line1_s[offsetof(SrvLine1, n_fresh) / 4];
+        s.n_extra = (int)line1_s[offsetof(SrvLine1, n_extra) / 4];
+        if (lane == 0) fresh_s = *reinterpret_cast<const FreshRow *>(line1_s + offsetof(SrvLine1, fr) / 4);
         __syncwarp();
       }
-      const int RW = s.excl_stride;
-      const int m = (valid && d.model >= 0 && d.model < s.n_models) ? d.model : 0;
-      const uint32_t *row = s.excl + (size_t)m * RW;
+      const int m = excl_row_id(s, d.model, d.flags);
+      const uint32_t *row = excl_row(s, m);
       uint4 q[LANE_WIN / 4];
 #pragma unroll
       for (int j = 0; j < LANE_WIN / 4; j++) {
@@ -841,7 +845,7 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
       }
       DecisionCtx c;
       c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
-      if (valid) prepare_ctx(s, d, &fresh_s, min(n_fresh, 1), extra, c);
+      if (valid) prepare_ctx(s, d, &fresh_s, min(n_fresh, 1), extra1, c);
       uint32_t self_eword = 0;
       if (valid && c.self_rank >= 0) self_eword = __ldg(row + (c.self_rank >> 5) - s.word_lo);
       uint32_t *w = win_s + lane * LANE_STRIDE;
@@ -861,7 +865,7 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
         if (lane == 0) ctx_one = c;
         __syncwarp();
         int32_t t2, c2, f2, g2;
-        decide_warp(s, ctx_one, s.excl + (size_t)__shfl_sync(0xffffffffu, m, 0) * RW, extra, now, seed, __shfl_sync(0xffffffffu, my_id, 0), &t2, &c2, &f2, &g2);
+        decide_warp(s, ctx_one, excl_row(s, __shfl_sync(0xffffffffu, m, 0)), extra1, now, seed, __shfl_sync(0xffffffffu, my_id, 0), &t2, &c2, &f2, &g2);
         if (lane == 0) { o.target = t2; o.n_candidates = c2; }
         __syncwarp();
       }
@@ -1176,6 +1180,7 @@ struct mmp_fleet {
   int32_t epoch = 0;
   cudaStream_t commit_stream = nullptr;
   DevBuf d_flush, d_dbg;
+  DevBuf zero_row;              // one all-zero exclusion row (SnapshotView::zero_row), unsharded fleets: allocated at the first commit
   ChurnState churn;             // the closed loop (churn_kernels.cuh)
   int64_t structural_epoch = 0; // bumped by every structural commit
   LiveState live;               // device-resident tables every non-structural commit works from (commit_kernels.cuh)
@@ -1800,7 +1805,7 @@ void mmp_fleet_destroy(mmp_fleet *f) {
                     &f->live.models, &f->live.ovf_pairs, &f->live.keys, &f->live.rs_words, &f->live.flags, &f->live.scratch_idx,
                     &f->live.scratch_rows, &f->live.scratch_edges, &f->live.edge_ts, &f->live.model_lul, &f->live.type_part_off, &f->live.type_parts})
     b->release();
-  for (DevBuf *b : {&f->d_flush, &f->lru_ts, &f->lru_seq, &f->lru_weight, &f->lru_model,
+  for (DevBuf *b : {&f->d_flush, &f->zero_row, &f->lru_ts, &f->lru_seq, &f->lru_weight, &f->lru_model,
                     &f->lru_cap, &f->lru_wsize, &f->lru_count, &f->lru_seqctr, &f->lru_loadts})
     b->release();
   if (f->commit_stream) cudaStreamDestroy(f->commit_stream);
@@ -2101,6 +2106,12 @@ static int32_t commit_locked(mmp_fleet *f) {
   const bool whole_rows = h.word_lo == 0 && h.word_hi == RW;
   if (whole_rows) CK(ds.excl_ranks.ensure((size_t)std::max(nm, 1) * 16));
   int4 *ranks = whole_rows ? ds.excl_ranks.as<int4>() : nullptr;
+  // the row of every request-model decision (MMP_DF_REQUEST_MODEL): the stride is fixed for the fleet, so it is zeroed once
+  // (cudaMalloc: 256-byte aligned, as the TMA copies of k_place_lanes and k_place need)
+  if (whole_rows && !f->zero_row.p) {
+    CK(f->zero_row.ensure((size_t)ST * 4));
+    CK(cudaMemsetAsync(f->zero_row.p, 0, (size_t)ST * 4, st));
+  }
   if (nm) {
     CK(cudaMemsetAsync(ds.excl.p, 0, (size_t)nm * ST * 4, st));
     k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, ST,
@@ -2144,6 +2155,7 @@ static int32_t commit_locked(mmp_fleet *f) {
   v.has_pref = ds.has_pref.as<uint8_t>(); v.type_slot = ds.type_slot.as<uint16_t>(); v.candx = ds.candx.as<uint32_t>();
   v.full = ds.full.as<uint32_t>(); v.rows = ds.rows.as<RankRow>(); v.rank_of = ds.rank_of.as<int32_t>();
   v.csum = ds.csum.as<WordSumI>(); v.lsum = ds.lsum.as<WordSumL>(); v.models = ds.models.as<mmp_model_row>();
+  v.zero_row = whole_rows ? f->zero_row.as<uint32_t>() : nullptr;
   {
     std::unique_lock<std::shared_mutex> w(f->snap_mu);  // waits for in-flight readers of the current epoch
     f->cur = 1 - f->cur;
@@ -2222,12 +2234,16 @@ static int32_t place_server(mmp_fleet *f, const DeviceSnapshot &ds, const mmp_de
   volatile SrvLine1 *l1 = reinterpret_cast<volatile SrvLine1 *>(h + 64);
   volatile ServerResp *resp = reinterpret_cast<volatile ServerResp *>(h + g_resp);
   if (sv.running && sv.epoch != f->epoch) server_stop(f);  // its snapshot view is another epoch's
-  // kind 1: one decision whose side tables are at most its own fresh row (the shape of getNext on a request thread)
-  const bool single = n == 1 && n_extra == 0 && (in[0].fresh < 0 || in[0].fresh == 0) && n_fresh <= 1;
+  // kind 1: one decision whose side tables are at most its own fresh row and a few extra excludes from the start of extra[]
+  // (the shape of getNext on a request thread: a request-model decision carries its model's copies and failures there)
+  const int32_t n_inline = n_extra == 0 ? 0 : in[0].extra_n;
+  const bool single = n == 1 && (n_extra == 0 || (in[0].extra_off == 0 && n_inline >= 0 && n_inline <= SRV_INLINE_EXTRA && n_inline <= n_extra)) &&
+                      (in[0].fresh < 0 || in[0].fresh == 0) && n_fresh <= 1;
   if (single) {
     mmp_decision_in d = in[0];
     if (n_fresh) { FreshRow fr = fresh[0]; memcpy((void *)&l1->fr, &fr, sizeof(fr)); }
-    l1->n = 1; l1->n_fresh = n_fresh; l1->n_extra = 0;
+    if (n_inline) memcpy((void *)l1->extra, extra, (size_t)n_inline * 4);
+    l1->n = 1; l1->n_fresh = n_fresh; l1->n_extra = n_inline;
     memcpy((void *)&l0->d, &d, sizeof(d));
   } else {
     memcpy(h + g_in, in, (size_t)n * sizeof(mmp_decision_in));

@@ -32,7 +32,7 @@
 namespace mmp {
 
 static constexpr uint32_t NONE_RANK = 0x7fffffffu;
-static constexpr int32_t TARGET_INVALID = -3;  // malformed decision (bad model/self index or no fresh row for a non-live self)
+static constexpr int32_t TARGET_INVALID = -3;  // malformed decision (bad model/self index or no fresh row for a non-live self; MMP_TARGET_INVALID)
 
 struct RankRow {  // one per PLACEMENT_ORDER rank, 32 bytes
   int64_t lru;    // published lruTime (IR:37)
@@ -96,7 +96,24 @@ struct SnapshotView {  // pointers into HBM (or host vectors in the CPU harness)
   const uint16_t *nzw;         // [n_slots][row_words] compressed word lists (see LaneTables), entries past nz_n[slot] unused
   const int32_t *nz_n;         // [n_slots]
   const mmp_model_row *models; // [n_models]
+  const uint32_t *zero_row;    // [excl_stride] all zero: the exclusion row of an MMP_DF_REQUEST_MODEL decision; null on
+                               // instance-sharded fleets, where such a decision is malformed
 };
+
+// ---- where a decision's model comes from.  Unflagged: the committed registry (models[d.model], its exclusion row).
+// MMP_DF_REQUEST_MODEL: the record the caller read for this request -- d.model is its type id, its loaded ∪ failed instances
+// travel in extra[] -- so no registry state is read and the exclusion row is the all-zero one. ----
+MMP_HD bool request_model(const mmp_decision_in &d) { return (d.flags & MMP_DF_REQUEST_MODEL) != 0; }
+// the exclusion row a decision reads, as an int that lanes can exchange: its model's row (index clamped: a malformed
+// decision is answered MMP_TARGET_INVALID, its row is fetched but never used) or ZERO_ROW
+static constexpr int32_t ZERO_ROW = -3;
+MMP_HD int32_t excl_row_id(const SnapshotView &s, int32_t model, uint32_t flags) {
+  if ((flags & MMP_DF_REQUEST_MODEL) && s.zero_row) return ZERO_ROW;
+  return (model >= 0 && model < s.n_models) ? model : 0;
+}
+MMP_HD const uint32_t *excl_row(const SnapshotView &s, int32_t id) {
+  return id == ZERO_ROW ? s.zero_row : s.excl + (size_t)id * (size_t)s.excl_stride;
+}
 
 // ---- PLACEMENT_ORDER (MM:4646-4703) on numeric columns + dense string ranks.  Host: merge sort at a structural commit
 // (host_state.hpp); device: rank = number of live instances that compare less (k_rank_count, the fast commit path). ----
@@ -504,13 +521,24 @@ MMP_HD bool ctx_has_pref(const DecisionCtx &c) { return (c.slot >> 16) & 1; }
 // the decision record: the model row from HBM, rank_of[self]) a whole step ahead of the second (what depends on them).
 struct CtxA { mmp_model_row mr; int32_t self_rank; int32_t ok; };
 MMP_HD void prepare_ctx_a(const SnapshotView &s, const mmp_decision_in &d, CtxA &a) {
-  a.ok = !(d.model < 0 || d.model >= s.n_models || d.self < 0 || d.self >= s.max_instances);
+  // a request-model decision names a type id (mmp_type_id: [0, 65535)); its last_used can only come from the decision, and
+  // only a fleet with the zero row (unsharded) takes it
+  const bool req = request_model(d);
+  a.ok = !(d.self < 0 || d.self >= s.max_instances);
+  if (req ? (d.model < 0 || d.model >= 65535 || (d.flags & MMP_DF_MODEL_LAST_USED) || !s.zero_row) : (d.model < 0 || d.model >= s.n_models)) a.ok = 0;
   // the decision's slice of extra[] must lie inside the table the caller passed (at most 16 entries, MMP_MAX_EXTRA):
   // anything else is a malformed decision (MMP_TARGET_INVALID), never an out-of-bounds read
   if (d.extra_n < 0 || d.extra_n > 16 || (d.extra_n > 0 && (d.extra_off < 0 || (int64_t)d.extra_off + d.extra_n > (int64_t)s.n_extra))) a.ok = 0;
   a.self_rank = -1;
   a.mr.last_used = 0; a.mr.size_units = 0; a.mr.rpm = 0; a.mr.type_id = 0; a.mr.copy_count = 0; a.mr.fail_count = 0; a.mr.reserved = 0;
-  if (a.ok) {
+  if (a.ok && req) {
+    a.mr.type_id = (uint16_t)d.model;  // (a type id past the snapshot's n_type_ids resolves as 0 in prepare_ctx_b, as a row's would)
+#if defined(__CUDA_ARCH__)
+    a.self_rank = __ldg(s.rank_of + d.self);
+#else
+    a.self_rank = s.rank_of[d.self];
+#endif
+  } else if (a.ok) {
 #if defined(__CUDA_ARCH__)
     // the 24-byte model row is read once per decision: keep it out of L1, where the lane routine's tables live
     const int2 *mp = reinterpret_cast<const int2 *>(s.models + d.model);
