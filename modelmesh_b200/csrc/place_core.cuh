@@ -752,7 +752,10 @@ MMP_HD bool decide_fast(const SnapshotView &s, const DecisionCtx &c, const uint3
 // 10 000 instances) a walk that crossed 50-300 empty words becomes a few steps.
 // row words of a decision's window in k_place_lanes (shared with the commit path: nz_skip is computed for this width)
 #define MMP_LANE_WIN 12
-#define MMP_CHUNK_WORDS 21  // decide_stream's per-lane chunk of 8 steps beyond the window (odd: conflict-free lane stride in shared memory)
+// decide_stream's per-lane slice of shared memory: the chunk of 8 steps beyond the window (21 words), then phase B's
+// checkpoints for phase C, MMP_LANE_WIN / 2 words of u16 window counts (27: odd, a conflict-free lane stride)
+#define MMP_CHUNK_WORDS 27
+typedef uint16_t mark16 __attribute__((may_alias));  // (the window counts are u16s in a slice of u32 words)
 struct LaneTables {
   const uint32_t *cx, *p;   // this decision's candidate (replicaset filter applied) and preferred mask rows, by absolute row word
   const uint32_t *full;
@@ -968,10 +971,13 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   // ---- beyond the window: a chunk of 8 consecutive steps [base, base + 8) in registers ----
   uint32_t base = 0xfffffff0u;  // no chunk loaded
   // chunk storage, MMP_CHUNK_WORDS words per lane: [0,4) the list entries (u16 pairs), [4,12) filtered words cx & ~row,
-  // [12,20) preferred words, [20] count classes against cls_lim (2 bits each).  The caller hands a shared-memory slice
-  // (dynamic indexing is one load); without one the array lives in local memory.
+  // [12,20) preferred words, [20] count classes against cls_lim (2 bits each), then phase B's checkpoints (mw below).
+  // The caller hands a shared-memory slice (dynamic indexing is one load); without one the array lives in local memory.
   uint32_t chunk_local[MMP_CHUNK_WORDS];
   uint32_t *ch = chunk ? chunk : chunk_local;
+  static_assert(MMP_CHUNK_WORDS >= 21 + MMP_LANE_WIN / 2, "slice too short for the checkpoints");
+  // mw[k]: members of S' phase B counted before window step k < MMP_LANE_WIN (at most 32 * MMP_LANE_WIN: a u16)
+  mark16 *const mw = reinterpret_cast<mark16 *>(ch + 21);
   int32_t cls_lim = 10;                             // the count limit the chunk's classes were computed for (phase B sets it and drops the chunk)
   auto wsel = [&](uint32_t j) -> uint32_t { return (ch[j >> 1] >> ((j & 1u) * 16u)) & 0xffffu; };
   auto refill = [&](uint32_t k) {
@@ -998,9 +1004,10 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   auto chunk_empty = [&]() -> bool { return (ch[4] | ch[5] | ch[6] | ch[7] | ch[8] | ch[9] | ch[10] | ch[11]) == 0u; };
   // One walk: BODY sees (K, wi, e) and sets go_ (true: next step).  WALKING is cleared when the lane stops: BODY said so, the
   // list ended (ENDED = true), or the budget / the reachable part of the row ran out (live = false).  CHARGE: the steps
-  // count against the budget (phase C re-walks words phase B has paid for).  BULK (beyond the window only): an expression
+  // count against the budget (phase C walks words phase B has paid for).  BULK (beyond the window only): an expression
   // that tries to take a freshly gathered chunk of 8 steps at once -- true: the 8 steps are done (its side effects are theirs).
-#define MMP_WALK(K, WALKING, ENDED, CHARGE, BULK, BODY)                                                                          \
+  // MARK_W: a statement run before a window step's BODY (phase B's checkpoints).
+#define MMP_WALK(K, WALKING, ENDED, CHARGE, BULK, MARK_W, BODY)                                                          \
   for (;;) { /* inside the window */                                                                                       \
     if (WALKING && K < win_words) {                                                                                        \
       if (CHARGE && left <= 0) { WALKING = false; live = false; }                                                          \
@@ -1008,6 +1015,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
         const uint32_t wi = WS + K, e = ewin[K];                                                                           \
         const TabWin &A = AW;                                                                                              \
         bool go_;                                                                                                          \
+        MARK_W;                                                                                                            \
         BODY;                                                                                                              \
         if (go_) { K++; if (CHARGE) left--; } else WALKING = false;                                                        \
       }                                                                                                                    \
@@ -1040,7 +1048,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   {
     uint32_t k = 0;
     bool walking = live, ended = false;
-    MMP_WALK(k, walking, ended, true, (!has_x && chunk_empty()), {
+    MMP_WALK(k, walking, ended, true, (!has_x && chunk_empty()), (void)0, {
       uint32_t x = A.cx(wi) & ~e;
       if (has_x) x &= ~xmask(wi);
       if (x) { b = wi * 32u + (uint32_t)ffs32(x); kb = k; }
@@ -1071,7 +1079,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
     const uint32_t b_w = b >> 5, m_b = mask_above(b_w * 32u, b);
     uint32_t k = kb;
     bool walking = live && !simple && !best_full, ended = false;
-    MMP_WALK(k, walking, ended, true, false, {
+    MMP_WALK(k, walking, ended, true, false, (void)0, {
       uint32_t x = A.cx(wi) & ~e & (A.p(wi) | A.full(wi));
       if (has_x) x &= ~xmask(wi);
       if (wi == b_w) x &= m_b;
@@ -1093,7 +1101,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
     bool pref_before = false;
     const bool case_b = live && !simple && best_full;
     bool walking = case_b, ended = false;
-    MMP_WALK(k, walking, ended, true, false, {
+    MMP_WALK(k, walking, ended, true, false, (void)0, {
       uint32_t x = A.cx(wi) & ~e;
       if (has_x) x &= ~xmask(wi);
       if (wi == b_w) x &= m_b;
@@ -1191,10 +1199,12 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
     n_in += n;
     return true;
   };
+  // checkpoints for phase C: n_in before every window step phase B takes (the first MMP_LANE_WIN)
+  uint32_t k_b = k_lo;  // where phase B stopped
   {
     uint32_t k = k_lo;
     bool walking = walk, ended = false;
-    MMP_WALK(k, walking, ended, true, (!has_x && chunk_plain() && bulk_b()), {
+    MMP_WALK(k, walking, ended, true, (!has_x && chunk_plain() && bulk_b()), if (k < MMP_LANE_WIN) mw[k] = (uint16_t)n_in, {
       go_ = true;
       if (wi >= stop_w) { ended = true; go_ = false; }  // the walk's natural end (everything at or beyond lim)
       else {
@@ -1217,6 +1227,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
       }
     })
     if (walk && live && ended && cut_others == NONE_RANK && lim == NONE_RANK && open_end) open = true;
+    k_b = k;
   }
   walk = walk && live && !open;
   const uint32_t cut = cut_others < cut_self ? cut_others : cut_self;
@@ -1250,14 +1261,31 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
       }
     }
   }
-  // ---- C: k-th survivor in rank order (re-walks words phase B has visited: the budget is not charged again) ----
+  // ---- C: k-th survivor in rank order, walked from the last checkpoint of phase B that lies before it (words phase B
+  // has visited: the budget is not charged again) ----
   {
     const bool drop_self = self_in_sl && !keep_self;
     const uint32_t cut_w = cut >> 5, m_cut = mask_below(cut_w * 32u, cut);
     uint32_t k = k_lo;
+    if (sel) {
+      // phase B counted self (a member of S') where phase C drops it: one fewer before every checkpoint past self's word
+      uint32_t n0 = 0;
+      const uint32_t mark_end = win_words < MMP_LANE_WIN ? win_words : MMP_LANE_WIN;  // (k_place_lanes: windows up to 20 words)
+      if (k_lo < mark_end) {  // the window steps phase B took and counted: [k_lo, min(k_b, mark_end - 1)], counts ascending from 0
+        uint32_t hi_k = k_b < mark_end ? k_b : mark_end - 1u;
+        while (k < hi_k) {
+          const uint32_t mid = (k + hi_k + 1u) >> 1;
+          const uint32_t n = (uint32_t)mw[mid] - ((drop_self && sw_ < WS + mid) ? 1u : 0u);
+          if (n <= kth) k = mid;
+          else hi_k = mid - 1u;
+        }
+        n0 = (uint32_t)mw[k] - ((drop_self && sw_ < WS + k) ? 1u : 0u);
+      }
+      kth -= n0;
+    }
     bool walking = sel, ended = false;
     auto bulk_c = [&]() -> bool { const uint32_t n = chunk_members(); if (kth < n) return false; kth -= n; return true; };
-    MMP_WALK(k, walking, ended, false, (!has_x && chunk_plain() && wsel(7) < cut_w && bulk_c()), {
+    MMP_WALK(k, walking, ended, false, (!has_x && chunk_plain() && wsel(7) < cut_w && bulk_c()), (void)0, {
       uint32_t x = Sw(A, wi, e);
       if (wi == cut_w) x &= m_cut;
       if (drop_self && wi == sw_) x &= ~sb_;
