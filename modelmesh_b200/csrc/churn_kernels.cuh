@@ -366,9 +366,8 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   LiveState &lv = f->live;
   const int32_t NI = f->hs.cfg.max_instances, NM = f->hs.n_models_used;
   const int32_t nF = cs.n_carry, Q = nF + n;
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   cudaEvent_t evs[8];
   for (auto &e : evs) CK(cudaEventCreate(&e));
   struct EvRel { cudaEvent_t *e; ~EvRel() { for (int i = 0; i < 8; i++) cudaEventDestroy(e[i]); } } evrel{evs};

@@ -295,6 +295,13 @@ class HostState {
     if (r.capacity < 0 || r.used < 0) return "capacity/used must be >= 0";
     return nullptr;
   }
+  // A caller's own instance record as the walk reads it (quirk N2): `out` is set when the row passes validate_row, whose
+  // message is returned otherwise.  Free space below zero reads as zero.
+  static const char *fresh_row(const mmp_instance_row &r, FreshRow &out) {
+    if (const char *m = validate_row(r)) return m;
+    out = FreshRow{r.lru_time, std::max<int64_t>(0, r.capacity - r.used), r.count, r.rpm};
+    return nullptr;
+  }
 
   int32_t intern_type(const std::string &name) {
     auto it = type_ids.find(name);

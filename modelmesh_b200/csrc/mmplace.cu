@@ -1280,10 +1280,26 @@ static PlaceCtx *acquire_ctx(mmp_fleet *f) {
   if (!ok) { delete c; return nullptr; }
   return c;
 }
-static void release_ctx(mmp_fleet *f, PlaceCtx *c) {
-  std::lock_guard<std::mutex> g(f->ctx_mu);
-  f->ctx_free.emplace_back(c);
-}
+// A PlaceCtx leased from the fleet's pool for the length of one call; it goes back to the pool when the lease goes out of
+// scope.  A lease is empty when a new context could not be created.
+class CtxLease {
+ public:
+  explicit CtxLease(mmp_fleet *f) : f_(f), c_(acquire_ctx(f)) {}
+  ~CtxLease() {
+    if (!c_) return;
+    std::lock_guard<std::mutex> g(f_->ctx_mu);
+    f_->ctx_free.emplace_back(c_);
+  }
+  CtxLease(const CtxLease &) = delete;
+  CtxLease &operator=(const CtxLease &) = delete;
+  explicit operator bool() const { return c_ != nullptr; }
+  PlaceCtx *operator->() const { return c_; }
+  PlaceCtx *get() const { return c_; }
+
+ private:
+  mmp_fleet *f_;
+  PlaceCtx *c_;
+};
 static void destroy_ctx(PlaceCtx *c) {
   for (DevBuf *b : {&c->d_in, &c->d_out, &c->d_fresh, &c->d_extra, &c->d_trace, &c->d_cand, &c->d_open_flag,
                     &c->d_open_idx, &c->d_n_open, &c->d_cub, &c->d_blocks, &c->d_gathered, &c->d_rows, &c->d_in_open, &c->d_out_open})
@@ -1317,7 +1333,6 @@ struct PlaceArgs {
   uint64_t seed, id_base;
   int emit_keys = 0;            // instance-sharded: write shard keys (uint64) into `out` instead of results
   const int32_t *orig_id = nullptr;  // gather pass: decision i reads row i of s.excl and hashes with id orig_id[i]
-  const int32_t *perm = nullptr;     // k_place_direct: position j of the launch resolves decision perm[j]
   struct PlaceCtx *ctx = nullptr;    // scratch for the slot sort (the call's own context)
   int sort_slot = 0;                 // ... which of its scratch sets (chunks in flight on different streams use different ones)
 };
@@ -1379,8 +1394,8 @@ static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
   if (!(a.tr || a.cand) && !a.emit_keys && !a.orig_id && f->direct && a.n > f->small_max && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words &&
       a.s.excl_ranks) {
     const int blocks = (a.n + 127) / 128;
-    const int32_t *perm = a.perm;
-    if (!perm && a.ctx && a.n >= 8192 && (f->sort_slots == 1 || (f->sort_slots == 2 && f->snaps[f->cur].sparse_slots))) {
+    const int32_t *perm = nullptr;  // k_place_direct: position j of the launch resolves decision perm[j]
+    if (a.ctx && a.n >= 8192 && (f->sort_slots == 1 || (f->sort_slots == 2 && f->snaps[f->cur].sparse_slots))) {
       PlaceCtx *c = a.ctx;  // slot order: key pass + 16-bit radix sort of the indices (a few tens of microseconds per million decisions)
       const int ss = a.sort_slot >= 0 && a.sort_slot < PlaceCtx::NSORT ? a.sort_slot : 0;
       cudaError_t e;
@@ -1578,6 +1593,54 @@ static int32_t place_sharded(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds
   k_shard_scatter<<<(n_open + 255) / 256, 256, 0, st>>>(c->d_out_open.as<mmp_decision_out>(), c->d_open_idx.as<int32_t>(), n_open, d_out);
   f->launches++;
   CK(cudaGetLastError());
+  return MMP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// the host side of a placement call: side tables, the sharded-or-not dispatch, the chunk pipeline
+// ---------------------------------------------------------------------------------------------------------------
+// Whether a call goes through place_sharded: always on an instance-sharded fleet, and for untraced calls on a fleet that
+// connected a communicator with one shard (a traced call there takes the unsharded traced kernel).
+static bool places_sharded(const mmp_fleet *f, bool traced) { return f->hs.cfg.shard_count > 1 || (f->comm && !traced); }
+
+// The call's fresh rows and extra excludes into d_fresh / d_extra on st.  Both buffers hold at least one entry, so the
+// kernels are given valid pointers when a call has none.
+static int32_t stage_side_tables(PlaceCtx *c, const FreshRow *fresh, int32_t n_fresh, const int32_t *extra, int32_t n_extra, cudaStream_t st) {
+  CK(c->d_fresh.ensure((size_t)std::max(n_fresh, 1) * sizeof(FreshRow)));
+  CK(c->d_extra.ensure((size_t)std::max(n_extra, 1) * 4));
+  if (n_fresh) CK(cudaMemcpyAsync(c->d_fresh.p, fresh, (size_t)n_fresh * sizeof(FreshRow), cudaMemcpyHostToDevice, st));
+  if (n_extra) CK(cudaMemcpyAsync(c->d_extra.p, extra, (size_t)n_extra * 4, cudaMemcpyHostToDevice, st));
+  return MMP_OK;
+}
+
+// Places the whole batch `a`, whose records, side tables and output are on the device, on stream st.  a.s.n_extra is the
+// size of the call's extra[] table.
+static int32_t place_on_device(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, const PlaceArgs &a, cudaStream_t st) {
+  const bool traced = a.tr || a.cand;
+  if (!places_sharded(f, traced)) { CK(launch_place(f, a, st)); return MMP_OK; }
+  if (traced) { g_err = "traces are not available on an instance-sharded fleet"; return MMP_E_STATE; }
+  return place_sharded(f, c, ds, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.s.n_extra, a.out, a.now, a.seed, st);
+}
+
+// A large unsharded, untraced batch in chunks: chunk i goes to stream pipe[i % NPIPE] with slot-sort scratch set
+// 1 + i % NPIPE, so that the H2D copy of chunk i+1, the kernel of chunk i and the D2H copy of chunk i-1 overlap (with
+// pinned caller buffers these are true DMA).  `a` is the whole batch, its records in c->d_in and its results in c->d_out;
+// the records are copied there chunk by chunk from `in` unless `in` is null.  Results go to `out` on the host.  Work
+// queued on c->stream before the call (the side tables, records built on the device) completes before the first chunk.
+static int32_t place_chunks(mmp_fleet *f, PlaceCtx *c, const PlaceArgs &a, int32_t chunk, const mmp_decision_in *in, mmp_decision_out *out) {
+  CK(cudaEventRecord(c->ready, c->stream));
+  for (int i = 0; i < PlaceCtx::NPIPE; i++) CK(cudaStreamWaitEvent(c->pipe[i], c->ready, 0));
+  int ci = 0;
+  for (int32_t lo = 0; lo < a.n; lo += chunk, ci++) {
+    cudaStream_t ps = c->pipe[ci % PlaceCtx::NPIPE];
+    PlaceArgs p = a;
+    p.in = a.in + lo; p.out = a.out + lo; p.n = std::min(chunk, a.n - lo);
+    p.id_base = a.id_base + (uint64_t)lo; p.sort_slot = 1 + ci % PlaceCtx::NPIPE;
+    if (in) CK(cudaMemcpyAsync(c->d_in.as<mmp_decision_in>() + lo, in + lo, (size_t)p.n * sizeof(mmp_decision_in), cudaMemcpyHostToDevice, ps));
+    CK(launch_place(f, p, ps));
+    CK(cudaMemcpyAsync(out + lo, p.out, (size_t)p.n * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, ps));
+  }
+  for (int i = 0; i < PlaceCtx::NPIPE; i++) CK(cudaStreamSynchronize(c->pipe[i]));
   return MMP_OK;
 }
 
@@ -2292,6 +2355,63 @@ static int32_t place_server(mmp_fleet *f, const DeviceSnapshot &ds, const mmp_de
   return MMP_OK;
 }
 
+// Tiny untraced, unsharded batches, zero-copy: the records, fresh rows (c->fresh_host) and extras are written into the
+// context's pinned mapped buffer, and the kernel reads them and writes its results there, so a call is one launch and one
+// synchronise with no copy calls.  The caller has checked that the batch fits the buffer.
+static int32_t place_mapped(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, const SnapshotView &vw, const mmp_decision_in *in, int32_t n,
+                            int32_t n_fresh, const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed) {
+  const bool fits32 = n <= 32 && n_fresh <= 32 && (size_t)n_extra <= 32 * MMP_MAX_EXTRA;
+  if (f->one_mode == 3 && fits32) {
+    std::unique_lock<std::mutex> lk(f->srv.mu, std::try_to_lock);
+    if (lk.owns_lock()) return place_server(f, ds, in, n, c->fresh_host.data(), n_fresh, extra, n_extra, out, now_ms, seed);
+  }  // (taken by another caller: this call goes the graph way)
+  // one 32-thread block as a replayed graph: the node's parameters are those of the epoch it was captured in (the snapshot
+  // view by value, the fixed offsets of a layout for 32 decisions behind a SmallHdr); what changes per call -- now, seed,
+  // id base, n -- is read from the header.  Other launches take the batch packed from offset 0.
+  const bool graph = f->one_mode >= 2 && fits32;
+  static_assert(64 + 32 * (sizeof(mmp_decision_in) + sizeof(mmp_decision_out) + sizeof(FreshRow)) + 32 * MMP_MAX_EXTRA * 4 <= PlaceCtx::MAPPED_BYTES, "mapped layout");
+  const size_t rows = graph ? 32 : (size_t)n;
+  const size_t o_in = graph ? 64 : 0, o_out = o_in + rows * sizeof(mmp_decision_in), o_fr = o_out + rows * sizeof(mmp_decision_out);
+  const size_t o_ex = graph ? o_fr + 32 * sizeof(FreshRow) : (o_fr + (size_t)n_fresh * sizeof(FreshRow) + 15) / 16 * 16;
+  unsigned char *h = c->mapped, *dbase = nullptr;
+  CK(cudaHostGetDevicePointer((void **)&dbase, h, 0));
+  memcpy(h + o_in, in, (size_t)n * sizeof(mmp_decision_in));
+  if (n_fresh) memcpy(h + o_fr, c->fresh_host.data(), (size_t)n_fresh * sizeof(FreshRow));
+  if (n_extra) memcpy(h + o_ex, extra, (size_t)n_extra * 4);
+  const mmp_decision_in *d_in = (const mmp_decision_in *)(dbase + o_in);
+  const FreshRow *d_fr = (const FreshRow *)(dbase + o_fr);
+  const int32_t *d_ex = (const int32_t *)(dbase + o_ex);
+  mmp_decision_out *d_out = (mmp_decision_out *)(dbase + o_out);
+  cudaStream_t st = c->stream;
+  if (graph) {
+    SmallHdr *hd = reinterpret_cast<SmallHdr *>(h);
+    hd->now = now_ms; hd->seed = seed; hd->id_base = f->id_base.load(); hd->n = n; hd->n_fresh = n_fresh; hd->n_extra = n_extra;
+    if (c->graph_epoch != f->epoch || !c->graph_exec) {
+      if (c->graph_exec) { cudaGraphExecDestroy(c->graph_exec); c->graph_exec = nullptr; }
+      if (c->graph) { cudaGraphDestroy(c->graph); c->graph = nullptr; }
+      SnapshotView gv = ds.view;
+      gv.n_extra = 32 * MMP_MAX_EXTRA;
+      CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+      k_place_small<<<1, 32, 0, st>>>(gv, d_in, 0, d_fr, 32, d_ex, d_out, 0, 0, 0, reinterpret_cast<const volatile SmallHdr *>(dbase), f->lane_budget);
+      CK(cudaStreamEndCapture(st, &c->graph));
+      CK(cudaGraphInstantiate(&c->graph_exec, c->graph, 0));
+      c->graph_epoch = f->epoch;
+    }
+    CK(cudaGraphLaunch(c->graph_exec, st));
+    f->launches++;
+  } else if (f->one_mode == 0 || n > 512) {
+    PlaceArgs a{vw, d_in, n, d_fr, n_fresh, d_ex, d_out, nullptr, nullptr, now_ms, seed, f->id_base.load()};
+    CK(launch_place(f, a, st));
+  } else {
+    k_place_small<<<(n + 31) / 32, 32, 0, st>>>(vw, d_in, n, d_fr, n_fresh, d_ex, d_out, now_ms, seed, f->id_base.load(), nullptr, f->lane_budget);
+    f->launches++;
+    CK(cudaGetLastError());
+  }
+  CK(cudaStreamSynchronize(st));
+  memcpy(out, h + o_out, (size_t)n * sizeof(mmp_decision_out));
+  return MMP_OK;
+}
+
 static int32_t place_impl(mmp_fleet *f, const mmp_decision_in *in, int32_t n, const mmp_instance_row *fresh, int32_t n_fresh,
                           const int32_t *extra, int32_t n_extra, mmp_decision_out *out, mmp_decision_trace *trace,
                           uint32_t *cand_mask, int64_t now_ms, uint64_t seed) {
@@ -2305,131 +2425,32 @@ static int32_t place_impl(mmp_fleet *f, const mmp_decision_in *in, int32_t n, co
   std::shared_lock<std::shared_mutex> rd(f->snap_mu);
   if (f->epoch == 0) { g_err = "no committed snapshot (call mmp_fleet_commit)"; return MMP_E_EPOCH; }
   const DeviceSnapshot &ds = f->snaps[f->cur];
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   c->fresh_host.resize((size_t)n_fresh);
-  for (int32_t i = 0; i < n_fresh; i++) {
-    if (const char *m = HostState::validate_row(fresh[i])) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
-    c->fresh_host[i] = FreshRow{fresh[i].lru_time, std::max<int64_t>(0, fresh[i].capacity - fresh[i].used), fresh[i].count, fresh[i].rpm};
-  }
+  for (int32_t i = 0; i < n_fresh; i++)
+    if (const char *m = HostState::fresh_row(fresh[i], c->fresh_host[i])) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
   const int RW = ds.view.row_words;
   cudaStream_t st = c->stream;
   const bool traced = trace || cand_mask;
+  const bool fast_paths = !traced && !places_sharded(f, traced);  // the mapped tiny-batch path and the chunk pipeline apply
   SnapshotView vw = ds.view;
   vw.n_extra = n_extra;  // per call: the device checks every decision's extra[] slice against it (prepare_ctx_a)
-  if (f->hs.cfg.shard_count > 1 || (f->comm && !traced)) {  // instance-sharded: keys, one all-reduce(min), decode (+ row gather for open walks)
-    if (traced) { g_err = "traces are not available on an instance-sharded fleet"; return MMP_E_STATE; }
-    CK(c->d_in.ensure((size_t)n * sizeof(mmp_decision_in)));
-    CK(c->d_out.ensure((size_t)n * sizeof(mmp_decision_out)));
-    CK(c->d_fresh.ensure((size_t)std::max(n_fresh, 1) * sizeof(FreshRow)));
-    CK(c->d_extra.ensure((size_t)std::max(n_extra, 1) * 4));
-    if (n_fresh) CK(cudaMemcpyAsync(c->d_fresh.p, c->fresh_host.data(), (size_t)n_fresh * sizeof(FreshRow), cudaMemcpyHostToDevice, st));
-    if (n_extra) CK(cudaMemcpyAsync(c->d_extra.p, extra, (size_t)n_extra * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_in.p, in, (size_t)n * sizeof(mmp_decision_in), cudaMemcpyHostToDevice, st));
-    int32_t rcs = place_sharded(f, c, ds, c->d_in.as<mmp_decision_in>(), n, c->d_fresh.as<FreshRow>(), n_fresh, c->d_extra.as<int32_t>(), n_extra,
-                                c->d_out.as<mmp_decision_out>(), now_ms, seed, st);
-    if (rcs < 0) return rcs;
-    CK(cudaMemcpyAsync(out, c->d_out.p, (size_t)n * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return MMP_OK;
-  }
-  // ---- tiny batches: zero-copy through pinned mapped memory (one launch + one synchronise) ----
-  {
-    const size_t need = (size_t)n * (sizeof(mmp_decision_in) + sizeof(mmp_decision_out)) + (size_t)n_fresh * sizeof(FreshRow) + (size_t)n_extra * 4 + 64;
-    if (!traced && need <= PlaceCtx::MAPPED_BYTES) {
-      if (f->one_mode == 3 && n <= 32 && n_fresh <= 32 && (size_t)n_extra <= 32 * MMP_MAX_EXTRA) {
-        std::unique_lock<std::mutex> lk(f->srv.mu, std::try_to_lock);
-        if (lk.owns_lock()) return place_server(f, ds, in, n, c->fresh_host.data(), n_fresh, extra, n_extra, out, now_ms, seed);
-      }  // (taken by another caller: this call goes the graph way)
-      unsigned char *h = c->mapped, *dbase = nullptr;
-      CK(cudaHostGetDevicePointer((void **)&dbase, h, 0));
-      size_t o_in = 0, o_out = o_in + (size_t)n * sizeof(mmp_decision_in), o_fr = o_out + (size_t)n * sizeof(mmp_decision_out);
-      size_t o_ex = (o_fr + (size_t)n_fresh * sizeof(FreshRow) + 15) / 16 * 16;
-      memcpy(h + o_in, in, (size_t)n * sizeof(mmp_decision_in));
-      if (n_fresh) memcpy(h + o_fr, c->fresh_host.data(), (size_t)n_fresh * sizeof(FreshRow));
-      if (n_extra) memcpy(h + o_ex, extra, (size_t)n_extra * 4);
-      if (f->one_mode == 0 || n > 512) {
-        PlaceArgs a{vw, (const mmp_decision_in *)(dbase + o_in), n, (const FreshRow *)(dbase + o_fr), n_fresh,
-                    (const int32_t *)(dbase + o_ex), (mmp_decision_out *)(dbase + o_out), nullptr, nullptr, now_ms, seed, f->id_base.load()};
-        CK(launch_place(f, a, st));
-      } else if (f->one_mode == 1 || n > 32 || n_fresh > 32 || (size_t)n_extra > 32 * MMP_MAX_EXTRA) {  // (the graph's mapped layout is laid out for 32 decisions)
-        k_place_small<<<(n + 31) / 32, 32, 0, st>>>(vw, (const mmp_decision_in *)(dbase + o_in), n, (const FreshRow *)(dbase + o_fr), n_fresh,
-                                                  (const int32_t *)(dbase + o_ex), (mmp_decision_out *)(dbase + o_out), now_ms, seed,
-                                                  f->id_base.load(), nullptr, f->lane_budget);
-        f->launches++;
-        CK(cudaGetLastError());
-      } else {
-        // one 32-thread block as a replayed graph: the node's parameters are those of the epoch it was captured in (the
-        // snapshot view by value, the fixed offsets of this context's mapped buffer laid out for 32 decisions); what changes
-        // per call -- now, seed, id base, n -- is read from the mapped header
-        const size_t g_in = 64, g_out = g_in + 32 * sizeof(mmp_decision_in), g_fr = g_out + 32 * sizeof(mmp_decision_out),
-                     g_ex = g_fr + 32 * sizeof(FreshRow);
-        static_assert(64 + 32 * (sizeof(mmp_decision_in) + sizeof(mmp_decision_out) + sizeof(FreshRow)) + 32 * MMP_MAX_EXTRA * 4 <= PlaceCtx::MAPPED_BYTES, "mapped layout");
-        SmallHdr *hd = reinterpret_cast<SmallHdr *>(h);
-        memmove(h + g_in, in, (size_t)n * sizeof(mmp_decision_in));  // (the generic layout above was filled first: move into the graph's)
-        if (n_fresh) memcpy(h + g_fr, c->fresh_host.data(), (size_t)n_fresh * sizeof(FreshRow));
-        if (n_extra) memcpy(h + g_ex, extra, (size_t)n_extra * 4);
-        hd->now = now_ms; hd->seed = seed; hd->id_base = f->id_base.load(); hd->n = n; hd->n_fresh = n_fresh; hd->n_extra = n_extra;
-        if (c->graph_epoch != f->epoch || !c->graph_exec) {
-          if (c->graph_exec) { cudaGraphExecDestroy(c->graph_exec); c->graph_exec = nullptr; }
-          if (c->graph) { cudaGraphDestroy(c->graph); c->graph = nullptr; }
-          SnapshotView gv = ds.view;
-          gv.n_extra = 32 * MMP_MAX_EXTRA;
-          CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-          k_place_small<<<1, 32, 0, st>>>(gv, (const mmp_decision_in *)(dbase + g_in), 0, (const FreshRow *)(dbase + g_fr), 32,
-                                        (const int32_t *)(dbase + g_ex), (mmp_decision_out *)(dbase + g_out), 0, 0, 0,
-                                        reinterpret_cast<const volatile SmallHdr *>(dbase), f->lane_budget);
-          CK(cudaStreamEndCapture(st, &c->graph));
-          CK(cudaGraphInstantiate(&c->graph_exec, c->graph, 0));
-          c->graph_epoch = f->epoch;
-        }
-        CK(cudaGraphLaunch(c->graph_exec, st));
-        f->launches++;
-        CK(cudaStreamSynchronize(st));
-        memcpy(out, h + g_out, (size_t)n * sizeof(mmp_decision_out));
-        return MMP_OK;
-      }
-      CK(cudaStreamSynchronize(st));
-      memcpy(out, h + o_out, (size_t)n * sizeof(mmp_decision_out));
-      return MMP_OK;
-    }
-  }
+  const size_t need = (size_t)n * (sizeof(mmp_decision_in) + sizeof(mmp_decision_out)) + (size_t)n_fresh * sizeof(FreshRow) + (size_t)n_extra * 4 + 64;
+  if (fast_paths && need <= PlaceCtx::MAPPED_BYTES) return place_mapped(f, c.get(), ds, vw, in, n, n_fresh, extra, n_extra, out, now_ms, seed);
   CK(c->d_in.ensure((size_t)n * sizeof(mmp_decision_in)));
   CK(c->d_out.ensure((size_t)n * sizeof(mmp_decision_out)));
-  CK(c->d_fresh.ensure((size_t)std::max(n_fresh, 1) * sizeof(FreshRow)));
-  CK(c->d_extra.ensure((size_t)std::max(n_extra, 1) * 4));
   if (trace) CK(c->d_trace.ensure((size_t)n * sizeof(mmp_decision_trace)));
   if (cand_mask) CK(c->d_cand.ensure((size_t)n * 2 * RW * 4));
-  if (n_fresh) CK(cudaMemcpyAsync(c->d_fresh.p, c->fresh_host.data(), (size_t)n_fresh * sizeof(FreshRow), cudaMemcpyHostToDevice, st));
-  if (n_extra) CK(cudaMemcpyAsync(c->d_extra.p, extra, (size_t)n_extra * 4, cudaMemcpyHostToDevice, st));
-  // ---- large untraced batches: chunks flow through NPIPE streams so that the H2D copy of chunk i+1, the kernel of
-  // chunk i and the D2H copy of chunk i-1 overlap (with pinned caller buffers these are true DMA) ----
-  const int32_t CHUNK = 1 << 17;
-  if (!traced && n > CHUNK) {
-    CK(cudaEventRecord(c->ready, st));  // fresh/extra tables uploaded
-    for (int i = 0; i < PlaceCtx::NPIPE; i++) CK(cudaStreamWaitEvent(c->pipe[i], c->ready, 0));
-    int ci = 0;
-    for (int32_t lo = 0; lo < n; lo += CHUNK, ci++) {
-      const int32_t cnt = std::min(CHUNK, n - lo);
-      cudaStream_t ps = c->pipe[ci % PlaceCtx::NPIPE];
-      CK(cudaMemcpyAsync(c->d_in.as<mmp_decision_in>() + lo, in + lo, (size_t)cnt * sizeof(mmp_decision_in), cudaMemcpyHostToDevice, ps));
-      PlaceArgs a{vw, c->d_in.as<mmp_decision_in>() + lo, cnt, c->d_fresh.as<FreshRow>(), n_fresh, c->d_extra.as<int32_t>(),
-                  c->d_out.as<mmp_decision_out>() + lo, nullptr, nullptr, now_ms, seed, f->id_base.load() + (uint64_t)lo};
-      a.ctx = c; a.sort_slot = 1 + ci % PlaceCtx::NPIPE;
-      CK(launch_place(f, a, ps));
-      CK(cudaMemcpyAsync(out + lo, c->d_out.as<mmp_decision_out>() + lo, (size_t)cnt * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, ps));
-    }
-    for (int i = 0; i < PlaceCtx::NPIPE; i++) CK(cudaStreamSynchronize(c->pipe[i]));
-    return MMP_OK;
-  }
-  CK(cudaMemcpyAsync(c->d_in.p, in, (size_t)n * sizeof(mmp_decision_in), cudaMemcpyHostToDevice, st));
-  if (cand_mask) CK(cudaMemsetAsync(c->d_cand.p, 0, (size_t)n * 2 * RW * 4, st));
+  if ((rc = stage_side_tables(c.get(), c->fresh_host.data(), n_fresh, extra, n_extra, st)) < 0) return rc;
   PlaceArgs a{vw, c->d_in.as<mmp_decision_in>(), n, c->d_fresh.as<FreshRow>(), n_fresh, c->d_extra.as<int32_t>(),
               c->d_out.as<mmp_decision_out>(), trace ? c->d_trace.as<mmp_decision_trace>() : nullptr,
               cand_mask ? c->d_cand.as<uint32_t>() : nullptr, now_ms, seed, f->id_base.load()};
-  a.ctx = c;
-  CK(launch_place(f, a, st));
+  a.ctx = c.get();
+  if (fast_paths && n > (1 << 17)) return place_chunks(f, c.get(), a, 1 << 17, in, out);
+  CK(cudaMemcpyAsync(c->d_in.p, in, (size_t)n * sizeof(mmp_decision_in), cudaMemcpyHostToDevice, st));
+  if (cand_mask) CK(cudaMemsetAsync(c->d_cand.p, 0, (size_t)n * 2 * RW * 4, st));
+  if ((rc = place_on_device(f, c.get(), ds, a, st)) < 0) return rc;
   CK(cudaMemcpyAsync(out, c->d_out.p, (size_t)n * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, st));
   if (trace) CK(cudaMemcpyAsync(trace, c->d_trace.p, (size_t)n * sizeof(mmp_decision_trace), cudaMemcpyDeviceToHost, st));
   if (cand_mask) CK(cudaMemcpyAsync(cand_mask, c->d_cand.p, (size_t)n * 2 * RW * 4, cudaMemcpyDeviceToHost, st));
@@ -2465,15 +2486,13 @@ int32_t mmp_place_sweep(mmp_fleet *f, int32_t first_model, int32_t n, const int3
   if (f->epoch == 0) { g_err = "no committed snapshot (call mmp_fleet_commit)"; return MMP_E_EPOCH; }
   const DeviceSnapshot &ds = f->snaps[f->cur];
   if ((int64_t)first_model + n > ds.n_models) { g_err = "sweep runs past the registry"; return MMP_E_ARG; }
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   cudaStream_t st = c->stream;
   const size_t n_self = self_stride ? (size_t)n : 1, n_fav = favour_bits ? ((size_t)n + 31) / 32 : 0;
   CK(c->d_in.ensure((size_t)n * sizeof(mmp_decision_in)));
   CK(c->d_out.ensure((size_t)n * sizeof(mmp_decision_out)));
-  CK(c->d_fresh.ensure(sizeof(FreshRow)));
-  CK(c->d_extra.ensure(4));
+  if ((rc = stage_side_tables(c.get(), nullptr, 0, nullptr, 0, st)) < 0) return rc;
   CK(c->d_trace.ensure(n_self * 4 + n_fav * 4 + 16));  // scratch: self[] then favour bits
   int32_t *d_self = c->d_trace.as<int32_t>();
   uint32_t *d_fav = n_fav ? reinterpret_cast<uint32_t *>(d_self + n_self) : nullptr;
@@ -2482,29 +2501,14 @@ int32_t mmp_place_sweep(mmp_fleet *f, int32_t first_model, int32_t n, const int3
   k_expand_sweep<<<(n + 255) / 256, 256, 0, st>>>(c->d_in.as<mmp_decision_in>(), n, first_model, d_self, self_stride, d_fav);
   f->launches++;
   CK(cudaGetLastError());
-  if (f->hs.cfg.shard_count > 1 || f->comm) {
-    int32_t rcs = place_sharded(f, c, ds, c->d_in.as<mmp_decision_in>(), n, c->d_fresh.as<FreshRow>(), 0, c->d_extra.as<int32_t>(), 0,
-                                c->d_out.as<mmp_decision_out>(), now_ms, seed, st);
-    if (rcs < 0) return rcs;
-    CK(cudaMemcpyAsync(out, c->d_out.p, (size_t)n * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    return MMP_OK;
-  }
-  // chunks: the results of chunk k travel to the host while chunk k + 1 is scored
-  const int32_t CHUNK = 1 << 18;
-  CK(cudaEventRecord(c->ready, st));
-  for (int i = 0; i < PlaceCtx::NPIPE; i++) CK(cudaStreamWaitEvent(c->pipe[i], c->ready, 0));
-  int ci = 0;
-  for (int32_t lo = 0; lo < n; lo += CHUNK, ci++) {
-    const int32_t cnt = std::min(CHUNK, n - lo);
-    cudaStream_t ps = c->pipe[ci % PlaceCtx::NPIPE];
-    PlaceArgs a{ds.view, c->d_in.as<mmp_decision_in>() + lo, cnt, c->d_fresh.as<FreshRow>(), 0, c->d_extra.as<int32_t>(),
-                c->d_out.as<mmp_decision_out>() + lo, nullptr, nullptr, now_ms, seed, f->id_base.load() + (uint64_t)lo};
-    a.ctx = c; a.sort_slot = 1 + ci % PlaceCtx::NPIPE;
-    CK(launch_place(f, a, ps));
-    CK(cudaMemcpyAsync(out + lo, c->d_out.as<mmp_decision_out>() + lo, (size_t)cnt * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, ps));
-  }
-  for (int i = 0; i < PlaceCtx::NPIPE; i++) CK(cudaStreamSynchronize(c->pipe[i]));
+  PlaceArgs a{ds.view, c->d_in.as<mmp_decision_in>(), n, c->d_fresh.as<FreshRow>(), 0, c->d_extra.as<int32_t>(),
+              c->d_out.as<mmp_decision_out>(), nullptr, nullptr, now_ms, seed, f->id_base.load()};
+  a.ctx = c.get();
+  // unsharded: the results of chunk k travel to the host while chunk k + 1 is scored
+  if (!places_sharded(f, false)) return place_chunks(f, c.get(), a, 1 << 18, nullptr, out);
+  if ((rc = place_on_device(f, c.get(), ds, a, st)) < 0) return rc;
+  CK(cudaMemcpyAsync(out, c->d_out.p, (size_t)n * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   return MMP_OK;
 }
 
@@ -2516,20 +2520,14 @@ int32_t mmp_place_batch_device(mmp_fleet *f, const void *d_in, int32_t n, void *
   std::shared_lock<std::shared_mutex> rd(f->snap_mu);
   if (f->epoch == 0) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
   const DeviceSnapshot &ds = f->snaps[f->cur];
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
-  CK(c->d_fresh.ensure(sizeof(FreshRow)));
-  CK(c->d_extra.ensure(4));
+  if ((rc = stage_side_tables(c.get(), nullptr, 0, nullptr, 0, c->stream)) < 0) return rc;
   PlaceArgs a{ds.view, (const mmp_decision_in *)d_in, n, c->d_fresh.as<FreshRow>(), 0, c->d_extra.as<int32_t>(),
               (mmp_decision_out *)d_out, nullptr, nullptr, now_ms, seed, f->id_base.load()};
-  a.ctx = c;
+  a.ctx = c.get();
   CK(cudaEventRecord(c->e0, c->stream));
-  if (f->hs.cfg.shard_count > 1 || f->comm) {
-    int32_t rcs = place_sharded(f, c, ds, (const mmp_decision_in *)d_in, n, c->d_fresh.as<FreshRow>(), 0, c->d_extra.as<int32_t>(), 0,
-                                (mmp_decision_out *)d_out, now_ms, seed, c->stream);
-    if (rcs < 0) return rcs;
-  } else CK(launch_place(f, a, c->stream));
+  if ((rc = place_on_device(f, c.get(), ds, a, c->stream)) < 0) return rc;
   CK(cudaEventRecord(c->e1, c->stream));
   CK(cudaEventSynchronize(c->e1));
   if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, c->e0, c->e1));

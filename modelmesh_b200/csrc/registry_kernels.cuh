@@ -205,9 +205,8 @@ int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mm
   if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
   const DeviceSnapshot &ds = f->snaps[f->cur];
   LiveState &lv = f->live;
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   cudaStream_t st = c->stream;
   const int np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks, nt = lv.n_type_ids;
   const size_t acc_bytes = (size_t)(np + 1) * sizeof(StatsAcc) + 8;
@@ -259,9 +258,8 @@ int32_t mmp_registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_t a
   LiveState &lv = f->live;
   const int32_t nm = f->hs.n_models_used, NI = f->hs.cfg.max_instances;
   if (nm == 0) return 0;
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   cudaStream_t st = c->stream;
   CK(c->d_in.ensure((size_t)NI * 8)); CK(c->d_out.ensure((size_t)std::max(cap, 1) * 4)); CK(c->d_extra.ensure((size_t)std::max(cap, 1)));
   CK(c->d_n_open.ensure(16));

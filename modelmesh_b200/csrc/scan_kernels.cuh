@@ -52,9 +52,8 @@ struct StatsResult {
 static int32_t run_stats(mmp_fleet *f, const DeviceSnapshot &ds, StatsResult &res) {
   const HostSnapshot &h = ds.host;
   const int np = (int)h.part_types.size();
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   size_t bytes = (size_t)(np + 1) * sizeof(StatsAcc) + 8;
   CK(c->d_trace.ensure(bytes));
   CK(cudaMemsetAsync(c->d_trace.p, 0, bytes, c->stream));
@@ -180,9 +179,8 @@ static int32_t reaper_impl(mmp_fleet *f, int32_t partition, int64_t now, uint8_t
       if (tid >= 0 && tid < (int32_t)excl.size()) excl[tid] = 1;
   const int nm = ds.n_models;
   if (nm == 0) return 0;
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   cudaStream_t s = c->stream;
   // Registry sweep -> candidates compacted in model order (stable) -> radix sort by ~lastUsed (stable: equal times keep the
   // lower model index first) -> first of every equal-time run (N12) -> only the first `total_count` survivors leave the device.
@@ -615,9 +613,8 @@ static int32_t lru_apply_impl(mmp_fleet *f, const mmp_lru_event *ev, int32_t n, 
   }
   for (int i = 0; i < f->lru_n; i++) off[i + 1] += off[i];
   { std::vector<int> pos(off.begin(), off.end() - 1); for (int32_t i = 0; i < n; i++) order[pos[ev[i].instance]++] = i; }
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   cudaStream_t s = c->stream;
   CK(c->d_in.ensure((size_t)n * sizeof(LruEv)));
   CK(c->d_extra.ensure((size_t)n * 4));
@@ -672,9 +669,8 @@ int32_t mmp_lru_state(mmp_fleet *f, int32_t n, int64_t *oldest, int64_t *weighte
   int32_t rc = set_device(f);
   if (rc < 0) return rc;
   std::lock_guard<std::mutex> g(f->ingest_mu);
-  PlaceCtx *c = acquire_ctx(f);
+  CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  struct Rel { mmp_fleet *f; PlaceCtx *c; ~Rel() { release_ctx(f, c); } } rel{f, c};
   CK(c->d_in.ensure((size_t)n * 8)); CK(c->d_out.ensure((size_t)n * 8)); CK(c->d_extra.ensure((size_t)n * 4));
   k_lru_state<<<(n + 3) / 4, 128, 0, c->stream>>>(lru_view(f), c->d_in.as<long long>(), c->d_out.as<long long>(), c->d_extra.as<int>());
   f->launches++;

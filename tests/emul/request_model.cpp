@@ -27,10 +27,8 @@ int32_t mmp_emul_place_request(mmp_fleet *f, const mmp_decision_in *in, int32_t 
   v.excl_ranks = sharded ? nullptr : ranks.data();
   v.n_extra = n_extra;
   std::vector<FreshRow> fr((size_t)(n_fresh > 0 ? n_fresh : 0));
-  for (int32_t i = 0; i < n_fresh; i++) {
-    if (const char *m = HostState::validate_row(fresh[i])) { g_err = m; return MMP_E_ARG; }
-    fr[i] = FreshRow{fresh[i].lru_time, std::max<int64_t>(0, fresh[i].capacity - fresh[i].used), fresh[i].count, fresh[i].rpm};
-  }
+  for (int32_t i = 0; i < n_fresh; i++)
+    if (const char *m = HostState::fresh_row(fresh[i], fr[i])) { g_err = m; return MMP_E_ARG; }
   const uint32_t ww = (uint32_t)std::min<int64_t>(window, v.row_words);
   Coop1 co;
   for (int32_t i = 0; i < n; i++) {

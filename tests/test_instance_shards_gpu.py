@@ -149,12 +149,29 @@ def test_sharded_matches_unsharded(product_lib, world):
 @pytest.mark.gpu
 def test_single_shard_takes_the_collective_path(product_lib, oracle_lib):
     """One GPU: a fleet of ONE shard that connects (ncclCommInitRank with one rank) sends its batches through the same
-    keys -> ncclAllReduce(min) -> decode path as a sharded fleet, over whole rows.  Results must equal the plain path's
-    (and the oracle's), including decisions the lane routine hands to the cooperative routine."""
+    keys -> ncclAllReduce(min) -> decode path as a sharded fleet, over whole rows, from each of the three batch entry
+    points (mmp_place_batch, mmp_place_sweep, mmp_place_batch_device).  Results must equal the plain path's (and the
+    oracle's), including decisions the lane routine hands to the cooperative routine."""
+    import ctypes as C
     import sys
     sys.path.insert(0, os.path.dirname(__file__))
     from helpers import oracle_from_synth, oracle_inputs_fast
+    from modelmesh_b200._lib import DECISION_OUT, DF_FAVOUR_SELF
     from modelmesh_b200.fleet import Fleet
+
+    def place_batch_device(fleet, dec):
+        dec = np.ascontiguousarray(dec)
+        d_in, d_out = C.c_void_p(), C.c_void_p()
+        fleet._ck(product_lib.mmp_device_alloc(fleet.h, dec.nbytes, C.byref(d_in)))
+        fleet._ck(product_lib.mmp_device_alloc(fleet.h, len(dec) * DECISION_OUT.itemsize, C.byref(d_out)))
+        fleet._ck(product_lib.mmp_device_upload(fleet.h, d_in, dec.ctypes.data_as(C.c_void_p), dec.nbytes))
+        ms = C.c_float()
+        fleet._ck(product_lib.mmp_place_batch_device(fleet.h, d_in, len(dec), d_out, fl.now_ms, 77, C.byref(ms)))
+        got = np.zeros(len(dec), dtype=DECISION_OUT)
+        fleet._ck(product_lib.mmp_device_download(fleet.h, got.ctypes.data_as(C.c_void_p), d_out, got.nbytes))
+        fleet._ck(product_lib.mmp_device_free(fleet.h, d_in)); fleet._ck(product_lib.mmp_device_free(fleet.h, d_out))
+        return got
+
     for config, nm, ni, seed in [("C3", 40_000, 10_000, 3), ("C5", 3000, 5000, 5), ("MIX", 500, 300, 14)]:
         fl = make_fleet(config, nm, ni, seed)
         plain_f = Fleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, fl.n_instances, fl.n_models, lib=product_lib)
@@ -168,6 +185,12 @@ def test_single_shard_takes_the_collective_path(product_lib, oracle_lib):
             want = plain_f.place_batch(sd.dec, fl.now_ms, 77, **kw)
             got = f.place_batch(sd.dec, fl.now_ms, 77, **kw)
             assert np.array_equal(got, want)
+            if plain:  # a registry sweep, and records that are already on the device
+                fav = (sd.dec["flags"] & DF_FAVOUR_SELF) != 0
+                assert np.array_equal(f.place_sweep(0, len(sd.dec), sd.dec["self"], fl.now_ms, 77, favour=fav),
+                                      plain_f.place_sweep(0, len(sd.dec), sd.dec["self"], fl.now_ms, 77, favour=fav))
+                assert np.array_equal(place_batch_device(f, sd.dec), want)
+                assert np.array_equal(place_batch_device(plain_f, sd.dec), want)
         assert f.shard_open_decisions() == 0  # a single shard's range is the whole row: no walk can leave it
         o = oracle_from_synth(fl)
         od, off, idx = oracle_inputs_fast(fl, sd)

@@ -81,7 +81,8 @@ def test_baseline_sized_fleets_match_oracle(product_lib, oracle_lib, config, nm,
 
 def test_batch_properties(product_lib, oracle_lib):
     """Size-independent properties of the batched entry points on a 10k-instance fleet: a batch is idempotent; a batch
-    equals its slices placed separately with mmp_fleet_set_id_base (what a registry shard does); the device-resident
+    equals its slices placed separately with mmp_fleet_set_id_base (what a registry shard does), also when it is large
+    enough to be pipelined in chunks and carries fresh rows and extra excludes; the device-resident
     entry point equals the host one; a one-decision call equals the batch's entry."""
     import ctypes as C
     from modelmesh_b200._lib import DECISION_OUT
@@ -100,6 +101,17 @@ def test_batch_properties(product_lib, oracle_lib):
         parts.append(s.place_batch(sd.dec[lo:hi], fl.now_ms, 5))
     s._ck(lib.mmp_fleet_set_id_base(s.h, 0))
     assert np.array_equal(np.concatenate(parts), a)
+    # a batch with fresh rows and extra excludes that spans two pipelined chunks (131 072 decisions each) equals its slices
+    big = make_decisions(fl, 200_000, 10)
+    kw = dict(fresh=big.fresh, extra=big.extra)
+    whole = s.place_batch(big.dec, fl.now_ms, 5, **kw)
+    parts = []
+    for lo, hi in ((0, 70_000), (70_000, 131_077), (131_077, 200_000)):
+        s._ck(lib.mmp_fleet_set_id_base(s.h, lo))
+        parts.append(s.place_batch(big.dec[lo:hi], fl.now_ms, 5, **kw))
+    s._ck(lib.mmp_fleet_set_id_base(s.h, 0))
+    assert len(big.fresh) and len(big.extra) and (whole["target"] >= 0).any()
+    assert np.array_equal(np.concatenate(parts), whole)
     # device-resident entry point
     d_in, d_out = C.c_void_p(), C.c_void_p()
     dec = np.ascontiguousarray(sd.dec)
