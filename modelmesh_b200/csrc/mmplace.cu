@@ -354,7 +354,7 @@ struct LaneLayout {
     ns = (uint32_t)ns_; warps = (uint32_t)warps_;
     off_bar = ns * stage_bytes; off_busy = off_bar + ns * 8u; off_uses = off_busy + ns * 4u;
     off_warp = (off_uses + ns * 4u + 127u) / 128u * 128u;
-    per_warp = 32u * LANE_STRIDE * 4u + (uint32_t)((sizeof(DecisionCtx) + 15) / 16 * 16);
+    per_warp = 32u * (LANE_STRIDE + MMP_CHUNK_WORDS) * 4u + (uint32_t)((sizeof(DecisionCtx) + 15) / 16 * 16);
     off_cx = (off_warp + warps * per_warp + 15u) / 16u * 16u;
     off_p = off_cx + LANE_SLOTS * LANE_WIN * 4u;
     off_full = off_p + LANE_SLOTS * LANE_WIN * 4u;
@@ -384,7 +384,8 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
   int *ticket = reinterpret_cast<int *>(smem_raw + lay.off_busy);               // next stage ticket of this block
   uint32_t *released = reinterpret_cast<uint32_t *>(smem_raw + lay.off_uses);  // [ns] completed uses per stage
   uint32_t *win = reinterpret_cast<uint32_t *>(smem_raw + lay.off_warp + (size_t)wib * lay.per_warp);  // [32][LANE_STRIDE]
-  DecisionCtx *ctx_one = reinterpret_cast<DecisionCtx *>(win + 32 * LANE_STRIDE);
+  uint32_t *chunk = win + 32 * LANE_STRIDE;                                                             // [32][MMP_CHUNK_WORDS]
+  DecisionCtx *ctx_one = reinterpret_cast<DecisionCtx *>(chunk + 32 * MMP_CHUNK_WORDS);
   if (threadIdx.x == 0) {
     for (int k = 0; k < ns; k++) { mbar_init(&bars[k], 32); released[k] = 0; }
     *ticket = 0;
@@ -536,7 +537,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
     }
     if ((mode & 1) == 0)
       handled = decide_stream(s, Tw, T, c, valid && !skip, win + lane * LANE_STRIDE, win_words, RowPtr{excl_row(s, m), (uint32_t)s.word_lo}, self_eword,
-                              now, seed, my_id, WarpVote(), o, budget);
+                              now, seed, my_id, WarpVote(), o, budget, chunk + lane * MMP_CHUNK_WORDS);
     else { o.target = (int32_t)(self_eword & 1u) - 1; o.n_candidates = 0; }  // MMP_LANE_MODE=1: stream-only probe (no decisions)
     // ---- what the lane routine declined: the whole warp redoes it, reading the row from global memory (L2) ----
     uint32_t pending = __ballot_sync(0xffffffffu, valid && !skip && !handled);
@@ -603,8 +604,8 @@ __device__ __forceinline__ void place_small_block(const SnapshotView &s, const m
   DecideOut o;
   const uint64_t my_id = pick_id(d, id_base + (uint64_t)i);
   __shared__ uint32_t chunk_b[32 * MMP_CHUNK_WORDS];  // (callers are one-warp blocks)
-  const bool handled = decide_stream(s, T, T, c, valid, nullptr, 0u, RowPtr{row, (uint32_t)s.word_lo}, self_eword, now, seed, my_id, WarpVote(), o, budget,
-                                     chunk_b + lane * MMP_CHUNK_WORDS);
+  const bool handled = decide_stream<TabGlob>(s, T, T, c, valid, nullptr, 0u, RowPtr{row, (uint32_t)s.word_lo}, self_eword,
+                                              now, seed, my_id, WarpVote(), o, budget, chunk_b + lane * MMP_CHUNK_WORDS);
   uint32_t pending = __ballot_sync(0xffffffffu, valid && !handled);
   while (pending) {
     const int l = __ffs((int)pending) - 1;
@@ -700,6 +701,8 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
   const bool ovf = valid && row.overflow();
   const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
   const uint32_t self_eword = c.self_rank >= 0 ? row.word((uint32_t)c.self_rank >> 5) : 0u;
+  // the window's words go to the warp's window buffer (one shared-memory load per window step: rebuilding each word from
+  // the ranks at every step measured slower), its tables are the snapshot's own (global memory: the read-only path)
   uint32_t *w = win_s[warp] + lane * LANE_STRIDE;
 #pragma unroll
   for (int j = 0; j < LANE_WIN; j++) w[j] = 0u;
@@ -712,8 +715,8 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
   const LaneTables T = lane_tables_global(s, c.slot >= 0 ? ctx_slot(c) : 0);
   DecideOut o;
   const uint64_t my_id = pick_id(d, id_base + (uint64_t)i);
-  const bool handled = decide_stream(s, T, T, c, valid && !ovf, w, win_words, row, self_eword, now, seed, my_id, WarpVote(), o, budget,
-                                     chunk_s[warp] + lane * MMP_CHUNK_WORDS);
+  const bool handled = decide_stream<TabGlob>(s, T, T, c, valid && !ovf, w, win_words, row, self_eword, now, seed, my_id, WarpVote(), o, budget,
+                                              chunk_s[warp] + lane * MMP_CHUNK_WORDS);
   uint32_t pending = __ballot_sync(0xffffffffu, valid && (ovf || !handled));
   while (pending) {
     const int l = __ffs((int)pending) - 1;
@@ -961,8 +964,8 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_dealt(const Snapshot
   DecideOut o;
   o.target = MMP_TARGET_NONE; o.n_candidates = 0;
   const uint64_t my_id = pick_id(d, id_base + (uint64_t)i);
-  const bool handled = decide_stream(s, T, T, c, valid, w, win_words < (uint32_t)LANE_WIN ? 0u : win_words, row, self_eword, now, seed, my_id, WarpVote(), o, budget,
-                                     chunk_d[warp] + lane * MMP_CHUNK_WORDS);
+  const bool handled = decide_stream<TabGlob>(s, T, T, c, valid, w, win_words < (uint32_t)LANE_WIN ? 0u : win_words, row, self_eword, now, seed, my_id,
+                                              WarpVote(), o, budget, chunk_d[warp] + lane * MMP_CHUNK_WORDS);
   uint32_t pending = __ballot_sync(0xffffffffu, valid && !handled);
   while (pending) {  // the cooperative general routine over the whole row, assembled in shared memory
     const int l = __ffs((int)pending) - 1;
@@ -1235,7 +1238,7 @@ struct mmp_fleet {
   } srv;
   int sort_slots = 2;           // MMP_SORT_SLOTS = 0 never | 1 always | 2 (default) when the snapshot's candidate sets are sparse: k_place_direct
                                 // resolves a large batch in type-slot order
-  int direct = 1, direct_minb = 6;  // MMP_KERNEL=direct: k_place_direct (no landing stages); MMP_DIRECT_MINB = 4 | 6 | 8 resident blocks per SM
+  int direct = 1, direct_minb = 5;  // MMP_KERNEL=direct: k_place_direct (no landing stages); MMP_DIRECT_MINB = 4 | 5 | 6 | 8 resident blocks per SM
   int small_max = 0;            // MMP_SMALL_MAX: untraced batches of up to this many decisions run on k_place_small (no landing stages:
                                 // one wave of 32-thread blocks), larger ones on the streaming kernel
   int lane_budget = LANE_BUDGET;  // MMP_LANE_BUDGET: walk steps per lane before a decision is handed to the whole warp
@@ -1411,7 +1414,7 @@ static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
     }
     int minb = f->direct_minb;
     if (minb == 6 && blocks > f->sm_count * 6 && blocks <= f->sm_count * 8) minb = 8;  // a launch of 1.0 .. 1.33 waves at 6 blocks per SM fits ONE wave at 8
-    auto kern = minb == 8 ? k_place_direct<4, 8> : (minb == 6 ? k_place_direct<4, 6> : k_place_direct<4, 4>);
+    auto kern = minb == 8 ? k_place_direct<4, 8> : minb == 6 ? k_place_direct<4, 6> : minb == 5 ? k_place_direct<4, 5> : k_place_direct<4, 4>;
     kern<<<blocks, 128, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, f->lane_budget, perm);
     f->launches++;
     return cudaGetLastError();
@@ -1836,7 +1839,7 @@ int32_t mmp_fleet_create(const mmp_config *cfg, mmp_fleet **out) {
   if (const char *t = getenv("MMP_ONE")) f->one_mode = !strcmp(t, "lanes") ? 0 : (!strcmp(t, "small") ? 1 : (!strcmp(t, "server") ? 3 : 2));
   if (const char *t = getenv("MMP_COMMIT")) f->commit_host_only = strcmp(t, "host") == 0;
   if (const char *t = getenv("MMP_SORT_SLOTS")) { int v = atoi(t); if (v >= 0 && v <= 2) f->sort_slots = v; }
-  if (const char *t = getenv("MMP_DIRECT_MINB")) { int v = atoi(t); f->direct_minb = v == 8 ? 8 : (v == 6 ? 6 : 4); }
+  if (const char *t = getenv("MMP_DIRECT_MINB")) { int v = atoi(t); f->direct_minb = v == 8 ? 8 : v == 6 ? 6 : v == 5 ? 5 : 4; }
   if (const char *t = getenv("MMP_SMALL_MAX")) { int v = atoi(t); if (v >= 0) f->small_max = v; }
   if (const char *t = getenv("MMP_LANE_BUDGET")) { int v = atoi(t); if (v >= 1 && v <= 4096) f->lane_budget = v; }
   if (const char *t = getenv("MMP_SHARD_CHUNKS")) f->shard_chunks = atoi(t);

@@ -794,14 +794,17 @@ MMP_HD WordSumI ldro_sum(const WordSumI *p) {
 #endif
 }
 
-// how the lane routine reads its tables: inside the window through plain loads (k_place_lanes points them at shared-memory
-// copies of the tables' window part), beyond it through the read-only path from the snapshot's own arrays
+// how the lane routine reads its tables: beyond the window through the read-only path from the snapshot's own arrays
+// (TabGlob); inside the window through plain loads (TabWin) where the caller points them at shared-memory copies of the
+// tables' window part (k_place_lanes, k_place_server), or through TabGlob too where its window tables are the global ones
 struct TabWin {
   const LaneTables &t;
   MMP_HD uint32_t cx(uint32_t wi) const { return t.cx[wi]; }
   MMP_HD uint32_t p(uint32_t wi) const { return t.p[wi]; }
   MMP_HD uint32_t full(uint32_t wi) const { return t.full[wi]; }
   MMP_HD WordSumI csum(uint32_t wi) const { return t.csum[wi]; }
+  MMP_HD RankRow row(uint32_t r) const { return load_row_any(t.rows + r); }
+  MMP_HD int32_t idx(uint32_t r) const { return t.rows[r].idx; }
   // count test of a whole word against lim: 0 no rank reaches it, 1 every rank does, 2 mixed (look at the 32 counts)
   MMP_HD int cls(uint32_t wi, int32_t lim) const { const WordSumI m = t.csum[wi]; return m.hi < lim ? 0 : (m.lo >= lim ? 1 : 2); }
   MMP_HD uint32_t ge_mask(uint32_t wi, int32_t lim) const {  // bit j: count of rank wi*32 + j >= lim (32 counts, zero-padded past the last rank)
@@ -826,6 +829,8 @@ struct TabGlob {
   MMP_HD uint32_t p(uint32_t wi) const { return ldro(t.p + wi); }
   MMP_HD uint32_t full(uint32_t wi) const { return ldro(t.full + wi); }
   MMP_HD WordSumI csum(uint32_t wi) const { return ldro_sum(t.csum + wi); }
+  MMP_HD RankRow row(uint32_t r) const { return load_row(t.rows + r); }
+  MMP_HD int32_t idx(uint32_t r) const { return ldro(&t.rows[r].idx); }
   MMP_HD int cls(uint32_t wi, int32_t lim) const { const WordSumI m = ldro_sum(t.csum + wi); return m.hi < lim ? 0 : (m.lo >= lim ? 1 : 2); }
   MMP_HD uint32_t ge_mask(uint32_t wi, int32_t lim) const {
     uint32_t vm = 0;
@@ -937,7 +942,10 @@ struct WarpVote { MMP_D bool any(bool p) const { return __any_sync(0xffffffffu, 
 // a walk of more than `budget` steps.  Instance-sharded: a walk that needs ranks beyond this shard's range sets MMP_TF_OPEN.
 // self_eword = the row word that holds self's bit (anywhere in the row).  Must be called by every lane of the vote group
 // (active = false for lanes without a decision).
-template <class V, class R>
+// AWT: how the window's tables Tw are read -- TabWin (plain loads: Tw points at shared memory) or TabGlob (Tw is global).
+// chunk: the lane's shared-memory slice of MMP_CHUNK_WORDS words; every kernel passes one (only the CPU harness may leave
+// it out).
+template <class AWT = TabWin, class V, class R>
 MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const LaneTables &T, const DecisionCtx &c, bool active,
                           const uint32_t *ewin, uint32_t win_words, const R &row, uint32_t self_eword, int64_t now, uint64_t seed,
                           uint64_t decision_id, const V &vote, DecideOut &o, int32_t budget, uint32_t *chunk = nullptr) {
@@ -952,7 +960,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   const uint32_t kz = win_words == 0 ? 0u : T.nz_skip;  // (the caller's window is the one nz_skip was counted for)
   const uint32_t koff = kz - win_words;                 // (mod 2^32)
   const uint32_t NZ = win_words + (T.nz_n - kz);        // virtual length of the walk
-  const TabWin AW{Tw};
+  const AWT AW{Tw};
   const TabGlob AG{T};
   const uint32_t win_end = WS + win_words;
   const bool favour_self = (d.flags & MMP_DF_FAVOUR_SELF) != 0;
@@ -967,14 +975,19 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
     return m;
   };
   auto pbit = [&](uint32_t r) -> bool { const uint32_t w = r >> 5; return ((w < win_end ? AW.p(w) : AG.p(w)) >> (r & 31)) & 1u; };
-  auto row_of = [&](uint32_t r) -> RankRow { return (r >> 5) < win_end ? load_row_any(Tw.rows + r) : load_row(T.rows + r); };
+  auto row_of = [&](uint32_t r) -> RankRow { return (r >> 5) < win_end ? AW.row(r) : AG.row(r); };
   // ---- beyond the window: a chunk of 8 consecutive steps [base, base + 8) in registers ----
   uint32_t base = 0xfffffff0u;  // no chunk loaded
   // chunk storage, MMP_CHUNK_WORDS words per lane: [0,4) the list entries (u16 pairs), [4,12) filtered words cx & ~row,
   // [12,20) preferred words, [20] count classes against cls_lim (2 bits each), then phase B's checkpoints (mw below).
-  // The caller hands a shared-memory slice (dynamic indexing is one load); without one the array lives in local memory.
+  // The caller hands a shared-memory slice (dynamic indexing is one load, and with no other candidate the compiler emits
+  // every access to it as a shared-memory one); the CPU harness may leave it out.
+#if defined(__CUDA_ARCH__)
+  uint32_t *const ch = chunk;
+#else
   uint32_t chunk_local[MMP_CHUNK_WORDS];
-  uint32_t *ch = chunk ? chunk : chunk_local;
+  uint32_t *const ch = chunk ? chunk : chunk_local;
+#endif
   static_assert(MMP_CHUNK_WORDS >= 21 + MMP_LANE_WIN / 2, "slice too short for the checkpoints");
   // mw[k]: members of S' phase B counted before window step k < MMP_LANE_WIN (at most 32 * MMP_LANE_WIN: a u16)
   mark16 *const mw = reinterpret_cast<mark16 *>(ch + 21);
@@ -1013,7 +1026,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
       if (CHARGE && left <= 0) { WALKING = false; live = false; }                                                          \
       else {                                                                                                               \
         const uint32_t wi = WS + K, e = ewin[K];                                                                           \
-        const TabWin &A = AW;                                                                                              \
+        const AWT &A = AW;                                                                                                 \
         bool go_;                                                                                                          \
         MARK_W;                                                                                                            \
         BODY;                                                                                                              \
@@ -1303,7 +1316,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   o.best = best_idx; o.best_rank = (int32_t)best_rank;
   if (open) { o.flags = MMP_TF_OPEN; return true; }
   if (!done) {
-    const int32_t cidx = chosen_rank == best_rank ? best_idx : ((int32_t)chosen_rank == self_rank ? d.self : ((chosen_rank >> 5) < win_end ? Tw.rows[chosen_rank].idx : ldro(&T.rows[chosen_rank].idx)));
+    const int32_t cidx = chosen_rank == best_rank ? best_idx : ((int32_t)chosen_rank == self_rank ? d.self : ((chosen_rank >> 5) < win_end ? AW.idx(chosen_rank) : AG.idx(chosen_rank)));
     o.target = (!favour_self && cidx == d.self) ? MMP_TARGET_SELF : cidx;
     o.n_candidates = ccount;
     o.n_remaining = remaining; o.pick_index = (int32_t)index;
