@@ -316,7 +316,10 @@ int32_t mmp_lru_apply(mmp_fleet *, const mmp_lru_event *ev, int32_t n, int64_t n
 /* the same, also returning the outcome of every event (status[i] = MMP_LOAD_* for MMP_LRU_LOAD events, -1 otherwise) */
 int32_t mmp_lru_apply_status(mmp_fleet *, const mmp_lru_event *ev, int32_t n, int64_t now_ms, mmp_eviction *out, int32_t cap,
                              int32_t *status);
-/* per-instance oldestTime() (CLHM:1125-1133, -1 if empty), weightedSize() and size() */
+/* per-instance oldestTime() (CLHM:1125-1133, -1 if empty), weightedSize() and size().  oldestTime() is the field CLHM
+ * caches: after an MMP_LRU_SET_CAPACITY it keeps the head from before that event's evictions until the next insert,
+ * read of a present key, resize with a new weight or removal of a present key (quirk N14); MMP_LRU_LOAD's churn guard
+ * reads the same value. */
 int32_t mmp_lru_state(mmp_fleet *, int32_t n_instances, int64_t *oldest, int64_t *weighted, int32_t *count);
 
 /* ---- the closed loop on the device (SURVEY.md §8a rows a11 admission, a12 rebalance; §8f-1 ingest / ordering maintenance,

@@ -330,6 +330,7 @@ int32_t mmp_churn_seed(mmp_fleet *f, int32_t n, const int32_t *instance, const i
   CK(upload_vec(cs.lev, lev, st)); CK(upload_vec(cs.vals, order, st)); CK(upload_vec(cs.off, off, st));
   CK(cs.evict.ensure(sizeof(EvictRec) * 16));
   CK(cudaMemsetAsync(cs.counters.p, 0, 64, st));
+  CK(cudaMemsetAsync(f->lru_pin.p, 0x80, (size_t)f->lru_n * 8, st));  // LRU_PIN_NONE: oldestTime() is the head (N14)
   ChurnHooks hk{};
   hk.min_space = f->hs.cfg.min_space_units; hk.min_churn_age = f->hs.cfg.min_churn_age_ms;
   const int grid = (f->lru_n + 3) / 4;

@@ -1246,7 +1246,7 @@ struct mmp_fleet {
   int lanes = 1;                // MMP_KERNEL=tile selects the cooperative-tile kernel (k_place) instead of k_place_lanes
   int lane_warps = 0;           // warps per block of k_place_lanes (MMP_LANE_WARPS = 8 | 10 | 12 | 14 | 16 | 20); 0 = by launch size
   // LRU store (plug point 3)
-  DevBuf lru_ts, lru_seq, lru_weight, lru_model, lru_cap, lru_wsize, lru_count, lru_seqctr, lru_loadts;
+  DevBuf lru_ts, lru_seq, lru_weight, lru_model, lru_cap, lru_wsize, lru_count, lru_seqctr, lru_loadts, lru_pin;
   int32_t lru_n = 0, lru_slots = 0;
 };
 
@@ -1872,7 +1872,7 @@ void mmp_fleet_destroy(mmp_fleet *f) {
                     &f->live.scratch_rows, &f->live.scratch_edges, &f->live.edge_ts, &f->live.model_lul, &f->live.type_part_off, &f->live.type_parts})
     b->release();
   for (DevBuf *b : {&f->d_flush, &f->zero_row, &f->lru_ts, &f->lru_seq, &f->lru_weight, &f->lru_model,
-                    &f->lru_cap, &f->lru_wsize, &f->lru_count, &f->lru_seqctr, &f->lru_loadts})
+                    &f->lru_cap, &f->lru_wsize, &f->lru_count, &f->lru_seqctr, &f->lru_loadts, &f->lru_pin})
     b->release();
   if (f->commit_stream) cudaStreamDestroy(f->commit_stream);
   delete f;

@@ -262,8 +262,14 @@ struct LruView {
   long long *ts; long long *seq; int *weight; int *model;   // [n][slots]
   long long *loadts;                                        // [n][slots] registration time of the copy (MR.instanceIds value), -1: not registered
   long long *cap, *wsize, *seqctr; int *count;              // [n]
+  long long *pin;                                           // [n] oldestTime() as a setCapacity left it (N14), LRU_PIN_NONE
   int n, slots;
 };
+// CLHM caches oldestTime and refreshes it after every write and read (updateOldestTime, CLHM:444, 463), but setCapacity
+// (CLHM:305-316) evicts without refreshing it: until the next refresh oldestTime() reports the head from before the
+// evictions (quirk N14).  The pin holds that value; LRU_PIN_NONE (a byte pattern, so cudaMemset clears the column) means
+// oldestTime() is the head of the deque.
+#define LRU_PIN_NONE ((long long)0x8080808080808080ULL)
 
 // one event of an instance's cache, as the kernels see it
 enum { LEV_INSERT = 0, LEV_TOUCH = 1, LEV_RESIZE = 2, LEV_REMOVE = 3, LEV_SET_CAPACITY = 4, LEV_LOAD = 5, LEV_SEED = 6 };
@@ -361,7 +367,7 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
     sv.ts = s_ts; sv.seq = s_seq; sv.loadts = s_lt; sv.weight = s_w; sv.model = s_m;
     hi = 0; base = 0;
   }
-  long long wsize = v.wsize[inst], capacity = v.cap[inst], ctr = v.seqctr[inst];
+  long long wsize = v.wsize[inst], capacity = v.cap[inst], ctr = v.seqctr[inst], pin = v.pin[inst];
   int count = v.count[inst];
   int evseq = 0;
   // evict() CLHM:329-352 + the listener; returns through *self_gone whether `watch_model` was among the victims
@@ -411,16 +417,16 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
     const long long now = use_ev_time ? e.t : now_param;
     int free_slot;
     int slot = (e.op == LEV_SET_CAPACITY) ? -1 : lru_find(sv, hi, lane, e.model, &free_slot);
-    if (e.op == LEV_SET_CAPACITY) { capacity = e.last_used; evict_loop(e, now, -1, nullptr); continue; }
-    if (e.op == LEV_LOAD) {
-      // limit the rate of cache churn (MM:3872-3884)
-      if (hk.min_churn_age > 0 && capacity - wsize < hk.min_space) {
-        long long t, s;
-        const int o = lru_min_slot(sv, hi, lane, false, 0, 0, &t, &s);
-        if (o >= 0 && t != 0x7fffffffffffffffLL && (t == 0 ? 0 : now - t) < hk.min_churn_age) { if (lane == 0) hk.status[e.dec] = CH_CHURN; continue; }
-      }
-      if (slot >= 0) { if (lane == 0) hk.status[e.dec] = CH_EXISTS; }  // putIfAbsent found an entry: afterRead below
+    // oldestTime() (N14) for a SET_CAPACITY, which keeps it, and for the churn guard of a load into a cache with less than
+    // min_space free (MM:3872-3884); one call site of the slot scan for both keeps the kernel's code as small as before
+    const bool guard = e.op == LEV_LOAD && hk.min_churn_age > 0 && capacity - wsize < hk.min_space;
+    if (e.op == LEV_SET_CAPACITY || guard) {
+      long long lru = pin, s;
+      if (lru == LRU_PIN_NONE && lru_min_slot(sv, hi, lane, false, 0, 0, &lru, &s) < 0) lru = -1;
+      if (!guard) { pin = lru; capacity = e.last_used; evict_loop(e, now, -1, nullptr); continue; }
+      if (lru >= 0 && lru != 0x7fffffffffffffffLL && (lru == 0 ? 0 : now - lru) < hk.min_churn_age) { if (lane == 0) hk.status[e.dec] = CH_CHURN; continue; }
     }
+    if (e.op == LEV_LOAD && slot >= 0) { if (lane == 0) hk.status[e.dec] = CH_EXISTS; }  // putIfAbsent found an entry: afterRead below
     if ((e.op == LEV_INSERT || e.op == LEV_SEED || e.op == LEV_LOAD) && slot < 0) {
       if (free_slot < 0) { if (lane == 0) atomicExch(err, 1); continue; }
       const int w0 = e.op == LEV_LOAD ? 1 : e.weight;  // INSERTION_WEIGHT MM:5011
@@ -432,6 +438,7 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
       } else ++ctr;
       __syncwarp();
       wsize += w0; count++;                                              // AddTask (CLHM:601-610)
+      pin = LRU_PIN_NONE;                                                // afterWrite: updateOldestTime (CLHM:444)
       bool gone = false;
       evict_loop(e, now, e.model, &gone);
       if (e.op != LEV_LOAD) continue;
@@ -457,7 +464,8 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
       continue;
     }
     if ((e.op == LEV_INSERT || e.op == LEV_TOUCH || e.op == LEV_LOAD || e.op == LEV_SEED) && slot >= 0) {
-      // afterRead -> touch + reposition (CLHM:383-388, 477-505; LD:243-255)
+      // afterRead -> touch + reposition (CLHM:383-388, 477-505; LD:243-255), then updateOldestTime (CLHM:463)
+      pin = LRU_PIN_NONE;
       long long old_t = sv.ts[base + slot], old_s = sv.seq[base + slot];
       long long lu = e.last_used > 0 ? (old_t > e.last_used ? old_t : e.last_used) : now;
       if (lu != old_t) {
@@ -482,6 +490,7 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
       int oldw = sv.weight[base + slot];
       if (lane == 0) sv.weight[base + slot] = e.weight;
       __syncwarp();
+      if (e.weight != oldw) pin = LRU_PIN_NONE;                          // no UpdateTask for an unchanged weight
       wsize += (long long)e.weight - oldw;                               // UpdateTask (CLHM:643-651), quiet
       evict_loop(e, now, -1, nullptr);
     } else if (e.op == LEV_REMOVE && slot >= 0) {
@@ -501,6 +510,7 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
       }
       __syncwarp();
       wsize -= (w < 0 ? -w : w); count--;                                // RemovalTask + makeDead (CLHM:614-628, 561-570)
+      pin = LRU_PIN_NONE;
     }
   }
   if (staged) {
@@ -510,7 +520,7 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
       v.ts[gb + i] = sv.ts[i]; v.seq[gb + i] = sv.seq[i]; v.loadts[gb + i] = sv.loadts[i]; v.weight[gb + i] = sv.weight[i]; v.model[gb + i] = sv.model[i];
     }
   }
-  if (lane == 0) { v.wsize[inst] = wsize; v.cap[inst] = capacity; v.seqctr[inst] = ctr; v.count[inst] = count; }
+  if (lane == 0) { v.wsize[inst] = wsize; v.cap[inst] = capacity; v.seqctr[inst] = ctr; v.count[inst] = count; v.pin[inst] = pin; }
 }
 
 __global__ void k_lru_state(LruView v, long long *oldest, long long *weighted, int *count) {
@@ -519,7 +529,8 @@ __global__ void k_lru_state(LruView v, long long *oldest, long long *weighted, i
   if (inst >= v.n) return;
   long long t, s;
   int slot = lru_min_slot(v, inst, lane, false, 0, 0, &t, &s);
-  if (lane == 0) { oldest[inst] = slot < 0 ? -1 : t; weighted[inst] = v.wsize[inst]; count[inst] = v.count[inst]; }
+  const long long pin = v.pin[inst];
+  if (lane == 0) { oldest[inst] = pin != LRU_PIN_NONE ? pin : slot < 0 ? -1 : t; weighted[inst] = v.wsize[inst]; count[inst] = v.count[inst]; }
 }
 
 // dynamic shared memory of a k_lru_events launch with 4 warps per block: room for every warp's staged slot arrays (32 B per
@@ -541,7 +552,7 @@ static LruView lru_view(mmp_fleet *f) {
   v.ts = f->lru_ts.as<long long>(); v.seq = f->lru_seq.as<long long>(); v.weight = f->lru_weight.as<int>(); v.model = f->lru_model.as<int>();
   v.loadts = f->lru_loadts.as<long long>();
   v.cap = f->lru_cap.as<long long>(); v.wsize = f->lru_wsize.as<long long>(); v.seqctr = f->lru_seqctr.as<long long>();
-  v.count = f->lru_count.as<int>(); v.n = f->lru_n; v.slots = f->lru_slots;
+  v.count = f->lru_count.as<int>(); v.pin = f->lru_pin.as<long long>(); v.n = f->lru_n; v.slots = f->lru_slots;
   return v;
 }
 
@@ -584,6 +595,8 @@ int32_t mmp_lru_init(mmp_fleet *f, int32_t n, const int64_t *capacity, int32_t s
   CK(f->lru_loadts.ensure(tot * 8));
   CK(cudaMemset(f->lru_loadts.p, 0xff, tot * 8));
   CK(f->lru_cap.ensure((size_t)n * 8)); CK(f->lru_wsize.ensure((size_t)n * 8)); CK(f->lru_seqctr.ensure((size_t)n * 8)); CK(f->lru_count.ensure((size_t)n * 4));
+  CK(f->lru_pin.ensure((size_t)n * 8));
+  CK(cudaMemset(f->lru_pin.p, 0x80, (size_t)n * 8));  // LRU_PIN_NONE
   CK(cudaMemset(f->lru_model.p, 0xff, tot * 4));
   CK(cudaMemset(f->lru_wsize.p, 0, (size_t)n * 8)); CK(cudaMemset(f->lru_count.p, 0, (size_t)n * 4));
   std::vector<long long> ctr((size_t)n, 1LL << 40);

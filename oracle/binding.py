@@ -295,7 +295,7 @@ class OracleLru:
 
     def apply(self, events: np.ndarray, now_ms: int) -> np.ndarray:
         events = np.ascontiguousarray(events, dtype=LRU_EVENT)
-        cap = max(16, 4 * len(events))
+        cap = max(16, 4 * len(events)) + self.size()  # evictions <= resident entries + inserts
         out = np.zeros(cap, dtype=EVICTION)
         n = self.L.orc_lru_apply(self.h, _ptr(events), len(events), now_ms, _ptr(out), cap)
         assert 0 <= n <= cap

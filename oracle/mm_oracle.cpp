@@ -48,6 +48,9 @@
  *       arrival order (see mm_oracle.h).
  *   N12 ModelToLoad.compareTo (MM:6405-6408) orders by lastUsed only, so the reaper's TreeSet drops a
  *       candidate whose lastUsed equals one already held.
+ *   N14 setCapacity (CLHM:305-316) evicts without updateOldestTime, which only afterWrite (CLHM:444) and
+ *       tryToDrainBuffers (CLHM:463) call: oldestTime() keeps the head from before the evictions until the
+ *       next write or read of a present key, and loadLocal's churn guard (MM:3876) reads that value.
  * Shutting-down records are treated as deletions (MM:1462-1464) so never sit in clusterState.
  * Java integer semantics: int/long arithmetic wraps, >> is arithmetic, / truncates toward zero,
  * (int)double saturates.

@@ -62,9 +62,14 @@ def _compare_window(ep, o, sim, s, ev, now0, now1, seed):
 
 @pytest.mark.parametrize("with_types,fill,seed", [(False, 0.90, 4), (True, 0.90, 5), (False, 0.97, 6), (True, 0.97, 7)])
 def test_closed_loop_matches_oracle_small(product_lib, oracle_lib, with_types, fill, seed):
+    run_small_closed_loop(product_lib, with_types, fill, seed, slots=256)
+
+
+def run_small_closed_loop(product_lib, with_types, fill, seed, slots):
+    """12 windows of a 20k-model x 200-instance churn trace, compared window by window, then the registry and ingest after it"""
     w = make_churn(20_000, 200, seed, fill=fill, with_types=with_types)
     fl = w.fleet
-    o, sim, s = _build(product_lib, w, slots=256)
+    o, sim, s = _build(product_lib, w, slots=slots)
     totals = dict(dec=0, acc=0, evict=0, reload=0, rejected=0, pub=0)
     for ep in range(12):
         ev = w.events(ep, 2000, seed)

@@ -87,7 +87,9 @@ def test_reaper_select_matches_oracle(product_lib, oracle_lib, config, nm, ni, s
 
 
 @pytest.mark.parametrize("seed", range(6))
-def test_lru_matches_oracle(product_lib, oracle_lib, seed):
+def test_lru_matches_oracle_cached_oldest_time(product_lib, oracle_lib, seed):
+    """evictions, weightedSize(), size() and oldestTime() -- the field CLHM caches, which a setCapacity leaves stale
+    (N14) -- against the oracle's LRU after every batch"""
     rng = SplitMix(1000 + seed)
     n_inst, slots = 37, 96
     caps = rng.randint(n_inst, 20_000, 60_000)
@@ -126,11 +128,8 @@ def test_lru_matches_oracle(product_lib, oracle_lib, seed):
         oldest, weighted, count = s.lru_state()
         assert [int(x) for x in weighted] == [o.weighted_size() for o in oracles]
         assert [int(x) for x in count] == [o.size() for o in oracles]
-        exp_oldest = []
-        for o in oracles:
-            k, t, w = o.dump()
-            exp_oldest.append(int(t[0]) if len(t) else -1)
-        assert [int(x) for x in oldest] == exp_oldest
+        # oldestTime() as CLHM caches it: stale after a setCapacity's evictions (N14)
+        assert [int(x) for x in oldest] == [o.oldest_time() for o in oracles]
         now += 7_000
 
 
