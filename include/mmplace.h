@@ -414,7 +414,7 @@ int32_t mmp_registry_prune(mmp_fleet *, int32_t self, int64_t now_ms, int64_t as
                            uint8_t *out_masks, int32_t cap);
 
 /* tuning / measurement knobs, same meaning as the MMP_* environment variables read at mmp_fleet_create:
- *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the streaming kernel (k_place_lanes), 1 the latency kernel
+ *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the batch kernel ("direct" below), 1 the latency kernel
  *                     k_place_small as a stream launch, 2 k_place_small as a replayed CUDA graph, 3 (default) a request to the
  *                     resident server kernel k_place_server (no launch per call: the host posts the request into mapped memory
  *                     and spins on the answer; one caller at a time, concurrent callers take the graph path)
@@ -424,10 +424,7 @@ int32_t mmp_registry_prune(mmp_fleet *, int32_t self, int64_t now_ms, int64_t as
  *                     kernel k_place_lanes (whole rows through TMA landing stages) -- MMP_KERNEL=direct | lanes | tile
  *   "sort_slots"      k_place_direct resolves a batch of >= 8192 decisions in type-slot order: 0 never, 1 always, 2 (default) when
  *                     the committed snapshot's candidate sets are sparse (long walks: lanes of a warp then finish together)
- *   "small_max"       untraced batches of up to this many decisions run on k_place_small (one wave of 32-thread blocks, rows
- *                     read straight from memory) instead of the streaming kernel
  *   "lane_budget"     walk steps a lane may spend before its decision is redone by the whole warp
- *   "lane_warps"      warps per block of k_place_lanes (0 = default 12)
  *   "commit_host_only" 1: every commit takes the structural (host) path */
 int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
 /* CUDA-event duration (ms) of the device part of the last mmp_stats ("stats"), mmp_reaper_select ("reaper": registry sweep +

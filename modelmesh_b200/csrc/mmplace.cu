@@ -15,9 +15,9 @@
 //   nzw/nz_n  [n_slots][row_words] u16    compressed word lists: the row words that hold any candidate of the slot (walks beyond the window)
 //   front     [n_models][16] u32          instance-sharded fleets: the first row words, replicated on every shard
 // Kernels (DESIGN.md §5, §7):
-//   k_place_direct<4, MINB>  the scoring kernel (default): one decision per lane, the row rebuilt from the model's excl_ranks,
+//   k_place_direct<4, 5>     the scoring kernel (default): one decision per lane, the row rebuilt from the model's excl_ranks,
 //                            longer walks through the word lists; optional slot-sorted batches (k_slot_keys + cub radix sort)
-//   k_place_lanes<WARPS>     round 1's streaming kernel (whole rows through TMA landing stages): MMP_KERNEL=lanes and the
+//   k_place_lanes            round 1's streaming kernel (whole rows through TMA landing stages): MMP_KERNEL=lanes and the
 //                            collective instance-shard path
 //   k_place_small            tiny batches as a stream launch / replayed CUDA graph;  k_place_server: the resident B = 1 server
 //   k_place_dealt, k_dealt_wait   instance shards over peer memory;  k_shard_*: the kernels around the NCCL all-reduce
@@ -343,6 +343,9 @@ static constexpr int LANE_WIN = MMP_LANE_WIN;  // row words copied out of the la
 static constexpr int LANE_STRIDE = LANE_WIN + 1;  // words per lane in the window buffer (odd: bank-conflict free)
 static constexpr int LANE_BUDGET = 192;  // walk steps a lane may spend before handing its decision to the whole warp
 static constexpr int LANE_SLOTS = 64;    // type-constraint mask slots whose window words are kept in shared memory
+static constexpr int LANE_WARPS = 12;    // warps per block of k_place_lanes
+static constexpr int LANE_STAGES = 4;    // landing stages per SM at most: a fifth takes the shared-memory carve-out from 196 to
+                                         // 228 KB and leaves too little L1 for the lane tables to stay resident
 struct LaneLayout {
   uint32_t row_bytes, stride, stage_bytes, ns, warps;
   uint32_t off_bar, off_busy, off_uses, off_warp, per_warp;
@@ -369,16 +372,14 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-template <int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
-                                                               const FreshRow *__restrict__ fresh, int n_fresh,
-                                                               const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
-                                                               int64_t now, uint64_t seed, uint64_t id_base, int ns,
-                                                               int mode, unsigned long long *__restrict__ dbg,
-                                                               int emit_keys, int shard_rank, const int32_t *__restrict__ orig_id, int budget) {
+__global__ void __launch_bounds__(LANE_WARPS * 32, 1) k_place_lanes(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
+                                                                    const FreshRow *__restrict__ fresh, int n_fresh,
+                                                                    const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
+                                                                    int64_t now, uint64_t seed, uint64_t id_base, int ns,
+                                                                    int emit_keys, int shard_rank, const int32_t *__restrict__ orig_id, int budget) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int RW = s.excl_stride;  // words per stored row (the whole row unless the fleet is instance-sharded)
-  const LaneLayout lay(RW, ns, WARPS, true);
+  const LaneLayout lay(RW, ns, LANE_WARPS, true);
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + lay.off_bar);
   int *ticket = reinterpret_cast<int *>(smem_raw + lay.off_busy);               // next stage ticket of this block
@@ -426,7 +427,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
   }
   __syncthreads();
   // batches of 32 decisions are dealt round-robin to the grid's warps (consecutive batches to the warps of one block)
-  const int gw = blockIdx.x * WARPS + wib, nw = gridDim.x * WARPS;
+  const int gw = blockIdx.x * LANE_WARPS + wib, nw = gridDim.x * LANE_WARPS;
   auto load_dec = [&](int b, mmp_decision_in &d) -> bool {
     const int i = b * 32 + lane;
     if (b >= nb || i >= n) return false;
@@ -450,13 +451,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
   int bn = b + nw;
   mmp_decision_in dn;
   bool valid_n = load_dec(bn, dn);
-  // MMP_LANE_MODE bit 1: per-phase cycle sums (measurement aid): wait-for-stage, issue, context, flight-left, copy-out, requests, decide
-  long long tsum[7] = {0, 0, 0, 0, 0, 0, 0};
-  long long tsteps = 0;
-  const bool timing = (mode & 2) != 0 && dbg != nullptr;
-#define LANE_T(k) do { if (timing) { const long long t_ = clock64(); tsum[k] += t_ - tprev; tprev = t_; } } while (0)
   while (b < nb) {
-    long long tprev = timing ? clock64() : 0;
     // ---- acquire a landing stage and send the 32 rows on their way ----
     int st = 0;
     uint32_t parity = 0;
@@ -474,7 +469,6 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
     }
     st = __shfl_sync(0xffffffffu, st, 0);
     parity = __shfl_sync(0xffffffffu, parity, 0);
-    LANE_T(0);
     unsigned char *stage = smem_raw + (size_t)st * lay.stage_bytes;
     const uint32_t *my_row = reinterpret_cast<const uint32_t *>(stage + (size_t)lane * lay.stride);
     // row of this decision: its model's, or row i of a gathered row set (orig_id != nullptr: the instance-shard gather pass)
@@ -490,13 +484,9 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
       mbar_expect_tx(&bars[st], lay.row_bytes);
       bulk_g2s(const_cast<uint32_t *>(my_row), excl_row(s, m), lay.row_bytes, &bars[st]);
     } else mbar_arrive(&bars[st]);
-    LANE_T(1);
     // ---- the rest of this batch's context while its rows are in flight ----
     if (s.word_lo == 0 && valid) prepare_ctx_b(s, d, ca, fresh, n_fresh, extra, c);
-    if (timing && __shfl_xor_sync(0xffffffffu, c.slot ^ (int)c.self_bits, 1) == 0x7fffffff) tsum[2]++;  // consume the gathers before the timestamp
-    LANE_T(2);
     while (!mbar_try_wait(&bars[st], parity)) {}
-    LANE_T(3);
     // ---- copy the window out and hand the stage on ----
     uint32_t self_eword = 0;
     {
@@ -515,7 +505,6 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
     }
     __syncwarp();
     if (lane == 0) { __threadfence_block(); atomicAdd(const_cast<uint32_t *>(released + st), 1u); }
-    LANE_T(4);
     // ---- requests for the batches behind this one ----
     CtxA cn;
     cn.ok = 0; cn.self_rank = -1;
@@ -523,10 +512,8 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
     const int bnn = bn + nw;
     mmp_decision_in dnn;
     const bool valid_nn = load_dec(bnn, dnn);
-    LANE_T(5);
     // ---- one decision per lane, the 32 lanes in lockstep ----
     DecideOut o;
-    bool handled = true;
     const uint64_t my_id = pick_id(d, id_base + (uint64_t)(orig_id ? (valid ? orig_id[b * 32 + lane] : 0) : b * 32 + lane));
     const int slot = c.slot >= 0 ? ctx_slot(c) : 0;
     const LaneTables T = lane_tables_global(s, slot);
@@ -535,13 +522,10 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
       if (slot < LANE_SLOTS) { Tw.cx = f_cx + slot * LANE_WIN - WS; Tw.p = f_p + slot * LANE_WIN - WS; }
       Tw.full = f_full - WS; Tw.csum = f_csum - WS; Tw.count_col = f_count - WS * 32; Tw.rows = f_rows - WS * 32;
     }
-    if ((mode & 1) == 0)
-      handled = decide_stream(s, Tw, T, c, valid && !skip, win + lane * LANE_STRIDE, win_words, RowPtr{excl_row(s, m), (uint32_t)s.word_lo}, self_eword,
-                              now, seed, my_id, WarpVote(), o, budget, chunk + lane * MMP_CHUNK_WORDS);
-    else { o.target = (int32_t)(self_eword & 1u) - 1; o.n_candidates = 0; }  // MMP_LANE_MODE=1: stream-only probe (no decisions)
+    const bool handled = decide_stream(s, Tw, T, c, valid && !skip, win + lane * LANE_STRIDE, win_words, RowPtr{excl_row(s, m), (uint32_t)s.word_lo},
+                                       self_eword, now, seed, my_id, WarpVote(), o, budget, chunk + lane * MMP_CHUNK_WORDS);
     // ---- what the lane routine declined: the whole warp redoes it, reading the row from global memory (L2) ----
     uint32_t pending = __ballot_sync(0xffffffffu, valid && !skip && !handled);
-    if (timing && lane == 0 && pending) atomicAdd(&dbg[8], (unsigned long long)__popc(pending));  // decisions redone by the whole warp
     while (pending) {
       const int l = __ffs((int)pending) - 1;
       pending &= pending - 1;
@@ -564,14 +548,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) k_place_lanes(const SnapshotVie
     b = bn; d = dn; valid = valid_n; ca = cn;
     bn = bnn; dn = dnn; valid_n = valid_nn;
     __syncwarp();
-    LANE_T(6);
-    tsteps++;
   }
-  if (timing && lane == 0) {
-    for (int k = 0; k < 7; k++) atomicAdd(&dbg[k], (unsigned long long)tsum[k]);
-    atomicAdd(&dbg[7], (unsigned long long)tsteps);
-  }
-#undef LANE_T
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1154,8 +1131,6 @@ struct PlaceCtx {
   static constexpr int NPIPE = 3;
   cudaStream_t pipe[NPIPE] = {nullptr, nullptr, nullptr};  // H2D / kernel / D2H of consecutive chunks overlap across these
   cudaEvent_t e0 = nullptr, e1 = nullptr, ready = nullptr;
-  static constexpr int NSHARD_CHUNKS = 4;  // instance-sharded batches: scoring of chunk k+1 overlaps the all-reduce of chunk k
-  cudaEvent_t shard_ev[NSHARD_CHUNKS + 1] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   DevBuf d_in, d_out, d_fresh, d_extra, d_trace, d_cand;
   // slot sort of a batch (k_slot_keys + cub radix sort -> perm): set 0 for single launches, 1 + pipe for the chunks of a pipelined call
   static constexpr int NSORT = 4;
@@ -1172,6 +1147,10 @@ struct PlaceCtx {
   int32_t graph_epoch = -1;
 };
 
+// The scoring kernel of untraced batches (MMP_KERNEL = direct | lanes | tile; launch_place): k_place_direct (rows rebuilt
+// from excl_ranks), k_place_lanes (whole rows through TMA landing stages) or the cooperative tile kernel k_place.
+enum class PlaceKernel { direct, lanes, tile };
+
 struct mmp_fleet {
   HostState hs;
   int device = 0;
@@ -1182,7 +1161,7 @@ struct mmp_fleet {
   int cur = 0;
   int32_t epoch = 0;
   cudaStream_t commit_stream = nullptr;
-  DevBuf d_flush, d_dbg;
+  DevBuf d_flush;
   DevBuf zero_row;              // one all-zero exclusion row (SnapshotView::zero_row), unsharded fleets: allocated at the first commit
   ChurnState churn;             // the closed loop (churn_kernels.cuh)
   int64_t structural_epoch = 0; // bumped by every structural commit
@@ -1207,7 +1186,6 @@ struct mmp_fleet {
     bool opened[MAX_SHARDS][4] = {};
     uint64_t step = 0;
     int64_t batches = 0, result_bytes = 0;
-    int minb = 6;
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // around k_place_dealt and k_dealt_wait of the last step
     float t_kernel_ms = 0, t_wait_ms = 0;
     int off = 0;                            // MMP_SHARD_PEERS=0 keeps the collective path although peers were imported
@@ -1218,12 +1196,7 @@ struct mmp_fleet {
   std::mutex ctx_mu;
   std::vector<std::unique_ptr<PlaceCtx>> ctx_free;
   std::atomic<int64_t> launches{0};
-  int tile = 16;                // lanes per decision in k_place (MMP_TILE = 8 | 16 | 32)
-  int ring_k = 4;               // ring depth for rows <= 2 KiB (MMP_RING_K = 2 | 4)
-  int lane_stages = 4;          // MMP_LANE_STAGES caps the landing stages per SM (0: as many as fit).  A fifth stage takes the
-                                // shared-memory carve-out from 196 to 228 KB and leaves too little L1 for the lane tables to stay resident
-  int shard_chunks = 1;         // MMP_SHARD_CHUNKS (see place_sharded)
-  int one_mode = 3;             // MMP_ONE = lanes | small | graph | server: how tiny batches are launched (0: the streaming kernel, 1: k_place_small
+  int one_mode = 3;             // MMP_ONE = lanes | small | graph | server: how tiny batches are launched (0: launch_place, 1: k_place_small
                                 // as a stream launch, 2: k_place_small as a replayed CUDA graph, 3: a request to the resident k_place_server)
   // the resident B = 1 server (one_mode 3, k_place_server)
   struct Server {
@@ -1238,13 +1211,8 @@ struct mmp_fleet {
   } srv;
   int sort_slots = 2;           // MMP_SORT_SLOTS = 0 never | 1 always | 2 (default) when the snapshot's candidate sets are sparse: k_place_direct
                                 // resolves a large batch in type-slot order
-  int direct = 1, direct_minb = 5;  // MMP_KERNEL=direct: k_place_direct (no landing stages); MMP_DIRECT_MINB = 4 | 5 | 6 | 8 resident blocks per SM
-  int small_max = 0;            // MMP_SMALL_MAX: untraced batches of up to this many decisions run on k_place_small (no landing stages:
-                                // one wave of 32-thread blocks), larger ones on the streaming kernel
+  PlaceKernel kernel = PlaceKernel::direct;  // MMP_KERNEL, mmp_tune("direct"): which kernel resolves untraced unsharded batches
   int lane_budget = LANE_BUDGET;  // MMP_LANE_BUDGET: walk steps per lane before a decision is handed to the whole warp
-  int lane_mode = 0;            // MMP_LANE_MODE=1: stream-only probe (rows staged, no decisions) -- measurement aid, results void
-  int lanes = 1;                // MMP_KERNEL=tile selects the cooperative-tile kernel (k_place) instead of k_place_lanes
-  int lane_warps = 0;           // warps per block of k_place_lanes (MMP_LANE_WARPS = 8 | 10 | 12 | 14 | 16 | 20); 0 = by launch size
   // LRU store (plug point 3)
   DevBuf lru_ts, lru_seq, lru_weight, lru_model, lru_cap, lru_wsize, lru_count, lru_seqctr, lru_loadts, lru_pin;
   int32_t lru_n = 0, lru_slots = 0;
@@ -1279,7 +1247,6 @@ static PlaceCtx *acquire_ctx(mmp_fleet *f) {
             cudaEventCreateWithFlags(&c->ready, cudaEventDisableTiming) == cudaSuccess &&
             cudaHostAlloc((void **)&c->mapped, PlaceCtx::MAPPED_BYTES, cudaHostAllocMapped) == cudaSuccess;
   for (int i = 0; ok && i < PlaceCtx::NPIPE; i++) ok = cudaStreamCreateWithFlags(&c->pipe[i], cudaStreamNonBlocking) == cudaSuccess;
-  for (int i = 0; ok && i <= PlaceCtx::NSHARD_CHUNKS; i++) ok = cudaEventCreateWithFlags(&c->shard_ev[i], cudaEventDisableTiming) == cudaSuccess;
   if (!ok) { delete c; return nullptr; }
   return c;
 }
@@ -1311,7 +1278,6 @@ static void destroy_ctx(PlaceCtx *c) {
   if (c->e0) cudaEventDestroy(c->e0);
   if (c->e1) cudaEventDestroy(c->e1);
   if (c->ready) cudaEventDestroy(c->ready);
-  for (int i = 0; i <= PlaceCtx::NSHARD_CHUNKS; i++) if (c->shard_ev[i]) cudaEventDestroy(c->shard_ev[i]);
   if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
   if (c->graph) cudaGraphDestroy(c->graph);
   if (c->mapped) cudaFreeHost(c->mapped);
@@ -1364,39 +1330,42 @@ static cudaError_t launch_place_t(mmp_fleet *f, const PlaceArgs &a, cudaStream_t
   return cudaGetLastError();
 }
 
-// stages x warps for a stored row width: as many 32-row landing stages as fit beside the warps' window buffers
-static bool lanes_geometry(int row_words, int warps, int &ns) {
-  for (ns = 8; ns >= 2; ns--)
-    if (LaneLayout(row_words, ns, warps, true).total <= (size_t)227 * 1024) return true;
+// landing stages of k_place_lanes for a stored row width: as many 32-row stages as fit beside the warps' window buffers, at
+// most LANE_STAGES; false when not even two fit (rows wider than about 580 words)
+static bool lanes_geometry(int row_words, int &ns) {
+  for (ns = LANE_STAGES; ns >= 2; ns--)
+    if (LaneLayout(row_words, ns, LANE_WARPS, true).total <= (size_t)227 * 1024) return true;
   return false;
 }
 
-template <int WARPS>
 static cudaError_t launch_place_lanes(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st, int ns) {
   static std::atomic<bool> attr_set[64];  // function attributes are per device
-  if (f->lane_stages >= 2 && f->lane_stages < ns) ns = f->lane_stages;
-  const LaneLayout lay(a.s.excl_stride, ns, WARPS, true);  // (instance-sharded rows are short: well under half an SM's shared memory)
-  auto kern = k_place_lanes<WARPS>;
+  const LaneLayout lay(a.s.excl_stride, ns, LANE_WARPS, true);  // (instance-sharded rows are short: well under half an SM's shared memory)
   if (!attr_set[f->device & 63].load()) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_place_lanes, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     attr_set[f->device & 63] = true;
   }
   const int nb = (a.n + 31) / 32;
-  const int grid = std::max(1, std::min((nb + WARPS - 1) / WARPS, f->sm_count));
-  kern<<<grid, WARPS * 32, lay.total, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, ns,
-                                            f->lane_mode, f->d_dbg.as<unsigned long long>(), a.emit_keys,
-                                            f->hs.cfg.shard_rank, a.orig_id, f->lane_budget);
+  const int grid = std::max(1, std::min((nb + LANE_WARPS - 1) / LANE_WARPS, f->sm_count));
+  k_place_lanes<<<grid, LANE_WARPS * 32, lay.total, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, ns,
+                                                          a.emit_keys, f->hs.cfg.shard_rank, a.orig_id, f->lane_budget);
   f->launches++;
   return cudaGetLastError();
 }
 
 static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st) {
   const int rw = a.s.row_words;
-  // the direct kernel: rows rebuilt from the snapshot's excl_ranks (whole-row fleets), no landing stages (MMP_KERNEL=direct | lanes)
-  if (!(a.tr || a.cand) && !a.emit_keys && !a.orig_id && f->direct && a.n > f->small_max && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words &&
-      a.s.excl_ranks) {
-    const int blocks = (a.n + 127) / 128;
+  int ns = 0;
+  // traced calls (parity tests): the single-decision-per-warp tile kernel, kept apart so that the untraced kernels'
+  // instruction footprint stays small
+  if (a.tr || a.cand)
+    return rw <= 512 ? launch_place_t<4, 4, 4, 32, true>(f, a, st) : rw <= 1024 ? launch_place_t<4, 4, 3, 32, true>(f, a, st) : launch_place_t<4, 2, 2, 32, true>(f, a, st);
+  // the instance-shard key pass and gather pass: only k_place_lanes writes shard keys and reads rows by batch position
+  // (place_sharded has checked that the rows fit its landing stages)
+  if (a.emit_keys || a.orig_id) return lanes_geometry(a.s.excl_stride, ns) ? launch_place_lanes(f, a, st, ns) : cudaErrorInvalidValue;
+  // the direct kernel: rows rebuilt from the snapshot's excl_ranks (whole-row fleets), no landing stages
+  if (f->kernel == PlaceKernel::direct && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words && a.s.excl_ranks) {
     const int32_t *perm = nullptr;  // k_place_direct: position j of the launch resolves decision perm[j]
     if (a.ctx && a.n >= 8192 && (f->sort_slots == 1 || (f->sort_slots == 2 && f->snaps[f->cur].sparse_slots))) {
       PlaceCtx *c = a.ctx;  // slot order: key pass + 16-bit radix sort of the indices (a few tens of microseconds per million decisions)
@@ -1412,45 +1381,17 @@ static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
       perm = c->d_sidx2[ss].as<int32_t>();
       f->launches += 2;
     }
-    int minb = f->direct_minb;
-    if (minb == 6 && blocks > f->sm_count * 6 && blocks <= f->sm_count * 8) minb = 8;  // a launch of 1.0 .. 1.33 waves at 6 blocks per SM fits ONE wave at 8
-    auto kern = minb == 8 ? k_place_direct<4, 8> : minb == 6 ? k_place_direct<4, 6> : minb == 5 ? k_place_direct<4, 5> : k_place_direct<4, 4>;
-    kern<<<blocks, 128, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, f->lane_budget, perm);
+    k_place_direct<4, 5><<<(a.n + 127) / 128, 128, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base,
+                                                           f->lane_budget, perm);
     f->launches++;
     return cudaGetLastError();
   }
-  // small launches: a batch that fits one wave of 32-decision blocks skips the landing-stage pipeline (its prologue and
-  // its one-block-per-SM shape cost more than they hide when every warp has a single step to do)
-  if (!(a.tr || a.cand) && !a.emit_keys && !a.orig_id && a.n <= f->small_max && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words) {
-    k_place_small<<<(a.n + 31) / 32, 32, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, nullptr, f->lane_budget);
-    f->launches++;
-    return cudaGetLastError();
-  }
-  // production path: one decision per lane (any row width of which at least two 32-row landing stages fit: ~3 KiB rows)
-  if (!(a.tr || a.cand) && f->lanes) {
-    int ns = 0;
-    const int lw = f->lane_warps ? f->lane_warps : 12;
-    if (lw == 8 && lanes_geometry(a.s.excl_stride, 8, ns)) return launch_place_lanes<8>(f, a, st, ns);
-    if (lw == 10 && lanes_geometry(a.s.excl_stride, 10, ns)) return launch_place_lanes<10>(f, a, st, ns);
-    if (lw == 14 && lanes_geometry(a.s.excl_stride, 14, ns)) return launch_place_lanes<14>(f, a, st, ns);
-    if (lw == 12 && lanes_geometry(a.s.excl_stride, 12, ns)) return launch_place_lanes<12>(f, a, st, ns);
-    if (lw == 20 && lanes_geometry(a.s.excl_stride, 20, ns)) return launch_place_lanes<20>(f, a, st, ns);
-    if (lw == 16 && lanes_geometry(a.s.excl_stride, 16, ns)) return launch_place_lanes<16>(f, a, st, ns);
-    if (lanes_geometry(a.s.excl_stride, 12, ns)) return launch_place_lanes<12>(f, a, st, ns);
-  }
-  // tile width: how many lanes (= window words) resolve one decision; 32/T decisions advance per warp step.
-  // The traced variant (parity tests) is a separate, single-decision-per-warp kernel so that the production kernel's
-  // instruction footprint stays small.
-  const bool traced = a.tr || a.cand;
-  if (rw <= 512) {  // rows <= 2 KiB (16k instances): 7 blocks x 4 warps per SM
-    if (traced) return launch_place_t<4, 4, 4, 32, true>(f, a, st);
-    if (f->tile == 8) return launch_place_t<4, 4, 7, 8, false>(f, a, st);
-    if (f->tile == 32) return launch_place_t<4, 4, 7, 32, false>(f, a, st);
-    if (f->ring_k == 2) return launch_place_t<4, 2, 8, 16, false>(f, a, st);  // no look-ahead, smaller footprint: 8 blocks/SM
-    return launch_place_t<4, 4, 7, 16, false>(f, a, st);
-  }
-  if (rw <= 1024) return traced ? launch_place_t<4, 4, 3, 32, true>(f, a, st) : launch_place_t<4, 4, 3, 16, false>(f, a, st);  // rows <= 4 KiB
-  return traced ? launch_place_t<4, 2, 2, 32, true>(f, a, st) : launch_place_t<4, 2, 2, 16, false>(f, a, st);
+  // one decision per lane with the rows through landing stages (any row width of which at least two stages fit)
+  if (f->kernel != PlaceKernel::tile && lanes_geometry(a.s.excl_stride, ns)) return launch_place_lanes(f, a, st, ns);
+  // the cooperative tile kernel by row width: rows <= 2 KiB (16k instances) 7 blocks x 4 warps per SM, then <= 4 KiB, then wider
+  if (rw <= 512) return launch_place_t<4, 4, 7, 16, false>(f, a, st);
+  if (rw <= 1024) return launch_place_t<4, 4, 3, 16, false>(f, a, st);
+  return launch_place_t<4, 2, 2, 16, false>(f, a, st);
 }
 
 // the peer-access path of place_sharded: one k_place_dealt over this shard's deal of the batch, the arrival wait, the
@@ -1480,8 +1421,7 @@ static int32_t place_dealt(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, 
   const long long mine = n_wb > me ? (n_wb - me + G - 1) / G : 0;      // ... dealt to this shard
   const int blocks = (int)std::max<long long>(1, (mine + WARPS - 1) / WARPS);  // (an empty deal still arrives)
   const size_t smem = (size_t)WARPS * vw.row_words * 4;
-  // MINB: resident blocks per SM the compiler must allow (4: no spills, 16 warps per SM; 6: 24 warps, some spills) -- MMP_DEALT_MINB
-  auto kern = pr.minb == 6 ? k_place_dealt<WARPS, 6> : k_place_dealt<WARPS, 4>;
+  auto kern = k_place_dealt<WARPS, 6>;  // 6 resident blocks per SM: 24 warps, some spills
   if (smem > 48 * 1024) CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   unsigned long long *stats = pr.flag_buf() + MAX_SHARDS;
   if (!pr.ev[0]) for (int k = 0; k < 3; k++) CK(cudaEventCreate(&pr.ev[k]));
@@ -1525,6 +1465,16 @@ static int32_t place_sharded(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds
   if (f->peers.ready && !f->peers.off && f->hs.cfg.shard_count > 1)
     return place_dealt(f, c, ds, d_in, n, d_fresh, n_fresh, d_extra, n_extra, d_out, now_ms, seed, st);
   if (!f->comm) { g_err = "instance-sharded fleet is not connected (mmp_shard_connect)"; return MMP_E_STATE; }
+  // the key pass stages this shard's stored rows, the gather pass whole rows, both through k_place_lanes' landing stages
+  const int ST = ds.view.excl_stride, NW = ds.view.row_words, widest = std::max(ST, NW);
+  int ns = 0;
+  if (!lanes_geometry(widest, ns)) {
+    int limit = widest;
+    while (limit > 0 && !lanes_geometry(limit, ns)) limit--;
+    g_err = "instance shards: rows of " + std::to_string(widest) + " words are wider than the " + std::to_string(limit) +
+            " words the collective path can stage (k_place_lanes)";
+    return MMP_E_STATE;
+  }
   NcclApi &nc = nccl_api();
   std::lock_guard<std::mutex> g(f->comm_mu);
   const int G = f->hs.cfg.shard_count;
@@ -1532,30 +1482,14 @@ static int32_t place_sharded(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds
   CK(c->d_open_idx.ensure((size_t)n * 4));
   CK(c->d_n_open.ensure(16));
   CK(cudaMemsetAsync(c->d_n_open.p, 0, sizeof(int), st));
-  // 1-3. per-shard keys (the scoring kernel), the min-loc combine over NVLink, keys -> results.  MMP_SHARD_CHUNKS = 2..4
-  // splits a large batch so that the all-reduce and decode of chunk k run on a second stream while the scoring kernel
-  // works on chunk k + 1.  Four short launches and four collectives can cost more than the 8 MB exchange of a 1 M-decision
-  // batch they hide, so the default is 1.
-  const int K = (n >= (1 << 18) && f->shard_chunks > 1) ? std::min(f->shard_chunks, (int)PlaceCtx::NSHARD_CHUNKS) : 1;
-  const int32_t chunk = ((n + K - 1) / K + 31) / 32 * 32;
-  cudaStream_t side = c->pipe[0];
-  CK(cudaEventRecord(c->shard_ev[PlaceCtx::NSHARD_CHUNKS], st));  // the side stream starts after what precedes this call on st
-  CK(cudaStreamWaitEvent(side, c->shard_ev[PlaceCtx::NSHARD_CHUNKS], 0));
-  int k = 0;
-  for (int32_t lo = 0; lo < n; lo += chunk, k++) {
-    const int32_t cnt = std::min(chunk, n - lo);
-    PlaceArgs a{vw, d_in + lo, cnt, d_fresh, n_fresh, d_extra, d_out + lo, nullptr, nullptr, now_ms, seed, f->id_base.load() + (uint64_t)lo};
-    a.emit_keys = 1;
-    CK(launch_place(f, a, st));
-    cudaStream_t cs = K > 1 ? side : st;
-    if (K > 1) { CK(cudaEventRecord(c->shard_ev[k], st)); CK(cudaStreamWaitEvent(side, c->shard_ev[k], 0)); }
-    NK(nc.AllReduce(d_out + lo, d_out + lo, (size_t)cnt, ncclUint64, ncclMin, f->comm, cs));
-    k_shard_decode<<<(cnt + 255) / 256, 256, 0, cs>>>(reinterpret_cast<uint64_t *>(d_out + lo), cnt, c->d_open_flag.as<uint8_t>() + lo,
-                                                       c->d_n_open.as<int>());
-    f->launches++;
-    CK(cudaGetLastError());
-  }
-  if (K > 1) { CK(cudaEventRecord(c->shard_ev[PlaceCtx::NSHARD_CHUNKS], side)); CK(cudaStreamWaitEvent(st, c->shard_ev[PlaceCtx::NSHARD_CHUNKS], 0)); }
+  // 1-3. per-shard keys (the scoring kernel), the min-loc combine over NVLink, keys -> results
+  PlaceArgs a{vw, d_in, n, d_fresh, n_fresh, d_extra, d_out, nullptr, nullptr, now_ms, seed, f->id_base.load()};
+  a.emit_keys = 1;
+  CK(launch_place(f, a, st));
+  NK(nc.AllReduce(d_out, d_out, (size_t)n, ncclUint64, ncclMin, f->comm, st));
+  k_shard_decode<<<(n + 255) / 256, 256, 0, st>>>(reinterpret_cast<uint64_t *>(d_out), n, c->d_open_flag.as<uint8_t>(), c->d_n_open.as<int>());
+  f->launches++;
+  CK(cudaGetLastError());
   int n_open = 0;
   CK(cudaMemcpyAsync(&n_open, c->d_n_open.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -1570,7 +1504,6 @@ static int32_t place_sharded(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds
   f->launches += 2;
   // 4. the open decisions, from whole rows: all-gather every shard's block of their exclusion rows (the same ordered
   // list on every rank), assemble, and run the same kernel on the assembled rows with the snapshot's whole rank range
-  const int ST = ds.view.excl_stride, NW = ds.view.row_words;
   CK(c->d_blocks.ensure((size_t)n_open * ST * 4));
   CK(c->d_gathered.ensure((size_t)G * n_open * ST * 4));
   CK(c->d_rows.ensure((size_t)n_open * NW * 4));
@@ -1789,7 +1722,6 @@ int32_t mmp_shard_ipc_import(mmp_fleet *f, const void *blobs) {
     }
   }
   if (const char *t = getenv("MMP_SHARD_PEERS")) pr.off = atoi(t) == 0;
-  if (const char *t = getenv("MMP_DEALT_MINB")) pr.minb = atoi(t) == 4 ? 4 : 6;
   pr.ready = true;
   return MMP_OK;
 }
@@ -1831,20 +1763,11 @@ int32_t mmp_fleet_create(const mmp_config *cfg, mmp_fleet **out) {
   f->sm_count = prop.multiProcessorCount;
   CK(cudaStreamCreateWithFlags(&f->commit_stream, cudaStreamNonBlocking));
   f->hs.init(*cfg);
-  if (const char *t = getenv("MMP_RING_K")) { int v = atoi(t); if (v == 2 || v == 4) f->ring_k = v; }
-  if (const char *t = getenv("MMP_KERNEL")) { f->lanes = strcmp(t, "tile") != 0; f->direct = strcmp(t, "lanes") != 0 && strcmp(t, "tile") != 0; }
-  if (const char *t = getenv("MMP_LANE_WARPS")) { int v = atoi(t); if (v == 8 || v == 10 || v == 12 || v == 14 || v == 16 || v == 20) f->lane_warps = v; }
-  if (const char *t = getenv("MMP_LANE_STAGES")) f->lane_stages = atoi(t);
-  if (const char *t = getenv("MMP_LANE_MODE")) f->lane_mode = atoi(t);
+  if (const char *t = getenv("MMP_KERNEL")) f->kernel = !strcmp(t, "tile") ? PlaceKernel::tile : !strcmp(t, "lanes") ? PlaceKernel::lanes : PlaceKernel::direct;
   if (const char *t = getenv("MMP_ONE")) f->one_mode = !strcmp(t, "lanes") ? 0 : (!strcmp(t, "small") ? 1 : (!strcmp(t, "server") ? 3 : 2));
   if (const char *t = getenv("MMP_COMMIT")) f->commit_host_only = strcmp(t, "host") == 0;
   if (const char *t = getenv("MMP_SORT_SLOTS")) { int v = atoi(t); if (v >= 0 && v <= 2) f->sort_slots = v; }
-  if (const char *t = getenv("MMP_DIRECT_MINB")) { int v = atoi(t); f->direct_minb = v == 8 ? 8 : v == 6 ? 6 : v == 5 ? 5 : 4; }
-  if (const char *t = getenv("MMP_SMALL_MAX")) { int v = atoi(t); if (v >= 0) f->small_max = v; }
   if (const char *t = getenv("MMP_LANE_BUDGET")) { int v = atoi(t); if (v >= 1 && v <= 4096) f->lane_budget = v; }
-  if (const char *t = getenv("MMP_SHARD_CHUNKS")) f->shard_chunks = atoi(t);
-  if (f->lane_mode & 2) { CK(f->d_dbg.ensure(128)); CK(cudaMemset(f->d_dbg.p, 0, 128)); }
-  if (const char *t = getenv("MMP_TILE")) { int v = atoi(t); if (v == 8 || v == 16 || v == 32) f->tile = v; }
   *out = f.release();
   return MMP_OK;
 }
@@ -1854,15 +1777,6 @@ void mmp_fleet_destroy(mmp_fleet *f) {
   cudaSetDevice(f->device);
   { std::lock_guard<std::mutex> lk(f->srv.mu); server_stop(f); if (f->srv.stream) cudaStreamDestroy(f->srv.stream); if (f->srv.mapped) cudaFreeHost(f->srv.mapped); f->srv.mapped = nullptr; }
   cudaDeviceSynchronize();
-  if ((f->lane_mode & 2) && f->d_dbg.p) {  // MMP_LANE_MODE bit 1: print the per-phase averages of k_place_lanes
-    unsigned long long h[9];
-    if (cudaMemcpy(h, f->d_dbg.p, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess && h[7]) {
-      static const char *nm[7] = {"wait-for-stage", "issue", "context", "flight-left", "copy-out+release", "requests", "decide+store"};
-      fprintf(stderr, "[k_place_lanes phases, cycles per warp step over %llu steps]", h[7]);
-      for (int k = 0; k < 7; k++) fprintf(stderr, " %s=%.0f", nm[k], (double)h[k] / (double)h[7]);
-      fprintf(stderr, " warp-redone decisions=%llu (%.2f%% of %llu)\n", h[8], 100.0 * (double)h[8] / (32.0 * (double)h[7]), 32 * h[7]);
-    }
-  }
   if (f->comm && nccl_api().ok) { nccl_api().CommDestroy(f->comm); f->comm = nullptr; }
   for (auto &c : f->ctx_free) { destroy_ctx(c.get()); }
   f->ctx_free.clear();
@@ -2240,11 +2154,9 @@ int32_t mmp_tune(mmp_fleet *f, const char *key, int64_t value) {
   if (!strcmp(key, "one_mode") && value >= 0 && value <= 3) f->one_mode = (int)value;
   else if (!strcmp(key, "server_life_us") && value >= 50 && value <= 1000000) f->srv.life_us = value;
   else if (!strcmp(key, "server_idle_us") && value >= 10 && value <= 1000000) f->srv.idle_us = value;
-  else if (!strcmp(key, "direct") && (value == 0 || value == 1)) f->direct = (int)value;
+  else if (!strcmp(key, "direct") && (value == 0 || value == 1)) f->kernel = value ? PlaceKernel::direct : PlaceKernel::lanes;
   else if (!strcmp(key, "sort_slots") && value >= 0 && value <= 2) f->sort_slots = (int)value;
-  else if (!strcmp(key, "small_max") && value >= 0 && value <= (1 << 24)) f->small_max = (int)value;
   else if (!strcmp(key, "lane_budget") && value >= 1 && value <= 4096) f->lane_budget = (int)value;
-  else if (!strcmp(key, "lane_warps") && (value == 0 || value == 8 || value == 10 || value == 12 || value == 14 || value == 16 || value == 20)) f->lane_warps = (int)value;
   else if (!strcmp(key, "commit_host_only") && (value == 0 || value == 1)) f->commit_host_only = (int)value;
   else { g_err = "unknown key or value out of range"; return MMP_E_ARG; }
   return MMP_OK;

@@ -1,7 +1,7 @@
-"""k_place_direct launch shapes against the oracle: each resident-blocks instantiation (MMP_DIRECT_MINB = 4, 6, 8), the
-automatic switch to 8 blocks per SM for launches of 6..8 blocks per SM, batch sizes around the warp, block and
-slot-sort edges with and without the slot sort, and an overflow-heavy fleet whose inline edges sit at the word edges and
-the edge of the 12-word window, decided by pods that hold the model beyond that window (self's word from RowRanks)."""
+"""k_place_direct launch shapes against the oracle: sweeps and mixed batches on C3 and C5, batch sizes around the warp,
+block and slot-sort edges with and without the slot sort, and an overflow-heavy fleet whose inline edges sit at the word
+edges and the edge of the 12-word window, decided by pods that hold the model beyond that window (self's word from
+RowRanks)."""
 import numpy as np
 import pytest
 
@@ -26,30 +26,13 @@ def _kw(sd):
 
 
 @pytest.mark.parametrize("config,seed", [("C3", 3), ("C5", 5)])
-def test_each_minb_instantiation_matches_oracle(product_lib, oracle_lib, monkeypatch, config, seed):
+def test_sweep_and_mixed_batches_match_oracle(product_lib, oracle_lib, config, seed):
     fl = make_fleet(config, 3000, 10_000, seed)
     o = oracle_from_synth(fl)
-    batches = [make_decisions(fl, 20_000, seed, sweep=True, plain=True), make_decisions(fl, 20_000, seed + 1)]
-    want = [_oracle(fl, sd, o, seed) for sd in batches]
-    for minb in (4, 6, 8):
-        monkeypatch.setenv("MMP_DIRECT_MINB", str(minb))  # read at mmp_fleet_create
-        s = solver_from_synth(fl, product_lib)
-        for sd, w in zip(batches, want):
-            _same(s.place_batch(sd.dec, fl.now_ms, seed, **_kw(sd)), w, (config, minb))
-        s.close()
-
-
-def test_automatic_switch_to_eight_blocks_per_sm(product_lib, oracle_lib):
-    """launch_place runs k_place_direct<4, 8> when 6·SM < ceil(n/128) <= 8·SM: one wave at 8 blocks per SM."""
-    import torch
-    sm = torch.cuda.get_device_properties(0).multi_processor_count
-    n = 128 * 7 * sm - 5
-    assert 6 * sm < (n + 127) // 128 <= 8 * sm
-    fl = make_fleet("C3", 20_000, 10_000, 31)
-    o = oracle_from_synth(fl)
     s = solver_from_synth(fl, product_lib)
-    for sd, seed in ((make_decisions(fl, n, 31, sweep=True, plain=True), 4), (make_decisions(fl, n, 32), 5)):
-        _same(s.place_batch(sd.dec, fl.now_ms, seed, **_kw(sd)), _oracle(fl, sd, o, seed), ("switch", n, seed))
+    for sd in (make_decisions(fl, 20_000, seed, sweep=True, plain=True), make_decisions(fl, 20_000, seed + 1)):
+        _same(s.place_batch(sd.dec, fl.now_ms, seed, **_kw(sd)), _oracle(fl, sd, o, seed), config)
+    s.close()
 
 
 def test_batch_sizes_at_warp_block_and_sort_edges(product_lib, oracle_lib):

@@ -146,31 +146,37 @@ def test_sharded_matches_unsharded(product_lib, world):
     assert peer_words > 0  # ... and so were reads from peers' column blocks
 
 
+def _place_batch_device(fleet, dec, now_ms):
+    """mmp_place_batch_device on records uploaded to device memory, seed 77"""
+    import ctypes as C
+    from modelmesh_b200._lib import DECISION_OUT
+    lib = fleet.lib
+    dec = np.ascontiguousarray(dec)
+    d_in, d_out = C.c_void_p(), C.c_void_p()
+    fleet._ck(lib.mmp_device_alloc(fleet.h, dec.nbytes, C.byref(d_in)))
+    fleet._ck(lib.mmp_device_alloc(fleet.h, len(dec) * DECISION_OUT.itemsize, C.byref(d_out)))
+    try:
+        fleet._ck(lib.mmp_device_upload(fleet.h, d_in, dec.ctypes.data_as(C.c_void_p), dec.nbytes))
+        ms = C.c_float()
+        fleet._ck(lib.mmp_place_batch_device(fleet.h, d_in, len(dec), d_out, now_ms, 77, C.byref(ms)))
+        got = np.zeros(len(dec), dtype=DECISION_OUT)
+        fleet._ck(lib.mmp_device_download(fleet.h, got.ctypes.data_as(C.c_void_p), d_out, got.nbytes))
+        return got
+    finally:
+        fleet._ck(lib.mmp_device_free(fleet.h, d_in)); fleet._ck(lib.mmp_device_free(fleet.h, d_out))
+
+
 @pytest.mark.gpu
 def test_single_shard_takes_the_collective_path(product_lib, oracle_lib):
     """One GPU: a fleet of ONE shard that connects (ncclCommInitRank with one rank) sends its batches through the same
     keys -> ncclAllReduce(min) -> decode path as a sharded fleet, over whole rows, from each of the three batch entry
     points (mmp_place_batch, mmp_place_sweep, mmp_place_batch_device).  Results must equal the plain path's (and the
     oracle's), including decisions the lane routine hands to the cooperative routine."""
-    import ctypes as C
     import sys
     sys.path.insert(0, os.path.dirname(__file__))
     from helpers import oracle_from_synth, oracle_inputs_fast
-    from modelmesh_b200._lib import DECISION_OUT, DF_FAVOUR_SELF
+    from modelmesh_b200._lib import DF_FAVOUR_SELF
     from modelmesh_b200.fleet import Fleet
-
-    def place_batch_device(fleet, dec):
-        dec = np.ascontiguousarray(dec)
-        d_in, d_out = C.c_void_p(), C.c_void_p()
-        fleet._ck(product_lib.mmp_device_alloc(fleet.h, dec.nbytes, C.byref(d_in)))
-        fleet._ck(product_lib.mmp_device_alloc(fleet.h, len(dec) * DECISION_OUT.itemsize, C.byref(d_out)))
-        fleet._ck(product_lib.mmp_device_upload(fleet.h, d_in, dec.ctypes.data_as(C.c_void_p), dec.nbytes))
-        ms = C.c_float()
-        fleet._ck(product_lib.mmp_place_batch_device(fleet.h, d_in, len(dec), d_out, fl.now_ms, 77, C.byref(ms)))
-        got = np.zeros(len(dec), dtype=DECISION_OUT)
-        fleet._ck(product_lib.mmp_device_download(fleet.h, got.ctypes.data_as(C.c_void_p), d_out, got.nbytes))
-        fleet._ck(product_lib.mmp_device_free(fleet.h, d_in)); fleet._ck(product_lib.mmp_device_free(fleet.h, d_out))
-        return got
 
     for config, nm, ni, seed in [("C3", 40_000, 10_000, 3), ("C5", 3000, 5000, 5), ("MIX", 500, 300, 14)]:
         fl = make_fleet(config, nm, ni, seed)
@@ -189,11 +195,51 @@ def test_single_shard_takes_the_collective_path(product_lib, oracle_lib):
                 fav = (sd.dec["flags"] & DF_FAVOUR_SELF) != 0
                 assert np.array_equal(f.place_sweep(0, len(sd.dec), sd.dec["self"], fl.now_ms, 77, favour=fav),
                                       plain_f.place_sweep(0, len(sd.dec), sd.dec["self"], fl.now_ms, 77, favour=fav))
-                assert np.array_equal(place_batch_device(f, sd.dec), want)
-                assert np.array_equal(place_batch_device(plain_f, sd.dec), want)
+                assert np.array_equal(_place_batch_device(f, sd.dec, fl.now_ms), want)
+                assert np.array_equal(_place_batch_device(plain_f, sd.dec, fl.now_ms), want)
         assert f.shard_open_decisions() == 0  # a single shard's range is the whole row: no walk can leave it
         o = oracle_from_synth(fl)
         od, off, idx = oracle_inputs_fast(fl, sd)
         res = o.get_next_batch(od, fl.type_names, off, idx, fl.now_ms, 77, fresh=sd.fresh if len(sd.fresh) else None)
         assert np.array_equal(got["target"], res["target"]) and np.array_equal(got["n_candidates"], res["n_candidates"])
+        f.close(); plain_f.close()
+
+
+@pytest.mark.gpu
+def test_collective_path_refuses_rows_it_cannot_stage(product_lib, oracle_lib):
+    """One GPU: the collective path's key and gather passes run on k_place_lanes, whose landing stages hold rows of at most
+    580 words: rows of 576 words, fleets of up to 18 432 instances.  A connected one-shard fleet of 18 432 instances places like its
+    unconnected twin and the oracle from all three batch entry points; at 18 433 instances (rows of 608 words) all three
+    refuse with MMP_E_STATE, and the unconnected twin still places the batch as the oracle does."""
+    import sys
+    sys.path.insert(0, os.path.dirname(__file__))
+    from helpers import oracle_from_synth, oracle_inputs_fast
+    from modelmesh_b200._lib import DF_FAVOUR_SELF, E_STATE
+    from modelmesh_b200.fleet import Fleet, MmpError
+
+    for ni in (18_432, 18_433):
+        fl = make_fleet("C3", 3000, ni, 3)
+        plain_f = Fleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, fl.n_instances, fl.n_models, lib=product_lib)
+        load_into_fleet(fl, plain_f)
+        f = Fleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, fl.n_instances, fl.n_models, lib=product_lib)
+        load_into_fleet(fl, f)
+        f.shard_connect(f.shard_unique_id())
+        sd = make_decisions(fl, fl.n_models, 3, sweep=True, plain=True)
+        fav = (sd.dec["flags"] & DF_FAVOUR_SELF) != 0
+        want = plain_f.place_batch(sd.dec, fl.now_ms, 77)
+        od, off, idx = oracle_inputs_fast(fl, sd)
+        res = oracle_from_synth(fl).get_next_batch(od, fl.type_names, off, idx, fl.now_ms, 77)
+        assert np.array_equal(want["target"], res["target"]) and np.array_equal(want["n_candidates"], res["n_candidates"])
+        calls = {"batch": lambda: f.place_batch(sd.dec, fl.now_ms, 77),
+                 "sweep": lambda: f.place_sweep(0, len(sd.dec), sd.dec["self"], fl.now_ms, 77, favour=fav),
+                 "device": lambda: _place_batch_device(f, sd.dec, fl.now_ms)}
+        if ni == 18_432:
+            assert np.array_equal(calls["batch"](), want)
+            assert np.array_equal(calls["sweep"](), plain_f.place_sweep(0, len(sd.dec), sd.dec["self"], fl.now_ms, 77, favour=fav))
+            assert np.array_equal(calls["device"](), want)
+        else:
+            for name, call in calls.items():
+                with pytest.raises(MmpError, match="rows of 608 words are wider than the 580 words the collective path can stage") as e:
+                    call()
+                assert e.value.code == E_STATE, name
         f.close(); plain_f.close()

@@ -1,5 +1,5 @@
-"""Request-model decisions (MMP_DF_REQUEST_MODEL) on every placement path of the H100 library: k_place_direct at each
-resident-blocks instantiation and in slot order, k_place_lanes, the traced tile kernel, the B = 1 paths (k_place_small
+"""Request-model decisions (MMP_DF_REQUEST_MODEL) on every placement path of the H100 library: k_place_direct in batch
+and in slot order, k_place_lanes, the traced tile kernel, the B = 1 paths (k_place_small
 as a launch and as a graph, k_place_server with its inline extras and with the mapped tables), the micro-batcher, mixed
 batches; a model registered or changed after the last commit; instance-sharded fleets (>= 2 GPUs).
 
@@ -55,32 +55,27 @@ FLEETS = [("C3", 3000, 10_000, 3), ("C5", 3000, 10_000, 5), ("MIX", 500, 700, 41
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", FLEETS)
-def test_direct_each_minb_lanes_and_slot_order(product_lib, oracle_lib, monkeypatch, config, nm, ni, seed):
+def test_direct_each_minb_lanes_and_slot_order(product_lib, oracle_lib, config, nm, ni, seed):
     fl, s, o, sd, rq, flagged, rw, seed = _setup(product_lib, config, nm, ni, seed)
     assert flagged.mean() > 0.95
     tid = {t: s.type_id(t) for t in fl.type_names}
+    _check(s, fl, sd, rq, rw, seed, (config, "direct"))
+    # slot-sorted launches (>= 8192 decisions): the sort key of a request-model decision is its own type id
+    big = make_decisions(fl, 9000, seed + 9)
+    brq, _ = as_request_model(fl, big, tid)
+    for sort in (0, 1):
+        s._ck(product_lib.mmp_tune(s.h, b"sort_slots", sort))
+        _same(s.place_batch(brq.dec, fl.now_ms, 2, **_kw(brq)), s.place_batch(big.dec, fl.now_ms, 2, **_kw(big)), ("sorted (a)", sort))
+    rnd, want = rw
+    rep = SynthDecisions(np.concatenate([rnd.dec, rnd.dec]), rnd.fresh, rnd.extra)  # 12 000 decisions: sorted too
+    s._ck(product_lib.mmp_tune(s.h, b"sort_slots", 1))
+    got = s.place_batch(rep.dec, fl.now_ms, seed, **_kw(rep))
+    _same(got[:len(rnd.dec)], want, ("sorted (b)", config))
+    s._ck(product_lib.mmp_tune(s.h, b"sort_slots", 2))
+    s._ck(product_lib.mmp_tune(s.h, b"direct", 0))  # k_place_lanes: the rows through the TMA landing stages
+    _check(s, fl, sd, rq, rw, seed, (config, "lanes"))
+    s._ck(product_lib.mmp_tune(s.h, b"direct", 1))
     s.close()
-    for minb in (4, 6, 8):
-        monkeypatch.setenv("MMP_DIRECT_MINB", str(minb))  # read at mmp_fleet_create
-        s = solver_from_synth(fl, product_lib)  # (same ingest order: the same type ids)
-        _check(s, fl, sd, rq, rw, seed, (config, "direct", minb))
-        if minb == 6:
-            # slot-sorted launches (>= 8192 decisions): the sort key of a request-model decision is its own type id
-            big = make_decisions(fl, 9000, seed + 9)
-            brq, _ = as_request_model(fl, big, tid)
-            for sort in (0, 1):
-                s._ck(product_lib.mmp_tune(s.h, b"sort_slots", sort))
-                _same(s.place_batch(brq.dec, fl.now_ms, 2, **_kw(brq)), s.place_batch(big.dec, fl.now_ms, 2, **_kw(big)), ("sorted (a)", sort))
-            rnd, want = rw
-            rep = SynthDecisions(np.concatenate([rnd.dec, rnd.dec]), rnd.fresh, rnd.extra)  # 12 000 decisions: sorted too
-            s._ck(product_lib.mmp_tune(s.h, b"sort_slots", 1))
-            got = s.place_batch(rep.dec, fl.now_ms, seed, **_kw(rep))
-            _same(got[:len(rnd.dec)], want, ("sorted (b)", config))
-            s._ck(product_lib.mmp_tune(s.h, b"sort_slots", 2))
-            s._ck(product_lib.mmp_tune(s.h, b"direct", 0))  # k_place_lanes: the rows through the TMA landing stages
-            _check(s, fl, sd, rq, rw, seed, (config, "lanes"))
-            s._ck(product_lib.mmp_tune(s.h, b"direct", 1))
-        s.close()
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", FLEETS)
