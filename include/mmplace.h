@@ -197,6 +197,21 @@ int32_t mmp_place_batch(mmp_fleet *, const mmp_decision_in *in, int32_t n, const
 int32_t mmp_place_batch_trace(mmp_fleet *, const mmp_decision_in *in, int32_t n, const mmp_instance_row *fresh,
                               int32_t n_fresh, const int32_t *extra, int32_t n_extra, mmp_decision_out *out,
                               mmp_decision_trace *trace, uint32_t *cand_mask, int64_t now_ms, uint64_t seed);
+/* Same with a CALL-WIDE exclude set of any size: every decision of the call behaves as if exclude[0, n_exclude) (instance
+ * indices) were added to its CacheMissExcludeSet -- the rate-tracking scale-up's getExcludeSet() ∪ copies (MM:5771-5806,
+ * 5835-5856), the janitor's every-copy-plus-self (MM:6915-6927), chained ensureLoadedElsewhere targets (MM:4575-4584) --
+ * on top of its own extras (still <= MMP_MAX_EXTRA) and MMP_DF_* flags.  Its members leave the filtered iterator like
+ * instances the type does not allow (MM:4760-4771).  trace / cand_mask may be NULL and mean what they mean for
+ * mmp_place_batch_trace.  Duplicate ids are allowed; ids of instances that are not live are ignored.  An id outside
+ * [0, max_instances), or exclude == NULL with n_exclude > 0, fails the call with MMP_E_ARG before anything is written.
+ * n_exclude == 0 is exactly mmp_place_batch / _trace.  A call with a set that would take the instance-sharded path (an
+ * instance-sharded fleet, or an untraced call on one that connected a communicator) fails with MMP_E_STATE.
+ * Latency: the call derives its own copy of the per-type-slot tables on the device (two small launches), so a batch of
+ * <= 32 decisions skips the resident server and the captured graph (one_mode 2 / 3, which hold the epoch's tables) and is
+ * launched as k_place_small (one_mode 0: the batch kernel).  The micro-batcher never sees such calls. */
+int32_t mmp_place_batch_excluding(mmp_fleet *, const mmp_decision_in *in, int32_t n, const mmp_instance_row *fresh, int32_t n_fresh,
+                                  const int32_t *extra, int32_t n_extra, const int32_t *exclude, int32_t n_exclude,
+                                  mmp_decision_out *out, mmp_decision_trace *trace, uint32_t *cand_mask, int64_t now_ms, uint64_t seed);
 /* Registry sweep -- the reference's natural batched caller: the leader's reaper walks the registry and calls
  * ensureLoadedInternal per model (MM:6616-6735), i.e. getNext for model first_model + i on behalf of instance self[i]
  * (self_stride = 1) or of one instance for the whole sweep (self_stride = 0: self[0]), lastUsedTime from the model record,

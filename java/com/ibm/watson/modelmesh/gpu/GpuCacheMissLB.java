@@ -41,7 +41,7 @@ public abstract class GpuCacheMissLB implements LoadBalancer {
         try {
             chosen = gpu.placeOne(host.requestModelType(), host.requestLoadedAndFailed(), host.instanceId(), host.requestLastUsedTime(),
                     host.requestFavourSelf(), host.freshInstanceRecord(), host.requestExcludes(), System.currentTimeMillis());
-        } catch (RuntimeException e) {  // library error, or more than MMP_MAX_EXTRA ids to exclude
+        } catch (RuntimeException e) {  // library error
             return host.fallback(sis, method, args);
         }
         if (chosen == null) return null;                                      // MM:4796, 4941: "Nowhere available to load" upstream

@@ -96,7 +96,9 @@ public final class GpuPlacement implements AutoCloseable {
      * The model travels as the record this request read (MMP_DF_REQUEST_MODEL): its type and its loaded ∪ failed instances,
      * as the reference builds the CacheMissExcludeSet from the record (MM:3537, 3782-3785), so a model registered or changed
      * since the last commit is placed on its current record.  Instance ids the dictionary does not know are dropped (they
-     * name no live instance); more than MMP_MAX_EXTRA ids in all throws, and GpuCacheMissLB falls back to the Java LB.
+     * name no live instance).  Up to MMP_MAX_EXTRA ids travel as the decision's extras; more (a scale-up's exclude set, the
+     * janitor's every-copy-plus-self, a long chain of ensureLoadedElsewhere targets) travel all together as the call's
+     * exclude set (mmp_place_batch_excluding, a batch of one with no extras), which excludes them the same way.
      */
     public String placeOne(String modelType, java.util.Set<String> loadedAndFailed, String selfId, long lastUsedTime, boolean favourSelf,
                            InstanceRecord fresh, java.util.Set<String> requestExcludes, long nowMs) {
@@ -111,19 +113,23 @@ public final class GpuPlacement implements AutoCloseable {
                 for (String e : set) {
                     Integer i = instanceIdx.get(e);
                     if (i == null) continue;
-                    if (n == extra.length) throw new IllegalStateException("more than " + MmPlace.MAX_EXTRA + " instances to exclude");
+                    if (n == extra.length) extra = java.util.Arrays.copyOf(extra, 2 * n);
                     extra[n++] = i;
                 }
         }
         if (self == null) return null;
+        final boolean asSet = n > MmPlace.MAX_EXTRA;
         ByteBuffer[] s = scratch.get();
         ByteBuffer in = s[0], fr = s[1], out = s[2];
         in.clear();
         in.putInt(type).putInt(self).putLong(lastUsedTime).putInt(MmPlace.DF_REQUEST_MODEL | (favourSelf ? MmPlace.DF_FAVOUR_SELF : 0))
-          .putInt(fresh != null ? 0 : -1).putInt(0).putInt(n);
+          .putInt(fresh != null ? 0 : -1).putInt(0).putInt(asSet ? 0 : n);
         extra = java.util.Arrays.copyOf(extra, n);
         if (fresh != null) encode(fresh, true, fr);
-        int rc = MmPlace.placeOne(h, in, fresh != null ? fr : null, extra.length > 0 ? extra : null, out, nowMs, pickSeed.incrementAndGet());
+        int rc = asSet
+                ? MmPlace.placeBatchExcluding(h, in, 1, fresh != null ? fr : null, fresh != null ? 1 : 0, null, 0, extra, out, null, null, nowMs,
+                                              pickSeed.incrementAndGet())
+                : MmPlace.placeOne(h, in, fresh != null ? fr : null, extra.length > 0 ? extra : null, out, nowMs, pickSeed.incrementAndGet());
         if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h));  // the caller falls back to the Java load balancer
         int target = out.getInt(0);
         if (target == MmPlace.TARGET_SELF) return SELF;

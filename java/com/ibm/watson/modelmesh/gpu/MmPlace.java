@@ -50,6 +50,8 @@ final class MmPlace {
                                  long nowMs, long seed);
     static native int placeBatchTrace(long h, ByteBuffer in, int n, ByteBuffer fresh, int nFresh, ByteBuffer extra, int nExtra,
                                       ByteBuffer out, ByteBuffer trace, ByteBuffer candMask, long nowMs, long seed);
+    static native int placeBatchExcluding(long h, ByteBuffer in, int n, ByteBuffer fresh, int nFresh, ByteBuffer extra, int nExtra,
+                                          int[] exclude, ByteBuffer out, ByteBuffer trace, ByteBuffer candMask, long nowMs, long seed);
     static native int placeSweep(long h, int firstModel, int n, ByteBuffer self, int selfStride, ByteBuffer favourBits, ByteBuffer out,
                                  long nowMs, long seed);
     static native int placeOne(long h, ByteBuffer in, ByteBuffer fresh, int[] extra, ByteBuffer out, long nowMs, long seed);

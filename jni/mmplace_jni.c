@@ -170,6 +170,18 @@ jint FN(placeBatchTrace)(JNIEnv *env, jclass c, jlong h, jobject in, jint n, job
                                (const int32_t *)BUF(extra), nExtra, (mmp_decision_out *)BUF(out), (mmp_decision_trace *)BUF(trace),
                                (uint32_t *)BUF(candMask), nowMs, (uint64_t)seed);
 }
+/* a call-wide exclude set (int[] of instance indices, or null) on top of every decision's own exclusions; trace / candMask may be null */
+jint FN(placeBatchExcluding)(JNIEnv *env, jclass c, jlong h, jobject in, jint n, jobject fresh, jint nFresh, jobject extra, jint nExtra,
+                             jintArray exclude, jobject out, jobject trace, jobject candMask, jlong nowMs, jlong seed) {
+  jsize nx = exclude ? (*env)->GetArrayLength(env, exclude) : 0;
+  jint *px = nx ? (jint *)(*env)->GetPrimitiveArrayCritical(env, exclude, NULL) : NULL;
+  jint rc = mmp_place_batch_excluding(H(h), (const mmp_decision_in *)BUF(in), n, (const mmp_instance_row *)BUF(fresh), nFresh,
+                                      (const int32_t *)BUF(extra), nExtra, (const int32_t *)px, nx, (mmp_decision_out *)BUF(out),
+                                      (mmp_decision_trace *)BUF(trace), (uint32_t *)BUF(candMask), nowMs, (uint64_t)seed);
+  (void)c;
+  if (px) (*env)->ReleasePrimitiveArrayCritical(env, exclude, px, JNI_ABORT);
+  return rc;
+}
 jint FN(placeSweep)(JNIEnv *env, jclass c, jlong h, jint first, jint n, jobject self, jint selfStride, jobject favour, jobject out,
                     jlong nowMs, jlong seed) {
   (void)c;

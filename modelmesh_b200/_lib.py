@@ -111,6 +111,7 @@ SYMBOLS = [
     ("mmp_fleet_commit", _I32, [_P]),
     ("mmp_place_batch", _I32, [_P, _P, _I32, _P, _I32, _P, _I32, _P, _I64, _U64]),
     ("mmp_place_batch_trace", _I32, [_P, _P, _I32, _P, _I32, _P, _I32, _P, _P, _P, _I64, _U64]),
+    ("mmp_place_batch_excluding", _I32, [_P, _P, _I32, _P, _I32, _P, _I32, _P, _I32, _P, _P, _P, _I64, _U64]),
     ("mmp_place_one", _I32, [_P, _P, _P, _P, _P, _I64, _U64]),
     ("mmp_place_sweep", _I32, [_P, _I32, _I32, _P, _I32, _P, _P, _I64, _U64]),
     ("mmp_place_batch_device", _I32, [_P, _P, _I32, _P, _I64, _U64, C.POINTER(C.c_float)]),

@@ -174,6 +174,31 @@ __global__ void k_slot_lists(const uint32_t *__restrict__ cand, const uint32_t *
   cand_before[sl] = before;
 }
 
+// A call-wide exclude set (mmp_place_batch_excluding): the snapshot's per-slot candidate, replicaset-filtered and preferred
+// masks with the set's ranks cleared, into the call's own tables.  An excluded instance then leaves the filter exactly as one
+// the type does not allow (MM:4760-4771), so the decision routine runs unchanged on a view of these tables.  One block per
+// type slot; each builds the set's rank-space mask in shared memory (row_words words, at most 8 KB) from the instance
+// indices, which the host has checked against [0, max_instances).  Indices of instances that are not live have no rank.
+__global__ void k_exclude_slots(const int32_t *__restrict__ ids, int n_ids, const int32_t *__restrict__ rank_of, int row_words,
+                                const uint32_t *__restrict__ cand, const uint32_t *__restrict__ candx, const uint32_t *__restrict__ pref,
+                                uint32_t *__restrict__ x_cand, uint32_t *__restrict__ x_candx, uint32_t *__restrict__ x_pref) {
+  extern __shared__ uint32_t xm[];
+  for (int w = threadIdx.x; w < row_words; w += blockDim.x) xm[w] = 0u;
+  __syncthreads();
+  for (int k = threadIdx.x; k < n_ids; k += blockDim.x) {
+    const int r = rank_of[ids[k]];
+    if (r >= 0) atomicOr(&xm[r >> 5], 1u << (r & 31));
+  }
+  __syncthreads();
+  const size_t so = (size_t)blockIdx.x * row_words;
+  for (int w = threadIdx.x; w < row_words; w += blockDim.x) {
+    const uint32_t keep = ~xm[w];
+    x_cand[so + w] = cand[so + w] & keep;
+    x_candx[so + w] = candx[so + w] & keep;
+    x_pref[so + w] = pref[so + w] & keep;
+  }
+}
+
 // deltas of a non-structural commit
 __global__ void k_scatter_inst_rows(const int32_t *__restrict__ idx, const mmp_instance_row *__restrict__ src, int n,
                                     mmp_instance_row *__restrict__ rows) {

@@ -454,26 +454,8 @@ class HostState {
     s.type_slot_hp.resize(s.type_slot.size());
     for (size_t t = 0; t < s.type_slot.size(); t++)
       s.type_slot_hp[t] = (uint16_t)(s.type_slot[t] | (s.has_pref[s.type_slot[t]] ? 0x8000u : 0u));
-    s.nzw.assign((size_t)s.n_slots * RW, 0xffff);
-    s.nz_n.assign((size_t)s.n_slots, 0);
-    for (int32_t sl = 0; sl < s.n_slots; sl++) {
-      const uint32_t *cx = (s.any_rs ? s.candx.data() : s.cand.data()) + (size_t)sl * RW;
-      int32_t k = 0, skip = 0;
-      for (int32_t w = s.word_lo; w < s.word_hi; w++)
-        if (cx[w]) { s.nzw[(size_t)sl * RW + k++] = (uint16_t)w; if (w < s.word_lo + MMP_LANE_WIN) skip++; }
-      s.nz_n[sl] = k | (skip << 24);  // (place_core.cuh nz_count / nz_skipped)
-    }
-    if (cfg.shard_count > 1) {
-      s.nzw_full.assign((size_t)s.n_slots * RW, 0xffff);
-      s.nz_n_full.assign((size_t)s.n_slots, 0);
-      for (int32_t sl = 0; sl < s.n_slots; sl++) {
-        const uint32_t *cx = (s.any_rs ? s.candx.data() : s.cand.data()) + (size_t)sl * RW;
-        int32_t k = 0, skip = 0;
-        for (int32_t w = 0; w < RW; w++)
-          if (cx[w]) { s.nzw_full[(size_t)sl * RW + k++] = (uint16_t)w; if (w < MMP_LANE_WIN) skip++; }
-        s.nz_n_full[sl] = k | (skip << 24);
-      }
-    }
+    slot_word_lists(s, s.word_lo, s.word_hi, s.nzw, s.nz_n);
+    if (cfg.shard_count > 1) slot_word_lists(s, 0, RW, s.nzw_full, s.nz_n_full);
     s.part_type_ids.assign(s.part_types.size(), {});
     for (size_t p = 0; p < s.part_types.size(); p++)
       for (const std::string &t : s.part_types[p]) {
@@ -484,6 +466,21 @@ class HostState {
     for (int32_t sl = 0; sl < s.n_slots; sl++)
       for (int32_t w = 0; w < s.word_lo; w++) s.candx_before[sl] += __builtin_popcount(s.candx[(size_t)sl * RW + w]);
     return nullptr;
+  }
+
+  // Compressed word lists of s's candidate masks (the host side of k_slot_lists): per slot the row words of [lo, hi) in which
+  // the mask the lane routine reads (candx when a replicaset is flagged, else cand) has any bit, ascending, then 0xffff
+  static void slot_word_lists(const HostSnapshot &s, int32_t lo, int32_t hi, std::vector<uint16_t> &nzw, std::vector<int32_t> &nz_n) {
+    const int32_t RW = s.row_words;
+    nzw.assign((size_t)s.n_slots * RW, 0xffff);
+    nz_n.assign((size_t)s.n_slots, 0);
+    for (int32_t sl = 0; sl < s.n_slots; sl++) {
+      const uint32_t *cx = (s.any_rs ? s.candx.data() : s.cand.data()) + (size_t)sl * RW;
+      int32_t k = 0, skip = 0;
+      for (int32_t w = lo; w < hi; w++)
+        if (cx[w]) { nzw[(size_t)sl * RW + k++] = (uint16_t)w; if (w < lo + MMP_LANE_WIN) skip++; }
+      nz_n[sl] = k | (skip << 24);  // (place_core.cuh nz_count / nz_skipped)
+    }
   }
 
   // Contiguous rank ranges per instance shard, in whole 16-byte granules (TMA bulk copies): shard k of n holds row words

@@ -1145,6 +1145,9 @@ struct PlaceCtx {
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
   int32_t graph_epoch = -1;
+  // a call-wide exclude set (mmp_place_batch_excluding): its ids and the per-slot tables derived from the snapshot's
+  // (k_exclude_slots, k_slot_lists) that the call's view points at
+  DevBuf d_xids, d_xcand, d_xcandx, d_xpref, d_xnzw, d_xnz_n, d_xbefore;
 };
 
 // The scoring kernel of untraced batches (MMP_KERNEL = direct | lanes | tile; launch_place): k_place_direct (rows rebuilt
@@ -1272,7 +1275,8 @@ class CtxLease {
 };
 static void destroy_ctx(PlaceCtx *c) {
   for (DevBuf *b : {&c->d_in, &c->d_out, &c->d_fresh, &c->d_extra, &c->d_trace, &c->d_cand, &c->d_open_flag,
-                    &c->d_open_idx, &c->d_n_open, &c->d_cub, &c->d_blocks, &c->d_gathered, &c->d_rows, &c->d_in_open, &c->d_out_open})
+                    &c->d_open_idx, &c->d_n_open, &c->d_cub, &c->d_blocks, &c->d_gathered, &c->d_rows, &c->d_in_open, &c->d_out_open,
+                    &c->d_xids, &c->d_xcand, &c->d_xcandx, &c->d_xpref, &c->d_xnzw, &c->d_xnz_n, &c->d_xbefore})
     b->release();
   for (int k = 0; k < PlaceCtx::NSORT; k++) { c->d_skey[k].release(); c->d_skey2[k].release(); c->d_sidx[k].release(); c->d_sidx2[k].release(); c->d_stmp[k].release(); }
   if (c->e0) cudaEventDestroy(c->e0);
@@ -2272,10 +2276,11 @@ static int32_t place_server(mmp_fleet *f, const DeviceSnapshot &ds, const mmp_de
 
 // Tiny untraced, unsharded batches, zero-copy: the records, fresh rows (c->fresh_host) and extras are written into the
 // context's pinned mapped buffer, and the kernel reads them and writes its results there, so a call is one launch and one
-// synchronise with no copy calls.  The caller has checked that the batch fits the buffer.
-static int32_t place_mapped(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, const SnapshotView &vw, const mmp_decision_in *in, int32_t n,
-                            int32_t n_fresh, const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed) {
-  const bool fits32 = n <= 32 && n_fresh <= 32 && (size_t)n_extra <= 32 * MMP_MAX_EXTRA;
+// synchronise with no copy calls.  The caller has checked that the batch fits the buffer.  A view with the call's own
+// slot tables (`derived`: an exclude set) skips the resident server and the captured graph, which both hold the epoch's.
+static int32_t place_mapped(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, const SnapshotView &vw, bool derived, const mmp_decision_in *in,
+                            int32_t n, int32_t n_fresh, const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed) {
+  const bool fits32 = n <= 32 && n_fresh <= 32 && (size_t)n_extra <= 32 * MMP_MAX_EXTRA && !derived;
   if (f->one_mode == 3 && fits32) {
     std::unique_lock<std::mutex> lk(f->srv.mu, std::try_to_lock);
     if (lk.owns_lock()) return place_server(f, ds, in, n, c->fresh_host.data(), n_fresh, extra, n_extra, out, now_ms, seed);
@@ -2327,12 +2332,43 @@ static int32_t place_mapped(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds,
   return MMP_OK;
 }
 
+// The call's view on the derived slot tables of an exclude set: k_exclude_slots clears the set's ranks from the snapshot's
+// cand / candx / pref, k_slot_lists builds their compressed word lists.  Queued on st; the ids are in host memory.
+static int32_t derive_exclude_tables(mmp_fleet *f, PlaceCtx *c, const int32_t *exclude, int32_t n_exclude, SnapshotView &vw, cudaStream_t st) {
+  const int32_t NS = vw.n_slots, RW = vw.row_words;
+  if (NS <= 0) return MMP_OK;  // (no live instance: no slot, nothing to derive)
+  const size_t words = (size_t)NS * RW;
+  CK(c->d_xids.ensure((size_t)n_exclude * 4));
+  CK(c->d_xcand.ensure(words * 4)); CK(c->d_xcandx.ensure(words * 4)); CK(c->d_xpref.ensure(words * 4));
+  CK(c->d_xnzw.ensure(words * 2)); CK(c->d_xnz_n.ensure((size_t)NS * 4)); CK(c->d_xbefore.ensure((size_t)NS * 4));
+  CK(cudaMemcpyAsync(c->d_xids.p, exclude, (size_t)n_exclude * 4, cudaMemcpyHostToDevice, st));
+  k_exclude_slots<<<NS, 256, (size_t)RW * 4, st>>>(c->d_xids.as<int32_t>(), n_exclude, vw.rank_of, RW, vw.cand, vw.candx, vw.pref,
+                                                   c->d_xcand.as<uint32_t>(), c->d_xcandx.as<uint32_t>(), c->d_xpref.as<uint32_t>());
+  k_slot_lists<<<(NS + 31) / 32, 32, 0, st>>>(c->d_xcand.as<uint32_t>(), c->d_xcandx.as<uint32_t>(), vw.any_rs, RW, NS, vw.word_lo, vw.word_hi,
+                                             c->d_xnzw.as<uint16_t>(), c->d_xnz_n.as<int32_t>(), c->d_xbefore.as<int32_t>());
+  f->launches += 2;
+  CK(cudaGetLastError());
+  vw.cand = c->d_xcand.as<uint32_t>(); vw.candx = c->d_xcandx.as<uint32_t>(); vw.pref = c->d_xpref.as<uint32_t>();
+  vw.nzw = c->d_xnzw.as<uint16_t>(); vw.nz_n = c->d_xnz_n.as<int32_t>(); vw.cand_before = c->d_xbefore.as<int32_t>();
+  return MMP_OK;
+}
+
+// The one host path of mmp_place_batch / _trace / _excluding / mmp_place_one.  exclude[0, n_exclude): the call-wide exclude
+// set; with n_exclude == 0 the call takes exactly the route it takes without one.
 static int32_t place_impl(mmp_fleet *f, const mmp_decision_in *in, int32_t n, const mmp_instance_row *fresh, int32_t n_fresh,
                           const int32_t *extra, int32_t n_extra, mmp_decision_out *out, mmp_decision_trace *trace,
-                          uint32_t *cand_mask, int64_t now_ms, uint64_t seed) {
+                          uint32_t *cand_mask, int64_t now_ms, uint64_t seed, const int32_t *exclude = nullptr, int32_t n_exclude = 0) {
   NEED(f);
   if (n < 0 || (n > 0 && (!in || !out)) || n_fresh < 0 || n_extra < 0 || (n_fresh > 0 && !fresh) || (n_extra > 0 && !extra)) {
     g_err = "bad argument"; return MMP_E_ARG;
+  }
+  if (n_exclude < 0 || (n_exclude > 0 && !exclude)) { g_err = "bad exclude set"; return MMP_E_ARG; }
+  for (int32_t k = 0; k < n_exclude; k++)
+    if (exclude[k] < 0 || exclude[k] >= f->hs.cfg.max_instances) {
+      g_err = "exclude set: instance index " + std::to_string(exclude[k]) + " outside [0, max_instances)"; return MMP_E_ARG;
+    }
+  if (n_exclude > 0 && places_sharded(f, trace || cand_mask)) {
+    g_err = "an exclude set is not available on an instance-sharded fleet or one that connected a communicator"; return MMP_E_STATE;
   }
   if (n == 0) return MMP_OK;
   int32_t rc = set_device(f);
@@ -2351,8 +2387,10 @@ static int32_t place_impl(mmp_fleet *f, const mmp_decision_in *in, int32_t n, co
   const bool fast_paths = !traced && !places_sharded(f, traced);  // the mapped tiny-batch path and the chunk pipeline apply
   SnapshotView vw = ds.view;
   vw.n_extra = n_extra;  // per call: the device checks every decision's extra[] slice against it (prepare_ctx_a)
+  if (n_exclude > 0 && (rc = derive_exclude_tables(f, c.get(), exclude, n_exclude, vw, st)) < 0) return rc;
   const size_t need = (size_t)n * (sizeof(mmp_decision_in) + sizeof(mmp_decision_out)) + (size_t)n_fresh * sizeof(FreshRow) + (size_t)n_extra * 4 + 64;
-  if (fast_paths && need <= PlaceCtx::MAPPED_BYTES) return place_mapped(f, c.get(), ds, vw, in, n, n_fresh, extra, n_extra, out, now_ms, seed);
+  if (fast_paths && need <= PlaceCtx::MAPPED_BYTES)
+    return place_mapped(f, c.get(), ds, vw, n_exclude > 0, in, n, n_fresh, extra, n_extra, out, now_ms, seed);
   CK(c->d_in.ensure((size_t)n * sizeof(mmp_decision_in)));
   CK(c->d_out.ensure((size_t)n * sizeof(mmp_decision_out)));
   if (trace) CK(c->d_trace.ensure((size_t)n * sizeof(mmp_decision_trace)));
@@ -2381,6 +2419,11 @@ int32_t mmp_place_batch_trace(mmp_fleet *f, const mmp_decision_in *in, int32_t n
                               const int32_t *extra, int32_t n_extra, mmp_decision_out *out, mmp_decision_trace *trace,
                               uint32_t *cand_mask, int64_t now_ms, uint64_t seed) {
   return place_impl(f, in, n, fresh, n_fresh, extra, n_extra, out, trace, cand_mask, now_ms, seed);
+}
+int32_t mmp_place_batch_excluding(mmp_fleet *f, const mmp_decision_in *in, int32_t n, const mmp_instance_row *fresh, int32_t n_fresh,
+                                  const int32_t *extra, int32_t n_extra, const int32_t *exclude, int32_t n_exclude, mmp_decision_out *out,
+                                  mmp_decision_trace *trace, uint32_t *cand_mask, int64_t now_ms, uint64_t seed) {
+  return place_impl(f, in, n, fresh, n_fresh, extra, n_extra, out, trace, cand_mask, now_ms, seed, exclude, n_exclude);
 }
 int32_t mmp_place_one(mmp_fleet *f, const mmp_decision_in *in, const mmp_instance_row *fresh, const int32_t *extra,
                       mmp_decision_out *out, int64_t now_ms, uint64_t seed) {

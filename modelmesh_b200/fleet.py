@@ -104,7 +104,9 @@ class Fleet:
     # ---- placement ----
     def place_batch(self, dec: np.ndarray, now_ms: int, seed: int, fresh: Optional[np.ndarray] = None,
                     extra: Optional[np.ndarray] = None, trace: bool = False, masks: bool = False,
-                    out: Optional[np.ndarray] = None):
+                    out: Optional[np.ndarray] = None, exclude: Optional[np.ndarray] = None):
+        """exclude: a call-wide exclude set (instance indices, any length) added to every decision's exclusions
+        (mmp_place_batch_excluding); None keeps the plain call, an array -- even an empty one -- takes that entry point."""
         dec = np.ascontiguousarray(dec, dtype=DECISION_IN)
         n = len(dec)
         if out is None:
@@ -113,6 +115,13 @@ class Fleet:
         extra_a = None if extra is None else np.ascontiguousarray(extra, dtype=np.int32)
         nf = 0 if fresh_a is None else len(fresh_a)
         ne = 0 if extra_a is None else len(extra_a)
+        if exclude is not None:
+            xs = np.ascontiguousarray(exclude, dtype=np.int32)
+            tr = np.zeros(n, dtype=DECISION_TRACE) if trace or masks else None
+            cm = np.zeros((n, 2, self.row_words()), dtype=np.uint32) if masks else None
+            self._ck(self.lib.mmp_place_batch_excluding(self.h, _ptr(dec), n, _ptr(fresh_a), nf, _ptr(extra_a), ne, _ptr(xs), len(xs),
+                                                        _ptr(out), _ptr(tr), _ptr(cm), now_ms, seed))
+            return out if tr is None else (out, tr, cm)
         if not trace and not masks:
             self._ck(self.lib.mmp_place_batch(self.h, _ptr(dec), n, _ptr(fresh_a), nf, _ptr(extra_a), ne, _ptr(out),
                                               now_ms, seed))
