@@ -380,8 +380,10 @@ int32_t mmp_churn_step(mmp_fleet *, const mmp_churn_event *ev, int32_t n, int64_
 /* registry state of one model as the device holds it: row + the 4 inline instance indices (first copy_count = loaded) */
 int32_t mmp_churn_model(mmp_fleet *, int32_t model, mmp_model_row *row, int32_t *instances4);
 /* ---- registry-side batch scans (SURVEY.md §8a row a14, §8f-2) ---- */
-/* MR.instanceIds / failedIn VALUES (load-start / failure times of the model's inline edges, same order as the ids given to
- * mmp_model_upsert) and MR.lastUnloadTime ("lul").  mmp_model_upsert_json takes them from the record.  0 = unknown. */
+/* MR.instanceIds / failedIn VALUES (load-start / failure times) and MR.lastUnloadTime ("lul").  edge_ts[i] is the time of the
+ * i-th id of the model's last mmp_model_upsert (loaded first, then failed), for every registration; times past the model's
+ * registration count are ignored, and a registration without one reads 0 (unknown).  A time stays with its position until the
+ * next call.  mmp_model_upsert_json takes them from the record. */
 int32_t mmp_model_times(mmp_fleet *, int32_t model, const int64_t *edge_ts, int32_t n, int64_t last_unload_time);
 /* One cache entry of one pod, as its rate-tracking / janitor tasks see it (CacheEntry counters are pod-local): */
 typedef struct {
@@ -408,7 +410,8 @@ typedef struct {
 } mmp_scale_params;
 typedef struct {
   int32_t action;          /* 0 nothing, 1 add a second copy (regular-usage trigger MM:5726-5758), 2 scale up by copies_to_load
-                              (MM:5760-5795), -1 the model has more registered instances than the device list holds: host path */
+                              (MM:5760-5795), -1 the entry's model or instance index is out of range, or its copy_count is saturated
+                              (255) while it holds more than 255 registrations: where the loaded copies end is unknown */
   int32_t copies_to_load;
   int64_t load_last_used;  /* lastUsed for the triggered loads: lastCheckTime (second copy) or now + 20 s (scale-up, MM:5675) */
   int32_t rpm, i1, i2;     /* measured rate; the updated usage iterations */
@@ -417,16 +420,24 @@ typedef struct {
 } mmp_scale_out;
 /* rateTrackingTask's loop body (MM:5684-5806, exclude set MM:5835-5856, loadedSince MM:5858-5870) and the janitor's
  * removeModelCopies (MM:6197-6310, who-drops-the-copy by PLACEMENT_ORDER MM:6314-6335) for a batch of cache entries,
- * against the committed snapshot (instance table, type-set stats) and the registry (copies, failures, load times). */
+ * against the committed snapshot (instance table, type-set stats) and the registry (copies, failures, load times): every
+ * registration of the model, the first copy_count of them loaded, the rest failed loads. */
 int32_t mmp_scale_eval(mmp_fleet *, const mmp_scale_in *in, int32_t n, const mmp_scale_params *params, mmp_scale_out *out);
 /* The reaper's prune pass (pruneModelRegistry MM:6524-6609, pruneMissingInstances MM:6752-6784) over the whole registry in one
  * sweep: registrations on instances that are not in the instance table, older than assume_gone_ms and missing for longer than
  * assume_gone_ms (ASSUME_INSTANCE_GONE_AFTER_MS, MM:270).  missing_since (max_instances entries, in/out) is the reaper's
- * `missings` map by instance index, 0 = absent.  Writes the models with entries to prune and, per model, the bit mask of the
+ * `missings` map by instance index, 0 = absent.  The four-registration view: it reads (and stamps missing_since for) the
+ * first four registrations of each model only.  Writes the models with entries to prune and, per model, the bit mask of the
  * pruned inline edges; returns how many (the registry itself is updated by the caller through mmp_model_upsert, as the
- * reference does through a conditional KV write). */
+ * reference does through a conditional KV write).  mmp_registry_prune_ids reads every registration. */
 int32_t mmp_registry_prune(mmp_fleet *, int32_t self, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since, int32_t *out_models,
                            uint8_t *out_masks, int32_t cap);
+/* The same pass over every registration of every model, stamping missing_since for each.  Reports each pruned registration
+ * as a (model, instance) pair, in (model, registration position) order, and returns how many there are; when that exceeds
+ * cap the outputs hold the first cap pairs of that order.  A second call with the same now_ms and the updated missing_since
+ * returns the same pairs.  assume_gone_ms >= 0.  Sets the "prune" timing. */
+int32_t mmp_registry_prune_ids(mmp_fleet *, int32_t self, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since,
+                               int32_t *out_models, int32_t *out_instances, int32_t cap);
 
 /* tuning / measurement knobs, same meaning as the MMP_* environment variables read at mmp_fleet_create:
  *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the batch kernel ("direct" below), 1 the latency kernel
@@ -443,7 +454,7 @@ int32_t mmp_registry_prune(mmp_fleet *, int32_t self, int64_t now_ms, int64_t as
  *   "commit_host_only" 1: every commit takes the structural (host) path */
 int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
 /* CUDA-event duration (ms) of the device part of the last mmp_stats ("stats"), mmp_reaper_select ("reaper": registry sweep +
- * sort + select), mmp_lru_apply ("lru_apply": the event kernel) on this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune;
+ * sort + select), mmp_lru_apply ("lru_apply": the event kernel) on this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device

@@ -43,6 +43,8 @@ final class MmPlace {
     static native int scaleEval(long h, ByteBuffer in, int n, ByteBuffer params, ByteBuffer out);
     static native int registryPrune(long h, int self, long nowMs, long assumeGoneMs, ByteBuffer missingSince, ByteBuffer outModels,
                                     ByteBuffer outMasks, int cap);
+    static native int registryPruneIds(long h, int self, long nowMs, long assumeGoneMs, ByteBuffer missingSince, ByteBuffer outModels,
+                                       ByteBuffer outInstances, int cap);
     static native int tune(long h, String key, long value);
     static native double lastTiming(long h, String key);
     // plug point 1: placement (CacheMissForwardingLB.getNext MM:4776-5004)

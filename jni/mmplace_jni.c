@@ -131,6 +131,13 @@ jint FN(registryPrune)(JNIEnv *env, jclass c, jlong h, jint self, jlong nowMs, j
   (void)c;
   return mmp_registry_prune(H(h), self, nowMs, assumeGoneMs, (int64_t *)BUF(missingSince), (int32_t *)BUF(outModels), (uint8_t *)BUF(outMasks), cap);
 }
+/* missingSince: int64[max_instances] (in/out), outModels / outInstances: int32[cap] -- direct buffers */
+jint FN(registryPruneIds)(JNIEnv *env, jclass c, jlong h, jint self, jlong nowMs, jlong assumeGoneMs, jobject missingSince, jobject outModels,
+                          jobject outInstances, jint cap) {
+  (void)c;
+  return mmp_registry_prune_ids(H(h), self, nowMs, assumeGoneMs, (int64_t *)BUF(missingSince), (int32_t *)BUF(outModels),
+                                (int32_t *)BUF(outInstances), cap);
+}
 jint FN(tune)(JNIEnv *env, jclass c, jlong h, jstring key, jlong value) {
   const char *ck = utf(env, key);
   jint rc = mmp_tune(H(h), ck, value);

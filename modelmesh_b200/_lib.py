@@ -142,6 +142,7 @@ SYMBOLS = [
     ("mmp_model_times", _I32, [_P, _I32, _P, _I32, _I64]),
     ("mmp_scale_eval", _I32, [_P, _P, _I32, _P, _P]),
     ("mmp_registry_prune", _I32, [_P, _I32, _I64, _I64, _P, _P, _P, _I32]),
+    ("mmp_registry_prune_ids", _I32, [_P, _I32, _I64, _I64, _P, _P, _P, _I32]),
     ("mmp_tune", _I32, [_P, C.c_char_p, _I64]),
     ("mmp_last_timing", _I32, [_P, C.c_char_p, C.POINTER(C.c_double)]),
     ("mmp_batcher_create", _I32, [_P, _I32, _I32, _U64, C.POINTER(_P)]),

@@ -20,8 +20,9 @@
 #pragma once
 
 struct LiveState {
-  DevBuf inst_rows, inst_tie, inst_meta, cand_idx, pref_idx, edges, models, ovf_pairs, keys, rs_words, flags, scratch_idx, scratch_rows,
+  DevBuf inst_rows, inst_tie, inst_meta, cand_idx, pref_idx, edges, models, keys, rs_words, flags, scratch_idx, scratch_rows,
       scratch_edges;
+  DevBuf ovf;                                 // [n_ovf] OvfEdge: registrations 4, 5, ... of every model, sorted by (model, position)
   DevBuf edge_ts, model_lul;                  // MR.instanceIds / failedIn values and MR.lastUnloadTime (registry_kernels.cuh), when given
   bool have_times = false;
   DevBuf type_part_off, type_parts;           // type id -> partitions whose instances may host the type (typeSetStats MM:1432-1438)

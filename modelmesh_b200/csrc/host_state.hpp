@@ -119,6 +119,10 @@ struct HostSnapshot {
   std::vector<uint32_t> tie_id, tie_loc, tie_zone, tie_lab;
 };
 
+// One registration past a model's four inline edges, as the device tables hold it: sorted by (model, registration position),
+// so the registrations 4, 5, ... of model m are the entries from the first one whose model is m on.
+struct OvfEdge { int32_t model, inst; int64_t ts; };
+
 class HostState {
  public:
   mmp_config cfg{};
@@ -138,6 +142,7 @@ class HostState {
   std::vector<int64_t> edge_ts, model_lul;
   bool times_dirty = false;
   std::unordered_map<int32_t, std::vector<int32_t>> edge_ovf;
+  std::unordered_map<int32_t, std::vector<int64_t>> edge_ovf_ts;  // the times of the overflow edges: same keys, same order
   int32_t n_models_used = 0;
   std::string err;
   // Instance ids -> indices, maintained by upsert/remove.  Model records ingested as JSON name instances BY ID (MR:69,73);
@@ -231,6 +236,9 @@ class HostState {
     if (m < 0 || m >= cfg.max_models || n < 0 || (n > 0 && !ts)) { err = "bad model index or null argument"; return MMP_E_ARG; }
     if (edge_ts.empty()) { edge_ts.assign((size_t)cfg.max_models * EDGE_INL, 0); model_lul.assign((size_t)cfg.max_models, 0); }
     for (int i = 0; i < EDGE_INL; i++) edge_ts[(size_t)m * EDGE_INL + i] = i < n ? ts[i] : 0;
+    auto ov = edge_ovf_ts.find(m);  // times past the registration count are ignored
+    if (ov != edge_ovf_ts.end())
+      for (size_t k = 0; k < ov->second.size(); k++) ov->second[k] = (int64_t)k + EDGE_INL < n ? ts[k + EDGE_INL] : 0;
     model_lul[m] = last_unload_time;
     times_dirty = true;
     return MMP_OK;
@@ -251,11 +259,25 @@ class HostState {
     models[m] = *row;
     models[m].reserved = (uint32_t)n_ids;  // library-private: size of the exclusion row (instance-shard early-out)
     for (int i = 0; i < EDGE_INL; i++) edge_inl[(size_t)m * EDGE_INL + i] = i < n_ids ? ids[i] : -1;
-    if (n_ids > EDGE_INL) { edge_ovf[m].assign(ids + EDGE_INL, ids + n_ids); ovf_dirty = true; }
-    else if (!edge_ovf.empty() && edge_ovf.erase(m)) ovf_dirty = true;
+    // an overflow position keeps its time until the next set_model_times, as an inline one does (new positions read 0)
+    if (n_ids > EDGE_INL) { edge_ovf[m].assign(ids + EDGE_INL, ids + n_ids); edge_ovf_ts[m].resize((size_t)(n_ids - EDGE_INL), 0); ovf_dirty = true; }
+    else if (!edge_ovf.empty() && edge_ovf.erase(m)) { edge_ovf_ts.erase(m); ovf_dirty = true; }
     mark_model(m);
     if (m + 1 > n_models_used) n_models_used = m + 1;
     return MMP_OK;
+  }
+  void ovf_table(std::vector<OvfEdge> &out) const {
+    std::vector<int32_t> keys;
+    size_t n = 0;
+    for (auto &kv : edge_ovf) { keys.push_back(kv.first); n += kv.second.size(); }
+    std::sort(keys.begin(), keys.end());
+    out.clear();
+    out.reserve(n);
+    for (int32_t m : keys) {
+      const std::vector<int32_t> &e = edge_ovf.at(m);
+      const std::vector<int64_t> &t = edge_ovf_ts.at(m);
+      for (size_t k = 0; k < e.size(); k++) out.push_back(OvfEdge{m, e[k], t[k]});
+    }
   }
   // Words per bitmap row, rounded up to 32 words so that every row starts on a 128-byte line and is a whole number
   // of 16-byte TMA units (10 000 instances -> 320 words = 1 280 B).
@@ -279,7 +301,7 @@ class HostState {
       }
       const mmp_model_row row = models[kv.first];
       set_model(kv.first, &row, ids.data(), (int32_t)ids.size(), true);
-      if (!edge_ts.empty()) set_model_times(kv.first, ts.data(), (int32_t)std::min<size_t>(ts.size(), EDGE_INL), model_lul[kv.first]);
+      if (!edge_ts.empty()) set_model_times(kv.first, ts.data(), (int32_t)ts.size(), model_lul[kv.first]);
     }
     json_resolved_gen = inst_gen;
   }
@@ -948,7 +970,7 @@ inline int32_t HostState::set_model_json(int32_t m, const char *json, int32_t si
     if (raw.empty()) { json_ids.erase(m); json_ts.erase(m); } else { json_ids[m] = std::move(raw); json_ts[m] = std::move(raw_ts); }
     bool any_time = lul != 0;
     for (int64_t t : ts) any_time = any_time || t != 0;
-    if (any_time || !edge_ts.empty()) set_model_times(m, ts.data(), (int32_t)std::min<size_t>(ts.size(), EDGE_INL), lul);
+    if (any_time || !edge_ts.empty()) set_model_times(m, ts.data(), (int32_t)ts.size(), lul);
   }
   return rc;
 }

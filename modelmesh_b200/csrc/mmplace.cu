@@ -86,16 +86,15 @@ __global__ void k_build_bitmap(uint32_t *__restrict__ excl, const int4 *__restri
   }
   if (ranks) ranks[m] = make_int4(rs[0], rs[1], rs[2], rs[3]);
 }
-// (launched after k_build_bitmap: a model with overflow pairs gets the EXCL_RANKS_OVF marker in its rank entry)
-__global__ void k_build_bitmap_ovf(uint32_t *__restrict__ excl, const int2 *__restrict__ pairs, int n_pairs,
+// (launched after k_build_bitmap: a model with overflow edges gets the EXCL_RANKS_OVF marker in its rank entry)
+__global__ void k_build_bitmap_ovf(uint32_t *__restrict__ excl, const OvfEdge *__restrict__ ovf, int n_ovf,
                                    const int32_t *__restrict__ rank_of, int stride, int word_lo, int word_hi, int4 *__restrict__ ranks) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_pairs) return;
-  int2 p = pairs[i];
-  int r = rank_of[p.y];
+  if (i >= n_ovf) return;
+  const int m = ovf[i].model, r = rank_of[ovf[i].inst];
   if (r >= 0 && (r >> 5) >= word_lo && (r >> 5) < word_hi)
-    atomicOr(&excl[(size_t)p.x * stride + ((r >> 5) - word_lo)], 1u << (r & 31));
-  if (ranks) ranks[p.x].x = EXCL_RANKS_OVF;
+    atomicOr(&excl[(size_t)m * stride + ((r >> 5) - word_lo)], 1u << (r & 31));
+  if (ranks) ranks[m].x = EXCL_RANKS_OVF;
 }
 
 // ---- TMA 1-D bulk copy + mbarrier helpers (cp.async.bulk: SASS UBLKCP) ----
@@ -1786,7 +1785,7 @@ void mmp_fleet_destroy(mmp_fleet *f) {
   f->ctx_free.clear();
   f->snaps[0].release(); f->snaps[1].release();
   for (DevBuf *b : {&f->live.inst_rows, &f->live.inst_tie, &f->live.inst_meta, &f->live.cand_idx, &f->live.pref_idx, &f->live.edges,
-                    &f->live.models, &f->live.ovf_pairs, &f->live.keys, &f->live.rs_words, &f->live.flags, &f->live.scratch_idx,
+                    &f->live.models, &f->live.ovf, &f->live.keys, &f->live.rs_words, &f->live.flags, &f->live.scratch_idx,
                     &f->live.scratch_rows, &f->live.scratch_edges, &f->live.edge_ts, &f->live.model_lul, &f->live.type_part_off, &f->live.type_parts})
     b->release();
   for (DevBuf *b : {&f->d_flush, &f->zero_row, &f->lru_ts, &f->lru_seq, &f->lru_weight, &f->lru_model,
@@ -2063,12 +2062,11 @@ static int32_t commit_locked(mmp_fleet *f) {
       CK(cudaGetLastError());
       CK(cudaStreamSynchronize(st));  // staging vectors
     }
-    if (structural || f->hs.ovf_dirty) {
-      std::vector<int2> pairs;
-      for (auto &kv : f->hs.edge_ovf)
-        for (int32_t e : kv.second) pairs.push_back(make_int2(kv.first, e));
-      lv.n_ovf = (int32_t)pairs.size();
-      CK(upload_vec(lv.ovf_pairs, pairs, st));
+    if (structural || f->hs.ovf_dirty || f->hs.times_dirty) {  // the overflow edges with their times (OvfEdge)
+      std::vector<OvfEdge> ovf;
+      f->hs.ovf_table(ovf);
+      lv.n_ovf = (int32_t)ovf.size();
+      CK(upload_vec(lv.ovf, ovf, st));
       CK(cudaStreamSynchronize(st));
     }
   }
@@ -2103,7 +2101,7 @@ static int32_t commit_locked(mmp_fleet *f) {
     f->launches++;
     CK(cudaGetLastError());
     if (lv.n_ovf) {
-      k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.ovf_pairs.as<int2>(), lv.n_ovf,
+      k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf,
                                                                  ds.rank_of.as<int32_t>(), ST, h.word_lo, h.word_hi, ranks);
       f->launches++;
       CK(cudaGetLastError());
@@ -2114,7 +2112,7 @@ static int32_t commit_locked(mmp_fleet *f) {
     CK(ds.front.ensure((size_t)nm * F * 4));
     CK(cudaMemsetAsync(ds.front.p, 0, (size_t)nm * F * 4, st));
     k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, F, 0, F, nullptr);
-    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf_pairs.as<int2>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F, nullptr);
+    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F, nullptr);
     f->launches += 2;
     CK(cudaGetLastError());
   }

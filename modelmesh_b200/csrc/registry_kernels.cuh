@@ -26,8 +26,34 @@ __global__ void k_type_stats(const StatsAcc *__restrict__ acc, const long long *
   out[t] = s;
 }
 
+// A model's registrations in the order of its last upsert (loaded first, then failed): positions 0-3 are the inline edges and
+// their times, positions 4, 5, ... the model's slice of the overflow table, found by a lower_bound on its model column.  Only
+// models with more than four registrations search.
+struct RegTables { const int4 *edges; const long long *edge_ts; const OvfEdge *ovf; int n_ovf; };
+struct ModelRegs { int m, ovf0; int4 e; };
+__device__ __forceinline__ ModelRegs model_regs(const RegTables &R, int m, unsigned reserved) {
+  ModelRegs g{m, 0, R.edges[m]};
+  if (reserved > 4u) {
+    int lo = 0, hi = R.n_ovf;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (R.ovf[mid].model < m) lo = mid + 1; else hi = mid; }
+    g.ovf0 = lo;
+  }
+  return g;
+}
+// registration j of the model -> its instance (-1: none) and its load / failure time (0: unknown)
+__device__ __forceinline__ int reg_at(const RegTables &R, const ModelRegs &g, int j, long long &ts) {
+  if (j < 4) {
+    ts = R.edge_ts ? R.edge_ts[(size_t)g.m * 4 + j] : 0;
+    return j == 0 ? g.e.x : j == 1 ? g.e.y : j == 2 ? g.e.z : g.e.w;
+  }
+  const int q = g.ovf0 + j - 4;
+  if (q >= R.n_ovf || R.ovf[q].model != g.m) { ts = 0; return -1; }
+  ts = R.ovf[q].ts;
+  return R.ovf[q].inst;
+}
+
 struct ScaleTables {
-  const mmp_model_row *models; const int4 *edges; const long long *edge_ts; const long long *model_lul;
+  const mmp_model_row *models; RegTables R; const long long *model_lul;
   const int32_t *rank_of; const RankRow *rows; const int32_t *part_of_rank; const uint4 *inst_tie;
   const TypeStat *type_stats; const StatsAcc *part_acc; const long long *min_lru; const int *sorted_rpm;
   int n_ranks, n_models, n_type_ids, max_instances, tc_enabled;
@@ -38,7 +64,6 @@ __device__ __forceinline__ int count_rpm_above(const int *sorted, int n, int thr
   while (lo < hi) { const int mid = (lo + hi) >> 1; if (sorted[mid] <= thr) lo = mid + 1; else hi = mid; }
   return n - lo;
 }
-__device__ __forceinline__ long long ts_of(const ScaleTables &T, int model, int j) { return T.edge_ts ? T.edge_ts[(size_t)model * 4 + j] : 0; }
 
 // one thread per cache entry: rateTrackingTask's loop body (MM:5684-5806) and removeModelCopies (MM:6197-6335)
 __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in, int n, mmp_scale_params p, mmp_scale_out *__restrict__ out) {
@@ -49,10 +74,12 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
   o.action = 0; o.copies_to_load = 0; o.load_last_used = 0; o.rpm = 0; o.i1 = e.i1; o.i2 = e.i2; o.set_heavy = 0; o.remove = 0;
   if (e.model < 0 || e.model >= T.n_models || e.instance < 0 || e.instance >= T.max_instances) { o.action = -1; out[r] = o; return; }
   const mmp_model_row mr = T.models[e.model];
-  if (mr.reserved > 4u) { o.action = -1; out[r] = o; return; }  // more registered instances than the inline list holds: host path
-  const int4 ed = T.edges[e.model];
-  const int es[4] = {ed.x, ed.y, ed.z, ed.w};
-  const int loaded = mr.copy_count < 4 ? mr.copy_count : 4, n_edges = (int)mr.reserved, failed = n_edges - loaded;
+  // a saturated copy count over more than 255 registrations: where the loaded copies end is unknown (mmplace.h)
+  if (mr.copy_count == 255 && mr.reserved > 255u) { o.action = -1; out[r] = o; return; }
+  const ModelRegs g = model_regs(T.R, e.model, mr.reserved);
+  long long ts;
+  // (up to four registrations: a copy count past them reads the inline positions, as the four-edge list always did)
+  const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4)), failed = n_edges - loaded;
   const int self_rank = T.rank_of[e.instance];
   const long long time_delta = p.now - p.last_check_time;
   // ---------------- scale-up (rateTrackingTask) ----------------
@@ -88,7 +115,7 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     if (rpm < thr) break;
     const long long cutoff = p.now - (time_delta + p.rate_check_interval_ms + 2 * p.assume_completed_ms);
     bool recent = false;
-    for (int j = 0; j < loaded; j++) if (es[j] != e.instance && ts_of(T, e.model, j) > cutoff) recent = true;  // loadedSince MM:5858-5870
+    for (int j = 0; j < loaded; j++) if (reg_at(T.R, g, j, ts) != e.instance && ts > cutoff) recent = true;  // loadedSince MM:5858-5870
     if (recent) break;
     const int our_rpm = self_rank >= 0 ? T.rows[self_rank].rpm : 0;
     const int max_rpm = max((int)((unsigned)thr * 4u), (int)((unsigned)our_rpm - 2u * (unsigned)thr));   // getExcludeSet MM:5835-5856
@@ -96,7 +123,7 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     if (excluded != 0) {
       int holding = 0;
       for (int j = 0; j < n_edges; j++) {
-        const int i = es[j];
+        const int i = reg_at(T.R, g, j, ts);
         if (i < 0 || i == e.instance) continue;
         const int rk = T.rank_of[i];
         if (rk >= 0 && T.rows[rk].rpm > max_rpm) holding++;
@@ -125,7 +152,7 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     int other = -1;
     unsigned best_id = 0xffffffffu;
     for (int j = 0; j < loaded; j++) {
-      const int i = es[j];
+      const int i = reg_at(T.R, g, j, ts);
       if (i < 0 || i == e.instance || T.rank_of[i] < 0) continue;
       const unsigned idr = T.inst_tie[i].x;
       if (idr < best_id) { best_id = idr; other = i; }
@@ -145,7 +172,10 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     const long long lul = T.model_lul ? T.model_lul[e.model] : 0;
     if (lul > 0 && p.now - lul < 8 * p.rate_check_interval_ms) break;
     bool recent = false;
-    for (int j = 0; j < loaded; j++) if (ts_of(T, e.model, j) > p.now - 1800000LL) recent = true;
+    for (int j = 0; j < loaded; j++) {
+      reg_at(T.R, g, j, ts);
+      if (ts > p.now - 1800000LL) recent = true;
+    }
     if (recent) break;
     long long min_age = (3 * glru + 10400000LL) / 100;
     if (min_age < 600000LL) min_age = 600000LL; else if (min_age > 18000000LL) min_age = 18000000LL;
@@ -159,27 +189,33 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
   out[r] = o;
 }
 
-// the reaper's prune pass: one thread per model record, 24 B row + 16 B edges + 32 B edge times.  missing_since = the
-// `missings` map by instance index (0 = absent); first-seen-missing instances are stamped (atomicCAS), pruned entries reported.
-__global__ void k_registry_prune(const mmp_model_row *__restrict__ models, const int4 *__restrict__ edges, const long long *__restrict__ edge_ts,
-                                 const int2 *__restrict__ inst_meta, int n_models, int max_instances, int self, long long now,
-                                 long long assume_gone, long long *__restrict__ missing_since, int *__restrict__ out_models,
-                                 unsigned char *__restrict__ out_masks, int cap, int *__restrict__ out_n) {
+// the reaper's prune pass: one thread per model record, 24 B row + 16 B edges + 32 B edge times (+ 16 B per overflow
+// registration).  missing_since = the `missings` map by instance index (0 = absent); first-seen-missing instances are stamped
+// (atomicCAS), pruned entries reported.  walk_ovf = 0: the first four registrations, one (model, mask) per model with pruned
+// entries (mmp_registry_prune); 1: every registration, one PrunedReg per pruned one, in no order (mmp_registry_prune_ids).
+struct PrunedReg { int32_t model, pos, inst; };
+__global__ void k_registry_prune(RegTables R, const mmp_model_row *__restrict__ models, const int2 *__restrict__ inst_meta, int n_models,
+                                 int max_instances, int self, long long now, long long assume_gone, long long *__restrict__ missing_since,
+                                 int walk_ovf, int *__restrict__ out_models, unsigned char *__restrict__ out_masks, PrunedReg *__restrict__ out_regs,
+                                 int cap, int *__restrict__ out_n) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= n_models) return;
   const mmp_model_row mr = models[m];
-  const int n_edges = mr.reserved < 4u ? (int)mr.reserved : 4;
+  const int n_edges = walk_ovf || mr.reserved < 4u ? (int)mr.reserved : 4;
   if (n_edges == 0) return;
-  const int4 ed = edges[m];
-  const int es[4] = {ed.x, ed.y, ed.z, ed.w};
+  const ModelRegs g = model_regs(R, m, walk_ovf ? mr.reserved : 0u);
   unsigned mask = 0;
   for (int j = 0; j < n_edges; j++) {
-    const int i = es[j];
+    long long ts;
+    const int i = reg_at(R, g, j, ts);
     if (i < 0 || i >= max_instances || i == self) continue;
-    if (now - (edge_ts ? edge_ts[(size_t)m * 4 + j] : 0) < assume_gone) continue;   // ignore recently loaded
-    if (inst_meta[i].y & 4) continue;                                               // the instance is in the table
+    if (now - ts < assume_gone) continue;        // ignore recently loaded
+    if (inst_meta[i].y & 4) continue;            // the instance is in the table
     const long long since = atomicCAS(reinterpret_cast<unsigned long long *>(&missing_since[i]), 0ull, (unsigned long long)now);
-    if (since != 0 && (now - since) > assume_gone) mask |= 1u << j;
+    if (since == 0 || (now - since) <= assume_gone) continue;
+    if (!walk_ovf) { mask |= 1u << j; continue; }
+    const int q = atomicAdd(out_n, 1);
+    if (q < cap) out_regs[q] = PrunedReg{m, j, i};
   }
   if (mask) {
     const int q = atomicAdd(out_n, 1);
@@ -190,6 +226,49 @@ __global__ void k_registry_prune(const mmp_model_row *__restrict__ models, const
 __global__ void k_extract_rpm(const RankRow *__restrict__ rows, int n, int *__restrict__ out) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r < n) out[r] = rows[r].rpm;
+}
+
+static RegTables reg_tables(const LiveState &lv) {
+  return RegTables{lv.edges.as<int4>(), lv.have_times ? lv.edge_ts.as<long long>() : nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
+}
+
+// One prune pass (k_registry_prune) over the live registry.  walk_ovf = 0 keeps at most `cap` (model, mask) records; 1 keeps
+// every pruned registration (at most 4 per model + the overflow table), so that the caller can hand out the first ones in
+// order.  `read(ctx, n)` copies the records out once missing_since is back; n = the kernel's count.
+template <class Read>
+static int32_t registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since, bool walk_ovf,
+                              int32_t cap, Read read) {
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  if (!f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  LiveState &lv = f->live;
+  const int32_t nm = f->hs.n_models_used, NI = f->hs.cfg.max_instances;
+  if (nm == 0) return 0;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  CK(c->d_in.ensure((size_t)NI * 8));
+  if (walk_ovf) {
+    cap = nm * HostState::EDGE_INL + lv.n_ovf;
+    CK(c->d_out.ensure((size_t)cap * sizeof(PrunedReg)));
+  } else { CK(c->d_out.ensure((size_t)std::max(cap, 1) * 4)); CK(c->d_extra.ensure((size_t)std::max(cap, 1))); }
+  CK(c->d_n_open.ensure(16));
+  CK(cudaMemcpyAsync(c->d_in.p, missing_since, (size_t)NI * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(c->d_n_open.p, 0, 4, st));
+  CK(cudaEventRecord(c->e0, st));
+  k_registry_prune<<<(nm + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.inst_meta.as<int2>(), nm, NI, self, now_ms,
+                                                    assume_gone_ms, c->d_in.as<long long>(), walk_ovf ? 1 : 0, c->d_out.as<int>(),
+                                                    c->d_extra.as<unsigned char>(), c->d_out.as<PrunedReg>(), cap, c->d_n_open.as<int>());
+  CK(cudaEventRecord(c->e1, st));
+  f->launches++;
+  CK(cudaGetLastError());
+  int n_out = 0;
+  CK(cudaMemcpyAsync(&n_out, c->d_n_open.p, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(missing_since, c->d_in.p, (size_t)NI * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_prune_ms = ms; }
+  return read(c.get(), n_out);
 }
 
 extern "C" {
@@ -234,8 +313,8 @@ int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mm
   }
   k_type_stats<<<(std::max(nt, 1) + 127) / 128, 128, 0, st>>>(acc, d_min, lv.type_part_off.as<int>(), lv.type_parts.as<int>(), nt, tstats);
   ScaleTables T;
-  T.models = lv.models.as<mmp_model_row>(); T.edges = lv.edges.as<int4>();
-  T.edge_ts = lv.have_times ? lv.edge_ts.as<long long>() : nullptr; T.model_lul = lv.have_times ? lv.model_lul.as<long long>() : nullptr;
+  T.models = lv.models.as<mmp_model_row>(); T.R = reg_tables(lv);
+  T.model_lul = lv.have_times ? lv.model_lul.as<long long>() : nullptr;
   T.rank_of = ds.rank_of.as<int32_t>(); T.rows = ds.rows.as<RankRow>(); T.part_of_rank = ds.part_of_rank.as<int32_t>();
   T.inst_tie = lv.inst_tie.as<uint4>(); T.type_stats = tstats; T.part_acc = acc; T.min_lru = d_min; T.sorted_rpm = rpm_sorted;
   T.n_ranks = nr; T.n_models = f->hs.n_models_used; T.n_type_ids = nt; T.max_instances = f->hs.cfg.max_instances; T.tc_enabled = ds.host.tc_enabled;
@@ -251,44 +330,33 @@ int32_t mmp_registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_t a
                            uint8_t *out_masks, int32_t cap) {
   NEED(f);
   if (!missing_since || cap < 0 || (cap > 0 && (!out_models || !out_masks))) { g_err = "bad argument"; return MMP_E_ARG; }
-  int32_t rc = set_device(f);
-  if (rc < 0) return rc;
-  std::lock_guard<std::mutex> g(f->ingest_mu);
-  if (!f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  LiveState &lv = f->live;
-  const int32_t nm = f->hs.n_models_used, NI = f->hs.cfg.max_instances;
-  if (nm == 0) return 0;
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  cudaStream_t st = c->stream;
-  CK(c->d_in.ensure((size_t)NI * 8)); CK(c->d_out.ensure((size_t)std::max(cap, 1) * 4)); CK(c->d_extra.ensure((size_t)std::max(cap, 1)));
-  CK(c->d_n_open.ensure(16));
-  CK(cudaMemcpyAsync(c->d_in.p, missing_since, (size_t)NI * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(c->d_n_open.p, 0, 4, st));
-  CK(cudaEventRecord(c->e0, st));
-  k_registry_prune<<<(nm + 255) / 256, 256, 0, st>>>(lv.models.as<mmp_model_row>(), lv.edges.as<int4>(), lv.have_times ? lv.edge_ts.as<long long>() : nullptr,
-                                                    lv.inst_meta.as<int2>(), nm, NI, self, now_ms, assume_gone_ms, c->d_in.as<long long>(),
-                                                    c->d_out.as<int>(), c->d_extra.as<unsigned char>(), cap, c->d_n_open.as<int>());
-  CK(cudaEventRecord(c->e1, st));
-  f->launches++;
-  CK(cudaGetLastError());
-  int n_out = 0;
-  CK(cudaMemcpyAsync(&n_out, c->d_n_open.p, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(missing_since, c->d_in.p, (size_t)NI * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_prune_ms = ms; }
-  const int got = std::min(n_out, cap);
-  if (got) {
-    std::vector<int32_t> ms((size_t)got);
-    std::vector<uint8_t> mk((size_t)got);
-    CK(cudaMemcpy(ms.data(), c->d_out.p, (size_t)got * 4, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(mk.data(), c->d_extra.p, (size_t)got, cudaMemcpyDeviceToHost));
-    std::vector<int32_t> ord((size_t)got);
-    for (int i = 0; i < got; i++) ord[i] = i;
-    std::sort(ord.begin(), ord.end(), [&](int a, int b) { return ms[a] < ms[b]; });  // registry order
-    for (int i = 0; i < got; i++) { out_models[i] = ms[ord[i]]; out_masks[i] = mk[ord[i]]; }
-  }
-  return n_out;
+  return registry_prune(f, self, now_ms, assume_gone_ms, missing_since, false, cap, [&](PlaceCtx *c, int n_out) -> int32_t {
+    const int got = std::min(n_out, cap);
+    if (got) {
+      std::vector<int32_t> ms((size_t)got);
+      std::vector<uint8_t> mk((size_t)got);
+      CK(cudaMemcpy(ms.data(), c->d_out.p, (size_t)got * 4, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(mk.data(), c->d_extra.p, (size_t)got, cudaMemcpyDeviceToHost));
+      std::vector<int32_t> ord((size_t)got);
+      for (int i = 0; i < got; i++) ord[i] = i;
+      std::sort(ord.begin(), ord.end(), [&](int a, int b) { return ms[a] < ms[b]; });  // registry order
+      for (int i = 0; i < got; i++) { out_models[i] = ms[ord[i]]; out_masks[i] = mk[ord[i]]; }
+    }
+    return n_out;
+  });
+}
+
+int32_t mmp_registry_prune_ids(mmp_fleet *f, int32_t self, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since, int32_t *out_models,
+                               int32_t *out_instances, int32_t cap) {
+  NEED(f);
+  if (!missing_since || cap < 0 || assume_gone_ms < 0 || (cap > 0 && (!out_models || !out_instances))) { g_err = "bad argument"; return MMP_E_ARG; }
+  return registry_prune(f, self, now_ms, assume_gone_ms, missing_since, true, cap, [&](PlaceCtx *c, int n_out) -> int32_t {
+    std::vector<PrunedReg> regs((size_t)n_out);
+    if (n_out) CK(cudaMemcpy(regs.data(), c->d_out.p, (size_t)n_out * sizeof(PrunedReg), cudaMemcpyDeviceToHost));
+    std::sort(regs.begin(), regs.end(), [](const PrunedReg &a, const PrunedReg &b) { return a.model != b.model ? a.model < b.model : a.pos < b.pos; });
+    for (int i = 0; i < std::min(n_out, cap); i++) { out_models[i] = regs[i].model; out_instances[i] = regs[i].inst; }
+    return n_out;
+  });
 }
 
 }  // extern "C"

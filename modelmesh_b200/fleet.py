@@ -290,6 +290,21 @@ class Fleet:
         self._ck(self.lib.mmp_churn_model(self.h, model, _ptr(row), _ptr(inst)))
         return row[0], inst
 
+    def model_times(self, m: int, edge_ts: np.ndarray, last_unload_time: int = 0):
+        ts = np.ascontiguousarray(edge_ts, dtype=np.int64)
+        self._ck(self.lib.mmp_model_times(self.h, m, _ptr(ts), len(ts), int(last_unload_time)))
+
+    def registry_prune_ids(self, self_idx: int, now_ms: int, assume_gone_ms: int, missing_since: np.ndarray, cap: int):
+        """mmp_registry_prune_ids: (total, models, instances) of the first min(total, cap) pruned registrations.
+        missing_since (int64[max_instances]) is updated in place."""
+        assert missing_since.dtype == np.int64 and missing_since.flags.c_contiguous
+        models = np.zeros(max(cap, 1), dtype=np.int32)
+        inst = np.zeros(max(cap, 1), dtype=np.int32)
+        n = self._ck(self.lib.mmp_registry_prune_ids(self.h, self_idx, now_ms, assume_gone_ms, _ptr(missing_since), _ptr(models),
+                                                     _ptr(inst), cap))
+        k = min(n, cap)
+        return n, models[:k], inst[:k]
+
     def commit_info(self):
         path, ms = C.c_int32(), C.c_double()
         self._ck(self.lib.mmp_commit_info(self.h, C.byref(path), C.byref(ms)))
