@@ -125,6 +125,39 @@ __global__ void k_unique_mark(const unsigned long long *__restrict__ keys, int n
   if (i < n) flags[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1 : 0;
 }
 
+// A size estimate of 0 is the reference's ArithmeticException (spaceToFill / sizeEstimate, MM:6651), but the reaper only gets
+// there when the candidate list is not empty (MM:6470): count the models that pass the base candidate rule alone (MM:6574-6577;
+// no `taken`, type exclusion or cutoff) and fail the call only when there is one.  Returns 0 (nothing to load) or MMP_E_ARG.
+static int32_t reaper_zero_estimate(mmp_fleet *f, const DeviceSnapshot &ds, long long global_lru) {
+  const int nm = ds.n_models;
+  if (nm == 0) return 0;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t s = c->stream;
+  CK(c->d_in.ensure((size_t)nm * 8 + 64));
+  CK(c->d_trace.ensure((size_t)nm * 4 + 64));
+  CK(c->d_cand.ensure((size_t)nm + 64));
+  CK(c->d_n_open.ensure(16));
+  uint8_t *flags = c->d_cand.as<uint8_t>();
+  int *d_n = c->d_n_open.as<int>();
+  k_reaper_flag<<<(nm + 255) / 256, 256, 0, s>>>(ds.models.as<mmp_model_row>(), nm, nullptr, 0, nullptr, global_lru, 0, 0, flags,
+                                               c->d_in.as<unsigned long long>());
+  f->launches++;
+  CK(cudaGetLastError());
+  thrust::counting_iterator<int32_t> iota(0);
+  size_t t = 0;
+  CK(cub::DeviceSelect::Flagged(nullptr, t, iota, flags, c->d_trace.as<int32_t>(), d_n, nm, s));
+  CK(c->d_cub.ensure(t + 64));
+  CK(cub::DeviceSelect::Flagged(c->d_cub.p, t, iota, flags, c->d_trace.as<int32_t>(), d_n, nm, s));
+  f->launches++;
+  int ncand = 0;
+  CK(cudaMemcpyAsync(&ncand, d_n, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (ncand == 0) return 0;
+  g_err = "size estimate is zero (the reference would throw ArithmeticException)";
+  return MMP_E_ARG;
+}
+
 static int32_t reaper_impl(mmp_fleet *f, int32_t partition, int64_t now, uint8_t *taken, int32_t *out_models, int32_t cap) {
   if (!out_models || cap < 0) { g_err = "bad argument"; return MMP_E_ARG; }
   int32_t rc = set_device(f);
@@ -155,7 +188,7 @@ static int32_t reaper_impl(mmp_fleet *f, int32_t partition, int64_t now, uint8_t
       int32_t avg = (int32_t)jsub(st.total_capacity, st.total_free) / st.model_copy_count;
       size_est = st.model_copy_count > 10 ? avg : jaddi(avg, def) / 2;
     }
-    if (size_est == 0) { g_err = "size estimate is zero (the reference would throw ArithmeticException)"; return MMP_E_ARG; }
+    if (size_est == 0) return reaper_zero_estimate(f, ds, global_lru);
     int64_t space = 0;
     for (int32_t r = 0; r < h.n_ranks; r++) {
       if (partition >= 0 && h.part_of_rank[r] != partition) continue;
