@@ -429,7 +429,8 @@ int32_t mmp_scale_eval(mmp_fleet *, const mmp_scale_in *in, int32_t n, const mmp
  * `missings` map by instance index, 0 = absent.  The four-registration view: it reads (and stamps missing_since for) the
  * first four registrations of each model only.  Writes the models with entries to prune and, per model, the bit mask of the
  * pruned inline edges; returns how many (the registry itself is updated by the caller through mmp_model_upsert, as the
- * reference does through a conditional KV write).  mmp_registry_prune_ids reads every registration. */
+ * reference does through a conditional KV write).  When that exceeds cap, the outputs hold the first cap of those models in
+ * model order.  mmp_registry_prune_ids reads every registration. */
 int32_t mmp_registry_prune(mmp_fleet *, int32_t self, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since, int32_t *out_models,
                            uint8_t *out_masks, int32_t cap);
 /* The same pass over every registration of every model, stamping missing_since for each.  Reports each pruned registration

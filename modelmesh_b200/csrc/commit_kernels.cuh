@@ -47,13 +47,9 @@ struct ChurnState {
 };
 
 
-__global__ void k_rank_keys(const mmp_instance_row *__restrict__ rows, const uint4 *__restrict__ tie, const int2 *__restrict__ meta,
-                            int n_idx, long long min_space, OrderKey *__restrict__ keys, long long vers0, int *__restrict__ flags) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_idx) return;
+// the PLACEMENT_ORDER key of a live instance's published record (HostState::build_snapshot builds the same on the host)
+__device__ __forceinline__ OrderKey order_key(const mmp_instance_row &r, const uint4 &t, long long min_space) {
   OrderKey k;
-  const mmp_instance_row r = rows[i];
-  const uint4 t = tie[i];
   k.vers = r.vers;
   k.rem = r.capacity - r.used > 0 ? r.capacity - r.used : 0;  // IR:203-205
   k.lru = r.lru_time; k.cap = r.capacity; k.count = r.count;
@@ -62,7 +58,15 @@ __global__ void k_rank_keys(const mmp_instance_row *__restrict__ rows, const uin
   k.id_rank = t.x; k.loc_rank = t.y; k.zone_rank = t.z; k.labels_rank = t.w;
   k.full = k.rem < min_space;
   k.shutting_down = false;
-  keys[i] = k;
+  return k;
+}
+
+__global__ void k_rank_keys(const mmp_instance_row *__restrict__ rows, const uint4 *__restrict__ tie, const int2 *__restrict__ meta,
+                            int n_idx, long long min_space, OrderKey *__restrict__ keys, long long vers0, int *__restrict__ flags) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_idx) return;
+  const mmp_instance_row r = rows[i];
+  keys[i] = order_key(r, tie[i], min_space);
   if ((meta[i].y & 1) && r.vers != vers0) atomicOr(flags, 1);  // mixed versions: the comparator may be non-transitive (N1): host path
 }
 

@@ -55,9 +55,14 @@ __device__ __forceinline__ int reg_at(const RegTables &R, const ModelRegs &g, in
 struct ScaleTables {
   const mmp_model_row *models; RegTables R; const long long *model_lul;
   const int32_t *rank_of; const RankRow *rows; const int32_t *part_of_rank; const uint4 *inst_tie;
+  const mmp_instance_row *inst_rows; long long min_space, churn2;  // PLACEMENT_ORDER keys of the live instances
   const TypeStat *type_stats; const StatsAcc *part_acc; const long long *min_lru; const int *sorted_rpm;
   int n_ranks, n_models, n_type_ids, max_instances, tc_enabled;
 };
+
+// Java long arithmetic: wraps
+__device__ __forceinline__ long long jmul64(long long a, long long b) { return (long long)((unsigned long long)a * (unsigned long long)b); }
+__device__ __forceinline__ long long jadd64(long long a, long long b) { return (long long)((unsigned long long)a + (unsigned long long)b); }
 
 __device__ __forceinline__ int count_rpm_above(const int *sorted, int n, int thr) {  // #{rpm > thr} in an ascending array
   int lo = 0, hi = n;
@@ -81,7 +86,7 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
   // (up to four registrations: a copy count past them reads the inline positions, as the four-edge list always did)
   const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4)), failed = n_edges - loaded;
   const int self_rank = T.rank_of[e.instance];
-  const long long time_delta = p.now - p.last_check_time;
+  const long long time_delta = jsub(p.now, p.last_check_time);
   // ---------------- scale-up (rateTrackingTask) ----------------
   do {
     const int inst_count = T.n_ranks;
@@ -91,14 +96,15 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     int suitable = inst_count;
     if (T.tc_enabled) { suitable = cs.count; if (suitable < 2) break; }
     const int thr = p.scale_up_rpm_threshold, heavy = (int)((unsigned)thr * 3u) / 4;
-    const int rpm = (int)((e.count * 60000LL) / time_delta);
+    const int rpm = (int)(jmul64(e.count, 60000) / time_delta);
     o.rpm = rpm;
     if (rpm > heavy) o.set_heavy = 1;
     if (loaded == 0) break;
     int cand = suitable - (loaded + failed);
     if (cand <= 0) break;
     if (loaded == 1) {
-      const int lower = p.iteration - p.second_copy_max_age_iters, upper = p.iteration - p.second_copy_min_age_iters;
+      const int lower = (int)((unsigned)p.iteration - (unsigned)p.second_copy_max_age_iters);
+      const int upper = (int)((unsigned)p.iteration - (unsigned)p.second_copy_min_age_iters);
       const int i1 = e.i1, i2 = e.i2;
       bool in1 = false, in2 = false;
       if (i2 >= lower && i1 <= upper) { in1 = i1 >= lower; in2 = i2 <= upper; }
@@ -106,14 +112,14 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
       o.i2 = p.iteration;
       if (in1 || in2) {
         if (cs.cap == 0) break;  // the reference's ArithmeticException -> entry skipped (MM:5797)
-        if ((10 * cs.free) / cs.cap >= 1 || (p.now - cs.lru) > p.second_copy_lru_threshold_ms) {
+        if (jmul64(10, cs.free) / cs.cap >= 1 || jsub(p.now, cs.lru) > p.second_copy_lru_threshold_ms) {
           o.action = 1; o.copies_to_load = 1; o.load_last_used = p.last_check_time;
           break;
         }
       }
     }
     if (rpm < thr) break;
-    const long long cutoff = p.now - (time_delta + p.rate_check_interval_ms + 2 * p.assume_completed_ms);
+    const long long cutoff = jsub(p.now, jadd64(jadd64(time_delta, p.rate_check_interval_ms), jmul64(2, p.assume_completed_ms)));
     bool recent = false;
     for (int j = 0; j < loaded; j++) if (reg_at(T.R, g, j, ts) != e.instance && ts > cutoff) recent = true;  // loadedSince MM:5858-5870
     if (recent) break;
@@ -147,7 +153,7 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
       const StatsAcc a = T.part_acc[1 + T.part_of_rank[self_rank]];
       cap = (long long)a.cap; fr = (long long)a.free;
     } else { cap = (long long)T.part_acc[0].cap; fr = (long long)T.part_acc[0].free; }
-    if (cap == 0 || (fr * 100) / cap > 5) break;
+    if (cap == 0 || jmul64(fr, 100) / cap > 5) break;
     // the first other copy in instance-ID order that is in the table and not shutting down (MM:6236-6245)
     int other = -1;
     unsigned best_id = 0xffffffffu;
@@ -159,30 +165,33 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     }
     if (other < 0) break;
     if (loaded == 2) {
-      const long long cache_age = p.now - glru;
+      const long long cache_age = jsub(p.now, glru);
       long long scale_down_age = cache_age / 10;
-      if (e.last_heavy == 0 || (p.now - e.last_heavy) < cache_age / 5) scale_down_age = p.second_copy_remove_max_age_ms < scale_down_age ? (long long)p.second_copy_remove_max_age_ms : scale_down_age;
-      if ((p.now - e.last_used) > scale_down_age) {
+      if (e.last_heavy == 0 || jsub(p.now, e.last_heavy) < cache_age / 5) scale_down_age = p.second_copy_remove_max_age_ms < scale_down_age ? (long long)p.second_copy_remove_max_age_ms : scale_down_age;
+      if (jsub(p.now, e.last_used) > scale_down_age) {
         if (self_rank < 0) break;
-        if (T.rank_of[other] > self_rank) break;  // PLACEMENT_ORDER.compare(other, this) > 0: the other pod should flush it (MM:6328)
+        // PLACEMENT_ORDER.compare(other, this) > 0: the other pod should flush it (MM:6328).  The comparator, not the ranks:
+        // with mixed versions (quirk N1) it is no total order, and the snapshot's linear order contradicts it on some pair
+        if (compare_keys(order_key(T.inst_rows[other], T.inst_tie[other], T.min_space),
+                         order_key(T.inst_rows[e.instance], T.inst_tie[e.instance], T.min_space), T.churn2) > 0) break;
         o.remove = 1;
       }
       break;
     }
     const long long lul = T.model_lul ? T.model_lul[e.model] : 0;
-    if (lul > 0 && p.now - lul < 8 * p.rate_check_interval_ms) break;
+    if (lul > 0 && jsub(p.now, lul) < jmul64(8, p.rate_check_interval_ms)) break;
     bool recent = false;
     for (int j = 0; j < loaded; j++) {
       reg_at(T.R, g, j, ts);
-      if (ts > p.now - 1800000LL) recent = true;
+      if (ts > jsub(p.now, 1800000LL)) recent = true;
     }
     if (recent) break;
-    long long min_age = (3 * glru + 10400000LL) / 100;
+    long long min_age = jadd64(jmul64(3, glru), 10400000LL) / 100;
     if (min_age < 600000LL) min_age = 600000LL; else if (min_age > 18000000LL) min_age = 18000000LL;
-    if (p.now - e.last_heavy < min_age) break;
-    const long long since = p.now - p.last_check_time;
+    if (jsub(p.now, e.last_heavy) < min_age) break;
+    const long long since = jsub(p.now, p.last_check_time);
     if (since < p.rate_check_interval_ms / 10) break;
-    const long long rpm2 = (e.count * 60000LL) / since;
+    const long long rpm2 = jmul64(e.count, 60000) / since;
     if (rpm2 > ((long long)p.scale_up_rpm_threshold * 2) / 3) break;
     o.remove = 1;
   } while (false);
@@ -232,12 +241,12 @@ static RegTables reg_tables(const LiveState &lv) {
   return RegTables{lv.edges.as<int4>(), lv.have_times ? lv.edge_ts.as<long long>() : nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
 }
 
-// One prune pass (k_registry_prune) over the live registry.  walk_ovf = 0 keeps at most `cap` (model, mask) records; 1 keeps
-// every pruned registration (at most 4 per model + the overflow table), so that the caller can hand out the first ones in
-// order.  `read(ctx, n)` copies the records out once missing_since is back; n = the kernel's count.
+// One prune pass (k_registry_prune) over the live registry.  It keeps every record -- walk_ovf = 0: one (model, mask) per
+// model; 1: every pruned registration (at most 4 per model + the overflow table) -- so that the caller can hand out the first
+// ones in order.  `read(ctx, n)` copies the records out once missing_since is back; n = the kernel's count.
 template <class Read>
 static int32_t registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since, bool walk_ovf,
-                              int32_t cap, Read read) {
+                              Read read) {
   int32_t rc = set_device(f);
   if (rc < 0) return rc;
   std::lock_guard<std::mutex> g(f->ingest_mu);
@@ -249,10 +258,9 @@ static int32_t registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
   cudaStream_t st = c->stream;
   CK(c->d_in.ensure((size_t)NI * 8));
-  if (walk_ovf) {
-    cap = nm * HostState::EDGE_INL + lv.n_ovf;
-    CK(c->d_out.ensure((size_t)cap * sizeof(PrunedReg)));
-  } else { CK(c->d_out.ensure((size_t)std::max(cap, 1) * 4)); CK(c->d_extra.ensure((size_t)std::max(cap, 1))); }
+  const int32_t cap = walk_ovf ? nm * HostState::EDGE_INL + lv.n_ovf : nm;
+  if (walk_ovf) CK(c->d_out.ensure((size_t)cap * sizeof(PrunedReg)));
+  else { CK(c->d_out.ensure((size_t)cap * 4)); CK(c->d_extra.ensure((size_t)cap)); }
   CK(c->d_n_open.ensure(16));
   CK(cudaMemcpyAsync(c->d_in.p, missing_since, (size_t)NI * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(c->d_n_open.p, 0, 4, st));
@@ -316,7 +324,9 @@ int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mm
   T.models = lv.models.as<mmp_model_row>(); T.R = reg_tables(lv);
   T.model_lul = lv.have_times ? lv.model_lul.as<long long>() : nullptr;
   T.rank_of = ds.rank_of.as<int32_t>(); T.rows = ds.rows.as<RankRow>(); T.part_of_rank = ds.part_of_rank.as<int32_t>();
-  T.inst_tie = lv.inst_tie.as<uint4>(); T.type_stats = tstats; T.part_acc = acc; T.min_lru = d_min; T.sorted_rpm = rpm_sorted;
+  T.inst_tie = lv.inst_tie.as<uint4>(); T.inst_rows = lv.inst_rows.as<mmp_instance_row>();
+  T.min_space = f->hs.cfg.min_space_units; T.churn2 = (long long)((uint64_t)f->hs.cfg.min_churn_age_ms * 2u);
+  T.type_stats = tstats; T.part_acc = acc; T.min_lru = d_min; T.sorted_rpm = rpm_sorted;
   T.n_ranks = nr; T.n_models = f->hs.n_models_used; T.n_type_ids = nt; T.max_instances = f->hs.cfg.max_instances; T.tc_enabled = ds.host.tc_enabled;
   k_scale_eval<<<(n + 127) / 128, 128, 0, st>>>(T, c->d_in.as<mmp_scale_in>(), n, *params, c->d_out.as<mmp_scale_out>());
   f->launches += 2;
@@ -330,18 +340,16 @@ int32_t mmp_registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_t a
                            uint8_t *out_masks, int32_t cap) {
   NEED(f);
   if (!missing_since || cap < 0 || (cap > 0 && (!out_models || !out_masks))) { g_err = "bad argument"; return MMP_E_ARG; }
-  return registry_prune(f, self, now_ms, assume_gone_ms, missing_since, false, cap, [&](PlaceCtx *c, int n_out) -> int32_t {
-    const int got = std::min(n_out, cap);
-    if (got) {
-      std::vector<int32_t> ms((size_t)got);
-      std::vector<uint8_t> mk((size_t)got);
-      CK(cudaMemcpy(ms.data(), c->d_out.p, (size_t)got * 4, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(mk.data(), c->d_extra.p, (size_t)got, cudaMemcpyDeviceToHost));
-      std::vector<int32_t> ord((size_t)got);
-      for (int i = 0; i < got; i++) ord[i] = i;
-      std::sort(ord.begin(), ord.end(), [&](int a, int b) { return ms[a] < ms[b]; });  // registry order
-      for (int i = 0; i < got; i++) { out_models[i] = ms[ord[i]]; out_masks[i] = mk[ord[i]]; }
-    }
+  return registry_prune(f, self, now_ms, assume_gone_ms, missing_since, false, [&](PlaceCtx *c, int n_out) -> int32_t {
+    if (n_out == 0) return 0;
+    std::vector<int32_t> ms((size_t)n_out);
+    std::vector<uint8_t> mk((size_t)n_out);
+    CK(cudaMemcpy(ms.data(), c->d_out.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(mk.data(), c->d_extra.p, (size_t)n_out, cudaMemcpyDeviceToHost));
+    std::vector<int32_t> ord((size_t)n_out);
+    for (int i = 0; i < n_out; i++) ord[i] = i;
+    std::sort(ord.begin(), ord.end(), [&](int a, int b) { return ms[a] < ms[b]; });  // model order: one record per model
+    for (int i = 0; i < std::min(n_out, cap); i++) { out_models[i] = ms[ord[i]]; out_masks[i] = mk[ord[i]]; }
     return n_out;
   });
 }
@@ -350,7 +358,7 @@ int32_t mmp_registry_prune_ids(mmp_fleet *f, int32_t self, int64_t now_ms, int64
                                int32_t *out_instances, int32_t cap) {
   NEED(f);
   if (!missing_since || cap < 0 || assume_gone_ms < 0 || (cap > 0 && (!out_models || !out_instances))) { g_err = "bad argument"; return MMP_E_ARG; }
-  return registry_prune(f, self, now_ms, assume_gone_ms, missing_since, true, cap, [&](PlaceCtx *c, int n_out) -> int32_t {
+  return registry_prune(f, self, now_ms, assume_gone_ms, missing_since, true, [&](PlaceCtx *c, int n_out) -> int32_t {
     std::vector<PrunedReg> regs((size_t)n_out);
     if (n_out) CK(cudaMemcpy(regs.data(), c->d_out.p, (size_t)n_out * sizeof(PrunedReg), cudaMemcpyDeviceToHost));
     std::sort(regs.begin(), regs.end(), [](const PrunedReg &a, const PrunedReg &b) { return a.model != b.model ? a.model < b.model : a.pos < b.pos; });
