@@ -289,6 +289,7 @@ int32_t mmp_churn_init(mmp_fleet *f, const mmp_churn_config *cfg) {
   std::lock_guard<std::mutex> g(f->ingest_mu);
   ChurnState &cs = f->churn;
   cs.load_timeout_ms = cfg->load_timeout_ms;
+  for (Event &e : cs.phase_ev) if (!e) CK(cudaEventCreate(e.put()));
   std::vector<long long> lp((size_t)NI, (long long)cfg->last_published_ms);
   CK(upload_vec(cs.last_published, lp, f->commit_stream));
   CK(cs.first_ev.ensure((size_t)NM * 4)); CK(cs.dec_of_model.ensure((size_t)NM * 4)); CK(cs.rm_mask.ensure((size_t)NM * 4));
@@ -369,9 +370,7 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   const int32_t nF = cs.n_carry, Q = nF + n;
   CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  cudaEvent_t evs[8];
-  for (auto &e : evs) CK(cudaEventCreate(&e));
-  struct EvRel { cudaEvent_t *e; ~EvRel() { for (int i = 0; i < 8; i++) cudaEventDestroy(e[i]); } } evrel{evs};
+  const Event *evs = cs.phase_ev;
   const size_t QQ = (size_t)std::max(Q, 1), NK = 5 * QQ;
   CK(cs.ev.ensure(QQ * sizeof(mmp_churn_event))); CK(cs.is_dec.ensure(QQ * 4 + 16)); CK(cs.dec_pos.ensure(QQ * 4 + 16));
   CK(cs.dec_in.ensure(QQ * sizeof(mmp_decision_in))); CK(cs.dec_out.ensure(QQ * sizeof(mmp_decision_out)));

@@ -41,7 +41,8 @@ struct ChurnState {
   DevBuf ev, is_dec, dec_pos, dec_in, dec_out, dec_meta, dec_target, extra, status, lev, keys, vals, keys2, vals2, cub_tmp, off, evict, fkeys,
       fvals, rows_changed;
   int32_t n_carry = 0;
-  // last step's phase timings (ms, CUDA events on the step's stream)
+  // last step's phase timings (ms, between these events on the step's stream; created by mmp_churn_init)
+  Event phase_ev[7];
   float t_classify = 0, t_place = 0, t_route = 0, t_apply = 0, t_registry = 0, t_commit = 0, t_total = 0;
   int32_t last_lru_events = 0;
 };

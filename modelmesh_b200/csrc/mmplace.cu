@@ -45,6 +45,7 @@
 #include <shared_mutex>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "host_state.hpp"
@@ -1090,13 +1091,21 @@ static NcclApi &nccl_api() {
 // ---------------------------------------------------------------------------------------------------------------
 // device-side containers
 // ---------------------------------------------------------------------------------------------------------------
+// Every CUDA resource a fleet holds is owned by one of these: it is freed when its owner goes out of scope, so a struct
+// that holds them needs no cleanup list.  A device buffer that grows on demand (ensure); the memory is its own.
 struct DevBuf {
   void *p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    if (this != &o) { release(); p = std::exchange(o.p, nullptr); cap = std::exchange(o.cap, 0); }
+    return *this;
+  }
+  ~DevBuf() { release(); }
   cudaError_t ensure(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; cap = 0;
+    release();
     size_t want = bytes + bytes / 8 + 256;
     cudaError_t e = cudaMalloc(&p, want);
     if (e == cudaSuccess) cap = want;
@@ -1105,6 +1114,31 @@ struct DevBuf {
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
   template <class T> T *as() const { return reinterpret_cast<T *>(p); }
 };
+
+// A runtime handle and the call that frees it.  It converts to the raw handle, so it is passed as one; put() frees the
+// handle held and hands the runtime's create call the slot for a new one.
+template <class T, cudaError_t (*Free)(T)>
+class Owned {
+ public:
+  Owned() = default;
+  Owned(Owned &&o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+  Owned &operator=(Owned &&o) noexcept { if (this != &o) { reset(); h_ = std::exchange(o.h_, nullptr); } return *this; }
+  ~Owned() { reset(); }
+  void reset() { if (h_) Free(h_); h_ = nullptr; }
+  T *put() { reset(); return &h_; }
+  T get() const { return h_; }
+  operator T() const { return h_; }
+
+ private:
+  T h_ = nullptr;
+};
+inline cudaError_t free_host(unsigned char *p) { return cudaFreeHost(p); }
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using Graph = Owned<cudaGraph_t, cudaGraphDestroy>;
+using GraphExec = Owned<cudaGraphExec_t, cudaGraphExecDestroy>;
+using PinnedBuf = Owned<unsigned char *, free_host>;        // cudaHostAlloc
+using IpcMapping = Owned<void *, cudaIpcCloseMemHandle>;   // cudaIpcOpenMemHandle
 
 #include "commit_kernels.cuh"
 
@@ -1118,18 +1152,13 @@ struct DeviceSnapshot {
   bool sparse_slots = false;  // most type slots have few candidates inside a decision's window: long walks (k_place_direct sorts big batches by slot)
   bool host_stale = false;  // built on the device: the rank-space vectors of `host` are downloaded on first use (host_mirror)
   int32_t n_models = 0;
-  void release() {
-    for (DevBuf *b : {&excl, &excl_ranks, &cand, &candx, &pref, &has_pref, &type_slot, &full, &rows, &rank_of, &csum, &lsum, &models,
-                      &cap_col, &lthreads_col, &linprog_col, &part_of_rank, &count_col, &cand_before, &nzw, &nz_n, &front, &nzw_full, &nz_n_full})
-      b->release();
-  }
 };
 
 struct PlaceCtx {
-  cudaStream_t stream = nullptr;
+  Stream stream;
   static constexpr int NPIPE = 3;
-  cudaStream_t pipe[NPIPE] = {nullptr, nullptr, nullptr};  // H2D / kernel / D2H of consecutive chunks overlap across these
-  cudaEvent_t e0 = nullptr, e1 = nullptr, ready = nullptr;
+  Stream pipe[NPIPE];  // H2D / kernel / D2H of consecutive chunks overlap across these
+  Event e0, e1, ready;
   DevBuf d_in, d_out, d_fresh, d_extra, d_trace, d_cand;
   // slot sort of a batch (k_slot_keys + cub radix sort -> perm): set 0 for single launches, 1 + pipe for the chunks of a pipelined call
   static constexpr int NSORT = 4;
@@ -1138,11 +1167,11 @@ struct PlaceCtx {
   std::vector<FreshRow> fresh_host;
   // pinned, device-mapped scratch for tiny batches: the kernel reads the decisions and writes the results straight
   // through PCIe, so a B = 1 call is one launch + one synchronise (no copy calls)
-  unsigned char *mapped = nullptr;
+  PinnedBuf mapped;
   static constexpr size_t MAPPED_BYTES = 16384;
   // the B = 1 path as a captured CUDA graph (one k_place_small node; now / seed / n travel through the mapped header)
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t graph_exec = nullptr;
+  Graph graph;
+  GraphExec graph_exec;  // (declared after the graph it was instantiated from: destroyed before it)
   int32_t graph_epoch = -1;
   // a call-wide exclude set (mmp_place_batch_excluding): its ids and the per-slot tables derived from the snapshot's
   // (k_exclude_slots, k_slot_lists) that the call's view points at
@@ -1162,7 +1191,7 @@ struct mmp_fleet {
   DeviceSnapshot snaps[2];
   int cur = 0;
   int32_t epoch = 0;
-  cudaStream_t commit_stream = nullptr;
+  Stream commit_stream;
   DevBuf d_flush;
   DevBuf zero_row;              // one all-zero exclusion row (SnapshotView::zero_row), unsharded fleets: allocated at the first commit
   ChurnState churn;             // the closed loop (churn_kernels.cuh)
@@ -1184,11 +1213,10 @@ struct mmp_fleet {
     mmp_decision_out *out_buf() const { return reinterpret_cast<mmp_decision_out *>(arena.as<unsigned char>() + 4096); }
     unsigned long long *flag_buf() const { return arena.as<unsigned long long>(); }
     void *peer_base[MAX_SHARDS][4] = {};    // every peer's buffers as mapped here: excl of snapshot 0 / 1, out, flags
-    void *block_base[MAX_SHARDS][4] = {};   // ... and the allocation blocks that were opened for them
-    bool opened[MAX_SHARDS][4] = {};
+    IpcMapping opened[MAX_SHARDS][3];       // ... and the allocation blocks opened for them (a peer in this process: none)
     uint64_t step = 0;
     int64_t batches = 0, result_bytes = 0;
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // around k_place_dealt and k_dealt_wait of the last step
+    Event ev[3];                            // around k_place_dealt and k_dealt_wait of the last step
     float t_kernel_ms = 0, t_wait_ms = 0;
     int off = 0;                            // MMP_SHARD_PEERS=0 keeps the collective path although peers were imported
   } peers;
@@ -1203,8 +1231,8 @@ struct mmp_fleet {
   // the resident B = 1 server (one_mode 3, k_place_server)
   struct Server {
     std::mutex mu;                 // one request at a time; a caller that finds it taken uses the graph path
-    unsigned char *mapped = nullptr;
-    cudaStream_t stream = nullptr;
+    PinnedBuf mapped;
+    Stream stream;
     int32_t epoch = -1;
     bool running = false;
     uint64_t seq = 0;
@@ -1243,14 +1271,13 @@ static PlaceCtx *acquire_ctx(mmp_fleet *f) {
       return c;
     }
   }
-  auto *c = new PlaceCtx();
-  bool ok = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) == cudaSuccess &&
-            cudaEventCreate(&c->e0) == cudaSuccess && cudaEventCreate(&c->e1) == cudaSuccess &&
-            cudaEventCreateWithFlags(&c->ready, cudaEventDisableTiming) == cudaSuccess &&
-            cudaHostAlloc((void **)&c->mapped, PlaceCtx::MAPPED_BYTES, cudaHostAllocMapped) == cudaSuccess;
-  for (int i = 0; ok && i < PlaceCtx::NPIPE; i++) ok = cudaStreamCreateWithFlags(&c->pipe[i], cudaStreamNonBlocking) == cudaSuccess;
-  if (!ok) { delete c; return nullptr; }
-  return c;
+  auto c = std::make_unique<PlaceCtx>();
+  bool ok = cudaStreamCreateWithFlags(c->stream.put(), cudaStreamNonBlocking) == cudaSuccess &&
+            cudaEventCreate(c->e0.put()) == cudaSuccess && cudaEventCreate(c->e1.put()) == cudaSuccess &&
+            cudaEventCreateWithFlags(c->ready.put(), cudaEventDisableTiming) == cudaSuccess &&
+            cudaHostAlloc((void **)c->mapped.put(), PlaceCtx::MAPPED_BYTES, cudaHostAllocMapped) == cudaSuccess;
+  for (int i = 0; ok && i < PlaceCtx::NPIPE; i++) ok = cudaStreamCreateWithFlags(c->pipe[i].put(), cudaStreamNonBlocking) == cudaSuccess;
+  return ok ? c.release() : nullptr;
 }
 // A PlaceCtx leased from the fleet's pool for the length of one call; it goes back to the pool when the lease goes out of
 // scope.  A lease is empty when a new context could not be created.
@@ -1272,21 +1299,6 @@ class CtxLease {
   mmp_fleet *f_;
   PlaceCtx *c_;
 };
-static void destroy_ctx(PlaceCtx *c) {
-  for (DevBuf *b : {&c->d_in, &c->d_out, &c->d_fresh, &c->d_extra, &c->d_trace, &c->d_cand, &c->d_open_flag,
-                    &c->d_open_idx, &c->d_n_open, &c->d_cub, &c->d_blocks, &c->d_gathered, &c->d_rows, &c->d_in_open, &c->d_out_open,
-                    &c->d_xids, &c->d_xcand, &c->d_xcandx, &c->d_xpref, &c->d_xnzw, &c->d_xnz_n, &c->d_xbefore})
-    b->release();
-  for (int k = 0; k < PlaceCtx::NSORT; k++) { c->d_skey[k].release(); c->d_skey2[k].release(); c->d_sidx[k].release(); c->d_sidx2[k].release(); c->d_stmp[k].release(); }
-  if (c->e0) cudaEventDestroy(c->e0);
-  if (c->e1) cudaEventDestroy(c->e1);
-  if (c->ready) cudaEventDestroy(c->ready);
-  if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
-  if (c->graph) cudaGraphDestroy(c->graph);
-  if (c->mapped) cudaFreeHost(c->mapped);
-  for (int i = 0; i < PlaceCtx::NPIPE; i++) if (c->pipe[i]) cudaStreamDestroy(c->pipe[i]);
-  if (c->stream) cudaStreamDestroy(c->stream);
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // kernel dispatch on the row width
@@ -1427,7 +1439,7 @@ static int32_t place_dealt(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, 
   auto kern = k_place_dealt<WARPS, 6>;  // 6 resident blocks per SM: 24 warps, some spills
   if (smem > 48 * 1024) CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   unsigned long long *stats = pr.flag_buf() + MAX_SHARDS;
-  if (!pr.ev[0]) for (int k = 0; k < 3; k++) CK(cudaEventCreate(&pr.ev[k]));
+  if (!pr.ev[0]) for (int k = 0; k < 3; k++) CK(cudaEventCreate(pr.ev[k].put()));
   CK(cudaEventRecord(pr.ev[0], st));
   kern<<<blocks, WARPS * 32, smem, st>>>(vw, ds.front.as<uint32_t>(), std::min(SHARD_FRONT_WORDS, vw.row_words), ds.nzw_full.as<uint16_t>(),
                                                        ds.nz_n_full.as<int32_t>(), P, G, me, d_in, n, d_fresh, n_fresh, d_extra, now_ms, seed,
@@ -1709,18 +1721,18 @@ int32_t mmp_shard_ipc_import(mmp_fleet *f, const void *blobs) {
       (void)cudaGetLastError();
       for (int k = 0; k < 3; k++) pr.peer_base[q][k] = (void *)(uintptr_t)bl.ptr[k];
     } else {
-      for (int k = 0; k < 3; k++)
-        if (pr.opened[q][k]) { cudaIpcCloseMemHandle(pr.block_base[q][k]); pr.opened[q][k] = false; }
+      for (IpcMapping &m : pr.opened[q]) m.reset();
+      void *block[3] = {};
       for (int k = 0; k < 3; k++) {
         int same = -1;
         for (int j = 0; j < k && same < 0; j++)
           if (bl.ptr[j] - bl.off[j] == bl.ptr[k] - bl.off[k]) same = j;  // the same block in the exporting process
-        if (same >= 0) pr.block_base[q][k] = pr.block_base[q][same];
+        if (same >= 0) block[k] = block[same];
         else {
-          CK(cudaIpcOpenMemHandle(&pr.block_base[q][k], bl.h[k], cudaIpcMemLazyEnablePeerAccess));
-          pr.opened[q][k] = true;
+          CK(cudaIpcOpenMemHandle(pr.opened[q][k].put(), bl.h[k], cudaIpcMemLazyEnablePeerAccess));
+          block[k] = pr.opened[q][k];
         }
-        pr.peer_base[q][k] = (unsigned char *)pr.block_base[q][k] + bl.off[k];
+        pr.peer_base[q][k] = (unsigned char *)block[k] + bl.off[k];
       }
     }
   }
@@ -1764,7 +1776,7 @@ int32_t mmp_fleet_create(const mmp_config *cfg, mmp_fleet **out) {
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, f->device));
   f->sm_count = prop.multiProcessorCount;
-  CK(cudaStreamCreateWithFlags(&f->commit_stream, cudaStreamNonBlocking));
+  CK(cudaStreamCreateWithFlags(f->commit_stream.put(), cudaStreamNonBlocking));
   f->hs.init(*cfg);
   if (const char *t = getenv("MMP_KERNEL")) f->kernel = !strcmp(t, "tile") ? PlaceKernel::tile : !strcmp(t, "lanes") ? PlaceKernel::lanes : PlaceKernel::direct;
   if (const char *t = getenv("MMP_ONE")) f->one_mode = !strcmp(t, "lanes") ? 0 : (!strcmp(t, "small") ? 1 : (!strcmp(t, "server") ? 3 : 2));
@@ -1778,21 +1790,10 @@ int32_t mmp_fleet_create(const mmp_config *cfg, mmp_fleet **out) {
 void mmp_fleet_destroy(mmp_fleet *f) {
   if (!f) return;
   cudaSetDevice(f->device);
-  { std::lock_guard<std::mutex> lk(f->srv.mu); server_stop(f); if (f->srv.stream) cudaStreamDestroy(f->srv.stream); if (f->srv.mapped) cudaFreeHost(f->srv.mapped); f->srv.mapped = nullptr; }
+  { std::lock_guard<std::mutex> lk(f->srv.mu); server_stop(f); }
   cudaDeviceSynchronize();
   if (f->comm && nccl_api().ok) { nccl_api().CommDestroy(f->comm); f->comm = nullptr; }
-  for (auto &c : f->ctx_free) { destroy_ctx(c.get()); }
-  f->ctx_free.clear();
-  f->snaps[0].release(); f->snaps[1].release();
-  for (DevBuf *b : {&f->live.inst_rows, &f->live.inst_tie, &f->live.inst_meta, &f->live.cand_idx, &f->live.pref_idx, &f->live.edges,
-                    &f->live.models, &f->live.ovf, &f->live.keys, &f->live.rs_words, &f->live.flags, &f->live.scratch_idx,
-                    &f->live.scratch_rows, &f->live.scratch_edges, &f->live.edge_ts, &f->live.model_lul, &f->live.type_part_off, &f->live.type_parts})
-    b->release();
-  for (DevBuf *b : {&f->d_flush, &f->zero_row, &f->lru_ts, &f->lru_seq, &f->lru_weight, &f->lru_model,
-                    &f->lru_cap, &f->lru_wsize, &f->lru_count, &f->lru_seqctr, &f->lru_loadts, &f->lru_pin})
-    b->release();
-  if (f->commit_stream) cudaStreamDestroy(f->commit_stream);
-  delete f;
+  delete f;  // (its members free the device buffers, streams, events, graphs, pinned buffers and IPC mappings they own)
 }
 
 #define NEED(f) do { if (!(f)) { g_err = "null fleet"; return MMP_E_ARG; } } while (0)
@@ -2189,7 +2190,7 @@ int32_t mmp_commit_info(mmp_fleet *f, int32_t *path, double *ms) {
 static void server_stop(mmp_fleet *f) {
   mmp_fleet::Server &sv = f->srv;
   if (!sv.mapped || !sv.running) return;
-  volatile SrvLine0 *l0 = reinterpret_cast<volatile SrvLine0 *>(sv.mapped);
+  volatile SrvLine0 *l0 = reinterpret_cast<volatile SrvLine0 *>(sv.mapped.get());
   sv.seq++;
   l0->seq = (sv.seq & 0x00ffffffffffffffull) | (0xffull << 56);  // kind 0xff: leave
   std::atomic_thread_fence(std::memory_order_seq_cst);
@@ -2201,9 +2202,9 @@ static int32_t place_server(mmp_fleet *f, const DeviceSnapshot &ds, const mmp_de
                             const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed) {
   mmp_fleet::Server &sv = f->srv;
   if (!sv.mapped) {
-    CK(cudaHostAlloc((void **)&sv.mapped, PlaceCtx::MAPPED_BYTES, cudaHostAllocMapped));
+    CK(cudaHostAlloc((void **)sv.mapped.put(), PlaceCtx::MAPPED_BYTES, cudaHostAllocMapped));
     memset(sv.mapped, 0, PlaceCtx::MAPPED_BYTES);
-    CK(cudaStreamCreateWithFlags(&sv.stream, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(sv.stream.put(), cudaStreamNonBlocking));
   }
   unsigned char *h = sv.mapped, *dbase = nullptr;
   CK(cudaHostGetDevicePointer((void **)&dbase, h, 0));
@@ -2305,14 +2306,14 @@ static int32_t place_mapped(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds,
     SmallHdr *hd = reinterpret_cast<SmallHdr *>(h);
     hd->now = now_ms; hd->seed = seed; hd->id_base = f->id_base.load(); hd->n = n; hd->n_fresh = n_fresh; hd->n_extra = n_extra;
     if (c->graph_epoch != f->epoch || !c->graph_exec) {
-      if (c->graph_exec) { cudaGraphExecDestroy(c->graph_exec); c->graph_exec = nullptr; }
-      if (c->graph) { cudaGraphDestroy(c->graph); c->graph = nullptr; }
+      c->graph_exec.reset();
+      c->graph.reset();  // (not inside the capture below)
       SnapshotView gv = ds.view;
       gv.n_extra = 32 * MMP_MAX_EXTRA;
       CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
       k_place_small<<<1, 32, 0, st>>>(gv, d_in, 0, d_fr, 32, d_ex, d_out, 0, 0, 0, reinterpret_cast<const volatile SmallHdr *>(dbase), f->lane_budget);
-      CK(cudaStreamEndCapture(st, &c->graph));
-      CK(cudaGraphInstantiate(&c->graph_exec, c->graph, 0));
+      CK(cudaStreamEndCapture(st, c->graph.put()));
+      CK(cudaGraphInstantiate(c->graph_exec.put(), c->graph, 0));
       c->graph_epoch = f->epoch;
     }
     CK(cudaGraphLaunch(c->graph_exec, st));
