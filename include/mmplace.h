@@ -348,7 +348,8 @@ int32_t mmp_lru_state(mmp_fleet *, int32_t n_instances, int64_t *oldest, int64_t
  *   REMOVE -> runtimeCache.remove on every registered copy;
  *   then the registry changes, publishInstanceRecord with its significance thresholds (MM:5390-5470) per instance, and a
  *   commit (re-rank under PLACEMENT_ORDER, tables, bitmap) -- all on the device.  The host only reads the reports.
- * Requires an unsharded fleet whose models have at most 4 registered copies + failed loads.  Replaces nothing in the
+ * Requires an unsharded fleet; a model may hold any number of registrations (loaded copies, then failed loads), as long as
+ * its copy_count tells its loaded copies apart (not saturated at 255 over more than 255 registrations).  Replaces nothing in the
  * reference 1:1 (each pod runs its own loop there); it is the batched, fleet-wide form of it for simulation / what-if runs. ---- */
 enum { MMP_CHURN_REQUEST = 0, MMP_CHURN_REMOVE = 1 };
 typedef struct { int32_t type; int32_t model; int32_t caller; uint32_t u; int64_t t; } mmp_churn_event;
@@ -379,6 +380,9 @@ int32_t mmp_churn_step(mmp_fleet *, const mmp_churn_event *ev, int32_t n, int64_
                        int32_t *n_evict, mmp_instance_row *rows_out, mmp_churn_report *report);
 /* registry state of one model as the device holds it: row + the 4 inline instance indices (first copy_count = loaded) */
 int32_t mmp_churn_model(mmp_fleet *, int32_t model, mmp_model_row *row, int32_t *instances4);
+/* the same, with every registration: ids[0 .. min(n, cap)) = the model's instance indices in registration order (the first
+ * copy_count loaded, then the failed loads); returns n, the model's registration count (row may be NULL) */
+int32_t mmp_churn_model_ids(mmp_fleet *, int32_t model, mmp_model_row *row, int32_t *ids, int32_t cap);
 /* ---- registry-side batch scans (SURVEY.md §8a row a14, §8f-2) ---- */
 /* MR.instanceIds / failedIn VALUES (load-start / failure times) and MR.lastUnloadTime ("lul").  edge_ts[i] is the time of the
  * i-th id of the model's last mmp_model_upsert (loaded first, then failed), for every registration; times past the model's

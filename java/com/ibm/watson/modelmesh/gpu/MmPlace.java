@@ -101,4 +101,5 @@ final class MmPlace {
     static native int churnStep(long h, ByteBuffer events, int n, long now0, long now1, long seed, ByteBuffer decOut, int decCap,
                                 ByteBuffer evictOut, int evictCap, ByteBuffer rowsOut, ByteBuffer report, int[] countsOut);
     static native int churnModel(long h, int model, ByteBuffer rowOut, ByteBuffer instances4);
+    static native int churnModelIds(long h, int model, ByteBuffer rowOut, ByteBuffer ids, int cap);
 }

@@ -384,3 +384,8 @@ jint FN(churnModel)(JNIEnv *env, jclass c, jlong h, jint model, jobject rowOut, 
   (void)c;
   return mmp_churn_model(H(h), model, (mmp_model_row *)BUF(rowOut), (int32_t *)BUF(instances4));
 }
+/* ids: int32[cap] direct buffer; returns the model's registration count */
+jint FN(churnModelIds)(JNIEnv *env, jclass c, jlong h, jint model, jobject rowOut, jobject ids, jint cap) {
+  (void)c;
+  return mmp_churn_model_ids(H(h), model, (mmp_model_row *)BUF(rowOut), (int32_t *)BUF(ids), cap);
+}

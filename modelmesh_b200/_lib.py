@@ -138,6 +138,7 @@ SYMBOLS = [
     ("mmp_churn_seed", _I32, [_P, _I32, _P, _P, _P, _P, _P, _I64]),
     ("mmp_churn_step", _I32, [_P, _P, _I32, _I64, _I64, _U64, _P, _I32, C.POINTER(_I32), _P, _I32, C.POINTER(_I32), _P, C.c_void_p]),
     ("mmp_churn_model", _I32, [_P, _I32, _P, _P]),
+    ("mmp_churn_model_ids", _I32, [_P, _I32, _P, _P, _I32]),
     ("mmp_commit_info", _I32, [_P, C.POINTER(_I32), C.POINTER(C.c_double)]),
     ("mmp_model_times", _I32, [_P, _I32, _P, _I32, _I64]),
     ("mmp_scale_eval", _I32, [_P, _P, _I32, _P, _P]),

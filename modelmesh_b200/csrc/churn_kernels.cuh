@@ -29,37 +29,41 @@ __global__ void k_churn_first(const Follow *__restrict__ carry, int n_follow, co
   if (model < 0 || model >= n_models) return;
   if (models[model].copy_count == 0) atomicMin(&first_ev[model], q);
 }
-// phase A.2: which items become decisions (every follow-on; the first miss of a model)
+// phase A.2: which items become decisions (every follow-on; the first miss of a model), and how many cache-event slots each
+// item owns: one for a decision's load (phase C) or a cache hit, one per loaded copy for a REMOVE.  x = decision, y = slots.
 __global__ void k_churn_flag(const Follow *__restrict__ carry, int n_follow, const mmp_churn_event *__restrict__ ev, int n,
                              const mmp_model_row *__restrict__ models, int n_models, const int *__restrict__ first_ev,
-                             int *__restrict__ is_dec, long long *__restrict__ used_t, int *__restrict__ counters) {
+                             int2 *__restrict__ is_dec, long long *__restrict__ used_t, int *__restrict__ counters) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_follow + n) return;
-  int d = 0;
+  int d = 0, slots = 0;
   if (q < n_follow) d = 1;
   else {
     const mmp_churn_event e = ev[q - n_follow];
-    if (e.model >= 0 && e.model < n_models && e.type == 0) {
-      atomicMax(&used_t[e.model], (long long)e.t);  // MR.updateLastUsed at the end of the window
-      if (models[e.model].copy_count == 0) { if (first_ev[e.model] == q) d = 1; else atomicAdd(&counters[3], 1); }  // coalesced
+    if (e.model >= 0 && e.model < n_models) {
+      const int cc = models[e.model].copy_count;
+      if (e.type == 0) {
+        atomicMax(&used_t[e.model], (long long)e.t);  // MR.updateLastUsed at the end of the window
+        if (cc > 0) slots = 1;
+        else if (first_ev[e.model] == q) d = 1;
+        else atomicAdd(&counters[3], 1);  // coalesced
+      } else if (e.type == 1) slots = cc;
     }
   }
-  is_dec[q] = d;
+  is_dec[q] = make_int2(d, slots + d);
 }
-// phase A.3: decision records + the cache events of hits and removals.  Every item owns 4 event slots (a REMOVE reaches up
-// to 4 registered copies); unused slots keep the key ~0 and sort to the end.
+// phase A.3: decision records + the cache events of hits and removals, each in the slots the scan of k_churn_flag gave its
+// item (pos.y); a slot whose copy names no instance keeps the key ~0 and sorts to the end.
 __global__ void k_churn_emit(const Follow *__restrict__ carry, int n_follow, const mmp_churn_event *__restrict__ ev, int n,
-                             const mmp_model_row *__restrict__ models, const int4 *__restrict__ edges, int n_models, int max_instances,
-                             const int *__restrict__ first_ev, const int *__restrict__ is_dec, const int *__restrict__ dec_pos,
+                             const mmp_model_row *__restrict__ models, RegTables R, int n_models, int max_instances,
+                             const int *__restrict__ first_ev, const int2 *__restrict__ is_dec, const int2 *__restrict__ dec_pos,
                              mmp_decision_in *__restrict__ dec_in, DecMeta *__restrict__ meta, int32_t *__restrict__ extra,
                              int *__restrict__ status, int *__restrict__ dec_of_model, LruEv *__restrict__ lev,
                              unsigned long long *__restrict__ keys, long long now0) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_follow + n) return;
-  unsigned long long *kq = keys + (size_t)q * 4;
-  kq[0] = kq[1] = kq[2] = kq[3] = ~0ull;
-  if (is_dec[q]) {
-    const int k = dec_pos[q];
+  if (is_dec[q].x) {
+    const int k = dec_pos[q].x;
     mmp_decision_in d;
     d.flags = 0; d.fresh = -1; d.extra_off = k; d.extra_n = 0;
     DecMeta m;
@@ -86,36 +90,39 @@ __global__ void k_churn_emit(const Follow *__restrict__ carry, int n_follow, con
   const mmp_churn_event e = ev[q - n_follow];
   if (e.model < 0 || e.model >= n_models) return;
   const int cc = models[e.model].copy_count;
-  if (cc == 0) return;
-  const int4 ed = edges[e.model];
-  const int es[4] = {ed.x, ed.y, ed.z, ed.w};
-  const int ncopy = cc < 4 ? cc : 4;
+  if (cc == 0 || e.type > 1) return;
+  const size_t s0 = (size_t)dec_pos[q].y;
+  const ModelRegs g = model_regs(R, e.model, (unsigned)cc);
+  long long ts;
   if (e.type == 0) {  // cache hit on copy (u mod copies) in registration order
-    const int inst = es[e.u % (unsigned)ncopy];
+    const int inst = reg_at(R, g, (int)(e.u % (unsigned)cc), ts);
+    keys[s0] = ~0ull;
     if (inst >= 0 && inst < max_instances) {
-      lev[(size_t)q * 4] = LruEv{LEV_TOUCH, e.model, 0, q, -1, 0, e.t, e.t};
-      kq[0] = ((unsigned long long)(unsigned)inst << 32) | (unsigned)q;
+      lev[s0] = LruEv{LEV_TOUCH, e.model, 0, q, -1, 0, e.t, e.t};
+      keys[s0] = ((unsigned long long)(unsigned)inst << 32) | (unsigned)q;
     }
-  } else if (e.type == 1) {
-    for (int j = 0; j < ncopy; j++) {
-      const int inst = es[j];
+  } else {
+    for (int j = 0; j < cc; j++) {
+      const int inst = reg_at(R, g, j, ts);
+      keys[s0 + j] = ~0ull;
       if (inst < 0 || inst >= max_instances) continue;
-      lev[(size_t)q * 4 + j] = LruEv{LEV_REMOVE, e.model, 0, q, -1, 0, 0, e.t};
-      kq[j] = ((unsigned long long)(unsigned)inst << 32) | (unsigned)q;
+      lev[s0 + j] = LruEv{LEV_REMOVE, e.model, 0, q, -1, 0, 0, e.t};
+      keys[s0 + j] = ((unsigned long long)(unsigned)inst << 32) | (unsigned)q;
     }
   }
 }
 // phase C.1: a decision that found a target becomes a checked load on that instance; its clock is the clock of the request
 // that caused it (queued follow-ons: the start of the window)
 __global__ void k_churn_route(const mmp_decision_in *__restrict__ dec_in, const mmp_decision_out *__restrict__ dec_out,
-                              const DecMeta *__restrict__ meta, const int *__restrict__ is_dec, const int *__restrict__ dec_pos, int n_items,
+                              const DecMeta *__restrict__ meta, const int2 *__restrict__ is_dec, const int2 *__restrict__ dec_pos, int n_items,
                               int max_instances, const mmp_churn_event *__restrict__ ev, long long now0, int *__restrict__ status,
-                              int *__restrict__ dec_target, LruEv *__restrict__ lev, unsigned long long *__restrict__ keys, size_t slot0) {
+                              int *__restrict__ dec_target, LruEv *__restrict__ lev, unsigned long long *__restrict__ keys) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_items) return;
-  keys[slot0 + q] = ~0ull;
-  if (!is_dec[q]) return;
-  const int k = dec_pos[q];
+  if (!is_dec[q].x) return;
+  const size_t slot = (size_t)dec_pos[q].y;
+  keys[slot] = ~0ull;
+  const int k = dec_pos[q].x;
   dec_target[k] = -1;
   if (status[k] == CH_SKIPPED) return;
   const mmp_decision_out o = dec_out[k];
@@ -125,8 +132,8 @@ __global__ void k_churn_route(const mmp_decision_in *__restrict__ dec_in, const 
   if (tgt < 0 || tgt >= max_instances) { status[k] = CH_INVALID; return; }
   dec_target[k] = tgt;
   const DecMeta m = meta[k];
-  lev[slot0 + q] = LruEv{LEV_LOAD, d.model, m.weight, m.order, k, 0, d.last_used, m.event >= 0 ? (long long)ev[m.event].t : now0};
-  keys[slot0 + q] = ((unsigned long long)(unsigned)tgt << 32) | (unsigned)m.order;
+  lev[slot] = LruEv{LEV_LOAD, d.model, m.weight, m.order, k, 0, d.last_used, m.event >= 0 ? (long long)ev[m.event].t : now0};
+  keys[slot] = ((unsigned long long)(unsigned)tgt << 32) | (unsigned)m.order;
 }
 // per-instance ranges of the sorted event list
 __global__ void k_churn_offsets(const unsigned long long *__restrict__ keys, int n_keys, int n_inst, int *__restrict__ off) {
@@ -137,8 +144,38 @@ __global__ void k_churn_offsets(const unsigned long long *__restrict__ keys, int
   while (lo < hi) { const int mid = (lo + hi) >> 1; if (keys[mid] < want) lo = mid + 1; else hi = mid; }
   off[i] = lo;  // (invalid keys are ~0: beyond every instance)
 }
-__global__ void k_iota(int *v, int n) { const int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) v[i] = i; }
-// phase D: edge lists, copy counts, lastUsed.  One thread per model; only models touched in the window do any work.
+// the sort's input: value = slot; the slots past the last item's (n_used = pos.y + slots of the last item) hold no event
+__global__ void k_churn_tail(unsigned long long *__restrict__ keys, int *__restrict__ vals, int n_keys, const int2 *__restrict__ is_dec,
+                             const int2 *__restrict__ dec_pos, int n_items) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_keys) return;
+  vals[i] = i;
+  if (i >= dec_pos[n_items - 1].y + is_dec[n_items - 1].y) keys[i] = ~0ull;
+}
+// A model's registrations after the window: the surviving loaded copies in order, the window's accepted load, the failed
+// loads.  emit(k, instance, ts) for each; returns {registrations, loaded}.  Each keeps the time it had (0 for the new load).
+template <class Emit>
+__device__ __forceinline__ int2 churn_regs_after(const RegTables &R, const ModelRegs &g, int cc, int nreg, unsigned rm, int add,
+                                                 const unsigned char *ovf_dead, Emit emit) {
+  int k = 0, loaded = 0;
+  bool have = false;
+  long long ts;
+  for (int j = 0; j < cc; j++) {
+    const int inst = reg_at(R, g, j, ts);
+    if (inst < 0 || (j < 4 ? (rm >> j) & 1u : ovf_dead[g.ovf0 + j - 4])) continue;
+    emit(k++, inst, ts); loaded++;
+    if (inst == add) have = true;
+  }
+  if (add >= 0 && !have) { emit(k++, add, 0ll); loaded++; }
+  for (int j = cc; j < nreg; j++) {
+    const int inst = reg_at(R, g, j, ts);
+    if (inst >= 0) emit(k++, inst, ts);
+  }
+  return make_int2(k, loaded);
+}
+// phase D: edge lists, copy counts, lastUsed.  One thread per model; only models touched in the window do any work.  A
+// touched model with overflow registrations before or after the window keeps its marks for the re-lay below (k_ovf_relay)
+// and raises counters[2].
 __global__ void k_churn_registry(mmp_model_row *__restrict__ models, int4 *__restrict__ edges, int n_models, unsigned *__restrict__ rm_mask,
                                  int *__restrict__ add_inst, long long *__restrict__ used_t, int *__restrict__ counters) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
@@ -149,27 +186,59 @@ __global__ void k_churn_registry(mmp_model_row *__restrict__ models, int4 *__res
   if (rm == 0 && add < 0 && ut == 0) return;
   mmp_model_row r = models[m];
   if (ut > r.last_used) r.last_used = ut;  // MR:239-246
-  if (rm != 0 || add >= 0) {
-    const int4 ed = edges[m];
-    const int es[4] = {ed.x, ed.y, ed.z, ed.w};
+  if ((rm != 0 || add >= 0) && (r.reserved > 4u || (r.reserved == 4u && add >= 0))) atomicOr(&counters[2], 1);
+  else if (rm != 0 || add >= 0) {
     int out[4] = {-1, -1, -1, -1};
-    int k = 0, loaded = 0;
-    const int cc = r.copy_count < 4 ? r.copy_count : 4;
-    bool have = false;
-    for (int j = 0; j < cc; j++)
-      if (!((rm >> j) & 1u) && es[j] >= 0) { out[k++] = es[j]; loaded++; if (es[j] == add) have = true; }
-    if (add >= 0 && !have) {
-      if (k < 4) { out[k++] = add; loaded++; } else atomicOr(&counters[2], 1);  // more registered copies than the inline list holds
-    }
-    for (int j = cc; j < 4; j++)  // failed-load records follow the loaded ones
-      if (es[j] >= 0) { if (k < 4) out[k++] = es[j]; else atomicOr(&counters[2], 1); }
+    const RegTables R{edges, nullptr, nullptr, 0};
+    const int2 kl = churn_regs_after(R, model_regs(R, m, 0u), r.copy_count, (int)r.reserved, rm, add, nullptr,
+                                     [&](int k, int inst, long long) { out[k] = inst; });
     edges[m] = make_int4(out[0], out[1], out[2], out[3]);
-    r.copy_count = (uint8_t)loaded;
-    r.reserved = (uint32_t)k;
+    r.copy_count = (uint8_t)kl.y;
+    r.reserved = (uint32_t)kl.x;
     rm_mask[m] = 0; add_inst[m] = -1;
   }
   used_t[m] = 0;
   models[m] = r;
+}
+// The re-lay of the overflow table, when counters[2] is up.  k_ovf_count: overflow registrations of every model after the
+// window (a marked model: its new list; any other: as before); an exclusive scan gives each model its slice of the new table.
+__global__ void k_ovf_count(RegTables R, const mmp_model_row *__restrict__ models, int n_models, const unsigned *__restrict__ rm_mask,
+                            const int *__restrict__ add_inst, const unsigned char *__restrict__ ovf_dead, int *__restrict__ n_out) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m > n_models) return;
+  if (m == n_models) { n_out[m] = 0; return; }
+  const mmp_model_row r = models[m];
+  int k = (int)r.reserved;
+  if (rm_mask[m] != 0 || add_inst[m] >= 0)
+    k = churn_regs_after(R, model_regs(R, m, r.reserved), r.copy_count, (int)r.reserved, rm_mask[m], add_inst[m], ovf_dead,
+                         [](int, int, long long) {}).x;
+  n_out[m] = k > 4 ? k - 4 : 0;
+}
+// k_ovf_relay: every model writes its slice of the new table (sorted by model, then position, as the old one); a marked
+// model also rewrites its inline edges, copy count and registration count, and clears its marks
+__global__ void k_ovf_relay(RegTables R, mmp_model_row *models, int4 *edges, int n_models, unsigned *__restrict__ rm_mask,
+                            int *__restrict__ add_inst, const unsigned char *__restrict__ ovf_dead, const int *__restrict__ off,
+                            OvfEdge *__restrict__ out) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n_models) return;
+  const unsigned rm = rm_mask[m];
+  const int add = add_inst[m];
+  mmp_model_row r = models[m];
+  OvfEdge *o = out + off[m];
+  if (rm == 0 && add < 0) {
+    if (r.reserved <= 4u) return;
+    const ModelRegs g = model_regs(R, m, r.reserved);
+    for (int j = 4; j < (int)r.reserved; j++) o[j - 4] = R.ovf[g.ovf0 + j - 4];
+    return;
+  }
+  int e[4] = {-1, -1, -1, -1};
+  const int2 kl = churn_regs_after(R, model_regs(R, m, r.reserved), r.copy_count, (int)r.reserved, rm, add, ovf_dead,
+                                   [&](int k, int inst, long long ts) { if (k < 4) e[k] = inst; else o[k - 4] = OvfEdge{m, inst, ts}; });
+  edges[m] = make_int4(e[0], e[1], e[2], e[3]);
+  r.copy_count = (uint8_t)kl.y;
+  r.reserved = (uint32_t)kl.x;
+  models[m] = r;
+  rm_mask[m] = 0; add_inst[m] = -1;
 }
 __global__ void k_churn_collect_adds(const mmp_decision_in *__restrict__ dec_in, const int *__restrict__ status, const int *__restrict__ dec_target,
                                      int n_dec, int *__restrict__ add_inst, int *__restrict__ dec_of_model) {
@@ -262,12 +331,48 @@ static int32_t commit_locked(mmp_fleet *f);  // mmplace.cu: mmp_fleet_commit wit
 static inline int32_t lv_n_types(mmp_fleet *f) { return f->live.n_type_ids; }
 
 static int32_t sync_host_from_device(mmp_fleet *f) {
-  const int32_t nm = f->hs.n_models_used;
+  HostState &hs = f->hs;
+  const int32_t nm = hs.n_models_used;
+  std::vector<OvfEdge> ovf((size_t)f->live.n_ovf);
   if (nm) {
-    CK(cudaMemcpy(f->hs.models.data(), f->live.models.p, (size_t)nm * sizeof(mmp_model_row), cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(f->hs.edge_inl.data(), f->live.edges.p, (size_t)nm * HostState::EDGE_INL * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(hs.models.data(), f->live.models.p, (size_t)nm * sizeof(mmp_model_row), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(hs.edge_inl.data(), f->live.edges.p, (size_t)nm * HostState::EDGE_INL * 4, cudaMemcpyDeviceToHost));
   }
+  if (!ovf.empty()) CK(cudaMemcpy(ovf.data(), f->live.ovf.p, ovf.size() * sizeof(OvfEdge), cudaMemcpyDeviceToHost));
+  // the overflow registrations as the loop left them: models that went back inline lose their entries
+  hs.edge_ovf.clear(); hs.edge_ovf_ts.clear();
+  for (const OvfEdge &e : ovf) { hs.edge_ovf[e.model].push_back(e.inst); hs.edge_ovf_ts[e.model].push_back(e.ts); }
+  hs.ovf_dirty = true;
   f->device_ahead = false;
+  return MMP_OK;
+}
+// Exclusive prefix sums of (decision, event slots) pairs
+struct Int2Sum { __host__ __device__ int2 operator()(const int2 &a, const int2 &b) const { return make_int2(a.x + b.x, a.y + b.y); } };
+
+// The registry phase's re-lay of the overflow table (lv.ovf / lv.n_ovf) after a window that touched a model with more than
+// four registrations or pushed one past four: count, scan, write the new table beside the old one, swap.
+static int32_t churn_relay_ovf(mmp_fleet *f, cudaStream_t st) {
+  ChurnState &cs = f->churn;
+  LiveState &lv = f->live;
+  const int32_t NM = f->hs.n_models_used;
+  CK(cs.ovf_count.ensure((size_t)(NM + 1) * 8));
+  int *cnt = cs.ovf_count.as<int>(), *off = cnt + NM + 1;
+  k_ovf_count<<<(NM + 1 + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), NM, cs.rm_mask.as<unsigned>(),
+                                                   cs.add_inst.as<int>(), cs.ovf_dead.as<unsigned char>(), cnt);
+  size_t tmp = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, cnt, off, NM + 1, st));
+  CK(cs.cub_tmp.ensure(tmp + 16));
+  CK(cub::DeviceScan::ExclusiveSum(cs.cub_tmp.p, tmp, cnt, off, NM + 1, st));
+  int total = 0;
+  CK(cudaMemcpyAsync(&total, off + NM, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  CK(cs.ovf_next.ensure((size_t)std::max(total, 1) * sizeof(OvfEdge)));
+  k_ovf_relay<<<(NM + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.edges.as<int4>(), NM, cs.rm_mask.as<unsigned>(),
+                                               cs.add_inst.as<int>(), cs.ovf_dead.as<unsigned char>(), off, cs.ovf_next.as<OvfEdge>());
+  f->launches += 4;
+  CK(cudaGetLastError());
+  std::swap(lv.ovf, cs.ovf_next);
+  lv.n_ovf = total;
   return MMP_OK;
 }
 
@@ -280,7 +385,11 @@ int32_t mmp_churn_init(mmp_fleet *f, const mmp_churn_config *cfg) {
   if (rc < 0) return rc;
   if (f->epoch == 0 || !f->live.valid) { g_err = "mmp_churn_init needs a committed snapshot"; return MMP_E_EPOCH; }
   if (f->hs.cfg.shard_count > 1) { g_err = "the closed loop runs on an unsharded fleet"; return MMP_E_STATE; }
-  if (!f->hs.edge_ovf.empty()) { g_err = "the closed loop keeps at most 4 registered copies + failures per model on the device"; return MMP_E_STATE; }
+  for (int32_t m = 0; m < f->hs.n_models_used; m++)
+    if (f->hs.models[m].copy_count == 255 && f->hs.models[m].reserved > 255u) {
+      g_err = "model " + std::to_string(m) + " holds more registrations than a copy count (255) can tell apart: its loaded copies are unknown";
+      return MMP_E_STATE;
+    }
   const int32_t NI = f->hs.cfg.max_instances, NM = f->hs.cfg.max_models;
   std::vector<int64_t> cap((size_t)NI, 0);
   for (int32_t i = 0; i < NI; i++) if (f->hs.inst[i].present) cap[i] = f->hs.inst[i].row.capacity;
@@ -302,6 +411,7 @@ int32_t mmp_churn_init(mmp_fleet *f, const mmp_churn_config *cfg) {
   CK(cudaMemsetAsync(cs.used_t.p, 0, (size_t)NM * 8, f->commit_stream));
   CK(cudaStreamSynchronize(f->commit_stream));
   cs.n_carry = 0;
+  cs.regs_from_host = true;
   cs.on = true;
   return MMP_OK;
 }
@@ -337,8 +447,8 @@ int32_t mmp_churn_seed(mmp_fleet *f, int32_t n, const int32_t *instance, const i
   const int grid = (f->lru_n + 3) / 4;
   size_t lsm = 0;
   const int lst = lru_stage_slots(f, &lsm);
-  k_lru_events<<<grid, 128, lsm, st>>>(lru_view(f), cs.lev.as<LruEv>(), cs.vals.as<int>(), cs.off.as<int>(), now_ms, 0, hk, cs.evict.as<EvictRec>(),
-                                      16, cs.counters.as<int>() + 4, cs.counters.as<int>() + 5, lst);
+  k_lru_events<false><<<grid, 128, lsm, st>>>(lru_view(f), cs.lev.as<LruEv>(), cs.vals.as<int>(), cs.off.as<int>(), now_ms, 0, hk, cs.evict.as<EvictRec>(),
+                                      16, cs.counters.as<int>() + 4, cs.counters.as<int>() + 5, lst, OvfHooks{});
   f->launches++;
   CK(cudaGetLastError());
   int hdr[8];
@@ -371,8 +481,25 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   CtxLease c(f);
   if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
   const Event *evs = cs.phase_ev;
-  const size_t QQ = (size_t)std::max(Q, 1), NK = 5 * QQ;
-  CK(cs.ev.ensure(QQ * sizeof(mmp_churn_event))); CK(cs.is_dec.ensure(QQ * 4 + 16)); CK(cs.dec_pos.ensure(QQ * 4 + 16));
+  if (cs.regs_from_host) {  // (see ChurnState)
+    cs.max_copies = 1; cs.deep_failed = false;
+    for (int32_t m = 0; m < NM; m++) {
+      const mmp_model_row &r = f->hs.models[m];
+      cs.max_copies = std::max<int32_t>(cs.max_copies, r.copy_count);
+      if (r.reserved >= 4u + r.copy_count) cs.deep_failed = true;
+    }
+    cs.regs_from_host = false;
+  }
+  // event slots: one per decision or cache hit, one per loaded copy of a REMOVE's model
+  size_t n_remove = 0;
+  for (int32_t i = 0; i < n; i++) n_remove += ev[i].type == 1;
+  const size_t QQ = (size_t)std::max(Q, 1), NK = QQ + n_remove * (size_t)(cs.max_copies - 1);
+  if (NK > (size_t)INT32_MAX) { g_err = "too many cache events in one window"; return MMP_E_ARG; }
+  // the window's marks may reach an overflow registration (a model with more than four), or its registry phase may push a
+  // model with four failed loads past four: then the registry phase reads the mark flag back and re-lays lv.ovf
+  const bool ovf_window = lv.n_ovf > 0 || cs.deep_failed;
+  if (lv.n_ovf > 0) CK(cs.ovf_dead.ensure((size_t)lv.n_ovf));
+  CK(cs.ev.ensure(QQ * sizeof(mmp_churn_event))); CK(cs.is_dec.ensure(QQ * 8 + 16)); CK(cs.dec_pos.ensure(QQ * 8 + 16));
   CK(cs.dec_in.ensure(QQ * sizeof(mmp_decision_in))); CK(cs.dec_out.ensure(QQ * sizeof(mmp_decision_out)));
   CK(cs.dec_meta.ensure(QQ * sizeof(DecMeta))); CK(cs.dec_target.ensure(QQ * 4)); CK(cs.extra.ensure(QQ * 4)); CK(cs.status.ensure(QQ * 4));
   CK(cs.lev.ensure(NK * sizeof(LruEv))); CK(cs.keys.ensure(NK * 8)); CK(cs.vals.ensure(NK * 4)); CK(cs.keys2.ensure(NK * 8)); CK(cs.vals2.ensure(NK * 4));
@@ -384,6 +511,7 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   if (n) CK(cudaMemcpyAsync(cs.ev.p, ev, (size_t)n * sizeof(mmp_churn_event), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(cs.counters.p, 0, 64, st));
   CK(cudaMemsetAsync(cs.force_publish.p, 0, (size_t)NI, st));
+  if (lv.n_ovf > 0) CK(cudaMemsetAsync(cs.ovf_dead.p, 0, (size_t)lv.n_ovf, st));
   // ---- the rebalance rule's fullness test reads the stats of the window's snapshot (MM:2918-2920) ----
   {
     const int np = (int)ds.host.part_types.size();
@@ -404,20 +532,22 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   const int qb = (Q + 255) / 256;
   const mmp_model_row *lmodels = lv.models.as<mmp_model_row>();
   const Follow *carry = cs.carry.as<Follow>();
+  const RegTables R{lv.edges.as<int4>(), nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
+  bool relaid = false;
   if (Q > 0) {
     // ---- A: classify ----
     k_churn_first<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, NM, cs.first_ev.as<int>());
-    k_churn_flag<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, NM, cs.first_ev.as<int>(), cs.is_dec.as<int>(),
+    k_churn_flag<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, NM, cs.first_ev.as<int>(), cs.is_dec.as<int2>(),
                                     cs.used_t.as<long long>(), cs.counters.as<int>());
     size_t tmp = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, cs.is_dec.as<int>(), cs.dec_pos.as<int>(), Q, st));
+    CK(cub::DeviceScan::ExclusiveScan(nullptr, tmp, cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), Int2Sum(), make_int2(0, 0), Q, st));
     CK(cs.cub_tmp.ensure(tmp + 16));
-    CK(cub::DeviceScan::ExclusiveSum(cs.cub_tmp.p, tmp, cs.is_dec.as<int>(), cs.dec_pos.as<int>(), Q, st));
+    CK(cub::DeviceScan::ExclusiveScan(cs.cub_tmp.p, tmp, cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), Int2Sum(), make_int2(0, 0), Q, st));
     // decision records beyond the window's count stay malformed (model -1): the scoring kernel answers them INVALID
     CK(cudaMemsetAsync(cs.dec_in.p, 0xff, QQ * sizeof(mmp_decision_in), st));
     CK(cudaMemsetAsync(cs.status.p, 0, QQ * 4, st));
-    k_churn_emit<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, lv.edges.as<int4>(), NM, NI, cs.first_ev.as<int>(),
-                                    cs.is_dec.as<int>(), cs.dec_pos.as<int>(), cs.dec_in.as<mmp_decision_in>(), cs.dec_meta.as<DecMeta>(),
+    k_churn_emit<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, R, NM, NI, cs.first_ev.as<int>(),
+                                    cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), cs.dec_in.as<mmp_decision_in>(), cs.dec_meta.as<DecMeta>(),
                                     cs.extra.as<int32_t>(), cs.status.as<int>(), cs.dec_of_model.as<int>(), cs.lev.as<LruEv>(),
                                     cs.keys.as<unsigned long long>(), now0);
     f->launches += 5;
@@ -433,16 +563,17 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
     CK(cudaEventRecord(evs[2], st));
     // ---- C: route every cache event to its instance ----
     k_churn_route<<<qb, 256, 0, st>>>(cs.dec_in.as<mmp_decision_in>(), cs.dec_out.as<mmp_decision_out>(), cs.dec_meta.as<DecMeta>(),
-                                     cs.is_dec.as<int>(), cs.dec_pos.as<int>(), Q, NI, cs.ev.as<mmp_churn_event>(), now0, cs.status.as<int>(),
-                                     cs.dec_target.as<int>(), cs.lev.as<LruEv>(), cs.keys.as<unsigned long long>(), 4 * (size_t)Q);
-    k_iota<<<(int)((NK + 255) / 256), 256, 0, st>>>(cs.vals.as<int>(), (int)(5 * (size_t)Q));
+                                     cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), Q, NI, cs.ev.as<mmp_churn_event>(), now0, cs.status.as<int>(),
+                                     cs.dec_target.as<int>(), cs.lev.as<LruEv>(), cs.keys.as<unsigned long long>());
+    k_churn_tail<<<(int)((NK + 255) / 256), 256, 0, st>>>(cs.keys.as<unsigned long long>(), cs.vals.as<int>(), (int)NK, cs.is_dec.as<int2>(),
+                                                          cs.dec_pos.as<int2>(), Q);
     tmp = 0;
     CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, cs.keys.as<unsigned long long>(), cs.keys2.as<unsigned long long>(), cs.vals.as<int>(),
-                                       cs.vals2.as<int>(), (int)(5 * (size_t)Q), 0, 64, st));
+                                       cs.vals2.as<int>(), (int)NK, 0, 64, st));
     CK(cs.cub_tmp.ensure(tmp + 16));
     CK(cub::DeviceRadixSort::SortPairs(cs.cub_tmp.p, tmp, cs.keys.as<unsigned long long>(), cs.keys2.as<unsigned long long>(), cs.vals.as<int>(),
-                                       cs.vals2.as<int>(), (int)(5 * (size_t)Q), 0, 64, st));
-    k_churn_offsets<<<(NI + 1 + 255) / 256, 256, 0, st>>>(cs.keys2.as<unsigned long long>(), (int)(5 * (size_t)Q), NI, cs.off.as<int>());
+                                       cs.vals2.as<int>(), (int)NK, 0, 64, st));
+    k_churn_offsets<<<(NI + 1 + 255) / 256, 256, 0, st>>>(cs.keys2.as<unsigned long long>(), (int)NK, NI, cs.off.as<int>());
     f->launches += 5;
     CK(cudaGetLastError());
     CK(cudaEventRecord(evs[3], st));
@@ -451,14 +582,17 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
     hk.enabled = 1;
     hk.min_space = f->hs.cfg.min_space_units; hk.min_churn_age = f->hs.cfg.min_churn_age_ms; hk.load_timeout = cs.load_timeout_ms;
     hk.status = cs.status.as<int>(); hk.dec_target = cs.dec_target.as<int>(); hk.dec_of_model = cs.dec_of_model.as<int>();
-    hk.edges = lv.edges.as<int4>(); hk.models = lmodels; hk.rm_mask = cs.rm_mask.as<unsigned>();
+    hk.edges = R.edges; hk.models = lmodels; hk.rm_mask = cs.rm_mask.as<unsigned>();
     hk.type_ok = cs.type_ok.as<unsigned char>(); hk.n_type_ids = lv.n_type_ids;
     hk.next = cs.next_carry.as<Follow>(); hk.n_next = cs.counters.as<int>() + 6; hk.next_cap = ecap;
     hk.force_publish = cs.force_publish.as<unsigned char>();
     size_t lsm = 0;
     const int lst = lru_stage_slots(f, &lsm);
-    k_lru_events<<<(f->lru_n + 3) / 4, 128, lsm, st>>>(lru_view(f), cs.lev.as<LruEv>(), cs.vals2.as<int>(), cs.off.as<int>(), now0, 1, hk,
-                                                      cs.evict.as<EvictRec>(), ecap, cs.counters.as<int>() + 4, cs.counters.as<int>() + 5, lst);
+    // (a fleet without overflow registrations runs the listener over the four inline positions only)
+    (lv.n_ovf > 0 ? k_lru_events<true> : k_lru_events<false>)<<<(f->lru_n + 3) / 4, 128, lsm, st>>>(
+        lru_view(f), cs.lev.as<LruEv>(), cs.vals2.as<int>(), cs.off.as<int>(), now0, 1, hk,
+                                                      cs.evict.as<EvictRec>(), ecap, cs.counters.as<int>() + 4, cs.counters.as<int>() + 5, lst,
+                                                      OvfHooks{R.ovf, R.n_ovf, cs.ovf_dead.as<unsigned char>()});
     f->launches++;
     CK(cudaGetLastError());
     CK(cudaEventRecord(evs[4], st));
@@ -470,6 +604,12 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
                                                       cs.add_inst.as<int>(), cs.used_t.as<long long>(), cs.counters.as<int>());
     f->launches += 3;
     CK(cudaGetLastError());
+    if (ovf_window) {
+      int marked = 0;
+      CK(cudaMemcpyAsync(&marked, cs.counters.as<int>() + 2, 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (marked) { rc = churn_relay_ovf(f, st); if (rc < 0) return rc; relaid = true; }
+    }
   } else {
     for (int i = 1; i <= 4; i++) CK(cudaEventRecord(evs[i], st));
   }
@@ -488,17 +628,17 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   // ---- reports ----
   int hdr[16];
   CK(cudaMemcpyAsync(hdr, cs.counters.p, 64, cudaMemcpyDeviceToHost, st));
-  int last_flag = 0, last_pos = 0;
+  int2 last_flag = make_int2(0, 0), last_pos = make_int2(0, 0);
   if (Q > 0) {
-    CK(cudaMemcpyAsync(&last_flag, cs.is_dec.as<int>() + (Q - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&last_pos, cs.dec_pos.as<int>() + (Q - 1), 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&last_flag, cs.is_dec.as<int2>() + (Q - 1), 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&last_pos, cs.dec_pos.as<int2>() + (Q - 1), 8, cudaMemcpyDeviceToHost, st));
   }
   std::vector<mmp_instance_row> rows((size_t)NI);
   CK(cudaMemcpyAsync(rows.data(), lv.inst_rows.p, (size_t)NI * sizeof(mmp_instance_row), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (hdr[5]) { g_err = "LRU slot capacity exceeded for some instance (raise slots_per_instance)"; return MMP_E_NOMEM; }
-  if (hdr[2]) { g_err = "a model reached more registered copies + failures than the device edge list holds (4)"; return MMP_E_STATE; }
-  const int32_t n_dec = Q > 0 ? last_pos + last_flag : 0, n_evict = hdr[4], n_next = hdr[6];
+  if (hdr[2] && !relaid) { g_err = "internal: a window changed overflow registrations the step did not expect"; return MMP_E_STATE; }
+  const int32_t n_dec = Q > 0 ? last_pos.x + last_flag.x : 0, n_evict = hdr[4], n_next = hdr[6];
   if (n_evict > ecap || n_next > ecap) { g_err = "eviction report overflow"; return MMP_E_NOMEM; }
   for (int32_t i = 0; i < NI; i++) if (f->hs.inst[i].present) f->hs.inst[i].row = rows[i];
   if (rows_out) memcpy(rows_out, rows.data(), (size_t)NI * sizeof(mmp_instance_row));
@@ -562,6 +702,32 @@ int32_t mmp_churn_model(mmp_fleet *f, int32_t model, mmp_model_row *row, int32_t
   if (row) CK(cudaMemcpy(row, f->live.models.as<mmp_model_row>() + model, sizeof(mmp_model_row), cudaMemcpyDeviceToHost));
   if (instances4) CK(cudaMemcpy(instances4, f->live.edges.as<int32_t>() + (size_t)model * 4, 16, cudaMemcpyDeviceToHost));
   return MMP_OK;
+}
+
+int32_t mmp_churn_model_ids(mmp_fleet *f, int32_t model, mmp_model_row *row, int32_t *ids, int32_t cap) {
+  NEED(f);
+  if (model < 0 || model >= f->hs.n_models_used || !f->live.valid || cap < 0 || (cap > 0 && !ids)) { g_err = "bad model index or argument"; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  const LiveState &lv = f->live;
+  mmp_model_row r;
+  int4 e;
+  CK(cudaMemcpy(&r, lv.models.as<mmp_model_row>() + model, sizeof(r), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(&e, lv.edges.as<int4>() + model, sizeof(e), cudaMemcpyDeviceToHost));
+  if (row) *row = r;
+  const int32_t n = (int32_t)r.reserved, inl[4] = {e.x, e.y, e.z, e.w};
+  for (int32_t j = 0; j < std::min(n, 4) && j < cap; j++) ids[j] = inl[j];
+  if (n > 4 && cap > 4) {  // the model's slice of the overflow table: the entries from the first of its model on
+    std::vector<OvfEdge> ovf((size_t)lv.n_ovf);
+    if (lv.n_ovf) CK(cudaMemcpy(ovf.data(), lv.ovf.p, ovf.size() * sizeof(OvfEdge), cudaMemcpyDeviceToHost));
+    const size_t q0 = std::lower_bound(ovf.begin(), ovf.end(), model, [](const OvfEdge &a, int32_t m) { return a.model < m; }) - ovf.begin();
+    for (int32_t j = 4; j < n && j < cap; j++) {
+      const size_t q = q0 + (size_t)(j - 4);
+      ids[j] = q < ovf.size() && ovf[q].model == model ? ovf[q].inst : -1;
+    }
+  }
+  return n;
 }
 
 }  // extern "C"

@@ -32,6 +32,35 @@ struct LiveState {
   mmp::HostSnapshot tmpl;       // the last structural snapshot: everything that does not depend on the numeric columns
 };
 
+// A model's registrations in the order of its last upsert (loaded first, then failed): positions 0-3 are the inline edges and
+// their times, positions 4, 5, ... the model's slice of the overflow table, found by a lower_bound on its model column.  Only
+// models with more than four registrations search.
+struct RegTables { const int4 *edges; const long long *edge_ts; const OvfEdge *ovf; int n_ovf; };
+struct ModelRegs { int m, ovf0; int4 e; };
+__device__ __forceinline__ ModelRegs model_regs(const RegTables &R, int m, unsigned reserved) {
+  ModelRegs g{m, 0, R.edges[m]};
+  if (reserved > 4u) {
+    int lo = 0, hi = R.n_ovf;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (R.ovf[mid].model < m) lo = mid + 1; else hi = mid; }
+    g.ovf0 = lo;
+  }
+  return g;
+}
+// registration j of the model -> its instance (-1: none) and its load / failure time (0: unknown)
+__device__ __forceinline__ int reg_at(const RegTables &R, const ModelRegs &g, int j, long long &ts) {
+  if (j < 4) {
+    ts = R.edge_ts ? R.edge_ts[(size_t)g.m * 4 + j] : 0;
+    return j == 0 ? g.e.x : j == 1 ? g.e.y : j == 2 ? g.e.z : g.e.w;
+  }
+  const int q = g.ovf0 + j - 4;
+  if (q >= R.n_ovf || R.ovf[q].model != g.m) { ts = 0; return -1; }
+  ts = R.ovf[q].ts;
+  return R.ovf[q].inst;
+}
+static RegTables reg_tables(const LiveState &lv) {
+  return RegTables{lv.edges.as<int4>(), lv.have_times ? lv.edge_ts.as<long long>() : nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
+}
+
 // state of the closed loop (churn_kernels.cuh), owned by the fleet
 struct ChurnState {
   bool on = false;
@@ -40,7 +69,13 @@ struct ChurnState {
   DevBuf carry, next_carry, counters;
   DevBuf ev, is_dec, dec_pos, dec_in, dec_out, dec_meta, dec_target, extra, status, lev, keys, vals, keys2, vals2, cub_tmp, off, evict, fkeys,
       fvals, rows_changed;
+  DevBuf ovf_dead, ovf_next, ovf_count;  // the registry phase's re-lay of LiveState::ovf (churn_kernels.cuh)
   int32_t n_carry = 0;
+  // what the step's host side knows of the registry without reading it back: the loop only removes loaded copies or loads the
+  // first one of a model without any, so the largest copy count does not grow past max(it, 1) and the failed loads of a model
+  // stay as they are.  Taken from the host tables when they were last uploaded (regs_from_host).
+  bool regs_from_host = true, deep_failed = false;
+  int32_t max_copies = 1;
   // last step's phase timings (ms, between these events on the step's stream; created by mmp_churn_init)
   Event phase_ev[7];
   float t_classify = 0, t_place = 0, t_route = 0, t_apply = 0, t_registry = 0, t_commit = 0, t_total = 0;

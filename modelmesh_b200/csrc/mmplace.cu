@@ -2041,6 +2041,7 @@ static int32_t commit_locked(mmp_fleet *f) {
   if (lv.models.cap != models_cap0) CK(cudaMemsetAsync(lv.models.p, 0, lv.models.cap, st));
   if (lv.edges.cap != edges_cap0) CK(cudaMemsetAsync(lv.edges.p, 0xff, lv.edges.cap, st));
   if (!f->device_ahead) {
+    f->churn.regs_from_host = true;
     if (structural || f->hs.all_models_dirty) {
       if (nm) {
         CK(cudaMemcpyAsync(lv.models.p, f->hs.models.data(), (size_t)nm * sizeof(mmp_model_row), cudaMemcpyHostToDevice, st));

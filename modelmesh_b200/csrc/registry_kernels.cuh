@@ -26,32 +26,6 @@ __global__ void k_type_stats(const StatsAcc *__restrict__ acc, const long long *
   out[t] = s;
 }
 
-// A model's registrations in the order of its last upsert (loaded first, then failed): positions 0-3 are the inline edges and
-// their times, positions 4, 5, ... the model's slice of the overflow table, found by a lower_bound on its model column.  Only
-// models with more than four registrations search.
-struct RegTables { const int4 *edges; const long long *edge_ts; const OvfEdge *ovf; int n_ovf; };
-struct ModelRegs { int m, ovf0; int4 e; };
-__device__ __forceinline__ ModelRegs model_regs(const RegTables &R, int m, unsigned reserved) {
-  ModelRegs g{m, 0, R.edges[m]};
-  if (reserved > 4u) {
-    int lo = 0, hi = R.n_ovf;
-    while (lo < hi) { const int mid = (lo + hi) >> 1; if (R.ovf[mid].model < m) lo = mid + 1; else hi = mid; }
-    g.ovf0 = lo;
-  }
-  return g;
-}
-// registration j of the model -> its instance (-1: none) and its load / failure time (0: unknown)
-__device__ __forceinline__ int reg_at(const RegTables &R, const ModelRegs &g, int j, long long &ts) {
-  if (j < 4) {
-    ts = R.edge_ts ? R.edge_ts[(size_t)g.m * 4 + j] : 0;
-    return j == 0 ? g.e.x : j == 1 ? g.e.y : j == 2 ? g.e.z : g.e.w;
-  }
-  const int q = g.ovf0 + j - 4;
-  if (q >= R.n_ovf || R.ovf[q].model != g.m) { ts = 0; return -1; }
-  ts = R.ovf[q].ts;
-  return R.ovf[q].inst;
-}
-
 struct ScaleTables {
   const mmp_model_row *models; RegTables R; const long long *model_lul;
   const int32_t *rank_of; const RankRow *rows; const int32_t *part_of_rank; const uint4 *inst_tie;
@@ -235,10 +209,6 @@ __global__ void k_registry_prune(RegTables R, const mmp_model_row *__restrict__ 
 __global__ void k_extract_rpm(const RankRow *__restrict__ rows, int n, int *__restrict__ out) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r < n) out[r] = rows[r].rpm;
-}
-
-static RegTables reg_tables(const LiveState &lv) {
-  return RegTables{lv.edges.as<int4>(), lv.have_times ? lv.edge_ts.as<long long>() : nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
 }
 
 // One prune pass (k_registry_prune) over the live registry.  It keeps every record -- walk_ovf = 0: one (model, mask) per

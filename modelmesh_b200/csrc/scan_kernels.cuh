@@ -325,14 +325,40 @@ struct ChurnHooks {
   int *status;                     // [n_decisions] CH_*
   const int *dec_target;           // [n_decisions] instance the decision resolved to
   const int *dec_of_model;         // [n_models] this epoch's decision for the model, -1
-  const int4 *edges;               // [n_models] registered instances (first copy_count = loaded)
+  const int4 *edges;               // [n_models] registrations 0-3 (first copy_count = loaded)
   const mmp_model_row *models;
-  unsigned *rm_mask;               // [n_models] bit j: edge j is deregistered at the end of the epoch
+  unsigned *rm_mask;               // [n_models] bit j < 4: registration j is deregistered at the end of the epoch; RM_OVF: a later one is
   const unsigned char *type_ok;    // [n_type_ids] the type set is < 95 % full (MM:2918-2920)
   int n_type_ids;
   Follow *next; int *n_next; int next_cap;
   unsigned char *force_publish;    // [n_instances]
 };
+// the hooks' overflow registrations (LiveState::ovf), a launch argument of their own after the others: as fields of ChurnHooks
+// they move every later argument, and the compiler gives the kernel another register allocation
+struct OvfHooks {
+  const OvfEdge *ovf; int n_ovf;
+  unsigned char *dead;             // [n_ovf] the overflow registration is deregistered at the end of the epoch
+};
+#define RM_OVF (1u << 4)
+
+// deregisterModel / the listener's deregistration (MM:2875-2931): mark the model's loaded copy on `inst` at whatever position it
+// holds.  Copies of one model on different instances are marked by different warps of the same launch: bits by atomicOr, and
+// each overflow position has a flag byte of its own.  OVF = false (no overflow table) compiles the four inline positions only.
+template <bool OVF>
+__device__ __forceinline__ void churn_deregister(const ChurnHooks &hk, const OvfHooks &ov, int m, int inst) {
+  const int4 ed = hk.edges[m];
+  const int cc = hk.models[m].copy_count;
+  const int es[4] = {ed.x, ed.y, ed.z, ed.w};
+  for (int j = 0; j < 4 && j < cc; j++) if (es[j] == inst) atomicOr(&hk.rm_mask[m], 1u << j);
+  if (OVF && cc > 4) {
+    const RegTables R{hk.edges, nullptr, ov.ovf, ov.n_ovf};
+    const ModelRegs g = model_regs(R, m, (unsigned)cc);
+    for (int j = 4; j < cc; j++) {
+      long long ts;
+      if (reg_at(R, g, j, ts) == inst) { ov.dead[g.ovf0 + j - 4] = 1; atomicOr(&hk.rm_mask[m], RM_OVF); }
+    }
+  }
+}
 
 __device__ __forceinline__ bool key_less(long long t1, long long s1, long long t2, long long s2) { return t1 < t2 || (t1 == t2 && s1 < s2); }
 
@@ -374,8 +400,11 @@ __device__ int lru_find(const LruView &v, int inst, int lane, int model, int *fr
 // placeholder insert (INSERTION_WEIGHT = 1, MM:5011, 5061), immediate-eviction fall-through MM:5145-5148, early reject
 // MM:5185-5190, registration, inflate to the predicted size + grow-then-check MM:2094-2106.  With hooks.enabled every eviction
 // also runs the eviction listener's bookkeeping (onEviction MM:2875-2931): deregistration mark, the reload-elsewhere rule (a12).
+// OVF: the hooks' registry has an overflow table (a model may hold more than four registrations).
+template <bool OVF>
 __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int *__restrict__ ev_order, const int *__restrict__ inst_off,
-                             long long now_param, int use_ev_time, ChurnHooks hk, EvictRec *out, int out_cap, int *out_n, int *err, int stage_slots) {
+                             long long now_param, int use_ev_time, ChurnHooks hk, EvictRec *out, int out_cap, int *out_n, int *err, int stage_slots,
+                             OvfHooks ov) {
   const int lane = threadIdx.x & 31;
   const int inst = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (inst >= v.n) return;
@@ -419,12 +448,7 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
         if (hk.enabled) {
           const bool in_registry = lt >= 0;
           const bool attempt = in_registry && (now - lt) > 2 * hk.load_timeout;  // MM:2901
-          if (in_registry) {
-            const int4 ed = hk.edges[m];
-            const int cc = hk.models[m].copy_count;
-            const int es[4] = {ed.x, ed.y, ed.z, ed.w};
-            for (int j = 0; j < 4 && j < cc; j++) if (es[j] == inst) atomicOr(&hk.rm_mask[m], 1u << j);
-          }
+          if (in_registry) churn_deregister<OVF>(hk, ov, m, inst);
           const int k2 = hk.dec_of_model[m];
           if (k2 >= 0 && hk.dec_target[k2] == inst && hk.status[k2] == CH_ACCEPTED) hk.status[k2] = CH_EVICTED_LATER;
           const int ty = hk.models[m].type_id;
@@ -533,12 +557,7 @@ __global__ void k_lru_events(LruView v, const LruEv *__restrict__ ev, const int 
         sv.model[base + slot] = -1;
         if (hk.enabled) {
           hk.force_publish[inst] = 1;
-          if (lt >= 0) {  // deregisterModel
-            const int4 ed = hk.edges[e.model];
-            const int cc = hk.models[e.model].copy_count;
-            const int es[4] = {ed.x, ed.y, ed.z, ed.w};
-            for (int j = 0; j < 4 && j < cc; j++) if (es[j] == inst) atomicOr(&hk.rm_mask[e.model], 1u << j);
-          }
+          if (lt >= 0) churn_deregister<OVF>(hk, ov, e.model, inst);  // deregisterModel
         }
       }
       __syncwarp();
@@ -574,7 +593,8 @@ static int lru_stage_slots(mmp_fleet *f, size_t *smem) {
   *smem = 0;
   if (f->lru_slots <= 0 || tot > (size_t)200 * 1024) return 0;
   if (!attr_set[f->device & 63].load()) {
-    if (cudaFuncSetAttribute(k_lru_events, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
+    if (cudaFuncSetAttribute(k_lru_events<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess ||
+        cudaFuncSetAttribute(k_lru_events<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
     attr_set[f->device & 63] = true;
   }
   *smem = tot;
@@ -681,8 +701,8 @@ static int32_t lru_apply_impl(mmp_fleet *f, const mmp_lru_event *ev, int32_t n, 
   size_t lsm = 0;
   const int lst = lru_stage_slots(f, &lsm);
   CK(cudaEventRecord(c->e0, s));
-  k_lru_events<<<grid, warps_per_block * 32, lsm, s>>>(lru_view(f), c->d_in.as<LruEv>(), c->d_extra.as<int>(), c->d_fresh.as<int>(), now_ms, 0, hk,
-                                                      c->d_out.as<EvictRec>(), cap, c->d_trace.as<int>(), c->d_trace.as<int>() + 1, lst);
+  k_lru_events<false><<<grid, warps_per_block * 32, lsm, s>>>(lru_view(f), c->d_in.as<LruEv>(), c->d_extra.as<int>(), c->d_fresh.as<int>(), now_ms, 0, hk,
+                                                      c->d_out.as<EvictRec>(), cap, c->d_trace.as<int>(), c->d_trace.as<int>() + 1, lst, OvfHooks{});
   CK(cudaEventRecord(c->e1, s));
   f->launches++;
   CK(cudaGetLastError());

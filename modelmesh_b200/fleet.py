@@ -290,6 +290,16 @@ class Fleet:
         self._ck(self.lib.mmp_churn_model(self.h, model, _ptr(row), _ptr(inst)))
         return row[0], inst
 
+    def churn_model_ids(self, model: int):
+        """mmp_churn_model_ids: (row, every registration's instance index: the first copy_count loaded, then the failed loads)"""
+        row = np.zeros(1, dtype=MODEL_ROW)
+        ids = np.zeros(16, dtype=np.int32)
+        n = self._ck(self.lib.mmp_churn_model_ids(self.h, model, _ptr(row), _ptr(ids), len(ids)))
+        if n > len(ids):
+            ids = np.zeros(n, dtype=np.int32)
+            n = self._ck(self.lib.mmp_churn_model_ids(self.h, model, _ptr(row), _ptr(ids), len(ids)))
+        return row[0], ids[:n].copy()
+
     def model_times(self, m: int, edge_ts: np.ndarray, last_unload_time: int = 0):
         ts = np.ascontiguousarray(edge_ts, dtype=np.int64)
         self._ck(self.lib.mmp_model_times(self.h, m, _ptr(ts), len(ts), int(last_unload_time)))

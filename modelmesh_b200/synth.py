@@ -567,3 +567,74 @@ def make_churn(n_models: int, n_instances: int, seed: int, fill: float = 0.97, w
     unloaded = np.nonzero(n_loaded == 0)[0]
     return ChurnWorkload(fl, rows["capacity"].astype(np.int64).copy(), seed_instance, seed_model, seed_lu, seed_w, seed_lt, hot_order,
                          unloaded, load_timeout)
+
+
+def make_churn_overflow(w: ChurnWorkload, frac: float, seed: int, regs=(5, 12)) -> ChurnWorkload:
+    """`w` with about `frac` of its models holding more registrations than the four inline ones.  A chosen model with a copy
+    gets further copies on other instances where they fit the caches (seeded resident, registered after its first copies) and
+    failed loads for the rest, regs[0]..regs[1] registrations in all; a chosen model without a copy gets failed loads only:
+    every other one exactly four, so that its first load makes a fifth registration, the rest regs[0]..regs[1].  Its own
+    random stream: `w`'s fleet, seeds and event trace stay as they are for the models not chosen."""
+    rng = SplitMix(seed ^ 0x0F5C4)
+    fl = w.fleet
+    nm, ni = fl.n_models, fl.n_instances
+    chosen = np.nonzero(rng.uniform(nm) < frac)[0]
+    target = rng.randint(len(chosen), regs[0], regs[1] + 1)
+    start = rng.randint(len(chosen), 0, ni)
+    rows = fl.inst_rows.copy()
+    used = rows["used"].astype(np.int64)
+    lu_of = fl.model_last_used
+    new_lists, s_inst, s_model, s_lu = {}, [], [], []
+    for k, m in enumerate(chosen):
+        m = int(m)
+        a, b = int(fl.edge_off[m]), int(fl.edge_off[m + 1])
+        loaded = [int(x) for x in fl.edge_inst[a:a + int(fl.n_loaded[m])]]
+        failed = [int(x) for x in fl.edge_inst[a + int(fl.n_loaded[m]):b]]
+        want = int(target[k]) if loaded or k % 2 else 4
+        size = int(fl.model_size[m])
+        taken = set(loaded) | set(failed)
+        for j in range(ni):
+            if len(loaded) + len(failed) >= want:
+                break
+            i = (int(start[k]) + j) % ni
+            if i in taken:
+                continue
+            taken.add(i)
+            if loaded and used[i] + size <= w.capacity[i]:  # another resident copy
+                used[i] += size
+                loaded.append(i)
+                s_inst.append(i); s_model.append(m); s_lu.append(int(lu_of[m]) - 11 * len(loaded))
+            else:
+                failed.append(i)
+        new_lists[m] = (loaded, failed)
+    n_loaded = fl.n_loaded.copy()
+    n_failed = fl.n_failed.copy()
+    for m, (ld, fd) in new_lists.items():
+        n_loaded[m], n_failed[m] = len(ld), len(fd)
+    cnt = (n_loaded + n_failed).astype(np.int64)
+    edge_off = np.zeros(nm + 1, dtype=np.int64)
+    np.cumsum(cnt, out=edge_off[1:])
+    edge_inst = np.full(int(edge_off[-1]), -1, dtype=np.int32)
+    old_cnt = np.diff(fl.edge_off)
+    keep = np.ones(nm, dtype=bool)
+    keep[chosen] = False
+    owner = np.repeat(np.arange(nm), old_cnt)
+    sel = keep[owner]
+    pos = np.arange(len(fl.edge_inst)) - fl.edge_off[owner]
+    edge_inst[(edge_off[owner] + pos)[sel]] = fl.edge_inst[sel]
+    for m, (ld, fd) in new_lists.items():
+        edge_inst[edge_off[m]:edge_off[m + 1]] = ld + fd
+    s_inst_a, s_model_a = np.asarray(s_inst, dtype=np.int32), np.asarray(s_model, dtype=np.int32)
+    s_lu_a = np.asarray(s_lu, dtype=np.int64)
+    rows["used"] = used
+    rows["count"] += np.bincount(s_inst_a, minlength=ni).astype(rows["count"].dtype)
+    oldest = rows["lru_time"].astype(np.int64)
+    np.minimum.at(oldest, s_inst_a, s_lu_a)
+    rows["lru_time"] = oldest
+    fl2 = SynthFleet(fl.name, fl.now_ms, fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, rows, fl.inst_ids,
+                     fl.inst_locs, fl.inst_zones, fl.inst_labels, fl.type_config, fl.type_names, fl.model_type, fl.model_last_used,
+                     fl.model_size, fl.model_rpm, edge_off, edge_inst, n_loaded, n_failed, fl.replaced_replicasets)
+    return ChurnWorkload(fl2, w.capacity, np.concatenate([w.seed_instance, s_inst_a]), np.concatenate([w.seed_model, s_model_a]),
+                         np.concatenate([w.seed_last_used, s_lu_a]), np.concatenate([w.seed_weight, fl.model_size[s_model_a].astype(np.int32)]),
+                         np.concatenate([w.seed_load_ts, np.full(len(s_inst_a), fl.now_ms - 3 * 3_600_000, dtype=np.int64)]),
+                         w.loaded_models, w.unloaded_models, w.load_timeout_ms, w.window_ms)
