@@ -17,6 +17,8 @@
 // Kernels (DESIGN.md §5, §7):
 //   k_place_direct<4, 5>     the scoring kernel (default): one decision per lane, the row rebuilt from the model's excl_ranks,
 //                            longer walks through the word lists; optional slot-sorted batches (k_slot_keys + cub radix sort)
+//   k_slot_summary, k_place_split, k_place_walk<4, 5>, k_place_ovf   large batches in two passes (launch_split): per-slot
+//                            summaries answer the decisions clear of their slot's reach, k_place_direct's body walks the rest
 //   k_place_lanes            round 1's streaming kernel (whole rows through TMA landing stages): MMP_KERNEL=lanes and the
 //                            collective instance-shard path
 //   k_place_small            tiny batches as a stream launch / replayed CUDA graph;  k_place_server: the resident B = 1 server
@@ -341,6 +343,7 @@ static constexpr int SHARD_FRONT_WORDS = 16;  // instance-sharded fleets: row wo
 static constexpr int LANE_WIN = MMP_LANE_WIN;  // row words copied out of the landing stage per decision: the first LANE_WIN words of the
                                                // stored row (384 ranks); later steps go through the compressed word list and read the row from L2
 static constexpr int LANE_STRIDE = LANE_WIN + 1;  // words per lane in the window buffer (odd: bank-conflict free)
+static constexpr int SPLIT_MIN_BATCH = 1 << 18;  // k_place_direct batches from this size take the two-pass path (launch_split)
 static constexpr int LANE_BUDGET = 192;  // walk steps a lane may spend before handing its decision to the whole warp
 static constexpr int LANE_SLOTS = 64;    // type-constraint mask slots whose window words are kept in shared memory
 static constexpr int LANE_WARPS = 12;    // warps per block of k_place_lanes
@@ -640,12 +643,11 @@ __global__ void k_slot_keys(const SnapshotView s, const mmp_decision_in *__restr
   keys[i] = (uint16_t)k;
   idx[i] = i;
 }
-template <int WARPS, int MINB>
-__global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
-                                                                  const FreshRow *__restrict__ fresh, int n_fresh,
-                                                                  const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
-                                                                  int64_t now, uint64_t seed, uint64_t id_base, int budget,
-                                                                  const int32_t *__restrict__ perm) {
+template <int WARPS>
+__device__ __forceinline__ void place_direct(const SnapshotView &s, const mmp_decision_in *__restrict__ in, int n,
+                                             const FreshRow *__restrict__ fresh, int n_fresh, const int32_t *__restrict__ extra,
+                                             mmp_decision_out *__restrict__ out, int64_t now, uint64_t seed, uint64_t id_base, int budget,
+                                             const int32_t *__restrict__ perm) {
   __shared__ uint32_t win_s[WARPS][32 * LANE_STRIDE];
   __shared__ uint32_t chunk_s[WARPS][32 * MMP_CHUNK_WORDS];
   __shared__ DecisionCtx ctx_w[WARPS];
@@ -708,6 +710,118 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
     __syncwarp();
   }
   if (valid) out[i] = mmp_decision_out{o.target, o.n_candidates};
+}
+template <int WARPS, int MINB>
+__global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
+                                                                  const FreshRow *__restrict__ fresh, int n_fresh,
+                                                                  const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
+                                                                  int64_t now, uint64_t seed, uint64_t id_base, int budget,
+                                                                  const int32_t *__restrict__ perm) {
+  place_direct<WARPS>(s, in, n, fresh, n_fresh, extra, out, now, seed, id_base, budget, perm);
+}
+// k_place_direct over the first *n_live positions of perm, a worklist whose length is on the device (the grid is sized
+// for n: blocks past the length leave at once)
+template <int WARPS, int MINB>
+__global__ void __launch_bounds__(WARPS * 32, MINB) k_place_walk(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
+                                                                const FreshRow *__restrict__ fresh, int n_fresh,
+                                                                const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
+                                                                int64_t now, uint64_t seed, uint64_t id_base, int budget,
+                                                                const int32_t *__restrict__ perm, const int32_t *__restrict__ n_live) {
+  n = min(n, __ldg(n_live));
+  if ((int)(blockIdx.x * WARPS * 32) >= n) return;
+  place_direct<WARPS>(s, in, n, fresh, n_fresh, extra, out, now, seed, id_base, budget, perm);
+}
+
+// ---- the two-pass path of a large batch (launch_place, DESIGN.md §5.2) ----
+// one lane per (type slot, c_self): the slot summaries of this call's view (slot_summary); also zeroes the worklist counters
+__global__ void __launch_bounds__(128) k_slot_summary(const SnapshotView s, int64_t now, SlotSummary *__restrict__ sums,
+                                                      int32_t *__restrict__ members, int32_t *__restrict__ counts) {
+  __shared__ uint32_t win_s[4][32 * LANE_STRIDE];
+  __shared__ uint32_t chunk_s[4][32 * MMP_CHUNK_WORDS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int t = blockIdx.x * 128 + threadIdx.x, sl = t >> 1, cs = t & 1;
+  if (t < 2) counts[t] = 0;
+  const bool active = sl < s.n_slots;
+  uint32_t *w = win_s[warp] + lane * LANE_STRIDE;
+#pragma unroll
+  for (int j = 0; j < LANE_WIN; j++) w[j] = 0u;
+  __syncwarp();
+  const int slot = active ? sl : 0;
+  const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
+  const LaneTables T = lane_tables_global(s, slot);
+  slot_summary(s, T, slot, active, cs, w, win_words, now, WarpVote(), chunk_s[warp] + lane * MMP_CHUNK_WORDS, sums[slot],
+               members + ((size_t)slot * 2 + cs) * SPLIT_CAP);
+}
+// appends v to list (length in *count) for the lanes where p holds: one atomic per warp
+__device__ __forceinline__ void warp_append(bool p, int32_t v, int32_t *list, int32_t *count) {
+  const uint32_t m = __ballot_sync(0xffffffffu, p);
+  if (!m) return;
+  const int lane = threadIdx.x & 31, leader = __ffs((int)m) - 1;
+  int base = 0;
+  if (lane == leader) base = atomicAdd(count, __popc(m));
+  base = __shfl_sync(0xffffffffu, base, leader);
+  if (p) list[base + __popc(m & ((1u << lane) - 1u))] = v;
+}
+// one thread per decision: answered from its slot's summary (split_answer), or put on a worklist -- a model with overflow
+// ids on ovf_list (k_place_ovf), everything else on walk_list (k_place_direct).  keys / key_idx (sparse snapshots): the
+// slot-order sort of the batch, the walked decisions' keys below everyone else's.
+__global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
+                                                     const FreshRow *__restrict__ fresh, int n_fresh, mmp_decision_out *__restrict__ out,
+                                                     int64_t now, uint64_t seed, uint64_t id_base, const SlotSummary *__restrict__ sums,
+                                                     const int32_t *__restrict__ members, int32_t *__restrict__ walk_list,
+                                                     int32_t *__restrict__ ovf_list, int32_t *__restrict__ counts, uint16_t *__restrict__ keys,
+                                                     int32_t *__restrict__ key_idx) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool valid = i < n;
+  mmp_decision_in d;
+  d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
+  if (valid) {
+    const int4 *dp = reinterpret_cast<const int4 *>(in + i);
+    int4 a, c;  // streamed once
+    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(dp));
+    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(c.x), "=r"(c.y), "=r"(c.z), "=r"(c.w) : "l"(dp + 1));
+    d.model = a.x; d.self = a.y; d.last_used = (int64_t)(((uint64_t)(uint32_t)a.w << 32) | (uint32_t)a.z);
+    d.flags = (uint32_t)c.x; d.fresh = c.y; d.extra_off = c.z; d.extra_n = c.w;
+  }
+  const int m = excl_row_id(s, d.model, d.flags);
+  RowRanks row;  // (read as k_place_direct reads it: its overflow mark routes the decision the same way)
+  row.r[0] = row.r[1] = row.r[2] = row.r[3] = -1;
+  if (valid && m != ZERO_ROW) row = load_ranks(s.excl_ranks + (size_t)m * 4);
+  CtxA a;
+  a.ok = 0; a.self_rank = -1; a.mr.type_id = 0;
+  if (valid) prepare_ctx_a(s, d, a);
+  mmp_decision_out r;
+  const bool fast = valid && split_answer(s, d, a, row, fresh, n_fresh, sums, members, now, seed, pick_id(d, id_base + (uint64_t)i), r);
+  if (fast) out[i] = r;
+  const bool ovf = valid && !fast && row.overflow();
+  const bool walk = valid && !fast && !ovf;
+  warp_append(walk, i, walk_list, counts);
+  warp_append(ovf, i, ovf_list, counts + 1);
+  if (keys && valid) {
+    uint32_t k = 0xffffu;
+    if (walk) k = a.ok ? (uint32_t)s.type_slot[a.mr.type_id < s.n_type_ids ? a.mr.type_id : 0] & 0x7fffu : 0xfffeu;
+    keys[i] = (uint16_t)k;
+    key_idx[i] = i;
+  }
+}
+// the decisions of ovf_list (length *count), one warp each, resolved as k_place_direct's warp redo resolves them
+__global__ void __launch_bounds__(128) k_place_ovf(const SnapshotView s, const mmp_decision_in *__restrict__ in, const int32_t *__restrict__ list,
+                                                   const int32_t *__restrict__ count, const FreshRow *__restrict__ fresh, int n_fresh,
+                                                   const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out, int64_t now,
+                                                   uint64_t seed, uint64_t id_base) {
+  __shared__ DecisionCtx ctx_w[4];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int n = __ldg(count);
+  for (int k = blockIdx.x * 4 + warp; k < n; k += gridDim.x * 4) {
+    const int i = list[k];
+    const mmp_decision_in d = in[i];
+    if (lane == 0) prepare_ctx(s, d, fresh, n_fresh, extra, ctx_w[warp]);
+    __syncwarp();
+    int32_t t, c;
+    decide_warp(s, ctx_w[warp], excl_row(s, excl_row_id(s, d.model, d.flags)), extra, now, seed, pick_id(d, id_base + (uint64_t)i), &t, &c);
+    if (lane == 0) out[i] = mmp_decision_out{t, c};
+    __syncwarp();
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1163,6 +1277,8 @@ struct PlaceCtx {
   // slot sort of a batch (k_slot_keys + cub radix sort -> perm): set 0 for single launches, 1 + pipe for the chunks of a pipelined call
   static constexpr int NSORT = 4;
   DevBuf d_skey[NSORT], d_skey2[NSORT], d_sidx[NSORT], d_sidx2[NSORT], d_stmp[NSORT];
+  // the two-pass path (same scratch sets): slot summaries, their shortlist members, the two worklists and their lengths
+  DevBuf d_sums[NSORT], d_members[NSORT], d_walk[NSORT], d_ovf[NSORT], d_counts[NSORT];
   DevBuf d_open_flag, d_open_idx, d_n_open, d_cub, d_blocks, d_gathered, d_rows, d_in_open, d_out_open;  // instance-shard combine
   std::vector<FreshRow> fresh_host;
   // pinned, device-mapped scratch for tiny batches: the kernel reads the decisions and writes the results straight
@@ -1243,6 +1359,8 @@ struct mmp_fleet {
                                 // resolves a large batch in type-slot order
   PlaceKernel kernel = PlaceKernel::direct;  // MMP_KERNEL, mmp_tune("direct"): which kernel resolves untraced unsharded batches
   int lane_budget = LANE_BUDGET;  // MMP_LANE_BUDGET: walk steps per lane before a decision is handed to the whole warp
+  int split = 2;                // mmp_tune("split"): 0 never | 1 always | 2 (default) from SPLIT_MIN_BATCH decisions on snapshots whose
+                                // candidate sets are not sparse: k_place_direct batches go through the two-pass path (launch_split)
   // LRU store (plug point 3)
   DevBuf lru_ts, lru_seq, lru_weight, lru_model, lru_cap, lru_wsize, lru_count, lru_seqctr, lru_loadts, lru_pin;
   int32_t lru_n = 0, lru_slots = 0;
@@ -1369,6 +1487,72 @@ static cudaError_t launch_place_lanes(mmp_fleet *f, const PlaceArgs &a, cudaStre
   return cudaGetLastError();
 }
 
+// k_place_direct's slot order (sparse snapshots, MMP_SORT_SLOTS): keys in ctx scratch set a.sort_slot, then a 16-bit radix
+// sort of the positions by key (a few tens of microseconds per million decisions)
+static bool sorts_slots(const mmp_fleet *f) { return f->sort_slots == 1 || (f->sort_slots == 2 && f->snaps[f->cur].sparse_slots); }
+static int sort_set(const PlaceArgs &a) { return a.sort_slot >= 0 && a.sort_slot < PlaceCtx::NSORT ? a.sort_slot : 0; }
+static cudaError_t slot_key_buffers(const PlaceArgs &a) {
+  PlaceCtx *c = a.ctx;
+  const int ss = sort_set(a);
+  cudaError_t e;
+  if ((e = c->d_skey[ss].ensure((size_t)a.n * 2)) != cudaSuccess || (e = c->d_skey2[ss].ensure((size_t)a.n * 2)) != cudaSuccess ||
+      (e = c->d_sidx[ss].ensure((size_t)a.n * 4)) != cudaSuccess || (e = c->d_sidx2[ss].ensure((size_t)a.n * 4)) != cudaSuccess) return e;
+  return cudaSuccess;
+}
+static cudaError_t slot_keys(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st) {
+  cudaError_t e;
+  if ((e = slot_key_buffers(a)) != cudaSuccess) return e;
+  PlaceCtx *c = a.ctx;
+  const int ss = sort_set(a);
+  k_slot_keys<<<(a.n + 255) / 256, 256, 0, st>>>(a.s, a.in, a.n, c->d_skey[ss].as<uint16_t>(), c->d_sidx[ss].as<int32_t>());
+  f->launches++;
+  return cudaSuccess;
+}
+static cudaError_t sort_slot_keys(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st, const int32_t **perm) {
+  PlaceCtx *c = a.ctx;
+  const int ss = sort_set(a);
+  size_t tmp = 0;
+  cudaError_t e;
+  if ((e = cub::DeviceRadixSort::SortPairs(nullptr, tmp, c->d_skey[ss].as<uint16_t>(), c->d_skey2[ss].as<uint16_t>(), c->d_sidx[ss].as<int32_t>(), c->d_sidx2[ss].as<int32_t>(), a.n, 0, 16, st)) != cudaSuccess) return e;
+  if ((e = c->d_stmp[ss].ensure(tmp + 16)) != cudaSuccess) return e;
+  if ((e = cub::DeviceRadixSort::SortPairs(c->d_stmp[ss].p, tmp, c->d_skey[ss].as<uint16_t>(), c->d_skey2[ss].as<uint16_t>(), c->d_sidx[ss].as<int32_t>(), c->d_sidx2[ss].as<int32_t>(), a.n, 0, 16, st)) != cudaSuccess) return e;
+  *perm = c->d_sidx2[ss].as<int32_t>();
+  f->launches++;
+  return cudaSuccess;
+}
+
+// The two-pass path of a k_place_direct batch (DESIGN.md §5.2): the slot summaries of the call's view (k_slot_summary), one
+// streaming pass that answers every decision lying clear of its slot's reach and lists the others (k_place_split), then
+// k_place_direct over the walk list -- in slot order on sparse snapshots -- and k_place_ovf over the models with overflow
+// ids.  The lists' lengths stay on the device: both launches are sized for the whole batch and stop at the length.
+static cudaError_t launch_split(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st) {
+  PlaceCtx *c = a.ctx;
+  const int ss = sort_set(a);
+  const int n_slots = std::max(a.s.n_slots, 1);
+  const bool sorted = sorts_slots(f);
+  cudaError_t e;
+  if ((e = c->d_sums[ss].ensure((size_t)n_slots * sizeof(SlotSummary))) != cudaSuccess ||
+      (e = c->d_members[ss].ensure((size_t)n_slots * 2 * SPLIT_CAP * 4)) != cudaSuccess ||
+      (e = c->d_walk[ss].ensure((size_t)a.n * 4)) != cudaSuccess || (e = c->d_ovf[ss].ensure((size_t)a.n * 4)) != cudaSuccess ||
+      (e = c->d_counts[ss].ensure(16)) != cudaSuccess) return e;
+  if (sorted && (e = slot_key_buffers(a)) != cudaSuccess) return e;
+  int32_t *counts = c->d_counts[ss].as<int32_t>();
+  k_slot_summary<<<(2 * n_slots + 127) / 128, 128, 0, st>>>(a.s, a.now, c->d_sums[ss].as<SlotSummary>(), c->d_members[ss].as<int32_t>(), counts);
+  k_place_split<<<(a.n + 255) / 256, 256, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.out, a.now, a.seed, a.id_base,
+                                                   c->d_sums[ss].as<SlotSummary>(), c->d_members[ss].as<int32_t>(), c->d_walk[ss].as<int32_t>(),
+                                                   c->d_ovf[ss].as<int32_t>(), counts, sorted ? c->d_skey[ss].as<uint16_t>() : nullptr,
+                                                   sorted ? c->d_sidx[ss].as<int32_t>() : nullptr);
+  f->launches += 2;
+  const int32_t *perm = c->d_walk[ss].as<int32_t>();
+  if (sorted && (e = sort_slot_keys(f, a, st, &perm)) != cudaSuccess) return e;
+  k_place_walk<4, 5><<<(a.n + 127) / 128, 128, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base,
+                                                       f->lane_budget, perm, counts);
+  k_place_ovf<<<std::max(1, std::min((a.n + 3) / 4, f->sm_count * 4)), 128, 0, st>>>(a.s, a.in, c->d_ovf[ss].as<int32_t>(), counts + 1, a.fresh, a.n_fresh,
+                                                                                   a.extra, a.out, a.now, a.seed, a.id_base);
+  f->launches += 2;
+  return cudaGetLastError();
+}
+
 static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st) {
   const int rw = a.s.row_words;
   int ns = 0;
@@ -1381,20 +1565,12 @@ static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
   if (a.emit_keys || a.orig_id) return lanes_geometry(a.s.excl_stride, ns) ? launch_place_lanes(f, a, st, ns) : cudaErrorInvalidValue;
   // the direct kernel: rows rebuilt from the snapshot's excl_ranks (whole-row fleets), no landing stages
   if (f->kernel == PlaceKernel::direct && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words && a.s.excl_ranks) {
+    if (a.ctx && a.s.n_slots > 0 && (f->split == 1 || (f->split == 2 && a.n >= SPLIT_MIN_BATCH && !f->snaps[f->cur].sparse_slots)))
+      return launch_split(f, a, st);
     const int32_t *perm = nullptr;  // k_place_direct: position j of the launch resolves decision perm[j]
-    if (a.ctx && a.n >= 8192 && (f->sort_slots == 1 || (f->sort_slots == 2 && f->snaps[f->cur].sparse_slots))) {
-      PlaceCtx *c = a.ctx;  // slot order: key pass + 16-bit radix sort of the indices (a few tens of microseconds per million decisions)
-      const int ss = a.sort_slot >= 0 && a.sort_slot < PlaceCtx::NSORT ? a.sort_slot : 0;
+    if (a.ctx && a.n >= 8192 && sorts_slots(f)) {
       cudaError_t e;
-      if ((e = c->d_skey[ss].ensure((size_t)a.n * 2)) != cudaSuccess || (e = c->d_skey2[ss].ensure((size_t)a.n * 2)) != cudaSuccess ||
-          (e = c->d_sidx[ss].ensure((size_t)a.n * 4)) != cudaSuccess || (e = c->d_sidx2[ss].ensure((size_t)a.n * 4)) != cudaSuccess) return e;
-      k_slot_keys<<<(a.n + 255) / 256, 256, 0, st>>>(a.s, a.in, a.n, c->d_skey[ss].as<uint16_t>(), c->d_sidx[ss].as<int32_t>());
-      size_t tmp = 0;
-      if ((e = cub::DeviceRadixSort::SortPairs(nullptr, tmp, c->d_skey[ss].as<uint16_t>(), c->d_skey2[ss].as<uint16_t>(), c->d_sidx[ss].as<int32_t>(), c->d_sidx2[ss].as<int32_t>(), a.n, 0, 16, st)) != cudaSuccess) return e;
-      if ((e = c->d_stmp[ss].ensure(tmp + 16)) != cudaSuccess) return e;
-      if ((e = cub::DeviceRadixSort::SortPairs(c->d_stmp[ss].p, tmp, c->d_skey[ss].as<uint16_t>(), c->d_skey2[ss].as<uint16_t>(), c->d_sidx[ss].as<int32_t>(), c->d_sidx2[ss].as<int32_t>(), a.n, 0, 16, st)) != cudaSuccess) return e;
-      perm = c->d_sidx2[ss].as<int32_t>();
-      f->launches += 2;
+      if ((e = slot_keys(f, a, st)) != cudaSuccess || (e = sort_slot_keys(f, a, st, &perm)) != cudaSuccess) return e;
     }
     k_place_direct<4, 5><<<(a.n + 127) / 128, 128, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base,
                                                            f->lane_budget, perm);
@@ -2161,6 +2337,7 @@ int32_t mmp_tune(mmp_fleet *f, const char *key, int64_t value) {
   else if (!strcmp(key, "direct") && (value == 0 || value == 1)) f->kernel = value ? PlaceKernel::direct : PlaceKernel::lanes;
   else if (!strcmp(key, "sort_slots") && value >= 0 && value <= 2) f->sort_slots = (int)value;
   else if (!strcmp(key, "lane_budget") && value >= 1 && value <= 4096) f->lane_budget = (int)value;
+  else if (!strcmp(key, "split") && value >= 0 && value <= 2) f->split = (int)value;
   else if (!strcmp(key, "commit_host_only") && (value == 0 || value == 1)) f->commit_host_only = (int)value;
   else { g_err = "unknown key or value out of range"; return MMP_E_ARG; }
   return MMP_OK;

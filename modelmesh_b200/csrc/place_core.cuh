@@ -454,6 +454,9 @@ struct DecideOut {
   int32_t target, n_candidates;
   int32_t best, n_remaining, pick_index, flags, cut_rank, best_rank;
   int32_t first_rank;  // rank of the first filtered entry (before preferred handling): the min-loc key of a shard
+  // decide_stream: every rank its answer depends on lies below reach (NONE_RANK: any rank may), so an exclusion or a self
+  // at or beyond it leaves the answer as it is (k_slot_summary)
+  int32_t reach;
 };
 
 // ---- instance-sharded combine (SURVEY.md §8e).  Every shard resolves the decision over its own rank range as if its
@@ -495,6 +498,43 @@ struct RpmFilter {
                           (ago < 720000 && rpm > jmuli(min_load, 3)) || (ago < 86400000 && rpm > jmuli(min_load, 4)));
   }
 };
+
+// The end of a simple-case decision once its shortlist is known (MM:4957-4986): the rpm filter over best, the other
+// members (N2: they all read the caller's record, other_rpm) and self (self_rpm), then the hash-indexed pick.  n_in =
+// members of the shortlist besides best, self included when self_in_sl.  kind: the pick is best, self, or member kth of
+// the shortlist in rank order (self left out when !keep_self).
+enum { PICK_BEST = 0, PICK_SELF = 1, PICK_MEMBER = 2 };
+struct PickOut { int32_t remaining; uint32_t index, kth; bool keep_best, keep_others, keep_self; int kind; };
+MMP_HD PickOut pick_survivor(int32_t n_in, bool self_in_sl, int32_t best_rpm, int32_t other_rpm, int32_t self_rpm, int64_t last_used,
+                             int64_t now, uint64_t seed, uint64_t decision_id) {
+  PickOut p;
+  p.keep_best = p.keep_others = p.keep_self = true; p.index = 0; p.kind = PICK_BEST;
+  const int32_t n_others = n_in - (self_in_sl ? 1 : 0);
+  const int32_t ccount = 1 + n_in;
+  p.remaining = ccount;
+  if (ccount > 1) {
+    const int64_t ago = age_of(last_used, now);
+    if (ago < 432000000LL) {  // FIVE_DAYS_MS
+      int32_t mn = best_rpm;
+      if (n_others > 0 && other_rpm < mn) mn = other_rpm;
+      if (self_in_sl && self_rpm < mn) mn = self_rpm;
+      RpmFilter rf; rf.init(mn, ago);
+      p.keep_best = !rf.drop(best_rpm); p.keep_others = !rf.drop(other_rpm); p.keep_self = !rf.drop(self_rpm);
+      p.remaining = (p.keep_best ? 1 : 0) + (p.keep_others ? n_others : 0) + ((self_in_sl && p.keep_self) ? 1 : 0);
+    }
+    p.index = p.remaining == 1 ? 0u : hash_index(seed, decision_id, (uint32_t)p.remaining);
+  }
+  p.kth = p.index;
+  if (!(p.keep_best && p.kth == 0)) {
+    if (p.keep_best) p.kth--;
+    p.kind = p.keep_others ? PICK_MEMBER : PICK_SELF;  // without the others the only other survivor can be the self candidate
+  }
+  return p;
+}
+// what the caller is told about the instance the pick chose
+MMP_HD int32_t target_of(int32_t cidx, const mmp_decision_in &d) {
+  return (!(d.flags & MMP_DF_FAVOUR_SELF) && cidx == d.self) ? MMP_TARGET_SELF : cidx;
+}
 
 // Everything about one decision that does not need its bitmap row (72 bytes).  k_place lets lane j prepare the
 // context of decision j of a 32-decision batch (the dependent gathers overlap across lanes) and stages it in shared memory.
@@ -1076,6 +1116,9 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   bool best_full = false;
   int32_t best_count = 0, best_rpm = 0, best_idx = -1;
   uint32_t best_rank = b, lo = b, hi = NONE_RANK, k_lo = kb;
+  // the highest rank a phase's answer rests on (o.reach).  A phase that finds nothing counts for nothing: exclusions only
+  // take entries out of F, so it would find nothing with them either.
+  uint32_t dep = b;
   if (live) {
     rb = row_of(b);
     us = rb.idx == d.self;
@@ -1100,6 +1143,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
       go_ = x == 0;
     })
     (void)ended;
+    if (r1 != NONE_RANK && r1 > dep) dep = r1;
   }
   bool open = false;
   // ---- A'': non-simple (b), MM:4853-4887 -- a full best that is not one of its type's preferred instances.  kb = the first
@@ -1132,6 +1176,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
         else if (v) { kb_rank = wi * 32u + (uint32_t)ffs32(v); go_ = false; }
       }
     })
+    if (kb_rank != NONE_RANK && kb_rank > dep) dep = kb_rank;
     if (case_b && live) {
       if (pref_before) live = false;                      // the preferred entries within the distance are the candidates: general routine
       else if (kb_rank == NONE_RANK && open_end) open = true;  // the deciding entry is in a later shard
@@ -1241,6 +1286,8 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
     })
     if (walk && live && ended && cut_others == NONE_RANK && lim == NONE_RANK && open_end) open = true;
     k_b = k;
+    if (cut_others != NONE_RANK) { if (cut_others > dep) dep = cut_others; }
+    else if (walk && (lim == NONE_RANK || lim > dep)) dep = lim;  // every member of S' below lim counted
   }
   walk = walk && live && !open;
   const uint32_t cut = cut_others < cut_self ? cut_others : cut_self;
@@ -1251,27 +1298,12 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   if (walk) {
     if (favour_self && self_in_sl) { o.target = MMP_TARGET_SELF; fl |= MMP_TF_FAVOUR_EXIT; done = true; }
     else {
-      const int32_t n_others = (int32_t)n_in - (self_in_sl ? 1 : 0);
       ccount = 1 + (int32_t)n_in;
-      remaining = ccount;
-      if (ccount > 1) {
-        const int64_t ago = age_of(c.last_used, now);
-        if (ago < 432000000LL) {  // FIVE_DAYS_MS
-          int32_t mn = best_rpm;
-          if (n_others > 0 && fr.rpm < mn) mn = fr.rpm;
-          if (self_in_sl && rb.rpm < mn) mn = rb.rpm;
-          RpmFilter rf; rf.init(mn, ago);
-          keep_best = !rf.drop(best_rpm); keep_others = !rf.drop(fr.rpm); keep_self = !rf.drop(rb.rpm);
-          remaining = (keep_best ? 1 : 0) + (keep_others ? n_others : 0) + ((self_in_sl && keep_self) ? 1 : 0);
-        }
-        index = remaining == 1 ? 0u : hash_index(seed, decision_id, (uint32_t)remaining);
-      }
-      kth = index;
-      if (!(keep_best && kth == 0)) {
-        if (keep_best) kth--;
-        if (!keep_others) chosen_rank = (uint32_t)self_rank;  // the only other survivor can be the self candidate
-        else sel = true;
-      }
+      const PickOut pk = pick_survivor((int32_t)n_in, self_in_sl, best_rpm, fr.rpm, rb.rpm, c.last_used, now, seed, decision_id);
+      keep_best = pk.keep_best; keep_others = pk.keep_others; keep_self = pk.keep_self;
+      remaining = pk.remaining; index = pk.index; kth = pk.kth;
+      if (pk.kind == PICK_SELF) chosen_rank = (uint32_t)self_rank;
+      else sel = pk.kind == PICK_MEMBER;
     }
   }
   // ---- C: k-th survivor in rank order, walked from the last checkpoint of phase B that lies before it (words phase B
@@ -1317,13 +1349,14 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   if (open) { o.flags = MMP_TF_OPEN; return true; }
   if (!done) {
     const int32_t cidx = chosen_rank == best_rank ? best_idx : ((int32_t)chosen_rank == self_rank ? d.self : ((chosen_rank >> 5) < win_end ? AW.idx(chosen_rank) : AG.idx(chosen_rank)));
-    o.target = (!favour_self && cidx == d.self) ? MMP_TARGET_SELF : cidx;
+    o.target = target_of(cidx, d);
     o.n_candidates = ccount;
     o.n_remaining = remaining; o.pick_index = (int32_t)index;
     fl |= (keep_best ? MMP_TF_KEEP_BEST : 0) | (keep_others ? MMP_TF_KEEP_OTHERS : 0) | (keep_self ? MMP_TF_KEEP_SELF : 0);
   }
   o.cut_rank = (int32_t)(walk || (done && cut != NONE_RANK) ? cut : NONE_RANK);
   o.flags = fl;
+  o.reach = (int32_t)(dep == NONE_RANK ? NONE_RANK : dep + 1u);
   return true;
 }
 
@@ -1583,6 +1616,113 @@ MMP_HD void decide_ctx(const SnapshotView &s, const DecisionCtx &c, const uint32
   }
   const int32_t cidx = chosen_rank == best_rank ? best_idx : s.rows[chosen_rank].idx;
   o.target = (!favour_self && cidx == d.self) ? MMP_TARGET_SELF : cidx;
+}
+
+// ---- two-pass placement of a large batch (k_slot_summary, k_place_split; DESIGN.md §5.2).  For a type slot, a plain
+// decision's best, shortlist and their order depend on the decision only through its exclusions and self when those lie
+// below the walk's reach, and through its own record only as c_self (N2: one test for every member other than self).
+// The summary is that decision worked out once per slot for each value of c_self; a decision whose exclusions and self
+// all lie at or past the reach is answered from it by the pick arithmetic alone. ----
+static constexpr int SPLIT_CAP = 256;  // shortlist members a summary lists; a longer shortlist is walked
+struct SlotSummary {
+  int64_t best_rem, best_lru;  // what c_self is tested against: the best's remaining, and the first entry's lruTime when it is full
+  int32_t best_idx, best_rpm, best_full;
+  int32_t reach[2];            // by c_self: DecideOut::reach; -1: the decisions of this slot are walked
+  int32_t n_in[2];             // shortlist members besides best
+  int32_t pad_;
+};
+
+// The summary of type slot `slot` for c_self = cs, and its shortlist members (instance indices, rank order) into
+// members[0, SPLIT_CAP): decide_stream on a decision without exclusions, with a self that is not live and a record
+// that makes c_self come out as cs.  Called by every lane of the vote group (active = false for lanes without a slot);
+// ewin: win_words zero words.
+template <class V>
+MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, bool active, int cs, const uint32_t *ewin,
+                         uint32_t win_words, int64_t now, const V &vote, uint32_t *chunk, SlotSummary &sum, int32_t *members) {
+  DecisionCtx c;
+  c.d.model = 0; c.d.self = -1; c.d.last_used = 0; c.d.flags = 0; c.d.fresh = -1; c.d.extra_off = 0; c.d.extra_n = 0;
+  c.last_used = 0; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
+  c.xr[0] = c.xr[1] = c.xr[2] = c.xr[3] = -1;
+  c.slot = active ? (slot | ((s.has_pref[slot] ? 1 : 0) << 16)) : -1;
+  // c_self against a best with room tests remaining: this record makes it come out as cs
+  c.fr.lru = 0; c.fr.rem = cs ? INT64_MIN : INT64_MAX; c.fr.count = 0; c.fr.rpm = 0;
+  RowRanks none;
+  none.r[0] = none.r[1] = none.r[2] = none.r[3] = -1;
+  // first pass: the best (phases A, A', A'' do not read the caller's record of a self that is not live), and the
+  // shortlist when the best has room
+  DecideOut o;
+  bool ok = decide_stream<TabGlob>(s, T, T, c, active, ewin, win_words, none, 0u, now, 0, 0, vote, o, 0x3fffffff, chunk) && active &&
+            o.best_rank >= 0 && !(o.flags & MMP_TF_OPEN);
+  RankRow r0, rb;
+  r0.lru = r0.rem = 0; r0.rpm = 0; rb = r0; rb.idx = -1;
+  bool full = false;
+  if (ok) {
+    r0 = load_row(s.rows + o.first_rank);
+    rb = load_row(s.rows + o.best_rank);
+    full = r0.rem < s.min_space;  // (a full first entry is never replaced as best: A' runs for a best with room only)
+    if (full) {
+      const int64_t a10 = age_of(r0.lru, now) / 10;
+      c.fr.lru = cs ? (int64_t)((uint64_t)r0.lru + (uint64_t)((a10 > 45000 ? a10 : 45000) + 1)) : r0.lru;
+    }
+  }
+  // second pass, for a full best: c_self tests lruTime against the best's, which the record now forces to come out as cs
+  const bool again = ok && full;
+  DecideOut ox;
+  const bool ok2 = decide_stream<TabGlob>(s, T, T, c, again, ewin, win_words, none, 0u, now, 0, 0, vote, ox, 0x3fffffff, chunk);
+  const DecideOut &o2 = again ? ox : o;
+  ok = ok && (!again || ok2) && o2.best_rank == o.best_rank && !(o2.flags & (MMP_TF_OPEN | MMP_TF_FAVOUR_EXIT)) && o2.n_candidates >= 1 &&
+       o2.n_candidates - 1 <= SPLIT_CAP;
+  const int32_t n_in = ok ? o2.n_candidates - 1 : 0;
+  if (ok) {  // the members: S' strictly between best and the cut (no cut: the end of S, one below the reach)
+    const uint32_t lo = (uint32_t)o2.best_rank;
+    const uint32_t lim = o2.cut_rank != (int32_t)NONE_RANK ? (uint32_t)o2.cut_rank : (o2.reach == (int32_t)NONE_RANK ? NONE_RANK : (uint32_t)o2.reach - 1u);
+    const bool use_pref = (c.slot >> 16) && ((T.p[lo >> 5] >> (lo & 31)) & 1u);
+    int32_t k = 0;
+    for (uint32_t w = lo >> 5; w < (uint32_t)s.row_words && w * 32u < lim && k <= n_in; w++) {
+      uint32_t x = T.cx[w] & (use_pref ? T.p[w] : 0xffffffffu) & mask_above(w * 32u, lo) & mask_below(w * 32u, lim);
+      for (; x; x &= x - 1u) {
+        if (k < SPLIT_CAP) members[k] = s.rows[w * 32u + (uint32_t)ffs32(x)].idx;
+        k++;
+      }
+    }
+    ok = k == n_in;
+  }
+  if (!active) return;
+  if (cs == 0) { sum.best_rem = rb.rem; sum.best_lru = r0.lru; sum.best_idx = rb.idx; sum.best_rpm = rb.rpm; sum.best_full = full ? 1 : 0; sum.pad_ = 0; }
+  sum.reach[cs] = ok ? o2.reach : -1;
+  sum.n_in[cs] = n_in;
+}
+
+// The fast answer of k_place_split: a valid, unflagged decision without extra excludes whose model has no overflow ids
+// and whose exclusions and self all lie at or past its slot's reach for its c_self.  a: prepare_ctx_a of d; row: its
+// model's excluded ranks.  Returns false, with nothing written, for every other decision.
+MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, const CtxA &a, const RowRanks &row, const FreshRow *fresh,
+                         int32_t n_fresh, const SlotSummary *sums, const int32_t *members, int64_t now, uint64_t seed,
+                         uint64_t decision_id, mmp_decision_out &out) {
+  if (!a.ok || request_model(d) || d.extra_n != 0 || row.overflow()) return false;
+  FreshRow fr;  // (as prepare_ctx_b)
+  if (d.fresh >= 0 && d.fresh < n_fresh) fr = fresh[d.fresh];
+  else if (a.self_rank >= 0) { const RankRow sr = load_row(s.rows + a.self_rank); fr.lru = sr.lru; fr.rem = sr.rem; fr.count = sr.count; fr.rpm = 0; }
+  else return false;
+  const int tid = a.mr.type_id < s.n_type_ids ? a.mr.type_id : 0;
+  const int slot = (int)(s.type_slot[tid] & 0x7fffu);
+  const SlotSummary &sm = sums[slot];
+  int cs;
+  if (sm.best_full) {  // (decide_stream's c_self)
+    const int64_t a10 = age_of(sm.best_lru, now) / 10, df = jsub(fr.lru, sm.best_lru);
+    cs = df > 45000 && df > a10;
+  } else cs = fr.rem < s.min_space || fr.rem < (sm.best_rem >> 2);
+  const int32_t reach = sm.reach[cs];
+  if (reach < 0 || (a.self_rank >= 0 && a.self_rank < reach)) return false;
+  for (int j = 0; j < 4; j++) if (row.r[j] >= 0 && row.r[j] < reach) return false;
+  const int32_t n_in = sm.n_in[cs];
+  const int64_t last_used = (d.flags & MMP_DF_MODEL_LAST_USED) ? a.mr.last_used : d.last_used;
+  const PickOut pk = pick_survivor(n_in, false, sm.best_rpm, fr.rpm, sm.best_rpm, last_used, now, seed, decision_id);
+  if (pk.kind == PICK_SELF) return false;
+  const int32_t cidx = pk.kind == PICK_BEST ? sm.best_idx : members[((size_t)slot * 2 + (size_t)cs) * SPLIT_CAP + pk.kth];
+  out.target = target_of(cidx, d);
+  out.n_candidates = 1 + n_in;
+  return true;
 }
 
 }  // namespace mmp
