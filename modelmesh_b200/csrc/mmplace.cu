@@ -24,6 +24,9 @@
 //   k_place_small            tiny batches as a stream launch / replayed CUDA graph;  k_place_server: the resident B = 1 server
 //   k_place_dealt, k_dealt_wait   instance shards over peer memory;  k_shard_*: the kernels around the NCCL all-reduce
 //   k_place<...>             cooperative tiles: traced calls / very wide rows
+//   The one-decision-per-lane kernels share their steps through one helper each: no_decision / no_ctx (an absent lane),
+//   load_decision_stream (the streamed record load), redo_declined (the warp redo of what the lane routine declined; not
+//   k_place_dealt, which assembles the row in shared memory), WinTabs (the window tables in shared memory) and slot_key.
 //   k_build_bitmap*, k_sparse_slots + commit_kernels.cuh (device-path commit), scan_kernels.cuh (k_stats, k_reaper_flag,
 //   k_lru_events), churn_kernels.cuh (the closed loop), registry_kernels.cuh (k_scale_eval, k_registry_prune)
 #include <cuda_runtime.h>
@@ -146,6 +149,49 @@ __device__ __noinline__ void decide_warp(const SnapshotView s, const DecisionCtx
   if (!whole_rows || !decide_fast<false>(s, c, erow, now, seed, decision_id, co, o)) decide_ctx(s, c, erow, extra, now, seed, decision_id, co, o, nullptr);
   *target = o.target; *n_candidates = o.n_candidates;
   if (first_rank) { *first_rank = o.first_rank; *flags = o.flags; }
+}
+
+// ---- what the one-decision-per-lane kernels share: the record of a lane without a decision, the context of a lane whose
+// decision is absent, the streamed record load and the warp redo of what the lane routine declined ----
+__device__ __forceinline__ mmp_decision_in no_decision() {
+  mmp_decision_in d;
+  d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
+  return d;
+}
+__device__ __forceinline__ DecisionCtx no_ctx() {
+  DecisionCtx c;
+  c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
+  return c;
+}
+// decision record i, read once as a stream: no L1 allocation (the lane routine's tables are what should stay there)
+__device__ __forceinline__ mmp_decision_in load_decision_stream(const mmp_decision_in *in, int i) {
+  const int4 *dp = reinterpret_cast<const int4 *>(in + i);
+  int4 v[2];
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(v[h].x), "=r"(v[h].y), "=r"(v[h].z), "=r"(v[h].w) : "l"(dp + h));
+  mmp_decision_in d;
+  d.model = v[0].x; d.self = v[0].y; d.last_used = (int64_t)(((uint64_t)(uint32_t)v[0].w << 32) | (uint32_t)v[0].z);
+  d.flags = (uint32_t)v[1].x; d.fresh = v[1].y; d.extra_off = v[1].z; d.extra_n = v[1].w;
+  return d;
+}
+// The lanes of `pending` declined their decisions: the whole warp redoes them one at a time with decide_warp, reading
+// the row of lane l's row_id (excl_row_id) from global memory, with lane l's context c staged in *ctx_s.  The answer
+// lands in lane l's o: target, n_candidates, first_rank and flags.
+__device__ __forceinline__ void redo_declined(uint32_t pending, int lane, const DecisionCtx &c, int32_t row_id, uint64_t my_id, DecisionCtx *ctx_s,
+                                              const SnapshotView &s, const int32_t *extra, int64_t now, uint64_t seed, DecideOut &o) {
+  while (pending) {
+    const int l = __ffs((int)pending) - 1;
+    pending &= pending - 1;
+    if (lane == l) *ctx_s = c;
+    const int32_t rl = __shfl_sync(0xffffffffu, row_id, l);
+    const uint64_t idl = __shfl_sync(0xffffffffu, my_id, l);
+    __syncwarp();
+    int32_t t2, c2, f2, g2;
+    decide_warp(s, *ctx_s, excl_row(s, rl), extra, now, seed, idl, &t2, &c2, &f2, &g2);
+    if (lane == l) { o.target = t2; o.n_candidates = c2; o.first_rank = f2; o.flags = g2; }
+    __syncwarp();
+  }
 }
 
 struct RingLayout {
@@ -349,10 +395,53 @@ static constexpr int LANE_SLOTS = 64;    // type-constraint mask slots whose win
 static constexpr int LANE_WARPS = 12;    // warps per block of k_place_lanes
 static constexpr int LANE_STAGES = 4;    // landing stages per SM at most: a fifth takes the shared-memory carve-out from 196 to
                                          // 228 KB and leaves too little L1 for the lane tables to stay resident
+// The window part of the lane tables in shared memory (k_place_lanes, k_place_server): the masks of the first LANE_SLOTS
+// slots and full / csum / count_col / rows over the first LANE_WIN words of this process's rows, zero past their end.
+struct WinTabs {
+  uint32_t cx[LANE_SLOTS * LANE_WIN], p[LANE_SLOTS * LANE_WIN], full[LANE_WIN];
+  WordSumI csum[LANE_WIN];
+  __align__(16) int32_t count[LANE_WIN * 32];
+  __align__(16) RankRow rows[LANE_WIN * 32];
+  // thread tid of nthreads copies its share of the tables (the caller synchronises).  N: the type of the stride, blockDim.x
+  // or a constant int, as each kernel steps its loops (it decides how far the compiler unrolls them)
+  template <class N>
+  __device__ __forceinline__ void fill(const SnapshotView &s, int tid, N nthreads) {
+    const int WS = s.word_lo;
+    const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
+    const int nsl = min(s.n_slots, LANE_SLOTS);
+    const uint32_t *gcx = s.any_rs ? s.candx : s.cand;
+    for (int i = tid; i < nsl * LANE_WIN; i += nthreads) {
+      const int sl = i / LANE_WIN, w = i - sl * LANE_WIN;
+      const bool in = (uint32_t)w < win_words;
+      cx[i] = in ? gcx[(size_t)sl * s.row_words + WS + w] : 0u;
+      p[i] = in ? s.pref[(size_t)sl * s.row_words + WS + w] : 0u;
+    }
+    for (int w = tid; w < LANE_WIN; w += nthreads) {
+      const bool in = (uint32_t)w < win_words;
+      full[w] = in ? s.full[WS + w] : 0u;
+      csum[w] = in ? s.csum[WS + w] : WordSumI{0, 0};
+    }
+    for (int i = tid; i < LANE_WIN * 32; i += nthreads) {
+      const int r = WS * 32 + i;
+      const bool in = (uint32_t)(i >> 5) < win_words && r < s.n_ranks;
+      count[i] = in ? s.count_col[r] : 0;
+      RankRow z; z.lru = 0; z.rem = 0; z.count = 0; z.rpm = 0; z.idx = -1; z.flags = 0;
+      rows[i] = in ? s.rows[r] : z;
+    }
+  }
+  // T (the slot's global tables) with its window part pointed here: indexed by absolute row word / rank, so biased by the
+  // window's first word
+  __device__ __forceinline__ LaneTables view(const LaneTables &T, int slot, int word_lo) const {
+    LaneTables Tw = T;
+    if (slot < LANE_SLOTS) { Tw.cx = cx + slot * LANE_WIN - word_lo; Tw.p = p + slot * LANE_WIN - word_lo; }
+    Tw.full = full - word_lo; Tw.csum = csum - word_lo; Tw.count_col = count - word_lo * 32; Tw.rows = rows - word_lo * 32;
+    return Tw;
+  }
+};
 struct LaneLayout {
   uint32_t row_bytes, stride, stage_bytes, ns, warps;
   uint32_t off_bar, off_busy, off_uses, off_warp, per_warp;
-  uint32_t off_cx, off_p, off_full, off_csum, off_count, off_rows;  // the window part of the lane tables (LaneTables Tw)
+  uint32_t off_tabs;  // the WinTabs
   size_t total;
   __host__ __device__ LaneLayout(int row_words, int ns_, int warps_, bool front) {
     row_bytes = (uint32_t)row_words * 4u; stride = row_bytes + 16u;  // + 16: lanes copying their windows out spread over the banks
@@ -361,13 +450,8 @@ struct LaneLayout {
     off_bar = ns * stage_bytes; off_busy = off_bar + ns * 8u; off_uses = off_busy + ns * 4u;
     off_warp = (off_uses + ns * 4u + 127u) / 128u * 128u;
     per_warp = 32u * (LANE_STRIDE + MMP_CHUNK_WORDS) * 4u + (uint32_t)((sizeof(DecisionCtx) + 15) / 16 * 16);
-    off_cx = (off_warp + warps * per_warp + 15u) / 16u * 16u;
-    off_p = off_cx + LANE_SLOTS * LANE_WIN * 4u;
-    off_full = off_p + LANE_SLOTS * LANE_WIN * 4u;
-    off_csum = off_full + ((LANE_WIN * 4u + 7u) / 8u) * 8u;
-    off_count = (off_csum + LANE_WIN * 8u + 15u) / 16u * 16u;
-    off_rows = off_count + LANE_WIN * 32u * 4u;
-    total = front ? (size_t)off_rows + (size_t)LANE_WIN * 32u * sizeof(RankRow) : (size_t)off_cx;
+    off_tabs = (off_warp + warps * per_warp + 15u) / 16u * 16u;
+    total = front ? (size_t)off_tabs + sizeof(WinTabs) : (size_t)off_tabs;
   }
 };
 
@@ -398,48 +482,17 @@ __global__ void __launch_bounds__(LANE_WARPS * 32, 1) k_place_lanes(const Snapsh
   const int nb = (n + 31) >> 5;
   // ---- the window part of the lane tables in shared memory (with the SM's shared memory given to the landing stages the
   // L1 is too small to keep them resident: every in-window gather would be an L2 round trip) ----
-  uint32_t *f_cx = reinterpret_cast<uint32_t *>(smem_raw + lay.off_cx), *f_p = reinterpret_cast<uint32_t *>(smem_raw + lay.off_p);
-  uint32_t *f_full = reinterpret_cast<uint32_t *>(smem_raw + lay.off_full);
-  WordSumI *f_csum = reinterpret_cast<WordSumI *>(smem_raw + lay.off_csum);
-  int32_t *f_count = reinterpret_cast<int32_t *>(smem_raw + lay.off_count);
-  RankRow *f_rows = reinterpret_cast<RankRow *>(smem_raw + lay.off_rows);
-  const int WS = s.word_lo;
+  WinTabs *tabs = reinterpret_cast<WinTabs *>(smem_raw + lay.off_tabs);
   const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
   const bool front = nb >= 64;  // tiny launches read the snapshot directly
-  if (front) {
-    const int nsl = min(s.n_slots, LANE_SLOTS);
-    const uint32_t *gcx = s.any_rs ? s.candx : s.cand;
-    for (int i = threadIdx.x; i < nsl * LANE_WIN; i += blockDim.x) {
-      const int sl = i / LANE_WIN, w = i - sl * LANE_WIN;
-      const bool in = (uint32_t)w < win_words;
-      f_cx[i] = in ? gcx[(size_t)sl * s.row_words + WS + w] : 0u;
-      f_p[i] = in ? s.pref[(size_t)sl * s.row_words + WS + w] : 0u;
-    }
-    for (int w = threadIdx.x; w < LANE_WIN; w += blockDim.x) {
-      const bool in = (uint32_t)w < win_words;
-      f_full[w] = in ? s.full[WS + w] : 0u;
-      f_csum[w] = in ? s.csum[WS + w] : WordSumI{0, 0};
-    }
-    for (int i = threadIdx.x; i < LANE_WIN * 32; i += blockDim.x) {
-      const int r = WS * 32 + i;
-      const bool in = (uint32_t)(i >> 5) < win_words && r < s.n_ranks;
-      f_count[i] = in ? s.count_col[r] : 0;
-      RankRow z; z.lru = 0; z.rem = 0; z.count = 0; z.rpm = 0; z.idx = -1; z.flags = 0;
-      f_rows[i] = in ? s.rows[r] : z;
-    }
-  }
+  if (front) tabs->fill(s, threadIdx.x, blockDim.x);
   __syncthreads();
   // batches of 32 decisions are dealt round-robin to the grid's warps (consecutive batches to the warps of one block)
   const int gw = blockIdx.x * LANE_WARPS + wib, nw = gridDim.x * LANE_WARPS;
   auto load_dec = [&](int b, mmp_decision_in &d) -> bool {
     const int i = b * 32 + lane;
     if (b >= nb || i >= n) return false;
-    const int4 *dp = reinterpret_cast<const int4 *>(in + i);
-    int4 a, c;  // streamed once: no L1 allocation (the lane routine's tables are what should stay there)
-    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(dp));
-    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(c.x), "=r"(c.y), "=r"(c.z), "=r"(c.w) : "l"(dp + 1));
-    d.model = a.x; d.self = a.y; d.last_used = (int64_t)(((uint64_t)(uint32_t)a.w << 32) | (uint32_t)a.z);
-    d.flags = (uint32_t)c.x; d.fresh = c.y; d.extra_off = c.z; d.extra_n = c.w;
+    d = load_decision_stream(in, i);
     return true;
   };
   // Software pipeline per warp (every load is issued at least one phase before its first use, because a warp stalls in
@@ -476,8 +529,7 @@ __global__ void __launch_bounds__(LANE_WARPS * 32, 1) k_place_lanes(const Snapsh
     const uint32_t *my_row = reinterpret_cast<const uint32_t *>(stage + (size_t)lane * lay.stride);
     // row of this decision: its model's, or row i of a gathered row set (orig_id != nullptr: the instance-shard gather pass)
     const int m = orig_id ? (valid ? b * 32 + lane : 0) : (valid ? excl_row_id(s, d.model, d.flags) : 0);
-    DecisionCtx c;
-    c.slot = -2; c.d.model = 0; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
+    DecisionCtx c = no_ctx();
     bool skip = false;  // instance-sharded, not the first shard: an entry in a lower shard wins, the row is not even read
     if (s.word_lo > 0) {
       if (valid) { prepare_ctx_b(s, d, ca, fresh, n_fresh, extra, c); skip = shard_cannot_win(s, c, ca.mr.reserved); }
@@ -520,27 +572,11 @@ __global__ void __launch_bounds__(LANE_WARPS * 32, 1) k_place_lanes(const Snapsh
     const uint64_t my_id = pick_id(d, id_base + (uint64_t)(orig_id ? (valid ? orig_id[b * 32 + lane] : 0) : b * 32 + lane));
     const int slot = c.slot >= 0 ? ctx_slot(c) : 0;
     const LaneTables T = lane_tables_global(s, slot);
-    LaneTables Tw = T;
-    if (front) {  // tables indexed by absolute row word / rank: bias the shared-memory copies by the window's first word
-      if (slot < LANE_SLOTS) { Tw.cx = f_cx + slot * LANE_WIN - WS; Tw.p = f_p + slot * LANE_WIN - WS; }
-      Tw.full = f_full - WS; Tw.csum = f_csum - WS; Tw.count_col = f_count - WS * 32; Tw.rows = f_rows - WS * 32;
-    }
+    const LaneTables Tw = front ? tabs->view(T, slot, s.word_lo) : T;
     const bool handled = decide_stream(s, Tw, T, c, valid && !skip, win + lane * LANE_STRIDE, win_words, RowPtr{excl_row(s, m), (uint32_t)s.word_lo},
                                        self_eword, now, seed, my_id, WarpVote(), o, budget, chunk + lane * MMP_CHUNK_WORDS);
     // ---- what the lane routine declined: the whole warp redoes it, reading the row from global memory (L2) ----
-    uint32_t pending = __ballot_sync(0xffffffffu, valid && !skip && !handled);
-    while (pending) {
-      const int l = __ffs((int)pending) - 1;
-      pending &= pending - 1;
-      if (lane == l) *ctx_one = c;
-      const int ml = __shfl_sync(0xffffffffu, m, l);
-      const uint64_t idl = __shfl_sync(0xffffffffu, my_id, l);
-      __syncwarp();
-      int32_t t2, c2, f2, g2;
-      decide_warp(s, *ctx_one, excl_row(s, ml), extra, now, seed, idl, &t2, &c2, &f2, &g2);
-      if (lane == l) { o.target = t2; o.n_candidates = c2; o.first_rank = f2; o.flags = g2; }
-      __syncwarp();
-    }
+    redo_declined(__ballot_sync(0xffffffffu, valid && !skip && !handled), lane, c, m, my_id, ctx_one, s, extra, now, seed, o);
     if (valid) {
       if (emit_keys) {  // instance-sharded: one min-loc key per decision instead of the result (same 8 bytes)
         uint64_t key = ~(uint64_t)0;
@@ -570,11 +606,9 @@ __device__ __forceinline__ void place_small_block(const SnapshotView &s, const m
   const int lane = threadIdx.x;
   const int i = blk * 32 + lane;
   const bool valid = i < n;
-  mmp_decision_in d;
-  d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
+  mmp_decision_in d = no_decision();
   if (valid) d = in[i];
-  DecisionCtx c;
-  c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
+  DecisionCtx c = no_ctx();
   if (valid) prepare_ctx(s, d, fresh, n_fresh, extra, c);
   const int m = excl_row_id(s, d.model, d.flags);
   const uint32_t *row = excl_row(s, m);
@@ -586,19 +620,7 @@ __device__ __forceinline__ void place_small_block(const SnapshotView &s, const m
   __shared__ uint32_t chunk_b[32 * MMP_CHUNK_WORDS];  // (callers are one-warp blocks)
   const bool handled = decide_stream<TabGlob>(s, T, T, c, valid, nullptr, 0u, RowPtr{row, (uint32_t)s.word_lo}, self_eword,
                                               now, seed, my_id, WarpVote(), o, budget, chunk_b + lane * MMP_CHUNK_WORDS);
-  uint32_t pending = __ballot_sync(0xffffffffu, valid && !handled);
-  while (pending) {
-    const int l = __ffs((int)pending) - 1;
-    pending &= pending - 1;
-    if (lane == l) *ctx_one = c;
-    const int ml = __shfl_sync(0xffffffffu, m, l);
-    const uint64_t idl = __shfl_sync(0xffffffffu, my_id, l);
-    __syncwarp();
-    int32_t t2, c2, f2, g2;
-    decide_warp(s, *ctx_one, excl_row(s, ml), extra, now, seed, idl, &t2, &c2, &f2, &g2);
-    if (lane == l) { o.target = t2; o.n_candidates = c2; }
-    __syncwarp();
-  }
+  redo_declined(__ballot_sync(0xffffffffu, valid && !handled), lane, c, m, my_id, ctx_one, s, extra, now, seed, o);
   if (valid) out[i] = mmp_decision_out{o.target, o.n_candidates};
 }
 __global__ void __launch_bounds__(32) k_place_small(const SnapshotView s_arg, const mmp_decision_in *__restrict__ in, int n_arg,
@@ -636,10 +658,8 @@ __global__ void k_slot_keys(const SnapshotView s, const mmp_decision_in *__restr
   if (i >= n) return;
   const mmp_decision_in d = in[i];
   uint32_t k = 0xffffu;
-  if (request_model(d) ? (d.model >= 0 && d.model < 65535) : (d.model >= 0 && d.model < s.n_models)) {
-    const int ty = request_model(d) ? d.model : s.models[d.model].type_id;
-    k = (uint32_t)s.type_slot[(ty >= 0 && ty < s.n_type_ids) ? ty : 0] & 0x7fffu;  // (as prepare_ctx_b resolves it)
-  }
+  if (request_model(d) ? (d.model >= 0 && d.model < 65535) : (d.model >= 0 && d.model < s.n_models))
+    k = slot_key(s, request_model(d) ? d.model : s.models[d.model].type_id);
   keys[i] = (uint16_t)k;
   idx[i] = i;
 }
@@ -657,24 +677,15 @@ __device__ __forceinline__ void place_direct(const SnapshotView &s, const mmp_de
   // perm (optional): the batch in type-slot order -- decisions of one slot walk the same masks, so the 32 lanes of a warp
   // finish their walks together instead of waiting for the longest (fleets with sparse candidate sets: C5)
   const int i = valid ? (perm ? perm[j_] : j_) : 0;
-  mmp_decision_in d;
-  d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
-  if (valid) {
-    const int4 *dp = reinterpret_cast<const int4 *>(in + i);
-    int4 a, c;  // streamed once
-    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(dp));
-    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(c.x), "=r"(c.y), "=r"(c.z), "=r"(c.w) : "l"(dp + 1));
-    d.model = a.x; d.self = a.y; d.last_used = (int64_t)(((uint64_t)(uint32_t)a.w << 32) | (uint32_t)a.z);
-    d.flags = (uint32_t)c.x; d.fresh = c.y; d.extra_off = c.z; d.extra_n = c.w;
-  }
+  mmp_decision_in d = no_decision();
+  if (valid) d = load_decision_stream(in, i);
   const int m = excl_row_id(s, d.model, d.flags);
   // the model's excluded ranks go out first: they depend on the record only (a request-model decision has none: its
   // model's instances are among its extras)
   RowRanks row;
   row.r[0] = row.r[1] = row.r[2] = row.r[3] = -1;
   if (valid && m != ZERO_ROW) row = load_ranks(s.excl_ranks + (size_t)m * 4);
-  DecisionCtx c;
-  c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
+  DecisionCtx c = no_ctx();
   if (valid) prepare_ctx(s, d, fresh, n_fresh, extra, c);
   // a model with overflow ids is resolved from its bitmap row by the warp (decide_warp)
   const bool ovf = valid && row.overflow();
@@ -696,19 +707,7 @@ __device__ __forceinline__ void place_direct(const SnapshotView &s, const mmp_de
   const uint64_t my_id = pick_id(d, id_base + (uint64_t)i);
   const bool handled = decide_stream<TabGlob>(s, T, T, c, valid && !ovf, w, win_words, row, self_eword, now, seed, my_id, WarpVote(), o, budget,
                                               chunk_s[warp] + lane * MMP_CHUNK_WORDS);
-  uint32_t pending = __ballot_sync(0xffffffffu, valid && (ovf || !handled));
-  while (pending) {
-    const int l = __ffs((int)pending) - 1;
-    pending &= pending - 1;
-    if (lane == l) ctx_w[warp] = c;
-    const int ml = __shfl_sync(0xffffffffu, m, l);
-    const uint64_t idl = __shfl_sync(0xffffffffu, my_id, l);
-    __syncwarp();
-    int32_t t2, c2, f2, g2;
-    decide_warp(s, ctx_w[warp], excl_row(s, ml), extra, now, seed, idl, &t2, &c2, &f2, &g2);
-    if (lane == l) { o.target = t2; o.n_candidates = c2; }
-    __syncwarp();
-  }
+  redo_declined(__ballot_sync(0xffffffffu, valid && (ovf || !handled)), lane, c, m, my_id, &ctx_w[warp], s, extra, now, seed, o);
   if (valid) out[i] = mmp_decision_out{o.target, o.n_candidates};
 }
 template <int WARPS, int MINB>
@@ -773,16 +772,8 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
                                                      int32_t *__restrict__ key_idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const bool valid = i < n;
-  mmp_decision_in d;
-  d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
-  if (valid) {
-    const int4 *dp = reinterpret_cast<const int4 *>(in + i);
-    int4 a, c;  // streamed once
-    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "l"(dp));
-    asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(c.x), "=r"(c.y), "=r"(c.z), "=r"(c.w) : "l"(dp + 1));
-    d.model = a.x; d.self = a.y; d.last_used = (int64_t)(((uint64_t)(uint32_t)a.w << 32) | (uint32_t)a.z);
-    d.flags = (uint32_t)c.x; d.fresh = c.y; d.extra_off = c.z; d.extra_n = c.w;
-  }
+  mmp_decision_in d = no_decision();
+  if (valid) d = load_decision_stream(in, i);
   const int m = excl_row_id(s, d.model, d.flags);
   RowRanks row;  // (read as k_place_direct reads it: its overflow mark routes the decision the same way)
   row.r[0] = row.r[1] = row.r[2] = row.r[3] = -1;
@@ -799,7 +790,7 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
   warp_append(ovf, i, ovf_list, counts + 1);
   if (keys && valid) {
     uint32_t k = 0xffffu;
-    if (walk) k = a.ok ? (uint32_t)s.type_slot[a.mr.type_id < s.n_type_ids ? a.mr.type_id : 0] & 0x7fffu : 0xfffeu;
+    if (walk) k = a.ok ? slot_key(s, a.mr.type_id) : 0xfffeu;
     keys[i] = (uint16_t)k;
     key_idx[i] = i;
   }
@@ -840,12 +831,6 @@ struct SrvLine0 { unsigned long long seq; long long now; unsigned long long seed
 struct SrvLine1 { int n, n_fresh, n_extra, pad; FreshRow fr; int32_t extra[SRV_INLINE_EXTRA]; unsigned long long pad2; };
 struct ServerResp { unsigned long long done_seq; int alive, served; mmp_decision_out out0; unsigned long long pad[5]; };
 static_assert(sizeof(SrvLine0) == 64 && sizeof(SrvLine1) == 64 && sizeof(ServerResp) == 64, "one line each");
-struct SrvTabs {
-  uint32_t cx[LANE_SLOTS * LANE_WIN], p[LANE_SLOTS * LANE_WIN], full[LANE_WIN];
-  WordSumI csum[LANE_WIN];
-  __align__(16) int32_t count[LANE_WIN * 32];
-  __align__(16) RankRow rows[LANE_WIN * 32];
-};
 __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, volatile SrvLine0 *l0, volatile SrvLine1 *l1, volatile ServerResp *resp,
                                                      const mmp_decision_in *in_tab, const FreshRow *fresh_tab, const int32_t *extra,
                                                      mmp_decision_out *out_tab, unsigned long long life_ns, unsigned long long idle_ns, int budget) {
@@ -856,37 +841,10 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
   __shared__ uint32_t win_s[32 * LANE_STRIDE];
   __shared__ uint32_t chunk_v[32 * MMP_CHUNK_WORDS];
   // the window part of the lane tables, as in k_place_lanes: the in-window steps of a decision read shared memory only
-  __shared__ SrvTabs tabs;
-  uint32_t *f_cx = tabs.cx, *f_p = tabs.p, *f_full = tabs.full;
-  WordSumI *f_csum = tabs.csum;
-  int32_t *f_count = tabs.count;
-  RankRow *f_rows = tabs.rows;
+  __shared__ WinTabs tabs;
   const int lane = threadIdx.x;
-  const SnapshotView &sv = s_arg;
-  const int WS = sv.word_lo;
-  const uint32_t win_words = (uint32_t)min(LANE_WIN, sv.word_hi - sv.word_lo);
-  {
-    const int nsl = min(sv.n_slots, LANE_SLOTS);
-    const uint32_t *gcx = sv.any_rs ? sv.candx : sv.cand;
-    for (int i = lane; i < nsl * LANE_WIN; i += 32) {
-      const int sl = i / LANE_WIN, w = i - sl * LANE_WIN;
-      const bool inw = (uint32_t)w < win_words;
-      f_cx[i] = inw ? gcx[(size_t)sl * sv.row_words + WS + w] : 0u;
-      f_p[i] = inw ? sv.pref[(size_t)sl * sv.row_words + WS + w] : 0u;
-    }
-    for (int w = lane; w < LANE_WIN; w += 32) {
-      const bool inw = (uint32_t)w < win_words;
-      f_full[w] = inw ? sv.full[WS + w] : 0u;
-      f_csum[w] = inw ? sv.csum[WS + w] : WordSumI{0, 0};
-    }
-    for (int i = lane; i < LANE_WIN * 32; i += 32) {
-      const int r = WS * 32 + i;
-      const bool inw = (uint32_t)(i >> 5) < win_words && r < sv.n_ranks;
-      f_count[i] = inw ? sv.count_col[r] : 0;
-      RankRow z; z.lru = 0; z.rem = 0; z.count = 0; z.rpm = 0; z.idx = -1; z.flags = 0;
-      f_rows[i] = inw ? sv.rows[r] : z;
-    }
-  }
+  const uint32_t win_words = (uint32_t)min(LANE_WIN, s_arg.word_hi - s_arg.word_lo);
+  tabs.fill(s_arg, lane, 32);
   __syncwarp();
   unsigned long long t0, t_last, t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
@@ -914,8 +872,7 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
     if (kind == 1u) {
       // ---- one decision: record from the line, window straight from the row, tables from shared memory ----
       const bool valid = lane == 0;
-      mmp_decision_in d;
-      d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
+      mmp_decision_in d = no_decision();
       if (valid) d = *reinterpret_cast<const mmp_decision_in *>(line_s + 8);
       int n_fresh = 0;
       s.n_extra = 0;
@@ -937,8 +894,7 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
         q[j] = make_uint4(0u, 0u, 0u, 0u);
         if (valid && (uint32_t)(j * 4) < win_words) q[j] = __ldg(reinterpret_cast<const uint4 *>(row) + j);
       }
-      DecisionCtx c;
-      c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
+      DecisionCtx c = no_ctx();
       if (valid) prepare_ctx(s, d, &fresh_s, min(n_fresh, 1), extra1, c);
       uint32_t self_eword = 0;
       if (valid && c.self_rank >= 0) self_eword = __ldg(row + (c.self_rank >> 5) - s.word_lo);
@@ -948,21 +904,13 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
       __syncwarp();
       const int slot = c.slot >= 0 ? ctx_slot(c) : 0;
       const LaneTables T = lane_tables_global(s, slot);
-      LaneTables Tw = T;
-      if (slot < LANE_SLOTS) { Tw.cx = f_cx + slot * LANE_WIN - WS; Tw.p = f_p + slot * LANE_WIN - WS; }
-      Tw.full = f_full - WS; Tw.csum = f_csum - WS; Tw.count_col = f_count - WS * 32; Tw.rows = f_rows - WS * 32;
+      const LaneTables Tw = tabs.view(T, slot, s.word_lo);
       DecideOut o;
       const uint64_t my_id = pick_id(d, id_base);
       const bool handled = decide_stream(s, Tw, T, c, valid, w, win_words, RowPtr{row, (uint32_t)s.word_lo}, self_eword, now, seed, my_id, WarpVote(), o, budget,
                                          chunk_v + lane * MMP_CHUNK_WORDS);
-      if (__shfl_sync(0xffffffffu, (int)(!handled), 0)) {
-        if (lane == 0) ctx_one = c;
-        __syncwarp();
-        int32_t t2, c2, f2, g2;
-        decide_warp(s, ctx_one, excl_row(s, __shfl_sync(0xffffffffu, m, 0)), extra1, now, seed, __shfl_sync(0xffffffffu, my_id, 0), &t2, &c2, &f2, &g2);
-        if (lane == 0) { o.target = t2; o.n_candidates = c2; }
-        __syncwarp();
-      }
+      // pending: lane 0, the only lane with a decision, if it declined
+      redo_declined(__shfl_sync(0xffffffffu, (uint32_t)!handled, 0), lane, c, m, my_id, &ctx_one, s, extra1, now, seed, o);
       if (lane == 0) { resp->out0.target = o.target; resp->out0.n_candidates = o.n_candidates; }
     } else {
       // ---- a batch of up to 32 through the mapped tables (sizes in line 1) ----
@@ -1021,11 +969,9 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_dealt(const Snapshot
   const long long wb = ((long long)blockIdx.x * WARPS + warp) * G + me;             // this warp's batch of 32 decisions
   const long long i = wb * 32 + lane;
   const bool valid = i < n;
-  mmp_decision_in d;
-  d.model = -1; d.self = -1; d.last_used = 0; d.flags = 0; d.fresh = -1; d.extra_off = 0; d.extra_n = 0;
+  mmp_decision_in d = no_decision();
   if (valid) d = in[i];
-  DecisionCtx c;
-  c.slot = -2; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
+  DecisionCtx c = no_ctx();
   if (valid) prepare_ctx(s, d, fresh, n_fresh, extra, c);
   const int m = (valid && d.model >= 0 && d.model < s.n_models) ? d.model : 0;
   LaneTables T = lane_tables_global(s, c.slot >= 0 ? ctx_slot(c) : 0);
@@ -1057,6 +1003,8 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_dealt(const Snapshot
   const uint64_t my_id = pick_id(d, id_base + (uint64_t)i);
   const bool handled = decide_stream<TabGlob>(s, T, T, c, valid, w, win_words < (uint32_t)LANE_WIN ? 0u : win_words, row, self_eword, now, seed, my_id,
                                               WarpVote(), o, budget, chunk_d[warp] + lane * MMP_CHUNK_WORDS);
+  // (redo_declined, but the row is assembled in shared memory: passing that step to the helper as a callable costs this
+  // kernel 8 B more stack and spills)
   uint32_t pending = __ballot_sync(0xffffffffu, valid && !handled);
   while (pending) {  // the cooperative general routine over the whole row, assembled in shared memory
     const int l = __ffs((int)pending) - 1;

@@ -596,6 +596,11 @@ MMP_HD void prepare_ctx_a(const SnapshotView &s, const mmp_decision_in &d, CtxA 
 #endif
   }
 }
+// the mask slot of a type id, resolved as prepare_ctx_b resolves it (an id the snapshot does not know is type 0): the key a
+// slot-ordered batch is sorted by (prepare_ctx_b reads the whole type_slot entry, has_pref included)
+MMP_HD uint32_t slot_key(const SnapshotView &s, int32_t type_id) {
+  return (uint32_t)s.type_slot[(type_id >= 0 && type_id < s.n_type_ids) ? type_id : 0] & 0x7fffu;
+}
 MMP_HD void prepare_ctx_b(const SnapshotView &s, const mmp_decision_in &d, const CtxA &a, const FreshRow *fresh_tab, int32_t n_fresh,
                           const int32_t *extra, DecisionCtx &c) {
   c.d = d; c.slot = -1; c.self_rank = -1; c.last_used = 0; c.self_bits = 0; c.self_count = 0;
@@ -1704,8 +1709,7 @@ MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, const 
   if (d.fresh >= 0 && d.fresh < n_fresh) fr = fresh[d.fresh];
   else if (a.self_rank >= 0) { const RankRow sr = load_row(s.rows + a.self_rank); fr.lru = sr.lru; fr.rem = sr.rem; fr.count = sr.count; fr.rpm = 0; }
   else return false;
-  const int tid = a.mr.type_id < s.n_type_ids ? a.mr.type_id : 0;
-  const int slot = (int)(s.type_slot[tid] & 0x7fffu);
+  const int slot = (int)slot_key(s, a.mr.type_id);
   const SlotSummary &sm = sums[slot];
   int cs;
   if (sm.best_full) {  // (decide_stream's c_self)
