@@ -336,6 +336,25 @@ int32_t mmp_lru_apply_status(mmp_fleet *, const mmp_lru_event *ev, int32_t n, in
  * read of a present key, resize with a new weight or removal of a present key (quirk N14); MMP_LRU_LOAD's churn guard
  * reads the same value. */
 int32_t mmp_lru_state(mmp_fleet *, int32_t n_instances, int64_t *oldest, int64_t *weighted, int32_t *count);
+/* The read side of the same caches (of the standalone store or of the closed loop's).  A read sees every event of every
+ * mmp_lru_apply(_status) / mmp_churn_seed / mmp_churn_step call that has returned and none of a call still in progress. */
+typedef struct {
+  int32_t model, weight;
+  int64_t last_used;
+  int64_t load_ts;    /* registration time of a closed-loop copy (MR.instanceIds value); -1 in the standalone store and when
+                         the copy is not registered */
+} mmp_lru_entry;      /* 24 B */
+/* descendingMapWithCutoff(used_since) of each listed cache (CLHM:1226-1260): from the most recently used entry down, up to
+ * the first with 0 < last_used < used_since; used_since <= 0 is descendingLruMap() (CLHM:1087-1116), the whole deque.
+ * instances: n cache indices, repeats allowed (listed again), NULL = 0 .. n-1.  offsets[0 .. n]: cache i's walk is entries
+ * offsets[i] .. offsets[i+1] of the concatenation, whatever cap is; out receives its first cap entries (MRU first within
+ * each cache).  Nothing is written on an error.  Sets the "lru_read" timing. */
+int32_t mmp_lru_read(mmp_fleet *, const int32_t *instances, int32_t n, int64_t used_since, int64_t *offsets, mmp_lru_entry *out,
+                     int64_t cap);
+/* getLastUsedTime (CLHM:742-746: -1 when absent or last_used <= 0) and getWeight (CLHM:768-771: -1 when absent) of n
+ * (instance, model) pairs, with the copy's load_ts as mmp_lru_entry has it (-1 when absent).  Nothing is written on an error. */
+int32_t mmp_lru_lookup(mmp_fleet *, int32_t n, const int32_t *instance, const int32_t *model, int64_t *last_used, int32_t *weight,
+                       int64_t *load_ts);
 
 /* ---- the closed loop on the device (SURVEY.md §8a rows a11 admission, a12 rebalance; §8f-1 ingest / ordering maintenance,
  * §8f-4 fleet simulator; BASELINE.json configs[3] "churn").  One call = one republish window (2 s, INSTANCE_REC_PUBLISH_MIN_
@@ -459,7 +478,8 @@ int32_t mmp_registry_prune_ids(mmp_fleet *, int32_t self, int64_t now_ms, int64_
  *   "commit_host_only" 1: every commit takes the structural (host) path */
 int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
 /* CUDA-event duration (ms) of the device part of the last mmp_stats ("stats"), mmp_reaper_select ("reaper": registry sweep +
- * sort + select), mmp_lru_apply ("lru_apply": the event kernel) on this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
+ * sort + select), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
+ * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device

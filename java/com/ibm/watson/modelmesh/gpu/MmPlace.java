@@ -94,6 +94,11 @@ final class MmPlace {
     static native int lruApply(long h, ByteBuffer events, int n, long nowMs, ByteBuffer out, int cap);
     static native int lruApplyStatus(long h, ByteBuffer events, int n, long nowMs, ByteBuffer out, int cap, ByteBuffer status);
     static native int lruState(long h, int nInstances, ByteBuffer oldest, ByteBuffer weighted, ByteBuffer count);
+    // read side: descendingMapWithCutoff / descendingLruMap (CLHM:1226-1260, 1087-1116), getLastUsedTime / getWeight (CLHM:742-771)
+    static final int LRU_ENTRY_BYTES = 24;
+    static native int lruRead(long h, ByteBuffer instances, int n, long usedSince, ByteBuffer offsets, ByteBuffer out, long cap);
+    static native int lruLookup(long h, int n, ByteBuffer instance, ByteBuffer model, ByteBuffer lastUsed, ByteBuffer weight,
+                                ByteBuffer loadTs);
     // the closed loop (simulation / what-if)
     static native int churnInit(long h, long loadTimeoutMs, long lastPublishedMs, int slotsPerInstance);
     static native int churnSeed(long h, int n, ByteBuffer instance, ByteBuffer model, ByteBuffer lastUsed, ByteBuffer weight,

@@ -353,6 +353,16 @@ jint FN(lruState)(JNIEnv *env, jclass c, jlong h, jint nInstances, jobject oldes
   (void)c;
   return mmp_lru_state(H(h), nInstances, (int64_t *)BUF(oldest), (int64_t *)BUF(weighted), (int32_t *)BUF(count));
 }
+/* instances: int32[n] direct buffer or null (caches 0 .. n-1); offsets: int64[n + 1]; out: cap mmp_lru_entry records (24 B) */
+jint FN(lruRead)(JNIEnv *env, jclass c, jlong h, jobject instances, jint n, jlong usedSince, jobject offsets, jobject out, jlong cap) {
+  (void)c;
+  return mmp_lru_read(H(h), (const int32_t *)BUF(instances), n, usedSince, (int64_t *)BUF(offsets), (mmp_lru_entry *)BUF(out), cap);
+}
+jint FN(lruLookup)(JNIEnv *env, jclass c, jlong h, jint n, jobject instance, jobject model, jobject lastUsed, jobject weight, jobject loadTs) {
+  (void)c;
+  return mmp_lru_lookup(H(h), n, (const int32_t *)BUF(instance), (const int32_t *)BUF(model), (int64_t *)BUF(lastUsed), (int32_t *)BUF(weight),
+                        (int64_t *)BUF(loadTs));
+}
 
 /* ---- the closed loop ---- */
 jint FN(churnInit)(JNIEnv *env, jclass c, jlong h, jlong loadTimeoutMs, jlong lastPublishedMs, jint slotsPerInstance) {

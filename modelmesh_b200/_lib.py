@@ -43,7 +43,8 @@ CHURN_DECISION = np.dtype([("model", "<i4"), ("self", "<i4"), ("target", "<i4"),
                            ("event", "<i4")], align=True)
 CHURN_EVICTION = np.dtype([("instance", "<i4"), ("model", "<i4"), ("last_used", "<i8"), ("weight", "<i4"), ("order", "<i4"),
                            ("reload", "<i4")], align=True)
-assert LRU_EVENT.itemsize == 24 and EVICTION.itemsize == 24
+LRU_ENTRY = np.dtype([("model", "<i4"), ("weight", "<i4"), ("last_used", "<i8"), ("load_ts", "<i8")], align=True)
+assert LRU_EVENT.itemsize == 24 and EVICTION.itemsize == 24 and LRU_ENTRY.itemsize == 24
 assert CHURN_EVENT.itemsize == 24 and CHURN_DECISION.itemsize == 24 and CHURN_EVICTION.itemsize == 32
 SCALE_IN = np.dtype([("instance", "<i4"), ("model", "<i4"), ("count", "<i8"), ("last_used", "<i8"), ("last_heavy", "<i8"), ("i1", "<i4"),
                      ("i2", "<i4"), ("weight", "<i4"), ("flags", "<i4")], align=True)
@@ -134,6 +135,8 @@ SYMBOLS = [
     ("mmp_lru_apply", _I32, [_P, _P, _I32, _I64, _P, _I32]),
     ("mmp_lru_state", _I32, [_P, _I32, _P, _P, _P]),
     ("mmp_lru_apply_status", _I32, [_P, _P, _I32, _I64, _P, _I32, _P]),
+    ("mmp_lru_read", _I32, [_P, _P, _I32, _I64, _P, _P, _I64]),
+    ("mmp_lru_lookup", _I32, [_P, _I32, _P, _P, _P, _P, _P]),
     ("mmp_churn_init", _I32, [_P, C.c_void_p]),
     ("mmp_churn_seed", _I32, [_P, _I32, _P, _P, _P, _P, _P, _I64]),
     ("mmp_churn_step", _I32, [_P, _P, _I32, _I64, _I64, _U64, _P, _I32, C.POINTER(_I32), _P, _I32, C.POINTER(_I32), _P, C.c_void_p]),

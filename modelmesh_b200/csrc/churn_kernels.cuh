@@ -413,6 +413,7 @@ int32_t mmp_churn_init(mmp_fleet *f, const mmp_churn_config *cfg) {
   cs.n_carry = 0;
   cs.regs_from_host = true;
   cs.on = true;
+  f->lru_loop = true;
   return MMP_OK;
 }
 

@@ -1265,6 +1265,7 @@ struct mmp_fleet {
   int commit_host_only = 0;     // MMP_COMMIT=host: every commit takes the structural (host) path (A/B and cross-check)
   bool device_ahead = false;    // the closed loop (churn_kernels.cuh) changed the registry on the device: host tables are behind
   float t_stats_ms = 0, t_reaper_ms = 0, t_lru_ms = 0, t_prune_ms = 0;  // CUDA-event time of the device part of the last mmp_stats / mmp_reaper_select / mmp_lru_apply
+  float t_lru_read_ms = 0;      // ... and of the last mmp_lru_read (its count + scan part plus its emit part)
   int32_t last_commit_path = 0; // 1 structural (host), 2 device
   double last_commit_ms = 0;
   ncclComm_t comm = nullptr;    // instance-shard communicator (mmp_shard_connect)
@@ -1312,6 +1313,7 @@ struct mmp_fleet {
   // LRU store (plug point 3)
   DevBuf lru_ts, lru_seq, lru_weight, lru_model, lru_cap, lru_wsize, lru_count, lru_seqctr, lru_loadts, lru_pin;
   int32_t lru_n = 0, lru_slots = 0;
+  bool lru_loop = false;        // the store was set up by mmp_churn_init: its load times are registrations (mmp_lru_read reports them)
 };
 
 static int32_t set_device(mmp_fleet *f) {
@@ -2297,6 +2299,7 @@ int32_t mmp_last_timing(mmp_fleet *f, const char *key, double *ms) {
   if (!strcmp(key, "stats")) *ms = f->t_stats_ms;
   else if (!strcmp(key, "reaper")) *ms = f->t_reaper_ms;
   else if (!strcmp(key, "lru_apply")) *ms = f->t_lru_ms;
+  else if (!strcmp(key, "lru_read")) *ms = f->t_lru_read_ms;
   else if (!strcmp(key, "prune")) *ms = f->t_prune_ms;
   else if (!strcmp(key, "commit")) *ms = f->last_commit_ms;
   else if (!strcmp(key, "dealt_kernel")) *ms = f->peers.t_kernel_ms;

@@ -1,6 +1,7 @@
 // scan_kernels.cuh — batch scans (plug points 3 and 4 of include/mmplace.h): ClusterStats reductions, the reaper's
 // registry sweep + top-K selection, and the per-instance time-ordered weighted LRU.  Included at the end of mmplace.cu.
 #pragma once
+#include <cuda/std/tuple>
 
 // ---------------------------------------------------------------------------------------------------------------
 // ClusterStats (MM:1570-1591) per prohibited-type-set partition: InstanceSetStatsTracker.add (ISST:63-72) as a
@@ -585,6 +586,133 @@ __global__ void k_lru_state(LruView v, long long *oldest, long long *weighted, i
   if (lane == 0) { oldest[inst] = pin != LRU_PIN_NONE ? pin : slot < 0 ? -1 : t; weighted[inst] = v.wsize[inst]; count[inst] = v.count[inst]; }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Read side: descendingMapWithCutoff / descendingLruMap (CLHM:1226-1260, 1087-1116), getLastUsedTime / getWeight
+// (CLHM:742-771).  The walk from the MRU end stops at the first node with 0 < lastUsed < usedSince.  The deque is in (ts, seq)
+// order, so the walk returns every entry with ts >= used_since, and the entries with ts <= 0 (which lie below every positive
+// time) only when no entry has 0 < ts < used_since.  The kernels only read the slot arrays k_lru_events writes.
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool lru_read_passes(long long ts, long long used_since, bool stops) {
+  return ts >= used_since || (ts <= 0 && !stops);
+}
+
+// one warp per listed cache: the length of its walk (cnt[k]) and whether the walk stops before its end (stops[k]);
+// cnt[n] is left for the caller to zero, so the exclusive scan of cnt[0 .. n] is the offsets array
+__global__ void k_lru_read_count(LruView v, const int *__restrict__ inst, int n, long long used_since, long long *__restrict__ cnt,
+                                 unsigned char *__restrict__ stops) {
+  const int lane = threadIdx.x & 31;
+  const int k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (k >= n) return;
+  const size_t base = (size_t)inst[k] * v.slots;
+  int since = 0, nonpos = 0;
+  bool stop = false;
+  for (int i = lane; i < v.slots; i += 32) {
+    if (v.model[base + i] < 0) continue;
+    const long long t = v.ts[base + i];
+    since += t >= used_since;
+    nonpos += t <= 0 && t < used_since;
+    stop |= t > 0 && t < used_since;
+  }
+  stop = __any_sync(0xffffffffu, stop);
+  since = __reduce_add_sync(0xffffffffu, since);
+  nonpos = __reduce_add_sync(0xffffffffu, nonpos);
+  if (lane == 0) { cnt[k] = since + (stop ? 0 : nonpos); stops[k] = stop; }
+}
+
+__device__ __forceinline__ mmp_lru_entry lru_read_entry(const LruView &v, size_t at, int loop) {
+  return mmp_lru_entry{v.model[at], v.weight[at], v.ts[at], loop ? v.loadts[at] : -1};
+}
+
+// One block per listed cache whose walk has at most LRU_READ_SMEM entries and starts before `cap`: the passing entries go to
+// shared memory, and each one's rank is the number of entries with a larger (ts, seq) key.  Keys are unique within a cache
+// (a fresh seq per insert or move, the successor's seq - 1 for a tie with it), so the ranks are a permutation.
+static constexpr int LRU_READ_SMEM = 2048;  // 20 B per entry: 40 KB of static shared memory
+__global__ void __launch_bounds__(256) k_lru_read_emit(LruView v, const int *__restrict__ inst, const long long *__restrict__ off,
+                                                       const unsigned char *__restrict__ stops, long long used_since, int loop,
+                                                       mmp_lru_entry *__restrict__ out, long long cap) {
+  __shared__ long long s_ts[LRU_READ_SMEM], s_seq[LRU_READ_SMEM];
+  __shared__ int s_slot[LRU_READ_SMEM];
+  __shared__ int s_n;
+  const int k = blockIdx.x;
+  const long long o = off[k], c = off[k + 1] - o;
+  if (c == 0 || c > LRU_READ_SMEM || o >= cap) return;
+  if (threadIdx.x == 0) s_n = 0;
+  __syncthreads();
+  const size_t base = (size_t)inst[k] * v.slots;
+  const bool stop = stops[k];
+  for (int i = threadIdx.x; i < v.slots; i += blockDim.x) {
+    if (v.model[base + i] < 0) continue;
+    const long long t = v.ts[base + i];
+    if (!lru_read_passes(t, used_since, stop)) continue;
+    const int p = atomicAdd(&s_n, 1);
+    s_ts[p] = t; s_seq[p] = v.seq[base + i]; s_slot[p] = i;
+  }
+  __syncthreads();
+  for (int p = threadIdx.x; p < (int)c; p += blockDim.x) {
+    const long long t = s_ts[p], q = s_seq[p];
+    int r = 0;
+    for (int j = 0; j < (int)c; j++) r += key_less(t, q, s_ts[j], s_seq[j]);
+    if (o + r < cap) out[o + r] = lru_read_entry(v, base + s_slot[p], loop);
+  }
+}
+
+// The global-memory path, for walks longer than LRU_READ_SMEM: the passing entries of every such cache are keyed
+// (segment, ~ts, ~seq), sorted ascending by one radix sort, and a position's rank is its distance from its segment's start.
+struct LruReadKey { unsigned seg; unsigned long long nts, nseq; };
+struct LruReadKeyParts {
+  __host__ __device__ ::cuda::std::tuple<unsigned &, unsigned long long &, unsigned long long &> operator()(LruReadKey &k) const {
+    return {k.seg, k.nts, k.nseq};
+  }
+};
+__device__ __forceinline__ unsigned long long lru_desc_bits(long long x) { return ~((unsigned long long)x ^ 0x8000000000000000ull); }
+
+// one block per segment (listed cache big[b]): its passing entries, keyed, from seg_off[b] on
+__global__ void k_lru_read_gather(LruView v, const int *__restrict__ inst, const unsigned char *__restrict__ stops, long long used_since,
+                                  const int *__restrict__ big, const long long *__restrict__ seg_off, LruReadKey *__restrict__ keys,
+                                  int *__restrict__ slot_of) {
+  __shared__ int s_n;
+  const int b = blockIdx.x, k = big[b];
+  if (threadIdx.x == 0) s_n = 0;
+  __syncthreads();
+  const size_t base = (size_t)inst[k] * v.slots;
+  const bool stop = stops[k];
+  for (int i = threadIdx.x; i < v.slots; i += blockDim.x) {
+    if (v.model[base + i] < 0) continue;
+    const long long t = v.ts[base + i];
+    if (!lru_read_passes(t, used_since, stop)) continue;
+    const long long p = seg_off[b] + atomicAdd(&s_n, 1);
+    keys[p] = LruReadKey{(unsigned)b, lru_desc_bits(t), lru_desc_bits(v.seq[base + i])};
+    slot_of[p] = i;
+  }
+}
+__global__ void k_lru_read_scatter(LruView v, const int *__restrict__ inst, const long long *__restrict__ off, const int *__restrict__ big,
+                                   const long long *__restrict__ seg_off, const LruReadKey *__restrict__ keys, const int *__restrict__ slot_of,
+                                   long long total, int loop, mmp_lru_entry *__restrict__ out, long long cap) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= total) return;
+  const unsigned b = keys[p].seg;
+  const int k = big[b];
+  const long long dst = off[k] + (p - seg_off[b]);
+  if (dst < cap) out[dst] = lru_read_entry(v, (size_t)inst[k] * v.slots + slot_of[p], loop);
+}
+
+// one warp per (instance, model) query
+__global__ void k_lru_lookup(LruView v, int n, const int *__restrict__ inst, const int *__restrict__ model, int loop,
+                             long long *__restrict__ last_used, int *__restrict__ weight, long long *__restrict__ load_ts) {
+  const int lane = threadIdx.x & 31;
+  const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (q >= n) return;
+  const int m = model[q];
+  int fr;
+  const int slot = m < 0 ? -1 : lru_find(v, inst[q], lane, m, &fr);  // (a negative key would match a free slot)
+  if (lane) return;
+  const size_t at = (size_t)inst[q] * v.slots + (slot < 0 ? 0 : slot);
+  const long long t = slot < 0 ? -1 : v.ts[at];
+  last_used[q] = t <= 0 ? -1 : t;
+  weight[q] = slot < 0 ? -1 : v.weight[at];
+  load_ts[q] = slot < 0 || !loop ? -1 : v.loadts[at];
+}
+
 // dynamic shared memory of a k_lru_events launch with 4 warps per block: room for every warp's staged slot arrays (32 B per
 // slot), or none when the instance caches are too large for it
 static int lru_stage_slots(mmp_fleet *f, size_t *smem) {
@@ -655,7 +783,7 @@ int32_t mmp_lru_init(mmp_fleet *f, int32_t n, const int64_t *capacity, int32_t s
   std::vector<long long> ctr((size_t)n, 1LL << 40);
   CK(cudaMemcpy(f->lru_seqctr.p, ctr.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(f->lru_cap.p, capacity, (size_t)n * 8, cudaMemcpyHostToDevice));
-  f->lru_n = n; f->lru_slots = slots;
+  f->lru_n = n; f->lru_slots = slots; f->lru_loop = false;
   return MMP_OK;
 }
 
@@ -745,6 +873,127 @@ int32_t mmp_lru_state(mmp_fleet *f, int32_t n, int64_t *oldest, int64_t *weighte
   CK(cudaMemcpyAsync(weighted, c->d_out.p, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaMemcpyAsync(count, c->d_extra.p, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
+  return MMP_OK;
+}
+
+int32_t mmp_lru_read(mmp_fleet *f, const int32_t *instances, int32_t n, int64_t used_since, int64_t *offsets, mmp_lru_entry *out,
+                     int64_t cap) {
+  NEED(f);
+  if (n < 0 || (n > 0 && !offsets) || cap < 0 || (cap > 0 && !out)) { g_err = "bad argument"; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  if (f->lru_n == 0) { g_err = "mmp_lru_init not called"; return MMP_E_STATE; }
+  std::vector<int32_t> inst((size_t)n);
+  for (int32_t k = 0; k < n; k++) {
+    inst[k] = instances ? instances[k] : k;
+    if (inst[k] < 0 || inst[k] >= f->lru_n) { g_err = "instance index out of range"; return MMP_E_ARG; }
+  }
+  if (n == 0) { if (offsets) offsets[0] = 0; return MMP_OK; }
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t s = c->stream;
+  const LruView v = lru_view(f);
+  const int loop = f->lru_loop ? 1 : 0;
+  // d_in: instances; d_trace: per-cache counts, then the offsets; d_cand: stop flags
+  const size_t n1 = (size_t)n + 1;
+  CK(c->d_in.ensure((size_t)n * 4));
+  CK(c->d_trace.ensure(2 * n1 * 8));
+  CK(c->d_cand.ensure((size_t)n));
+  long long *d_cnt = c->d_trace.as<long long>(), *d_off = d_cnt + n1;
+  int *d_inst = c->d_in.as<int>();
+  unsigned char *d_stop = c->d_cand.as<unsigned char>();
+  size_t tscan = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tscan, d_cnt, d_off, (int)n1, s));
+  CK(c->d_cub.ensure(tscan + 64));
+  CK(cudaMemcpyAsync(d_inst, inst.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(d_cnt + n, 0, 8, s));
+  CK(cudaEventRecord(c->e0, s));
+  k_lru_read_count<<<(n + 3) / 4, 128, 0, s>>>(v, d_inst, n, used_since, d_cnt, d_stop);
+  CK(cub::DeviceScan::ExclusiveSum(c->d_cub.p, tscan, d_cnt, d_off, (int)n1, s));
+  CK(cudaEventRecord(c->e1, s));
+  f->launches += 2;
+  CK(cudaGetLastError());
+  std::vector<int64_t> off(n1);
+  CK(cudaMemcpyAsync(off.data(), d_off, n1 * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  float ms_count = 0;
+  if (cudaEventElapsedTime(&ms_count, c->e0, c->e1) != cudaSuccess) ms_count = 0;
+  const int64_t total = off[n], written = std::min(total, cap);
+  // the walks longer than the shared-memory path holds, among those that start before cap: one segment each
+  std::vector<int32_t> big;
+  std::vector<int64_t> seg_off(1, 0);
+  for (int32_t k = 0; k < n; k++)
+    if (off[k] < cap && off[k + 1] - off[k] > LRU_READ_SMEM) { big.push_back(k); seg_off.push_back(seg_off.back() + off[k + 1] - off[k]); }
+  const int64_t n_sort = seg_off.back();
+  if (written > 0) {
+    CK(c->d_out.ensure((size_t)written * sizeof(mmp_lru_entry)));
+    mmp_lru_entry *d_out = c->d_out.as<mmp_lru_entry>();
+    // d_extra: big + seg_off; d_fresh: keys in / out; d_rows: slots in / out
+    LruReadKey *k_in = nullptr, *k_out = nullptr;
+    int *s_in = nullptr, *s_out = nullptr, *d_big = nullptr;
+    long long *d_seg = nullptr;
+    size_t tsort = 0;
+    if (n_sort > 0) {
+      CK(c->d_extra.ensure(seg_off.size() * 8 + big.size() * 4));
+      CK(c->d_fresh.ensure((size_t)n_sort * 2 * sizeof(LruReadKey)));
+      CK(c->d_rows.ensure((size_t)n_sort * 2 * 4));
+      d_seg = c->d_extra.as<long long>(); d_big = reinterpret_cast<int *>(d_seg + seg_off.size());
+      k_in = c->d_fresh.as<LruReadKey>(); k_out = k_in + n_sort;
+      s_in = c->d_rows.as<int>(); s_out = s_in + n_sort;
+      CK(cub::DeviceRadixSort::SortPairs(nullptr, tsort, k_in, k_out, s_in, s_out, n_sort, LruReadKeyParts{}, s));
+      CK(c->d_cub.ensure(tsort + 64));
+      CK(cudaMemcpyAsync(d_seg, seg_off.data(), seg_off.size() * 8, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync(d_big, big.data(), big.size() * 4, cudaMemcpyHostToDevice, s));
+    }
+    CK(cudaEventRecord(c->e0, s));
+    k_lru_read_emit<<<n, 256, 0, s>>>(v, d_inst, d_off, d_stop, used_since, loop, d_out, cap);
+    f->launches++;
+    if (n_sort > 0) {
+      k_lru_read_gather<<<(int)big.size(), 256, 0, s>>>(v, d_inst, d_stop, used_since, d_big, d_seg, k_in, s_in);
+      CK(cub::DeviceRadixSort::SortPairs(c->d_cub.p, tsort, k_in, k_out, s_in, s_out, n_sort, LruReadKeyParts{}, s));
+      k_lru_read_scatter<<<(unsigned)((n_sort + 255) / 256), 256, 0, s>>>(v, d_inst, d_off, d_big, d_seg, k_out, s_out, n_sort, loop, d_out, cap);
+      f->launches += 3;
+    }
+    CK(cudaEventRecord(c->e1, s));
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, d_out, (size_t)written * sizeof(mmp_lru_entry), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    float ms = 0;
+    if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) ms_count += ms;
+  }
+  f->t_lru_read_ms = ms_count;
+  std::memcpy(offsets, off.data(), n1 * 8);
+  return MMP_OK;
+}
+
+int32_t mmp_lru_lookup(mmp_fleet *f, int32_t n, const int32_t *instance, const int32_t *model, int64_t *last_used, int32_t *weight,
+                       int64_t *load_ts) {
+  NEED(f);
+  if (n < 0 || (n > 0 && (!instance || !model || !last_used || !weight || !load_ts))) { g_err = "bad argument"; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  if (f->lru_n == 0) { g_err = "mmp_lru_init not called"; return MMP_E_STATE; }
+  for (int32_t q = 0; q < n; q++)
+    if (instance[q] < 0 || instance[q] >= f->lru_n) { g_err = "instance index out of range"; return MMP_E_ARG; }
+  if (n == 0) return MMP_OK;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t s = c->stream;
+  // d_in: instances, models; d_out: last_used, load_ts; d_extra: weights
+  CK(c->d_in.ensure((size_t)n * 8)); CK(c->d_out.ensure((size_t)n * 16)); CK(c->d_extra.ensure((size_t)n * 4));
+  int *d_inst = c->d_in.as<int>(), *d_model = d_inst + n;
+  long long *d_lu = c->d_out.as<long long>(), *d_lt = d_lu + n;
+  CK(cudaMemcpyAsync(d_inst, instance, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_model, model, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  k_lru_lookup<<<(n + 3) / 4, 128, 0, s>>>(lru_view(f), n, d_inst, d_model, f->lru_loop ? 1 : 0, d_lu, c->d_extra.as<int>(), d_lt);
+  f->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(last_used, d_lu, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(load_ts, d_lt, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(weight, c->d_extra.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
   return MMP_OK;
 }
 

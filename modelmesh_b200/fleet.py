@@ -13,7 +13,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CLUSTER_STATS, DECISION_IN, DECISION_OUT, DECISION_TRACE, EVICTION,
-                   INSTANCE_ROW, LRU_EVENT, MODEL_ROW, ChurnConfig, ChurnReport, MmpConfig)
+                   INSTANCE_ROW, LRU_ENTRY, LRU_EVENT, MODEL_ROW, ChurnConfig, ChurnReport, MmpConfig)
 
 
 class MmpError(RuntimeError):
@@ -256,6 +256,30 @@ class Fleet:
         if n > cap:
             raise MmpError(-1, f"eviction buffer too small ({n} > {cap})")
         return out[:n].copy(), status
+
+    def lru_read(self, instances: Optional[Sequence[int]] = None, used_since: int = 0):
+        """mmp_lru_read: descendingMapWithCutoff(used_since) of each listed cache (None: every cache), as (offsets, entries):
+        cache k's walk is entries[offsets[k]:offsets[k + 1]], most recently used first (LRU_ENTRY records)."""
+        ids = None if instances is None else np.ascontiguousarray(instances, dtype=np.int32)
+        n = self._lru_n if ids is None else len(ids)
+        offsets = np.zeros(n + 1, dtype=np.int64)
+        cap = getattr(self, "_lru_read_cap", 1024)
+        while True:  # one call unless the caches grew past the last read's total
+            out = np.zeros(max(cap, 1), dtype=LRU_ENTRY)
+            self._ck(self.lib.mmp_lru_read(self.h, _ptr(ids), n, used_since, _ptr(offsets), _ptr(out), cap))
+            if offsets[n] <= cap:
+                return offsets, out[:offsets[n]].copy()
+            cap = self._lru_read_cap = int(offsets[n])
+
+    def lru_lookup(self, instance, model):
+        """mmp_lru_lookup: getLastUsedTime / getWeight and the copy's load_ts for (instance, model) pairs; -1 where absent"""
+        inst = np.ascontiguousarray(instance, dtype=np.int32)
+        mod = np.ascontiguousarray(model, dtype=np.int32)
+        assert inst.shape == mod.shape
+        n = len(inst)
+        last_used, weight, load_ts = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.int32), np.zeros(n, dtype=np.int64)
+        self._ck(self.lib.mmp_lru_lookup(self.h, n, _ptr(inst), _ptr(mod), _ptr(last_used), _ptr(weight), _ptr(load_ts)))
+        return last_used, weight, load_ts
 
     # ---- the closed loop (churn) ----
     def churn_init(self, load_timeout_ms: int, last_published_ms: int, slots_per_instance: int):
