@@ -365,25 +365,43 @@ int32_t mmp_lru_lookup(mmp_fleet *, int32_t n, const int32_t *instance, const in
  *     a copy loaded more than 2 x load_timeout_ms ago whose type set is < 95 % full is queued for ensureLoadedElsewhere and
  *     placed first in the next window, MM:2915-2931); later misses of the same model in the window are coalesced;
  *   REMOVE -> runtimeCache.remove on every registered copy;
+ *   REAPER (caller = the leader instance, t = the reaper's clock; model and u ignored) -> one run of the reaper's proactive
+ *     loads (MM:6456-6494): the gate and globalLru of MM:6456-6463, the candidates of MM:6574-6577 (no loaded copy, fewer
+ *     than 2 failed loads, used after globalLru unless the cluster has free space), then triggerProactiveLoadsForInstanceSubset
+ *     (MM:6616-6747) for the whole cluster, or with type constraints for each partition in mmp_stats order with one `taken`
+ *     set: size estimate, spaceToFill, the free-space and total counts and the lastUsed cutoff (age() at t), the bounded
+ *     most-recently-used selection (N12: of equal lastUsed the first model in index order) and the emission rule of
+ *     MM:6711-6719.  Every emitted model is a decision getNext(model, self = caller, lastUsed = the model's lastUsed) with no
+ *     extra excludes, loaded on its target at last_used = the model's lastUsed on the clock t (ensureLoadedInternal MM:6727);
+ *     its decisions stand at the REAPER's trace position, in emission order, and coalesce with the window's other decisions
+ *     as misses do (a model already decided in the window is not decided again; a later miss of a model the reaper decided
+ *     is coalesced).  A size estimate of 0 (the reference's ArithmeticException, MM:6651) ends the run at that partition.
+ *     An out-of-range caller makes the run's decisions malformed (status 8), as for a REQUEST.
+ *     Epoch-batching choices (the oracle makes the same): every partition reads the one snapshot of the window's start (the
+ *     reference sleeps 2 x INSTANCE_REC_PUBLISH_MIN_PERIOD_MS between partitions, MM:6481-6484: put the runs in separate
+ *     windows for that); the prune half of pruneModelRegistry is a no-op (no instance leaves the table in the loop);
+ *     repairLastUsedTimeIfNeeded, vmodels and leaseless-record cleanup are not modelled; the caller picks the leader;
+ *     DISABLE_PROACTIVE_LOADING is a trace without REAPER events.  A window with REAPER events reads the selections' count
+ *     back once (one host synchronisation) to size its decision buffers; a window without them runs as before;
  *   then the registry changes, publishInstanceRecord with its significance thresholds (MM:5390-5470) per instance, and a
  *   commit (re-rank under PLACEMENT_ORDER, tables, bitmap) -- all on the device.  The host only reads the reports.
  * Requires an unsharded fleet; a model may hold any number of registrations (loaded copies, then failed loads), as long as
  * its copy_count tells its loaded copies apart (not saturated at 255 over more than 255 registrations).  Replaces nothing in the
  * reference 1:1 (each pod runs its own loop there); it is the batched, fleet-wide form of it for simulation / what-if runs. ---- */
-enum { MMP_CHURN_REQUEST = 0, MMP_CHURN_REMOVE = 1 };
+enum { MMP_CHURN_REQUEST = 0, MMP_CHURN_REMOVE = 1, MMP_CHURN_REAPER = 2 };
 typedef struct { int32_t type; int32_t model; int32_t caller; uint32_t u; int64_t t; } mmp_churn_event;
 typedef struct {
   int32_t model, self, target, n_candidates;
   int32_t status;  /* MMP_LOAD_* of the load, 1 = nowhere to load (getNext null), 7 = queued reload skipped (the model has a
                       copy again), 8 = malformed, 9 = accepted but evicted again later in the window */
-  int32_t event;   /* index of the REQUEST that caused it, or -1 - k for the k-th queued ensureLoadedElsewhere */
+  int32_t event;   /* index of the REQUEST or REAPER event that caused it, or -1 - k for the k-th queued ensureLoadedElsewhere */
 } mmp_churn_decision;
 typedef struct { int32_t instance, model; int64_t last_used; int32_t weight, order, reload; } mmp_churn_eviction;
 typedef struct { int64_t load_timeout_ms; int64_t last_published_ms; int32_t slots_per_instance; int32_t reserved; } mmp_churn_config;
 typedef struct {
   int32_t n_published, n_carry, n_coalesced, n_lru_events;
   float ms_classify, ms_place, ms_route, ms_apply, ms_registry, ms_commit, ms_total;  /* CUDA-event times of the phases */
-  float reserved;
+  float ms_reaper; /* the reaper pass of the window's REAPER events, its read-back included (0 without them); not in ms_classify */
 } mmp_churn_report;
 /* one cache per instance index (capacity = its published capacity), empty; needs a committed snapshot */
 int32_t mmp_churn_init(mmp_fleet *, const mmp_churn_config *cfg);

@@ -56,7 +56,7 @@ SCALE_OUT = np.dtype([("action", "<i4"), ("copies_to_load", "<i4"), ("load_last_
                       ("set_heavy", "<i4"), ("remove", "<i4")], align=True)
 assert SCALE_IN.itemsize == 48 and SCALE_PARAMS.itemsize == 72 and SCALE_OUT.itemsize == 40
 LRU_LOAD = 5
-CHURN_REQUEST, CHURN_REMOVE = 0, 1
+CHURN_REQUEST, CHURN_REMOVE, CHURN_REAPER = 0, 1, 2
 
 
 class ChurnConfig(C.Structure):
@@ -67,7 +67,7 @@ class ChurnConfig(C.Structure):
 class ChurnReport(C.Structure):
     _fields_ = [("n_published", C.c_int32), ("n_carry", C.c_int32), ("n_coalesced", C.c_int32), ("n_lru_events", C.c_int32),
                 ("ms_classify", C.c_float), ("ms_place", C.c_float), ("ms_route", C.c_float), ("ms_apply", C.c_float),
-                ("ms_registry", C.c_float), ("ms_commit", C.c_float), ("ms_total", C.c_float), ("reserved", C.c_float)]
+                ("ms_registry", C.c_float), ("ms_commit", C.c_float), ("ms_total", C.c_float), ("ms_reaper", C.c_float)]
 
 DF_FAVOUR_SELF = 1
 DF_MODEL_LAST_USED = 2

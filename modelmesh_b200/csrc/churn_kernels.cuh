@@ -1,7 +1,9 @@
 // churn_kernels.cuh — the closed loop of the placement / eviction path ON THE DEVICE (SURVEY.md §8a rows a11, a12; §8f-1,
 // §8f-4): one call of mmp_churn_step = one republish window (2 s, MM:232) of the whole fleet:
+//   reaper      (windows with REAPER events only) the reaper's selections, k_rp_* below; their count is read back once
 //   classify    requests -> cache hits (runtimeCache.get on a registered copy) / cache misses (the first request of an unloaded
-//               model in the window -> a getNext decision) / removals; queued ensureLoadedElsewhere calls go first
+//               model in the window -> a getNext decision) / removals / the reaper's selections (decisions at the REAPER's
+//               position); queued ensureLoadedElsewhere calls go first
 //   place       the scoring kernel (k_place_lanes) over the window's decisions against the committed snapshot
 //   route       every cache event to its instance: radix sort by (instance, position in the trace)
 //   apply       k_lru_events: one warp per instance, events in order -- loadLocal's admission rules, the time-ordered
@@ -9,14 +11,26 @@
 //   registry    edge lists / copy counts / lastUsed of the models touched (MR:69, 239-246)
 //   republish   getFreshInstanceRecord + publishInstanceRecord's significance thresholds (MM:5369-5470) per instance
 //   commit      the device path of mmp_fleet_commit (commit_kernels.cuh): re-rank, rebuild tables and bitmap
-// No host work between the phases; the host reads the reports (decisions, evictions, rows) once at the end.
-// Epoch semantics = oracle/mm_sim.inc (the parity tests drive the same trace through both).  Included by mmplace.cu.
+// No host work between the phases (but the reaper's one read-back); the host reads the reports (decisions, evictions, rows)
+// once at the end.
+// Epoch semantics = oracle/mm_sim.inc, REAPER events = its step as tests/emul/reaper_sim.cpp extends it (the parity tests
+// drive the same trace through both).  Included by mmplace.cu.
 #pragma once
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 struct DecMeta { int event, weight, order, exclude; };
+// The window's REAPER events for the classify kernels: ev_idx[0 .. n) their trace indices (ascending); event r selected
+// models off[r] .. off[r + 1] of the selection list, and fpos (exclusive scan of the selections' first-decision flags, null
+// when nothing was selected) says how many of them became decisions.
+struct RpView { const int *ev_idx; int n; const int *off; const int *fpos; };
+__device__ __forceinline__ int rp_decisions(const RpView &rp, int i) {
+  if (!rp.fpos) return 0;
+  int lo = 0, hi = rp.n;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (rp.ev_idx[mid] < i) lo = mid + 1; else hi = mid; }
+  return rp.fpos[rp.off[lo + 1]] - rp.fpos[rp.off[lo]];
+}
 
 // phase A.1: the first cache miss of every unloaded model in the window (queued follow-ons count and come first)
 __global__ void k_churn_first(const Follow *__restrict__ carry, int n_follow, const mmp_churn_event *__restrict__ ev, int n,
@@ -31,16 +45,18 @@ __global__ void k_churn_first(const Follow *__restrict__ carry, int n_follow, co
 }
 // phase A.2: which items become decisions (every follow-on; the first miss of a model), and how many cache-event slots each
 // item owns: one for a decision's load (phase C) or a cache hit, one per loaded copy for a REMOVE.  x = decision, y = slots.
+// A REAPER item owns one decision and one slot per selection that is the first decision of its model in the window.
 __global__ void k_churn_flag(const Follow *__restrict__ carry, int n_follow, const mmp_churn_event *__restrict__ ev, int n,
                              const mmp_model_row *__restrict__ models, int n_models, const int *__restrict__ first_ev,
-                             int2 *__restrict__ is_dec, long long *__restrict__ used_t, int *__restrict__ counters) {
+                             int2 *__restrict__ is_dec, long long *__restrict__ used_t, int *__restrict__ counters, RpView rp) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_follow + n) return;
   int d = 0, slots = 0;
   if (q < n_follow) d = 1;
   else {
     const mmp_churn_event e = ev[q - n_follow];
-    if (e.model >= 0 && e.model < n_models) {
+    if (e.type == MMP_CHURN_REAPER) d = rp_decisions(rp, q - n_follow);
+    else if (e.model >= 0 && e.model < n_models) {
       const int cc = models[e.model].copy_count;
       if (e.type == 0) {
         atomicMax(&used_t[e.model], (long long)e.t);  // MR.updateLastUsed at the end of the window
@@ -78,6 +94,7 @@ __global__ void k_churn_emit(const Follow *__restrict__ carry, int n_follow, con
       else dec_of_model[c.model] = k;
     } else {
       const mmp_churn_event e = ev[q - n_follow];
+      if (e.type == MMP_CHURN_REAPER) return;  // (k_rp_emit writes its decisions)
       d.model = e.model; d.self = e.caller; d.last_used = e.t;
       extra[k] = -1;
       m = DecMeta{q - n_follow, models[e.model].size_units, q, -1};
@@ -113,16 +130,12 @@ __global__ void k_churn_emit(const Follow *__restrict__ carry, int n_follow, con
 }
 // phase C.1: a decision that found a target becomes a checked load on that instance; its clock is the clock of the request
 // that caused it (queued follow-ons: the start of the window)
-__global__ void k_churn_route(const mmp_decision_in *__restrict__ dec_in, const mmp_decision_out *__restrict__ dec_out,
-                              const DecMeta *__restrict__ meta, const int2 *__restrict__ is_dec, const int2 *__restrict__ dec_pos, int n_items,
-                              int max_instances, const mmp_churn_event *__restrict__ ev, long long now0, int *__restrict__ status,
-                              int *__restrict__ dec_target, LruEv *__restrict__ lev, unsigned long long *__restrict__ keys) {
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= n_items) return;
-  if (!is_dec[q].x) return;
-  const size_t slot = (size_t)dec_pos[q].y;
+__device__ __forceinline__ void churn_route_one(int k, size_t slot, const mmp_decision_in *__restrict__ dec_in,
+                                                const mmp_decision_out *__restrict__ dec_out, const DecMeta *__restrict__ meta,
+                                                int max_instances, const mmp_churn_event *__restrict__ ev, long long now0,
+                                                int *__restrict__ status, int *__restrict__ dec_target, LruEv *__restrict__ lev,
+                                                unsigned long long *__restrict__ keys) {
   keys[slot] = ~0ull;
-  const int k = dec_pos[q].x;
   dec_target[k] = -1;
   if (status[k] == CH_SKIPPED) return;
   const mmp_decision_out o = dec_out[k];
@@ -134,6 +147,18 @@ __global__ void k_churn_route(const mmp_decision_in *__restrict__ dec_in, const 
   const DecMeta m = meta[k];
   lev[slot] = LruEv{LEV_LOAD, d.model, m.weight, m.order, k, 0, d.last_used, m.event >= 0 ? (long long)ev[m.event].t : now0};
   keys[slot] = ((unsigned long long)(unsigned)tgt << 32) | (unsigned)m.order;
+}
+__global__ void k_churn_route(const mmp_decision_in *__restrict__ dec_in, const mmp_decision_out *__restrict__ dec_out,
+                              const DecMeta *__restrict__ meta, const int2 *__restrict__ is_dec, const int2 *__restrict__ dec_pos, int n_items,
+                              int max_instances, const mmp_churn_event *__restrict__ ev, long long now0, int *__restrict__ status,
+                              int *__restrict__ dec_target, LruEv *__restrict__ lev, unsigned long long *__restrict__ keys) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n_items) return;
+  if (!is_dec[q].x) return;
+  const int k = dec_pos[q].x;
+  const int e = meta[k].event;
+  if (e >= 0 && ev[e].type == MMP_CHURN_REAPER) return;  // (k_rp_route routes its decisions)
+  churn_route_one(k, (size_t)dec_pos[q].y, dec_in, dec_out, meta, max_instances, ev, now0, status, dec_target, lev, keys);
 }
 // per-instance ranges of the sorted event list
 __global__ void k_churn_offsets(const unsigned long long *__restrict__ keys, int n_keys, int n_inst, int *__restrict__ off) {
@@ -325,6 +350,238 @@ __global__ void k_churn_type_ok(const StatsAcc *__restrict__ acc, const int *__r
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// The reaper's proactive loads (MMP_CHURN_REAPER; MM:6456-6494, 6574-6577, 6616-6747), on the step's stream against the
+// window's snapshot: the stats of k_stats -> per-partition plan and PARTITION_STATS_COMP order (k_rp_plan) -> candidates
+// (k_rp_flag, compaction) -> one radix sort by (lastUsed desc, model asc) -> spaceToFill per partition (k_rp_space) -> one
+// block walks the sorted list per event and partition (k_rp_walk).  reaper_impl (scan_kernels.cuh) is the same arithmetic
+// with its host parts; the parity tests hold the two equal.
+// ---------------------------------------------------------------------------------------------------------------
+// one slot per partition (the whole cluster when the fleet has no type constraints), as run_stats reports them
+struct RpPart { long long cap, free, glru; int copies, count, size_est, pad; };
+struct RpPlan { int go, n_order; long long global_lru; };
+__device__ __forceinline__ long long rp_last_used(unsigned long long key) { return (long long)((~key) ^ 0x8000000000000000ull); }
+
+__global__ void k_rp_plan(const StatsAcc *__restrict__ acc, const long long *__restrict__ min_lru, int n_slots, int tc, int def_size,
+                          RpPart *__restrict__ parts, int *__restrict__ order, RpPlan *__restrict__ plan) {
+  const long long mn = *min_lru;
+  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) {
+    const StatsAcc a = acc[tc ? 1 + s : 0];
+    RpPart p{(long long)a.cap, (long long)a.free, (a.count > 0 || !tc) ? mn : 0x7fffffffffffffffLL, a.copies, a.count, 0, 0};
+    if (p.copies < 3) p.size_est = def_size;  // MM:6622-6629
+    else {
+      const int32_t avg = (int32_t)jsub(p.cap, p.free) / p.copies;
+      p.size_est = p.copies > 10 ? avg : jaddi(avg, def_size) / 2;
+    }
+    parts[s] = p;
+  }
+  __syncthreads();
+  // PARTITION_STATS_COMP (TCM:264-271) as partition_order: free desc, lru asc, capacity desc, partition id; with instances only
+  __shared__ int n_in;
+  if (threadIdx.x == 0) n_in = 0;
+  __syncthreads();
+  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) {
+    const RpPart x = parts[s];
+    if (tc && x.count == 0) continue;
+    int rank = 0;
+    for (int o = 0; o < n_slots; o++) {
+      const RpPart y = parts[o];
+      if (o == s || (tc && y.count == 0)) continue;
+      rank += y.free != x.free ? y.free > x.free : y.glru != x.glru ? y.glru < x.glru : y.cap != x.cap ? y.cap > x.cap : o < s;
+    }
+    order[rank] = s;
+    atomicAdd(&n_in, 1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {  // MM:6456-6463
+    plan->go = (long long)acc[0].cap > 0;
+    plan->global_lru = (long long)acc[0].free > 0 ? 0 : mn;
+    plan->n_order = n_in;
+  }
+}
+__global__ void k_rp_flag(const mmp_model_row *__restrict__ models, int n_models, const RpPlan *__restrict__ plan, uint8_t *__restrict__ flag) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n_models) return;
+  const RpPlan p = *plan;
+  flag[m] = p.go && reaper_candidate(models[m], p.global_lru) ? 1 : 0;
+}
+// sort keys of the compacted candidates (in model order); the positions past them sort last
+__global__ void k_rp_keys(const mmp_model_row *__restrict__ models, const int *__restrict__ idx, const int *__restrict__ n_cand, int n,
+                          unsigned long long *__restrict__ key) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  key[i] = i < *n_cand ? ~((unsigned long long)models[idx[i]].last_used ^ 0x8000000000000000ull) : ~0ull;
+}
+// spaceToFill (MM:6633-6649) per partition: one segmented reduction over the rank-ordered instance columns, in the reference's
+// wrapping int / long arithmetic (the sum wraps too, so the order of the additions does not matter)
+__global__ void k_rp_space(const RankRow *__restrict__ rows, const int64_t *__restrict__ cap_col, const int32_t *__restrict__ lthreads,
+                           const int32_t *__restrict__ linprog, const int32_t *__restrict__ part_of_rank, int n_ranks, int tc, int n_slots,
+                           const RpPart *__restrict__ parts, unsigned long long *__restrict__ space) {
+  __shared__ unsigned long long sacc[STATS_SMEM_PARTS + 1];
+  const bool use_smem = n_slots <= STATS_SMEM_PARTS + 1;
+  if (use_smem) for (int i = threadIdx.x; i < n_slots; i += blockDim.x) sacc[i] = 0ull;
+  __syncthreads();
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n_ranks; r += gridDim.x * blockDim.x) {
+    const int s = tc ? part_of_rank[r] : 0;
+    if (s < 0 || s >= n_slots) continue;
+    const int32_t max_loads = (int32_t)((uint32_t)jmuli(lthreads[r], 50) - (uint32_t)linprog[r]);
+    if (max_loads <= 0) continue;
+    const int64_t avail = jsub(rows[r].rem, cap_col[r] / 8);
+    if (avail <= 0) continue;
+    const int64_t lim = (int64_t)jmuli(max_loads, parts[s].size_est);
+    atomicAdd(use_smem ? &sacc[s] : &space[s], (unsigned long long)(avail < lim ? avail : lim));
+  }
+  if (use_smem) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_slots; i += blockDim.x) if (sacc[i]) atomicAdd(&space[i], sacc[i]);
+  }
+}
+// The selection of every REAPER event, one after the other, by one block: for each partition in order, the sorted candidates
+// are walked in chunks of RP_WALK.  Per chunk: eligible = not taken by this run, type allowed in the partition (MM:6681-6683)
+// and (free space or lastUsed > cutoff) (MM:6685-6688); of an equal-lastUsed run of eligible entries only the first counts
+// (N12; a block-wide max scan finds each entry's previous eligible entry); the counted entries take ranks k by a block-wide
+// sum scan, and the first totalProactiveLoadCount of them go through the emission rule (MM:6711-6719), which, the list
+// being in descending lastUsed, emits a prefix of them.  The walk stops at the count, at the rule's break, or (full
+// partition) at the first entry at or under the cutoff.  Emitted models are tagged taken and appended as (model, event).
+constexpr int RP_WALK = 1024;
+__global__ void __launch_bounds__(RP_WALK) k_rp_walk(const mmp_model_row *__restrict__ models, const unsigned long long *__restrict__ skey,
+                                                      const int *__restrict__ sidx, const int *__restrict__ n_cand, const RpPlan *__restrict__ plan,
+                                                      const RpPart *__restrict__ parts, const int *__restrict__ order,
+                                                      const unsigned long long *__restrict__ space, int tc, const int *__restrict__ pt_off,
+                                                      const int *__restrict__ pt_ids, const mmp_churn_event *__restrict__ ev,
+                                                      const int *__restrict__ rp_ev, int n_rp, int gen0, int *__restrict__ taken,
+                                                      int2 *__restrict__ sel, long long sel_cap, int *__restrict__ sel_off) {
+  using Scan = cub::BlockScan<int, RP_WALK>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ unsigned long long chunk_key[RP_WALK];
+  const int tid = threadIdx.x;
+  const int ncand = *n_cand;
+  const RpPlan P = *plan;
+  long long out = 0;
+  for (int r = 0; r < n_rp; r++) {
+    if (tid == 0) sel_off[r] = (int)out;
+    const int gen = gen0 + r;
+    const long long t = ev[rp_ev[r]].t;
+    for (int oi = 0; P.go && ncand > 0 && oi < P.n_order; oi++) {
+      const int s = order[oi];
+      const RpPart p = parts[s];
+      int free_count = 0, total = 0;
+      if (p.cap > 0 && p.free > 0) {  // MM:6621-6657
+        if (p.size_est == 0) break;   // spaceToFill / sizeEstimate throws (MM:6651): the run ends here
+        const long long fill = (long long)space[s] / 2;
+        free_count = (int32_t)(fill / p.size_est);
+        const long long d = (long long)(20ull * (unsigned long long)(long long)p.size_est);
+        const int32_t cap_count = d == 0 ? 0 : (int32_t)(d == -1 ? -p.cap : p.cap / d);
+        total = free_count > cap_count ? free_count : cap_count;
+      }
+      if (total <= 0) continue;
+      const long long a3 = age_of(p.glru, t) / 3;
+      const long long cutoff = p.glru == 0x7fffffffffffffffLL ? 0 : (long long)((unsigned long long)p.glru + (unsigned long long)(a3 > 1200000 ? a3 : 1200000));
+      const int *ex = tc ? pt_ids + pt_off[s] : nullptr;
+      const int nex = tc ? pt_off[s + 1] - pt_off[s] : 0;
+      int kept = 0, emitted = 0;
+      bool have_prev = false;
+      unsigned long long prev_key = 0;
+      for (int base = 0; base < ncand; base += RP_WALK) {
+        const int i = base + tid;
+        int m = -1;
+        unsigned long long key = ~0ull;
+        bool elig = false;
+        if (i < ncand) {
+          m = sidx[i]; key = skey[i];
+          elig = taken[m] != gen && (free_count > 0 || rp_last_used(key) > cutoff);
+          if (elig && nex) {  // the partition's prohibited type ids, sorted
+            const int ty = models[m].type_id;
+            int lo = 0, hi = nex;
+            while (lo < hi) { const int mid = (lo + hi) >> 1; if (ex[mid] < ty) lo = mid + 1; else hi = mid; }
+            elig = !(lo < nex && ex[lo] == ty);
+          }
+        }
+        chunk_key[tid] = key;
+        int prev, last;
+        Scan(tmp).ExclusiveScan(elig ? tid : -1, prev, -1, cub::Max(), last);
+        __syncthreads();
+        const bool hp = prev >= 0 || have_prev;
+        const unsigned long long pk = prev >= 0 ? chunk_key[prev] : prev_key;
+        const int first = elig && !(hp && pk == key) ? 1 : 0;
+        int j, n_first;
+        Scan(tmp).ExclusiveSum(first, j, n_first);
+        const int k = kept + j;
+        const bool emit = first && k < total && (k < free_count || !(rp_last_used(key) < cutoff));
+        const int n_emit = __syncthreads_count(emit);
+        if (emit) {
+          taken[m] = gen;
+          const long long pos = out + k;
+          if (pos < sel_cap) sel[pos] = make_int2(m, r);
+        }
+        kept += n_first; emitted += n_emit;
+        if (last >= 0) { have_prev = true; prev_key = chunk_key[last]; }
+        bool stop = n_emit < n_first || kept >= total || base + RP_WALK >= ncand;
+        if (free_count == 0 && rp_last_used(chunk_key[RP_WALK - 1]) <= cutoff) stop = true;  // nothing eligible past it
+        __syncthreads();
+        if (stop) break;
+      }
+      out += emitted;
+    }
+  }
+  if (tid == 0) sel_off[n_rp] = (int)out;
+}
+// the window's items see the selections at their REAPER's position: first decisions (k_churn_first's rule), flags, records
+__global__ void k_rp_first(const int2 *__restrict__ sel, int n_sel, const int *__restrict__ rp_ev, int n_follow, int *__restrict__ first_ev) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_sel) return;
+  const int2 x = sel[s];
+  atomicMin(&first_ev[x.x], n_follow + rp_ev[x.y]);
+}
+__global__ void k_rp_mark(const int2 *__restrict__ sel, int n_sel, const int *__restrict__ rp_ev, int n_follow, const int *__restrict__ first_ev,
+                          int *__restrict__ flag, int *__restrict__ counters) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s > n_sel) return;
+  if (s == n_sel) { flag[s] = 0; return; }
+  const int2 x = sel[s];
+  const int f = first_ev[x.x] == n_follow + rp_ev[x.y];
+  flag[s] = f;
+  if (!f) atomicAdd(&counters[3], 1);  // coalesced
+}
+// decision k and event slot of selection s (which must be a first decision)
+__device__ __forceinline__ int2 rp_dec_slot(const RpView &rp, int s, int r, const int2 *__restrict__ dec_pos, int n_follow) {
+  const int2 p = dec_pos[n_follow + rp.ev_idx[r]];
+  const int j = rp.fpos[s] - rp.fpos[rp.off[r]];
+  return make_int2(p.x + j, p.y + j);
+}
+__global__ void k_rp_emit(const int2 *__restrict__ sel, int n_sel, const int *__restrict__ flag, RpView rp, int n_follow,
+                          const mmp_churn_event *__restrict__ ev, const mmp_model_row *__restrict__ models, const int2 *__restrict__ dec_pos,
+                          mmp_decision_in *__restrict__ dec_in, DecMeta *__restrict__ meta, int32_t *__restrict__ extra,
+                          int *__restrict__ status, int *__restrict__ dec_of_model) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_sel || !flag[s]) return;
+  const int2 x = sel[s];
+  const int k = rp_dec_slot(rp, s, x.y, dec_pos, n_follow).x, e = rp.ev_idx[x.y];
+  const mmp_model_row r = models[x.x];
+  mmp_decision_in d;  // getNext(model, self = leader, lastUsed = the model's), UNBALANCED_KEY: no flags (MM:6727, 6940-6943)
+  d.flags = 0; d.fresh = -1; d.extra_off = k; d.extra_n = 0;
+  d.model = x.x; d.self = ev[e].caller; d.last_used = r.last_used;
+  dec_in[k] = d;
+  extra[k] = -1;
+  meta[k] = DecMeta{e, r.size_units, n_follow + e, -1};
+  status[k] = CH_INVALID;
+  dec_of_model[x.x] = k;
+}
+__global__ void k_rp_route(const int2 *__restrict__ sel, int n_sel, const int *__restrict__ flag, RpView rp, int n_follow,
+                           const int2 *__restrict__ dec_pos, const mmp_decision_in *__restrict__ dec_in,
+                           const mmp_decision_out *__restrict__ dec_out, const DecMeta *__restrict__ meta, int max_instances,
+                           const mmp_churn_event *__restrict__ ev, long long now0, int *__restrict__ status, int *__restrict__ dec_target,
+                           LruEv *__restrict__ lev, unsigned long long *__restrict__ keys) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_sel || !flag[s]) return;
+  const int2 ks = rp_dec_slot(rp, s, sel[s].y, dec_pos, n_follow);
+  churn_route_one(ks.x, (size_t)ks.y, dec_in, dec_out, meta, max_instances, ev, now0, status, dec_target, lev, keys);
+}
+__global__ void k_rp_reset(const int2 *__restrict__ sel, int n_sel, int *__restrict__ first_ev) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < n_sel) first_ev[sel[s].x] = 0x7fffffff;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
 static int32_t commit_locked(mmp_fleet *f);  // mmplace.cu: mmp_fleet_commit without taking the ingest lock
@@ -374,6 +631,81 @@ static int32_t churn_relay_ovf(mmp_fleet *f, cudaStream_t st) {
   std::swap(lv.ovf, cs.ovf_next);
   lv.n_ovf = total;
   return MMP_OK;
+}
+
+// The reaper pass of a window with REAPER events (rp_ev: their trace indices), after k_stats filled acc / min_lru: every
+// event's selections in cs.rp_sel as (model, event) in emission order, cs.rp_ev = [rp_ev | selection offsets].  The total is
+// read back (the window's one synchronisation for it: the decision buffers are sized from it); a second walk follows only
+// when several events selected more models in all than the fleet has.
+static int32_t churn_reaper_pass(mmp_fleet *f, const DeviceSnapshot &ds, const StatsAcc *acc, const long long *min_lru,
+                                 const std::vector<int> &rp_ev, cudaStream_t st, int32_t *n_sel) {
+  ChurnState &cs = f->churn;
+  const HostSnapshot &h = ds.host;
+  const int NM = f->hs.n_models_used, R = (int)rp_ev.size(), tc = h.tc_enabled ? 1 : 0;
+  const int ns = tc ? (int)h.part_types.size() : 1;
+  const size_t nmx = (size_t)std::max(NM, 1);
+  // each partition's prohibited type ids of this epoch (reaper_impl's `excl`), sorted: [offsets (ns + 1) | ids]
+  std::vector<int> pt((size_t)ns + 1, 0);
+  for (int p = 0; tc && p < ns; p++) {
+    std::vector<int> ids;
+    for (int32_t tid : h.part_type_ids[p]) if (tid >= 0 && tid < (int32_t)h.type_slot.size()) ids.push_back(tid);
+    std::sort(ids.begin(), ids.end());
+    pt.insert(pt.end(), ids.begin(), ids.end());
+    pt[p + 1] = pt[p] + (int)ids.size();
+  }
+  std::vector<int> evo(rp_ev);
+  evo.resize((size_t)2 * R + 1, 0);
+  CK(upload_vec(cs.rp_pt, pt, st));
+  CK(upload_vec(cs.rp_ev, evo, st));
+  CK(cs.rp_keys.ensure(nmx * 16)); CK(cs.rp_idx.ensure(nmx * 8 + 16)); CK(cs.rp_flag.ensure(nmx));
+  CK(cs.rp_sel.ensure(nmx * sizeof(int2)));  // (one event selects each model at most once)
+  const size_t parts_b = (size_t)ns * sizeof(RpPart), space_b = (size_t)ns * 8;
+  CK(cs.rp_plan.ensure(parts_b + space_b + sizeof(RpPlan) + (size_t)ns * 4 + 16));
+  const size_t taken_cap = cs.rp_taken.cap;
+  CK(cs.rp_taken.ensure(nmx * 4));
+  if (cs.rp_taken.cap != taken_cap || cs.rp_gen > INT32_MAX / 2) {  // tags start over on a zeroed array
+    CK(cudaMemsetAsync(cs.rp_taken.p, 0, cs.rp_taken.cap, st));
+    cs.rp_gen = 0;
+  }
+  RpPart *parts = cs.rp_plan.as<RpPart>();
+  unsigned long long *space = reinterpret_cast<unsigned long long *>(cs.rp_plan.as<char>() + parts_b);
+  RpPlan *plan = reinterpret_cast<RpPlan *>(cs.rp_plan.as<char>() + parts_b + space_b);
+  int *order = reinterpret_cast<int *>(plan + 1);
+  unsigned long long *keys = cs.rp_keys.as<unsigned long long>(), *skeys = keys + nmx;
+  int *idx = cs.rp_idx.as<int>(), *sidx = idx + nmx, *d_n = sidx + nmx;
+  CK(cudaMemsetAsync(space, 0, space_b, st));
+  k_rp_plan<<<1, 256, 0, st>>>(acc, min_lru, ns, tc, f->hs.cfg.default_model_size_units, parts, order, plan);
+  k_rp_flag<<<(int)((nmx + 255) / 256), 256, 0, st>>>(f->live.models.as<mmp_model_row>(), NM, plan, cs.rp_flag.as<uint8_t>());
+  thrust::counting_iterator<int32_t> iota(0);
+  size_t t1 = 0, t2 = 0;
+  CK(cub::DeviceSelect::Flagged(nullptr, t1, iota, cs.rp_flag.as<uint8_t>(), idx, d_n, NM, st));
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, t2, keys, skeys, idx, sidx, NM, 0, 64, st));
+  CK(cs.cub_tmp.ensure(std::max(t1, t2) + 16));
+  CK(cub::DeviceSelect::Flagged(cs.cub_tmp.p, t1, iota, cs.rp_flag.as<uint8_t>(), idx, d_n, NM, st));
+  k_rp_keys<<<(int)((nmx + 255) / 256), 256, 0, st>>>(f->live.models.as<mmp_model_row>(), idx, d_n, NM, keys);
+  CK(cub::DeviceRadixSort::SortPairs(cs.cub_tmp.p, t2, keys, skeys, idx, sidx, NM, 0, 64, st));
+  if (h.n_ranks > 0)
+    k_rp_space<<<std::min(f->sm_count, (h.n_ranks + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(),
+                                                                            ds.lthreads_col.as<int32_t>(), ds.linprog_col.as<int32_t>(),
+                                                                            ds.part_of_rank.as<int32_t>(), h.n_ranks, tc, ns, parts, space);
+  f->launches += 6 + (h.n_ranks > 0);
+  CK(cudaGetLastError());
+  int *d_off = cs.rp_ev.as<int>() + R;
+  for (int pass = 0;; pass++) {
+    const long long sel_cap = (long long)(cs.rp_sel.cap / sizeof(int2));
+    k_rp_walk<<<1, RP_WALK, 0, st>>>(f->live.models.as<mmp_model_row>(), skeys, sidx, d_n, plan, parts, order, space, tc,
+                                     cs.rp_pt.as<int>(), cs.rp_pt.as<int>() + ns + 1, cs.ev.as<mmp_churn_event>(), cs.rp_ev.as<int>(), R,
+                                     cs.rp_gen + 1, cs.rp_taken.as<int>(), cs.rp_sel.as<int2>(), sel_cap, d_off);
+    f->launches++;
+    CK(cudaGetLastError());
+    cs.rp_gen += R;
+    int total = 0;
+    CK(cudaMemcpyAsync(&total, d_off + R, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (total <= sel_cap) { *n_sel = total; return MMP_OK; }
+    if (pass) { g_err = "internal: the reaper's selections changed between two walks"; return MMP_E_STATE; }
+    CK(cs.rp_sel.ensure((size_t)total * sizeof(int2)));
+  }
 }
 
 extern "C" {
@@ -493,20 +825,19 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   }
   // event slots: one per decision or cache hit, one per loaded copy of a REMOVE's model
   size_t n_remove = 0;
-  for (int32_t i = 0; i < n; i++) n_remove += ev[i].type == 1;
-  const size_t QQ = (size_t)std::max(Q, 1), NK = QQ + n_remove * (size_t)(cs.max_copies - 1);
-  if (NK > (size_t)INT32_MAX) { g_err = "too many cache events in one window"; return MMP_E_ARG; }
+  std::vector<int> rp_ev;  // the REAPER events
+  for (int32_t i = 0; i < n; i++) {
+    n_remove += ev[i].type == 1;
+    if (ev[i].type == MMP_CHURN_REAPER) rp_ev.push_back(i);
+  }
+  const int n_rp = (int)rp_ev.size();
+  const size_t QQ = (size_t)std::max(Q, 1);
   // the window's marks may reach an overflow registration (a model with more than four), or its registry phase may push a
   // model with four failed loads past four: then the registry phase reads the mark flag back and re-lays lv.ovf
   const bool ovf_window = lv.n_ovf > 0 || cs.deep_failed;
   if (lv.n_ovf > 0) CK(cs.ovf_dead.ensure((size_t)lv.n_ovf));
   CK(cs.ev.ensure(QQ * sizeof(mmp_churn_event))); CK(cs.is_dec.ensure(QQ * 8 + 16)); CK(cs.dec_pos.ensure(QQ * 8 + 16));
-  CK(cs.dec_in.ensure(QQ * sizeof(mmp_decision_in))); CK(cs.dec_out.ensure(QQ * sizeof(mmp_decision_out)));
-  CK(cs.dec_meta.ensure(QQ * sizeof(DecMeta))); CK(cs.dec_target.ensure(QQ * 4)); CK(cs.extra.ensure(QQ * 4)); CK(cs.status.ensure(QQ * 4));
-  CK(cs.lev.ensure(NK * sizeof(LruEv))); CK(cs.keys.ensure(NK * 8)); CK(cs.vals.ensure(NK * 4)); CK(cs.keys2.ensure(NK * 8)); CK(cs.vals2.ensure(NK * 4));
   CK(cs.off.ensure((size_t)(NI + 2) * 4));
-  const int32_t ecap = (int32_t)std::min<size_t>(4 * QQ + 65536, (size_t)1 << 26);
-  CK(cs.evict.ensure((size_t)ecap * sizeof(EvictRec))); CK(cs.next_carry.ensure((size_t)ecap * sizeof(Follow)));
   CK(cs.stats_acc.ensure(((size_t)ds.host.part_types.size() + 2) * sizeof(StatsAcc) + 16));
   CK(cudaEventRecord(evs[0], st));
   if (n) CK(cudaMemcpyAsync(cs.ev.p, ev, (size_t)n * sizeof(mmp_churn_event), cudaMemcpyHostToDevice, st));
@@ -514,11 +845,16 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   CK(cudaMemsetAsync(cs.force_publish.p, 0, (size_t)NI, st));
   if (lv.n_ovf > 0) CK(cudaMemsetAsync(cs.ovf_dead.p, 0, (size_t)lv.n_ovf, st));
   // ---- the rebalance rule's fullness test reads the stats of the window's snapshot (MM:2918-2920) ----
+  int32_t n_sel = 0;  // the reaper's selections (one decision each at most)
   {
     const int np = (int)ds.host.part_types.size();
     const size_t bytes = (size_t)(np + 1) * sizeof(StatsAcc) + 8;
     CK(cudaMemsetAsync(cs.stats_acc.p, 0, bytes, st));
     long long *d_min = reinterpret_cast<long long *>(cs.stats_acc.as<char>() + (size_t)(np + 1) * sizeof(StatsAcc));
+    if (n_rp) {  // the reaper reads the cluster's LRU too: start it at Long.MAX_VALUE (ISST)
+      CK(cudaMemsetAsync(d_min, 0xff, 7, st));
+      CK(cudaMemsetAsync(reinterpret_cast<char *>(d_min) + 7, 0x7f, 1, st));
+    }
     if (ds.host.n_ranks > 0) {
       k_stats<<<std::min(f->sm_count, (ds.host.n_ranks + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(),
                                                                                   ds.part_of_rank.as<int32_t>(), ds.host.n_ranks,
@@ -529,36 +865,71 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
                                                                 lv.n_type_ids, cs.type_ok.as<unsigned char>());
     f->launches++;
     CK(cudaGetLastError());
+    // ---- the reaper's proactive loads: selections of the window's REAPER events (then one read-back of their count) ----
+    if (n_rp) {
+      CK(cudaEventRecord(evs[7], st));
+      rc = churn_reaper_pass(f, ds, cs.stats_acc.as<StatsAcc>(), d_min, rp_ev, st, &n_sel);
+      if (rc < 0) return rc;
+      CK(cudaEventRecord(evs[8], st));
+    }
   }
-  const int qb = (Q + 255) / 256;
+  // decision records: one per item, one more per selection of the reaper (at most: the coalesced ones stay malformed)
+  const size_t QD = QQ + (size_t)n_sel, NK = QD + n_remove * (size_t)(cs.max_copies - 1);
+  if (NK > (size_t)INT32_MAX) { g_err = "too many cache events in one window"; return MMP_E_ARG; }
+  CK(cs.dec_in.ensure(QD * sizeof(mmp_decision_in))); CK(cs.dec_out.ensure(QD * sizeof(mmp_decision_out)));
+  CK(cs.dec_meta.ensure(QD * sizeof(DecMeta))); CK(cs.dec_target.ensure(QD * 4)); CK(cs.extra.ensure(QD * 4)); CK(cs.status.ensure(QD * 4));
+  CK(cs.lev.ensure(NK * sizeof(LruEv))); CK(cs.keys.ensure(NK * 8)); CK(cs.vals.ensure(NK * 4)); CK(cs.keys2.ensure(NK * 8)); CK(cs.vals2.ensure(NK * 4));
+  const int32_t ecap = (int32_t)std::min<size_t>(4 * QD + 65536, (size_t)1 << 26);
+  CK(cs.evict.ensure((size_t)ecap * sizeof(EvictRec))); CK(cs.next_carry.ensure((size_t)ecap * sizeof(Follow)));
+  const int qb = (Q + 255) / 256, qdb = (int)((QD + 255) / 256), sb = (n_sel + 255) / 256;
+  const int QDi = Q + n_sel;  // (decisions placed / collected: == Q without REAPER events)
   const mmp_model_row *lmodels = lv.models.as<mmp_model_row>();
   const Follow *carry = cs.carry.as<Follow>();
   const RegTables R{lv.edges.as<int4>(), nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
+  if (n_sel) CK(cs.rp_fpos.ensure((size_t)(n_sel + 1) * 8));
+  const int2 *sel = cs.rp_sel.as<int2>();
+  int *sel_flag = cs.rp_fpos.as<int>(), *sel_fpos = sel_flag + n_sel + 1;  // first-decision flags, their exclusive scan
+  const RpView rp{cs.rp_ev.as<int>(), n_rp, cs.rp_ev.as<int>() + n_rp, n_sel ? sel_fpos : nullptr};
   bool relaid = false;
   if (Q > 0) {
     // ---- A: classify ----
     k_churn_first<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, NM, cs.first_ev.as<int>());
+    if (n_sel) {  // the reaper's selections take part in the first-miss rule at their event's position
+      k_rp_first<<<sb, 256, 0, st>>>(sel, n_sel, rp.ev_idx, nF, cs.first_ev.as<int>());
+      k_rp_mark<<<(n_sel + 1 + 255) / 256, 256, 0, st>>>(sel, n_sel, rp.ev_idx, nF, cs.first_ev.as<int>(), sel_flag, cs.counters.as<int>());
+      size_t t = 0;
+      CK(cub::DeviceScan::ExclusiveSum(nullptr, t, sel_flag, sel_fpos, n_sel + 1, st));
+      CK(cs.cub_tmp.ensure(t + 16));
+      CK(cub::DeviceScan::ExclusiveSum(cs.cub_tmp.p, t, sel_flag, sel_fpos, n_sel + 1, st));
+      f->launches += 3;
+    }
     k_churn_flag<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, NM, cs.first_ev.as<int>(), cs.is_dec.as<int2>(),
-                                    cs.used_t.as<long long>(), cs.counters.as<int>());
+                                    cs.used_t.as<long long>(), cs.counters.as<int>(), rp);
     size_t tmp = 0;
     CK(cub::DeviceScan::ExclusiveScan(nullptr, tmp, cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), Int2Sum(), make_int2(0, 0), Q, st));
     CK(cs.cub_tmp.ensure(tmp + 16));
     CK(cub::DeviceScan::ExclusiveScan(cs.cub_tmp.p, tmp, cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), Int2Sum(), make_int2(0, 0), Q, st));
     // decision records beyond the window's count stay malformed (model -1): the scoring kernel answers them INVALID
-    CK(cudaMemsetAsync(cs.dec_in.p, 0xff, QQ * sizeof(mmp_decision_in), st));
-    CK(cudaMemsetAsync(cs.status.p, 0, QQ * 4, st));
+    CK(cudaMemsetAsync(cs.dec_in.p, 0xff, QD * sizeof(mmp_decision_in), st));
+    CK(cudaMemsetAsync(cs.status.p, 0, QD * 4, st));
     k_churn_emit<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, lmodels, R, NM, NI, cs.first_ev.as<int>(),
                                     cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), cs.dec_in.as<mmp_decision_in>(), cs.dec_meta.as<DecMeta>(),
                                     cs.extra.as<int32_t>(), cs.status.as<int>(), cs.dec_of_model.as<int>(), cs.lev.as<LruEv>(),
                                     cs.keys.as<unsigned long long>(), now0);
     f->launches += 5;
+    if (n_sel) {
+      k_rp_emit<<<sb, 256, 0, st>>>(sel, n_sel, sel_flag, rp, nF, cs.ev.as<mmp_churn_event>(), lmodels, cs.dec_pos.as<int2>(),
+                                    cs.dec_in.as<mmp_decision_in>(), cs.dec_meta.as<DecMeta>(), cs.extra.as<int32_t>(), cs.status.as<int>(),
+                                    cs.dec_of_model.as<int>());
+      f->launches++;
+    }
     CK(cudaGetLastError());
     CK(cudaEventRecord(evs[1], st));
     // ---- B: placement of the window's decisions against the committed snapshot (one clock for the batch: now0) ----
     SnapshotView vw = ds.view;
-    vw.n_extra = Q;
+    vw.n_extra = QDi;
     CK(c->d_fresh.ensure(sizeof(FreshRow)));
-    PlaceArgs a{vw, cs.dec_in.as<mmp_decision_in>(), Q, c->d_fresh.as<FreshRow>(), 0, cs.extra.as<int32_t>(), cs.dec_out.as<mmp_decision_out>(),
+    PlaceArgs a{vw, cs.dec_in.as<mmp_decision_in>(), QDi, c->d_fresh.as<FreshRow>(), 0, cs.extra.as<int32_t>(), cs.dec_out.as<mmp_decision_out>(),
                 nullptr, nullptr, now0, seed, 0};
     CK(launch_place(f, a, st));
     CK(cudaEventRecord(evs[2], st));
@@ -566,6 +937,12 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
     k_churn_route<<<qb, 256, 0, st>>>(cs.dec_in.as<mmp_decision_in>(), cs.dec_out.as<mmp_decision_out>(), cs.dec_meta.as<DecMeta>(),
                                      cs.is_dec.as<int2>(), cs.dec_pos.as<int2>(), Q, NI, cs.ev.as<mmp_churn_event>(), now0, cs.status.as<int>(),
                                      cs.dec_target.as<int>(), cs.lev.as<LruEv>(), cs.keys.as<unsigned long long>());
+    if (n_sel) {
+      k_rp_route<<<sb, 256, 0, st>>>(sel, n_sel, sel_flag, rp, nF, cs.dec_pos.as<int2>(), cs.dec_in.as<mmp_decision_in>(),
+                                     cs.dec_out.as<mmp_decision_out>(), cs.dec_meta.as<DecMeta>(), NI, cs.ev.as<mmp_churn_event>(), now0,
+                                     cs.status.as<int>(), cs.dec_target.as<int>(), cs.lev.as<LruEv>(), cs.keys.as<unsigned long long>());
+      f->launches++;
+    }
     k_churn_tail<<<(int)((NK + 255) / 256), 256, 0, st>>>(cs.keys.as<unsigned long long>(), cs.vals.as<int>(), (int)NK, cs.is_dec.as<int2>(),
                                                           cs.dec_pos.as<int2>(), Q);
     tmp = 0;
@@ -598,9 +975,10 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
     CK(cudaGetLastError());
     CK(cudaEventRecord(evs[4], st));
     // ---- D: registry ----
-    k_churn_collect_adds<<<qb, 256, 0, st>>>(cs.dec_in.as<mmp_decision_in>(), cs.status.as<int>(), cs.dec_target.as<int>(), Q, cs.add_inst.as<int>(),
-                                            cs.dec_of_model.as<int>());
+    k_churn_collect_adds<<<qdb, 256, 0, st>>>(cs.dec_in.as<mmp_decision_in>(), cs.status.as<int>(), cs.dec_target.as<int>(), QDi, cs.add_inst.as<int>(),
+                                             cs.dec_of_model.as<int>());
     k_churn_reset_first<<<qb, 256, 0, st>>>(carry, nF, cs.ev.as<mmp_churn_event>(), n, NM, cs.first_ev.as<int>());
+    if (n_sel) { k_rp_reset<<<sb, 256, 0, st>>>(sel, n_sel, cs.first_ev.as<int>()); f->launches++; }
     k_churn_registry<<<(NM + 255) / 256, 256, 0, st>>>(lv.models.as<mmp_model_row>(), lv.edges.as<int4>(), NM, cs.rm_mask.as<unsigned>(),
                                                       cs.add_inst.as<int>(), cs.used_t.as<long long>(), cs.counters.as<int>());
     f->launches += 3;
@@ -683,11 +1061,13 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   float ms[7] = {0, 0, 0, 0, 0, 0, 0};
   for (int i = 0; i < 6; i++) cudaEventElapsedTime(&ms[i], evs[i], evs[i + 1]);
   cudaEventElapsedTime(&ms[6], evs[0], evs[6]);
+  float ms_reaper = 0;  // (inside the classify interval: taken out of it)
+  if (n_rp) { cudaEventElapsedTime(&ms_reaper, evs[7], evs[8]); ms[0] -= ms_reaper; }
   cs.t_classify = ms[0]; cs.t_place = ms[1]; cs.t_route = ms[2]; cs.t_apply = ms[3]; cs.t_registry = ms[4]; cs.t_commit = ms[5]; cs.t_total = ms[6];
   if (report) {
     report->n_published = hdr[1]; report->n_carry = n_next; report->n_coalesced = hdr[3]; report->n_lru_events = 0;
     report->ms_classify = ms[0]; report->ms_place = ms[1]; report->ms_route = ms[2]; report->ms_apply = ms[3]; report->ms_registry = ms[4];
-    report->ms_commit = ms[5]; report->ms_total = ms[6];
+    report->ms_commit = ms[5]; report->ms_total = ms[6]; report->ms_reaper = ms_reaper;
     int noff = 0;
     if (Q > 0 && cudaMemcpy(&noff, cs.off.as<int>() + NI, 4, cudaMemcpyDeviceToHost) == cudaSuccess) report->n_lru_events = noff;
   }

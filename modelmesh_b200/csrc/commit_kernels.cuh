@@ -70,6 +70,11 @@ struct ChurnState {
   DevBuf ev, is_dec, dec_pos, dec_in, dec_out, dec_meta, dec_target, extra, status, lev, keys, vals, keys2, vals2, cub_tmp, off, evict, fkeys,
       fvals, rows_changed;
   DevBuf ovf_dead, ovf_next, ovf_count;  // the registry phase's re-lay of LiveState::ovf (churn_kernels.cuh)
+  // the reaper pass of a window with MMP_CHURN_REAPER events (churn_kernels.cuh): sort keys / model indices, the per-partition
+  // plan, the partitions' prohibited type ids, the events' selections and their first-decision flags; rp_taken[m] holds the tag
+  // of the last reaper run that selected model m (tags grow across windows: no reset per run)
+  DevBuf rp_keys, rp_idx, rp_flag, rp_plan, rp_pt, rp_ev, rp_sel, rp_fpos, rp_taken;
+  int32_t rp_gen = 0;
   int32_t n_carry = 0;
   // what the step's host side knows of the registry without reading it back: the loop only removes loaded copies or loads the
   // first one of a model without any, so the largest copy count does not grow past max(it, 1) and the failed loads of a model
@@ -77,7 +82,7 @@ struct ChurnState {
   bool regs_from_host = true, deep_failed = false;
   int32_t max_copies = 1;
   // last step's phase timings (ms, between these events on the step's stream; created by mmp_churn_init)
-  Event phase_ev[7];
+  Event phase_ev[9];  // [7], [8]: around the reaper pass
   float t_classify = 0, t_place = 0, t_route = 0, t_apply = 0, t_registry = 0, t_commit = 0, t_total = 0;
   int32_t last_lru_events = 0;
 };

@@ -106,6 +106,11 @@ static std::vector<int> partition_order(const StatsResult &res) {
 // Reaper: registry sweep (MM:6536-6590 candidate rule MM:6574-6577) + bounded most-recently-used selection
 // (MM:6675-6698) as  flag/compact -> bitonic sort by (lastUsed desc, model asc) -> first-of-run.
 // ---------------------------------------------------------------------------------------------------------------
+// the candidate rule of the registry sweep (MM:6574-6577): no loaded copy, fewer than 2 failed loads, used after globalLru
+// (0 when the cluster has free space)
+__device__ __forceinline__ bool reaper_candidate(const mmp_model_row &r, long long global_lru) {
+  return r.copy_count == 0 && r.fail_count < 2 && (global_lru == 0 || r.last_used > global_lru);
+}
 // key: ~biased(lastUsed), so that ascending keys = descending time.  One thread per model: 24 B read, 1 + 8 B written.
 __global__ void k_reaper_flag(const mmp_model_row *__restrict__ models, int n_models, const uint8_t *__restrict__ type_excluded,
                               int n_type_ids, const uint8_t *__restrict__ taken, long long global_lru, int need_cutoff,
@@ -113,7 +118,7 @@ __global__ void k_reaper_flag(const mmp_model_row *__restrict__ models, int n_mo
   int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= n_models) return;
   mmp_model_row r = models[m];
-  bool ok = r.copy_count == 0 && r.fail_count < 2 && (global_lru == 0 || r.last_used > global_lru);  // MM:6574-6577
+  bool ok = reaper_candidate(r, global_lru);                                                         // MM:6574-6577
   if (ok && taken && taken[m]) ok = false;                                                           // allCandidates.set(i, null)
   if (ok && r.type_id < n_type_ids && type_excluded[r.type_id]) ok = false;                          // MM:6681-6683
   if (ok && need_cutoff && !(r.last_used > cutoff)) ok = false;                                      // MM:6685-6687

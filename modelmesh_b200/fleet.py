@@ -12,8 +12,8 @@ from typing import Iterable, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CLUSTER_STATS, DECISION_IN, DECISION_OUT, DECISION_TRACE, EVICTION,
-                   INSTANCE_ROW, LRU_ENTRY, LRU_EVENT, MODEL_ROW, ChurnConfig, ChurnReport, MmpConfig)
+from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CHURN_REAPER, CLUSTER_STATS, DECISION_IN, DECISION_OUT,
+                   DECISION_TRACE, EVICTION, INSTANCE_ROW, LRU_ENTRY, LRU_EVENT, MODEL_ROW, ChurnConfig, ChurnReport, MmpConfig)
 
 
 class MmpError(RuntimeError):
@@ -295,8 +295,10 @@ class Fleet:
 
     def churn_step(self, events: np.ndarray, now0: int, now1: int, seed: int, want_rows: bool = True):
         ev = np.ascontiguousarray(events, dtype=CHURN_EVENT)
-        cap_d = len(ev) + 65536
-        cap_e = 4 * len(ev) + 65536
+        # (a CHURN_REAPER event decides up to one load per model)
+        n_rp = int(np.count_nonzero(ev["type"] == CHURN_REAPER)) * self.max_models
+        cap_d = len(ev) + 65536 + n_rp
+        cap_e = 4 * (len(ev) + n_rp) + 65536
         dec = np.zeros(cap_d, dtype=CHURN_DECISION)
         evi = np.zeros(cap_e, dtype=CHURN_EVICTION)
         rows = np.zeros(self.max_instances, dtype=INSTANCE_ROW) if want_rows else None
