@@ -584,18 +584,26 @@ __global__ void k_rp_reset(const int2 *__restrict__ sel, int n_sel, int *__restr
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-static int32_t commit_locked(mmp_fleet *f);  // mmplace.cu: mmp_fleet_commit without taking the ingest lock
+static int32_t commit_locked(mmp_fleet *f, bool rows_on_device);  // mmplace.cu: mmp_fleet_commit without taking the ingest lock
 static inline int32_t lv_n_types(mmp_fleet *f) { return f->live.n_type_ids; }
 
-static int32_t sync_host_from_device(mmp_fleet *f) {
+// rows: also take every present instance's row from lv.inst_rows (inside a window, after its republish; the caller makes sure
+// no host row holds an update the device has not seen).  The copies go on the commit stream, behind the window's kernels.
+static int32_t sync_host_from_device(mmp_fleet *f, bool rows) {
   HostState &hs = f->hs;
-  const int32_t nm = hs.n_models_used;
+  cudaStream_t st = f->commit_stream;
+  const int32_t nm = hs.n_models_used, NI = hs.cfg.max_instances;
   std::vector<OvfEdge> ovf((size_t)f->live.n_ovf);
+  std::vector<mmp_instance_row> inst_rows(rows ? (size_t)NI : 0);
   if (nm) {
-    CK(cudaMemcpy(hs.models.data(), f->live.models.p, (size_t)nm * sizeof(mmp_model_row), cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(hs.edge_inl.data(), f->live.edges.p, (size_t)nm * HostState::EDGE_INL * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpyAsync(hs.models.data(), f->live.models.p, (size_t)nm * sizeof(mmp_model_row), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(hs.edge_inl.data(), f->live.edges.p, (size_t)nm * HostState::EDGE_INL * 4, cudaMemcpyDeviceToHost, st));
   }
-  if (!ovf.empty()) CK(cudaMemcpy(ovf.data(), f->live.ovf.p, ovf.size() * sizeof(OvfEdge), cudaMemcpyDeviceToHost));
+  if (!ovf.empty()) CK(cudaMemcpyAsync(ovf.data(), f->live.ovf.p, ovf.size() * sizeof(OvfEdge), cudaMemcpyDeviceToHost, st));
+  if (rows) CK(cudaMemcpyAsync(inst_rows.data(), f->live.inst_rows.p, (size_t)NI * sizeof(mmp_instance_row), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (rows)
+    for (int32_t i = 0; i < NI; i++) if (hs.inst[i].present) hs.inst[i].row = inst_rows[i];
   // the overflow registrations as the loop left them: models that went back inline lose their entries
   hs.edge_ovf.clear(); hs.edge_ovf_ts.clear();
   for (const OvfEdge &e : ovf) { hs.edge_ovf[e.model].push_back(e.inst); hs.edge_ovf_ts[e.model].push_back(e.ts); }
@@ -999,9 +1007,10 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   f->launches++;
   CK(cudaGetLastError());
   CK(cudaEventRecord(evs[5], st));
-  // ---- commit: the device path (re-rank, tables, bitmap from the device-resident edges) ----
+  // ---- commit: the device path (re-rank, tables, bitmap from the device-resident edges); the host path, when the fleet
+  // needs it, from the device's registry and instance rows ----
   f->device_ahead = true;
-  rc = commit_locked(f);
+  rc = commit_locked(f, true);
   if (rc < 0) return rc;
   CK(cudaEventRecord(evs[6], st));
   // ---- reports ----

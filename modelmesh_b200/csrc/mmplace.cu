@@ -2130,16 +2130,17 @@ static int32_t host_mirror(mmp_fleet *f, const DeviceSnapshot &cds, const HostSn
   return MMP_OK;
 }
 
-static int32_t sync_host_from_device(mmp_fleet *f);  // churn_kernels.cuh: registry changes made on the device -> host tables
-static int32_t commit_locked(mmp_fleet *f);
+static int32_t sync_host_from_device(mmp_fleet *f, bool rows);  // churn_kernels.cuh: closed-loop changes on the device -> host tables
+static int32_t commit_locked(mmp_fleet *f, bool rows_on_device);
 
 int32_t mmp_fleet_commit(mmp_fleet *f) {
   NEED(f);
   std::lock_guard<std::mutex> g(f->ingest_mu);
-  return commit_locked(f);
+  return commit_locked(f, false);
 }
 }  // extern "C"
-static int32_t commit_locked(mmp_fleet *f) {
+// rows_on_device: called by mmp_churn_step after its republish, when lv.inst_rows is ahead of the host's instance rows
+static int32_t commit_locked(mmp_fleet *f, bool rows_on_device) {
   int32_t rc = set_device(f);
   if (rc < 0) return rc;
   const auto t0 = std::chrono::steady_clock::now();
@@ -2147,13 +2148,19 @@ static int32_t commit_locked(mmp_fleet *f) {
   cudaStream_t st = f->commit_stream;
   LiveState &lv = f->live;
   bool structural = f->hs.structural_dirty || !lv.valid || f->commit_host_only;
-  if (structural && f->device_ahead) { rc = sync_host_from_device(f); if (rc < 0) return rc; }
   if (!structural) {
     rc = commit_device(f, ds, st);
     if (rc < 0) return rc;
     if (rc == 1) structural = true;  // mixed versions: the literal comparator needs the host's merge sort (N1)
   }
-  if (structural) { rc = commit_structural(f, ds, st); if (rc < 0) return rc; }
+  if (structural) {
+    // the host path builds from the host tables: first bring over what the closed loop changed on the device (either route:
+    // a structural commit, or the device path's fallback above).  Outside a window the host rows are current -- the window
+    // copied them back -- and may hold updates not yet scattered, so only the registry comes over.
+    if (f->device_ahead) { rc = sync_host_from_device(f, rows_on_device); if (rc < 0) return rc; }
+    rc = commit_structural(f, ds, st);
+    if (rc < 0) return rc;
+  }
   const HostSnapshot &h = ds.host;
   const int RW = h.row_words;
   const int32_t nm = f->hs.n_models_used;

@@ -7,8 +7,10 @@
 #include "row_ranks.cpp"
 
 extern "C" {
-// counts (4 entries): decisions the summary answered, of those the ones whose walk differs, slots summarised for
-// c_self = 0 and for c_self = 1.  out: the walked results (the summary's where it answered and agreed).
+// counts (6 entries): decisions the summary answered, of those the ones whose walk differs, slots summarised for
+// c_self = 0 and for c_self = 1, summaries (slot, c_self) whose best and shortlist members run on more than one instance
+// version (a rolling upgrade), decisions answered in a slot with such a summary.  out: the walked results (the summary's
+// where it answered and agreed).
 int32_t mmp_emul_place_split(mmp_fleet *f, const mmp_decision_in *in, int32_t n, const mmp_instance_row *fresh, int32_t n_fresh,
                              const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed, int64_t *counts) {
   if (f->epoch == 0) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
@@ -26,17 +28,25 @@ int32_t mmp_emul_place_split(mmp_fleet *f, const mmp_decision_in *in, int32_t n,
   std::vector<int32_t> members((size_t)ns * 2 * SPLIT_CAP, -1);
   const uint32_t ww = (uint32_t)std::min<int64_t>(MMP_LANE_WIN, v.row_words);
   std::vector<uint32_t> ewin(ww, 0u);
-  int64_t summarised[2] = {0, 0};
+  int64_t summarised[2] = {0, 0}, crossing = 0;
+  std::vector<char> slot_crosses((size_t)ns, 0);
   for (int sl = 0; sl < v.n_slots; sl++) {
     LaneTables T = lane_tables_global(v, sl);
     T.nz_skip = 0;  // list entries inside this window
     while (T.nz_skip < T.nz_n && (uint32_t)T.nzw[T.nz_skip] < ww) T.nz_skip++;
     for (int cs = 0; cs < 2; cs++) {
-      slot_summary(v, T, sl, true, cs, ewin.data(), ww, now_ms, SoloVote(), nullptr, sums[sl], members.data() + ((size_t)sl * 2 + cs) * SPLIT_CAP);
-      if (sums[sl].reach[cs] >= 0) summarised[cs]++;
+      int32_t *mem = members.data() + ((size_t)sl * 2 + cs) * SPLIT_CAP;
+      slot_summary(v, T, sl, true, cs, ewin.data(), ww, now_ms, SoloVote(), nullptr, sums[sl], mem);
+      if (sums[sl].reach[cs] < 0) continue;
+      summarised[cs]++;
+      const int32_t vers = f->hs.inst[sums[sl].best_idx].row.vers;
+      bool mixed = false;
+      for (int32_t k = 0; k < sums[sl].n_in[cs] && k < SPLIT_CAP; k++) mixed |= f->hs.inst[mem[k]].row.vers != vers;
+      crossing += mixed;
+      slot_crosses[sl] |= mixed;
     }
   }
-  int64_t fast = 0, mismatch = 0;
+  int64_t fast = 0, mismatch = 0, fast_crossing = 0;
   for (int32_t i = 0; i < n; i++) {
     const mmp_decision_in &d = in[i];
     const int32_t m = excl_row_id(v, d.model, d.flags);
@@ -48,9 +58,11 @@ int32_t mmp_emul_place_split(mmp_fleet *f, const mmp_decision_in *in, int32_t n,
     mmp_decision_out r;
     if (!split_answer(v, d, a, row, fr.data(), n_fresh, sums.data(), members.data(), now_ms, seed, pick_id(d, f->id_base + (uint64_t)i), r)) continue;
     fast++;
+    fast_crossing += slot_crosses[(size_t)slot_key(v, a.mr.type_id)];
     if (r.target != out[i].target || r.n_candidates != out[i].n_candidates) mismatch++;
   }
   counts[0] = fast; counts[1] = mismatch; counts[2] = summarised[0]; counts[3] = summarised[1];
+  counts[4] = crossing; counts[5] = fast_crossing;
   return MMP_OK;
 }
 }  // extern "C"

@@ -8,8 +8,8 @@ fleet under test did incrementally (dirty rows scattered on the device, overflow
 re-resolved by id, registry rows past the old end) is compared with a state that was never incremental.
 
 Windows come in two kinds: "numeric" windows carry numeric instance updates and model-record edits only (the device
-path of a commit, path 2), "structural" windows also add, remove, re-register and relabel instances or change the type
-config or the replicaset list (the host path, path 1)."""
+path of a commit, path 2, unless the live instances run more than one version), "structural" windows also add, remove,
+re-register and relabel instances or change the type config or the replicaset list (the host path, path 1)."""
 from __future__ import annotations
 
 import copy
@@ -367,6 +367,12 @@ class Replay:
         """More distinct dirty models than this in one window and the commit uploads the whole registry instead."""
         return self.nm_max // 8 + 1024
 
+    def expected_path(self, kind: str) -> int:
+        """A numeric window commits on the device (2) while every live instance runs one version; a live set of several
+        versions (a rolling upgrade: PLACEMENT_ORDER's version clause, N1) takes the host path (1), as structural windows do."""
+        one_version = len(np.unique(self.rows["vers"][self._live()])) <= 1
+        return 2 if kind == NUMERIC and one_version else 1
+
     def commit(self, kind: str, n_model_edits: int, events=()):
         self.f.commit()
         self.last_touched = np.asarray(sorted(self.touched), dtype=np.int64)
@@ -374,7 +380,7 @@ class Replay:
         self.front = self._front()
         path = self.f.commit_info()[0] if self.has_path else None
         if self.has_path:
-            assert path == (2 if kind == NUMERIC else 1), (kind, path, len(self.windows))
+            assert path == self.expected_path(kind), (kind, path, len(self.windows))
         self.windows.append((kind, path, n_model_edits, tuple(events)))
         return path
 

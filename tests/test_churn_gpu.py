@@ -37,7 +37,9 @@ def _build(product_lib, w, slots):
     return o, sim, s
 
 
-def _compare_window(ep, o, sim, s, ev, now0, now1, seed):
+def _compare_window(ep, o, sim, s, ev, now0, now1, seed, path=2):
+    """path: the commit path the window must end with (mmp_commit_info): 2, the device path; 1, the host path (a live set
+    of more than one instance version, or commit_host_only)"""
     dec_o, evi_o, rows_o, npub_o, carry_o = sim.step(ev, now0, now1, seed)
     dec_p, evi_p, rows_p, rep = s.churn_step(ev, now0, now1, seed)
     assert len(dec_p) == len(dec_o), (ep, len(dec_p), len(dec_o))
@@ -56,7 +58,7 @@ def _compare_window(ep, o, sim, s, ev, now0, now1, seed):
         assert np.array_equal(rows_p[k], rows_o[k]), (ep, k, np.nonzero(rows_p[k] != rows_o[k])[0][:5])
     assert rep.n_published == npub_o and rep.n_carry == carry_o, (ep, rep.n_published, npub_o, rep.n_carry, carry_o)
     assert np.array_equal(s.cluster_order(), o.cluster_order()), ep
-    assert s.commit_info()[0] == 2  # the window ended with a device-path commit
+    assert s.commit_info()[0] == path, (ep, s.commit_info()[0], path)
     return dec_o, evi_o, rep
 
 
@@ -65,16 +67,17 @@ def test_closed_loop_matches_oracle_small(product_lib, oracle_lib, with_types, f
     run_small_closed_loop(product_lib, with_types, fill, seed, slots=256)
 
 
-def run_small_closed_loop(product_lib, with_types, fill, seed, slots):
-    """12 windows of a 20k-model x 200-instance churn trace, compared window by window, then the registry and ingest after it"""
-    w = make_churn(20_000, 200, seed, fill=fill, with_types=with_types)
+def run_small_closed_loop(product_lib, with_types, fill, seed, slots, w=None, path=2):
+    """12 windows of a 20k-model x 200-instance churn trace (or of the workload w), compared window by window, then the
+    registry and ingest after it; path: the commit path of every window"""
+    w = w or make_churn(20_000, 200, seed, fill=fill, with_types=with_types)
     fl = w.fleet
     o, sim, s = _build(product_lib, w, slots=slots)
     totals = dict(dec=0, acc=0, evict=0, reload=0, rejected=0, pub=0)
     for ep in range(12):
         ev = w.events(ep, 2000, seed)
         now0 = fl.now_ms + ep * w.window_ms
-        dec, evi, rep = _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
+        dec, evi, rep = _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep, path=path)
         totals["dec"] += len(dec); totals["acc"] += int(np.count_nonzero(dec["status"] == ob.SIM_ACCEPTED))
         totals["rejected"] += int(np.count_nonzero((dec["status"] >= 1) & (dec["status"] <= 5)))
         totals["evict"] += len(evi); totals["reload"] += int(evi["reload"].sum()); totals["pub"] += rep.n_published

@@ -9,6 +9,7 @@ import pytest
 from modelmesh_b200.synth import make_decisions, make_fleet
 
 from helpers import compare_decisions, oracle_from_synth, solver_from_synth
+from test_rolling_upgrade_gpu import fleet_for
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [
@@ -40,12 +41,13 @@ def test_mixed_regimes_match_oracle(emul_lib, oracle_lib, seed):
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [("C2", 2000, 1000, 12), ("C3", 4000, 700, 3), ("C5", 3000, 500, 5), ("MIX", 600, 160, 8),
-                                               ("MIX", 600, 300, 14), ("C3", 1500, 1300, 33)])
+                                               ("MIX", 600, 300, 14), ("C3", 1500, 1300, 33), ("C3/half", 4000, 700, 3),
+                                               ("MIX/saturated", 600, 300, 14)])
 def test_half_warp_window_matches_oracle(emul_lib, oracle_lib, config, nm, ni, seed):
     """The fast path with 16-word windows (the half-warp tile of the GPU kernel: two decisions per warp)."""
     emul_lib.mmp_emul_set_window(16)
     try:
-        fl = make_fleet(config, nm, ni, seed)
+        fl = fleet_for(config, nm, ni, seed)
         o = oracle_from_synth(fl)
         s = solver_from_synth(fl, emul_lib)
         sd = make_decisions(fl, 2500, seed)
@@ -59,7 +61,8 @@ def test_half_warp_window_matches_oracle(emul_lib, oracle_lib, config, nm, ni, s
 @pytest.mark.parametrize("budget", [1, 48])
 @pytest.mark.parametrize("shape", [1, 2])
 @pytest.mark.parametrize("config,nm,ni,seed", [("C2", 2000, 1000, 12), ("C3", 4000, 700, 3), ("C5", 3000, 500, 5), ("MIX", 600, 160, 8),
-                                               ("MIX", 600, 300, 14), ("MIX", 600, 97, 21), ("C3", 1500, 1300, 33)])
+                                               ("MIX", 600, 300, 14), ("MIX", 600, 97, 21), ("C3", 1500, 1300, 33),
+                                               ("C3/half", 4000, 700, 3), ("MIX/saturated", 600, 300, 14)])
 def test_lane_shape_matches_oracle(emul_lib, oracle_lib, config, nm, ni, seed, budget, shape):
     """The lane-per-decision shapes: 1 = the general routine as a budgeted single-lane walk (CoopLane), 2 = the lockstep
     streaming routine k_place_lanes runs (decide_stream); both with the cooperative redo when the lane declines.
@@ -69,7 +72,7 @@ def test_lane_shape_matches_oracle(emul_lib, oracle_lib, config, nm, ni, seed, b
     emul_lib.mmp_emul_set_window(shape)
     emul_lib.mmp_emul_set_lane_budget(budget)
     try:
-        fl = make_fleet(config, nm, ni, seed)
+        fl = fleet_for(config, nm, ni, seed)
         o = oracle_from_synth(fl)
         s = solver_from_synth(fl, emul_lib)
         emul_lib.mmp_emul_lane_bails(None)
@@ -151,7 +154,8 @@ def test_registry_sweep_equals_the_batch_of_records(emul_lib, oracle_lib):
 
 @pytest.mark.parametrize("second_chance", [0, 1])
 @pytest.mark.parametrize("window", [1, 2, 5, 10])
-@pytest.mark.parametrize("config,nm,ni,seed", [("C3", 2000, 1300, 33), ("C5", 1500, 500, 5), ("MIX", 500, 300, 14), ("MIX", 500, 700, 41)])
+@pytest.mark.parametrize("config,nm,ni,seed", [("C3", 2000, 1300, 33), ("C5", 1500, 500, 5), ("MIX", 500, 300, 14), ("MIX", 500, 700, 41),
+                                               ("C3/three", 2000, 1300, 33), ("MIX/saturated", 500, 700, 41)])
 def test_stream_routine_window_widths(emul_lib, oracle_lib, config, nm, ni, seed, window, second_chance):
     """decide_stream sees a window of the decision's exclusion row: its first `window` words (the kernels copy MMP_LANE_WIN = 12);
     beyond it a walk steps through the type slot's compressed word list.  second_chance = 0: a walk that leaves the window must be
@@ -163,7 +167,7 @@ def test_stream_routine_window_widths(emul_lib, oracle_lib, config, nm, ni, seed
     emul_lib.mmp_emul_set_lane_global(second_chance)
     emul_lib.mmp_emul_set_lane_budget(64)
     try:
-        fl = make_fleet(config, nm, ni, seed)
+        fl = fleet_for(config, nm, ni, seed)
         o = oracle_from_synth(fl)
         s = solver_from_synth(fl, emul_lib)
         emul_lib.mmp_emul_lane_bails(None)

@@ -40,7 +40,7 @@ def place_split(lib, s, sd, now_ms, seed):
     fresh = np.ascontiguousarray(sd.fresh, dtype=_lib.INSTANCE_ROW) if len(sd.fresh) else None
     extra = np.ascontiguousarray(sd.extra, dtype=np.int32) if len(sd.extra) else None
     out = np.zeros(len(dec), dtype=_lib.DECISION_OUT)
-    counts = np.zeros(4, dtype=np.int64)
+    counts = np.zeros(6, dtype=np.int64)
     s._ck(lib.mmp_emul_place_split(s.h, _ptr(dec), len(dec), _ptr(fresh), 0 if fresh is None else len(fresh), _ptr(extra),
                                    0 if extra is None else len(extra), _ptr(out), now_ms, seed, _ptr(counts)))
     return out, counts
