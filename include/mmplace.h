@@ -495,8 +495,8 @@ int32_t mmp_registry_prune_ids(mmp_fleet *, int32_t self, int64_t now_ms, int64_
  *   "lane_budget"     walk steps a lane may spend before its decision is redone by the whole warp
  *   "commit_host_only" 1: every commit takes the structural (host) path */
 int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
-/* CUDA-event duration (ms) of the device part of the last mmp_stats ("stats"), mmp_reaper_select ("reaper": registry sweep +
- * sort + select), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
+/* CUDA-event duration (ms) of the device part of the last mmp_stats ("stats"), mmp_reaper_select ("reaper": the candidate
+ * sweep through the selection, k_rp_flag to k_rp_pick, without the stats and plan), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
  * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);

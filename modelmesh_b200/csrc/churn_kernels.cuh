@@ -1,6 +1,7 @@
 // churn_kernels.cuh — the closed loop of the placement / eviction path ON THE DEVICE (SURVEY.md §8a rows a11, a12; §8f-1,
 // §8f-4): one call of mmp_churn_step = one republish window (2 s, MM:232) of the whole fleet:
-//   reaper      (windows with REAPER events only) the reaper's selections, k_rp_* below; their count is read back once
+//   reaper      (windows with REAPER events only) the reaper's selections (reaper_pass, scan_kernels.cuh); their count is
+//               read back once
 //   classify    requests -> cache hits (runtimeCache.get on a registered copy) / cache misses (the first request of an unloaded
 //               model in the window -> a getNext decision) / removals / the reaper's selections (decisions at the REAPER's
 //               position); queued ensureLoadedElsewhere calls go first
@@ -349,183 +350,9 @@ __global__ void k_churn_type_ok(const StatsAcc *__restrict__ acc, const int *__r
   type_ok[t] = ((long long)cap > 0 && cnt > 1 && (long long)(20ull * fr) / (long long)cap >= 1) ? 1 : 0;
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// The reaper's proactive loads (MMP_CHURN_REAPER; MM:6456-6494, 6574-6577, 6616-6747), on the step's stream against the
-// window's snapshot: the stats of k_stats -> per-partition plan and PARTITION_STATS_COMP order (k_rp_plan) -> candidates
-// (k_rp_flag, compaction) -> one radix sort by (lastUsed desc, model asc) -> spaceToFill per partition (k_rp_space) -> one
-// block walks the sorted list per event and partition (k_rp_walk).  reaper_impl (scan_kernels.cuh) is the same arithmetic
-// with its host parts; the parity tests hold the two equal.
-// ---------------------------------------------------------------------------------------------------------------
-// one slot per partition (the whole cluster when the fleet has no type constraints), as run_stats reports them
-struct RpPart { long long cap, free, glru; int copies, count, size_est, pad; };
-struct RpPlan { int go, n_order; long long global_lru; };
-__device__ __forceinline__ long long rp_last_used(unsigned long long key) { return (long long)((~key) ^ 0x8000000000000000ull); }
-
-__global__ void k_rp_plan(const StatsAcc *__restrict__ acc, const long long *__restrict__ min_lru, int n_slots, int tc, int def_size,
-                          RpPart *__restrict__ parts, int *__restrict__ order, RpPlan *__restrict__ plan) {
-  const long long mn = *min_lru;
-  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) {
-    const StatsAcc a = acc[tc ? 1 + s : 0];
-    RpPart p{(long long)a.cap, (long long)a.free, (a.count > 0 || !tc) ? mn : 0x7fffffffffffffffLL, a.copies, a.count, 0, 0};
-    if (p.copies < 3) p.size_est = def_size;  // MM:6622-6629
-    else {
-      const int32_t avg = (int32_t)jsub(p.cap, p.free) / p.copies;
-      p.size_est = p.copies > 10 ? avg : jaddi(avg, def_size) / 2;
-    }
-    parts[s] = p;
-  }
-  __syncthreads();
-  // PARTITION_STATS_COMP (TCM:264-271) as partition_order: free desc, lru asc, capacity desc, partition id; with instances only
-  __shared__ int n_in;
-  if (threadIdx.x == 0) n_in = 0;
-  __syncthreads();
-  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) {
-    const RpPart x = parts[s];
-    if (tc && x.count == 0) continue;
-    int rank = 0;
-    for (int o = 0; o < n_slots; o++) {
-      const RpPart y = parts[o];
-      if (o == s || (tc && y.count == 0)) continue;
-      rank += y.free != x.free ? y.free > x.free : y.glru != x.glru ? y.glru < x.glru : y.cap != x.cap ? y.cap > x.cap : o < s;
-    }
-    order[rank] = s;
-    atomicAdd(&n_in, 1);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {  // MM:6456-6463
-    plan->go = (long long)acc[0].cap > 0;
-    plan->global_lru = (long long)acc[0].free > 0 ? 0 : mn;
-    plan->n_order = n_in;
-  }
-}
-__global__ void k_rp_flag(const mmp_model_row *__restrict__ models, int n_models, const RpPlan *__restrict__ plan, uint8_t *__restrict__ flag) {
-  const int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= n_models) return;
-  const RpPlan p = *plan;
-  flag[m] = p.go && reaper_candidate(models[m], p.global_lru) ? 1 : 0;
-}
-// sort keys of the compacted candidates (in model order); the positions past them sort last
-__global__ void k_rp_keys(const mmp_model_row *__restrict__ models, const int *__restrict__ idx, const int *__restrict__ n_cand, int n,
-                          unsigned long long *__restrict__ key) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  key[i] = i < *n_cand ? ~((unsigned long long)models[idx[i]].last_used ^ 0x8000000000000000ull) : ~0ull;
-}
-// spaceToFill (MM:6633-6649) per partition: one segmented reduction over the rank-ordered instance columns, in the reference's
-// wrapping int / long arithmetic (the sum wraps too, so the order of the additions does not matter)
-__global__ void k_rp_space(const RankRow *__restrict__ rows, const int64_t *__restrict__ cap_col, const int32_t *__restrict__ lthreads,
-                           const int32_t *__restrict__ linprog, const int32_t *__restrict__ part_of_rank, int n_ranks, int tc, int n_slots,
-                           const RpPart *__restrict__ parts, unsigned long long *__restrict__ space) {
-  __shared__ unsigned long long sacc[STATS_SMEM_PARTS + 1];
-  const bool use_smem = n_slots <= STATS_SMEM_PARTS + 1;
-  if (use_smem) for (int i = threadIdx.x; i < n_slots; i += blockDim.x) sacc[i] = 0ull;
-  __syncthreads();
-  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n_ranks; r += gridDim.x * blockDim.x) {
-    const int s = tc ? part_of_rank[r] : 0;
-    if (s < 0 || s >= n_slots) continue;
-    const int32_t max_loads = (int32_t)((uint32_t)jmuli(lthreads[r], 50) - (uint32_t)linprog[r]);
-    if (max_loads <= 0) continue;
-    const int64_t avail = jsub(rows[r].rem, cap_col[r] / 8);
-    if (avail <= 0) continue;
-    const int64_t lim = (int64_t)jmuli(max_loads, parts[s].size_est);
-    atomicAdd(use_smem ? &sacc[s] : &space[s], (unsigned long long)(avail < lim ? avail : lim));
-  }
-  if (use_smem) {
-    __syncthreads();
-    for (int i = threadIdx.x; i < n_slots; i += blockDim.x) if (sacc[i]) atomicAdd(&space[i], sacc[i]);
-  }
-}
-// The selection of every REAPER event, one after the other, by one block: for each partition in order, the sorted candidates
-// are walked in chunks of RP_WALK.  Per chunk: eligible = not taken by this run, type allowed in the partition (MM:6681-6683)
-// and (free space or lastUsed > cutoff) (MM:6685-6688); of an equal-lastUsed run of eligible entries only the first counts
-// (N12; a block-wide max scan finds each entry's previous eligible entry); the counted entries take ranks k by a block-wide
-// sum scan, and the first totalProactiveLoadCount of them go through the emission rule (MM:6711-6719), which, the list
-// being in descending lastUsed, emits a prefix of them.  The walk stops at the count, at the rule's break, or (full
-// partition) at the first entry at or under the cutoff.  Emitted models are tagged taken and appended as (model, event).
-constexpr int RP_WALK = 1024;
-__global__ void __launch_bounds__(RP_WALK) k_rp_walk(const mmp_model_row *__restrict__ models, const unsigned long long *__restrict__ skey,
-                                                      const int *__restrict__ sidx, const int *__restrict__ n_cand, const RpPlan *__restrict__ plan,
-                                                      const RpPart *__restrict__ parts, const int *__restrict__ order,
-                                                      const unsigned long long *__restrict__ space, int tc, const int *__restrict__ pt_off,
-                                                      const int *__restrict__ pt_ids, const mmp_churn_event *__restrict__ ev,
-                                                      const int *__restrict__ rp_ev, int n_rp, int gen0, int *__restrict__ taken,
-                                                      int2 *__restrict__ sel, long long sel_cap, int *__restrict__ sel_off) {
-  using Scan = cub::BlockScan<int, RP_WALK>;
-  __shared__ typename Scan::TempStorage tmp;
-  __shared__ unsigned long long chunk_key[RP_WALK];
-  const int tid = threadIdx.x;
-  const int ncand = *n_cand;
-  const RpPlan P = *plan;
-  long long out = 0;
-  for (int r = 0; r < n_rp; r++) {
-    if (tid == 0) sel_off[r] = (int)out;
-    const int gen = gen0 + r;
-    const long long t = ev[rp_ev[r]].t;
-    for (int oi = 0; P.go && ncand > 0 && oi < P.n_order; oi++) {
-      const int s = order[oi];
-      const RpPart p = parts[s];
-      int free_count = 0, total = 0;
-      if (p.cap > 0 && p.free > 0) {  // MM:6621-6657
-        if (p.size_est == 0) break;   // spaceToFill / sizeEstimate throws (MM:6651): the run ends here
-        const long long fill = (long long)space[s] / 2;
-        free_count = (int32_t)(fill / p.size_est);
-        const long long d = (long long)(20ull * (unsigned long long)(long long)p.size_est);
-        const int32_t cap_count = d == 0 ? 0 : (int32_t)(d == -1 ? -p.cap : p.cap / d);
-        total = free_count > cap_count ? free_count : cap_count;
-      }
-      if (total <= 0) continue;
-      const long long a3 = age_of(p.glru, t) / 3;
-      const long long cutoff = p.glru == 0x7fffffffffffffffLL ? 0 : (long long)((unsigned long long)p.glru + (unsigned long long)(a3 > 1200000 ? a3 : 1200000));
-      const int *ex = tc ? pt_ids + pt_off[s] : nullptr;
-      const int nex = tc ? pt_off[s + 1] - pt_off[s] : 0;
-      int kept = 0, emitted = 0;
-      bool have_prev = false;
-      unsigned long long prev_key = 0;
-      for (int base = 0; base < ncand; base += RP_WALK) {
-        const int i = base + tid;
-        int m = -1;
-        unsigned long long key = ~0ull;
-        bool elig = false;
-        if (i < ncand) {
-          m = sidx[i]; key = skey[i];
-          elig = taken[m] != gen && (free_count > 0 || rp_last_used(key) > cutoff);
-          if (elig && nex) {  // the partition's prohibited type ids, sorted
-            const int ty = models[m].type_id;
-            int lo = 0, hi = nex;
-            while (lo < hi) { const int mid = (lo + hi) >> 1; if (ex[mid] < ty) lo = mid + 1; else hi = mid; }
-            elig = !(lo < nex && ex[lo] == ty);
-          }
-        }
-        chunk_key[tid] = key;
-        int prev, last;
-        Scan(tmp).ExclusiveScan(elig ? tid : -1, prev, -1, cub::Max(), last);
-        __syncthreads();
-        const bool hp = prev >= 0 || have_prev;
-        const unsigned long long pk = prev >= 0 ? chunk_key[prev] : prev_key;
-        const int first = elig && !(hp && pk == key) ? 1 : 0;
-        int j, n_first;
-        Scan(tmp).ExclusiveSum(first, j, n_first);
-        const int k = kept + j;
-        const bool emit = first && k < total && (k < free_count || !(rp_last_used(key) < cutoff));
-        const int n_emit = __syncthreads_count(emit);
-        if (emit) {
-          taken[m] = gen;
-          const long long pos = out + k;
-          if (pos < sel_cap) sel[pos] = make_int2(m, r);
-        }
-        kept += n_first; emitted += n_emit;
-        if (last >= 0) { have_prev = true; prev_key = chunk_key[last]; }
-        bool stop = n_emit < n_first || kept >= total || base + RP_WALK >= ncand;
-        if (free_count == 0 && rp_last_used(chunk_key[RP_WALK - 1]) <= cutoff) stop = true;  // nothing eligible past it
-        __syncthreads();
-        if (stop) break;
-      }
-      out += emitted;
-    }
-  }
-  if (tid == 0) sel_off[n_rp] = (int)out;
-}
-// the window's items see the selections at their REAPER's position: first decisions (k_churn_first's rule), flags, records
+// The reaper's proactive loads (MMP_CHURN_REAPER): reaper_pass (scan_kernels.cuh) selects them against the window's snapshot,
+// one run per REAPER event at its time t, every partition in PARTITION_STATS_COMP order; the kernels below make them decisions.
+// The window's items see the selections at their REAPER's position: first decisions (k_churn_first's rule), flags, records
 __global__ void k_rp_first(const int2 *__restrict__ sel, int n_sel, const int *__restrict__ rp_ev, int n_follow, int *__restrict__ first_ev) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n_sel) return;
@@ -641,79 +468,25 @@ static int32_t churn_relay_ovf(mmp_fleet *f, cudaStream_t st) {
   return MMP_OK;
 }
 
-// The reaper pass of a window with REAPER events (rp_ev: their trace indices), after k_stats filled acc / min_lru: every
-// event's selections in cs.rp_sel as (model, event) in emission order, cs.rp_ev = [rp_ev | selection offsets].  The total is
-// read back (the window's one synchronisation for it: the decision buffers are sized from it); a second walk follows only
-// when several events selected more models in all than the fleet has.
+// The reaper pass of a window with REAPER events (rp_ev: their trace indices), after k_stats filled acc / min_lru: one run per
+// event at its time, every partition in PARTITION_STATS_COMP order.  The selections land in cs.rp.sel as (model, run) in
+// emission order, their offsets per run in cs.rp.off; cs.rp_ev holds rp_ev.  The total is read back (the window's one
+// synchronisation for it: the decision buffers are sized from it).
 static int32_t churn_reaper_pass(mmp_fleet *f, const DeviceSnapshot &ds, const StatsAcc *acc, const long long *min_lru,
-                                 const std::vector<int> &rp_ev, cudaStream_t st, int32_t *n_sel) {
+                                 const mmp_churn_event *ev, const std::vector<int> &rp_ev, cudaStream_t st, int32_t *n_sel) {
   ChurnState &cs = f->churn;
-  const HostSnapshot &h = ds.host;
-  const int NM = f->hs.n_models_used, R = (int)rp_ev.size(), tc = h.tc_enabled ? 1 : 0;
-  const int ns = tc ? (int)h.part_types.size() : 1;
-  const size_t nmx = (size_t)std::max(NM, 1);
-  // each partition's prohibited type ids of this epoch (reaper_impl's `excl`), sorted: [offsets (ns + 1) | ids]
-  std::vector<int> pt((size_t)ns + 1, 0);
-  for (int p = 0; tc && p < ns; p++) {
-    std::vector<int> ids;
-    for (int32_t tid : h.part_type_ids[p]) if (tid >= 0 && tid < (int32_t)h.type_slot.size()) ids.push_back(tid);
-    std::sort(ids.begin(), ids.end());
-    pt.insert(pt.end(), ids.begin(), ids.end());
-    pt[p + 1] = pt[p] + (int)ids.size();
-  }
-  std::vector<int> evo(rp_ev);
-  evo.resize((size_t)2 * R + 1, 0);
-  CK(upload_vec(cs.rp_pt, pt, st));
-  CK(upload_vec(cs.rp_ev, evo, st));
-  CK(cs.rp_keys.ensure(nmx * 16)); CK(cs.rp_idx.ensure(nmx * 8 + 16)); CK(cs.rp_flag.ensure(nmx));
-  CK(cs.rp_sel.ensure(nmx * sizeof(int2)));  // (one event selects each model at most once)
-  const size_t parts_b = (size_t)ns * sizeof(RpPart), space_b = (size_t)ns * 8;
-  CK(cs.rp_plan.ensure(parts_b + space_b + sizeof(RpPlan) + (size_t)ns * 4 + 16));
-  const size_t taken_cap = cs.rp_taken.cap;
-  CK(cs.rp_taken.ensure(nmx * 4));
-  if (cs.rp_taken.cap != taken_cap || cs.rp_gen > INT32_MAX / 2) {  // tags start over on a zeroed array
-    CK(cudaMemsetAsync(cs.rp_taken.p, 0, cs.rp_taken.cap, st));
+  const int NM = f->hs.n_models_used;
+  std::vector<long long> run_t;
+  for (int i : rp_ev) run_t.push_back(ev[i].t);
+  CK(upload_vec(cs.rp_ev, rp_ev, st));
+  const size_t taken_cap = cs.rp.taken.cap;
+  CK(cs.rp.taken.ensure((size_t)std::max(NM, 1) * 4));
+  if (cs.rp.taken.cap != taken_cap || cs.rp_gen > INT32_MAX / 2) {  // tags start over on a zeroed array
+    CK(cudaMemsetAsync(cs.rp.taken.p, 0, cs.rp.taken.cap, st));
     cs.rp_gen = 0;
   }
-  RpPart *parts = cs.rp_plan.as<RpPart>();
-  unsigned long long *space = reinterpret_cast<unsigned long long *>(cs.rp_plan.as<char>() + parts_b);
-  RpPlan *plan = reinterpret_cast<RpPlan *>(cs.rp_plan.as<char>() + parts_b + space_b);
-  int *order = reinterpret_cast<int *>(plan + 1);
-  unsigned long long *keys = cs.rp_keys.as<unsigned long long>(), *skeys = keys + nmx;
-  int *idx = cs.rp_idx.as<int>(), *sidx = idx + nmx, *d_n = sidx + nmx;
-  CK(cudaMemsetAsync(space, 0, space_b, st));
-  k_rp_plan<<<1, 256, 0, st>>>(acc, min_lru, ns, tc, f->hs.cfg.default_model_size_units, parts, order, plan);
-  k_rp_flag<<<(int)((nmx + 255) / 256), 256, 0, st>>>(f->live.models.as<mmp_model_row>(), NM, plan, cs.rp_flag.as<uint8_t>());
-  thrust::counting_iterator<int32_t> iota(0);
-  size_t t1 = 0, t2 = 0;
-  CK(cub::DeviceSelect::Flagged(nullptr, t1, iota, cs.rp_flag.as<uint8_t>(), idx, d_n, NM, st));
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, t2, keys, skeys, idx, sidx, NM, 0, 64, st));
-  CK(cs.cub_tmp.ensure(std::max(t1, t2) + 16));
-  CK(cub::DeviceSelect::Flagged(cs.cub_tmp.p, t1, iota, cs.rp_flag.as<uint8_t>(), idx, d_n, NM, st));
-  k_rp_keys<<<(int)((nmx + 255) / 256), 256, 0, st>>>(f->live.models.as<mmp_model_row>(), idx, d_n, NM, keys);
-  CK(cub::DeviceRadixSort::SortPairs(cs.cub_tmp.p, t2, keys, skeys, idx, sidx, NM, 0, 64, st));
-  if (h.n_ranks > 0)
-    k_rp_space<<<std::min(f->sm_count, (h.n_ranks + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(),
-                                                                            ds.lthreads_col.as<int32_t>(), ds.linprog_col.as<int32_t>(),
-                                                                            ds.part_of_rank.as<int32_t>(), h.n_ranks, tc, ns, parts, space);
-  f->launches += 6 + (h.n_ranks > 0);
-  CK(cudaGetLastError());
-  int *d_off = cs.rp_ev.as<int>() + R;
-  for (int pass = 0;; pass++) {
-    const long long sel_cap = (long long)(cs.rp_sel.cap / sizeof(int2));
-    k_rp_walk<<<1, RP_WALK, 0, st>>>(f->live.models.as<mmp_model_row>(), skeys, sidx, d_n, plan, parts, order, space, tc,
-                                     cs.rp_pt.as<int>(), cs.rp_pt.as<int>() + ns + 1, cs.ev.as<mmp_churn_event>(), cs.rp_ev.as<int>(), R,
-                                     cs.rp_gen + 1, cs.rp_taken.as<int>(), cs.rp_sel.as<int2>(), sel_cap, d_off);
-    f->launches++;
-    CK(cudaGetLastError());
-    cs.rp_gen += R;
-    int total = 0;
-    CK(cudaMemcpyAsync(&total, d_off + R, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (total <= sel_cap) { *n_sel = total; return MMP_OK; }
-    if (pass) { g_err = "internal: the reaper's selections changed between two walks"; return MMP_E_STATE; }
-    CK(cs.rp_sel.ensure((size_t)total * sizeof(int2)));
-  }
+  return reaper_pass(f, ds, f->live.models.as<mmp_model_row>(), NM, ds.host.tc_enabled ? 1 : 0, acc, min_lru, run_t, cs.rp_gen,
+                     cs.rp, cs.cub_tmp, st, n_sel);
 }
 
 extern "C" {
@@ -876,7 +649,7 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
     // ---- the reaper's proactive loads: selections of the window's REAPER events (then one read-back of their count) ----
     if (n_rp) {
       CK(cudaEventRecord(evs[7], st));
-      rc = churn_reaper_pass(f, ds, cs.stats_acc.as<StatsAcc>(), d_min, rp_ev, st, &n_sel);
+      rc = churn_reaper_pass(f, ds, cs.stats_acc.as<StatsAcc>(), d_min, ev, rp_ev, st, &n_sel);
       if (rc < 0) return rc;
       CK(cudaEventRecord(evs[8], st));
     }
@@ -895,9 +668,9 @@ int32_t mmp_churn_step(mmp_fleet *f, const mmp_churn_event *ev, int32_t n, int64
   const Follow *carry = cs.carry.as<Follow>();
   const RegTables R{lv.edges.as<int4>(), nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
   if (n_sel) CK(cs.rp_fpos.ensure((size_t)(n_sel + 1) * 8));
-  const int2 *sel = cs.rp_sel.as<int2>();
+  const int2 *sel = cs.rp.sel.as<int2>();
   int *sel_flag = cs.rp_fpos.as<int>(), *sel_fpos = sel_flag + n_sel + 1;  // first-decision flags, their exclusive scan
-  const RpView rp{cs.rp_ev.as<int>(), n_rp, cs.rp_ev.as<int>() + n_rp, n_sel ? sel_fpos : nullptr};
+  const RpView rp{cs.rp_ev.as<int>(), n_rp, cs.rp.off.as<int>(), n_sel ? sel_fpos : nullptr};
   bool relaid = false;
   if (Q > 0) {
     // ---- A: classify ----

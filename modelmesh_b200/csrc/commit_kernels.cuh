@@ -61,6 +61,11 @@ static RegTables reg_tables(const LiveState &lv) {
   return RegTables{lv.edges.as<int4>(), lv.have_times ? lv.edge_ts.as<long long>() : nullptr, lv.ovf.as<OvfEdge>(), lv.n_ovf};
 }
 
+// scratch of the reaper's selection pass (reaper_pass, scan_kernels.cuh), owned by its caller: sort keys, model indices and
+// their count, candidate flags, the per-partition plan, the runs' clocks with the partitions' prohibited type ids, the
+// selections and their offsets per run; taken[m] holds the tag of the last run that selected model m
+struct RpScratch { DevBuf keys, idx, flag, plan, runs, sel, off, taken; };
+
 // state of the closed loop (churn_kernels.cuh), owned by the fleet
 struct ChurnState {
   bool on = false;
@@ -70,10 +75,10 @@ struct ChurnState {
   DevBuf ev, is_dec, dec_pos, dec_in, dec_out, dec_meta, dec_target, extra, status, lev, keys, vals, keys2, vals2, cub_tmp, off, evict, fkeys,
       fvals, rows_changed;
   DevBuf ovf_dead, ovf_next, ovf_count;  // the registry phase's re-lay of LiveState::ovf (churn_kernels.cuh)
-  // the reaper pass of a window with MMP_CHURN_REAPER events (churn_kernels.cuh): sort keys / model indices, the per-partition
-  // plan, the partitions' prohibited type ids, the events' selections and their first-decision flags; rp_taken[m] holds the tag
-  // of the last reaper run that selected model m (tags grow across windows: no reset per run)
-  DevBuf rp_keys, rp_idx, rp_flag, rp_plan, rp_pt, rp_ev, rp_sel, rp_fpos, rp_taken;
+  // the reaper pass of a window with MMP_CHURN_REAPER events (churn_kernels.cuh): its scratch, the events' trace indices and
+  // their selections' first-decision flags; rp_gen: the last tag in rp.taken (tags grow across windows: no reset per run)
+  RpScratch rp;
+  DevBuf rp_ev, rp_fpos;
   int32_t rp_gen = 0;
   int32_t n_carry = 0;
   // what the step's host side knows of the registry without reading it back: the loop only removes loaded copies or loads the

@@ -27,8 +27,8 @@
 //   The one-decision-per-lane kernels share their steps through one helper each: no_decision / no_ctx (an absent lane),
 //   load_decision_stream (the streamed record load), redo_declined (the warp redo of what the lane routine declined; not
 //   k_place_dealt, which assembles the row in shared memory), WinTabs (the window tables in shared memory) and slot_key.
-//   k_build_bitmap*, k_sparse_slots + commit_kernels.cuh (device-path commit), scan_kernels.cuh (k_stats, k_reaper_flag,
-//   k_lru_events), churn_kernels.cuh (the closed loop), registry_kernels.cuh (k_scale_eval, k_registry_prune)
+//   k_build_bitmap*, k_sparse_slots + commit_kernels.cuh (device-path commit), scan_kernels.cuh (k_stats, k_rp_* the
+//   reaper's selection, k_lru_events), churn_kernels.cuh (the closed loop), registry_kernels.cuh (k_scale_eval, k_registry_prune)
 #include <cuda_runtime.h>
 #include <unistd.h>
 #include <dlfcn.h>
@@ -1209,7 +1209,7 @@ struct DeviceSnapshot {
   DevBuf cap_col, lthreads_col, linprog_col, part_of_rank, count_col, cand_before, nzw, nz_n;
   DevBuf front, nzw_full, nz_n_full;  // instance-sharded fleets: replicated first words of every row; word lists over the whole row
   SnapshotView view{};
-  HostSnapshot host;  // kept for introspection and the small host-side parts of stats / reaper
+  HostSnapshot host;  // kept for introspection and the small host-side parts of stats / reaper (partition tables)
   DevBuf sparse_dev;
   bool sparse_slots = false;  // most type slots have few candidates inside a decision's window: long walks (k_place_direct sorts big batches by slot)
   bool host_stale = false;  // built on the device: the rank-space vectors of `host` are downloaded on first use (host_mirror)
@@ -1240,6 +1240,7 @@ struct PlaceCtx {
   // a call-wide exclude set (mmp_place_batch_excluding): its ids and the per-slot tables derived from the snapshot's
   // (k_exclude_slots, k_slot_lists) that the call's view points at
   DevBuf d_xids, d_xcand, d_xcandx, d_xpref, d_xnzw, d_xnz_n, d_xbefore;
+  RpScratch rp;  // mmp_reaper_select's pass (scan_kernels.cuh)
 };
 
 // The scoring kernel of untraced batches (MMP_KERNEL = direct | lanes | tile; launch_place): k_place_direct (rows rebuilt
@@ -2105,7 +2106,7 @@ static int32_t commit_device(mmp_fleet *f, DeviceSnapshot &ds, cudaStream_t st) 
   return MMP_OK;
 }
 
-// rank-space vectors of a device-built snapshot, downloaded on first use (introspection, the reaper's host part)
+// rank-space vectors of a device-built snapshot, downloaded on first use (introspection)
 static int32_t host_mirror(mmp_fleet *f, const DeviceSnapshot &cds, const HostSnapshot **out) {
   DeviceSnapshot &ds = const_cast<DeviceSnapshot &>(cds);
   std::lock_guard<std::mutex> g(f->mirror_mu);
@@ -2299,7 +2300,8 @@ int32_t mmp_tune(mmp_fleet *f, const char *key, int64_t value) {
   else { g_err = "unknown key or value out of range"; return MMP_E_ARG; }
   return MMP_OK;
 }
-/* CUDA-event duration (ms) of the device part of the last call of a scan: "stats", "reaper", "lru_apply", "commit" */
+/* CUDA-event duration (ms) of the device part of the last call of a scan: "stats", "reaper" (the candidate sweep through
+ * the selection, k_rp_flag to k_rp_pick, without the stats and plan), "lru_apply", "commit" */
 int32_t mmp_last_timing(mmp_fleet *f, const char *key, double *ms) {
   NEED(f);
   if (!key || !ms) { g_err = "null argument"; return MMP_E_ARG; }

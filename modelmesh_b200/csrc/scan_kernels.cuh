@@ -2,6 +2,7 @@
 // registry sweep + top-K selection, and the per-instance time-ordered weighted LRU.  Included at the end of mmplace.cu.
 #pragma once
 #include <cuda/std/tuple>
+#include <thrust/iterator/transform_iterator.h>
 
 // ---------------------------------------------------------------------------------------------------------------
 // ClusterStats (MM:1570-1591) per prohibited-type-set partition: InstanceSetStatsTracker.add (ISST:63-72) as a
@@ -103,191 +104,339 @@ static std::vector<int> partition_order(const StatsResult &res) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Reaper: registry sweep (MM:6536-6590 candidate rule MM:6574-6577) + bounded most-recently-used selection
-// (MM:6675-6698) as  flag/compact -> bitonic sort by (lastUsed desc, model asc) -> first-of-run.
+// The reaper's proactive loads (MM:6456-6494, 6574-6577, 6616-6747) for mmp_reaper_select and the closed loop's REAPER
+// events, on the caller's stream against one snapshot: the stats of k_stats -> per-partition plan and PARTITION_STATS_COMP
+// order (k_rp_plan) -> candidates (k_rp_flag, compaction) -> one radix sort by (lastUsed desc, model asc) -> spaceToFill per
+// partition (k_rp_space) -> one block walks the sorted list per run and partition (k_rp_walk; reaper_pass, the closed loop).
+// mmp_reaper_select's one run in one partition runs the same stages with its filter in k_rp_flag and k_rp_pick for the walk.
 // ---------------------------------------------------------------------------------------------------------------
 // the candidate rule of the registry sweep (MM:6574-6577): no loaded copy, fewer than 2 failed loads, used after globalLru
 // (0 when the cluster has free space)
 __device__ __forceinline__ bool reaper_candidate(const mmp_model_row &r, long long global_lru) {
   return r.copy_count == 0 && r.fail_count < 2 && (global_lru == 0 || r.last_used > global_lru);
 }
-// key: ~biased(lastUsed), so that ascending keys = descending time.  One thread per model: 24 B read, 1 + 8 B written.
-__global__ void k_reaper_flag(const mmp_model_row *__restrict__ models, int n_models, const uint8_t *__restrict__ type_excluded,
-                              int n_type_ids, const uint8_t *__restrict__ taken, long long global_lru, int need_cutoff,
-                              long long cutoff, uint8_t *__restrict__ flag, unsigned long long *__restrict__ key) {
-  int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= n_models) return;
-  mmp_model_row r = models[m];
-  bool ok = reaper_candidate(r, global_lru);                                                         // MM:6574-6577
-  if (ok && taken && taken[m]) ok = false;                                                           // allCandidates.set(i, null)
-  if (ok && r.type_id < n_type_ids && type_excluded[r.type_id]) ok = false;                          // MM:6681-6683
-  if (ok && need_cutoff && !(r.last_used > cutoff)) ok = false;                                      // MM:6685-6687
-  flag[m] = ok ? 1 : 0;
-  key[m] = ~((unsigned long long)r.last_used ^ 0x8000000000000000ull);
+// one slot per partition (the whole cluster when the pass runs without type constraints), as run_stats reports them
+struct RpPart { long long cap, free, glru; int copies, count, size_est, pad; };
+struct RpPlan { int go, n_order; long long global_lru; };
+MMP_HD long long rp_last_used(unsigned long long key) { return (long long)((~key) ^ 0x8000000000000000ull); }
+// One run at clock t in one partition (MM:6621-6664): the free-space count, totalProactiveLoadCount and the lastUsed cutoff from
+// the plan and spaceToFill.  false: the size estimate is 0 and spaceToFill / sizeEstimate throws (MM:6651)
+MMP_HD bool rp_counts(const RpPart &p, unsigned long long space, long long t, int &free_count, int &total, long long &cutoff) {
+  free_count = 0; total = 0;
+  if (p.cap > 0 && p.free > 0) {
+    if (p.size_est == 0) return false;
+    const long long fill = (long long)space / 2;
+    free_count = (int32_t)(fill / p.size_est);
+    const long long d = (long long)(20ull * (unsigned long long)(long long)p.size_est);
+    const int32_t cap_count = d == 0 ? 0 : (int32_t)(d == -1 ? -p.cap : p.cap / d);
+    total = free_count > cap_count ? free_count : cap_count;
+  }
+  const long long a3 = age_of(p.glru, t) / 3;
+  cutoff = p.glru == 0x7fffffffffffffffLL ? 0 : (long long)((unsigned long long)p.glru + (unsigned long long)(a3 > 1200000 ? a3 : 1200000));
+  return true;
 }
-// keep the first record of every equal-lastUsed run (TreeSet<ModelToLoad> drops equal keys, MM:6405-6408), in order
-__global__ void k_unique_mark(const unsigned long long *__restrict__ keys, int n, uint8_t *__restrict__ flags) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) flags[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1 : 0;
-}
-
-// A size estimate of 0 is the reference's ArithmeticException (spaceToFill / sizeEstimate, MM:6651), but the reaper only gets
-// there when the candidate list is not empty (MM:6470): count the models that pass the base candidate rule alone (MM:6574-6577;
-// no `taken`, type exclusion or cutoff) and fail the call only when there is one.  Returns 0 (nothing to load) or MMP_E_ARG.
-static int32_t reaper_zero_estimate(mmp_fleet *f, const DeviceSnapshot &ds, long long global_lru) {
-  const int nm = ds.n_models;
-  if (nm == 0) return 0;
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  cudaStream_t s = c->stream;
-  CK(c->d_in.ensure((size_t)nm * 8 + 64));
-  CK(c->d_trace.ensure((size_t)nm * 4 + 64));
-  CK(c->d_cand.ensure((size_t)nm + 64));
-  CK(c->d_n_open.ensure(16));
-  uint8_t *flags = c->d_cand.as<uint8_t>();
-  int *d_n = c->d_n_open.as<int>();
-  k_reaper_flag<<<(nm + 255) / 256, 256, 0, s>>>(ds.models.as<mmp_model_row>(), nm, nullptr, 0, nullptr, global_lru, 0, 0, flags,
-                                               c->d_in.as<unsigned long long>());
-  f->launches++;
-  CK(cudaGetLastError());
-  thrust::counting_iterator<int32_t> iota(0);
-  size_t t = 0;
-  CK(cub::DeviceSelect::Flagged(nullptr, t, iota, flags, c->d_trace.as<int32_t>(), d_n, nm, s));
-  CK(c->d_cub.ensure(t + 64));
-  CK(cub::DeviceSelect::Flagged(c->d_cub.p, t, iota, flags, c->d_trace.as<int32_t>(), d_n, nm, s));
-  f->launches++;
-  int ncand = 0;
-  CK(cudaMemcpyAsync(&ncand, d_n, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  if (ncand == 0) return 0;
-  g_err = "size estimate is zero (the reference would throw ArithmeticException)";
-  return MMP_E_ARG;
+// the emission rule (MM:6711-6719) for the k-th counted entry of a run in a partition
+MMP_HD bool rp_emits(int k, int free_count, int total, long long last_used, long long cutoff) {
+  return k < total && (k < free_count || !(last_used < cutoff));
 }
 
-static int32_t reaper_impl(mmp_fleet *f, int32_t partition, int64_t now, uint8_t *taken, int32_t *out_models, int32_t cap) {
-  if (!out_models || cap < 0) { g_err = "bad argument"; return MMP_E_ARG; }
-  int32_t rc = set_device(f);
-  if (rc < 0) return rc;
-  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
-  if (f->epoch == 0) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  const DeviceSnapshot &ds = f->snaps[f->cur];
-  const HostSnapshot *hp = nullptr;
-  rc = host_mirror(f, ds, &hp);
-  if (rc < 0) return rc;
-  const HostSnapshot &h = *hp;
-  const int np = (int)h.part_types.size();
-  if (partition >= np || (partition >= 0 && !h.tc_enabled)) { g_err = "no such partition"; return MMP_E_ARG; }
-  StatsResult sr;
-  rc = run_stats(f, ds, sr);
-  if (rc < 0) return rc;
-  const mmp_cluster_stats &g = sr.parts[0];
-  if (!(g.total_capacity > 0)) return 0;                                   // MM:6456
-  const int64_t global_lru = g.total_free > 0 ? 0 : g.global_lru;          // MM:6460
-  const mmp_cluster_stats &st = partition < 0 ? g : sr.parts[partition + 1];
-  // triggerProactiveLoadsForInstanceSubset MM:6616-6664
-  int32_t free_count = 0, total_count = 0;
-  if (st.total_capacity > 0 && st.total_free > 0) {
-    int32_t size_est;
-    const int32_t def = f->hs.cfg.default_model_size_units;
-    if (st.model_copy_count < 3) size_est = def;
+// slot >= 0: the runs walk that partition alone, whatever its stats.  Also zeroes the spaceToFill sums k_rp_space adds into.
+__global__ void k_rp_plan(const StatsAcc *__restrict__ acc, const long long *__restrict__ min_lru, int n_slots, int tc, int slot,
+                          int def_size, RpPart *__restrict__ parts, int *__restrict__ order, RpPlan *__restrict__ plan,
+                          unsigned long long *__restrict__ space) {
+  const long long mn = *min_lru;
+  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) {
+    space[s] = 0;
+    const StatsAcc a = acc[tc ? 1 + s : 0];
+    RpPart p{(long long)a.cap, (long long)a.free, (a.count > 0 || !tc) ? mn : 0x7fffffffffffffffLL, a.copies, a.count, 0, 0};
+    if (p.copies < 3) p.size_est = def_size;  // MM:6622-6629
     else {
-      int32_t avg = (int32_t)jsub(st.total_capacity, st.total_free) / st.model_copy_count;
-      size_est = st.model_copy_count > 10 ? avg : jaddi(avg, def) / 2;
+      const int32_t avg = (int32_t)jsub(p.cap, p.free) / p.copies;
+      p.size_est = p.copies > 10 ? avg : jaddi(avg, def_size) / 2;
     }
-    if (size_est == 0) return reaper_zero_estimate(f, ds, global_lru);
-    int64_t space = 0;
-    for (int32_t r = 0; r < h.n_ranks; r++) {
-      if (partition >= 0 && h.part_of_rank[r] != partition) continue;
-      int32_t max_loads = (int32_t)((uint32_t)jmuli(h.lthreads_col[r], 50) - (uint32_t)h.linprog_col[r]);
-      if (max_loads <= 0) continue;
-      int64_t avail = jsub(h.rows[r].rem, h.cap_col[r] / 8);
-      if (avail > 0) space = (int64_t)((uint64_t)space + (uint64_t)std::min<int64_t>(avail, (int64_t)jmuli(max_loads, size_est)));
-    }
-    space /= 2;
-    free_count = (int32_t)(space / size_est);
-    int64_t d = (int64_t)((uint64_t)20 * (uint64_t)(int64_t)size_est);
-    total_count = std::max(free_count, d == 0 ? 0 : (int32_t)(d == -1 ? -st.total_capacity : st.total_capacity / d));
+    parts[s] = p;
   }
-  const int64_t cutoff = st.global_lru == INT64_MAX ? 0
-      : (int64_t)((uint64_t)st.global_lru + (uint64_t)std::max<int64_t>(age_of(st.global_lru, now) / 3, 1200000));
-  if (total_count <= 0) return 0;
-  // prohibited types of this partition -> per type id flag
-  std::vector<uint8_t> excl(h.type_slot.size(), 0);
-  if (partition >= 0)  // ids as interned when this epoch was committed: the ingest-side name table is never read here
-    for (int32_t tid : h.part_type_ids[partition])
-      if (tid >= 0 && tid < (int32_t)excl.size()) excl[tid] = 1;
-  const int nm = ds.n_models;
-  if (nm == 0) return 0;
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  cudaStream_t s = c->stream;
-  // Registry sweep -> candidates compacted in model order (stable) -> radix sort by ~lastUsed (stable: equal times keep the
-  // lower model index first) -> first of every equal-time run (N12) -> only the first `total_count` survivors leave the device.
-  // All on the device; the host applies the emission rule (MM:6711-6719) to at most total_count records.
-  const size_t n8 = (size_t)nm * 8, n4 = (size_t)nm * 4;
-  CK(c->d_in.ensure(2 * n8 + 64));        // keys[nm], keys_sel[nm]
-  CK(c->d_out.ensure(2 * n8 + 64));       // keys_sorted[nm], keys_uniq[nm]
-  CK(c->d_trace.ensure(4 * n4 + 64));     // idx_sel, idx_sorted, idx_uniq, (spare)
-  CK(c->d_cand.ensure((size_t)nm + 64));  // flags
-  CK(c->d_extra.ensure(excl.size() + 16));
-  CK(c->d_fresh.ensure((size_t)nm + 16));
-  CK(c->d_n_open.ensure(16));
-  unsigned long long *keys = c->d_in.as<unsigned long long>(), *keys_sel = keys + nm;
-  unsigned long long *keys_sorted = c->d_out.as<unsigned long long>(), *keys_uniq = keys_sorted + nm;
-  int32_t *idx_sel = c->d_trace.as<int32_t>(), *idx_sorted = idx_sel + nm, *idx_uniq = idx_sorted + nm;
-  uint8_t *flags = c->d_cand.as<uint8_t>();
-  int *d_n = c->d_n_open.as<int>();
-  CK(cudaMemcpyAsync(c->d_extra.p, excl.data(), excl.size(), cudaMemcpyHostToDevice, s));
-  if (taken) CK(cudaMemcpyAsync(c->d_fresh.p, taken, (size_t)nm, cudaMemcpyHostToDevice, s));
-  CK(cudaEventRecord(c->e0, s));
-  k_reaper_flag<<<(nm + 255) / 256, 256, 0, s>>>(ds.models.as<mmp_model_row>(), nm, c->d_extra.as<uint8_t>(), (int)excl.size(),
-                                               taken ? c->d_fresh.as<uint8_t>() : nullptr, global_lru, free_count > 0 ? 0 : 1, cutoff, flags, keys);
-  f->launches++;
+  __syncthreads();
+  // PARTITION_STATS_COMP (TCM:264-271) as partition_order: free desc, lru asc, capacity desc, partition id; with instances only
+  __shared__ int n_in;
+  if (threadIdx.x == 0) n_in = 0;
+  __syncthreads();
+  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) {
+    const RpPart x = parts[s];
+    if (tc && x.count == 0) continue;
+    int rank = 0;
+    for (int o = 0; o < n_slots; o++) {
+      const RpPart y = parts[o];
+      if (o == s || (tc && y.count == 0)) continue;
+      rank += y.free != x.free ? y.free > x.free : y.glru != x.glru ? y.glru < x.glru : y.cap != x.cap ? y.cap > x.cap : o < s;
+    }
+    order[rank] = s;
+    atomicAdd(&n_in, 1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {  // MM:6456-6463
+    plan->go = (long long)acc[0].cap > 0;
+    plan->global_lru = (long long)acc[0].free > 0 ? 0 : mn;
+    plan->n_order = slot < 0 ? n_in : 1;
+    if (slot >= 0) order[0] = slot;
+  }
+}
+// With a filter (mmp_reaper_select: one run in one partition) the candidates are only those the run may select: not taken
+// (allCandidates.set(i, null)), type allowed in the partition (MM:6681-6683), used after the cutoff without free space (MM:6685-6687)
+struct RpFilter { const uint8_t *taken, *type_excluded; int n_type_ids, need_cutoff; long long cutoff; };
+__global__ void k_rp_flag(const mmp_model_row *__restrict__ models, int n_models, const RpPlan *__restrict__ plan, RpFilter flt,
+                          uint8_t *__restrict__ flag) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n_models) return;
+  const RpPlan p = *plan;
+  const mmp_model_row r = models[m];
+  bool ok = p.go && reaper_candidate(r, p.global_lru);
+  if (ok && flt.taken && flt.taken[m]) ok = false;
+  if (ok && r.type_id < flt.n_type_ids && flt.type_excluded[r.type_id]) ok = false;
+  if (ok && flt.need_cutoff && !(r.last_used > flt.cutoff)) ok = false;
+  flag[m] = ok ? 1 : 0;
+}
+// sort keys of the compacted candidates (in model order), ~biased(lastUsed) so that ascending keys = descending time; the
+// positions past them sort last
+__global__ void k_rp_keys(const mmp_model_row *__restrict__ models, const int *__restrict__ idx, const int *__restrict__ n_cand, int n,
+                          unsigned long long *__restrict__ key) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  key[i] = i < *n_cand ? ~((unsigned long long)models[idx[i]].last_used ^ 0x8000000000000000ull) : ~0ull;
+}
+// spaceToFill (MM:6633-6649) per partition: one segmented reduction over the rank-ordered instance columns, in the reference's
+// wrapping int / long arithmetic (the sum wraps too, so the order of the additions does not matter)
+__global__ void k_rp_space(const RankRow *__restrict__ rows, const int64_t *__restrict__ cap_col, const int32_t *__restrict__ lthreads,
+                           const int32_t *__restrict__ linprog, const int32_t *__restrict__ part_of_rank, int n_ranks, int tc, int n_slots,
+                           const RpPart *__restrict__ parts, unsigned long long *__restrict__ space) {
+  __shared__ unsigned long long sacc[STATS_SMEM_PARTS + 1];
+  const bool use_smem = n_slots <= STATS_SMEM_PARTS + 1;
+  if (use_smem) for (int i = threadIdx.x; i < n_slots; i += blockDim.x) sacc[i] = 0ull;
+  __syncthreads();
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n_ranks; r += gridDim.x * blockDim.x) {
+    const int s = tc ? part_of_rank[r] : 0;
+    if (s < 0 || s >= n_slots) continue;
+    const int32_t max_loads = (int32_t)((uint32_t)jmuli(lthreads[r], 50) - (uint32_t)linprog[r]);
+    if (max_loads <= 0) continue;
+    const int64_t avail = jsub(rows[r].rem, cap_col[r] / 8);
+    if (avail <= 0) continue;
+    const int64_t lim = (int64_t)jmuli(max_loads, parts[s].size_est);
+    atomicAdd(use_smem ? &sacc[s] : &space[s], (unsigned long long)(avail < lim ? avail : lim));
+  }
+  if (use_smem) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_slots; i += blockDim.x) if (sacc[i]) atomicAdd(&space[i], sacc[i]);
+  }
+}
+// The selection of every run (clock run_t[r]), one after the other, by one block: for each partition in the plan's order, the
+// sorted candidates are walked in chunks of RP_WALK.  Per chunk: eligible = not taken by
+// this run, type allowed in the partition (MM:6681-6683) and (free space or lastUsed > cutoff) (MM:6685-6688); of an
+// equal-lastUsed run of eligible entries only the first counts (N12; a block-wide max scan finds each entry's previous
+// eligible entry); the counted entries take ranks k by a block-wide sum scan, and the first totalProactiveLoadCount of them
+// go through the emission rule (MM:6711-6719), which, the list being in descending lastUsed, emits a prefix of them.  The walk
+// stops at the count, at the rule's break, or (full partition) at the first entry at or under the cutoff.  Emitted models are
+// tagged taken and appended as (model, run).  sel_off = [the runs' offsets | total].
+constexpr int RP_WALK = 1024;
+__global__ void __launch_bounds__(RP_WALK) k_rp_walk(const mmp_model_row *__restrict__ models, const unsigned long long *__restrict__ skey,
+                                                      const int *__restrict__ sidx, const int *__restrict__ n_cand, const RpPlan *__restrict__ plan,
+                                                      const RpPart *__restrict__ parts, const int *__restrict__ order,
+                                                      const unsigned long long *__restrict__ space, int tc, const int *__restrict__ pt_off,
+                                                      const int *__restrict__ pt_ids, const long long *__restrict__ run_t, int n_rp, int gen0,
+                                                      int *__restrict__ taken, int2 *__restrict__ sel, long long sel_cap, int *__restrict__ sel_off) {
+  using Scan = cub::BlockScan<int, RP_WALK>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ unsigned long long chunk_key[RP_WALK];
+  const int tid = threadIdx.x;
+  const int ncand = *n_cand;
+  const RpPlan P = *plan;
+  long long out = 0;
+  for (int r = 0; r < n_rp; r++) {
+    if (tid == 0) sel_off[r] = (int)out;
+    const int gen = gen0 + r;
+    const long long t = run_t[r];
+    for (int oi = 0; P.go && ncand > 0 && oi < P.n_order; oi++) {
+      const int s = order[oi];
+      const RpPart p = parts[s];
+      int free_count, total;
+      long long cutoff;
+      if (!rp_counts(p, space[s], t, free_count, total, cutoff)) break;  // the exception: the run ends here
+      if (total <= 0) continue;
+      const int *ex = tc ? pt_ids + pt_off[s] : nullptr;
+      const int nex = tc ? pt_off[s + 1] - pt_off[s] : 0;
+      int kept = 0, emitted = 0;
+      bool have_prev = false;
+      unsigned long long prev_key = 0;
+      for (int base = 0; base < ncand; base += RP_WALK) {
+        const int i = base + tid;
+        int m = -1;
+        unsigned long long key = ~0ull;
+        bool elig = false;
+        if (i < ncand) {
+          m = sidx[i]; key = skey[i];
+          elig = taken[m] != gen && (free_count > 0 || rp_last_used(key) > cutoff);
+          if (elig && nex) {  // the partition's prohibited type ids, sorted
+            const int ty = models[m].type_id;
+            int lo = 0, hi = nex;
+            while (lo < hi) { const int mid = (lo + hi) >> 1; if (ex[mid] < ty) lo = mid + 1; else hi = mid; }
+            elig = !(lo < nex && ex[lo] == ty);
+          }
+        }
+        chunk_key[tid] = key;
+        int prev, last;
+        Scan(tmp).ExclusiveScan(elig ? tid : -1, prev, -1, cub::Max(), last);
+        __syncthreads();
+        const bool hp = prev >= 0 || have_prev;
+        const unsigned long long pk = prev >= 0 ? chunk_key[prev] : prev_key;
+        const int first = elig && !(hp && pk == key) ? 1 : 0;
+        int j, n_first;
+        Scan(tmp).ExclusiveSum(first, j, n_first);
+        const int k = kept + j;
+        const bool emit = first && rp_emits(k, free_count, total, rp_last_used(key), cutoff);
+        const int n_emit = __syncthreads_count(emit);
+        if (emit) {
+          taken[m] = gen;
+          const long long pos = out + k;
+          if (pos < sel_cap) sel[pos] = make_int2(m, r);
+        }
+        kept += n_first; emitted += n_emit;
+        if (last >= 0) { have_prev = true; prev_key = chunk_key[last]; }
+        bool stop = n_emit < n_first || kept >= total || base + RP_WALK >= ncand;
+        if (free_count == 0 && rp_last_used(chunk_key[RP_WALK - 1]) <= cutoff) stop = true;  // nothing eligible past it
+        __syncthreads();
+        if (stop) break;
+      }
+      out += emitted;
+    }
+  }
+  if (tid == 0) sel_off[n_rp] = (int)out;
+}
+
+// mmp_reaper_select's run over its filtered candidates, sorted: only the first of an equal-lastUsed run counts (N12, an entry
+// whose key differs from its predecessor's); rank[i] = the counted entries before i.  The emission rule then emits a prefix of
+// the counted entries (the list descends in lastUsed): out[k] = the k-th, n_out = how many.
+struct RpFirst {
+  const unsigned long long *key;
+  __device__ int operator()(int i) const { return i == 0 || key[i] != key[i - 1] ? 1 : 0; }
+};
+__global__ void k_rp_pick(const unsigned long long *__restrict__ skey, const int *__restrict__ sidx, const int *__restrict__ rank, int n,
+                          int free_count, int total, long long cutoff, int *__restrict__ out, int *__restrict__ n_out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long key = skey[i];
+  if (i > 0 && skey[i - 1] == key) return;
+  const int k = rank[i];
+  if (!rp_emits(k, free_count, total, rp_last_used(key), cutoff)) return;
+  out[k] = sidx[i];
+  atomicMax(n_out, k + 1);
+}
+
+// The pass's stages, on stream st after k_stats filled acc / min_lru for the snapshot ds.  tc = 0: one slot, the whole
+// cluster with no type exclusion; slot >= 0: the runs take that partition alone.
+struct RpBufs { RpPart *parts; unsigned long long *space; RpPlan *plan; int *order; };
+// plan and PARTITION_STATS_COMP order (k_rp_plan), spaceToFill per partition (k_rp_space)
+static int32_t rp_plan_stage(mmp_fleet *f, const DeviceSnapshot &ds, int tc, int slot, const StatsAcc *acc, const long long *min_lru,
+                             RpScratch &rs, cudaStream_t st, RpBufs &b) {
+  const HostSnapshot &h = ds.host;
+  const int ns = tc ? (int)h.part_types.size() : 1;
+  const size_t parts_b = (size_t)ns * sizeof(RpPart), space_b = (size_t)ns * 8;
+  CK(rs.plan.ensure(parts_b + space_b + sizeof(RpPlan) + (size_t)ns * 4 + 16));
+  b.parts = rs.plan.as<RpPart>();
+  b.space = reinterpret_cast<unsigned long long *>(rs.plan.as<char>() + parts_b);
+  b.plan = reinterpret_cast<RpPlan *>(rs.plan.as<char>() + parts_b + space_b);
+  b.order = reinterpret_cast<int *>(b.plan + 1);
+  k_rp_plan<<<1, 256, 0, st>>>(acc, min_lru, ns, tc, slot, f->hs.cfg.default_model_size_units, b.parts, b.order, b.plan, b.space);
+  if (h.n_ranks > 0)
+    k_rp_space<<<std::min(f->sm_count, (h.n_ranks + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(),
+                                                                            ds.lthreads_col.as<int32_t>(), ds.linprog_col.as<int32_t>(),
+                                                                            ds.part_of_rank.as<int32_t>(), h.n_ranks, tc, ns, b.parts, b.space);
+  f->launches += 1 + (h.n_ranks > 0);
   CK(cudaGetLastError());
+  return MMP_OK;
+}
+// the candidates (k_rp_flag) compacted in model order into rs.idx, their count behind the sorted indices; cub_tmp is sized for
+// the compaction and for a sort of every model
+static int32_t rp_candidates(mmp_fleet *f, const mmp_model_row *models, int NM, const RpPlan *plan, const RpFilter &flt, RpScratch &rs,
+                             DevBuf &cub_tmp, cudaStream_t st, int **d_n) {
+  const size_t nmx = (size_t)std::max(NM, 1);
+  CK(rs.keys.ensure(nmx * 16)); CK(rs.idx.ensure(nmx * 8 + 16)); CK(rs.flag.ensure(nmx));
+  unsigned long long *keys = rs.keys.as<unsigned long long>();
+  int *idx = rs.idx.as<int>();
+  *d_n = idx + 2 * nmx;
+  k_rp_flag<<<(int)((nmx + 255) / 256), 256, 0, st>>>(models, NM, plan, flt, rs.flag.as<uint8_t>());
   thrust::counting_iterator<int32_t> iota(0);
-  size_t t1 = 0, t2 = 0, t3 = 0;
-  CK(cub::DeviceSelect::Flagged(nullptr, t1, keys, flags, keys_sel, d_n, nm, s));
-  CK(cub::DeviceSelect::Flagged(nullptr, t2, iota, flags, idx_sel, d_n, nm, s));
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, t3, keys_sel, keys_sorted, idx_sel, idx_sorted, nm, 0, 64, s));
-  CK(c->d_cub.ensure(std::max(t1, std::max(t2, t3)) + 64));
-  CK(cub::DeviceSelect::Flagged(c->d_cub.p, t1, keys, flags, keys_sel, d_n, nm, s));
-  CK(cub::DeviceSelect::Flagged(c->d_cub.p, t2, iota, flags, idx_sel, d_n, nm, s));
-  int ncand = 0;
-  CK(cudaMemcpyAsync(&ncand, d_n, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  size_t t1 = 0, t2 = 0;
+  CK(cub::DeviceSelect::Flagged(nullptr, t1, iota, rs.flag.as<uint8_t>(), idx, *d_n, NM, st));
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, t2, keys, keys + nmx, idx, idx + nmx, NM, 0, 64, st));
+  CK(cub_tmp.ensure(std::max(t1, t2) + 16));
+  CK(cub::DeviceSelect::Flagged(cub_tmp.p, t1, iota, rs.flag.as<uint8_t>(), idx, *d_n, NM, st));
   f->launches += 2;
-  if (ncand == 0) return 0;
-  CK(cub::DeviceRadixSort::SortPairs(c->d_cub.p, t3, keys_sel, keys_sorted, idx_sel, idx_sorted, ncand, 0, 64, s));
-  k_unique_mark<<<(ncand + 255) / 256, 256, 0, s>>>(keys_sorted, ncand, flags);
-  CK(cub::DeviceSelect::Flagged(c->d_cub.p, t1, keys_sorted, flags, keys_uniq, d_n, ncand, s));
-  CK(cub::DeviceSelect::Flagged(c->d_cub.p, t2, idx_sorted, flags, idx_uniq, d_n, ncand, s));
-  f->launches += 4;
   CK(cudaGetLastError());
-  CK(cudaEventRecord(c->e1, s));
-  int nuniq = 0;
-  CK(cudaMemcpyAsync(&nuniq, d_n, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_reaper_ms = ms; }
-  const int take = std::min(nuniq, total_count);
-  std::vector<unsigned long long> hk((size_t)take);
-  std::vector<int32_t> hm((size_t)take);
-  if (take) {
-    CK(cudaMemcpyAsync(hk.data(), keys_uniq, (size_t)take * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(hm.data(), idx_uniq, (size_t)take * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+  return MMP_OK;
+}
+// the first n compacted entries by (lastUsed desc, model asc) (k_rp_keys + a stable radix sort) into rs.keys + nmx / rs.idx + nmx
+static int32_t rp_sort(mmp_fleet *f, const mmp_model_row *models, int NM, int n, RpScratch &rs, DevBuf &cub_tmp, cudaStream_t st) {
+  const size_t nmx = (size_t)std::max(NM, 1);
+  unsigned long long *keys = rs.keys.as<unsigned long long>();
+  int *idx = rs.idx.as<int>();
+  k_rp_keys<<<(int)((std::max(n, 1) + 255) / 256), 256, 0, st>>>(models, idx, idx + 2 * nmx, n, keys);
+  size_t t = cub_tmp.cap;
+  CK(cub::DeviceRadixSort::SortPairs(cub_tmp.p, t, keys, keys + nmx, idx, idx + nmx, n, 0, 64, st));
+  f->launches += 3;
+  CK(cudaGetLastError());
+  return MMP_OK;
+}
+
+// The closed loop's selection for the runs run_t (their clocks): every run walks the partitions in PARTITION_STATS_COMP
+// order over all the candidates, sorted once (k_rp_walk).  Run r tags the models it selects gen + 1 + r in rs.taken, which the
+// caller fills (tags other than the run's own do not count as taken); gen advances past the tags used.  Selections land in
+// rs.sel as (model, run) in emission order, their offsets per run in rs.off.  The total is read back (one synchronisation);
+// a second walk follows only when the selections outgrow rs.sel.
+static int32_t reaper_pass(mmp_fleet *f, const DeviceSnapshot &ds, const mmp_model_row *models, int n_models, int tc,
+                           const StatsAcc *acc, const long long *min_lru, const std::vector<long long> &run_t, int32_t &gen,
+                           RpScratch &rs, DevBuf &cub_tmp, cudaStream_t st, int32_t *n_sel) {
+  const HostSnapshot &h = ds.host;
+  const int NM = n_models, R = (int)run_t.size(), ns = tc ? (int)h.part_types.size() : 1;
+  const size_t nmx = (size_t)std::max(NM, 1);
+  // one upload: the runs' clocks, then each partition's prohibited type ids of this epoch, sorted: [offsets (ns + 1) | ids]
+  std::vector<int> pt((size_t)ns + 1, 0);
+  for (int p = 0; tc && p < ns; p++) {
+    std::vector<int> ids;
+    for (int32_t tid : h.part_type_ids[p]) if (tid >= 0 && tid < (int32_t)h.type_slot.size()) ids.push_back(tid);
+    std::sort(ids.begin(), ids.end());
+    pt.insert(pt.end(), ids.begin(), ids.end());
+    pt[p + 1] = pt[p] + (int)ids.size();
   }
-  int64_t emitted = 0;
-  int32_t free_left = free_count;
-  for (int i = 0; i < take; i++) {
-    const int64_t ts = (int64_t)((~hk[i]) ^ 0x8000000000000000ull);
-    if (free_left > 0) free_left--;          // MM:6713-6714
-    else if (ts < cutoff) break;             // MM:6715-6717
-    const int32_t m = hm[i];
-    if (taken) taken[m] = 1;
-    if (emitted < cap) out_models[emitted] = m;
-    emitted++;
+  std::vector<long long> up(run_t);
+  up.resize((size_t)R + (pt.size() + 1) / 2);
+  memcpy(up.data() + R, pt.data(), pt.size() * 4);
+  CK(upload_vec(rs.runs, up, st));
+  const long long *d_t = rs.runs.as<long long>();
+  const int *pt_off = reinterpret_cast<const int *>(d_t + R), *pt_ids = pt_off + ns + 1;
+  CK(rs.sel.ensure(nmx * sizeof(int2)));  // (one run selects each model at most once)
+  CK(rs.off.ensure((size_t)(R + 1) * 4));
+  RpBufs b;
+  int *d_n = nullptr;
+  int32_t rc = rp_plan_stage(f, ds, tc, -1, acc, min_lru, rs, st, b);
+  if (rc == MMP_OK) rc = rp_candidates(f, models, NM, b.plan, RpFilter{}, rs, cub_tmp, st, &d_n);
+  if (rc == MMP_OK) rc = rp_sort(f, models, NM, NM, rs, cub_tmp, st);  // (the positions past the candidates sort last)
+  if (rc < 0) return rc;
+  const unsigned long long *skeys = rs.keys.as<unsigned long long>() + nmx;
+  const int *sidx = rs.idx.as<int>() + nmx;
+  int *d_off = rs.off.as<int>();
+  for (int pass = 0;; pass++) {
+    const long long sel_cap = (long long)(rs.sel.cap / sizeof(int2));
+    k_rp_walk<<<1, RP_WALK, 0, st>>>(models, skeys, sidx, d_n, b.plan, b.parts, b.order, b.space, tc, pt_off, pt_ids, d_t, R, gen + 1,
+                                     rs.taken.as<int>(), rs.sel.as<int2>(), sel_cap, d_off);
+    f->launches++;
+    CK(cudaGetLastError());
+    gen += R;
+    int total = 0;
+    CK(cudaMemcpyAsync(&total, d_off + R, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (total <= sel_cap) { *n_sel = total; return MMP_OK; }
+    if (pass) { g_err = "internal: the reaper's selections changed between two walks"; return MMP_E_STATE; }
+    CK(rs.sel.ensure((size_t)total * sizeof(int2)));
   }
-  return (int32_t)std::min<int64_t>(emitted, INT32_MAX);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -765,9 +914,121 @@ int32_t mmp_stats(mmp_fleet *f, mmp_cluster_stats *out, int32_t *part_ids, int32
   return n;
 }
 
+// One run at now_ms on the lease's stream, in one partition: -1 is the whole cluster without type exclusion (on a constrained
+// fleet too), p >= 0 that partition alone.  The pass's stages with a read-back after each: the plan (the call ends when the
+// run has nothing to select), the candidates the run may select (k_rp_flag with its filter: ends when there are none), their
+// sort, and k_rp_pick, the walk's N12 and emission rule over one run's list in parallel.
 int32_t mmp_reaper_select(mmp_fleet *f, int32_t partition, int64_t now_ms, uint8_t *taken, int32_t *out_models, int32_t cap) {
   NEED(f);
-  return reaper_impl(f, partition, now_ms, taken, out_models, cap);
+  if (!out_models || cap < 0) { g_err = "bad argument"; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
+  if (f->epoch == 0) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  const DeviceSnapshot &ds = f->snaps[f->cur];
+  const HostSnapshot &h = ds.host;
+  const int np = (int)h.part_types.size(), nm = ds.n_models, tc = partition >= 0 ? 1 : 0;
+  if (partition >= np || (partition >= 0 && !h.tc_enabled)) { g_err = "no such partition"; return MMP_E_ARG; }
+  if (nm == 0) return 0;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t s = c->stream;
+  RpScratch &rs = c->rp;
+  const mmp_model_row *models = ds.models.as<mmp_model_row>();
+  // stats: [acc (np + 1) | the cluster's LRU, from Long.MAX_VALUE (ISST)]
+  const size_t acc_b = (size_t)(np + 1) * sizeof(StatsAcc);
+  CK(c->d_trace.ensure(acc_b + 8));
+  long long *d_min = reinterpret_cast<long long *>(c->d_trace.as<char>() + acc_b);
+  static const long long lru_init = 0x7fffffffffffffffLL;
+  CK(cudaMemsetAsync(c->d_trace.p, 0, acc_b, s));
+  CK(cudaMemcpyAsync(d_min, &lru_init, 8, cudaMemcpyHostToDevice, s));
+  if (h.n_ranks > 0) {
+    k_stats<<<std::min(f->sm_count, (h.n_ranks + 255) / 256), 256, 0, s>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(),
+                                                                          ds.part_of_rank.as<int32_t>(), h.n_ranks, f->hs.cfg.min_space_units,
+                                                                          c->d_trace.as<StatsAcc>(), d_min, np);
+    f->launches++;
+  }
+  RpBufs b;
+  const int slot = tc ? partition : 0, ns = tc ? np : 1;
+  rc = rp_plan_stage(f, ds, tc, slot, c->d_trace.as<StatsAcc>(), d_min, rs, s, b);
+  if (rc < 0) return rc;
+  // one read-back of [parts | space | plan] (b's layout in rs.plan)
+  std::vector<char> hb((size_t)ns * (sizeof(RpPart) + 8) + sizeof(RpPlan));
+  CK(cudaMemcpyAsync(hb.data(), rs.plan.p, hb.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  RpPart part;
+  RpPlan plan;
+  unsigned long long space;
+  memcpy(&part, hb.data() + (size_t)slot * sizeof(RpPart), sizeof(RpPart));
+  memcpy(&space, hb.data() + (size_t)ns * sizeof(RpPart) + (size_t)slot * 8, 8);
+  memcpy(&plan, hb.data() + (size_t)ns * (sizeof(RpPart) + 8), sizeof(RpPlan));
+  if (!plan.go) return 0;  // MM:6456
+  int free_count = 0, total = 0;
+  long long cutoff = 0;
+  const bool counted = rp_counts(part, space, now_ms, free_count, total, cutoff);
+  if (counted && total <= 0) return 0;
+  auto timed = [&](int32_t r) {  // t_reaper_ms: from the candidate sweep to the last stage run
+    float ms = 0;
+    if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_reaper_ms = ms;
+    return r;
+  };
+  // the candidates: those of the base rule alone when the size estimate is 0 (the reference throws only when there is one,
+  // MM:6470), else those this run may select
+  RpFilter flt{};
+  std::vector<uint8_t> excl(tc ? h.type_slot.size() : 0, 0);
+  if (counted) {
+    for (int32_t tid : tc ? h.part_type_ids[partition] : std::vector<int32_t>())
+      if (tid >= 0 && tid < (int32_t)excl.size()) excl[tid] = 1;
+    CK(c->d_extra.ensure(excl.size() + 16));
+    if (!excl.empty()) CK(cudaMemcpyAsync(c->d_extra.p, excl.data(), excl.size(), cudaMemcpyHostToDevice, s));
+    if (taken) {
+      CK(c->d_fresh.ensure((size_t)nm));
+      CK(cudaMemcpyAsync(c->d_fresh.p, taken, (size_t)nm, cudaMemcpyHostToDevice, s));
+    }
+    flt = RpFilter{taken ? c->d_fresh.as<uint8_t>() : nullptr, c->d_extra.as<uint8_t>(), (int)excl.size(), free_count > 0 ? 0 : 1, cutoff};
+  }
+  int *d_n = nullptr;
+  CK(cudaEventRecord(c->e0, s));
+  rc = rp_candidates(f, models, nm, b.plan, flt, rs, c->d_cub, s, &d_n);
+  if (rc < 0) return rc;
+  int ncand = 0;
+  CK(cudaMemcpyAsync(&ncand, d_n, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaEventRecord(c->e1, s));
+  CK(cudaStreamSynchronize(s));
+  if (ncand == 0) return timed(0);
+  if (!counted) { timed(0); g_err = "size estimate is zero (the reference would throw ArithmeticException)"; return MMP_E_ARG; }
+  rc = rp_sort(f, models, nm, ncand, rs, c->d_cub, s);
+  if (rc < 0) return rc;
+  const size_t nmx = (size_t)nm;
+  int *rank = rs.idx.as<int>();  // (the unsorted indices are spent)
+  int *out = reinterpret_cast<int *>(rs.keys.as<unsigned long long>());
+  CK(rs.sel.ensure(16));
+  int *d_out_n = rs.sel.as<int>();
+  auto first = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), RpFirst{rs.keys.as<unsigned long long>() + nmx});
+  size_t t = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t, first, rank, ncand, s));
+  CK(c->d_cub.ensure(t + 16));
+  CK(cub::DeviceScan::ExclusiveSum(c->d_cub.p, t, first, rank, ncand, s));
+  CK(cudaMemsetAsync(d_out_n, 0, 4, s));
+  k_rp_pick<<<(ncand + 255) / 256, 256, 0, s>>>(rs.keys.as<unsigned long long>() + nmx, rs.idx.as<int>() + nmx, rank, ncand, free_count,
+                                                total, cutoff, out, d_out_n);
+  f->launches += 2;
+  CK(cudaGetLastError());
+  int n = 0;
+  CK(cudaMemcpyAsync(&n, d_out_n, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaEventRecord(c->e1, s));
+  CK(cudaStreamSynchronize(s));
+  timed(0);
+  std::vector<int32_t> sel((size_t)n);
+  if (n) {
+    CK(cudaMemcpyAsync(sel.data(), out, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  for (int32_t i = 0; i < n; i++) {  // every selection is taken, those past cap too
+    if (taken) taken[sel[i]] = 1;
+    if (i < cap) out_models[i] = sel[i];
+  }
+  return n;
 }
 
 int32_t mmp_lru_init(mmp_fleet *f, int32_t n, const int64_t *capacity, int32_t slots) {

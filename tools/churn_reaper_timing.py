@@ -6,13 +6,17 @@ int cast, the size estimate is negative and the reaper selects nothing, so the p
 Prints one JSON line per workload: medians over the timed windows of the host clock around the step, the step's CUDA-event
 total and its reaper pass (ms_reaper, its one read-back included), the models the reaper decided in each timed window and
 the median of all decisions per window, and the GPU's name and power limit with the clocks and throttle reasons sampled in
-the timed region.  MMP_LIB selects another build of the library.
+the timed region.  A second leg times mmp_reaper_select on each fleet's committed snapshot: one round calls it for every
+partition in mmp_stats order (the cluster, -1, on a fleet without type constraints) with one taken array, as the leader's
+reaper does; medians over the timed rounds of the host clock around each call (its read-backs included) and of its
+CUDA-event time (mmp_last_timing "reaper"), and the models a round selects.  MMP_LIB selects another build of the library.
 
-    python tools/churn_reaper_timing.py [--windows 10] [--warmup 3]
+    python tools/churn_reaper_timing.py [--windows 10] [--warmup 3] [--calls 30]
 """
 from __future__ import annotations
 
 import argparse
+import ctypes as C
 import json
 import os
 import subprocess
@@ -66,18 +70,52 @@ def time_windows(lib, w, windows: int, warmup: int, events: int, seed: int, reap
             "reaper_decisions": picked, "decisions": int(np.median(decided)), "clocks_sm_max_throttle": clocks}
 
 
+def time_select(lib, w, calls: int, warmup: int) -> dict:
+    fl = w.fleet
+    s = Fleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, fl.n_instances, fl.n_models, lib=lib)
+    load_into_fleet(fl, s)
+    _, ids = s.stats()
+    parts = [int(p) for p in ids[1:]] or [-1]
+    taken = np.zeros(s.max_models, dtype=np.uint8)
+    out = np.zeros(s.max_models, dtype=np.int32)
+    ms = C.c_double()
+    wall, dev, picked = [], [], []
+    for it in range(warmup + calls):
+        taken[:] = 0
+        n_round = 0
+        for p in parts:
+            s._ck(lib.mmp_flush_l2(s.h))
+            t0 = time.perf_counter()
+            n = s._ck(lib.mmp_reaper_select(s.h, p, fl.now_ms, taken.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p), len(out)))
+            dt = time.perf_counter() - t0
+            s._ck(lib.mmp_last_timing(s.h, b"reaper", C.byref(ms)))
+            n_round += n
+            if it >= warmup:
+                wall.append(1e3 * dt); dev.append(float(ms.value))
+        if it >= warmup:
+            picked.append(n_round)
+    s.close()
+    return {"leg": "mmp_reaper_select", "calls": calls, "partitions": len(parts), "ms_call_wall": float(np.median(wall)),
+            "ms_call_wall_min_max": [float(np.min(wall)), float(np.max(wall))], "ms_reaper": float(np.median(dev)),
+            "ms_reaper_min_max": [float(np.min(dev)), float(np.max(dev))], "selected_per_round": int(np.median(picked))}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--windows", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--events", type=int, default=20_000)
+    ap.add_argument("--calls", type=int, default=30)
+    ap.add_argument("--select-only", action="store_true", help="only the mmp_reaper_select leg")
     args = ap.parse_args()
     lib = _lib.load_product()
     gpu = nvidia_smi("name,power.limit")
     for name in ("C4", "C4 at 80 % fill"):
         w = make_churn(500_000, 2_500, 4, fill=0.8 if "80" in name else 0.97)
-        for reaper in (False, True):
-            res = time_windows(lib, w, args.windows, args.warmup, args.events, 4, reaper)
+        legs = [] if args.select_only else [lambda r=r: time_windows(lib, w, args.windows, args.warmup, args.events, 4, r) for r in (False, True)]
+        legs.append(lambda: time_select(lib, w, args.calls, args.warmup))
+        for leg in legs:
+            res = leg()
             res.update({"workload": name, "gpu": gpu, "lib": os.environ.get("MMP_LIB", "in-tree")})
             print(json.dumps(res), flush=True)
 
