@@ -17,8 +17,9 @@
 // Kernels (DESIGN.md §5, §7):
 //   k_place_direct<4, 5>     the scoring kernel (default): one decision per lane, the row rebuilt from the model's excl_ranks,
 //                            longer walks through the word lists; optional slot-sorted batches (k_slot_keys + cub radix sort)
-//   k_slot_summary, k_place_split, k_place_walk<4, 5>, k_place_ovf   large batches in two passes (launch_split): per-slot
-//                            summaries answer the decisions clear of their slot's reach, k_place_direct's body walks the rest
+//   k_slot_summary, k_place_split, k_place_tail<4, 5>   large batches in two passes (launch_split): per-slot summaries
+//                            answer the decisions clear of their slot's reach, k_place_direct's body walks the rest and a
+//                            warp resolves each decision of a model with overflow ids
 //   k_place_lanes            round 1's streaming kernel (whole rows through TMA landing stages): MMP_KERNEL=lanes and the
 //                            collective instance-shard path
 //   k_place_small            tiny batches as a stream launch / replayed CUDA graph;  k_place_server: the resident B = 1 server
@@ -663,16 +664,25 @@ __global__ void k_slot_keys(const SnapshotView s, const mmp_decision_in *__restr
   keys[i] = (uint16_t)k;
   idx[i] = i;
 }
+// a warp's slices of shared memory in place_direct: its lanes' window buffers and walk chunks, and the context of the
+// decision its warp redo is resolving
 template <int WARPS>
-__device__ __forceinline__ void place_direct(const SnapshotView &s, const mmp_decision_in *__restrict__ in, int n,
+struct DirectSmem {
+  uint32_t win_s[WARPS][32 * LANE_STRIDE];
+  uint32_t chunk_s[WARPS][32 * MMP_CHUNK_WORDS];
+  DecisionCtx ctx_w[WARPS];
+};
+// the tile of 32 positions of the batch from j0 (perm: through it), one per lane of the calling warp
+template <int WARPS>
+__device__ __forceinline__ void place_direct(DirectSmem<WARPS> &sm, int j0, const SnapshotView &s, const mmp_decision_in *__restrict__ in, int n,
                                              const FreshRow *__restrict__ fresh, int n_fresh, const int32_t *__restrict__ extra,
                                              mmp_decision_out *__restrict__ out, int64_t now, uint64_t seed, uint64_t id_base, int budget,
                                              const int32_t *__restrict__ perm) {
-  __shared__ uint32_t win_s[WARPS][32 * LANE_STRIDE];
-  __shared__ uint32_t chunk_s[WARPS][32 * MMP_CHUNK_WORDS];
-  __shared__ DecisionCtx ctx_w[WARPS];
+  auto &win_s = sm.win_s;
+  auto &chunk_s = sm.chunk_s;
+  auto &ctx_w = sm.ctx_w;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int j_ = (blockIdx.x * WARPS + warp) * 32 + lane;
+  const int j_ = j0 + lane;
   const bool valid = j_ < n;
   // perm (optional): the batch in type-slot order -- decisions of one slot walk the same masks, so the 32 lanes of a warp
   // finish their walks together instead of waiting for the longest (fleets with sparse candidate sets: C5)
@@ -716,30 +726,20 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
                                                                   const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
                                                                   int64_t now, uint64_t seed, uint64_t id_base, int budget,
                                                                   const int32_t *__restrict__ perm) {
-  place_direct<WARPS>(s, in, n, fresh, n_fresh, extra, out, now, seed, id_base, budget, perm);
-}
-// k_place_direct over the first *n_live positions of perm, a worklist whose length is on the device (the grid is sized
-// for n: blocks past the length leave at once)
-template <int WARPS, int MINB>
-__global__ void __launch_bounds__(WARPS * 32, MINB) k_place_walk(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
-                                                                const FreshRow *__restrict__ fresh, int n_fresh,
-                                                                const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
-                                                                int64_t now, uint64_t seed, uint64_t id_base, int budget,
-                                                                const int32_t *__restrict__ perm, const int32_t *__restrict__ n_live) {
-  n = min(n, __ldg(n_live));
-  if ((int)(blockIdx.x * WARPS * 32) >= n) return;
-  place_direct<WARPS>(s, in, n, fresh, n_fresh, extra, out, now, seed, id_base, budget, perm);
+  __shared__ DirectSmem<WARPS> sm;
+  place_direct<WARPS>(sm, (blockIdx.x * WARPS + (threadIdx.x >> 5)) * 32, s, in, n, fresh, n_fresh, extra, out, now, seed, id_base, budget, perm);
 }
 
 // ---- the two-pass path of a large batch (launch_place, DESIGN.md §5.2) ----
 // one lane per (type slot, c_self): the slot summaries of this call's view (slot_summary); also zeroes the worklist counters
+// and k_place_tail's work counter
 __global__ void __launch_bounds__(128) k_slot_summary(const SnapshotView s, int64_t now, SlotSummary *__restrict__ sums,
                                                       int32_t *__restrict__ members, int32_t *__restrict__ counts) {
   __shared__ uint32_t win_s[4][32 * LANE_STRIDE];
   __shared__ uint32_t chunk_s[4][32 * MMP_CHUNK_WORDS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int t = blockIdx.x * 128 + threadIdx.x, sl = t >> 1, cs = t & 1;
-  if (t < 2) counts[t] = 0;
+  if (t < 3) counts[t] = 0;
   const bool active = sl < s.n_slots;
   uint32_t *w = win_s[warp] + lane * LANE_STRIDE;
 #pragma unroll
@@ -762,7 +762,7 @@ __device__ __forceinline__ void warp_append(bool p, int32_t v, int32_t *list, in
   if (p) list[base + __popc(m & ((1u << lane) - 1u))] = v;
 }
 // one thread per decision: answered from its slot's summary (split_answer), or put on a worklist -- a model with overflow
-// ids on ovf_list (k_place_ovf), everything else on walk_list (k_place_direct).  keys / key_idx (sparse snapshots): the
+// ids on ovf_list, everything else on walk_list (k_place_tail takes both).  keys / key_idx (sparse snapshots): the
 // slot-order sort of the batch, the walked decisions' keys below everyone else's.
 __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
                                                      const FreshRow *__restrict__ fresh, int n_fresh, mmp_decision_out *__restrict__ out,
@@ -795,23 +795,39 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
     key_idx[i] = i;
   }
 }
-// the decisions of ovf_list (length *count), one warp each, resolved as k_place_direct's warp redo resolves them
-__global__ void __launch_bounds__(128) k_place_ovf(const SnapshotView s, const mmp_decision_in *__restrict__ in, const int32_t *__restrict__ list,
-                                                   const int32_t *__restrict__ count, const FreshRow *__restrict__ fresh, int n_fresh,
-                                                   const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out, int64_t now,
-                                                   uint64_t seed, uint64_t id_base) {
-  __shared__ DecisionCtx ctx_w[4];
+// The decisions k_place_split could not answer, in one persistent launch (resident blocks of 4 warps): each warp takes
+// work items from counts[2] until none is left.  Items 0 .. ceil(counts[0] / 32) - 1 are tiles of 32 positions of perm
+// (the walk list, or its slot-order sort), resolved by k_place_direct's body; the next counts[1] are the decisions of
+// ovf_list, one each, resolved from the model's bitmap row as the warp redo resolves them.  Walk tiles go first: on C3
+// that measured 20.7 us per call against 22.8 with the overflow decisions first (DESIGN.md §5.2.1).
+template <int WARPS, int MINB>
+__global__ void __launch_bounds__(WARPS * 32, MINB) k_place_tail(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
+                                                                const FreshRow *__restrict__ fresh, int n_fresh,
+                                                                const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
+                                                                int64_t now, uint64_t seed, uint64_t id_base, int budget,
+                                                                const int32_t *__restrict__ perm, const int32_t *__restrict__ ovf_list,
+                                                                int32_t *__restrict__ counts) {
+  __shared__ DirectSmem<WARPS> sm;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int n = __ldg(count);
-  for (int k = blockIdx.x * 4 + warp; k < n; k += gridDim.x * 4) {
-    const int i = list[k];
-    const mmp_decision_in d = in[i];
-    if (lane == 0) prepare_ctx(s, d, fresh, n_fresh, extra, ctx_w[warp]);
-    __syncwarp();
-    int32_t t, c;
-    decide_warp(s, ctx_w[warp], excl_row(s, excl_row_id(s, d.model, d.flags)), extra, now, seed, pick_id(d, id_base + (uint64_t)i), &t, &c);
-    if (lane == 0) out[i] = mmp_decision_out{t, c};
-    __syncwarp();
+  const int n_walk = min(n, __ldg(counts)), n_ovf = __ldg(counts + 1);
+  const int walk_items = (n_walk + 31) >> 5;
+  for (;;) {
+    int item = 0;
+    if (lane == 0) item = atomicAdd(counts + 2, 1);
+    item = __shfl_sync(0xffffffffu, item, 0);
+    if (item >= walk_items + n_ovf) break;
+    if (item < walk_items) {
+      place_direct<WARPS>(sm, item * 32, s, in, n_walk, fresh, n_fresh, extra, out, now, seed, id_base, budget, perm);
+    } else {
+      const int i = ovf_list[item - walk_items];
+      const mmp_decision_in d = in[i];
+      if (lane == 0) prepare_ctx(s, d, fresh, n_fresh, extra, sm.ctx_w[warp]);
+      __syncwarp();
+      int32_t t, c;
+      decide_warp(s, sm.ctx_w[warp], excl_row(s, excl_row_id(s, d.model, d.flags)), extra, now, seed, pick_id(d, id_base + (uint64_t)i), &t, &c);
+      if (lane == 0) out[i] = mmp_decision_out{t, c};
+    }
+    __syncwarp();  // the warp's slices of sm are the next item's
   }
 }
 
@@ -1474,8 +1490,9 @@ static cudaError_t sort_slot_keys(mmp_fleet *f, const PlaceArgs &a, cudaStream_t
 
 // The two-pass path of a k_place_direct batch (DESIGN.md §5.2): the slot summaries of the call's view (k_slot_summary), one
 // streaming pass that answers every decision lying clear of its slot's reach and lists the others (k_place_split), then
-// k_place_direct over the walk list -- in slot order on sparse snapshots -- and k_place_ovf over the models with overflow
-// ids.  The lists' lengths stay on the device: both launches are sized for the whole batch and stop at the length.
+// one launch over both lists (k_place_tail): k_place_direct's body over the walk list -- in slot order on sparse
+// snapshots -- and a warp per decision of a model with overflow ids.  The lists' lengths stay on the device: k_place_tail
+// is a persistent grid of resident blocks that takes its work from a device-side counter.
 static cudaError_t launch_split(mmp_fleet *f, const PlaceArgs &a, cudaStream_t st) {
   PlaceCtx *c = a.ctx;
   const int ss = sort_set(a);
@@ -1496,11 +1513,9 @@ static cudaError_t launch_split(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
   f->launches += 2;
   const int32_t *perm = c->d_walk[ss].as<int32_t>();
   if (sorted && (e = sort_slot_keys(f, a, st, &perm)) != cudaSuccess) return e;
-  k_place_walk<4, 5><<<(a.n + 127) / 128, 128, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base,
-                                                       f->lane_budget, perm, counts);
-  k_place_ovf<<<std::max(1, std::min((a.n + 3) / 4, f->sm_count * 4)), 128, 0, st>>>(a.s, a.in, c->d_ovf[ss].as<int32_t>(), counts + 1, a.fresh, a.n_fresh,
-                                                                                   a.extra, a.out, a.now, a.seed, a.id_base);
-  f->launches += 2;
+  k_place_tail<4, 5><<<std::max(1, std::min((a.n + 127) / 128, f->sm_count * 5)), 128, 0, st>>>(
+      a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, f->lane_budget, perm, c->d_ovf[ss].as<int32_t>(), counts);
+  f->launches++;
   return cudaGetLastError();
 }
 
