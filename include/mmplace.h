@@ -298,6 +298,48 @@ int32_t mmp_instance_partition(mmp_fleet *, int32_t idx);
  * constraints).  taken[] (max_models bytes, in/out, may be NULL) mirrors allCandidates.set(i, null).
  * Writes the selected model indices most-recently-used first; returns how many. */
 int32_t mmp_reaper_select(mmp_fleet *, int32_t partition, int64_t now_ms, uint8_t *taken, int32_t *out_models, int32_t cap);
+/* One run of the leader's reaper task (MM:6436-6494) against the committed epoch and the registry as of the last commit, in
+ * one call: the prune of pruneModelRegistry (MM:6536-6590, 6752-6784), repairLastUsedTimeIfNeeded (MM:6837-6850), the
+ * candidates of MM:6574-6577 on the pruned and repaired records, the selection of mmp_reaper_select over every partition and
+ * the placement of every selected model, in the reference's order:
+ *   prune     every registration, loaded and failed, exactly as mmp_registry_prune_ids (self = leader: the leader's own
+ *             registrations are never pruned; missing_since stamped the same way).  Pruned pairs in (model, registration
+ *             position) order: pruned_models[k] / pruned_instances[k].
+ *   repair    every model whose last_used is INT64_MAX (mmp_model_upsert and mmp_model_upsert_json accept the value) is taken as
+ *             now_ms - 3 x 3 600 000 (LASTUSED_AGE_ON_ADD_MS x 3) from here on: its sort position and its load's lastUsed.
+ *             Repaired models in model order.
+ *   select    the gate and globalLru of MM:6456-6463 from the epoch's stats; the candidates of a pruned record count its
+ *             remaining registrations (a pruned registration at position < copy_count was a loaded copy, any other a failed
+ *             load).  Then the closed loop's REAPER run at t = now_ms: the whole cluster without type constraints, otherwise
+ *             every partition in mmp_stats order with one shared taken set; N12 and the emission rule as mmp_reaper_select.  A
+ *             size estimate of 0 (the reference's ArithmeticException, MM:6651) ends the run at that partition: not an error,
+ *             the report names it and everything before it is real.
+ *   place     each selected model, in emission order, is getNext(model, self = leader, lastUsed = its (repaired) lastUsed)
+ *             with no flags and no extra excludes, all against the one epoch (N6); decision k draws with id k (+ id_base):
+ *             loads[k] equals mmp_place_batch of those records with the same seed.  A leader that is not live in the epoch
+ *             gets MMP_TARGET_INVALID, as mmp_place_batch answers such a decision.
+ * missing_since (max_instances entries, in/out) comes back as the reaper's `missings` map after its cleanup (MM:6601-6607):
+ * entries with now_ms - v > assume_gone_ms, or whose instance is in the instance table, are cleared (0).  This is the one
+ * difference from mmp_registry_prune_ids, which leaves the cleanup to its caller.
+ * The caller writes the pruned and repaired records back (KV conditional writes) and calls ensureLoadedInternal(model,
+ * last_used, ...) for each load whose target is not MMP_TARGET_NONE.  The outputs hold the first cap of each list; the report
+ * gives the totals.  Returns the number of loads.  Errors (nothing written): MMP_E_ARG for a leader outside
+ * [0, max_instances), a negative cap or assume_gone_ms, missing_since or report NULL, or a NULL output with a positive cap;
+ * MMP_E_EPOCH without a commit; MMP_E_STATE on an instance-sharded fleet or one that connected a communicator (placement there
+ * is a collective call every shard makes: keep mmp_registry_prune_ids + mmp_reaper_select + mmp_place_batch).  Sets the
+ * "reaper_run" timing. */
+typedef struct {
+  int32_t model, target, n_candidates, reserved;  /* target: instance index, MMP_TARGET_NONE, MMP_TARGET_SELF or MMP_TARGET_INVALID */
+  int64_t last_used;  /* the lastUsed ensureLoadedInternal is called with (MM:6712, 6727): the repaired value where repaired */
+} mmp_reaper_load;    /* 24 B */
+typedef struct {
+  int32_t n_pruned, n_repaired, n_loads;  /* totals; the outputs hold the first cap of each */
+  int32_t stopped_partition;  /* mmp_stats index of the partition whose size estimate was 0 (0: the whole cluster), -1 when
+                                 the run completed */
+} mmp_reaper_report;
+int32_t mmp_reaper_run(mmp_fleet *, int32_t leader, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since, uint64_t seed,
+                       int32_t *pruned_models, int32_t *pruned_instances, int32_t pruned_cap, int32_t *repaired_models,
+                       int32_t repaired_cap, mmp_reaper_load *loads, int32_t loads_cap, mmp_reaper_report *report);
 
 /* ---- plug point 3: per-instance time-ordered weighted LRU (CLHM:821-858, 590-652, 329-352; LD:243-288) ---- */
 enum { MMP_LRU_INSERT = 0, MMP_LRU_TOUCH = 1, MMP_LRU_RESIZE = 2, MMP_LRU_REMOVE = 3, MMP_LRU_SET_CAPACITY = 4,
@@ -498,6 +540,7 @@ int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
 /* CUDA-event duration (ms) of the device part of the last mmp_stats ("stats"), mmp_reaper_select ("reaper": the candidate
  * sweep through the selection, k_rp_flag to k_rp_pick, without the stats and plan), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
  * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
+ * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device

@@ -141,6 +141,13 @@ public final class GpuPlacement implements AutoCloseable {
     public int reaperSelect(int partition, long nowMs, ByteBuffer taken, ByteBuffer outModels, int cap) {
         return check(MmPlace.reaperSelect(h, partition, nowMs, taken, outModels, cap));
     }
+    // one run of the leader's reaper task (ModelMesh.java:6436-6494): returns the number of loads; report gets the totals
+    public int reaperRun(int leader, long nowMs, long assumeGoneMs, ByteBuffer missingSince, ByteBuffer prunedModels,
+                         ByteBuffer prunedInstances, int prunedCap, ByteBuffer repairedModels, int repairedCap, ByteBuffer loads,
+                         int loadsCap, ByteBuffer report) {
+        return check(MmPlace.reaperRun(h, leader, nowMs, assumeGoneMs, missingSince, pickSeed.incrementAndGet(), prunedModels,
+                                       prunedInstances, prunedCap, repairedModels, repairedCap, loads, loadsCap, report));
+    }
 
     private int check(int rc) { if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h)); return rc; }
     @Override public void close() { committer.shutdownNow(); MmPlace.destroy(h); }

@@ -45,6 +45,10 @@ final class MmPlace {
                                     ByteBuffer outMasks, int cap);
     static native int registryPruneIds(long h, int self, long nowMs, long assumeGoneMs, ByteBuffer missingSince, ByteBuffer outModels,
                                        ByteBuffer outInstances, int cap);
+    // the leader's reaper task in one call (MM:6436-6494): prune, repair, select over every partition, place (mmp_reaper_run)
+    static native int reaperRun(long h, int leader, long nowMs, long assumeGoneMs, ByteBuffer missingSince, long seed,
+                                ByteBuffer prunedModels, ByteBuffer prunedInstances, int prunedCap, ByteBuffer repairedModels,
+                                int repairedCap, ByteBuffer loads, int loadsCap, ByteBuffer report);
     static native int tune(long h, String key, long value);
     static native double lastTiming(long h, String key);
     // plug point 1: placement (CacheMissForwardingLB.getNext MM:4776-5004)

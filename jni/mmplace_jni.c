@@ -138,6 +138,17 @@ jint FN(registryPruneIds)(JNIEnv *env, jclass c, jlong h, jint self, jlong nowMs
   return mmp_registry_prune_ids(H(h), self, nowMs, assumeGoneMs, (int64_t *)BUF(missingSince), (int32_t *)BUF(outModels),
                                 (int32_t *)BUF(outInstances), cap);
 }
+/* one run of the leader's reaper task.  missingSince: int64[max_instances] (in/out), prunedModels / prunedInstances:
+ * int32[prunedCap], repairedModels: int32[repairedCap], loads: loadsCap x mmp_reaper_load (24 B), report: one
+ * mmp_reaper_report (16 B) -- direct buffers */
+jint FN(reaperRun)(JNIEnv *env, jclass c, jlong h, jint leader, jlong nowMs, jlong assumeGoneMs, jobject missingSince, jlong seed,
+                   jobject prunedModels, jobject prunedInstances, jint prunedCap, jobject repairedModels, jint repairedCap, jobject loads,
+                   jint loadsCap, jobject report) {
+  (void)c;
+  return mmp_reaper_run(H(h), leader, nowMs, assumeGoneMs, (int64_t *)BUF(missingSince), (uint64_t)seed, (int32_t *)BUF(prunedModels),
+                        (int32_t *)BUF(prunedInstances), prunedCap, (int32_t *)BUF(repairedModels), repairedCap,
+                        (mmp_reaper_load *)BUF(loads), loadsCap, (mmp_reaper_report *)BUF(report));
+}
 jint FN(tune)(JNIEnv *env, jclass c, jlong h, jstring key, jlong value) {
   const char *ck = utf(env, key);
   jint rc = mmp_tune(H(h), ck, value);

@@ -55,6 +55,9 @@ SCALE_PARAMS = np.dtype([("now", "<i8"), ("last_check_time", "<i8"), ("iteration
 SCALE_OUT = np.dtype([("action", "<i4"), ("copies_to_load", "<i4"), ("load_last_used", "<i8"), ("rpm", "<i4"), ("i1", "<i4"), ("i2", "<i4"),
                       ("set_heavy", "<i4"), ("remove", "<i4")], align=True)
 assert SCALE_IN.itemsize == 48 and SCALE_PARAMS.itemsize == 72 and SCALE_OUT.itemsize == 40
+REAPER_LOAD = np.dtype([("model", "<i4"), ("target", "<i4"), ("n_candidates", "<i4"), ("reserved", "<i4"), ("last_used", "<i8")],
+                       align=True)
+assert REAPER_LOAD.itemsize == 24
 LRU_LOAD = 5
 CHURN_REQUEST, CHURN_REMOVE, CHURN_REAPER = 0, 1, 2
 
@@ -68,6 +71,10 @@ class ChurnReport(C.Structure):
     _fields_ = [("n_published", C.c_int32), ("n_carry", C.c_int32), ("n_coalesced", C.c_int32), ("n_lru_events", C.c_int32),
                 ("ms_classify", C.c_float), ("ms_place", C.c_float), ("ms_route", C.c_float), ("ms_apply", C.c_float),
                 ("ms_registry", C.c_float), ("ms_commit", C.c_float), ("ms_total", C.c_float), ("ms_reaper", C.c_float)]
+
+class ReaperReport(C.Structure):
+    _fields_ = [("n_pruned", C.c_int32), ("n_repaired", C.c_int32), ("n_loads", C.c_int32), ("stopped_partition", C.c_int32)]
+
 
 DF_FAVOUR_SELF = 1
 DF_MODEL_LAST_USED = 2
@@ -131,6 +138,7 @@ SYMBOLS = [
     ("mmp_stats", _I32, [_P, _P, _P, _I32]),
     ("mmp_instance_partition", _I32, [_P, _I32]),
     ("mmp_reaper_select", _I32, [_P, _I32, _I64, _P, _P, _I32]),
+    ("mmp_reaper_run", _I32, [_P, _I32, _I64, _I64, _P, _U64, _P, _P, _I32, _P, _I32, _P, _I32, C.c_void_p]),
     ("mmp_lru_init", _I32, [_P, _I32, _P, _I32]),
     ("mmp_lru_apply", _I32, [_P, _P, _I32, _I64, _P, _I32]),
     ("mmp_lru_state", _I32, [_P, _I32, _P, _P, _P]),

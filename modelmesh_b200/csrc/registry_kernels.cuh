@@ -176,18 +176,23 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
 // registration).  missing_since = the `missings` map by instance index (0 = absent); first-seen-missing instances are stamped
 // (atomicCAS), pruned entries reported.  walk_ovf = 0: the first four registrations, one (model, mask) per model with pruned
 // entries (mmp_registry_prune); 1: every registration, one PrunedReg per pruned one, in no order (mmp_registry_prune_ids).
+// With a view (mmp_reaper_run, walk_ovf = 1) every model's row is also written as the reaper's loop sees it after the prune
+// and repairLastUsedTimeIfNeeded (MM:6837-6850): a pruned registration at a position < copy_count leaves copy_count, any
+// other fail_count; a last_used of Long.MAX_VALUE becomes now - 3 x LASTUSED_AGE_ON_ADD_MS, the model listed as repaired.
 struct PrunedReg { int32_t model, pos, inst; };
+struct PruneView { mmp_model_row *rows; int *repaired, *n_repaired; };
 __global__ void k_registry_prune(RegTables R, const mmp_model_row *__restrict__ models, const int2 *__restrict__ inst_meta, int n_models,
                                  int max_instances, int self, long long now, long long assume_gone, long long *__restrict__ missing_since,
                                  int walk_ovf, int *__restrict__ out_models, unsigned char *__restrict__ out_masks, PrunedReg *__restrict__ out_regs,
-                                 int cap, int *__restrict__ out_n) {
+                                 int cap, int *__restrict__ out_n, PruneView view) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= n_models) return;
   const mmp_model_row mr = models[m];
   const int n_edges = walk_ovf || mr.reserved < 4u ? (int)mr.reserved : 4;
-  if (n_edges == 0) return;
+  if (n_edges == 0 && !view.rows) return;
   const ModelRegs g = model_regs(R, m, walk_ovf ? mr.reserved : 0u);
   unsigned mask = 0;
+  int gone_loaded = 0, gone_failed = 0;
   for (int j = 0; j < n_edges; j++) {
     long long ts;
     const int i = reg_at(R, g, j, ts);
@@ -197,12 +202,23 @@ __global__ void k_registry_prune(RegTables R, const mmp_model_row *__restrict__ 
     const long long since = atomicCAS(reinterpret_cast<unsigned long long *>(&missing_since[i]), 0ull, (unsigned long long)now);
     if (since == 0 || (now - since) <= assume_gone) continue;
     if (!walk_ovf) { mask |= 1u << j; continue; }
+    if (j < mr.copy_count) gone_loaded++; else gone_failed++;
     const int q = atomicAdd(out_n, 1);
     if (q < cap) out_regs[q] = PrunedReg{m, j, i};
   }
   if (mask) {
     const int q = atomicAdd(out_n, 1);
     if (q < cap) { out_models[q] = m; out_masks[q] = (unsigned char)mask; }
+  }
+  if (view.rows) {
+    mmp_model_row v = mr;
+    v.copy_count = (uint8_t)max((int)mr.copy_count - gone_loaded, 0);
+    v.fail_count = (uint8_t)max((int)mr.fail_count - gone_failed, 0);
+    if (mr.last_used == 0x7fffffffffffffffLL) {
+      v.last_used = jsub(now, 3LL * 3600000LL);
+      view.repaired[atomicAdd(view.n_repaired, 1)] = m;
+    }
+    view.rows[m] = v;
   }
 }
 
@@ -237,7 +253,8 @@ static int32_t registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_
   CK(cudaEventRecord(c->e0, st));
   k_registry_prune<<<(nm + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.inst_meta.as<int2>(), nm, NI, self, now_ms,
                                                     assume_gone_ms, c->d_in.as<long long>(), walk_ovf ? 1 : 0, c->d_out.as<int>(),
-                                                    c->d_extra.as<unsigned char>(), c->d_out.as<PrunedReg>(), cap, c->d_n_open.as<int>());
+                                                    c->d_extra.as<unsigned char>(), c->d_out.as<PrunedReg>(), cap, c->d_n_open.as<int>(),
+                                                    PruneView{});
   CK(cudaEventRecord(c->e1, st));
   f->launches++;
   CK(cudaGetLastError());
@@ -247,6 +264,31 @@ static int32_t registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_
   CK(cudaStreamSynchronize(st));
   { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_prune_ms = ms; }
   return read(c.get(), n_out);
+}
+
+// mmp_reaper_run's decisions: selection k (rs.sel, emission order) is getNext(model, self = leader, lastUsed = the model's
+// row in the view, i.e. the repaired value where repaired), no flags, no extra excludes
+__global__ void k_reaper_decisions(const int2 *__restrict__ sel, int n, const mmp_model_row *__restrict__ view, int leader,
+                                   mmp_decision_in *__restrict__ out) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int m = sel[k].x;
+  out[k] = mmp_decision_in{m, leader, view[m].last_used, 0u, -1, 0, 0};
+}
+// ... and its loads, from the placed decisions
+__global__ void k_reaper_loads(const mmp_decision_in *__restrict__ in, const mmp_decision_out *__restrict__ res, int n,
+                               mmp_reaper_load *__restrict__ out) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  out[k] = mmp_reaper_load{in[k].model, res[k].target, res[k].n_candidates, 0, in[k].last_used};
+}
+// the reaper's cleanup of its `missings` map after the registry loop (MM:6601-6607)
+__global__ void k_missing_cleanup(long long *__restrict__ missing_since, const int2 *__restrict__ inst_meta, int n, long long now,
+                                  long long assume_gone) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const long long v = missing_since[i];
+  if (v != 0 && (jsub(now, v) > assume_gone || (inst_meta[i].y & 4))) missing_since[i] = 0;
 }
 
 extern "C" {
@@ -335,6 +377,152 @@ int32_t mmp_registry_prune_ids(mmp_fleet *f, int32_t self, int64_t now_ms, int64
     for (int i = 0; i < std::min(n_out, cap); i++) { out_models[i] = regs[i].model; out_instances[i] = regs[i].inst; }
     return n_out;
   });
+}
+
+
+int32_t mmp_reaper_run(mmp_fleet *f, int32_t leader, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since, uint64_t seed,
+                       int32_t *pruned_models, int32_t *pruned_instances, int32_t pruned_cap, int32_t *repaired_models,
+                       int32_t repaired_cap, mmp_reaper_load *loads, int32_t loads_cap, mmp_reaper_report *report) {
+  NEED(f);
+  if (leader < 0 || leader >= f->hs.cfg.max_instances || assume_gone_ms < 0 || !missing_since || !report || pruned_cap < 0 ||
+      repaired_cap < 0 || loads_cap < 0 || (pruned_cap > 0 && (!pruned_models || !pruned_instances)) ||
+      (repaired_cap > 0 && !repaired_models) || (loads_cap > 0 && !loads)) {
+    g_err = "bad argument"; return MMP_E_ARG;
+  }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  // The prune reads the live registry (as registry_prune does), the selection and the placement the epoch (as mmp_reaper_select
+  // and mmp_place_batch do): ingest_mu, then snap_mu shared -- the order of a commit, which flips the epoch under snap_mu while
+  // it holds ingest_mu.  Holding both, the registry read is the one the epoch was built from.
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
+  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  if (places_sharded(f, false)) {
+    g_err = "mmp_reaper_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
+    return MMP_E_STATE;
+  }
+  const DeviceSnapshot &ds = f->snaps[f->cur];
+  const HostSnapshot &h = ds.host;
+  LiveState &lv = f->live;
+  const int32_t NM = ds.n_models, NI = f->hs.cfg.max_instances, np = (int)h.part_types.size();
+  const int tc = h.tc_enabled ? 1 : 0, ns = tc ? np : 1;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  RpScratch &rs = c->rp;
+  const size_t nmx = (size_t)std::max(NM, 1);
+  const int32_t reg_cap = NM * HostState::EDGE_INL + lv.n_ovf;  // every registration
+  CK(c->d_view.ensure(nmx * sizeof(mmp_model_row)));
+  CK(c->d_pruned.ensure((size_t)std::max(reg_cap, 1) * sizeof(PrunedReg)));
+  CK(c->d_repaired.ensure(nmx * 4));
+  CK(c->d_n_open.ensure(16));
+  // [missing_since (NI) | stats (np + 1) | the cluster's LRU, from Long.MAX_VALUE (ISST)]
+  const size_t acc_b = (size_t)(np + 1) * sizeof(StatsAcc);
+  CK(c->d_trace.ensure((size_t)NI * 8 + acc_b + 8));
+  long long *d_miss = c->d_trace.as<long long>();
+  StatsAcc *acc = reinterpret_cast<StatsAcc *>(d_miss + NI);
+  long long *d_min = reinterpret_cast<long long *>(reinterpret_cast<char *>(acc) + acc_b);
+  int *d_cnt = c->d_n_open.as<int>();                         // [0] pruned registrations, [1] repaired models
+  int *h_cnt = reinterpret_cast<int *>(c->mapped.get());      // ... read back with the selection count (pinned)
+  mmp_model_row *view = c->d_view.as<mmp_model_row>();
+  static const long long lru_init = 0x7fffffffffffffffLL;
+  CK(cudaMemcpyAsync(d_miss, missing_since, (size_t)NI * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(d_cnt, 0, 8, st));
+  CK(cudaMemsetAsync(acc, 0, acc_b, st));
+  CK(cudaMemcpyAsync(d_min, &lru_init, 8, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(c->e0, st));
+  if (NM) {
+    k_registry_prune<<<(NM + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.inst_meta.as<int2>(), NM, NI, leader,
+                                                      now_ms, assume_gone_ms, d_miss, 1, nullptr, nullptr, c->d_pruned.as<PrunedReg>(), reg_cap,
+                                                      d_cnt, PruneView{view, c->d_repaired.as<int>(), d_cnt + 1});
+    f->launches++;
+    CK(cudaGetLastError());
+  }
+  CK(cudaMemcpyAsync(h_cnt, d_cnt, 8, cudaMemcpyDeviceToHost, st));
+  k_missing_cleanup<<<(NI + 255) / 256, 256, 0, st>>>(d_miss, lv.inst_meta.as<int2>(), NI, now_ms, assume_gone_ms);
+  f->launches++;
+  if (h.n_ranks > 0) {
+    k_stats<<<std::min(f->sm_count, (h.n_ranks + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(),
+                                                                           ds.part_of_rank.as<int32_t>(), h.n_ranks, f->hs.cfg.min_space_units,
+                                                                           acc, d_min, np);
+    f->launches++;
+  }
+  CK(cudaGetLastError());
+  // the selection over the view: one run at now_ms, taken tags from a zeroed array (the pass reads the count back)
+  int32_t n_sel = 0;
+  if (NM) {
+    CK(rs.taken.ensure(nmx * 4));
+    CK(cudaMemsetAsync(rs.taken.p, 0, nmx * 4, st));
+    int32_t gen = 0;
+    rc = reaper_pass(f, ds, view, NM, tc, acc, d_min, std::vector<long long>{(long long)now_ms}, gen, rs, c->d_cub, st, &n_sel);
+    if (rc < 0) return rc;
+  }
+  const int n_pruned = NM ? h_cnt[0] : 0, n_repaired = NM ? h_cnt[1] : 0;
+  // the decisions, built on the device from the selections, placed as mmp_place_batch_device places a batch
+  const int n_loads = std::min(n_sel, loads_cap);
+  if (n_sel) {
+    if ((rc = stage_side_tables(c.get(), nullptr, 0, nullptr, 0, st)) < 0) return rc;
+    CK(c->d_in.ensure((size_t)n_sel * sizeof(mmp_decision_in)));
+    CK(c->d_out.ensure((size_t)n_sel * sizeof(mmp_decision_out)));
+    CK(c->d_loads.ensure((size_t)n_sel * sizeof(mmp_reaper_load)));
+    k_reaper_decisions<<<(n_sel + 255) / 256, 256, 0, st>>>(rs.sel.as<int2>(), n_sel, view, leader, c->d_in.as<mmp_decision_in>());
+    f->launches++;
+    CK(cudaGetLastError());
+    PlaceArgs a{ds.view, c->d_in.as<mmp_decision_in>(), n_sel, c->d_fresh.as<FreshRow>(), 0, c->d_extra.as<int32_t>(),
+                c->d_out.as<mmp_decision_out>(), nullptr, nullptr, now_ms, seed, f->id_base.load()};
+    a.ctx = c.get();
+    CK(launch_place(f, a, st));
+  }
+  CK(cudaEventRecord(c->e1, st));
+  if (n_loads) {
+    k_reaper_loads<<<(n_loads + 255) / 256, 256, 0, st>>>(c->d_in.as<mmp_decision_in>(), c->d_out.as<mmp_decision_out>(), n_loads,
+                                                         c->d_loads.as<mmp_reaper_load>());
+    f->launches++;
+    CK(cudaGetLastError());
+  }
+  // one copy back: the lists, the cleaned map, and the plan of the walk ([parts | space | plan | order], rp_plan_stage's layout)
+  // with the candidate count, from which the partition a size estimate of 0 stopped at is named
+  std::vector<PrunedReg> regs((size_t)n_pruned);
+  std::vector<int32_t> rep((size_t)n_repaired);
+  std::vector<mmp_reaper_load> ld((size_t)n_loads);
+  std::vector<int64_t> miss((size_t)NI);
+  const size_t parts_b = (size_t)ns * sizeof(RpPart), space_b = (size_t)ns * 8;
+  std::vector<char> hb(parts_b + space_b + sizeof(RpPlan) + (size_t)ns * 4);
+  int ncand = 0;
+  if (n_pruned) CK(cudaMemcpyAsync(regs.data(), c->d_pruned.p, regs.size() * sizeof(PrunedReg), cudaMemcpyDeviceToHost, st));
+  if (n_repaired) CK(cudaMemcpyAsync(rep.data(), c->d_repaired.p, rep.size() * 4, cudaMemcpyDeviceToHost, st));
+  if (n_loads) CK(cudaMemcpyAsync(ld.data(), c->d_loads.p, ld.size() * sizeof(mmp_reaper_load), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(miss.data(), d_miss, (size_t)NI * 8, cudaMemcpyDeviceToHost, st));
+  if (NM) {
+    CK(cudaMemcpyAsync(hb.data(), rs.plan.p, hb.size(), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&ncand, rs.idx.as<int>() + 2 * nmx, 4, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_reaper_run_ms = ms; }
+  int stopped = -1;
+  if (NM) {  // k_rp_walk's loop over the partitions: the first whose counts throw
+    RpPlan plan;
+    memcpy(&plan, hb.data() + parts_b + space_b, sizeof(RpPlan));
+    for (int oi = 0; plan.go && ncand > 0 && oi < plan.n_order; oi++) {
+      int s;
+      RpPart p;
+      unsigned long long space;
+      memcpy(&s, hb.data() + parts_b + space_b + sizeof(RpPlan) + (size_t)oi * 4, 4);
+      memcpy(&p, hb.data() + (size_t)s * sizeof(RpPart), sizeof(RpPart));
+      memcpy(&space, hb.data() + parts_b + (size_t)s * 8, 8);
+      int free_count, total;
+      long long cutoff;
+      if (!rp_counts(p, space, now_ms, free_count, total, cutoff)) { stopped = tc ? 1 + oi : 0; break; }
+    }
+  }
+  std::sort(regs.begin(), regs.end(), [](const PrunedReg &a, const PrunedReg &b) { return a.model != b.model ? a.model < b.model : a.pos < b.pos; });
+  std::sort(rep.begin(), rep.end());
+  for (int i = 0; i < std::min(n_pruned, pruned_cap); i++) { pruned_models[i] = regs[i].model; pruned_instances[i] = regs[i].inst; }
+  for (int i = 0; i < std::min(n_repaired, repaired_cap); i++) repaired_models[i] = rep[i];
+  if (n_loads) memcpy(loads, ld.data(), ld.size() * sizeof(mmp_reaper_load));
+  memcpy(missing_since, miss.data(), (size_t)NI * 8);
+  *report = mmp_reaper_report{n_pruned, n_repaired, n_sel, stopped};
+  return n_sel;
 }
 
 }  // extern "C"

@@ -13,7 +13,8 @@ import numpy as np
 
 from . import _lib
 from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CHURN_REAPER, CLUSTER_STATS, DECISION_IN, DECISION_OUT,
-                   DECISION_TRACE, EVICTION, INSTANCE_ROW, LRU_ENTRY, LRU_EVENT, MODEL_ROW, ChurnConfig, ChurnReport, MmpConfig)
+                   DECISION_TRACE, EVICTION, INSTANCE_ROW, LRU_ENTRY, LRU_EVENT, MODEL_ROW, REAPER_LOAD, ChurnConfig, ChurnReport,
+                   MmpConfig, ReaperReport)
 
 
 class MmpError(RuntimeError):
@@ -340,6 +341,23 @@ class Fleet:
                                                      _ptr(inst), cap))
         k = min(n, cap)
         return n, models[:k], inst[:k]
+
+    def reaper_run(self, leader: int, now_ms: int, assume_gone_ms: int, missing_since: np.ndarray, seed: int,
+                   pruned_cap: Optional[int] = None, repaired_cap: Optional[int] = None, loads_cap: Optional[int] = None):
+        """mmp_reaper_run, one run of the leader's reaper task: ((models, instances) of the pruned registrations, repaired model
+        ids, loads (REAPER_LOAD records), report).  Each list holds the first min(total, cap) entries; the caps default to
+        room for every entry.  missing_since (int64[max_instances]) is updated in place, cleaned up as the reaper does."""
+        assert missing_since.dtype == np.int64 and missing_since.flags.c_contiguous
+        caps = [self.max_models * 4 if pruned_cap is None else pruned_cap, self.max_models if repaired_cap is None else repaired_cap,
+                self.max_models if loads_cap is None else loads_cap]
+        pm, pi = np.zeros(max(caps[0], 1), dtype=np.int32), np.zeros(max(caps[0], 1), dtype=np.int32)
+        rep = np.zeros(max(caps[1], 1), dtype=np.int32)
+        loads = np.zeros(max(caps[2], 1), dtype=REAPER_LOAD)
+        r = ReaperReport()
+        self._ck(self.lib.mmp_reaper_run(self.h, leader, now_ms, assume_gone_ms, _ptr(missing_since), seed, _ptr(pm), _ptr(pi), caps[0],
+                                         _ptr(rep), caps[1], _ptr(loads), caps[2], C.byref(r)))
+        k = min(r.n_pruned, caps[0])
+        return (pm[:k].copy(), pi[:k].copy()), rep[:min(r.n_repaired, caps[1])].copy(), loads[:min(r.n_loads, caps[2])].copy(), r
 
     def commit_info(self):
         path, ms = C.c_int32(), C.c_double()
