@@ -522,6 +522,60 @@ int32_t mmp_registry_prune(mmp_fleet *, int32_t self, int64_t now_ms, int64_t as
  * returns the same pairs.  assume_gone_ms >= 0.  Sets the "prune" timing. */
 int32_t mmp_registry_prune_ids(mmp_fleet *, int32_t self, int64_t now_ms, int64_t assume_gone_ms, int64_t *missing_since,
                                int32_t *out_models, int32_t *out_instances, int32_t cap);
+/* The registry loop of one pod's janitor task (MM:6013-6145) against the committed epoch and the registry as of the last
+ * commit, in one call.  entries[] is the pod's runtimeCache.descendingMap() (MM:5892) as the loop reads it, at most one entry per
+ * model, in any order.  For every model with a registration of `self` (every registration, the overflow ones included):
+ *   loaded     self is among the first copy_count registrations; failedTime = the time of self's first failed registration
+ *   remLoaded  loaded && (no entry || the entry is MMP_JANITOR_FAILED)
+ *   remFailed  there is a failure record, and: an entry that is not failed; or now - failedTime > expiry (Java long
+ *              arithmetic), expiry = load_failure_expiry_ms / 2 when lu > 0 && now - lu < 180 000, load_failure_expiry_ms
+ *              otherwise, lu = the entry's last_used (-1 without one)
+ *   candidate  loaded && !remLoaded && the entry's last_used > 0, keyed by that last_used.  VALUE_COMP compares the value only, so
+ *              of candidates with equal last_used only the first in model order stays (quirk N15; N12's stand-in for registry
+ *              order)
+ * then, over the candidates by ascending last_used, the budget walk of MM:6117-6140: canRemove = removed == 0 || weight <= budget
+ * (budget from adjusted_capacity / 20, less each removed weight: it may go negative), and removeModelCopies is mmp_scale_eval's
+ * scale-down with that canRemove, and the registration time of self's copy equal to the entry's load_ts
+ * (removeLocalModelCopyAsync MM:6347-6349).
+ * One edit per model that has anything to do, in model order, what[] the OR of the MMP_JE_* bits; last_used / last_unload_time
+ * are the record's after the edit (updateLastUsed of the entry's last_used where it is > 0, MR:239-246; updateLastUnloadTime:
+ * 0 when at most 2 loaded copies remain, else now).  The edits hold the first cap; the report gives the totals (n_referencing:
+ * the reference's j, the models that reference self; n_candidates after the VALUE_COMP ties are dropped).
+ * Not modelled (stays in the pod): the first loop over the local cache (MM:5892-6008), shuttingDown, the KV conditional writes
+ * and their retry on conflict, and the async removal's isLoadedElsewhere and ce.remove() (MM:6353-6373).
+ * Returns the number of edits.  Errors (nothing written): MMP_E_ARG for self outside [0, max_instances), an entry's model out
+ * of range or two entries of one model, n < 0, p or report NULL, edits NULL with cap > 0, or a p->scale mmp_scale_eval refuses;
+ * MMP_E_EPOCH without a commit; MMP_E_STATE when the committed registry holds no registration times (neither mmp_model_times
+ * nor a JSON record supplied any: every failure would read as expired).  Sets the "janitor_run" timing. */
+#define MMP_JANITOR_FAILED 1u              /* ce.isFailed() */
+typedef struct {
+  int32_t model, weight;                   /* model index; ce.getWeight() */
+  int64_t last_used;                       /* runtimeCache.getLastUsedTime(model): -1 when absent or <= 0 (CLHM:742-746) */
+  int64_t load_ts;                         /* ce.loadTimestamp (removeLocalModelCopyAsync compares it, MM:6347-6349) */
+  int64_t last_heavy;                      /* ce.getLastHeavyTime() */
+  int64_t count;                           /* the interval count ce.getRpm(timeSinceLastCheck) divides (MM:6292) */
+  uint32_t flags, reserved;                /* MMP_JANITOR_FAILED */
+} mmp_janitor_entry;                       /* 48 B */
+typedef struct {
+  mmp_scale_params scale;                  /* now, last_check_time, scale_up_rpm_threshold, rate_check_interval_ms,
+                                              second_copy_remove_max_age_ms as mmp_scale_eval reads them; can_remove ignored */
+  int64_t load_failure_expiry_ms;          /* LOAD_FAILURE_EXPIRY_MS (MM:219); the in-use expiry is half of it (MM:221) */
+  int64_t adjusted_capacity;               /* getAdjustedCacheCapacity() (MM:5363): the budget is a twentieth of it (MM:6117) */
+  uint32_t flags, reserved;                /* MMP_SCALE_NO_LOCAL_STATS for this pod (quirk N13) */
+} mmp_janitor_params;
+#define MMP_JE_UNREGISTER   1u  /* remLoaded: remove self from instanceIds, updateLastUnloadTime (MM:6059-6062) */
+#define MMP_JE_DROP_FAILURE 2u  /* remFailed: removeLoadFailure(self) (MM:6063-6065) */
+#define MMP_JE_REMOVE_LOCAL 4u  /* the pod's failed cache entry goes too (MM:6089-6091) */
+#define MMP_JE_SCALE_DOWN   8u  /* removeModelCopies returned true under the budget: the async removal of MM:6353-6373 starts */
+#define MMP_JE_UNDECIDED   16u  /* copy_count saturated at 255 over > 255 registrations: nothing decided (as mmp_scale_eval's -1) */
+typedef struct {
+  int32_t model; uint32_t what;
+  int64_t last_used;         /* the record's lastUsed after the updateLastUsed calls of the edit (MR:239-246) */
+  int64_t last_unload_time;  /* after updateLastUnloadTime where the edit unregisters self, else the record's value */
+} mmp_janitor_edit;          /* 24 B */
+typedef struct { int32_t n_referencing, n_edits, n_candidates, n_removed; int64_t weight_removed; } mmp_janitor_report;
+int32_t mmp_janitor_run(mmp_fleet *, int32_t self, const mmp_janitor_entry *entries, int32_t n, const mmp_janitor_params *p,
+                        mmp_janitor_edit *edits, int32_t cap, mmp_janitor_report *report);
 
 /* tuning / measurement knobs, same meaning as the MMP_* environment variables read at mmp_fleet_create:
  *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the batch kernel ("direct" below), 1 the latency kernel
@@ -540,7 +594,8 @@ int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
 /* CUDA-event duration (ms) of the device part of the last mmp_stats ("stats"), mmp_reaper_select ("reaper": the candidate
  * sweep through the selection, k_rp_flag to k_rp_pick, without the stats and plan), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
  * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
- * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel;
+ * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel; "janitor_run": mmp_janitor_run from its stats
+ * kernel to its budget walk;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device

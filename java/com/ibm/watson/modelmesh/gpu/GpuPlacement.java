@@ -149,6 +149,11 @@ public final class GpuPlacement implements AutoCloseable {
                                        prunedInstances, prunedCap, repairedModels, repairedCap, loads, loadsCap, report));
     }
 
+    // the registry loop of this pod's janitor task (ModelMesh.java:6013-6145): returns the number of edits; report gets the totals
+    public int janitorRun(int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer edits, int cap, ByteBuffer report) {
+        return check(MmPlace.janitorRun(h, self, entries, n, params, edits, cap, report));
+    }
+
     private int check(int rc) { if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h)); return rc; }
     @Override public void close() { committer.shutdownNow(); MmPlace.destroy(h); }
 }

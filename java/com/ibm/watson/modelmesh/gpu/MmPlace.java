@@ -49,6 +49,9 @@ final class MmPlace {
     static native int reaperRun(long h, int leader, long nowMs, long assumeGoneMs, ByteBuffer missingSince, long seed,
                                 ByteBuffer prunedModels, ByteBuffer prunedInstances, int prunedCap, ByteBuffer repairedModels,
                                 int repairedCap, ByteBuffer loads, int loadsCap, ByteBuffer report);
+    // the registry loop of one pod's janitor task (MM:6013-6145): stale registrations, expired failures, budgeted scale-down
+    static native int janitorRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer edits, int cap,
+                                 ByteBuffer report);
     static native int tune(long h, String key, long value);
     static native double lastTiming(long h, String key);
     // plug point 1: placement (CacheMissForwardingLB.getNext MM:4776-5004)

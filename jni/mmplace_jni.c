@@ -149,6 +149,14 @@ jint FN(reaperRun)(JNIEnv *env, jclass c, jlong h, jint leader, jlong nowMs, jlo
                         (int32_t *)BUF(prunedInstances), prunedCap, (int32_t *)BUF(repairedModels), repairedCap,
                         (mmp_reaper_load *)BUF(loads), loadsCap, (mmp_reaper_report *)BUF(report));
 }
+/* the registry loop of one pod's janitor task.  entries: n x mmp_janitor_entry (48 B), params: one mmp_janitor_params (96 B),
+ * edits: cap x mmp_janitor_edit (24 B), report: one mmp_janitor_report (24 B) -- direct buffers */
+jint FN(janitorRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, jint n, jobject params, jobject edits, jint cap,
+                    jobject report) {
+  (void)c;
+  return mmp_janitor_run(H(h), self, (const mmp_janitor_entry *)BUF(entries), n, (const mmp_janitor_params *)BUF(params),
+                         (mmp_janitor_edit *)BUF(edits), cap, (mmp_janitor_report *)BUF(report));
+}
 jint FN(tune)(JNIEnv *env, jclass c, jlong h, jstring key, jlong value) {
   const char *ck = utf(env, key);
   jint rc = mmp_tune(H(h), ck, value);

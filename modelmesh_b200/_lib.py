@@ -58,6 +58,14 @@ assert SCALE_IN.itemsize == 48 and SCALE_PARAMS.itemsize == 72 and SCALE_OUT.ite
 REAPER_LOAD = np.dtype([("model", "<i4"), ("target", "<i4"), ("n_candidates", "<i4"), ("reserved", "<i4"), ("last_used", "<i8")],
                        align=True)
 assert REAPER_LOAD.itemsize == 24
+JANITOR_FAILED = 1
+JE_UNREGISTER, JE_DROP_FAILURE, JE_REMOVE_LOCAL, JE_SCALE_DOWN, JE_UNDECIDED = 1, 2, 4, 8, 16
+JANITOR_ENTRY = np.dtype([("model", "<i4"), ("weight", "<i4"), ("last_used", "<i8"), ("load_ts", "<i8"), ("last_heavy", "<i8"),
+                          ("count", "<i8"), ("flags", "<u4"), ("reserved", "<u4")], align=True)
+JANITOR_PARAMS = np.dtype([("scale", SCALE_PARAMS), ("load_failure_expiry_ms", "<i8"), ("adjusted_capacity", "<i8"), ("flags", "<u4"),
+                           ("reserved", "<u4")], align=True)
+JANITOR_EDIT = np.dtype([("model", "<i4"), ("what", "<u4"), ("last_used", "<i8"), ("last_unload_time", "<i8")], align=True)
+assert JANITOR_ENTRY.itemsize == 48 and JANITOR_PARAMS.itemsize == 96 and JANITOR_EDIT.itemsize == 24
 LRU_LOAD = 5
 CHURN_REQUEST, CHURN_REMOVE, CHURN_REAPER = 0, 1, 2
 
@@ -74,6 +82,11 @@ class ChurnReport(C.Structure):
 
 class ReaperReport(C.Structure):
     _fields_ = [("n_pruned", C.c_int32), ("n_repaired", C.c_int32), ("n_loads", C.c_int32), ("stopped_partition", C.c_int32)]
+
+
+class JanitorReport(C.Structure):
+    _fields_ = [("n_referencing", C.c_int32), ("n_edits", C.c_int32), ("n_candidates", C.c_int32), ("n_removed", C.c_int32),
+                ("weight_removed", C.c_int64)]
 
 
 DF_FAVOUR_SELF = 1
@@ -139,6 +152,7 @@ SYMBOLS = [
     ("mmp_instance_partition", _I32, [_P, _I32]),
     ("mmp_reaper_select", _I32, [_P, _I32, _I64, _P, _P, _I32]),
     ("mmp_reaper_run", _I32, [_P, _I32, _I64, _I64, _P, _U64, _P, _P, _I32, _P, _I32, _P, _I32, C.c_void_p]),
+    ("mmp_janitor_run", _I32, [_P, _I32, _P, _I32, _P, _P, _I32, C.c_void_p]),
     ("mmp_lru_init", _I32, [_P, _I32, _P, _I32]),
     ("mmp_lru_apply", _I32, [_P, _P, _I32, _I64, _P, _I32]),
     ("mmp_lru_state", _I32, [_P, _I32, _P, _P, _P]),

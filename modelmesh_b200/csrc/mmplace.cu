@@ -1258,6 +1258,7 @@ struct PlaceCtx {
   DevBuf d_xids, d_xcand, d_xcandx, d_xpref, d_xnzw, d_xnz_n, d_xbefore;
   RpScratch rp;  // mmp_reaper_select's pass (scan_kernels.cuh)
   DevBuf d_view, d_pruned, d_repaired, d_loads;  // mmp_reaper_run (registry_kernels.cuh): the pruned and repaired model rows, its lists
+  DevBuf d_jslot, d_jent, d_jcand, d_jout;        // mmp_janitor_run (registry_kernels.cuh): entry by model, entries, candidates, results
 };
 
 // The scoring kernel of untraced batches (MMP_KERNEL = direct | lanes | tile; launch_place): k_place_direct (rows rebuilt
@@ -1285,6 +1286,7 @@ struct mmp_fleet {
   float t_stats_ms = 0, t_reaper_ms = 0, t_lru_ms = 0, t_prune_ms = 0;  // CUDA-event time of the device part of the last mmp_stats / mmp_reaper_select / mmp_lru_apply
   float t_lru_read_ms = 0;      // ... and of the last mmp_lru_read (its count + scan part plus its emit part)
   float t_reaper_run_ms = 0;    // ... and of the last mmp_reaper_run (its prune sweep to its last placement kernel)
+  float t_janitor_ms = 0;       // ... and of the last mmp_janitor_run (its stats kernel to its budget walk)
   int32_t last_commit_path = 0; // 1 structural (host), 2 device
   double last_commit_ms = 0;
   ncclComm_t comm = nullptr;    // instance-shard communicator (mmp_shard_connect)
@@ -2328,6 +2330,7 @@ int32_t mmp_last_timing(mmp_fleet *f, const char *key, double *ms) {
   else if (!strcmp(key, "lru_read")) *ms = f->t_lru_read_ms;
   else if (!strcmp(key, "prune")) *ms = f->t_prune_ms;
   else if (!strcmp(key, "reaper_run")) *ms = f->t_reaper_run_ms;
+  else if (!strcmp(key, "janitor_run")) *ms = f->t_janitor_ms;
   else if (!strcmp(key, "commit")) *ms = f->last_commit_ms;
   else if (!strcmp(key, "dealt_kernel")) *ms = f->peers.t_kernel_ms;
   else if (!strcmp(key, "dealt_wait")) *ms = f->peers.t_wait_ms;

@@ -44,6 +44,65 @@ __device__ __forceinline__ int count_rpm_above(const int *sorted, int n, int thr
   return n - lo;
 }
 
+// removeModelCopies (MM:6197-6335) with canRemove = true for `instance`'s copy of `model` (who-drops-the-copy by PLACEMENT_ORDER
+// MM:6314-6335 included): k_scale_eval's scale-down and the janitor's registry pass (k_janitor_eval) both run it.  g / loaded:
+// the model's registrations and how many of them are loaded copies; self_rank: `instance`'s rank in the snapshot (-1: none)
+__device__ __forceinline__ bool scale_down_removes(const ScaleTables &T, const mmp_scale_params &p, int instance, int model, long long last_used,
+                                                   long long last_heavy, long long count, int flags, const ModelRegs &g, int loaded,
+                                                   int self_rank) {
+  long long ts;
+  if (last_used == 0 || loaded < 2) return false;
+  // instanceSetStats(): the local instance's partition with type constraints, else the cluster (MM:1440-1446, TCM:236-239)
+  long long cap, fr;
+  const long long glru = *T.min_lru;
+  if (T.tc_enabled) {
+    if (self_rank < 0 || (flags & MMP_SCALE_NO_LOCAL_STATS)) return false;  // EMPTY_STATS: totalCapacity == 0 (quirk N13, mmplace.h)
+    const StatsAcc a = T.part_acc[1 + T.part_of_rank[self_rank]];
+    cap = (long long)a.cap; fr = (long long)a.free;
+  } else { cap = (long long)T.part_acc[0].cap; fr = (long long)T.part_acc[0].free; }
+  if (cap == 0 || jmul64(fr, 100) / cap > 5) return false;
+  // the first other copy in instance-ID order that is in the table and not shutting down (MM:6236-6245)
+  int other = -1;
+  unsigned best_id = 0xffffffffu;
+  for (int j = 0; j < loaded; j++) {
+    const int i = reg_at(T.R, g, j, ts);
+    if (i < 0 || i == instance || T.rank_of[i] < 0) continue;
+    const unsigned idr = T.inst_tie[i].x;
+    if (idr < best_id) { best_id = idr; other = i; }
+  }
+  if (other < 0) return false;
+  if (loaded == 2) {
+    const long long cache_age = jsub(p.now, glru);
+    long long scale_down_age = cache_age / 10;
+    if (last_heavy == 0 || jsub(p.now, last_heavy) < cache_age / 5) scale_down_age = p.second_copy_remove_max_age_ms < scale_down_age ? (long long)p.second_copy_remove_max_age_ms : scale_down_age;
+    if (jsub(p.now, last_used) > scale_down_age) {
+      if (self_rank < 0) return false;
+      // PLACEMENT_ORDER.compare(other, this) > 0: the other pod should flush it (MM:6328).  The comparator, not the ranks:
+      // with mixed versions (quirk N1) it is no total order, and the snapshot's linear order contradicts it on some pair
+      if (compare_keys(order_key(T.inst_rows[other], T.inst_tie[other], T.min_space),
+                       order_key(T.inst_rows[instance], T.inst_tie[instance], T.min_space), T.churn2) > 0) return false;
+      return true;
+    }
+    return false;
+  }
+  const long long lul = T.model_lul ? T.model_lul[model] : 0;
+  if (lul > 0 && jsub(p.now, lul) < jmul64(8, p.rate_check_interval_ms)) return false;
+  bool recent = false;
+  for (int j = 0; j < loaded; j++) {
+    reg_at(T.R, g, j, ts);
+    if (ts > jsub(p.now, 1800000LL)) recent = true;
+  }
+  if (recent) return false;
+  long long min_age = jadd64(jmul64(3, glru), 10400000LL) / 100;
+  if (min_age < 600000LL) min_age = 600000LL; else if (min_age > 18000000LL) min_age = 18000000LL;
+  if (jsub(p.now, last_heavy) < min_age) return false;
+  const long long since = jsub(p.now, p.last_check_time);
+  if (since < p.rate_check_interval_ms / 10) return false;
+  const long long rpm2 = jmul64(count, 60000) / since;
+  if (rpm2 > ((long long)p.scale_up_rpm_threshold * 2) / 3) return false;
+  return true;
+}
+
 // one thread per cache entry: rateTrackingTask's loop body (MM:5684-5806) and removeModelCopies (MM:6197-6335)
 __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in, int n, mmp_scale_params p, mmp_scale_out *__restrict__ out) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -117,58 +176,7 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     o.action = 2; o.copies_to_load = copies; o.load_last_used = p.now + 20000;
   } while (false);
   // ---------------- scale-down (janitor: removeModelCopies) ----------------
-  do {
-    if (!p.can_remove || e.last_used == 0 || loaded < 2) break;
-    // instanceSetStats(): the local instance's partition with type constraints, else the cluster (MM:1440-1446, TCM:236-239)
-    long long cap, fr;
-    const long long glru = *T.min_lru;
-    if (T.tc_enabled) {
-      if (self_rank < 0 || (e.flags & MMP_SCALE_NO_LOCAL_STATS)) break;  // EMPTY_STATS: totalCapacity == 0 (quirk N13, mmplace.h)
-      const StatsAcc a = T.part_acc[1 + T.part_of_rank[self_rank]];
-      cap = (long long)a.cap; fr = (long long)a.free;
-    } else { cap = (long long)T.part_acc[0].cap; fr = (long long)T.part_acc[0].free; }
-    if (cap == 0 || jmul64(fr, 100) / cap > 5) break;
-    // the first other copy in instance-ID order that is in the table and not shutting down (MM:6236-6245)
-    int other = -1;
-    unsigned best_id = 0xffffffffu;
-    for (int j = 0; j < loaded; j++) {
-      const int i = reg_at(T.R, g, j, ts);
-      if (i < 0 || i == e.instance || T.rank_of[i] < 0) continue;
-      const unsigned idr = T.inst_tie[i].x;
-      if (idr < best_id) { best_id = idr; other = i; }
-    }
-    if (other < 0) break;
-    if (loaded == 2) {
-      const long long cache_age = jsub(p.now, glru);
-      long long scale_down_age = cache_age / 10;
-      if (e.last_heavy == 0 || jsub(p.now, e.last_heavy) < cache_age / 5) scale_down_age = p.second_copy_remove_max_age_ms < scale_down_age ? (long long)p.second_copy_remove_max_age_ms : scale_down_age;
-      if (jsub(p.now, e.last_used) > scale_down_age) {
-        if (self_rank < 0) break;
-        // PLACEMENT_ORDER.compare(other, this) > 0: the other pod should flush it (MM:6328).  The comparator, not the ranks:
-        // with mixed versions (quirk N1) it is no total order, and the snapshot's linear order contradicts it on some pair
-        if (compare_keys(order_key(T.inst_rows[other], T.inst_tie[other], T.min_space),
-                         order_key(T.inst_rows[e.instance], T.inst_tie[e.instance], T.min_space), T.churn2) > 0) break;
-        o.remove = 1;
-      }
-      break;
-    }
-    const long long lul = T.model_lul ? T.model_lul[e.model] : 0;
-    if (lul > 0 && jsub(p.now, lul) < jmul64(8, p.rate_check_interval_ms)) break;
-    bool recent = false;
-    for (int j = 0; j < loaded; j++) {
-      reg_at(T.R, g, j, ts);
-      if (ts > jsub(p.now, 1800000LL)) recent = true;
-    }
-    if (recent) break;
-    long long min_age = jadd64(jmul64(3, glru), 10400000LL) / 100;
-    if (min_age < 600000LL) min_age = 600000LL; else if (min_age > 18000000LL) min_age = 18000000LL;
-    if (jsub(p.now, e.last_heavy) < min_age) break;
-    const long long since = jsub(p.now, p.last_check_time);
-    if (since < p.rate_check_interval_ms / 10) break;
-    const long long rpm2 = jmul64(e.count, 60000) / since;
-    if (rpm2 > ((long long)p.scale_up_rpm_threshold * 2) / 3) break;
-    o.remove = 1;
-  } while (false);
+  if (p.can_remove && scale_down_removes(T, p, e.instance, e.model, e.last_used, e.last_heavy, e.count, e.flags, g, loaded, self_rank)) o.remove = 1;
   out[r] = o;
 }
 
@@ -291,6 +299,144 @@ __global__ void k_missing_cleanup(long long *__restrict__ missing_since, const i
   if (v != 0 && (jsub(now, v) > assume_gone || (inst_meta[i].y & 4))) missing_since[i] = 0;
 }
 
+// the tables k_scale_eval and k_janitor_eval read: the snapshot's, the live registry's, and the call's stats (the type-set
+// stats and the sorted rpm column only the scale-up reads: NULL where no scale-up runs)
+static ScaleTables scale_tables(mmp_fleet *f, const DeviceSnapshot &ds, LiveState &lv, const StatsAcc *acc, const long long *d_min,
+                                const TypeStat *tstats, const int *rpm_sorted) {
+  ScaleTables T;
+  T.models = lv.models.as<mmp_model_row>(); T.R = reg_tables(lv);
+  T.model_lul = lv.have_times ? lv.model_lul.as<long long>() : nullptr;
+  T.rank_of = ds.rank_of.as<int32_t>(); T.rows = ds.rows.as<RankRow>(); T.part_of_rank = ds.part_of_rank.as<int32_t>();
+  T.inst_tie = lv.inst_tie.as<uint4>(); T.inst_rows = lv.inst_rows.as<mmp_instance_row>();
+  T.min_space = f->hs.cfg.min_space_units; T.churn2 = (long long)((uint64_t)f->hs.cfg.min_churn_age_ms * 2u);
+  T.type_stats = tstats; T.part_acc = acc; T.min_lru = d_min; T.sorted_rpm = rpm_sorted;
+  T.n_ranks = ds.host.n_ranks; T.n_models = f->hs.n_models_used; T.n_type_ids = lv.n_type_ids; T.max_instances = f->hs.cfg.max_instances;
+  T.tc_enabled = ds.host.tc_enabled;
+  return T;
+}
+
+// mmp_janitor_run: the registry loop of one pod's janitor task (MM:6013-6145).  The pod's entries are indexed by model in
+// slot[] (max_models ints, -1 = no entry): k_janitor_index sets the call's, k_janitor_clear resets the same ones afterwards, so
+// the scratch is filled with -1 only when it is allocated.  A second entry of one model is reported through cnt[JC_DUP].
+enum { JC_EDITS = 0, JC_CANDS = 1, JC_REFS = 2, JC_DUP = 3 };
+struct JanitorCand { int model, entry, edit, removes; long long reg_ts; };  // reg_ts: the time of self's loaded registration
+struct JanitorBufs {
+  const mmp_janitor_entry *entries; int *slot;
+  mmp_janitor_edit *edits;             // one per model at most, in no order
+  unsigned long long *keys; int *vals; // candidate keys (last_used; ~0 past the candidates) and their JanitorCand index
+  JanitorCand *cand;
+  int *cnt;                            // JC_*
+  mmp_janitor_report *report;
+};
+__global__ void k_janitor_index(JanitorBufs J, int n) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n && atomicCAS(&J.slot[J.entries[k].model], -1, k) != -1) J.cnt[JC_DUP] = 1;
+}
+__global__ void k_janitor_clear(JanitorBufs J, int n) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) J.slot[J.entries[k].model] = -1;
+}
+// one thread per model record, in the shape of k_registry_prune: self's loaded and failed registrations, remLoaded / remFailed
+// (MM:6028-6053), the record changes of the edit (MM:6059-6073), REMOVE_LOCAL (MM:6089-6091) and the scale-down candidates
+// (MM:6092-6100) with their last_used as the key
+__global__ void k_janitor_sweep(RegTables R, const mmp_model_row *__restrict__ models, const long long *__restrict__ model_lul, int n_models,
+                                int self, long long now, long long expiry_ms, JanitorBufs J) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n_models) return;
+  const mmp_model_row mr = models[m];
+  const int n_regs = (int)mr.reserved, cc = mr.copy_count;
+  if (n_regs == 0) return;
+  const ModelRegs g = model_regs(R, m, mr.reserved);
+  int loaded_pos = -1;
+  bool failed = false;
+  long long loaded_ts = 0, failed_ts = 0;
+  for (int j = 0; j < n_regs; j++) {
+    long long ts;
+    if (reg_at(R, g, j, ts) != self) continue;
+    if (j < cc) { if (loaded_pos < 0) { loaded_pos = j; loaded_ts = ts; } }
+    else if (!failed) { failed = true; failed_ts = ts; }
+  }
+  if (loaded_pos < 0 && !failed) return;
+  atomicAdd(&J.cnt[JC_REFS], 1);
+  const long long lul0 = model_lul[m];
+  if (cc == 255 && n_regs > 255) {  // where the loaded copies end is unknown (mmp_scale_eval's -1)
+    J.edits[atomicAdd(&J.cnt[JC_EDITS], 1)] = mmp_janitor_edit{m, MMP_JE_UNDECIDED, mr.last_used, lul0};
+    return;
+  }
+  const int k = J.slot[m];
+  mmp_janitor_entry ce{};
+  if (k >= 0) ce = J.entries[k];
+  const bool has = k >= 0, ce_failed = has && (ce.flags & MMP_JANITOR_FAILED), loaded = loaded_pos >= 0;
+  const bool rem_loaded = loaded && (!has || ce_failed);
+  bool rem_failed = false;
+  if (failed) {
+    if (has && !ce_failed) rem_failed = true;
+    else {
+      const long long lu = has ? ce.last_used : -1;
+      // IN_USE_LOAD_FAILURE_EXPIRY_MS when used in the last SHORT_EXPIRY_RECENT_USE_TIME_MS (MM:221, 280)
+      const long long expiry = lu > 0 && jsub(now, lu) < 180000LL ? expiry_ms / 2 : expiry_ms;
+      rem_failed = jsub(now, failed_ts) > expiry;
+    }
+  }
+  unsigned what = 0;
+  long long lu_rec = mr.last_used, lul = lul0;
+  if (rem_loaded || rem_failed) {
+    if (rem_loaded) { what |= MMP_JE_UNREGISTER; lul = cc - 1 <= 2 ? 0 : now; }  // updateLastUnloadTime after the removal
+    if (rem_failed) what |= MMP_JE_DROP_FAILURE;
+    if (has && ce.last_used > lu_rec) lu_rec = ce.last_used;                   // updateLastUsed(lastUsed) where lastUsed > 0
+  }
+  if (rem_failed && ce_failed) what |= MMP_JE_REMOVE_LOCAL;
+  int q = -1;
+  if (what) J.edits[q = atomicAdd(&J.cnt[JC_EDITS], 1)] = mmp_janitor_edit{m, what, lu_rec, lul};
+  if (loaded && !rem_loaded && ce.last_used > 0) {  // (an entry that is present and not failed)
+    const int c = atomicAdd(&J.cnt[JC_CANDS], 1);
+    J.keys[c] = (unsigned long long)ce.last_used;
+    J.vals[c] = c;
+    J.cand[c] = JanitorCand{m, k, q, 0, loaded_ts};
+  }
+}
+// removeModelCopies of every candidate with canRemove = true, and removeLocalModelCopyAsync's check of the registration time
+// against the entry's loadTimestamp (MM:6347-6349); the budget walk decides which of them run
+__global__ void k_janitor_eval(ScaleTables T, mmp_scale_params p, int self, int flags, JanitorBufs J, int n) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n || c >= J.cnt[JC_CANDS]) return;
+  const JanitorCand x = J.cand[c];
+  const mmp_janitor_entry ce = J.entries[x.entry];
+  const mmp_model_row mr = T.models[x.model];
+  const ModelRegs g = model_regs(T.R, x.model, mr.reserved);
+  const int loaded = min((int)mr.copy_count, max((int)mr.reserved, 4));  // as k_scale_eval counts them
+  J.cand[c].removes = scale_down_removes(T, p, self, x.model, ce.last_used, ce.last_heavy, ce.count, flags, g, loaded, T.rank_of[self]) &&
+                      x.reg_ts == ce.load_ts;
+}
+// one thread: the TreeSet(VALUE_COMP) over the sorted candidates (of an equal-last_used run the first model in index order,
+// quirk N15) and the budget of MM:6117-6140; SCALE_DOWN joins the model's edit or adds one; the report
+__global__ void k_janitor_walk(JanitorBufs J, const mmp_model_row *__restrict__ models, long long budget, long long now) {
+  const int nc = J.cnt[JC_CANDS];
+  int n_edits = J.cnt[JC_EDITS], kept = 0, removed = 0;
+  long long weight_removed = 0;
+  for (int s = 0; s < nc;) {
+    const unsigned long long key = J.keys[s];
+    int best = J.vals[s];
+    for (s++; s < nc && J.keys[s] == key; s++)
+      if (J.cand[J.vals[s]].model < J.cand[best].model) best = J.vals[s];
+    kept++;
+    const JanitorCand x = J.cand[best];
+    const mmp_janitor_entry ce = J.entries[x.entry];
+    if (!((removed == 0 || ce.weight <= budget) && x.removes)) continue;
+    removed++;
+    budget -= ce.weight;
+    weight_removed += ce.weight;
+    // the async removal's record changes (MM:6363-6365) on the record after this run's edit of it
+    const int cc = models[x.model].copy_count;
+    mmp_janitor_edit &e = x.edit >= 0 ? J.edits[x.edit] : J.edits[n_edits++];
+    if (x.edit < 0) e = mmp_janitor_edit{x.model, 0u, models[x.model].last_used, 0};
+    e.what |= MMP_JE_SCALE_DOWN;
+    if (ce.last_used > e.last_used) e.last_used = ce.last_used;
+    e.last_unload_time = cc - 1 <= 2 ? 0 : now;
+  }
+  *J.report = mmp_janitor_report{J.cnt[JC_REFS], n_edits, kept, removed, weight_removed};
+}
+
 extern "C" {
 
 int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mmp_scale_params *params, mmp_scale_out *out) {
@@ -332,14 +478,7 @@ int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mm
     f->launches += 3;
   }
   k_type_stats<<<(std::max(nt, 1) + 127) / 128, 128, 0, st>>>(acc, d_min, lv.type_part_off.as<int>(), lv.type_parts.as<int>(), nt, tstats);
-  ScaleTables T;
-  T.models = lv.models.as<mmp_model_row>(); T.R = reg_tables(lv);
-  T.model_lul = lv.have_times ? lv.model_lul.as<long long>() : nullptr;
-  T.rank_of = ds.rank_of.as<int32_t>(); T.rows = ds.rows.as<RankRow>(); T.part_of_rank = ds.part_of_rank.as<int32_t>();
-  T.inst_tie = lv.inst_tie.as<uint4>(); T.inst_rows = lv.inst_rows.as<mmp_instance_row>();
-  T.min_space = f->hs.cfg.min_space_units; T.churn2 = (long long)((uint64_t)f->hs.cfg.min_churn_age_ms * 2u);
-  T.type_stats = tstats; T.part_acc = acc; T.min_lru = d_min; T.sorted_rpm = rpm_sorted;
-  T.n_ranks = nr; T.n_models = f->hs.n_models_used; T.n_type_ids = nt; T.max_instances = f->hs.cfg.max_instances; T.tc_enabled = ds.host.tc_enabled;
+  const ScaleTables T = scale_tables(f, ds, lv, acc, d_min, tstats, rpm_sorted);
   k_scale_eval<<<(n + 127) / 128, 128, 0, st>>>(T, c->d_in.as<mmp_scale_in>(), n, *params, c->d_out.as<mmp_scale_out>());
   f->launches += 2;
   CK(cudaGetLastError());
@@ -523,6 +662,111 @@ int32_t mmp_reaper_run(mmp_fleet *f, int32_t leader, int64_t now_ms, int64_t ass
   memcpy(missing_since, miss.data(), (size_t)NI * 8);
   *report = mmp_reaper_report{n_pruned, n_repaired, n_sel, stopped};
   return n_sel;
+}
+
+int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *entries, int32_t n, const mmp_janitor_params *p,
+                        mmp_janitor_edit *edits, int32_t cap, mmp_janitor_report *report) {
+  NEED(f);
+  if (self < 0 || self >= f->hs.cfg.max_instances || n < 0 || (n > 0 && !entries) || !p || !report || cap < 0 || (cap > 0 && !edits)) {
+    g_err = "bad argument"; return MMP_E_ARG;
+  }
+  if (p->scale.now - p->scale.last_check_time <= 0 || p->scale.scale_up_rpm_threshold <= 0) {
+    g_err = "now must be after last_check_time and the threshold positive"; return MMP_E_ARG;
+  }
+  const int32_t max_models = f->hs.cfg.max_models;
+  for (int32_t k = 0; k < n; k++)
+    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_reaper_run)
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
+  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  LiveState &lv = f->live;
+  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
+  const DeviceSnapshot &ds = f->snaps[f->cur];
+  const int32_t NM = ds.n_models, np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  const size_t slot_b = (size_t)max_models * 4;
+  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
+    CK(c->d_jslot.ensure(slot_b));
+    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
+  }
+  const size_t nx = (size_t)std::max(n, 1), hdr_b = sizeof(mmp_janitor_report) + 8 + 16;  // [report | pad | cnt[4] | edits]
+  CK(c->d_jent.ensure(nx * sizeof(mmp_janitor_entry)));
+  CK(c->d_jcand.ensure(nx * (16 + 8 + sizeof(JanitorCand))));
+  CK(c->d_jout.ensure(hdr_b + (size_t)std::max(NM, 1) * sizeof(mmp_janitor_edit)));
+  const size_t acc_b = (size_t)(np + 1) * sizeof(StatsAcc);
+  CK(c->d_trace.ensure(acc_b + 8));
+  StatsAcc *acc = c->d_trace.as<StatsAcc>();
+  long long *d_min = reinterpret_cast<long long *>(c->d_trace.as<char>() + acc_b);
+  char *out = c->d_jout.as<char>();
+  unsigned long long *keys = c->d_jcand.as<unsigned long long>();
+  int *vals = reinterpret_cast<int *>(keys + 2 * nx);
+  JanitorBufs J{c->d_jent.as<mmp_janitor_entry>(), c->d_jslot.as<int>(), reinterpret_cast<mmp_janitor_edit *>(out + hdr_b), keys, vals,
+                reinterpret_cast<JanitorCand *>(vals + 2 * nx), reinterpret_cast<int *>(out + sizeof(mmp_janitor_report) + 8),
+                reinterpret_cast<mmp_janitor_report *>(out)};
+  JanitorBufs Js = J;  // the same with the sorted keys and values
+  Js.keys = keys + nx; Js.vals = vals + nx;
+  static const long long lru_init = 0x7fffffffffffffffLL;
+  CK(cudaMemsetAsync(acc, 0, acc_b, st));
+  CK(cudaMemcpyAsync(d_min, &lru_init, 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(J.cnt, 0, 16, st));
+  if (n) {
+    CK(cudaMemcpyAsync(c->d_jent.p, entries, (size_t)n * sizeof(mmp_janitor_entry), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(keys, 0xff, (size_t)n * 8, st));
+  }
+  CK(cudaEventRecord(c->e0, st));
+  if (nr > 0) {  // instanceSetStats / globalLru for the scale-down
+    k_stats<<<std::min(f->sm_count, (nr + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(), ds.part_of_rank.as<int32_t>(), nr,
+                                                                     f->hs.cfg.min_space_units, acc, d_min, np);
+    f->launches++;
+  }
+  if (n) { k_janitor_index<<<(n + 255) / 256, 256, 0, st>>>(J, n); f->launches++; }
+  if (NM) {
+    k_janitor_sweep<<<(NM + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.model_lul.as<long long>(), NM, self,
+                                                      p->scale.now, p->load_failure_expiry_ms, J);
+    f->launches++;
+  }
+  CK(cudaGetLastError());
+  if (n) {  // the candidates (at most one per entry) by ascending last_used; eval before the sort reads them by JanitorCand index
+    mmp_scale_params sp = p->scale;
+    sp.can_remove = 1;
+    k_janitor_eval<<<(n + 127) / 128, 128, 0, st>>>(scale_tables(f, ds, lv, acc, d_min, nullptr, nullptr), sp, self, (int)p->flags, J, n);
+    size_t tmp = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, Js.keys, vals, Js.vals, n, 0, 64, st));
+    CK(c->d_cub.ensure(tmp + 16));
+    CK(cub::DeviceRadixSort::SortPairs(c->d_cub.p, tmp, keys, Js.keys, vals, Js.vals, n, 0, 64, st));
+    f->launches += 2;
+  }
+  k_janitor_walk<<<1, 1, 0, st>>>(Js, lv.models.as<mmp_model_row>(), p->adjusted_capacity / 20, p->scale.now);
+  CK(cudaEventRecord(c->e1, st));
+  if (n) k_janitor_clear<<<(n + 255) / 256, 256, 0, st>>>(J, n);
+  f->launches += n ? 2 : 1;
+  CK(cudaGetLastError());
+  // one copy back: the report, the counters and the edits, as many as a pod is likely to have (twice its entries + 1024: most
+  // edits are of models the pod holds); more take a second copy
+  const size_t first = (size_t)std::min<int64_t>(std::max(NM, 1), 2 * (int64_t)n + 1024);
+  std::vector<char> hb(hdr_b + first * sizeof(mmp_janitor_edit));
+  CK(cudaMemcpyAsync(hb.data(), out, hb.size(), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_janitor_ms = ms; }
+  mmp_janitor_report r;
+  int cnt[4];
+  memcpy(&r, hb.data(), sizeof(r));
+  memcpy(cnt, hb.data() + sizeof(r) + 8, 16);
+  if (cnt[JC_DUP]) { g_err = "two entries of one model"; return MMP_E_ARG; }
+  std::vector<mmp_janitor_edit> ed((size_t)r.n_edits);
+  memcpy(ed.data(), hb.data() + hdr_b, std::min(ed.size(), first) * sizeof(mmp_janitor_edit));
+  if (ed.size() > first)
+    CK(cudaMemcpy(ed.data() + first, out + hdr_b + first * sizeof(mmp_janitor_edit), (ed.size() - first) * sizeof(mmp_janitor_edit),
+                  cudaMemcpyDeviceToHost));
+  std::sort(ed.begin(), ed.end(), [](const mmp_janitor_edit &a, const mmp_janitor_edit &b) { return a.model < b.model; });
+  if (cap > 0 && r.n_edits) memcpy(edits, ed.data(), (size_t)std::min(r.n_edits, cap) * sizeof(mmp_janitor_edit));
+  *report = r;
+  return r.n_edits;
 }
 
 }  // extern "C"

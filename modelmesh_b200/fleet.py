@@ -13,8 +13,8 @@ import numpy as np
 
 from . import _lib
 from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CHURN_REAPER, CLUSTER_STATS, DECISION_IN, DECISION_OUT,
-                   DECISION_TRACE, EVICTION, INSTANCE_ROW, LRU_ENTRY, LRU_EVENT, MODEL_ROW, REAPER_LOAD, ChurnConfig, ChurnReport,
-                   MmpConfig, ReaperReport)
+                   DECISION_TRACE, EVICTION, INSTANCE_ROW, JANITOR_EDIT, JANITOR_ENTRY, JANITOR_PARAMS, LRU_ENTRY, LRU_EVENT, MODEL_ROW,
+                   REAPER_LOAD, ChurnConfig, ChurnReport, JanitorReport, MmpConfig, ReaperReport)
 
 
 class MmpError(RuntimeError):
@@ -358,6 +358,20 @@ class Fleet:
                                          _ptr(rep), caps[1], _ptr(loads), caps[2], C.byref(r)))
         k = min(r.n_pruned, caps[0])
         return (pm[:k].copy(), pi[:k].copy()), rep[:min(r.n_repaired, caps[1])].copy(), loads[:min(r.n_loads, caps[2])].copy(), r
+
+    def janitor_run(self, self_idx: int, entries: np.ndarray, params: np.ndarray, cap: Optional[int] = None):
+        """mmp_janitor_run, the registry loop of one pod's janitor task: (edits (JANITOR_EDIT records, model order), report).
+        entries: JANITOR_ENTRY records of the pod's cache; params: one JANITOR_PARAMS record.  The edits hold the first
+        min(n_edits, cap); without a cap every edit (a second call when they outnumber 2 x entries + 1024)."""
+        assert entries.dtype == JANITOR_ENTRY and params.dtype == JANITOR_PARAMS and entries.flags.c_contiguous
+        room = 2 * len(entries) + 1024 if cap is None else cap
+        while True:
+            edits = np.zeros(max(room, 1), dtype=JANITOR_EDIT)
+            r = JanitorReport()
+            self._ck(self.lib.mmp_janitor_run(self.h, self_idx, _ptr(entries), len(entries), _ptr(params), _ptr(edits), room, C.byref(r)))
+            if cap is not None or r.n_edits <= room:
+                return edits[:min(r.n_edits, room)].copy(), r
+            room = r.n_edits
 
     def commit_info(self):
         path, ms = C.c_int32(), C.c_double()
