@@ -576,6 +576,81 @@ typedef struct {
 typedef struct { int32_t n_referencing, n_edits, n_candidates, n_removed; int64_t weight_removed; } mmp_janitor_report;
 int32_t mmp_janitor_run(mmp_fleet *, int32_t self, const mmp_janitor_entry *entries, int32_t n, const mmp_janitor_params *p,
                         mmp_janitor_edit *edits, int32_t cap, mmp_janitor_report *report);
+/* One run of one pod's rate-tracking task (rateTrackingTask MM:5619-5858) against the committed epoch and the registry as of
+ * the last commit, in one call: the loop body of every cache entry and the loads it triggers, placed.  entries[] is the
+ * pod's runtimeCache as the loop reads it, every entry's instance == self, at most one entry per model, in any order.
+ *   gates     report.gate (MM:5646-5670):
+ *               MMP_RATE_TOO_SOON        timeDelta * 5 < rate_check_interval_ms * 3 (Java long arithmetic): nothing is
+ *                                        evaluated, and the pod does NOT advance lastCheckTime or iterationCounter (the
+ *                                        return comes before the task's finally block)
+ *               MMP_RATE_FEW_INSTANCES   clusterStats.instanceCount < 2: nothing is evaluated (no interval count is reset);
+ *                                        the pod advances its clock and iteration
+ *               MMP_RATE_NO_ENTRIES      n == 0: as MMP_RATE_FEW_INSTANCES
+ *               MMP_RATE_RAN             the loop ran
+ *             Under a gate out[r] is action 0 with rpm 0 and the entry's own i1 / i2.
+ *   out[r]    exactly mmp_scale_eval's result for entries[r] with can_remove = 0: rpm, set_heavy, i1 / i2, action,
+ *             copies_to_load and load_last_used.
+ *   refusal   checkLoadFailureCount (MM:3771, 4607-4627): a model with 3 or more failure records (registrations past its
+ *             loaded copies) whose time is > now - load_failure_expiry_ms / 2 gets no decision (report.n_refused_failures).
+ *             checkLoadLocationCount cannot fire on these paths: the explicit excludes hold every copy.
+ *   second    action 1: one decision getNext(model, self, lastUsed = lastCheckTime) with extras {self}, no heavy set,
+ *   copy      favourSelf set (self is in toExclude, so UNBALANCED is not set: MM:6940-6943, 3526, 3782).
+ *   scale-up  action 2: a chain of copies_to_load decisions (triggerChainedLoadIfNecessary MM:4560-4585, ensureLoadedInternal
+ *             MM:6930-6952), lastUsed = now + 20 000 (MM:5675), every one excluding the call-wide heavy set of getExcludeSet
+ *             (MM:5835-5856): the instances of the epoch other than self whose published rpm is > max(4 thr, ourRpm - 2 thr),
+ *             ourRpm self's published rpm (0 when self is not in the epoch), as mmp_scale_eval reads it.
+ *               decision 0      self = the pod; favourSelf only when the pod is a loaded registration of the model
+ *               decision j > 0  self = target j-1 (the pod where target j-1 was MMP_TARGET_SELF), extras = targets 0..j-1
+ *                               (the pod for a MMP_TARGET_SELF), favourSelf set
+ *             A target of MMP_TARGET_NONE or MMP_TARGET_INVALID ends the chain (no chained trigger fires).  Decision j needs j
+ *             extras: a chain longer than MMP_RATE_CHAIN_MAX is cut after its MMP_RATE_CHAIN_MAX-th decision, which carries
+ *             MMP_RL_CHAIN_CUT and the copies not yet placed in `remaining`; the pod continues it with
+ *             mmp_place_batch_excluding (INTEGRATION.md §9).
+ *   fresh     every decision whose self is the pod reads fresh_self when given (getFreshInstanceRecord MM:5369), any other
+ *             self its published row.
+ *   draws     decision j of the chain of entries[r] (a second copy: j = 0) draws with id off[r] + j (MMP_DF_OWN_ID: id_base
+ *             plays no part), off the exclusive prefix sum in entry order of each entry's decisions: 1 for a second copy,
+ *             min(copies_to_load, MMP_RATE_CHAIN_MAX) for a scale-up, 0 when refused.  A call whose ids pass 2^24 is refused.
+ * Epoch batching: every decision reads the one committed epoch; a chained decision's self is its target's published row,
+ * not the record the target publishes mid-load; the chain assumes every target accepts its load (in the reference a
+ * rejection ends the chain: the pod drops the rest of that chain, INTEGRATION.md §9).  The latency-based mode
+ * (limitModelConcurrency, MaxConcCacheEntry) is not modelled.
+ * Loads come back in (entry, chain_pos) order, the first loads_cap of them; the report gives the totals.  Returns the number
+ * of loads.  Errors (nothing written): MMP_E_ARG for self outside [0, max_instances), an entry whose instance is not self,
+ * an entry's model out of range or two entries of one model, n < 0, p or report NULL, out NULL with n > 0, loads NULL with
+ * loads_cap > 0, a p->scale mmp_scale_eval refuses, a bad fresh_self, or ids past 2^24; MMP_E_EPOCH without a commit;
+ * MMP_E_STATE when the committed registry holds no registration times, on an instance-sharded fleet or one that connected a
+ * communicator.  Sets the "rate_run" timing. */
+#define MMP_RATE_CHAIN_MAX (MMP_MAX_EXTRA + 1)
+#define MMP_RATE_RAN 0
+#define MMP_RATE_TOO_SOON 1
+#define MMP_RATE_FEW_INSTANCES 2
+#define MMP_RATE_NO_ENTRIES 3
+typedef struct {
+  mmp_scale_params scale;          /* as mmp_scale_eval reads them; can_remove ignored (no scale-down here) */
+  int64_t load_failure_expiry_ms;  /* LOAD_FAILURE_EXPIRY_MS (MM:219); checkLoadFailureCount counts failures younger than half
+                                      of it (IN_USE_LOAD_FAILURE_EXPIRY_MS, MM:221, 4607-4627) */
+} mmp_rate_params;                 /* 80 B */
+#define MMP_RL_SECOND_COPY 1u      /* a second copy (action 1), else a decision of a scale-up chain */
+#define MMP_RL_CHAIN_CUT 2u        /* the chain was cut after this load: `remaining` copies are still to place */
+typedef struct {
+  int32_t entry, model;            /* index into entries[]; model */
+  int32_t chain_pos;               /* 0 for a second copy; 0 .. MMP_RATE_CHAIN_MAX - 1 along a scale-up chain */
+  int32_t self;                    /* the decision's self: the pod, or the previous load's target */
+  int32_t target, n_candidates;    /* as mmp_decision_out; MMP_TARGET_INVALID also for a pod not live without fresh_self */
+  int64_t last_used;               /* lastCheckTime (second copy, MM:5755) or now + 20 000 (scale-up, MM:5675) */
+  uint32_t flags, remaining;       /* MMP_RL_*; remaining: copies of the chain not yet placed when it was cut */
+} mmp_rate_load;                   /* 40 B */
+typedef struct {
+  int32_t gate;                    /* MMP_RATE_* */
+  int32_t n_second, n_scale_up;    /* entries with action 1 / 2 */
+  int32_t n_loads;                 /* decisions placed, every one of them in loads[] up to loads_cap */
+  int32_t n_heavy;                 /* size of the heavy-instance exclude set */
+  int32_t n_chains_cut, n_refused_failures, reserved;
+} mmp_rate_report;
+int32_t mmp_rate_run(mmp_fleet *, int32_t self, const mmp_scale_in *entries, int32_t n, const mmp_rate_params *p,
+                     const mmp_instance_row *fresh_self, uint64_t seed, mmp_scale_out *out, mmp_rate_load *loads,
+                     int32_t loads_cap, mmp_rate_report *report);
 
 /* tuning / measurement knobs, same meaning as the MMP_* environment variables read at mmp_fleet_create:
  *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the batch kernel ("direct" below), 1 the latency kernel
@@ -595,7 +670,7 @@ int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
  * sweep through the selection, k_rp_flag to k_rp_pick, without the stats and plan), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
  * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
  * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel; "janitor_run": mmp_janitor_run from its stats
- * kernel to its budget walk;
+ * kernel to its budget walk; "rate_run": mmp_rate_run from its stats kernel to its last placement round;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device

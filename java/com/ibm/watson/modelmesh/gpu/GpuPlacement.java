@@ -154,6 +154,13 @@ public final class GpuPlacement implements AutoCloseable {
         return check(MmPlace.janitorRun(h, self, entries, n, params, edits, cap, report));
     }
 
+    // one run of this pod's rate-tracking task (ModelMesh.java:5619-5858): returns the number of loads; report gets the gate
+    // and the totals.  freshSelf may be null
+    public int rateRun(int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, ByteBuffer out, ByteBuffer loads,
+                       int loadsCap, ByteBuffer report) {
+        return check(MmPlace.rateRun(h, self, entries, n, params, freshSelf, pickSeed.incrementAndGet(), out, loads, loadsCap, report));
+    }
+
     private int check(int rc) { if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h)); return rc; }
     @Override public void close() { committer.shutdownNow(); MmPlace.destroy(h); }
 }

@@ -52,6 +52,9 @@ final class MmPlace {
     // the registry loop of one pod's janitor task (MM:6013-6145): stale registrations, expired failures, budgeted scale-down
     static native int janitorRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer edits, int cap,
                                  ByteBuffer report);
+    // one run of one pod's rate-tracking task (MM:5619-5858): second copies, scale-up chains under the heavy-instance set (mmp_rate_run)
+    static native int rateRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, long seed,
+                              ByteBuffer out, ByteBuffer loads, int loadsCap, ByteBuffer report);
     static native int tune(long h, String key, long value);
     static native double lastTiming(long h, String key);
     // plug point 1: placement (CacheMissForwardingLB.getNext MM:4776-5004)

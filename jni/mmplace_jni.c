@@ -157,6 +157,16 @@ jint FN(janitorRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, 
   return mmp_janitor_run(H(h), self, (const mmp_janitor_entry *)BUF(entries), n, (const mmp_janitor_params *)BUF(params),
                          (mmp_janitor_edit *)BUF(edits), cap, (mmp_janitor_report *)BUF(report));
 }
+/* one run of one pod's rate-tracking task.  entries: n x mmp_scale_in (48 B), params: one mmp_rate_params (80 B), freshSelf:
+ * one mmp_instance_row (64 B) or null, out: n x mmp_scale_out (40 B), loads: loadsCap x mmp_rate_load (40 B), report: one
+ * mmp_rate_report (32 B) -- direct buffers */
+jint FN(rateRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, jint n, jobject params, jobject freshSelf, jlong seed,
+                 jobject out, jobject loads, jint loadsCap, jobject report) {
+  (void)c;
+  return mmp_rate_run(H(h), self, (const mmp_scale_in *)BUF(entries), n, (const mmp_rate_params *)BUF(params),
+                      (const mmp_instance_row *)BUF(freshSelf), (uint64_t)seed, (mmp_scale_out *)BUF(out), (mmp_rate_load *)BUF(loads),
+                      loadsCap, (mmp_rate_report *)BUF(report));
+}
 jint FN(tune)(JNIEnv *env, jclass c, jlong h, jstring key, jlong value) {
   const char *ck = utf(env, key);
   jint rc = mmp_tune(H(h), ck, value);

@@ -66,6 +66,13 @@ JANITOR_PARAMS = np.dtype([("scale", SCALE_PARAMS), ("load_failure_expiry_ms", "
                            ("reserved", "<u4")], align=True)
 JANITOR_EDIT = np.dtype([("model", "<i4"), ("what", "<u4"), ("last_used", "<i8"), ("last_unload_time", "<i8")], align=True)
 assert JANITOR_ENTRY.itemsize == 48 and JANITOR_PARAMS.itemsize == 96 and JANITOR_EDIT.itemsize == 24
+RATE_PARAMS = np.dtype([("scale", SCALE_PARAMS), ("load_failure_expiry_ms", "<i8")], align=True)
+RATE_LOAD = np.dtype([("entry", "<i4"), ("model", "<i4"), ("chain_pos", "<i4"), ("self", "<i4"), ("target", "<i4"), ("n_candidates", "<i4"),
+                      ("last_used", "<i8"), ("flags", "<u4"), ("remaining", "<u4")], align=True)
+assert RATE_PARAMS.itemsize == 80 and RATE_LOAD.itemsize == 40
+RL_SECOND_COPY, RL_CHAIN_CUT = 1, 2
+RATE_RAN, RATE_TOO_SOON, RATE_FEW_INSTANCES, RATE_NO_ENTRIES = 0, 1, 2, 3
+RATE_CHAIN_MAX = 17   # decisions one chain places: decision j carries the j targets before it as extras (MAX_EXTRA)
 LRU_LOAD = 5
 CHURN_REQUEST, CHURN_REMOVE, CHURN_REAPER = 0, 1, 2
 
@@ -87,6 +94,11 @@ class ReaperReport(C.Structure):
 class JanitorReport(C.Structure):
     _fields_ = [("n_referencing", C.c_int32), ("n_edits", C.c_int32), ("n_candidates", C.c_int32), ("n_removed", C.c_int32),
                 ("weight_removed", C.c_int64)]
+
+
+class RateReport(C.Structure):
+    _fields_ = [("gate", C.c_int32), ("n_second", C.c_int32), ("n_scale_up", C.c_int32), ("n_loads", C.c_int32), ("n_heavy", C.c_int32),
+                ("n_chains_cut", C.c_int32), ("n_refused_failures", C.c_int32), ("reserved", C.c_int32)]
 
 
 DF_FAVOUR_SELF = 1
@@ -153,6 +165,7 @@ SYMBOLS = [
     ("mmp_reaper_select", _I32, [_P, _I32, _I64, _P, _P, _I32]),
     ("mmp_reaper_run", _I32, [_P, _I32, _I64, _I64, _P, _U64, _P, _P, _I32, _P, _I32, _P, _I32, C.c_void_p]),
     ("mmp_janitor_run", _I32, [_P, _I32, _P, _I32, _P, _P, _I32, C.c_void_p]),
+    ("mmp_rate_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, _P, _I32, C.c_void_p]),
     ("mmp_lru_init", _I32, [_P, _I32, _P, _I32]),
     ("mmp_lru_apply", _I32, [_P, _P, _I32, _I64, _P, _I32]),
     ("mmp_lru_state", _I32, [_P, _I32, _P, _P, _P]),

@@ -1259,6 +1259,7 @@ struct PlaceCtx {
   RpScratch rp;  // mmp_reaper_select's pass (scan_kernels.cuh)
   DevBuf d_view, d_pruned, d_repaired, d_loads;  // mmp_reaper_run (registry_kernels.cuh): the pruned and repaired model rows, its lists
   DevBuf d_jslot, d_jent, d_jcand, d_jout;        // mmp_janitor_run (registry_kernels.cuh): entry by model, entries, candidates, results
+  DevBuf d_rate, d_rate_rpm;                      // mmp_rate_run (registry_kernels.cuh): its tables up to round 0, the rpm column
 };
 
 // The scoring kernel of untraced batches (MMP_KERNEL = direct | lanes | tile; launch_place): k_place_direct (rows rebuilt
@@ -1287,6 +1288,7 @@ struct mmp_fleet {
   float t_lru_read_ms = 0;      // ... and of the last mmp_lru_read (its count + scan part plus its emit part)
   float t_reaper_run_ms = 0;    // ... and of the last mmp_reaper_run (its prune sweep to its last placement kernel)
   float t_janitor_ms = 0;       // ... and of the last mmp_janitor_run (its stats kernel to its budget walk)
+  float t_rate_ms = 0;          // ... and of the last mmp_rate_run that ran the task (its stats kernel to its last placement round)
   int32_t last_commit_path = 0; // 1 structural (host), 2 device
   double last_commit_ms = 0;
   ncclComm_t comm = nullptr;    // instance-shard communicator (mmp_shard_connect)
@@ -2331,6 +2333,7 @@ int32_t mmp_last_timing(mmp_fleet *f, const char *key, double *ms) {
   else if (!strcmp(key, "prune")) *ms = f->t_prune_ms;
   else if (!strcmp(key, "reaper_run")) *ms = f->t_reaper_run_ms;
   else if (!strcmp(key, "janitor_run")) *ms = f->t_janitor_ms;
+  else if (!strcmp(key, "rate_run")) *ms = f->t_rate_ms;
   else if (!strcmp(key, "commit")) *ms = f->last_commit_ms;
   else if (!strcmp(key, "dealt_kernel")) *ms = f->peers.t_kernel_ms;
   else if (!strcmp(key, "dealt_wait")) *ms = f->peers.t_wait_ms;
@@ -2491,16 +2494,15 @@ static int32_t place_mapped(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds,
 }
 
 // The call's view on the derived slot tables of an exclude set: k_exclude_slots clears the set's ranks from the snapshot's
-// cand / candx / pref, k_slot_lists builds their compressed word lists.  Queued on st; the ids are in host memory.
-static int32_t derive_exclude_tables(mmp_fleet *f, PlaceCtx *c, const int32_t *exclude, int32_t n_exclude, SnapshotView &vw, cudaStream_t st) {
+// cand / candx / pref, k_slot_lists builds their compressed word lists.  Queued on st; d_ids[0, n_ids) on the device, checked
+// against [0, max_instances) by whoever made them.
+static int32_t derive_exclude_tables_dev(mmp_fleet *f, PlaceCtx *c, const int32_t *d_ids, int32_t n_ids, SnapshotView &vw, cudaStream_t st) {
   const int32_t NS = vw.n_slots, RW = vw.row_words;
   if (NS <= 0) return MMP_OK;  // (no live instance: no slot, nothing to derive)
   const size_t words = (size_t)NS * RW;
-  CK(c->d_xids.ensure((size_t)n_exclude * 4));
   CK(c->d_xcand.ensure(words * 4)); CK(c->d_xcandx.ensure(words * 4)); CK(c->d_xpref.ensure(words * 4));
   CK(c->d_xnzw.ensure(words * 2)); CK(c->d_xnz_n.ensure((size_t)NS * 4)); CK(c->d_xbefore.ensure((size_t)NS * 4));
-  CK(cudaMemcpyAsync(c->d_xids.p, exclude, (size_t)n_exclude * 4, cudaMemcpyHostToDevice, st));
-  k_exclude_slots<<<NS, 256, (size_t)RW * 4, st>>>(c->d_xids.as<int32_t>(), n_exclude, vw.rank_of, RW, vw.cand, vw.candx, vw.pref,
+  k_exclude_slots<<<NS, 256, (size_t)RW * 4, st>>>(d_ids, n_ids, vw.rank_of, RW, vw.cand, vw.candx, vw.pref,
                                                    c->d_xcand.as<uint32_t>(), c->d_xcandx.as<uint32_t>(), c->d_xpref.as<uint32_t>());
   k_slot_lists<<<(NS + 31) / 32, 32, 0, st>>>(c->d_xcand.as<uint32_t>(), c->d_xcandx.as<uint32_t>(), vw.any_rs, RW, NS, vw.word_lo, vw.word_hi,
                                              c->d_xnzw.as<uint16_t>(), c->d_xnz_n.as<int32_t>(), c->d_xbefore.as<int32_t>());
@@ -2509,6 +2511,13 @@ static int32_t derive_exclude_tables(mmp_fleet *f, PlaceCtx *c, const int32_t *e
   vw.cand = c->d_xcand.as<uint32_t>(); vw.candx = c->d_xcandx.as<uint32_t>(); vw.pref = c->d_xpref.as<uint32_t>();
   vw.nzw = c->d_xnzw.as<uint16_t>(); vw.nz_n = c->d_xnz_n.as<int32_t>(); vw.cand_before = c->d_xbefore.as<int32_t>();
   return MMP_OK;
+}
+// ... with the ids in host memory
+static int32_t derive_exclude_tables(mmp_fleet *f, PlaceCtx *c, const int32_t *exclude, int32_t n_exclude, SnapshotView &vw, cudaStream_t st) {
+  if (vw.n_slots <= 0) return MMP_OK;
+  CK(c->d_xids.ensure((size_t)n_exclude * 4));
+  CK(cudaMemcpyAsync(c->d_xids.p, exclude, (size_t)n_exclude * 4, cudaMemcpyHostToDevice, st));
+  return derive_exclude_tables_dev(f, c, c->d_xids.as<int32_t>(), n_exclude, vw, st);
 }
 
 // The one host path of mmp_place_batch / _trace / _excluding / mmp_place_one.  exclude[0, n_exclude): the call-wide exclude

@@ -4,6 +4,7 @@
 // MM:6752-6784) as ONE pass over the registry -- the part the reference's author notes "have seen it take ~10min".
 // Oracle: orc_rate_task_eval / orc_janitor_eval / orc_prune_missing (oracle/mm_sim.inc).  Included by mmplace.cu.
 #pragma once
+#include <cub/block/block_scan.cuh>
 
 struct TypeStat { long long cap, free, lru; int count, copies; };
 
@@ -42,6 +43,12 @@ __device__ __forceinline__ int count_rpm_above(const int *sorted, int n, int thr
   int lo = 0, hi = n;
   while (lo < hi) { const int mid = (lo + hi) >> 1; if (sorted[mid] <= thr) lo = mid + 1; else hi = mid; }
   return n - lo;
+}
+
+// getExcludeSet's bound (MM:5835-5856): instances whose published rpm is above it are excluded from a scale-up's loads.
+// k_scale_eval counts them, k_rate_heavy lists them.  our_rpm: the pod's published rpm (0 when it is not in the snapshot)
+__device__ __forceinline__ int exclude_set_max_rpm(int thr, int our_rpm) {
+  return max((int)((unsigned)thr * 4u), (int)((unsigned)our_rpm - 2u * (unsigned)thr));
 }
 
 // removeModelCopies (MM:6197-6335) with canRemove = true for `instance`'s copy of `model` (who-drops-the-copy by PLACEMENT_ORDER
@@ -157,7 +164,7 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
     for (int j = 0; j < loaded; j++) if (reg_at(T.R, g, j, ts) != e.instance && ts > cutoff) recent = true;  // loadedSince MM:5858-5870
     if (recent) break;
     const int our_rpm = self_rank >= 0 ? T.rows[self_rank].rpm : 0;
-    const int max_rpm = max((int)((unsigned)thr * 4u), (int)((unsigned)our_rpm - 2u * (unsigned)thr));   // getExcludeSet MM:5835-5856
+    const int max_rpm = exclude_set_max_rpm(thr, our_rpm);
     int excluded = count_rpm_above(T.sorted_rpm, T.n_ranks, max_rpm) - ((self_rank >= 0 && our_rpm > max_rpm) ? 1 : 0);
     if (excluded != 0) {
       int holding = 0;
@@ -437,36 +444,21 @@ __global__ void k_janitor_walk(JanitorBufs J, const mmp_model_row *__restrict__ 
   *J.report = mmp_janitor_report{J.cnt[JC_REFS], n_edits, kept, removed, weight_removed};
 }
 
-extern "C" {
-
-int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mmp_scale_params *params, mmp_scale_out *out) {
-  NEED(f);
-  if (n < 0 || (n > 0 && (!in || !out)) || !params) { g_err = "bad argument"; return MMP_E_ARG; }
-  if (params->now - params->last_check_time <= 0 || params->scale_up_rpm_threshold <= 0) { g_err = "now must be after last_check_time and the threshold positive"; return MMP_E_ARG; }
-  if (n == 0) return MMP_OK;
-  int32_t rc = set_device(f);
-  if (rc < 0) return rc;
-  std::lock_guard<std::mutex> g(f->ingest_mu);  // reads the live registry tables a commit rewrites
-  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  const DeviceSnapshot &ds = f->snaps[f->cur];
-  LiveState &lv = f->live;
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  cudaStream_t st = c->stream;
+// mmp_scale_eval's device part, queued on st: the stats (into c->d_trace), the sorted rpm column (into rpm), the type-set
+// stats and k_scale_eval of in[0, n) into out (both on the device).  mmp_rate_run runs the same.
+static int32_t queue_scale_eval(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, LiveState &lv, const mmp_scale_in *in, int32_t n,
+                                const mmp_scale_params &params, DevBuf &rpm, mmp_scale_out *out, cudaStream_t st) {
   const int np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks, nt = lv.n_type_ids;
   const size_t acc_bytes = (size_t)(np + 1) * sizeof(StatsAcc) + 8;
   CK(c->d_trace.ensure(acc_bytes + (size_t)std::max(nt, 1) * sizeof(TypeStat) + 64));
-  CK(c->d_fresh.ensure((size_t)std::max(nr, 1) * 8 + 64));
-  CK(c->d_in.ensure((size_t)n * sizeof(mmp_scale_in)));
-  CK(c->d_out.ensure((size_t)n * sizeof(mmp_scale_out)));
+  CK(rpm.ensure((size_t)std::max(nr, 1) * 8 + 64));
   StatsAcc *acc = c->d_trace.as<StatsAcc>();
   long long *d_min = reinterpret_cast<long long *>(c->d_trace.as<char>() + (size_t)(np + 1) * sizeof(StatsAcc));
   TypeStat *tstats = reinterpret_cast<TypeStat *>(c->d_trace.as<char>() + ((acc_bytes + 15) / 16) * 16);
-  int *rpm_raw = c->d_fresh.as<int>(), *rpm_sorted = rpm_raw + std::max(nr, 1);
+  int *rpm_raw = rpm.as<int>(), *rpm_sorted = rpm_raw + std::max(nr, 1);
   CK(cudaMemsetAsync(c->d_trace.p, 0, acc_bytes, st));
   const long long init = 0x7fffffffffffffffLL;
   CK(cudaMemcpyAsync(d_min, &init, 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(c->d_in.p, in, (size_t)n * sizeof(mmp_scale_in), cudaMemcpyHostToDevice, st));
   if (nr > 0) {
     k_stats<<<std::min(f->sm_count, (nr + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(), ds.part_of_rank.as<int32_t>(), nr,
                                                                      f->hs.cfg.min_space_units, acc, d_min, np);
@@ -479,9 +471,156 @@ int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mm
   }
   k_type_stats<<<(std::max(nt, 1) + 127) / 128, 128, 0, st>>>(acc, d_min, lv.type_part_off.as<int>(), lv.type_parts.as<int>(), nt, tstats);
   const ScaleTables T = scale_tables(f, ds, lv, acc, d_min, tstats, rpm_sorted);
-  k_scale_eval<<<(n + 127) / 128, 128, 0, st>>>(T, c->d_in.as<mmp_scale_in>(), n, *params, c->d_out.as<mmp_scale_out>());
+  k_scale_eval<<<(n + 127) / 128, 128, 0, st>>>(T, in, n, params, out);
   f->launches += 2;
   CK(cudaGetLastError());
+  return MMP_OK;
+}
+
+// mmp_rate_run: one pod's rate-tracking task (MM:5619-5858).  After k_scale_eval, k_rate_heavy lists getExcludeSet and
+// k_rate_plan (one block) applies checkLoadFailureCount and numbers the decisions: each entry's second copy (per entry, an
+// inactive record where there is none) and decision 0 of each scale-up chain (compacted in entry order).  The host reads the
+// counts back once, then places the second copies under the epoch's tables and the chains round by round under the tables
+// derived for the heavy set; k_rate_step builds round j from round j - 1.  An inactive decision has model -1: a malformed
+// record, answered MMP_TARGET_INVALID without a walk.  The pod's entries are indexed by model in the janitor's slot[] only to
+// find two entries of one model.
+struct RateHdr { int n_heavy, dup, n_second, n_scale_up, n_refused, n_sec_place, n_chain, longest; long long n_ids; };
+struct RateChain { int entry, copies, id0, len; };  // len: the decisions the chain places at most (min(copies, MMP_RATE_CHAIN_MAX))
+struct RateBufs {
+  const mmp_scale_in *entries; const mmp_scale_out *sout; int *slot;
+  mmp_decision_in *sec;    // per entry
+  mmp_decision_in *c0;     // per chain: decision 0
+  RateChain *chains;
+  int32_t *extra;          // [the pod | MMP_MAX_EXTRA per chain: its targets so far]
+  int32_t *heavy;
+  RateHdr *hdr;
+};
+__device__ __forceinline__ mmp_decision_in rate_inactive(int pod) { return mmp_decision_in{-1, pod, 0, 0u, -1, 0, 0}; }
+__global__ void k_rate_index(RateBufs B, int n) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n && atomicCAS(&B.slot[B.entries[k].model], -1, k) != -1) B.hdr->dup = 1;
+}
+__global__ void k_rate_clear(RateBufs B, int n) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) B.slot[B.entries[k].model] = -1;
+}
+// getExcludeSet (MM:5835-5856): the instances of the snapshot other than the pod whose published rpm is above the bound, in
+// no order (the derived tables do not depend on it)
+__global__ void k_rate_heavy(const int32_t *__restrict__ rank_of, const RankRow *__restrict__ rows, int max_instances, int pod, int thr,
+                             RateBufs B) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= max_instances || i == pod) return;
+  const int rk = rank_of[i];
+  if (rk < 0) return;
+  const int pr = rank_of[pod];
+  if (rows[rk].rpm > exclude_set_max_rpm(thr, pr >= 0 ? rows[pr].rpm : 0)) B.heavy[atomicAdd(&B.hdr->n_heavy, 1)] = i;
+}
+// One block over the entries in order, a tile of RATE_PLAN_THREADS at a time: checkLoadFailureCount (MM:4607-4627: 3 or more
+// failure records younger than fail_since), the ids (exclusive prefix sum of the decisions per entry) and the round-0 records
+constexpr int RATE_PLAN_THREADS = 512;
+__global__ void __launch_bounds__(RATE_PLAN_THREADS) k_rate_plan(RegTables R, const mmp_model_row *__restrict__ models, RateBufs B, int n,
+                                                                 int pod, long long fail_since, int fresh) {
+  using IdScan = cub::BlockScan<long long, RATE_PLAN_THREADS>;
+  using ChainScan = cub::BlockScan<int, RATE_PLAN_THREADS>;
+  __shared__ union { typename IdScan::TempStorage ids; typename ChainScan::TempStorage chains; } tmp;
+  __shared__ long long ids_before;
+  __shared__ int chains_before, tot[5];  // n_second, n_scale_up, n_refused, n_sec_place, longest
+  if (threadIdx.x < 5) tot[threadIdx.x] = 0;
+  if (threadIdx.x == 0) { ids_before = 0; chains_before = 0; B.extra[0] = pod; }
+  __syncthreads();
+  for (int base = 0; base < n; base += RATE_PLAN_THREADS) {
+    const int r = base + threadIdx.x;
+    int len = 0, chain = 0, favour = 0, model = -1;
+    mmp_scale_out o{};
+    if (r < n) {
+      o = B.sout[r];
+      model = B.entries[r].model;
+      if (o.action == 1 || o.action == 2) {
+        const mmp_model_row mr = models[model];
+        const ModelRegs g = model_regs(R, model, mr.reserved);
+        const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4));  // as k_scale_eval counts them
+        long long ts;
+        int recent = 0;
+        for (int j = loaded; j < n_edges; j++) {
+          reg_at(R, g, j, ts);
+          if (ts > fail_since) recent++;
+        }
+        atomicAdd(&tot[o.action == 1 ? 0 : 1], 1);
+        if (recent >= 3) atomicAdd(&tot[2], 1);
+        else if (o.action == 1) { len = 1; atomicAdd(&tot[3], 1); }
+        else if (o.copies_to_load > 0) {
+          len = min(o.copies_to_load, MMP_RATE_CHAIN_MAX);
+          chain = 1;
+          for (int j = 0; j < loaded; j++) if (reg_at(R, g, j, ts) == pod) favour = 1;
+          atomicMax(&tot[4], len);
+        }
+      }
+    }
+    long long id, ids_tile;
+    int q, chains_tile;
+    IdScan(tmp.ids).ExclusiveSum((long long)len, id, ids_tile);
+    __syncthreads();
+    ChainScan(tmp.chains).ExclusiveSum(chain, q, chains_tile);
+    id += ids_before;
+    q += chains_before;
+    if (r < n) {
+      const unsigned own = MMP_DF_OWN_ID | ((unsigned)id << 8);
+      B.sec[r] = len && !chain ? mmp_decision_in{model, pod, o.load_last_used, MMP_DF_FAVOUR_SELF | own, fresh, 0, 1} : rate_inactive(pod);
+      if (chain) {
+        B.chains[q] = RateChain{r, o.copies_to_load, (int)id, len};
+        B.c0[q] = mmp_decision_in{model, pod, o.load_last_used, (favour ? MMP_DF_FAVOUR_SELF : 0u) | own, fresh, 1 + q * MMP_MAX_EXTRA, 0};
+      }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { ids_before += ids_tile; chains_before += chains_tile; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    RateHdr *h = B.hdr;
+    h->n_second = tot[0]; h->n_scale_up = tot[1]; h->n_refused = tot[2]; h->n_sec_place = tot[3]; h->longest = tot[4];
+    h->n_chain = chains_before; h->n_ids = ids_before;
+  }
+}
+// round j >= 1 of every chain from round j - 1: self = target j - 1 (the pod for MMP_TARGET_SELF), appended to the chain's
+// extras; a chain whose target was MMP_TARGET_NONE / INVALID, or that has placed its len decisions, goes inactive
+__global__ void k_rate_step(const mmp_decision_in *__restrict__ prev, const mmp_decision_out *__restrict__ res,
+                            const RateChain *__restrict__ chains, int n_chain, int j, int pod, int fresh, int32_t *__restrict__ extra,
+                            mmp_decision_in *__restrict__ next) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n_chain) return;
+  mmp_decision_in d = prev[q];
+  const int t = res[q].target;
+  const RateChain ch = chains[q];
+  if (d.model < 0 || t == MMP_TARGET_NONE || t == MMP_TARGET_INVALID || j >= ch.len) { next[q] = rate_inactive(pod); return; }
+  const int s = t == MMP_TARGET_SELF ? pod : t;
+  extra[d.extra_off + j - 1] = s;
+  d.self = s;
+  d.fresh = s == pod ? fresh : -1;
+  d.extra_n = j;
+  d.flags = MMP_DF_FAVOUR_SELF | MMP_DF_OWN_ID | ((unsigned)(ch.id0 + j) << 8);
+  next[q] = d;
+}
+
+extern "C" {
+
+int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mmp_scale_params *params, mmp_scale_out *out) {
+  NEED(f);
+  if (n < 0 || (n > 0 && (!in || !out)) || !params) { g_err = "bad argument"; return MMP_E_ARG; }
+  if (params->now - params->last_check_time <= 0 || params->scale_up_rpm_threshold <= 0) { g_err = "now must be after last_check_time and the threshold positive"; return MMP_E_ARG; }
+  if (n == 0) return MMP_OK;
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  std::lock_guard<std::mutex> g(f->ingest_mu);  // reads the live registry tables a commit rewrites
+  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  CK(c->d_in.ensure((size_t)n * sizeof(mmp_scale_in)));
+  CK(c->d_out.ensure((size_t)n * sizeof(mmp_scale_out)));
+  CK(cudaMemcpyAsync(c->d_in.p, in, (size_t)n * sizeof(mmp_scale_in), cudaMemcpyHostToDevice, st));
+  if ((rc = queue_scale_eval(f, c.get(), f->snaps[f->cur], f->live, c->d_in.as<mmp_scale_in>(), n, *params, c->d_fresh,
+                             c->d_out.as<mmp_scale_out>(), st)) < 0)
+    return rc;
   CK(cudaMemcpyAsync(out, c->d_out.p, (size_t)n * sizeof(mmp_scale_out), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return MMP_OK;
@@ -767,6 +906,177 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
   if (cap > 0 && r.n_edits) memcpy(edits, ed.data(), (size_t)std::min(r.n_edits, cap) * sizeof(mmp_janitor_edit));
   *report = r;
   return r.n_edits;
+}
+
+
+int32_t mmp_rate_run(mmp_fleet *f, int32_t self, const mmp_scale_in *entries, int32_t n, const mmp_rate_params *p,
+                     const mmp_instance_row *fresh_self, uint64_t seed, mmp_scale_out *out, mmp_rate_load *loads, int32_t loads_cap,
+                     mmp_rate_report *report) {
+  NEED(f);
+  if (self < 0 || self >= f->hs.cfg.max_instances || n < 0 || (n > 0 && (!entries || !out)) || !p || !report || loads_cap < 0 ||
+      (loads_cap > 0 && !loads)) {
+    g_err = "bad argument"; return MMP_E_ARG;
+  }
+  mmp_scale_params sp = p->scale;
+  if (sp.now - sp.last_check_time <= 0 || sp.scale_up_rpm_threshold <= 0) {
+    g_err = "now must be after last_check_time and the threshold positive"; return MMP_E_ARG;
+  }
+  sp.can_remove = 0;
+  const int32_t max_models = f->hs.cfg.max_models;
+  for (int32_t k = 0; k < n; k++) {
+    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
+    if (entries[k].instance != self) { g_err = "an entry of another instance than self"; return MMP_E_ARG; }
+  }
+  FreshRow fr{};
+  if (fresh_self)
+    if (const char *m = HostState::fresh_row(*fresh_self, fr)) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_reaper_run)
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
+  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  LiveState &lv = f->live;
+  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
+  if (places_sharded(f, false)) {
+    g_err = "mmp_rate_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
+    return MMP_E_STATE;
+  }
+  const DeviceSnapshot &ds = f->snaps[f->cur];
+  const int32_t NI = f->hs.cfg.max_instances, fresh_idx = fresh_self ? 0 : -1;
+  // the gates of MM:5646-5670, in Java long arithmetic
+  const int64_t delta = (int64_t)((uint64_t)sp.now - (uint64_t)sp.last_check_time);
+  const bool too_soon = (int64_t)((uint64_t)delta * 5u) < (int64_t)((uint64_t)sp.rate_check_interval_ms * 3u);
+  const int gate = too_soon ? MMP_RATE_TOO_SOON : ds.host.n_ranks < 2 ? MMP_RATE_FEW_INSTANCES : n == 0 ? MMP_RATE_NO_ENTRIES : MMP_RATE_RAN;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  const size_t slot_b = (size_t)max_models * 4;
+  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
+    CK(c->d_jslot.ensure(slot_b));
+    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
+  }
+  // [header | entries | k_scale_eval's results | second copies | chains' decision 0 | chains | second copies' results | heavy set]
+  const size_t nx = (size_t)std::max(n, 1);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
+  const size_t o_hdr = take(sizeof(RateHdr)), o_ent = take(nx * sizeof(mmp_scale_in)), o_sout = take(nx * sizeof(mmp_scale_out));
+  const size_t o_sec = take(nx * sizeof(mmp_decision_in)), o_c0 = take(nx * sizeof(mmp_decision_in)), o_ch = take(nx * sizeof(RateChain));
+  const size_t o_sres = take(nx * sizeof(mmp_decision_out)), o_heavy = take((size_t)NI * 4);
+  CK(c->d_rate.ensure(off));
+  char *base = c->d_rate.as<char>();
+  RateBufs B{reinterpret_cast<mmp_scale_in *>(base + o_ent), reinterpret_cast<mmp_scale_out *>(base + o_sout), c->d_jslot.as<int>(),
+             reinterpret_cast<mmp_decision_in *>(base + o_sec), reinterpret_cast<mmp_decision_in *>(base + o_c0),
+             reinterpret_cast<RateChain *>(base + o_ch), nullptr, reinterpret_cast<int32_t *>(base + o_heavy),
+             reinterpret_cast<RateHdr *>(base + o_hdr)};
+  mmp_decision_out *sres = reinterpret_cast<mmp_decision_out *>(base + o_sres);
+  RateHdr *h_hdr = reinterpret_cast<RateHdr *>(c->mapped.get());  // the one read-back before the placement (pinned)
+  CK(cudaMemsetAsync(B.hdr, 0, sizeof(RateHdr), st));
+  if (n) CK(cudaMemcpyAsync(const_cast<mmp_scale_in *>(B.entries), entries, (size_t)n * sizeof(mmp_scale_in), cudaMemcpyHostToDevice, st));
+  if (gate != MMP_RATE_RAN) {  // nothing is evaluated; two entries of one model are still refused
+    if (n) {
+      k_rate_index<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+      k_rate_clear<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+      f->launches += 2;
+      CK(cudaGetLastError());
+      CK(cudaMemcpyAsync(h_hdr, B.hdr, sizeof(RateHdr), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (h_hdr->dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
+    }
+    for (int32_t r = 0; r < n; r++) out[r] = mmp_scale_out{0, 0, 0, 0, entries[r].i1, entries[r].i2, 0, 0};
+    *report = mmp_rate_report{gate, 0, 0, 0, 0, 0, 0, 0};
+    return 0;
+  }
+  c->fresh_host.assign(fresh_self ? 1 : 0, fr);
+  if ((rc = stage_side_tables(c.get(), c->fresh_host.data(), fresh_self ? 1 : 0, nullptr, 0, st)) < 0) return rc;
+  CK(c->d_extra.ensure(((size_t)n * MMP_MAX_EXTRA + 1) * 4));
+  B.extra = c->d_extra.as<int32_t>();
+  CK(cudaEventRecord(c->e0, st));
+  k_rate_index<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+  f->launches++;
+  if ((rc = queue_scale_eval(f, c.get(), ds, lv, B.entries, n, sp, c->d_rate_rpm, const_cast<mmp_scale_out *>(B.sout), st)) < 0) return rc;
+  k_rate_clear<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+  k_rate_heavy<<<(NI + 255) / 256, 256, 0, st>>>(ds.rank_of.as<int32_t>(), ds.rows.as<RankRow>(), NI, self, sp.scale_up_rpm_threshold, B);
+  const long long fail_since = (long long)((uint64_t)sp.now - (uint64_t)(p->load_failure_expiry_ms / 2));
+  k_rate_plan<<<1, RATE_PLAN_THREADS, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), B, n, self, fail_since, fresh_idx);
+  f->launches += 3;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(h_hdr, B.hdr, sizeof(RateHdr), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const RateHdr H = *h_hdr;
+  if (H.dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
+  if (H.n_ids > (1LL << 24)) { g_err = "the call's decision ids do not fit in 24 bits (MMP_DF_OWN_ID)"; return MMP_E_ARG; }
+  // the second copies under the epoch's tables, the chains round by round under the tables derived for the heavy set
+  const int nq = H.n_chain, L = H.longest;
+  SnapshotView vw = ds.view;
+  vw.n_extra = 1 + MMP_MAX_EXTRA * nq;
+  const int64_t now = sp.now;
+  auto place = [&](const SnapshotView &v, const mmp_decision_in *in, int cnt, mmp_decision_out *res) -> cudaError_t {
+    PlaceArgs a{v, in, cnt, c->d_fresh.as<FreshRow>(), fresh_self ? 1 : 0, B.extra, res, nullptr, nullptr, now, seed, f->id_base.load()};
+    a.ctx = c.get();
+    return launch_place(f, a, st);
+  };
+  if (H.n_sec_place) CK(place(vw, B.sec, n, sres));
+  if (nq) {
+    CK(c->d_out.ensure((size_t)L * nq * sizeof(mmp_decision_out)));
+    if (L > 1) CK(c->d_in.ensure((size_t)(L - 1) * nq * sizeof(mmp_decision_in)));
+    SnapshotView xv = vw;
+    if (H.n_heavy && (rc = derive_exclude_tables_dev(f, c.get(), B.heavy, H.n_heavy, xv, st)) < 0) return rc;
+    for (int j = 0; j < L; j++) {
+      const mmp_decision_in *dj = j ? c->d_in.as<mmp_decision_in>() + (size_t)(j - 1) * nq : B.c0;
+      if (j) {
+        const mmp_decision_in *dp = j > 1 ? c->d_in.as<mmp_decision_in>() + (size_t)(j - 2) * nq : B.c0;
+        k_rate_step<<<(nq + 255) / 256, 256, 0, st>>>(dp, c->d_out.as<mmp_decision_out>() + (size_t)(j - 1) * nq, B.chains, nq, j, self,
+                                                      fresh_idx, B.extra, const_cast<mmp_decision_in *>(dj));
+        f->launches++;
+        CK(cudaGetLastError());
+      }
+      CK(place(xv, dj, nq, c->d_out.as<mmp_decision_out>() + (size_t)j * nq));
+    }
+  }
+  CK(cudaEventRecord(c->e1, st));
+  // one copy back: the per-entry results, the second copies, the chains and every round
+  std::vector<mmp_decision_in> sec((size_t)n), dec((size_t)L * nq);
+  std::vector<mmp_decision_out> sr((size_t)n), res((size_t)L * nq);
+  std::vector<RateChain> chains((size_t)nq);
+  CK(cudaMemcpyAsync(out, B.sout, (size_t)n * sizeof(mmp_scale_out), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(sec.data(), B.sec, (size_t)n * sizeof(mmp_decision_in), cudaMemcpyDeviceToHost, st));
+  if (H.n_sec_place) CK(cudaMemcpyAsync(sr.data(), sres, (size_t)n * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, st));
+  if (nq) {
+    CK(cudaMemcpyAsync(chains.data(), B.chains, (size_t)nq * sizeof(RateChain), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(dec.data(), B.c0, (size_t)nq * sizeof(mmp_decision_in), cudaMemcpyDeviceToHost, st));
+    if (L > 1) CK(cudaMemcpyAsync(dec.data() + nq, c->d_in.p, (size_t)(L - 1) * nq * sizeof(mmp_decision_in), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(res.data(), c->d_out.p, (size_t)L * nq * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_rate_ms = ms; }
+  // the loads in (entry, chain_pos) order; a chain whose last decision would continue and that has copies left is cut there
+  std::vector<mmp_rate_load> ld;
+  int n_cut = 0;
+  for (int32_t r = 0, q = 0; r < n; r++) {
+    if (sec[r].model >= 0) {
+      ld.push_back(mmp_rate_load{r, sec[r].model, 0, self, sr[r].target, sr[r].n_candidates, sec[r].last_used, MMP_RL_SECOND_COPY, 0u});
+      continue;
+    }
+    if (q >= nq || chains[q].entry != r) continue;
+    const RateChain &ch = chains[q];
+    for (int j = 0; j < L; j++) {
+      const mmp_decision_in &d = dec[(size_t)j * nq + q];
+      if (d.model < 0) break;
+      const mmp_decision_out &o = res[(size_t)j * nq + q];
+      ld.push_back(mmp_rate_load{r, d.model, j, d.self, o.target, o.n_candidates, d.last_used, 0u, 0u});
+      if (j == MMP_RATE_CHAIN_MAX - 1 && ch.copies > MMP_RATE_CHAIN_MAX && o.target != MMP_TARGET_NONE && o.target != MMP_TARGET_INVALID) {
+        ld.back().flags |= MMP_RL_CHAIN_CUT;
+        ld.back().remaining = (uint32_t)(ch.copies - MMP_RATE_CHAIN_MAX);
+        n_cut++;
+      }
+    }
+    q++;
+  }
+  const int32_t n_loads = (int32_t)ld.size();
+  if (loads_cap > 0 && n_loads) memcpy(loads, ld.data(), (size_t)std::min(n_loads, loads_cap) * sizeof(mmp_rate_load));
+  *report = mmp_rate_report{MMP_RATE_RAN, H.n_second, H.n_scale_up, n_loads, H.n_heavy, n_cut, H.n_refused, 0};
+  return n_loads;
 }
 
 }  // extern "C"

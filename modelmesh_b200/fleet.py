@@ -14,7 +14,8 @@ import numpy as np
 from . import _lib
 from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CHURN_REAPER, CLUSTER_STATS, DECISION_IN, DECISION_OUT,
                    DECISION_TRACE, EVICTION, INSTANCE_ROW, JANITOR_EDIT, JANITOR_ENTRY, JANITOR_PARAMS, LRU_ENTRY, LRU_EVENT, MODEL_ROW,
-                   REAPER_LOAD, ChurnConfig, ChurnReport, JanitorReport, MmpConfig, ReaperReport)
+                   RATE_LOAD, RATE_PARAMS, REAPER_LOAD, SCALE_IN, SCALE_OUT, ChurnConfig, ChurnReport, JanitorReport, MmpConfig,
+                   RateReport, ReaperReport)
 
 
 class MmpError(RuntimeError):
@@ -372,6 +373,25 @@ class Fleet:
             if cap is not None or r.n_edits <= room:
                 return edits[:min(r.n_edits, room)].copy(), r
             room = r.n_edits
+
+    def rate_run(self, self_idx: int, entries: np.ndarray, params: np.ndarray, seed: int, fresh_self: Optional[np.ndarray] = None,
+                 loads_cap: Optional[int] = None):
+        """mmp_rate_run, one run of one pod's rate-tracking task: (out (SCALE_OUT per entry), loads (RATE_LOAD records in
+        (entry, chain_pos) order), report).  entries: SCALE_IN records of the pod's cache; params: one RATE_PARAMS record;
+        fresh_self: the pod's own INSTANCE_ROW or None.  The loads hold the first min(n_loads, loads_cap); without a cap
+        every load (a second call when they outnumber 2 x entries + 64)."""
+        assert entries.dtype == SCALE_IN and params.dtype == RATE_PARAMS and entries.flags.c_contiguous
+        fr = None if fresh_self is None else np.ascontiguousarray(fresh_self, dtype=INSTANCE_ROW).reshape(1)
+        room = 2 * len(entries) + 64 if loads_cap is None else loads_cap
+        while True:
+            out = np.zeros(len(entries), dtype=SCALE_OUT)
+            loads = np.zeros(max(room, 1), dtype=RATE_LOAD)
+            r = RateReport()
+            self._ck(self.lib.mmp_rate_run(self.h, self_idx, _ptr(entries), len(entries), _ptr(params), _ptr(fr), seed, _ptr(out),
+                                           _ptr(loads), room, C.byref(r)))
+            if loads_cap is not None or r.n_loads <= room:
+                return out, loads[:min(r.n_loads, room)].copy(), r
+            room = r.n_loads
 
     def commit_info(self):
         path, ms = C.c_int32(), C.c_double()
