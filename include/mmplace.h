@@ -651,6 +651,80 @@ typedef struct {
 int32_t mmp_rate_run(mmp_fleet *, int32_t self, const mmp_scale_in *entries, int32_t n, const mmp_rate_params *p,
                      const mmp_instance_row *fresh_self, uint64_t seed, mmp_scale_out *out, mmp_rate_load *loads,
                      int32_t loads_cap, mmp_rate_report *report);
+/* One pod's pre-shutdown migration (preShutdown MM:6959-7147, the distribution loop MM:6990-7047) against the committed epoch
+ * and the registry as of the last commit, in one call: for every cache entry the pod holds and is registered for, a new copy
+ * elsewhere (triggerNewModelCopyElsewhere MM:6913-6928), placed.  entries[] is runtimeCache.descendingLruMap() (MM:6990), most
+ * recently used first, at most one entry per model.  In Java long arithmetic, cutoff = now - cutoff_age_ms (MM:7000):
+ *   foundOther  some ranked instance of the epoch other than self (MM:6968-6976).  Without one nothing is evaluated or placed
+ *               (every out[r] has what 0): report.found_other = 0 and the pod deregisters every entry (MM:7133-7143).
+ *   registered  self is among the model's LOADED registrations in the committed registry, every registration looked at
+ *               (MM:7007-7010).  Otherwise (registered only as a failed load, or no record) MMP_SD_NOT_REGISTERED and nothing
+ *               else.  The registered entries are the reference's waitFor (report.n_registered).
+ *   stale       a registered entry with lru_t < cutoff: MMP_SD_STALE, counted in report.will_be_skipped (MM:7011-7014).
+ *   task body   (MM:7016-7040), registered entries:
+ *                 MMP_SD_ENTRY_GONE or _FAILED: nothing more (MM:7017-7020)
+ *                 lruTime = lru_t != 0 ? lru_t : last_used (MM:7021), into out[r].last_used
+ *                 lruTime >= 0: MMP_SD_REMOVE_LOCAL (ce.remove(), MM:7022-7024)
+ *                 MMP_SD_ENTRY_ABORTED: MMP_SD_DEREGISTER_NOW (deregisterModelAsync now, MM:7027-7030)
+ *                 lruTime > 0: checkLoadFailureCount (MM:3771, 4607-4627): 3 or more failure records (registrations past the
+ *                   loaded copies) whose time is > now - load_failure_expiry_ms / 2 refuse the load: MMP_SD_REFUSED, no decision.
+ *                   Otherwise MMP_SD_PLACED: one decision getNext(model, self, lastUsed = lruTime) excluding loaded u failed
+ *                   (the committed row) and {self}, favourSelf set (self is in toExclude, so UNBALANCED is not set:
+ *                   MM:6940-6943; with self excluded the flag cannot change the answer).  checkLoadLocationCount cannot fire:
+ *                   every copy is excluded.
+ *                 target an instance (>= 0) and lruTime >= cutoff: MMP_SD_WAIT, the `return ent` of MM:7037-7038 -- the pod
+ *                   waits for this load.  MMP_TARGET_NONE is "Nowhere available to load": logged, not waited for.
+ *   fresh       every decision reads fresh_self when given, else the pod's published row; a pod that is not ranked and has no
+ *               fresh_self is answered MMP_TARGET_INVALID (as by mmp_rate_run).  The answers do not depend on whether the pod's
+ *               own shutting-down record has been committed: self is excluded, and an unranked instance is in no candidate set.
+ *   draws       entries[r]'s decision draws with id r (MMP_DF_OWN_ID: id_base plays no part), so an answer does not depend on
+ *               which other entries were placed, and equals mmp_place_batch's on the same 32-byte record with the same seed.
+ * Epoch batching: every decision reads the one committed epoch (the reference's tasks run concurrently on taskPool against a
+ * clusterState that has not seen their loads yet); one fresh_self for every decision (the reference's fresh record drifts
+ * as the tasks' ce.remove() calls empty the cache); the registry as of the last commit (the pod's KV writes catch the
+ * difference).  Not modelled (stays in the pod): abortLoadings, publishInstanceRecord, removeUnloadBufferEntry, the wait
+ * phase (MM:7048-7122) and every deregisterModelAsync write (INTEGRATION.md §10).
+ * out[r] is entries[r]'s action, in entry order; without a decision target is MMP_TARGET_INVALID and n_candidates 0, and
+ * last_used is 0 where the task body did not compute lruTime.  Returns n.  Errors (nothing written): MMP_E_ARG for self
+ * outside [0, max_instances), an entry's model out of range or two entries of one model, n < 0 or n > 2^24, p or report
+ * NULL, entries or out NULL with n > 0, or a bad fresh_self; MMP_E_EPOCH without a commit; MMP_E_STATE when the committed
+ * registry holds no registration times, on an instance-sharded fleet or one that connected a communicator.  Sets the
+ * "shutdown_run" timing. */
+#define MMP_SD_ENTRY_GONE 1u       /* runtimeCache.getQuietly(model) returned null */
+#define MMP_SD_ENTRY_FAILED 2u     /* ce.isFailed() */
+#define MMP_SD_ENTRY_ABORTED 4u    /* ce.isAborted() after abortLoadings() */
+typedef struct {
+  int32_t model; uint32_t flags;   /* model index; MMP_SD_ENTRY_* */
+  int64_t lru_t;                   /* the descendingLruMap value */
+  int64_t last_used;               /* runtimeCache.getLastUsedTime(model): -1 when absent or <= 0 (CLHM:742-746) */
+} mmp_shutdown_entry;              /* 24 B */
+typedef struct {
+  int64_t now;
+  int64_t cutoff_age_ms;           /* CUTOFF_AGE_MS (MM:276): 3 600 000 */
+  int64_t load_failure_expiry_ms;  /* LOAD_FAILURE_EXPIRY_MS (MM:219); checkLoadFailureCount counts failures younger than half */
+} mmp_shutdown_params;             /* 24 B */
+#define MMP_SD_NOT_REGISTERED 1u   /* self is not a loaded registration of the model: skipped (MM:7008-7010) */
+#define MMP_SD_STALE 2u            /* lru_t < cutoff: counted in willBeSkipped (MM:7012-7014) */
+#define MMP_SD_REMOVE_LOCAL 4u     /* lruTime >= 0: ce.remove() (MM:7022-7024) */
+#define MMP_SD_DEREGISTER_NOW 8u   /* aborted: deregisterModelAsync(model, lruTime, loadTimestamp, ...) now (MM:7027-7030) */
+#define MMP_SD_PLACED 16u          /* a decision was made: target / n_candidates are its answer */
+#define MMP_SD_REFUSED 32u         /* lruTime > 0, but checkLoadFailureCount refused the load: no decision */
+#define MMP_SD_WAIT 64u            /* target is an instance and lruTime >= cutoff: the pod waits for the load (MM:7037-7038) */
+typedef struct {
+  int32_t model; uint32_t what;    /* model; the OR of MMP_SD_* */
+  int32_t target, n_candidates;    /* as mmp_decision_out with MMP_SD_PLACED, else MMP_TARGET_INVALID and 0 */
+  int64_t last_used;               /* the lruTime used, 0 where it was not computed */
+} mmp_shutdown_action;             /* 24 B */
+typedef struct {
+  int32_t found_other;             /* 1: some ranked instance other than self; 0: nothing was evaluated */
+  int32_t n_registered;            /* entries registered for self: the reference's waitFor.size() */
+  int32_t will_be_skipped;         /* registered entries with lru_t < cutoff */
+  int32_t n_placed, n_none, n_refused, n_wait;  /* entries with MMP_SD_PLACED, of them target MMP_TARGET_NONE; MMP_SD_REFUSED;
+                                                   MMP_SD_WAIT */
+  int32_t reserved;
+} mmp_shutdown_report;             /* 32 B */
+int32_t mmp_shutdown_run(mmp_fleet *, int32_t self, const mmp_shutdown_entry *entries, int32_t n, const mmp_shutdown_params *p,
+                         const mmp_instance_row *fresh_self, uint64_t seed, mmp_shutdown_action *out, mmp_shutdown_report *report);
 
 /* tuning / measurement knobs, same meaning as the MMP_* environment variables read at mmp_fleet_create:
  *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the batch kernel ("direct" below), 1 the latency kernel
@@ -670,7 +744,8 @@ int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
  * sweep through the selection, k_rp_flag to k_rp_pick, without the stats and plan), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
  * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
  * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel; "janitor_run": mmp_janitor_run from its stats
- * kernel to its budget walk; "rate_run": mmp_rate_run from its stats kernel to its last placement round;
+ * kernel to its budget walk; "rate_run": mmp_rate_run from its stats kernel to its last placement round; "shutdown_run":
+ * mmp_shutdown_run from its index kernel to its pack kernel;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device

@@ -161,6 +161,12 @@ public final class GpuPlacement implements AutoCloseable {
         return check(MmPlace.rateRun(h, self, entries, n, params, freshSelf, pickSeed.incrementAndGet(), out, loads, loadsCap, report));
     }
 
+    // this pod's pre-shutdown migration (ModelMesh.java:6990-7047): out gets one action per entry of descendingLruMap(), report
+    // foundOther and the totals; returns n.  freshSelf may be null
+    public int shutdownRun(int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, ByteBuffer out, ByteBuffer report) {
+        return check(MmPlace.shutdownRun(h, self, entries, n, params, freshSelf, pickSeed.incrementAndGet(), out, report));
+    }
+
     private int check(int rc) { if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h)); return rc; }
     @Override public void close() { committer.shutdownNow(); MmPlace.destroy(h); }
 }

@@ -55,6 +55,9 @@ final class MmPlace {
     // one run of one pod's rate-tracking task (MM:5619-5858): second copies, scale-up chains under the heavy-instance set (mmp_rate_run)
     static native int rateRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, long seed,
                               ByteBuffer out, ByteBuffer loads, int loadsCap, ByteBuffer report);
+    // one pod's pre-shutdown migration (MM:6990-7047): a new copy elsewhere for every registered cache entry (mmp_shutdown_run)
+    static native int shutdownRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, long seed,
+                                  ByteBuffer out, ByteBuffer report);
     static native int tune(long h, String key, long value);
     static native double lastTiming(long h, String key);
     // plug point 1: placement (CacheMissForwardingLB.getNext MM:4776-5004)

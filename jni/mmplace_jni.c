@@ -167,6 +167,16 @@ jint FN(rateRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, jin
                       (const mmp_instance_row *)BUF(freshSelf), (uint64_t)seed, (mmp_scale_out *)BUF(out), (mmp_rate_load *)BUF(loads),
                       loadsCap, (mmp_rate_report *)BUF(report));
 }
+/* one pod's pre-shutdown migration.  entries: n x mmp_shutdown_entry (24 B), params: one mmp_shutdown_params (24 B), freshSelf:
+ * one mmp_instance_row (64 B) or null, out: n x mmp_shutdown_action (24 B), report: one mmp_shutdown_report (32 B) -- direct
+ * buffers */
+jint FN(shutdownRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, jint n, jobject params, jobject freshSelf, jlong seed,
+                     jobject out, jobject report) {
+  (void)c;
+  return mmp_shutdown_run(H(h), self, (const mmp_shutdown_entry *)BUF(entries), n, (const mmp_shutdown_params *)BUF(params),
+                          (const mmp_instance_row *)BUF(freshSelf), (uint64_t)seed, (mmp_shutdown_action *)BUF(out),
+                          (mmp_shutdown_report *)BUF(report));
+}
 jint FN(tune)(JNIEnv *env, jclass c, jlong h, jstring key, jlong value) {
   const char *ck = utf(env, key);
   jint rc = mmp_tune(H(h), ck, value);

@@ -73,6 +73,13 @@ assert RATE_PARAMS.itemsize == 80 and RATE_LOAD.itemsize == 40
 RL_SECOND_COPY, RL_CHAIN_CUT = 1, 2
 RATE_RAN, RATE_TOO_SOON, RATE_FEW_INSTANCES, RATE_NO_ENTRIES = 0, 1, 2, 3
 RATE_CHAIN_MAX = 17   # decisions one chain places: decision j carries the j targets before it as extras (MAX_EXTRA)
+SHUTDOWN_ENTRY = np.dtype([("model", "<i4"), ("flags", "<u4"), ("lru_t", "<i8"), ("last_used", "<i8")], align=True)
+SHUTDOWN_PARAMS = np.dtype([("now", "<i8"), ("cutoff_age_ms", "<i8"), ("load_failure_expiry_ms", "<i8")], align=True)
+SHUTDOWN_ACTION = np.dtype([("model", "<i4"), ("what", "<u4"), ("target", "<i4"), ("n_candidates", "<i4"), ("last_used", "<i8")],
+                           align=True)
+assert SHUTDOWN_ENTRY.itemsize == 24 and SHUTDOWN_PARAMS.itemsize == 24 and SHUTDOWN_ACTION.itemsize == 24
+SD_ENTRY_GONE, SD_ENTRY_FAILED, SD_ENTRY_ABORTED = 1, 2, 4
+SD_NOT_REGISTERED, SD_STALE, SD_REMOVE_LOCAL, SD_DEREGISTER_NOW, SD_PLACED, SD_REFUSED, SD_WAIT = 1, 2, 4, 8, 16, 32, 64
 LRU_LOAD = 5
 CHURN_REQUEST, CHURN_REMOVE, CHURN_REAPER = 0, 1, 2
 
@@ -99,6 +106,11 @@ class JanitorReport(C.Structure):
 class RateReport(C.Structure):
     _fields_ = [("gate", C.c_int32), ("n_second", C.c_int32), ("n_scale_up", C.c_int32), ("n_loads", C.c_int32), ("n_heavy", C.c_int32),
                 ("n_chains_cut", C.c_int32), ("n_refused_failures", C.c_int32), ("reserved", C.c_int32)]
+
+
+class ShutdownReport(C.Structure):
+    _fields_ = [("found_other", C.c_int32), ("n_registered", C.c_int32), ("will_be_skipped", C.c_int32), ("n_placed", C.c_int32),
+                ("n_none", C.c_int32), ("n_refused", C.c_int32), ("n_wait", C.c_int32), ("reserved", C.c_int32)]
 
 
 DF_FAVOUR_SELF = 1
@@ -166,6 +178,7 @@ SYMBOLS = [
     ("mmp_reaper_run", _I32, [_P, _I32, _I64, _I64, _P, _U64, _P, _P, _I32, _P, _I32, _P, _I32, C.c_void_p]),
     ("mmp_janitor_run", _I32, [_P, _I32, _P, _I32, _P, _P, _I32, C.c_void_p]),
     ("mmp_rate_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, _P, _I32, C.c_void_p]),
+    ("mmp_shutdown_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, C.c_void_p]),
     ("mmp_lru_init", _I32, [_P, _I32, _P, _I32]),
     ("mmp_lru_apply", _I32, [_P, _P, _I32, _I64, _P, _I32]),
     ("mmp_lru_state", _I32, [_P, _I32, _P, _P, _P]),

@@ -515,8 +515,18 @@ __global__ void k_rate_heavy(const int32_t *__restrict__ rank_of, const RankRow 
   const int pr = rank_of[pod];
   if (rows[rk].rpm > exclude_set_max_rpm(thr, pr >= 0 ? rows[pr].rpm : 0)) B.heavy[atomicAdd(&B.hdr->n_heavy, 1)] = i;
 }
-// One block over the entries in order, a tile of RATE_PLAN_THREADS at a time: checkLoadFailureCount (MM:4607-4627: 3 or more
-// failure records younger than fail_since), the ids (exclusive prefix sum of the decisions per entry) and the round-0 records
+// checkLoadFailureCount (MM:3771, 4607-4627): 3 or more failure records (the registrations past the `loaded` copies) whose time
+// is after fail_since refuse the load.  k_rate_plan and k_shutdown_plan both ask it
+__device__ __forceinline__ bool load_failures_refuse(const RegTables &R, const ModelRegs &g, int loaded, int n_edges, long long fail_since) {
+  int recent = 0;
+  long long ts;
+  for (int j = loaded; j < n_edges; j++) {
+    reg_at(R, g, j, ts);
+    if (ts > fail_since) recent++;
+  }
+  return recent >= 3;
+}
+// One block over the entries in order, a tile of RATE_PLAN_THREADS at a time: checkLoadFailureCount (load_failures_refuse), the ids (exclusive prefix sum of the decisions per entry) and the round-0 records
 constexpr int RATE_PLAN_THREADS = 512;
 __global__ void __launch_bounds__(RATE_PLAN_THREADS) k_rate_plan(RegTables R, const mmp_model_row *__restrict__ models, RateBufs B, int n,
                                                                  int pod, long long fail_since, int fresh) {
@@ -540,13 +550,8 @@ __global__ void __launch_bounds__(RATE_PLAN_THREADS) k_rate_plan(RegTables R, co
         const ModelRegs g = model_regs(R, model, mr.reserved);
         const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4));  // as k_scale_eval counts them
         long long ts;
-        int recent = 0;
-        for (int j = loaded; j < n_edges; j++) {
-          reg_at(R, g, j, ts);
-          if (ts > fail_since) recent++;
-        }
         atomicAdd(&tot[o.action == 1 ? 0 : 1], 1);
-        if (recent >= 3) atomicAdd(&tot[2], 1);
+        if (load_failures_refuse(R, g, loaded, n_edges, fail_since)) atomicAdd(&tot[2], 1);
         else if (o.action == 1) { len = 1; atomicAdd(&tot[3], 1); }
         else if (o.copies_to_load > 0) {
           len = min(o.copies_to_load, MMP_RATE_CHAIN_MAX);
@@ -599,6 +604,72 @@ __global__ void k_rate_step(const mmp_decision_in *__restrict__ prev, const mmp_
   d.extra_n = j;
   d.flags = MMP_DF_FAVOUR_SELF | MMP_DF_OWN_ID | ((unsigned)(ch.id0 + j) << 8);
   next[q] = d;
+}
+
+// mmp_shutdown_run: one pod's pre-shutdown migration (MM:6990-7047).  k_shutdown_plan classifies every entry and writes its
+// decision, or rate_inactive's record where there is none; launch_place answers all n; k_shutdown_pack adds the answers and
+// the wait test.  The entries take their model's slot of the janitor's slot[] in k_shutdown_plan and give it back in
+// k_shutdown_pack, a later launch on the same stream: two entries of one model are found without a launch of their own.
+struct SdHdr { mmp_shutdown_report rep; int dup, pad[3]; };  // (48 B: the actions follow it in one copy back)
+struct SdBufs {
+  const mmp_shutdown_entry *entries; int *slot;
+  mmp_decision_in *dec; const mmp_decision_out *res;
+  SdHdr *hdr; mmp_shutdown_action *out;
+  int32_t *extra;  // [the pod]
+};
+// one thread per entry: foundOther (MM:6968-6976), the registry test over every registration (MM:7007-7010), willBeSkipped
+// (MM:7011-7014), the task body up to its getNext (MM:7017-7032) with checkLoadFailureCount
+__global__ void k_shutdown_plan(RegTables R, const mmp_model_row *__restrict__ models, const int32_t *__restrict__ rank_of, int n_ranks,
+                                SdBufs B, int n, int pod, long long cutoff, long long fail_since, int fresh) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool found_other = n_ranks - (rank_of[pod] >= 0 ? 1 : 0) > 0;
+  if (r == 0) { B.hdr->rep.found_other = found_other; B.extra[0] = pod; }
+  if (r >= n) return;
+  const mmp_shutdown_entry e = B.entries[r];
+  if (atomicCAS(&B.slot[e.model], -1, r) != -1) B.hdr->dup = 1;
+  unsigned what = 0;
+  long long lru = 0;
+  if (found_other) {
+    const mmp_model_row mr = models[e.model];
+    const ModelRegs g = model_regs(R, e.model, mr.reserved);
+    const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4));  // as k_rate_plan counts them
+    bool registered = false;
+    long long ts;
+    for (int j = 0; j < loaded && !registered; j++) registered = reg_at(R, g, j, ts) == pod;
+    if (!registered) {
+      what = MMP_SD_NOT_REGISTERED;
+    } else {
+      atomicAdd(&B.hdr->rep.n_registered, 1);
+      if (e.lru_t < cutoff) { what |= MMP_SD_STALE; atomicAdd(&B.hdr->rep.will_be_skipped, 1); }
+      if (!(e.flags & (MMP_SD_ENTRY_GONE | MMP_SD_ENTRY_FAILED))) {
+        lru = e.lru_t != 0 ? e.lru_t : e.last_used;
+        if (lru >= 0) what |= MMP_SD_REMOVE_LOCAL;
+        if (e.flags & MMP_SD_ENTRY_ABORTED) what |= MMP_SD_DEREGISTER_NOW;
+        if (lru > 0) {
+          if (load_failures_refuse(R, g, loaded, n_edges, fail_since)) { what |= MMP_SD_REFUSED; atomicAdd(&B.hdr->rep.n_refused, 1); }
+          else what |= MMP_SD_PLACED;
+        }
+      }
+    }
+  }
+  B.dec[r] = (what & MMP_SD_PLACED) ? mmp_decision_in{e.model, pod, lru, MMP_DF_FAVOUR_SELF | MMP_DF_OWN_ID | ((unsigned)r << 8), fresh, 0, 1}
+                                    : rate_inactive(pod);
+  B.out[r] = mmp_shutdown_action{e.model, what, MMP_TARGET_INVALID, 0, lru};
+}
+// one thread per entry: the answer, Status.LOADING && lruTime >= cutoff (MM:7037-7038) as a target that is an instance
+__global__ void k_shutdown_pack(SdBufs B, int n, long long cutoff) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  mmp_shutdown_action a = B.out[r];
+  B.slot[a.model] = -1;
+  if (!(a.what & MMP_SD_PLACED)) return;
+  const mmp_decision_out o = B.res[r];
+  a.target = o.target;
+  a.n_candidates = o.n_candidates;
+  atomicAdd(&B.hdr->rep.n_placed, 1);
+  if (o.target == MMP_TARGET_NONE) atomicAdd(&B.hdr->rep.n_none, 1);
+  else if (o.target >= 0 && a.last_used >= cutoff) { a.what |= MMP_SD_WAIT; atomicAdd(&B.hdr->rep.n_wait, 1); }
+  B.out[r] = a;
 }
 
 extern "C" {
@@ -1077,6 +1148,88 @@ int32_t mmp_rate_run(mmp_fleet *f, int32_t self, const mmp_scale_in *entries, in
   if (loads_cap > 0 && n_loads) memcpy(loads, ld.data(), (size_t)std::min(n_loads, loads_cap) * sizeof(mmp_rate_load));
   *report = mmp_rate_report{MMP_RATE_RAN, H.n_second, H.n_scale_up, n_loads, H.n_heavy, n_cut, H.n_refused, 0};
   return n_loads;
+}
+
+int32_t mmp_shutdown_run(mmp_fleet *f, int32_t self, const mmp_shutdown_entry *entries, int32_t n, const mmp_shutdown_params *p,
+                         const mmp_instance_row *fresh_self, uint64_t seed, mmp_shutdown_action *out, mmp_shutdown_report *report) {
+  NEED(f);
+  if (self < 0 || self >= f->hs.cfg.max_instances || n < 0 || n > (1 << 24) || (n > 0 && (!entries || !out)) || !p || !report) {
+    g_err = "bad argument"; return MMP_E_ARG;  // (n <= 2^24: entry r draws with id r, MMP_DF_OWN_ID's 24 bits)
+  }
+  const int32_t max_models = f->hs.cfg.max_models;
+  for (int32_t k = 0; k < n; k++)
+    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
+  FreshRow fr{};
+  if (fresh_self)
+    if (const char *m = HostState::fresh_row(*fresh_self, fr)) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_rate_run)
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
+  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  LiveState &lv = f->live;
+  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
+  if (places_sharded(f, false)) {
+    g_err = "mmp_shutdown_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
+    return MMP_E_STATE;
+  }
+  const DeviceSnapshot &ds = f->snaps[f->cur];
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  const size_t slot_b = (size_t)max_models * 4;
+  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
+    CK(c->d_jslot.ensure(slot_b));
+    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
+  }
+  // [entries | decisions | results | header | actions]: the header and the actions come back in one copy
+  const size_t nx = (size_t)std::max(n, 1);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
+  const size_t o_ent = take(nx * sizeof(mmp_shutdown_entry)), o_dec = take(nx * sizeof(mmp_decision_in));
+  const size_t o_res = take(nx * sizeof(mmp_decision_out)), o_hdr = take(sizeof(SdHdr)), o_out = take(nx * sizeof(mmp_shutdown_action));
+  static_assert(sizeof(SdHdr) % 16 == 0, "the actions follow the header");
+  CK(c->d_sd.ensure(off));
+  char *base = c->d_sd.as<char>();
+  SdBufs B{reinterpret_cast<mmp_shutdown_entry *>(base + o_ent), c->d_jslot.as<int>(), reinterpret_cast<mmp_decision_in *>(base + o_dec),
+           reinterpret_cast<mmp_decision_out *>(base + o_res), reinterpret_cast<SdHdr *>(base + o_hdr),
+           reinterpret_cast<mmp_shutdown_action *>(base + o_out), nullptr};
+  c->fresh_host.assign(fresh_self ? 1 : 0, fr);
+  if ((rc = stage_side_tables(c.get(), c->fresh_host.data(), fresh_self ? 1 : 0, nullptr, 0, st)) < 0) return rc;
+  B.extra = c->d_extra.as<int32_t>();
+  CK(cudaMemsetAsync(B.hdr, 0, sizeof(SdHdr), st));
+  if (n) CK(cudaMemcpyAsync(const_cast<mmp_shutdown_entry *>(B.entries), entries, (size_t)n * sizeof(mmp_shutdown_entry), cudaMemcpyHostToDevice, st));
+  const int64_t now = p->now;
+  const long long cutoff = (long long)((uint64_t)now - (uint64_t)p->cutoff_age_ms);
+  const long long fail_since = (long long)((uint64_t)now - (uint64_t)(p->load_failure_expiry_ms / 2));
+  CK(cudaEventRecord(c->e0, st));
+  k_shutdown_plan<<<std::max((n + 255) / 256, 1), 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), ds.rank_of.as<int32_t>(),
+                                                                ds.host.n_ranks, B, n, self, cutoff, fail_since, fresh_self ? 0 : -1);
+  f->launches++;
+  CK(cudaGetLastError());
+  if (n) {
+    SnapshotView vw = ds.view;
+    vw.n_extra = 1;
+    PlaceArgs a{vw, B.dec, n, c->d_fresh.as<FreshRow>(), fresh_self ? 1 : 0, B.extra, const_cast<mmp_decision_out *>(B.res), nullptr,
+                nullptr, now, seed, f->id_base.load()};
+    a.ctx = c.get();
+    CK(launch_place(f, a, st));
+    k_shutdown_pack<<<(n + 255) / 256, 256, 0, st>>>(B, n, cutoff);
+    f->launches++;
+    CK(cudaGetLastError());
+  }
+  CK(cudaEventRecord(c->e1, st));
+  std::vector<char> back(sizeof(SdHdr) + (size_t)n * sizeof(mmp_shutdown_action));
+  CK(cudaMemcpyAsync(back.data(), B.hdr, back.size(), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_shutdown_ms = ms; }
+  SdHdr H;
+  memcpy(&H, back.data(), sizeof(SdHdr));
+  if (H.dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
+  if (n) memcpy(out, back.data() + sizeof(SdHdr), (size_t)n * sizeof(mmp_shutdown_action));
+  *report = H.rep;
+  return n;
 }
 
 }  // extern "C"

@@ -14,8 +14,8 @@ import numpy as np
 from . import _lib
 from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CHURN_REAPER, CLUSTER_STATS, DECISION_IN, DECISION_OUT,
                    DECISION_TRACE, EVICTION, INSTANCE_ROW, JANITOR_EDIT, JANITOR_ENTRY, JANITOR_PARAMS, LRU_ENTRY, LRU_EVENT, MODEL_ROW,
-                   RATE_LOAD, RATE_PARAMS, REAPER_LOAD, SCALE_IN, SCALE_OUT, ChurnConfig, ChurnReport, JanitorReport, MmpConfig,
-                   RateReport, ReaperReport)
+                   RATE_LOAD, RATE_PARAMS, REAPER_LOAD, SCALE_IN, SCALE_OUT, SHUTDOWN_ACTION, SHUTDOWN_ENTRY, SHUTDOWN_PARAMS,
+                   ChurnConfig, ChurnReport, JanitorReport, MmpConfig, RateReport, ReaperReport, ShutdownReport)
 
 
 class MmpError(RuntimeError):
@@ -392,6 +392,22 @@ class Fleet:
             if loads_cap is not None or r.n_loads <= room:
                 return out, loads[:min(r.n_loads, room)].copy(), r
             room = r.n_loads
+
+    def shutdown_run(self, self_idx: int, entries: np.ndarray, params: np.ndarray, seed: int, fresh_self: Optional[np.ndarray] = None,
+                     out: Optional[np.ndarray] = None):
+        """mmp_shutdown_run, one pod's pre-shutdown migration: (out (SHUTDOWN_ACTION per entry, entry order), report).
+        entries: SHUTDOWN_ENTRY records of runtimeCache.descendingLruMap(); params: one SHUTDOWN_PARAMS record; fresh_self: the
+        pod's own INSTANCE_ROW or None.  out: a caller-allocated SHUTDOWN_ACTION array of len(entries) to write into (one is
+        allocated when None); a caller that runs the call often allocates it once."""
+        assert entries.dtype == SHUTDOWN_ENTRY and params.dtype == SHUTDOWN_PARAMS and entries.flags.c_contiguous
+        if out is None:
+            out = np.zeros(len(entries), dtype=SHUTDOWN_ACTION)
+        assert out.dtype == SHUTDOWN_ACTION and len(out) == len(entries) and out.flags.c_contiguous
+        fr = None if fresh_self is None else np.ascontiguousarray(fresh_self, dtype=INSTANCE_ROW).reshape(1)
+        r = ShutdownReport()
+        self._ck(self.lib.mmp_shutdown_run(self.h, self_idx, _ptr(entries), len(entries), _ptr(params), _ptr(fr), seed, _ptr(out),
+                                           C.byref(r)))
+        return out, r
 
     def commit_info(self):
         path, ms = C.c_int32(), C.c_double()
