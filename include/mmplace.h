@@ -725,6 +725,77 @@ typedef struct {
 } mmp_shutdown_report;             /* 32 B */
 int32_t mmp_shutdown_run(mmp_fleet *, int32_t self, const mmp_shutdown_entry *entries, int32_t n, const mmp_shutdown_params *p,
                          const mmp_instance_row *fresh_self, uint64_t seed, mmp_shutdown_action *out, mmp_shutdown_report *report);
+/* One pod's eviction listener (onEviction MM:2867-2933) for a burst of evictions, against the committed epoch and the registry
+ * as of the last commit, in one call: every evicted copy deregistered (deregisterModel MM:2936-2962), and a copy elsewhere
+ * placed for each one the rebalance rule reloads (ensureLoadedElsewhere MM:6905).  entries[] are the evictions the pod's cache
+ * reported, in listener order, at most one entry per model.  Per entry, in Java long arithmetic, over every registration of the
+ * model (the overflow ones included), loaded = the first copy_count registrations, the rest failed loads:
+ *   deregister  MMP_EV_UNREGISTER: the pod's loaded registration has time load_ts (instanceIds.remove(self, loadTime)).
+ *               MMP_EV_DROP_FAILURE: the pod's failed registration has time load_complete_ts (removeLoadFailure, MR:173-179).
+ *               Neither: no write.  Otherwise out[r].last_used is the record's lastUsed after updateLastUsed(last_used) (0 reads
+ *               as now, MR:239-246) and last_unload_time after updateLastUnloadTime where the pod is unregistered (0 when at
+ *               most 2 loaded copies remain, else now, MR:260-262); both are mmp_janitor_run's record arithmetic.  Without a
+ *               write, and for last_unload_time without MMP_EV_UNREGISTER, they are the record's own values.
+ *   reload      MMP_EV_RELOAD (attemptReload, MM:2886-2896): the entry is not MMP_EV_ENTRY_FAILED, the pod has a registration,
+ *               and now - t > 2 * load_timeout_ms, t the time of its loaded registration, else of its failed one (the record
+ *               before the edit).
+ *   gate        a reload whose model's type set is full (MM:2918-2920): typeSetStats of the model's committed type in the
+ *               epoch, totalCapacity > 0 && instanceCount > 1 && 20 * totalFree / totalCapacity >= 1, fails:
+ *               MMP_EV_CLUSTER_FULL, nothing more.
+ *   elsewhere   ensureLoadedElsewhere on the record after the edit (MM:6905-6907, ensureLoadedInternal with {self} excluded):
+ *                 MMP_EV_LOADED_ELSEWHERE  a loaded registration other than the pod on an instance the epoch ranks: the
+ *                                          reference forwards to it and returns LOADED without a load (MM:3540-3760), so
+ *                                          checkLoadLocationCount cannot fire either
+ *                 MMP_EV_REFUSED           checkLoadFailureCount (MM:3771, 4607-4627): 3 or more failure records whose time is
+ *                                          > now - load_failure_expiry_ms / 2; a failure record the edit dropped does not count
+ *                 MMP_EV_PLACED            one decision getNext(model, self, lastUsed = last_used) excluding the committed
+ *                                          registrations and {self}, favourSelf set (self is in toExclude, so UNBALANCED is
+ *                                          not set: MM:6940-6943)
+ *   fresh       every decision reads fresh_self when given, else the pod's published row; a pod that is not ranked and has no
+ *               fresh_self is answered MMP_TARGET_INVALID (as by mmp_shutdown_run).
+ *   draws       entries[r]'s decision draws with id r (MMP_DF_OWN_ID), so an answer equals mmp_place_batch's on the same 32-byte
+ *               record with the same seed and does not depend on the other entries.
+ * Epoch batching: every reload reads the one committed epoch and one fresh_self (the reference's tasks run concurrently on
+ * taskPool against a clusterState that has not seen their loads yet); the registry is read as of the last commit, and the
+ * pod's KV writes catch the difference; "live" is "ranked by the epoch".  Not modelled (stays in the pod): ce.doRemove, the
+ * unload-buffer accounting, the conditional write and its retry, and issuing the load (INTEGRATION.md §11).
+ * out[r] is entries[r]'s action, in entry order; without a decision target is MMP_TARGET_INVALID and n_candidates 0.  Returns
+ * n.  Errors (nothing written): MMP_E_ARG for self outside [0, max_instances), an entry's model out of range or two entries
+ * of one model, n < 0 or n > 2^24, p or report NULL, entries or out NULL with n > 0, or a bad fresh_self; MMP_E_EPOCH without
+ * a commit; MMP_E_STATE when the committed registry holds no registration times, on an instance-sharded fleet or one that
+ * connected a communicator.  Sets the "evict_run" timing. */
+#define MMP_EV_ENTRY_FAILED 1u     /* ce.isFailed(): a cached load failure */
+typedef struct {
+  int32_t model; uint32_t flags;   /* model index; MMP_EV_ENTRY_* */
+  int64_t last_used;               /* the listener's lastUsed */
+  int64_t load_ts;                 /* ce.loadTimestamp */
+  int64_t load_complete_ts;        /* ce.loadCompleteTimestamp */
+} mmp_evict_entry;                 /* 32 B */
+typedef struct {
+  int64_t now;
+  int64_t load_timeout_ms;         /* loadTimeoutMs: attemptReload needs the registration to be older than twice it */
+  int64_t load_failure_expiry_ms;  /* LOAD_FAILURE_EXPIRY_MS (MM:219); checkLoadFailureCount counts failures younger than half */
+} mmp_evict_params;                /* 24 B */
+#define MMP_EV_UNREGISTER 1u       /* the pod's loaded registration (time load_ts) is removed, updateLastUnloadTime */
+#define MMP_EV_DROP_FAILURE 2u     /* the pod's failed registration (time load_complete_ts) is removed */
+#define MMP_EV_RELOAD 4u           /* attemptReload */
+#define MMP_EV_CLUSTER_FULL 8u     /* a reload the rebalance gate stops: the model's type set is 95 % full or has one instance */
+#define MMP_EV_LOADED_ELSEWHERE 16u /* a reload answered by a loaded copy on another ranked instance: no load */
+#define MMP_EV_REFUSED 32u         /* a reload checkLoadFailureCount refused: no decision */
+#define MMP_EV_PLACED 64u          /* a decision was made: target / n_candidates are its answer */
+typedef struct {
+  int32_t model; uint32_t what;    /* model; the OR of MMP_EV_* */
+  int32_t target, n_candidates;    /* as mmp_decision_out with MMP_EV_PLACED, else MMP_TARGET_INVALID and 0 */
+  int64_t last_used;               /* the record's lastUsed after the edit (its own without a write) */
+  int64_t last_unload_time;        /* the record's lastUnloadTime after the edit (its own without MMP_EV_UNREGISTER) */
+} mmp_evict_action;                /* 32 B */
+typedef struct {
+  int32_t n_unregister, n_drop_failure, n_reload, n_cluster_full;  /* entries with each MMP_EV_* bit */
+  int32_t n_loaded_elsewhere, n_refused, n_placed;
+  int32_t n_none;                  /* of the MMP_EV_PLACED entries, those answered MMP_TARGET_NONE */
+} mmp_evict_report;                /* 32 B */
+int32_t mmp_evict_run(mmp_fleet *, int32_t self, const mmp_evict_entry *entries, int32_t n, const mmp_evict_params *p,
+                      const mmp_instance_row *fresh_self, uint64_t seed, mmp_evict_action *out, mmp_evict_report *report);
 
 /* tuning / measurement knobs, same meaning as the MMP_* environment variables read at mmp_fleet_create:
  *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the batch kernel ("direct" below), 1 the latency kernel
@@ -745,7 +816,7 @@ int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
  * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
  * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel; "janitor_run": mmp_janitor_run from its stats
  * kernel to its budget walk; "rate_run": mmp_rate_run from its stats kernel to its last placement round; "shutdown_run":
- * mmp_shutdown_run from its index kernel to its pack kernel;
+ * mmp_shutdown_run from its index kernel to its pack kernel; "evict_run": mmp_evict_run from its stats kernel to its pack kernel;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device

@@ -167,6 +167,12 @@ public final class GpuPlacement implements AutoCloseable {
         return check(MmPlace.shutdownRun(h, self, entries, n, params, freshSelf, pickSeed.incrementAndGet(), out, report));
     }
 
+    // this pod's eviction listener (ModelMesh.java:2867-2933) for the evictions its cache reported, in listener order: out gets
+    // one action per entry (the deregistration edit, and the reload's answer), report the totals; returns n.  freshSelf may be null
+    public int evictRun(int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, ByteBuffer out, ByteBuffer report) {
+        return check(MmPlace.evictRun(h, self, entries, n, params, freshSelf, pickSeed.incrementAndGet(), out, report));
+    }
+
     private int check(int rc) { if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h)); return rc; }
     @Override public void close() { committer.shutdownNow(); MmPlace.destroy(h); }
 }

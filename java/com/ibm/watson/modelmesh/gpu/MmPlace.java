@@ -58,6 +58,9 @@ final class MmPlace {
     // one pod's pre-shutdown migration (MM:6990-7047): a new copy elsewhere for every registered cache entry (mmp_shutdown_run)
     static native int shutdownRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, long seed,
                                   ByteBuffer out, ByteBuffer report);
+    // one pod's eviction listener (MM:2867-2933) over a burst of evictions: deregistration edits and reloads elsewhere (mmp_evict_run)
+    static native int evictRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, long seed,
+                               ByteBuffer out, ByteBuffer report);
     static native int tune(long h, String key, long value);
     static native double lastTiming(long h, String key);
     // plug point 1: placement (CacheMissForwardingLB.getNext MM:4776-5004)

@@ -177,6 +177,16 @@ jint FN(shutdownRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries,
                           (const mmp_instance_row *)BUF(freshSelf), (uint64_t)seed, (mmp_shutdown_action *)BUF(out),
                           (mmp_shutdown_report *)BUF(report));
 }
+/* one pod's eviction listener over a burst of evictions.  entries: n x mmp_evict_entry (32 B), params: one mmp_evict_params
+ * (24 B), freshSelf: one mmp_instance_row (64 B) or null, out: n x mmp_evict_action (32 B), report: one mmp_evict_report
+ * (32 B) -- direct buffers */
+jint FN(evictRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, jint n, jobject params, jobject freshSelf, jlong seed,
+                  jobject out, jobject report) {
+  (void)c;
+  return mmp_evict_run(H(h), self, (const mmp_evict_entry *)BUF(entries), n, (const mmp_evict_params *)BUF(params),
+                       (const mmp_instance_row *)BUF(freshSelf), (uint64_t)seed, (mmp_evict_action *)BUF(out),
+                       (mmp_evict_report *)BUF(report));
+}
 jint FN(tune)(JNIEnv *env, jclass c, jlong h, jstring key, jlong value) {
   const char *ck = utf(env, key);
   jint rc = mmp_tune(H(h), ck, value);

@@ -80,6 +80,14 @@ SHUTDOWN_ACTION = np.dtype([("model", "<i4"), ("what", "<u4"), ("target", "<i4")
 assert SHUTDOWN_ENTRY.itemsize == 24 and SHUTDOWN_PARAMS.itemsize == 24 and SHUTDOWN_ACTION.itemsize == 24
 SD_ENTRY_GONE, SD_ENTRY_FAILED, SD_ENTRY_ABORTED = 1, 2, 4
 SD_NOT_REGISTERED, SD_STALE, SD_REMOVE_LOCAL, SD_DEREGISTER_NOW, SD_PLACED, SD_REFUSED, SD_WAIT = 1, 2, 4, 8, 16, 32, 64
+EVICT_ENTRY = np.dtype([("model", "<i4"), ("flags", "<u4"), ("last_used", "<i8"), ("load_ts", "<i8"), ("load_complete_ts", "<i8")],
+                       align=True)
+EVICT_PARAMS = np.dtype([("now", "<i8"), ("load_timeout_ms", "<i8"), ("load_failure_expiry_ms", "<i8")], align=True)
+EVICT_ACTION = np.dtype([("model", "<i4"), ("what", "<u4"), ("target", "<i4"), ("n_candidates", "<i4"), ("last_used", "<i8"),
+                         ("last_unload_time", "<i8")], align=True)
+assert EVICT_ENTRY.itemsize == 32 and EVICT_PARAMS.itemsize == 24 and EVICT_ACTION.itemsize == 32
+EV_ENTRY_FAILED = 1
+EV_UNREGISTER, EV_DROP_FAILURE, EV_RELOAD, EV_CLUSTER_FULL, EV_LOADED_ELSEWHERE, EV_REFUSED, EV_PLACED = 1, 2, 4, 8, 16, 32, 64
 LRU_LOAD = 5
 CHURN_REQUEST, CHURN_REMOVE, CHURN_REAPER = 0, 1, 2
 
@@ -111,6 +119,11 @@ class RateReport(C.Structure):
 class ShutdownReport(C.Structure):
     _fields_ = [("found_other", C.c_int32), ("n_registered", C.c_int32), ("will_be_skipped", C.c_int32), ("n_placed", C.c_int32),
                 ("n_none", C.c_int32), ("n_refused", C.c_int32), ("n_wait", C.c_int32), ("reserved", C.c_int32)]
+
+
+class EvictReport(C.Structure):
+    _fields_ = [("n_unregister", C.c_int32), ("n_drop_failure", C.c_int32), ("n_reload", C.c_int32), ("n_cluster_full", C.c_int32),
+                ("n_loaded_elsewhere", C.c_int32), ("n_refused", C.c_int32), ("n_placed", C.c_int32), ("n_none", C.c_int32)]
 
 
 DF_FAVOUR_SELF = 1
@@ -179,6 +192,7 @@ SYMBOLS = [
     ("mmp_janitor_run", _I32, [_P, _I32, _P, _I32, _P, _P, _I32, C.c_void_p]),
     ("mmp_rate_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, _P, _I32, C.c_void_p]),
     ("mmp_shutdown_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, C.c_void_p]),
+    ("mmp_evict_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, C.c_void_p]),
     ("mmp_lru_init", _I32, [_P, _I32, _P, _I32]),
     ("mmp_lru_apply", _I32, [_P, _P, _I32, _I64, _P, _I32]),
     ("mmp_lru_state", _I32, [_P, _I32, _P, _P, _P]),

@@ -1261,6 +1261,7 @@ struct PlaceCtx {
   DevBuf d_jslot, d_jent, d_jcand, d_jout;        // mmp_janitor_run (registry_kernels.cuh): entry by model, entries, candidates, results
   DevBuf d_rate, d_rate_rpm;                      // mmp_rate_run (registry_kernels.cuh): its tables up to round 0, the rpm column
   DevBuf d_sd;                                    // mmp_shutdown_run (registry_kernels.cuh): entries, decisions, results, report, actions
+  DevBuf d_ev;                                    // mmp_evict_run (registry_kernels.cuh): entries, decisions, results, report, actions
 };
 
 // The scoring kernel of untraced batches (MMP_KERNEL = direct | lanes | tile; launch_place): k_place_direct (rows rebuilt
@@ -1291,6 +1292,7 @@ struct mmp_fleet {
   float t_janitor_ms = 0;       // ... and of the last mmp_janitor_run (its stats kernel to its budget walk)
   float t_rate_ms = 0;          // ... and of the last mmp_rate_run that ran the task (its stats kernel to its last placement round)
   float t_shutdown_ms = 0;      // ... and of the last mmp_shutdown_run (its index kernel to its pack kernel)
+  float t_evict_ms = 0;         // ... and of the last mmp_evict_run (its stats kernel to its pack kernel)
   int32_t last_commit_path = 0; // 1 structural (host), 2 device
   double last_commit_ms = 0;
   ncclComm_t comm = nullptr;    // instance-shard communicator (mmp_shard_connect)
@@ -2337,6 +2339,7 @@ int32_t mmp_last_timing(mmp_fleet *f, const char *key, double *ms) {
   else if (!strcmp(key, "janitor_run")) *ms = f->t_janitor_ms;
   else if (!strcmp(key, "rate_run")) *ms = f->t_rate_ms;
   else if (!strcmp(key, "shutdown_run")) *ms = f->t_shutdown_ms;
+  else if (!strcmp(key, "evict_run")) *ms = f->t_evict_ms;
   else if (!strcmp(key, "commit")) *ms = f->last_commit_ms;
   else if (!strcmp(key, "dealt_kernel")) *ms = f->peers.t_kernel_ms;
   else if (!strcmp(key, "dealt_wait")) *ms = f->peers.t_wait_ms;

@@ -343,6 +343,14 @@ __global__ void k_janitor_clear(JanitorBufs J, int n) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k < n) J.slot[J.entries[k].model] = -1;
 }
+// a deregistration's record changes (the janitor's MM:6059-6073, deregisterModel's MM:2955-2957): updateLastUnloadTime where
+// self's loaded copy left the record's cc loaded copies (MR:260-262), and updateLastUsed(lu) where use_lu (MR:239-246; the
+// callers decide what lu is and when it applies).  k_janitor_sweep, k_janitor_walk and k_evict_plan all make it
+__device__ __forceinline__ void dereg_record_edit(bool unregistered, bool use_lu, long long lu, int cc, long long now, int64_t &lu_rec,
+                                                  int64_t &lul) {
+  if (unregistered) lul = cc - 1 <= 2 ? 0 : now;
+  if (use_lu && lu > lu_rec) lu_rec = lu;
+}
 // one thread per model record, in the shape of k_registry_prune: self's loaded and failed registrations, remLoaded / remFailed
 // (MM:6028-6053), the record changes of the edit (MM:6059-6073), REMOVE_LOCAL (MM:6089-6091) and the scale-down candidates
 // (MM:6092-6100) with their last_used as the key
@@ -386,11 +394,11 @@ __global__ void k_janitor_sweep(RegTables R, const mmp_model_row *__restrict__ m
     }
   }
   unsigned what = 0;
-  long long lu_rec = mr.last_used, lul = lul0;
+  int64_t lu_rec = mr.last_used, lul = lul0;
   if (rem_loaded || rem_failed) {
-    if (rem_loaded) { what |= MMP_JE_UNREGISTER; lul = cc - 1 <= 2 ? 0 : now; }  // updateLastUnloadTime after the removal
+    if (rem_loaded) what |= MMP_JE_UNREGISTER;
     if (rem_failed) what |= MMP_JE_DROP_FAILURE;
-    if (has && ce.last_used > lu_rec) lu_rec = ce.last_used;                   // updateLastUsed(lastUsed) where lastUsed > 0
+    dereg_record_edit(rem_loaded, has, ce.last_used, cc, now, lu_rec, lul);  // updateLastUsed(lastUsed) where lastUsed > 0
   }
   if (rem_failed && ce_failed) what |= MMP_JE_REMOVE_LOCAL;
   int q = -1;
@@ -438,41 +446,56 @@ __global__ void k_janitor_walk(JanitorBufs J, const mmp_model_row *__restrict__ 
     mmp_janitor_edit &e = x.edit >= 0 ? J.edits[x.edit] : J.edits[n_edits++];
     if (x.edit < 0) e = mmp_janitor_edit{x.model, 0u, models[x.model].last_used, 0};
     e.what |= MMP_JE_SCALE_DOWN;
-    if (ce.last_used > e.last_used) e.last_used = ce.last_used;
-    e.last_unload_time = cc - 1 <= 2 ? 0 : now;
+    dereg_record_edit(true, true, ce.last_used, cc, now, e.last_used, e.last_unload_time);
   }
   *J.report = mmp_janitor_report{J.cnt[JC_REFS], n_edits, kept, removed, weight_removed};
 }
 
-// mmp_scale_eval's device part, queued on st: the stats (into c->d_trace), the sorted rpm column (into rpm), the type-set
-// stats and k_scale_eval of in[0, n) into out (both on the device).  mmp_rate_run runs the same.
-static int32_t queue_scale_eval(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, LiveState &lv, const mmp_scale_in *in, int32_t n,
-                                const mmp_scale_params &params, DevBuf &rpm, mmp_scale_out *out, cudaStream_t st) {
+// the epoch's type-set stats, queued on st: k_stats (the per-partition accumulators and the global LRU, into c->d_trace) and
+// k_type_stats per type id.  queue_scale_eval and mmp_evict_run read them
+struct TypeSetStats { StatsAcc *acc; long long *d_min; TypeStat *types; };
+static int32_t queue_type_stats(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, LiveState &lv, TypeSetStats &S, cudaStream_t st) {
   const int np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks, nt = lv.n_type_ids;
   const size_t acc_bytes = (size_t)(np + 1) * sizeof(StatsAcc) + 8;
   CK(c->d_trace.ensure(acc_bytes + (size_t)std::max(nt, 1) * sizeof(TypeStat) + 64));
-  CK(rpm.ensure((size_t)std::max(nr, 1) * 8 + 64));
-  StatsAcc *acc = c->d_trace.as<StatsAcc>();
-  long long *d_min = reinterpret_cast<long long *>(c->d_trace.as<char>() + (size_t)(np + 1) * sizeof(StatsAcc));
-  TypeStat *tstats = reinterpret_cast<TypeStat *>(c->d_trace.as<char>() + ((acc_bytes + 15) / 16) * 16);
-  int *rpm_raw = rpm.as<int>(), *rpm_sorted = rpm_raw + std::max(nr, 1);
+  S.acc = c->d_trace.as<StatsAcc>();
+  S.d_min = reinterpret_cast<long long *>(c->d_trace.as<char>() + (size_t)(np + 1) * sizeof(StatsAcc));
+  S.types = reinterpret_cast<TypeStat *>(c->d_trace.as<char>() + ((acc_bytes + 15) / 16) * 16);
   CK(cudaMemsetAsync(c->d_trace.p, 0, acc_bytes, st));
-  const long long init = 0x7fffffffffffffffLL;
-  CK(cudaMemcpyAsync(d_min, &init, 8, cudaMemcpyHostToDevice, st));
+  static const long long init = 0x7fffffffffffffffLL;
+  CK(cudaMemcpyAsync(S.d_min, &init, 8, cudaMemcpyHostToDevice, st));
   if (nr > 0) {
     k_stats<<<std::min(f->sm_count, (nr + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(), ds.part_of_rank.as<int32_t>(), nr,
-                                                                     f->hs.cfg.min_space_units, acc, d_min, np);
+                                                                     f->hs.cfg.min_space_units, S.acc, S.d_min, np);
+    f->launches++;
+  }
+  k_type_stats<<<(std::max(nt, 1) + 127) / 128, 128, 0, st>>>(S.acc, S.d_min, lv.type_part_off.as<int>(), lv.type_parts.as<int>(), nt, S.types);
+  f->launches++;
+  CK(cudaGetLastError());
+  return MMP_OK;
+}
+
+// mmp_scale_eval's device part, queued on st: the type-set stats (queue_type_stats), the sorted rpm column (into rpm) and
+// k_scale_eval of in[0, n) into out (both on the device).  mmp_rate_run runs the same.
+static int32_t queue_scale_eval(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, LiveState &lv, const mmp_scale_in *in, int32_t n,
+                                const mmp_scale_params &params, DevBuf &rpm, mmp_scale_out *out, cudaStream_t st) {
+  const int nr = ds.host.n_ranks;
+  TypeSetStats S;
+  const int32_t rc = queue_type_stats(f, c, ds, lv, S, st);
+  if (rc < 0) return rc;
+  CK(rpm.ensure((size_t)std::max(nr, 1) * 8 + 64));
+  int *rpm_raw = rpm.as<int>(), *rpm_sorted = rpm_raw + std::max(nr, 1);
+  if (nr > 0) {
     k_extract_rpm<<<(nr + 255) / 256, 256, 0, st>>>(ds.rows.as<RankRow>(), nr, rpm_raw);
     size_t tmp = 0;
     CK(cub::DeviceRadixSort::SortKeys(nullptr, tmp, rpm_raw, rpm_sorted, nr, 0, 32, st));
     CK(c->d_cub.ensure(tmp + 16));
     CK(cub::DeviceRadixSort::SortKeys(c->d_cub.p, tmp, rpm_raw, rpm_sorted, nr, 0, 32, st));
-    f->launches += 3;
+    f->launches += 2;
   }
-  k_type_stats<<<(std::max(nt, 1) + 127) / 128, 128, 0, st>>>(acc, d_min, lv.type_part_off.as<int>(), lv.type_parts.as<int>(), nt, tstats);
-  const ScaleTables T = scale_tables(f, ds, lv, acc, d_min, tstats, rpm_sorted);
+  const ScaleTables T = scale_tables(f, ds, lv, S.acc, S.d_min, S.types, rpm_sorted);
   k_scale_eval<<<(n + 127) / 128, 128, 0, st>>>(T, in, n, params, out);
-  f->launches += 2;
+  f->launches++;
   CK(cudaGetLastError());
   return MMP_OK;
 }
@@ -516,9 +539,11 @@ __global__ void k_rate_heavy(const int32_t *__restrict__ rank_of, const RankRow 
   if (rows[rk].rpm > exclude_set_max_rpm(thr, pr >= 0 ? rows[pr].rpm : 0)) B.heavy[atomicAdd(&B.hdr->n_heavy, 1)] = i;
 }
 // checkLoadFailureCount (MM:3771, 4607-4627): 3 or more failure records (the registrations past the `loaded` copies) whose time
-// is after fail_since refuse the load.  k_rate_plan and k_shutdown_plan both ask it
-__device__ __forceinline__ bool load_failures_refuse(const RegTables &R, const ModelRegs &g, int loaded, int n_edges, long long fail_since) {
-  int recent = 0;
+// is after fail_since refuse the load.  dropped: how many of those records the caller's own edit removed first (k_evict_plan:
+// the pod's failure record that deregisterModel dropped).  k_rate_plan, k_shutdown_plan and k_evict_plan all ask it
+__device__ __forceinline__ bool load_failures_refuse(const RegTables &R, const ModelRegs &g, int loaded, int n_edges, long long fail_since,
+                                                     int dropped = 0) {
+  int recent = -dropped;
   long long ts;
   for (int j = loaded; j < n_edges; j++) {
     reg_at(R, g, j, ts);
@@ -669,6 +694,81 @@ __global__ void k_shutdown_pack(SdBufs B, int n, long long cutoff) {
   atomicAdd(&B.hdr->rep.n_placed, 1);
   if (o.target == MMP_TARGET_NONE) atomicAdd(&B.hdr->rep.n_none, 1);
   else if (o.target >= 0 && a.last_used >= cutoff) { a.what |= MMP_SD_WAIT; atomicAdd(&B.hdr->rep.n_wait, 1); }
+  B.out[r] = a;
+}
+
+// mmp_evict_run: one pod's eviction listener (MM:2867-2933) for a burst of evictions.  The type-set stats come from
+// queue_type_stats; k_evict_plan makes every entry's deregistration edit and decides its reload, writing the decision or
+// rate_inactive's record; launch_place answers all n; k_evict_pack adds the answers and the report.  The entries take their
+// model's slot of the janitor's slot[] in k_evict_plan and give it back in k_evict_pack, as mmp_shutdown_run's do.
+struct EvHdr { mmp_evict_report rep; int dup, pad[3]; };  // (48 B: the actions follow it in one copy back)
+struct EvBufs {
+  const mmp_evict_entry *entries; int *slot;
+  mmp_decision_in *dec; const mmp_decision_out *res;
+  EvHdr *hdr; mmp_evict_action *out;
+  int32_t *extra;  // [the pod]
+};
+// one thread per entry: the pod's registrations over every registration of the model, deregisterModel's edit (MM:2948-2957,
+// the record arithmetic through dereg_record_edit), attemptReload on the record before it (MM:2886-2896), the rebalance gate
+// (MM:2918-2920) and ensureLoadedElsewhere up to its getNext on the record after it: a live copy elsewhere, then
+// checkLoadFailureCount without the failure record the edit dropped
+__global__ void k_evict_plan(RegTables R, const mmp_model_row *__restrict__ models, const long long *__restrict__ model_lul,
+                             const int32_t *__restrict__ rank_of, const TypeStat *__restrict__ type_stats, int n_type_ids, EvBufs B, int n,
+                             int pod, long long now, long long reload_age, long long fail_since, int fresh) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0) B.extra[0] = pod;
+  if (r >= n) return;
+  const mmp_evict_entry e = B.entries[r];
+  if (atomicCAS(&B.slot[e.model], -1, r) != -1) B.hdr->dup = 1;
+  const mmp_model_row mr = models[e.model];
+  const ModelRegs g = model_regs(R, e.model, mr.reserved);
+  const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4));  // as k_shutdown_plan counts them
+  // the pod's first loaded and first failed registration (as k_janitor_sweep finds them), and a loaded copy on another ranked
+  // instance
+  int loaded_at = -1, failed_at = -1;
+  long long loaded_ts = 0, failed_ts = 0;
+  bool live_elsewhere = false;
+  for (int j = 0, top = max(loaded, n_edges); j < top; j++) {
+    long long ts;
+    const int i = reg_at(R, g, j, ts);
+    if (i == pod) {
+      if (j < loaded) { if (loaded_at < 0) { loaded_at = j; loaded_ts = ts; } }
+      else if (failed_at < 0) { failed_at = j; failed_ts = ts; }
+    } else if (j < loaded && i >= 0 && rank_of[i] >= 0) {
+      live_elsewhere = true;
+    }
+  }
+  const bool unreg = loaded_at >= 0 && loaded_ts == e.load_ts, drop = failed_at >= 0 && failed_ts == e.load_complete_ts;
+  unsigned what = (unreg ? MMP_EV_UNREGISTER : 0u) | (drop ? MMP_EV_DROP_FAILURE : 0u);
+  int64_t lu_rec = mr.last_used, lul = model_lul[e.model];
+  if (unreg || drop) dereg_record_edit(unreg, true, e.last_used == 0 ? now : e.last_used, mr.copy_count, now, lu_rec, lul);
+  if (!(e.flags & MMP_EV_ENTRY_FAILED) && (loaded_at >= 0 || failed_at >= 0) && jsub(now, loaded_at >= 0 ? loaded_ts : failed_ts) > reload_age) {
+    what |= MMP_EV_RELOAD;
+    const TypeStat cs = type_stats[mr.type_id < n_type_ids ? mr.type_id : 0];
+    if (!(cs.cap > 0 && cs.count > 1 && jmul64(20, cs.free) / cs.cap >= 1)) what |= MMP_EV_CLUSTER_FULL;
+    else if (live_elsewhere) what |= MMP_EV_LOADED_ELSEWHERE;
+    else if (load_failures_refuse(R, g, loaded, n_edges, fail_since, drop && failed_ts > fail_since)) what |= MMP_EV_REFUSED;
+    else what |= MMP_EV_PLACED;
+  }
+  B.dec[r] = (what & MMP_EV_PLACED) ? mmp_decision_in{e.model, pod, e.last_used, MMP_DF_FAVOUR_SELF | MMP_DF_OWN_ID | ((unsigned)r << 8), fresh, 0, 1}
+                                    : rate_inactive(pod);
+  B.out[r] = mmp_evict_action{e.model, what, MMP_TARGET_INVALID, 0, lu_rec, lul};
+}
+// one thread per entry: the answer, and the report (one counter per MMP_EV_* bit, in bit order, then n_none)
+__global__ void k_evict_pack(EvBufs B, int n) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  mmp_evict_action a = B.out[r];
+  B.slot[a.model] = -1;
+  int32_t *cnt = &B.hdr->rep.n_unregister;
+#pragma unroll
+  for (int b = 0; b < 7; b++)
+    if (a.what & (1u << b)) atomicAdd(cnt + b, 1);
+  if (!(a.what & MMP_EV_PLACED)) return;
+  const mmp_decision_out o = B.res[r];
+  a.target = o.target;
+  a.n_candidates = o.n_candidates;
+  if (o.target == MMP_TARGET_NONE) atomicAdd(&B.hdr->rep.n_none, 1);
   B.out[r] = a;
 }
 
@@ -1228,6 +1328,89 @@ int32_t mmp_shutdown_run(mmp_fleet *f, int32_t self, const mmp_shutdown_entry *e
   memcpy(&H, back.data(), sizeof(SdHdr));
   if (H.dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
   if (n) memcpy(out, back.data() + sizeof(SdHdr), (size_t)n * sizeof(mmp_shutdown_action));
+  *report = H.rep;
+  return n;
+}
+
+int32_t mmp_evict_run(mmp_fleet *f, int32_t self, const mmp_evict_entry *entries, int32_t n, const mmp_evict_params *p,
+                      const mmp_instance_row *fresh_self, uint64_t seed, mmp_evict_action *out, mmp_evict_report *report) {
+  NEED(f);
+  if (self < 0 || self >= f->hs.cfg.max_instances || n < 0 || n > (1 << 24) || (n > 0 && (!entries || !out)) || !p || !report) {
+    g_err = "bad argument"; return MMP_E_ARG;  // (n <= 2^24: entry r draws with id r, MMP_DF_OWN_ID's 24 bits)
+  }
+  const int32_t max_models = f->hs.cfg.max_models;
+  for (int32_t k = 0; k < n; k++)
+    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
+  FreshRow fr{};
+  if (fresh_self)
+    if (const char *m = HostState::fresh_row(*fresh_self, fr)) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_shutdown_run)
+  std::lock_guard<std::mutex> g(f->ingest_mu);
+  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
+  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  LiveState &lv = f->live;
+  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
+  if (places_sharded(f, false)) {
+    g_err = "mmp_evict_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
+    return MMP_E_STATE;
+  }
+  const DeviceSnapshot &ds = f->snaps[f->cur];
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  const size_t slot_b = (size_t)max_models * 4;
+  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
+    CK(c->d_jslot.ensure(slot_b));
+    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
+  }
+  // [entries | decisions | results | header | actions]: the header and the actions come back in one copy
+  const size_t nx = (size_t)std::max(n, 1);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
+  const size_t o_ent = take(nx * sizeof(mmp_evict_entry)), o_dec = take(nx * sizeof(mmp_decision_in));
+  const size_t o_res = take(nx * sizeof(mmp_decision_out)), o_hdr = take(sizeof(EvHdr)), o_out = take(nx * sizeof(mmp_evict_action));
+  static_assert(sizeof(EvHdr) % 16 == 0, "the actions follow the header");
+  CK(c->d_ev.ensure(off));
+  char *base = c->d_ev.as<char>();
+  EvBufs B{reinterpret_cast<mmp_evict_entry *>(base + o_ent), c->d_jslot.as<int>(), reinterpret_cast<mmp_decision_in *>(base + o_dec),
+           reinterpret_cast<mmp_decision_out *>(base + o_res), reinterpret_cast<EvHdr *>(base + o_hdr),
+           reinterpret_cast<mmp_evict_action *>(base + o_out), nullptr};
+  c->fresh_host.assign(fresh_self ? 1 : 0, fr);
+  if ((rc = stage_side_tables(c.get(), c->fresh_host.data(), fresh_self ? 1 : 0, nullptr, 0, st)) < 0) return rc;
+  B.extra = c->d_extra.as<int32_t>();
+  CK(cudaMemsetAsync(B.hdr, 0, sizeof(EvHdr), st));
+  if (n) CK(cudaMemcpyAsync(const_cast<mmp_evict_entry *>(B.entries), entries, (size_t)n * sizeof(mmp_evict_entry), cudaMemcpyHostToDevice, st));
+  const int64_t now = p->now;
+  const long long reload_age = (long long)(2u * (uint64_t)p->load_timeout_ms);
+  const long long fail_since = (long long)((uint64_t)now - (uint64_t)(p->load_failure_expiry_ms / 2));
+  CK(cudaEventRecord(c->e0, st));
+  if (n) {
+    TypeSetStats S;
+    if ((rc = queue_type_stats(f, c.get(), ds, lv, S, st)) < 0) return rc;
+    k_evict_plan<<<(n + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.model_lul.as<long long>(),
+                                                  ds.rank_of.as<int32_t>(), S.types, lv.n_type_ids, B, n, self, now, reload_age, fail_since,
+                                                  fresh_self ? 0 : -1);
+    SnapshotView vw = ds.view;
+    vw.n_extra = 1;
+    PlaceArgs a{vw, B.dec, n, c->d_fresh.as<FreshRow>(), fresh_self ? 1 : 0, B.extra, const_cast<mmp_decision_out *>(B.res), nullptr,
+                nullptr, now, seed, f->id_base.load()};
+    a.ctx = c.get();
+    CK(launch_place(f, a, st));
+    k_evict_pack<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+    f->launches += 2;
+    CK(cudaGetLastError());
+  }
+  CK(cudaEventRecord(c->e1, st));
+  std::vector<char> back(sizeof(EvHdr) + (size_t)n * sizeof(mmp_evict_action));
+  CK(cudaMemcpyAsync(back.data(), B.hdr, back.size(), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_evict_ms = ms; }
+  EvHdr H;
+  memcpy(&H, back.data(), sizeof(EvHdr));
+  if (H.dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
+  if (n) memcpy(out, back.data() + sizeof(EvHdr), (size_t)n * sizeof(mmp_evict_action));
   *report = H.rep;
   return n;
 }

@@ -13,9 +13,10 @@ import numpy as np
 
 from . import _lib
 from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CHURN_REAPER, CLUSTER_STATS, DECISION_IN, DECISION_OUT,
-                   DECISION_TRACE, EVICTION, INSTANCE_ROW, JANITOR_EDIT, JANITOR_ENTRY, JANITOR_PARAMS, LRU_ENTRY, LRU_EVENT, MODEL_ROW,
-                   RATE_LOAD, RATE_PARAMS, REAPER_LOAD, SCALE_IN, SCALE_OUT, SHUTDOWN_ACTION, SHUTDOWN_ENTRY, SHUTDOWN_PARAMS,
-                   ChurnConfig, ChurnReport, JanitorReport, MmpConfig, RateReport, ReaperReport, ShutdownReport)
+                   DECISION_TRACE, EVICT_ACTION, EVICT_ENTRY, EVICT_PARAMS, EVICTION, INSTANCE_ROW, JANITOR_EDIT, JANITOR_ENTRY,
+                   JANITOR_PARAMS, LRU_ENTRY, LRU_EVENT, MODEL_ROW, RATE_LOAD, RATE_PARAMS, REAPER_LOAD, SCALE_IN, SCALE_OUT,
+                   SHUTDOWN_ACTION, SHUTDOWN_ENTRY, SHUTDOWN_PARAMS, ChurnConfig, ChurnReport, EvictReport, JanitorReport, MmpConfig,
+                   RateReport, ReaperReport, ShutdownReport)
 
 
 class MmpError(RuntimeError):
@@ -407,6 +408,22 @@ class Fleet:
         r = ShutdownReport()
         self._ck(self.lib.mmp_shutdown_run(self.h, self_idx, _ptr(entries), len(entries), _ptr(params), _ptr(fr), seed, _ptr(out),
                                            C.byref(r)))
+        return out, r
+
+    def evict_run(self, self_idx: int, entries: np.ndarray, params: np.ndarray, seed: int, fresh_self: Optional[np.ndarray] = None,
+                  out: Optional[np.ndarray] = None):
+        """mmp_evict_run, one pod's eviction listener over a burst of evictions: (out (EVICT_ACTION per entry, entry order),
+        report).  entries: EVICT_ENTRY records in listener order; params: one EVICT_PARAMS record; fresh_self: the pod's own
+        INSTANCE_ROW or None.  out: a caller-allocated EVICT_ACTION array of len(entries) to write into (one is allocated when
+        None); a caller that runs the call often allocates it once."""
+        assert entries.dtype == EVICT_ENTRY and params.dtype == EVICT_PARAMS and entries.flags.c_contiguous
+        if out is None:
+            out = np.zeros(len(entries), dtype=EVICT_ACTION)
+        assert out.dtype == EVICT_ACTION and len(out) == len(entries) and out.flags.c_contiguous
+        fr = None if fresh_self is None else np.ascontiguousarray(fresh_self, dtype=INSTANCE_ROW).reshape(1)
+        r = EvictReport()
+        self._ck(self.lib.mmp_evict_run(self.h, self_idx, _ptr(entries), len(entries), _ptr(params), _ptr(fr), seed, _ptr(out),
+                                        C.byref(r)))
         return out, r
 
     def commit_info(self):
