@@ -231,6 +231,8 @@ int32_t mmp_place_submit(mmp_batcher *, const mmp_decision_in *in, const mmp_ins
                          mmp_decision_out *out, uint32_t *decision_id);
 int32_t mmp_batcher_stats(mmp_batcher *, int64_t *batches, int64_t *decisions);
 /* Single decision (latency path, B = 1). */
+#define MMP_SERVER_SLOTS 8  /* concurrent callers the resident server (one_mode 3) answers without a launch: one slot and one
+                               warp of k_place_server each; a call that finds every slot taken takes the graph path */
 int32_t mmp_place_one(mmp_fleet *, const mmp_decision_in *in, const mmp_instance_row *fresh, const int32_t *extra,
                       mmp_decision_out *out, int64_t now_ms, uint64_t seed);
 /* Device-resident variant used to time the kernel alone: d_in/d_out are device pointers obtained from
@@ -801,7 +803,8 @@ int32_t mmp_evict_run(mmp_fleet *, int32_t self, const mmp_evict_entry *entries,
  *   "one_mode"        how a batch of <= 32 decisions is launched: 0 the batch kernel ("direct" below), 1 the latency kernel
  *                     k_place_small as a stream launch, 2 k_place_small as a replayed CUDA graph, 3 (default) a request to the
  *                     resident server kernel k_place_server (no launch per call: the host posts the request into mapped memory
- *                     and spins on the answer; one caller at a time, concurrent callers take the graph path)
+ *                     and spins on the answer; up to MMP_SERVER_SLOTS concurrent callers each have a slot of their own,
+ *                     a caller that finds every slot taken takes the graph path -- see mmp_server_stats)
  *   "server_life_us"  longest residence of one k_place_server launch (default 2000): bounds how long a device-wide wait
  *                     (cudaFree inside a commit) can be held up; "server_idle_us" (default 300): it leaves earlier when idle
  *   "direct"          1 (default): batches are resolved by k_place_direct (rows read straight from memory); 0: by the streaming
@@ -823,6 +826,10 @@ int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
  * (numeric instance updates / model-record deltas only: scattered into the device-resident tables, re-ranked and rebuilt
  * there); and its duration on the host clock */
 int32_t mmp_commit_info(mmp_fleet *, int32_t *path, double *ms);
+/* the resident server (one_mode 3) since mmp_fleet_create: out4[0] requests it answered, out4[1] calls that found all
+ * MMP_SERVER_SLOTS slots taken and took the graph path, out4[2] launches of k_place_server, out4[3] the most slots busy at
+ * once.  Its answers equal the graph path's by design: these counts are how a caller sees which path answered */
+int32_t mmp_server_stats(mmp_fleet *, int64_t *out4);
 
 #ifdef __cplusplus
 }

@@ -173,6 +173,14 @@ public final class GpuPlacement implements AutoCloseable {
         return check(MmPlace.evictRun(h, self, entries, n, params, freshSelf, pickSeed.incrementAndGet(), out, report));
     }
 
+    // for the pod's metrics: {requests the resident placement server answered, calls that found all its slots taken and took
+    // the graph path, its launches, the most slots busy at once}, since this placement was created
+    public long[] serverStats() {
+        long[] out = new long[4];
+        check(MmPlace.serverStats(h, out));
+        return out;
+    }
+
     private int check(int rc) { if (rc < 0) throw new IllegalStateException(MmPlace.lastError(h)); return rc; }
     @Override public void close() { committer.shutdownNow(); MmPlace.destroy(h); }
 }

@@ -63,6 +63,8 @@ final class MmPlace {
                                ByteBuffer out, ByteBuffer report);
     static native int tune(long h, String key, long value);
     static native double lastTiming(long h, String key);
+    // the resident placement server (one_mode 3): out[0..3] = requests answered, graph-path fallbacks, launches, most slots busy
+    static native int serverStats(long h, long[] out);
     // plug point 1: placement (CacheMissForwardingLB.getNext MM:4776-5004)
     static native int placeBatch(long h, ByteBuffer in, int n, ByteBuffer fresh, int nFresh, ByteBuffer extra, int nExtra, ByteBuffer out,
                                  long nowMs, long seed);

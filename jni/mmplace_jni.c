@@ -212,6 +212,18 @@ jdouble FN(commitInfo)(JNIEnv *env, jclass c, jlong h, jintArray pathOut) {
   return ms;
 }
 
+/* out[0..3] = the resident server's requests answered, graph-path fallbacks, launches, most slots busy at once */
+jint FN(serverStats)(JNIEnv *env, jclass c, jlong h, jlongArray out) {
+  int64_t v[4] = {0, 0, 0, 0};
+  jint rc = mmp_server_stats(H(h), v);
+  (void)c;
+  if (rc >= 0 && out) {
+    jlong j[4] = {v[0], v[1], v[2], v[3]};
+    (*env)->SetLongArrayRegion(env, out, 0, 4, j);
+  }
+  return rc;
+}
+
 /* ---- plug point 1: placement ---- */
 jint FN(placeBatch)(JNIEnv *env, jclass c, jlong h, jobject in, jint n, jobject fresh, jint nFresh, jobject extra, jint nExtra, jobject out,
                     jlong nowMs, jlong seed) {

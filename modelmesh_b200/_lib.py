@@ -205,6 +205,7 @@ SYMBOLS = [
     ("mmp_churn_model", _I32, [_P, _I32, _P, _P]),
     ("mmp_churn_model_ids", _I32, [_P, _I32, _P, _P, _I32]),
     ("mmp_commit_info", _I32, [_P, C.POINTER(_I32), C.POINTER(C.c_double)]),
+    ("mmp_server_stats", _I32, [_P, _P]),
     ("mmp_model_times", _I32, [_P, _I32, _P, _I32, _I64]),
     ("mmp_scale_eval", _I32, [_P, _P, _I32, _P, _P]),
     ("mmp_registry_prune", _I32, [_P, _I32, _I64, _I64, _P, _P, _P, _I32]),

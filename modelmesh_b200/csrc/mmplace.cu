@@ -601,10 +601,10 @@ __global__ void __launch_bounds__(LANE_WARPS * 32, 1) k_place_lanes(const Snapsh
 struct SmallHdr { long long now; unsigned long long seed, id_base; int n, n_fresh, n_extra, stop; unsigned long long seq; unsigned long long pad[2]; };
 static_assert(sizeof(SmallHdr) == 64, "header is one 64-byte line");
 // one block of 32 threads resolves decisions [blk * 32, blk * 32 + 32) of a small batch
+// (lane: the thread's lane; ctx_one and chunk_b: the warp's own shared memory)
 __device__ __forceinline__ void place_small_block(const SnapshotView &s, const mmp_decision_in *in, int n, const FreshRow *fresh, int n_fresh,
                                                   const int32_t *extra, mmp_decision_out *out, int64_t now, uint64_t seed, uint64_t id_base,
-                                                  int budget, int blk, DecisionCtx *ctx_one) {
-  const int lane = threadIdx.x;
+                                                  int budget, int blk, DecisionCtx *ctx_one, int lane, uint32_t *chunk_b) {
   const int i = blk * 32 + lane;
   const bool valid = i < n;
   mmp_decision_in d = no_decision();
@@ -618,7 +618,6 @@ __device__ __forceinline__ void place_small_block(const SnapshotView &s, const m
   if (valid && c.self_rank >= 0) self_eword = __ldg(row + (c.self_rank >> 5));
   DecideOut o;
   const uint64_t my_id = pick_id(d, id_base + (uint64_t)i);
-  __shared__ uint32_t chunk_b[32 * MMP_CHUNK_WORDS];  // (callers are one-warp blocks)
   const bool handled = decide_stream<TabGlob>(s, T, T, c, valid, nullptr, 0u, RowPtr{row, (uint32_t)s.word_lo}, self_eword,
                                               now, seed, my_id, WarpVote(), o, budget, chunk_b + lane * MMP_CHUNK_WORDS);
   redo_declined(__ballot_sync(0xffffffffu, valid && !handled), lane, c, m, my_id, ctx_one, s, extra, now, seed, o);
@@ -629,10 +628,11 @@ __global__ void __launch_bounds__(32) k_place_small(const SnapshotView s_arg, co
                                                     mmp_decision_out *__restrict__ out, int64_t now_arg, uint64_t seed_arg, uint64_t id_base_arg,
                                                     const volatile SmallHdr *hdr, int budget) {
   __shared__ DecisionCtx ctx_one;
+  __shared__ uint32_t chunk_b[32 * MMP_CHUNK_WORDS];
   SnapshotView s = s_arg;
   if (hdr) s.n_extra = hdr->n_extra;
   place_small_block(s, in, hdr ? hdr->n : n_arg, fresh, hdr ? hdr->n_fresh : n_fresh_arg, extra, out, hdr ? hdr->now : now_arg,
-                    hdr ? hdr->seed : seed_arg, hdr ? hdr->id_base : id_base_arg, budget, blockIdx.x, &ctx_one);
+                    hdr ? hdr->seed : seed_arg, hdr ? hdr->id_base : id_base_arg, budget, blockIdx.x, &ctx_one, threadIdx.x, chunk_b);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -832,10 +832,11 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_tail(const SnapshotV
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// k_place_server -- the B = 1 path without a launch per call.  One warp stays resident for a BOUNDED time (life_ns, or
-// idle_ns without a request), polling the sequence word of a request header in pinned mapped host memory; a request (up to
-// 32 decisions, laid out like the graph path's buffer) is resolved with the same routine as k_place_small and answered by
-// a release store of the sequence number into the response line.  The host posts a request with one store and spins on
+// k_place_server -- the B = 1 path without a launch per call, for up to MMP_SERVER_SLOTS concurrent callers.  One block of
+// MMP_SERVER_SLOTS warps stays resident for a BOUNDED time (life_ns, or idle_ns in which no slot received a request); warp w
+// serves slot w, polling the sequence word of the slot's request header in pinned mapped host memory.  A request (up to 32
+// decisions, laid out like the graph path's buffer) is resolved with the same routine as k_place_small and answered by a
+// release store of the sequence number into the slot's response line.  The host posts a request with one store and spins on
 // the response: two PCIe round trips instead of launch + synchronise.  Bounded lifetime: anything that waits for the
 // device to drain (cudaFree inside a commit) waits at most life_ns, and a crashed host leaves no kernel behind.
 // ---------------------------------------------------------------------------------------------------------------
@@ -847,24 +848,42 @@ struct SrvLine0 { unsigned long long seq; long long now; unsigned long long seed
 struct SrvLine1 { int n, n_fresh, n_extra, pad; FreshRow fr; int32_t extra[SRV_INLINE_EXTRA]; unsigned long long pad2; };
 struct ServerResp { unsigned long long done_seq; int alive, served; mmp_decision_out out0; unsigned long long pad[5]; };
 static_assert(sizeof(SrvLine0) == 64 && sizeof(SrvLine1) == 64 && sizeof(ServerResp) == 64, "one line each");
-__global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, volatile SrvLine0 *l0, volatile SrvLine1 *l1, volatile ServerResp *resp,
-                                                     const mmp_decision_in *in_tab, const FreshRow *fresh_tab, const int32_t *extra,
-                                                     mmp_decision_out *out_tab, unsigned long long life_ns, unsigned long long idle_ns, int budget) {
-  __shared__ DecisionCtx ctx_one;
-  __shared__ __align__(16) uint32_t line_s[16];
-  __shared__ __align__(16) uint32_t line1_s[16];  // kind 1's line 1: fresh row and inline extras (extra[] of the decision)
-  __shared__ FreshRow fresh_s;
-  __shared__ uint32_t win_s[32 * LANE_STRIDE];
-  __shared__ uint32_t chunk_v[32 * MMP_CHUNK_WORDS];
+// one slot of the mapped buffer: [line 0][line 1][32 decisions][32 results][32 fresh rows][32 x MMP_MAX_EXTRA extras] ... [response line]
+struct SrvSlot {
+  static constexpr size_t BYTES = 16384, IN = 128, OUT = IN + 32 * sizeof(mmp_decision_in), FR = OUT + 32 * sizeof(mmp_decision_out),
+                          EX = FR + 32 * sizeof(FreshRow), RESP = BYTES - 64;
+};
+static_assert(SrvSlot::EX + 32 * MMP_MAX_EXTRA * 4 <= SrvSlot::RESP, "mapped layout");
+// a warp's own part of the server's shared memory (dynamic: with the WinTabs it is above the 48 KB static limit)
+struct __align__(16) SrvWarp {
+  DecisionCtx ctx_one;
+  __align__(16) uint32_t line_s[16];
+  __align__(16) uint32_t line1_s[16];  // kind 1's line 1: fresh row and inline extras (extra[] of the decision)
+  FreshRow fresh_s;
+  uint32_t win_s[32 * LANE_STRIDE];
+  uint32_t chunk_v[32 * MMP_CHUNK_WORDS];
+};
+__global__ void __launch_bounds__(MMP_SERVER_SLOTS * 32, 1) k_place_server(const SnapshotView s_arg, unsigned char *slots, unsigned long long life_ns,
+                                                                          unsigned long long idle_ns, int budget) {
+  extern __shared__ __align__(16) unsigned char srv_smem[];
   // the window part of the lane tables, as in k_place_lanes: the in-window steps of a decision read shared memory only
   __shared__ WinTabs tabs;
-  const int lane = threadIdx.x;
+  __shared__ unsigned long long last_act;  // globaltimer of the last request any slot received or answered
+  __shared__ int leave;                    // set by the first warp to leave: the others follow once their request is answered
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  SrvWarp &sw = reinterpret_cast<SrvWarp *>(srv_smem)[warp];
+  unsigned char *slot = slots + (size_t)warp * SrvSlot::BYTES;
+  volatile SrvLine0 *l0 = reinterpret_cast<volatile SrvLine0 *>(slot);
+  volatile SrvLine1 *l1 = reinterpret_cast<volatile SrvLine1 *>(slot + 64);
+  volatile ServerResp *resp = reinterpret_cast<volatile ServerResp *>(slot + SrvSlot::RESP);
   const uint32_t win_words = (uint32_t)min(LANE_WIN, s_arg.word_hi - s_arg.word_lo);
-  tabs.fill(s_arg, lane, 32);
-  __syncwarp();
+  tabs.fill(s_arg, threadIdx.x, MMP_SERVER_SLOTS * 32);
   unsigned long long t0, t_last, t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  t_last = t0;
+  if (threadIdx.x == 0) { last_act = t0; leave = 0; }
+  __syncthreads();
+  volatile unsigned long long *act = &last_act;
+  volatile int *go = &leave;
   unsigned long long last = resp->done_seq;
   int served = 0;
   for (;;) {
@@ -872,15 +891,18 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
     uint32_t v = 0;
     if (lane < 16) v = reinterpret_cast<volatile uint32_t *>(l0)[lane];
     const unsigned long long seq = (unsigned long long)__shfl_sync(0xffffffffu, v, 0) | ((unsigned long long)__shfl_sync(0xffffffffu, v, 1) << 32);
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     if (seq == last) {
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      if (t - t0 > life_ns || t - t_last > idle_ns) break;
+      // (signed: another warp may have stored a later activity time than this warp's clock reading)
+      if (__shfl_sync(0xffffffffu, (int)(*go || t - t0 > life_ns || (long long)(t - *act) > (long long)idle_ns), 0)) break;
       continue;
     }
     const unsigned kind = (unsigned)(seq >> 56);
     if (kind == 0xffu) break;
-    if (lane < 16) line_s[lane] = v;
+    if (lane == 0) *act = t;
+    if (lane < 16) sw.line_s[lane] = v;
     __syncwarp();
+    const uint32_t *line_s = sw.line_s, *line1_s = sw.line1_s;
     const long long now = (long long)((unsigned long long)line_s[2] | ((unsigned long long)line_s[3] << 32));
     const unsigned long long seed = (unsigned long long)line_s[4] | ((unsigned long long)line_s[5] << 32);
     const unsigned long long id_base = (unsigned long long)line_s[6] | ((unsigned long long)line_s[7] << 32);
@@ -895,11 +917,11 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
       // the decision's extra[] is line 1's inline part (extra_off = 0, at most SRV_INLINE_EXTRA entries: place_server)
       const int32_t *extra1 = reinterpret_cast<const int32_t *>(line1_s + offsetof(SrvLine1, extra) / 4);
       if (__shfl_sync(0xffffffffu, d.fresh, 0) >= 0 || __shfl_sync(0xffffffffu, d.extra_n, 0) > 0) {  // side tables: a second read, one line
-        if (lane < 16) line1_s[lane] = reinterpret_cast<volatile uint32_t *>(l1)[lane];
+        if (lane < 16) sw.line1_s[lane] = reinterpret_cast<volatile uint32_t *>(l1)[lane];
         __syncwarp();
         n_fresh = (int)line1_s[offsetof(SrvLine1, n_fresh) / 4];
         s.n_extra = (int)line1_s[offsetof(SrvLine1, n_extra) / 4];
-        if (lane == 0) fresh_s = *reinterpret_cast<const FreshRow *>(line1_s + offsetof(SrvLine1, fr) / 4);
+        if (lane == 0) sw.fresh_s = *reinterpret_cast<const FreshRow *>(line1_s + offsetof(SrvLine1, fr) / 4);
         __syncwarp();
       }
       const int m = excl_row_id(s, d.model, d.flags);
@@ -911,22 +933,22 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
         if (valid && (uint32_t)(j * 4) < win_words) q[j] = __ldg(reinterpret_cast<const uint4 *>(row) + j);
       }
       DecisionCtx c = no_ctx();
-      if (valid) prepare_ctx(s, d, &fresh_s, min(n_fresh, 1), extra1, c);
+      if (valid) prepare_ctx(s, d, &sw.fresh_s, min(n_fresh, 1), extra1, c);
       uint32_t self_eword = 0;
       if (valid && c.self_rank >= 0) self_eword = __ldg(row + (c.self_rank >> 5) - s.word_lo);
-      uint32_t *w = win_s + lane * LANE_STRIDE;
+      uint32_t *w = sw.win_s + lane * LANE_STRIDE;
 #pragma unroll
       for (int j = 0; j < LANE_WIN / 4; j++) { w[j * 4] = q[j].x; w[j * 4 + 1] = q[j].y; w[j * 4 + 2] = q[j].z; w[j * 4 + 3] = q[j].w; }
       __syncwarp();
-      const int slot = c.slot >= 0 ? ctx_slot(c) : 0;
-      const LaneTables T = lane_tables_global(s, slot);
-      const LaneTables Tw = tabs.view(T, slot, s.word_lo);
+      const int slot_t = c.slot >= 0 ? ctx_slot(c) : 0;
+      const LaneTables T = lane_tables_global(s, slot_t);
+      const LaneTables Tw = tabs.view(T, slot_t, s.word_lo);
       DecideOut o;
       const uint64_t my_id = pick_id(d, id_base);
       const bool handled = decide_stream(s, Tw, T, c, valid, w, win_words, RowPtr{row, (uint32_t)s.word_lo}, self_eword, now, seed, my_id, WarpVote(), o, budget,
-                                         chunk_v + lane * MMP_CHUNK_WORDS);
+                                         sw.chunk_v + lane * MMP_CHUNK_WORDS);
       // pending: lane 0, the only lane with a decision, if it declined
-      redo_declined(__shfl_sync(0xffffffffu, (uint32_t)!handled, 0), lane, c, m, my_id, &ctx_one, s, extra1, now, seed, o);
+      redo_declined(__shfl_sync(0xffffffffu, (uint32_t)!handled, 0), lane, c, m, my_id, &sw.ctx_one, s, extra1, now, seed, o);
       if (lane == 0) { resp->out0.target = o.target; resp->out0.n_candidates = o.n_candidates; }
     } else {
       // ---- a batch of up to 32 through the mapped tables (sizes in line 1) ----
@@ -934,7 +956,9 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
       if (lane == 0) { n = l1->n; n_fresh = l1->n_fresh; n_extra = l1->n_extra; }
       n = __shfl_sync(0xffffffffu, n, 0); n_fresh = __shfl_sync(0xffffffffu, n_fresh, 0); n_extra = __shfl_sync(0xffffffffu, n_extra, 0);
       s.n_extra = n_extra;
-      place_small_block(s, in_tab, n, fresh_tab, n_fresh, extra, out_tab, now, seed, id_base, budget, 0, &ctx_one);
+      place_small_block(s, reinterpret_cast<const mmp_decision_in *>(slot + SrvSlot::IN), n, reinterpret_cast<const FreshRow *>(slot + SrvSlot::FR),
+                        n_fresh, reinterpret_cast<const int32_t *>(slot + SrvSlot::EX), reinterpret_cast<mmp_decision_out *>(slot + SrvSlot::OUT),
+                        now, seed, id_base, budget, 0, &sw.ctx_one, lane, sw.chunk_v);
     }
     __threadfence_system();
     __syncwarp();
@@ -942,8 +966,12 @@ __global__ void __launch_bounds__(32) k_place_server(const SnapshotView s_arg, v
     last = seq;
     served++;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_last));
-    if (t_last - t0 > life_ns) break;  // (a busy server leaves too: the host restarts it with its next request)
+    if (lane == 0) *act = t_last;
+    // (a busy server leaves too: the host restarts it with its next request)
+    if (__shfl_sync(0xffffffffu, (int)(*go || t_last - t0 > life_ns), 0)) break;
   }
+  if (lane == 0) *go = 1;
+  __syncthreads();  // every warp has answered its last request: the block leaves as one
   if (lane == 0) {
     resp->served = served;
     __threadfence_system();
@@ -1320,15 +1348,21 @@ struct mmp_fleet {
   std::atomic<int64_t> launches{0};
   int one_mode = 3;             // MMP_ONE = lanes | small | graph | server: how tiny batches are launched (0: launch_place, 1: k_place_small
                                 // as a stream launch, 2: k_place_small as a replayed CUDA graph, 3: a request to the resident k_place_server)
-  // the resident B = 1 server (one_mode 3, k_place_server)
+  // the resident B = 1 server (one_mode 3, k_place_server): MMP_SERVER_SLOTS slots, one request each at a time; a caller
+  // that finds every slot taken uses the graph path
   struct Server {
-    std::mutex mu;                 // one request at a time; a caller that finds it taken uses the graph path
-    PinnedBuf mapped;
+    struct Slot {
+      std::mutex mu;
+      uint64_t seq = 0;
+    } slot[MMP_SERVER_SLOTS];
+    std::mutex launch_mu;                // launch and stop of the block; epoch and the stream's work change under it
+    PinnedBuf mapped;                    // MMP_SERVER_SLOTS x SrvSlot::BYTES
+    unsigned char *dmapped = nullptr;
     Stream stream;
-    int32_t epoch = -1;
-    bool running = false;
-    uint64_t seq = 0;
-    int64_t launches = 0, requests = 0;
+    std::atomic<int32_t> epoch{-1};      // the running block's epoch, -1 when none runs (stopped, or never launched)
+    std::atomic<uint64_t> gen{0};        // launches so far: a caller relaunches a block it saw leave only if none came after it
+    std::atomic<int64_t> launches{0}, requests{0}, fallbacks{0};
+    std::atomic<int32_t> busy{0}, max_busy{0};
     int64_t life_us = 2000, idle_us = 300;
   } srv;
   int sort_slots = 2;           // MMP_SORT_SLOTS = 0 never | 1 always | 2 (default) when the snapshot's candidate sets are sparse: k_place_direct
@@ -1752,7 +1786,7 @@ static int32_t place_chunks(mmp_fleet *f, PlaceCtx *c, const PlaceArgs &a, int32
 // ---------------------------------------------------------------------------------------------------------------
 extern "C" {
 
-static void server_stop(mmp_fleet *f);
+static void server_stop(mmp_fleet *f, int k);
 
 int32_t mmp_shard_unique_id(void *id128) {
   if (!id128) { g_err = "null argument"; return MMP_E_ARG; }
@@ -1942,7 +1976,10 @@ int32_t mmp_fleet_create(const mmp_config *cfg, mmp_fleet **out) {
 void mmp_fleet_destroy(mmp_fleet *f) {
   if (!f) return;
   cudaSetDevice(f->device);
-  { std::lock_guard<std::mutex> lk(f->srv.mu); server_stop(f); }
+  {
+    std::lock_guard<std::mutex> slot(f->srv.slot[0].mu), lk(f->srv.launch_mu);
+    server_stop(f, 0);
+  }
   cudaDeviceSynchronize();
   if (f->comm && nccl_api().ok) { nccl_api().CommDestroy(f->comm); f->comm = nullptr; }
   delete f;  // (its members free the device buffers, streams, events, graphs, pinned buffers and IPC mappings they own)
@@ -2346,6 +2383,14 @@ int32_t mmp_last_timing(mmp_fleet *f, const char *key, double *ms) {
   else { g_err = "unknown key"; return MMP_E_ARG; }
   return MMP_OK;
 }
+/* the resident server since fleet creation: requests answered, calls that took the graph path because every slot was
+ * taken, launches, the most slots busy at once */
+int32_t mmp_server_stats(mmp_fleet *f, int64_t *out4) {
+  NEED(f);
+  if (!out4) { g_err = "null argument"; return MMP_E_ARG; }
+  out4[0] = f->srv.requests.load(); out4[1] = f->srv.fallbacks.load(); out4[2] = f->srv.launches.load(); out4[3] = f->srv.max_busy.load();
+  return MMP_OK;
+}
 /* which path the last commit took (1 = structural / host, 2 = device) and how long it took on the host clock */
 int32_t mmp_commit_info(mmp_fleet *f, int32_t *path, double *ms) {
   NEED(f);
@@ -2354,35 +2399,62 @@ int32_t mmp_commit_info(mmp_fleet *f, int32_t *path, double *ms) {
   return MMP_OK;
 }
 
-// ---- the resident B = 1 server (k_place_server): post a request of up to 32 decisions, spin on the response ----
-static void server_stop(mmp_fleet *f) {
+// ---- the resident B = 1 server (k_place_server): post a request of up to 32 decisions into a slot, spin on the response ----
+static unsigned char *server_slot(mmp_fleet *f, int k) { return f->srv.mapped.get() + (size_t)k * SrvSlot::BYTES; }
+// Stop the block through slot k (its caller holds the slot and launch_mu): a "leave" request, then wait for the block.
+static void server_stop(mmp_fleet *f, int k) {
   mmp_fleet::Server &sv = f->srv;
-  if (!sv.mapped || !sv.running) return;
-  volatile SrvLine0 *l0 = reinterpret_cast<volatile SrvLine0 *>(sv.mapped.get());
-  sv.seq++;
-  l0->seq = (sv.seq & 0x00ffffffffffffffull) | (0xffull << 56);  // kind 0xff: leave
+  if (!sv.mapped || sv.epoch.load() < 0) return;
+  volatile SrvLine0 *l0 = reinterpret_cast<volatile SrvLine0 *>(server_slot(f, k));
+  volatile ServerResp *resp = reinterpret_cast<volatile ServerResp *>(server_slot(f, k) + SrvSlot::RESP);
+  sv.slot[k].seq++;
+  l0->seq = (sv.slot[k].seq & 0x00ffffffffffffffull) | (0xffull << 56);  // kind 0xff: leave
   std::atomic_thread_fence(std::memory_order_seq_cst);
   cudaStreamSynchronize(sv.stream);
-  sv.running = false;
+  l0->seq = resp->done_seq;  // (the "leave" is not for the next block)
+  sv.epoch.store(-1);
 }
-// mapped buffer: [line 0][line 1][32 decisions][32 results][32 fresh rows][32 x MMP_MAX_EXTRA extras] ... [response line]
-static int32_t place_server(mmp_fleet *f, const DeviceSnapshot &ds, const mmp_decision_in *in, int32_t n, const FreshRow *fresh, int32_t n_fresh,
-                            const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed) {
+// Launch a block on the current epoch's view (launch_mu held).  The previous block has left or is leaving: wait for it, so
+// that its last stores into the response lines land before this launch marks every slot alive.
+static int32_t server_launch(mmp_fleet *f, const DeviceSnapshot &ds) {
   mmp_fleet::Server &sv = f->srv;
+  const size_t smem = sizeof(SrvWarp) * MMP_SERVER_SLOTS;
   if (!sv.mapped) {
-    CK(cudaHostAlloc((void **)sv.mapped.put(), PlaceCtx::MAPPED_BYTES, cudaHostAllocMapped));
-    memset(sv.mapped, 0, PlaceCtx::MAPPED_BYTES);
+    CK(cudaHostAlloc((void **)sv.mapped.put(), SrvSlot::BYTES * MMP_SERVER_SLOTS, cudaHostAllocMapped));
+    memset(sv.mapped, 0, SrvSlot::BYTES * MMP_SERVER_SLOTS);
+    CK(cudaHostGetDevicePointer((void **)&sv.dmapped, sv.mapped.get(), 0));
     CK(cudaStreamCreateWithFlags(sv.stream.put(), cudaStreamNonBlocking));
+    CK(cudaFuncSetAttribute(k_place_server, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
-  unsigned char *h = sv.mapped, *dbase = nullptr;
-  CK(cudaHostGetDevicePointer((void **)&dbase, h, 0));
-  const size_t g_in = 128, g_out = g_in + 32 * sizeof(mmp_decision_in), g_fr = g_out + 32 * sizeof(mmp_decision_out), g_ex = g_fr + 32 * sizeof(FreshRow),
-               g_resp = PlaceCtx::MAPPED_BYTES - 64;
-  static_assert(128 + 32 * (sizeof(mmp_decision_in) + sizeof(mmp_decision_out) + sizeof(FreshRow)) + 32 * MMP_MAX_EXTRA * 4 + 64 <= PlaceCtx::MAPPED_BYTES, "mapped layout");
+  CK(cudaStreamSynchronize(sv.stream));
+  for (int k = 0; k < MMP_SERVER_SLOTS; k++) reinterpret_cast<volatile ServerResp *>(server_slot(f, k) + SrvSlot::RESP)->alive = 1;
+  std::atomic_thread_fence(std::memory_order_seq_cst);
+  k_place_server<<<1, MMP_SERVER_SLOTS * 32, smem, sv.stream>>>(ds.view, sv.dmapped, (unsigned long long)sv.life_us * 1000ull,
+                                                              (unsigned long long)sv.idle_us * 1000ull, f->lane_budget);
+  CK(cudaGetLastError());
+  sv.epoch.store(f->epoch);
+  sv.gen++; sv.launches++; f->launches++;
+  return MMP_OK;
+}
+// One request through slot k, whose mutex the caller holds.
+static int32_t place_server(mmp_fleet *f, int k, const DeviceSnapshot &ds, const mmp_decision_in *in, int32_t n, const FreshRow *fresh,
+                            int32_t n_fresh, const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed) {
+  mmp_fleet::Server &sv = f->srv;
+  // a block on this epoch's view must be running before the request is posted; one on another epoch's view is stopped
+  // (no caller of that epoch is still in flight: the commit that ended it waited for them)
+  if (sv.epoch.load() != f->epoch ||
+      reinterpret_cast<volatile ServerResp *>(server_slot(f, k) + SrvSlot::RESP)->alive == 0) {
+    std::lock_guard<std::mutex> lk(sv.launch_mu);
+    if (sv.epoch.load() >= 0 && sv.epoch.load() != f->epoch) server_stop(f, k);
+    if (sv.epoch.load() < 0 || reinterpret_cast<volatile ServerResp *>(server_slot(f, k) + SrvSlot::RESP)->alive == 0) {
+      int32_t rc = server_launch(f, ds);
+      if (rc < 0) return rc;
+    }
+  }
+  unsigned char *h = server_slot(f, k);
   volatile SrvLine0 *l0 = reinterpret_cast<volatile SrvLine0 *>(h);
   volatile SrvLine1 *l1 = reinterpret_cast<volatile SrvLine1 *>(h + 64);
-  volatile ServerResp *resp = reinterpret_cast<volatile ServerResp *>(h + g_resp);
-  if (sv.running && sv.epoch != f->epoch) server_stop(f);  // its snapshot view is another epoch's
+  volatile ServerResp *resp = reinterpret_cast<volatile ServerResp *>(h + SrvSlot::RESP);
   // kind 1: one decision whose side tables are at most its own fresh row and a few extra excludes from the start of extra[]
   // (the shape of getNext on a request thread: a request-model decision carries its model's copies and failures there)
   const int32_t n_inline = n_extra == 0 ? 0 : in[0].extra_n;
@@ -2395,50 +2467,59 @@ static int32_t place_server(mmp_fleet *f, const DeviceSnapshot &ds, const mmp_de
     l1->n = 1; l1->n_fresh = n_fresh; l1->n_extra = n_inline;
     memcpy((void *)&l0->d, &d, sizeof(d));
   } else {
-    memcpy(h + g_in, in, (size_t)n * sizeof(mmp_decision_in));
-    if (n_fresh) memcpy(h + g_fr, fresh, (size_t)n_fresh * sizeof(FreshRow));
-    if (n_extra) memcpy(h + g_ex, extra, (size_t)n_extra * 4);
+    memcpy(h + SrvSlot::IN, in, (size_t)n * sizeof(mmp_decision_in));
+    if (n_fresh) memcpy(h + SrvSlot::FR, fresh, (size_t)n_fresh * sizeof(FreshRow));
+    if (n_extra) memcpy(h + SrvSlot::EX, extra, (size_t)n_extra * 4);
     l1->n = n; l1->n_fresh = n_fresh; l1->n_extra = n_extra;
   }
   l0->now = now_ms; l0->seed = seed; l0->id_base = f->id_base.load();
-  auto launch = [&]() -> int32_t {
-    if ((l0->seq >> 56) == 0xffull) l0->seq = resp->done_seq;  // (a "leave" left behind by server_stop is not for the new server)
-    resp->alive = 1;
-    std::atomic_thread_fence(std::memory_order_seq_cst);
-    k_place_server<<<1, 32, 0, sv.stream>>>(ds.view, reinterpret_cast<volatile SrvLine0 *>(dbase), reinterpret_cast<volatile SrvLine1 *>(dbase + 64),
-                                          reinterpret_cast<volatile ServerResp *>(dbase + g_resp), (const mmp_decision_in *)(dbase + g_in),
-                                          (const FreshRow *)(dbase + g_fr), (const int32_t *)(dbase + g_ex), (mmp_decision_out *)(dbase + g_out),
-                                          (unsigned long long)sv.life_us * 1000ull, (unsigned long long)sv.idle_us * 1000ull, f->lane_budget);
-    CK(cudaGetLastError());
-    sv.running = true; sv.epoch = f->epoch; sv.launches++; f->launches++;
-    return MMP_OK;
-  };
-  if (!sv.running || resp->alive == 0) { int32_t rc = launch(); if (rc < 0) return rc; }
-  sv.seq++;
-  const uint64_t seq = (sv.seq & 0x00ffffffffffffffull) | ((uint64_t)(single ? 1 : 2) << 56);
+  sv.slot[k].seq++;
+  const uint64_t seq = (sv.slot[k].seq & 0x00ffffffffffffffull) | ((uint64_t)(single ? 1 : 2) << 56);
   std::atomic_thread_fence(std::memory_order_seq_cst);
   l0->seq = seq;  // (the last store into line 0: a reader that sees it sees the request)
   std::atomic_thread_fence(std::memory_order_seq_cst);
   const auto t0 = std::chrono::steady_clock::now();
   for (uint32_t spins = 0;; spins++) {
     if (resp->done_seq == seq) break;
-    if (resp->alive == 0) {  // the server's lifetime ended -- before or after it saw this request?
-      CK(cudaStreamSynchronize(sv.stream));
-      if (resp->done_seq == seq) break;
-      int32_t rc = launch();
-      if (rc < 0) return rc;
+    const uint64_t g = sv.gen.load();
+    if (resp->alive == 0) {  // the block's lifetime ended -- before or after it saw this request?
+      std::lock_guard<std::mutex> lk(sv.launch_mu);
+      if (sv.gen.load() == g) {  // (else a later block was launched: it reads this slot's request when it starts)
+        CK(cudaStreamSynchronize(sv.stream));
+        if (resp->done_seq == seq) break;
+        int32_t rc = server_launch(f, ds);
+        if (rc < 0) return rc;
+      }
     }
     if ((spins & 0xfff) == 0xfff && std::chrono::steady_clock::now() - t0 > std::chrono::seconds(2)) {
-      server_stop(f);
+      std::lock_guard<std::mutex> lk(sv.launch_mu);
+      server_stop(f, k);
       g_err = "the placement server did not answer within 2 s";
       return MMP_E_CUDA;
     }
   }
   std::atomic_thread_fence(std::memory_order_seq_cst);
   if (single) { out[0].target = resp->out0.target; out[0].n_candidates = resp->out0.n_candidates; }
-  else memcpy(out, h + g_out, (size_t)n * sizeof(mmp_decision_out));
+  else memcpy(out, h + SrvSlot::OUT, (size_t)n * sizeof(mmp_decision_out));
   sv.requests++;
   return MMP_OK;
+}
+// A free slot for this call, trying the slots from the calling thread's own index on: its mutex locked, or false when every
+// slot is taken.
+static bool server_acquire(mmp_fleet *f, std::unique_lock<std::mutex> &lk, int &k) {
+  static std::atomic<int> threads{0};
+  thread_local const int first = threads.fetch_add(1) % MMP_SERVER_SLOTS;
+  mmp_fleet::Server &sv = f->srv;
+  for (int i = 0; i < MMP_SERVER_SLOTS; i++) {
+    k = (first + i) % MMP_SERVER_SLOTS;
+    lk = std::unique_lock<std::mutex>(sv.slot[k].mu, std::try_to_lock);
+    if (!lk.owns_lock()) continue;
+    const int32_t b = ++sv.busy;
+    for (int32_t m = sv.max_busy.load(); b > m && !sv.max_busy.compare_exchange_weak(m, b);) {}
+    return true;
+  }
+  sv.fallbacks++;
+  return false;
 }
 
 // Tiny untraced, unsharded batches, zero-copy: the records, fresh rows (c->fresh_host) and extras are written into the
@@ -2449,9 +2530,14 @@ static int32_t place_mapped(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds,
                             int32_t n, int32_t n_fresh, const int32_t *extra, int32_t n_extra, mmp_decision_out *out, int64_t now_ms, uint64_t seed) {
   const bool fits32 = n <= 32 && n_fresh <= 32 && (size_t)n_extra <= 32 * MMP_MAX_EXTRA && !derived;
   if (f->one_mode == 3 && fits32) {
-    std::unique_lock<std::mutex> lk(f->srv.mu, std::try_to_lock);
-    if (lk.owns_lock()) return place_server(f, ds, in, n, c->fresh_host.data(), n_fresh, extra, n_extra, out, now_ms, seed);
-  }  // (taken by another caller: this call goes the graph way)
+    std::unique_lock<std::mutex> lk;
+    int k;
+    if (server_acquire(f, lk, k)) {
+      const int32_t rc = place_server(f, k, ds, in, n, c->fresh_host.data(), n_fresh, extra, n_extra, out, now_ms, seed);
+      f->srv.busy--;
+      return rc;
+    }
+  }  // (every slot taken by other callers: this call goes the graph way)
   // one 32-thread block as a replayed graph: the node's parameters are those of the epoch it was captured in (the snapshot
   // view by value, the fixed offsets of a layout for 32 decisions behind a SmallHdr); what changes per call -- now, seed,
   // id base, n -- is read from the header.  Other launches take the batch packed from offset 0.

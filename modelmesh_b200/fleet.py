@@ -431,6 +431,14 @@ class Fleet:
         self._ck(self.lib.mmp_commit_info(self.h, C.byref(path), C.byref(ms)))
         return int(path.value), float(ms.value)
 
+    def server_stats(self):
+        """The resident server (one_mode 3) since the fleet was created: {"answered": requests it answered, "fallbacks": calls
+        that found every one of its MMP_SERVER_SLOTS slots taken and took the graph path, "launches": its launches,
+        "max_busy": the most slots busy at once}."""
+        out = np.zeros(4, dtype=np.int64)
+        self._ck(self.lib.mmp_server_stats(self.h, _ptr(out)))
+        return dict(zip(("answered", "fallbacks", "launches", "max_busy"), (int(v) for v in out)))
+
     def lru_state(self):
         n = self._lru_n
         oldest = np.zeros(n, dtype=np.int64)
