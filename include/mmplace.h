@@ -662,6 +662,9 @@ int32_t mmp_rate_run(mmp_fleet *, int32_t self, const mmp_scale_in *entries, int
  *   registered  self is among the model's LOADED registrations in the committed registry, every registration looked at
  *               (MM:7007-7010).  Otherwise (registered only as a failed load, or no record) MMP_SD_NOT_REGISTERED and nothing
  *               else.  The registered entries are the reference's waitFor (report.n_registered).
+ *   undecided   a model whose copy_count is saturated at 255 over more than 255 registrations (where its loaded copies end is
+ *               unknown, as for mmp_scale_eval's -1 and MMP_JE_UNDECIDED): MMP_SD_UNDECIDED alone, no decision, counted in no
+ *               report field; the pod runs the reference's loop body for that entry itself.
  *   stale       a registered entry with lru_t < cutoff: MMP_SD_STALE, counted in report.will_be_skipped (MM:7011-7014).
  *   task body   (MM:7016-7040), registered entries:
  *                 MMP_SD_ENTRY_GONE or _FAILED: nothing more (MM:7017-7020)
@@ -712,6 +715,7 @@ typedef struct {
 #define MMP_SD_PLACED 16u          /* a decision was made: target / n_candidates are its answer */
 #define MMP_SD_REFUSED 32u         /* lruTime > 0, but checkLoadFailureCount refused the load: no decision */
 #define MMP_SD_WAIT 64u            /* target is an instance and lruTime >= cutoff: the pod waits for the load (MM:7037-7038) */
+#define MMP_SD_UNDECIDED 128u      /* copy_count saturated at 255 over > 255 registrations: alone, nothing decided or counted */
 typedef struct {
   int32_t model; uint32_t what;    /* model; the OR of MMP_SD_* */
   int32_t target, n_candidates;    /* as mmp_decision_out with MMP_SD_PLACED, else MMP_TARGET_INVALID and 0 */
@@ -732,6 +736,10 @@ int32_t mmp_shutdown_run(mmp_fleet *, int32_t self, const mmp_shutdown_entry *en
  * placed for each one the rebalance rule reloads (ensureLoadedElsewhere MM:6905).  entries[] are the evictions the pod's cache
  * reported, in listener order, at most one entry per model.  Per entry, in Java long arithmetic, over every registration of the
  * model (the overflow ones included), loaded = the first copy_count registrations, the rest failed loads:
+ *   undecided   a model whose copy_count is saturated at 255 over more than 255 registrations (where its loaded copies end is
+ *               unknown, as for mmp_scale_eval's -1 and MMP_JE_UNDECIDED): MMP_EV_UNDECIDED alone, no decision, the record's
+ *               own last_used / last_unload_time, counted in no report field; the pod runs the reference's listener task for
+ *               that entry itself.
  *   deregister  MMP_EV_UNREGISTER: the pod's loaded registration has time load_ts (instanceIds.remove(self, loadTime)).
  *               MMP_EV_DROP_FAILURE: the pod's failed registration has time load_complete_ts (removeLoadFailure, MR:173-179).
  *               Neither: no write.  Otherwise out[r].last_used is the record's lastUsed after updateLastUsed(last_used) (0 reads
@@ -785,6 +793,7 @@ typedef struct {
 #define MMP_EV_LOADED_ELSEWHERE 16u /* a reload answered by a loaded copy on another ranked instance: no load */
 #define MMP_EV_REFUSED 32u         /* a reload checkLoadFailureCount refused: no decision */
 #define MMP_EV_PLACED 64u          /* a decision was made: target / n_candidates are its answer */
+#define MMP_EV_UNDECIDED 128u      /* copy_count saturated at 255 over > 255 registrations: alone, nothing decided or counted */
 typedef struct {
   int32_t model; uint32_t what;    /* model; the OR of MMP_EV_* */
   int32_t target, n_candidates;    /* as mmp_decision_out with MMP_EV_PLACED, else MMP_TARGET_INVALID and 0 */

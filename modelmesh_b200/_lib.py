@@ -79,7 +79,7 @@ SHUTDOWN_ACTION = np.dtype([("model", "<i4"), ("what", "<u4"), ("target", "<i4")
                            align=True)
 assert SHUTDOWN_ENTRY.itemsize == 24 and SHUTDOWN_PARAMS.itemsize == 24 and SHUTDOWN_ACTION.itemsize == 24
 SD_ENTRY_GONE, SD_ENTRY_FAILED, SD_ENTRY_ABORTED = 1, 2, 4
-SD_NOT_REGISTERED, SD_STALE, SD_REMOVE_LOCAL, SD_DEREGISTER_NOW, SD_PLACED, SD_REFUSED, SD_WAIT = 1, 2, 4, 8, 16, 32, 64
+SD_NOT_REGISTERED, SD_STALE, SD_REMOVE_LOCAL, SD_DEREGISTER_NOW, SD_PLACED, SD_REFUSED, SD_WAIT, SD_UNDECIDED = 1, 2, 4, 8, 16, 32, 64, 128
 EVICT_ENTRY = np.dtype([("model", "<i4"), ("flags", "<u4"), ("last_used", "<i8"), ("load_ts", "<i8"), ("load_complete_ts", "<i8")],
                        align=True)
 EVICT_PARAMS = np.dtype([("now", "<i8"), ("load_timeout_ms", "<i8"), ("load_failure_expiry_ms", "<i8")], align=True)
@@ -87,7 +87,7 @@ EVICT_ACTION = np.dtype([("model", "<i4"), ("what", "<u4"), ("target", "<i4"), (
                          ("last_unload_time", "<i8")], align=True)
 assert EVICT_ENTRY.itemsize == 32 and EVICT_PARAMS.itemsize == 24 and EVICT_ACTION.itemsize == 32
 EV_ENTRY_FAILED = 1
-EV_UNREGISTER, EV_DROP_FAILURE, EV_RELOAD, EV_CLUSTER_FULL, EV_LOADED_ELSEWHERE, EV_REFUSED, EV_PLACED = 1, 2, 4, 8, 16, 32, 64
+EV_UNREGISTER, EV_DROP_FAILURE, EV_RELOAD, EV_CLUSTER_FULL, EV_LOADED_ELSEWHERE, EV_REFUSED, EV_PLACED, EV_UNDECIDED = 1, 2, 4, 8, 16, 32, 64, 128
 LRU_LOAD = 5
 CHURN_REQUEST, CHURN_REMOVE, CHURN_REAPER = 0, 1, 2
 

@@ -39,6 +39,15 @@ struct ScaleTables {
 __device__ __forceinline__ long long jmul64(long long a, long long b) { return (long long)((unsigned long long)a * (unsigned long long)b); }
 __device__ __forceinline__ long long jadd64(long long a, long long b) { return (long long)((unsigned long long)a + (unsigned long long)b); }
 
+// how many of a model's registrations are loaded copies: the first copy_count of them (up to four registrations, a copy count
+// past them reads the inline positions, as the four-edge list always did).  -1 for a copy count saturated at 255 over more
+// than 255 registrations, where the loaded copies end is unknown (mmplace.h): k_scale_eval answers -1, the pod tasks
+// MMP_*_UNDECIDED
+__device__ __forceinline__ int loaded_copies(const mmp_model_row &mr) {
+  if (mr.copy_count == 255 && mr.reserved > 255u) return -1;
+  return min((int)mr.copy_count, max((int)mr.reserved, 4));
+}
+
 __device__ __forceinline__ int count_rpm_above(const int *sorted, int n, int thr) {  // #{rpm > thr} in an ascending array
   int lo = 0, hi = n;
   while (lo < hi) { const int mid = (lo + hi) >> 1; if (sorted[mid] <= thr) lo = mid + 1; else hi = mid; }
@@ -119,12 +128,11 @@ __global__ void k_scale_eval(ScaleTables T, const mmp_scale_in *__restrict__ in,
   o.action = 0; o.copies_to_load = 0; o.load_last_used = 0; o.rpm = 0; o.i1 = e.i1; o.i2 = e.i2; o.set_heavy = 0; o.remove = 0;
   if (e.model < 0 || e.model >= T.n_models || e.instance < 0 || e.instance >= T.max_instances) { o.action = -1; out[r] = o; return; }
   const mmp_model_row mr = T.models[e.model];
-  // a saturated copy count over more than 255 registrations: where the loaded copies end is unknown (mmplace.h)
-  if (mr.copy_count == 255 && mr.reserved > 255u) { o.action = -1; out[r] = o; return; }
+  const int loaded = loaded_copies(mr);
+  if (loaded < 0) { o.action = -1; out[r] = o; return; }
   const ModelRegs g = model_regs(T.R, e.model, mr.reserved);
   long long ts;
-  // (up to four registrations: a copy count past them reads the inline positions, as the four-edge list always did)
-  const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4)), failed = n_edges - loaded;
+  const int n_edges = (int)mr.reserved, failed = n_edges - loaded;
   const int self_rank = T.rank_of[e.instance];
   const long long time_delta = jsub(p.now, p.last_check_time);
   // ---------------- scale-up (rateTrackingTask) ----------------
@@ -374,7 +382,7 @@ __global__ void k_janitor_sweep(RegTables R, const mmp_model_row *__restrict__ m
   if (loaded_pos < 0 && !failed) return;
   atomicAdd(&J.cnt[JC_REFS], 1);
   const long long lul0 = model_lul[m];
-  if (cc == 255 && n_regs > 255) {  // where the loaded copies end is unknown (mmp_scale_eval's -1)
+  if (loaded_copies(mr) < 0) {  // where the loaded copies end is unknown (mmp_scale_eval's -1)
     J.edits[atomicAdd(&J.cnt[JC_EDITS], 1)] = mmp_janitor_edit{m, MMP_JE_UNDECIDED, mr.last_used, lul0};
     return;
   }
@@ -419,7 +427,7 @@ __global__ void k_janitor_eval(ScaleTables T, mmp_scale_params p, int self, int 
   const mmp_janitor_entry ce = J.entries[x.entry];
   const mmp_model_row mr = T.models[x.model];
   const ModelRegs g = model_regs(T.R, x.model, mr.reserved);
-  const int loaded = min((int)mr.copy_count, max((int)mr.reserved, 4));  // as k_scale_eval counts them
+  const int loaded = loaded_copies(mr);  // (>= 0: k_janitor_sweep makes no candidate of a saturated record)
   J.cand[c].removes = scale_down_removes(T, p, self, x.model, ce.last_used, ce.last_heavy, ce.count, flags, g, loaded, T.rank_of[self]) &&
                       x.reg_ts == ce.load_ts;
 }
@@ -573,7 +581,7 @@ __global__ void __launch_bounds__(RATE_PLAN_THREADS) k_rate_plan(RegTables R, co
       if (o.action == 1 || o.action == 2) {
         const mmp_model_row mr = models[model];
         const ModelRegs g = model_regs(R, model, mr.reserved);
-        const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4));  // as k_scale_eval counts them
+        const int n_edges = (int)mr.reserved, loaded = loaded_copies(mr);  // (>= 0: k_scale_eval answered -1 for a saturated record)
         long long ts;
         atomicAdd(&tot[o.action == 1 ? 0 : 1], 1);
         if (load_failures_refuse(R, g, loaded, n_edges, fail_since)) atomicAdd(&tot[2], 1);
@@ -657,11 +665,13 @@ __global__ void k_shutdown_plan(RegTables R, const mmp_model_row *__restrict__ m
   if (found_other) {
     const mmp_model_row mr = models[e.model];
     const ModelRegs g = model_regs(R, e.model, mr.reserved);
-    const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4));  // as k_rate_plan counts them
+    const int n_edges = (int)mr.reserved, loaded = loaded_copies(mr);
     bool registered = false;
     long long ts;
     for (int j = 0; j < loaded && !registered; j++) registered = reg_at(R, g, j, ts) == pod;
-    if (!registered) {
+    if (loaded < 0) {
+      what = MMP_SD_UNDECIDED;
+    } else if (!registered) {
       what = MMP_SD_NOT_REGISTERED;
     } else {
       atomicAdd(&B.hdr->rep.n_registered, 1);
@@ -721,8 +731,14 @@ __global__ void k_evict_plan(RegTables R, const mmp_model_row *__restrict__ mode
   const mmp_evict_entry e = B.entries[r];
   if (atomicCAS(&B.slot[e.model], -1, r) != -1) B.hdr->dup = 1;
   const mmp_model_row mr = models[e.model];
+  const int loaded = loaded_copies(mr);
+  if (loaded < 0) {
+    B.dec[r] = rate_inactive(pod);
+    B.out[r] = mmp_evict_action{e.model, MMP_EV_UNDECIDED, MMP_TARGET_INVALID, 0, mr.last_used, model_lul[e.model]};
+    return;
+  }
   const ModelRegs g = model_regs(R, e.model, mr.reserved);
-  const int n_edges = (int)mr.reserved, loaded = min((int)mr.copy_count, max(n_edges, 4));  // as k_shutdown_plan counts them
+  const int n_edges = (int)mr.reserved;
   // the pod's first loaded and first failed registration (as k_janitor_sweep finds them), and a loaded copy on another ranked
   // instance
   int loaded_at = -1, failed_at = -1;
@@ -754,7 +770,8 @@ __global__ void k_evict_plan(RegTables R, const mmp_model_row *__restrict__ mode
                                     : rate_inactive(pod);
   B.out[r] = mmp_evict_action{e.model, what, MMP_TARGET_INVALID, 0, lu_rec, lul};
 }
-// one thread per entry: the answer, and the report (one counter per MMP_EV_* bit, in bit order, then n_none)
+// one thread per entry: the answer, and the report (one counter per MMP_EV_* bit below MMP_EV_UNDECIDED, in bit order, then
+// n_none)
 __global__ void k_evict_pack(EvBufs B, int n) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;

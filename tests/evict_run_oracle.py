@@ -3,6 +3,7 @@ getNext answered by OracleFleet.get_next_batch: the reference mmp_evict_run is c
 its own check without a GPU: tests/test_evict_run_oracle.py).
 
 For each eviction, in listener order (the task each one puts on taskPool, MM:2882-2932):
+    a saturated record (rate_run_oracle.saturated): MMP_EV_UNDECIDED alone, the record's own values; the pod decides it
     attemptReload (MM:2886-2896), on the record before the write: !ce.isFailed() and the record holds the pod;
         loadedTime = instanceIds.get(pod), else loadFailedInstanceIds.get(pod); now - loadedTime > 2 * loadTimeoutMs
     deregisterModel(key, lastUsed, ce.loadTimestamp, ce.loadCompleteTimestamp) (MM:2936-2962):
@@ -24,7 +25,7 @@ import numpy as np
 
 from modelmesh_b200 import _lib as L
 from oracle import binding as ob
-from rate_run_oracle import jdiv, jlong, refused
+from rate_run_oracle import jdiv, jlong, refused, saturated
 
 REPORT_KEYS = ("n_unregister", "n_drop_failure", "n_reload", "n_cluster_full", "n_loaded_elsewhere", "n_refused", "n_placed")
 BITS = (L.EV_UNREGISTER, L.EV_DROP_FAILURE, L.EV_RELOAD, L.EV_CLUSTER_FULL, L.EV_LOADED_ELSEWHERE, L.EV_REFUSED, L.EV_PLACED)
@@ -49,6 +50,10 @@ def evict_run(o: ob.OracleFleet, fl, ts, lul, pod: int, entries, params, seed: i
     tasks = []   # (r, model, lastUsed) of each getNext
     for r, ent in enumerate(entries):
         m = int(ent["model"])
+        if saturated(fl, m):   # the pod decides it itself: no edit, the record's own values
+            out["what"][r] = L.EV_UNDECIDED
+            out["last_used"][r], out["last_unload_time"][r] = int(fl.model_last_used[m]), int(lul[m])
+            continue
         a, k, b = int(fl.edge_off[m]), int(fl.n_loaded[m]), int(fl.edge_off[m + 1])
         regs = [int(i) for i in fl.edge_inst[a:b]]
         loaded_at = next((j for j in range(k) if regs[j] == pod), None)

@@ -14,6 +14,7 @@ import numpy as np
 
 from modelmesh_b200 import _lib as L
 from oracle import binding as ob
+from rate_run_oracle import saturated
 
 SHORT_EXPIRY_RECENT_USE_TIME_MS = 180_000
 vp = lambda a: a.ctypes.data_as(C.c_void_p)
@@ -58,7 +59,7 @@ def janitor_run(o: ob.OracleFleet, fl, ts, lul, self_idx: int, entries, params):
         a, b = int(fl.edge_off[m]), int(fl.edge_off[m + 1])
         nl = int(fl.n_loaded[m])
         rec_lu, rec_lul = int(fl.model_last_used[m]), int(lul[m])
-        if min(nl, 255) == 255 and b - a > 255:
+        if saturated(fl, m):
             edits[m] = [L.JE_UNDECIDED, rec_lu, rec_lul]
             continue
         pos = [q - a for q in range(a, b) if fl.edge_inst[q] == self_idx]

@@ -32,13 +32,20 @@ def jdiv(a: int, b: int) -> int:
     return q if (a >= 0) == (b >= 0) else -q
 
 
+def saturated(fl, m: int) -> bool:
+    """the committed record's copy count (min(255, loaded)) is saturated over more than 255 registrations: where its loaded
+    copies end is unknown, and the library decides nothing for the model (mmp_scale_eval's -1, MMP_*_UNDECIDED)"""
+    return min(int(fl.n_loaded[m]), 255) == 255 and int(fl.edge_off[m + 1] - fl.edge_off[m]) > 255
+
+
 def too_soon(scale) -> bool:
     delta = jlong(int(scale["now"]) - int(scale["last_check_time"]))
     return jlong(delta * 5) < jlong(int(scale["rate_check_interval_ms"]) * 3)
 
 
 def evaluate(o: ob.OracleFleet, fl, ts, entries, scale):
-    """orc_rate_task_eval per entry (can_remove has no part in it) as L.SCALE_OUT records"""
+    """orc_rate_task_eval per entry (can_remove has no part in it) as L.SCALE_OUT records; a saturated record's entry is
+    action -1 with i1 / i2 kept and nothing else, as mmp_scale_eval answers it"""
     n = len(entries)
     m64 = entries["model"].astype(np.int64)
     deg = (fl.edge_off[m64 + 1] - fl.edge_off[m64]).astype(np.int64)
@@ -63,6 +70,9 @@ def evaluate(o: ob.OracleFleet, fl, ts, entries, scale):
     out = np.zeros(n, dtype=L.SCALE_OUT)
     for k in L.SCALE_OUT.names:
         out[k] = up[k]
+    for r in range(n):
+        if saturated(fl, int(m64[r])):
+            out[r] = (-1, 0, 0, 0, entries["i1"][r], entries["i2"][r], 0, 0)
     return out
 
 

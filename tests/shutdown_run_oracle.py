@@ -4,6 +4,7 @@ with every getNext answered by OracleFleet.get_next_batch: the reference mmp_shu
 
     foundOther   clusterState holds an instance other than the pod (MM:6968-6976); without one no entry is evaluated
     for each entry of descendingLruMap(), most recently used first (MM:7005):
+      a saturated record (rate_run_oracle.saturated)             ->  MMP_SD_UNDECIDED alone: the pod decides it itself
       mr == null || !mr.getInstanceIds().containsKey(instanceId)  ->  skipped (MM:7007-7010)
       lruT < cutoff                                               ->  willBeSkipped++ (MM:7011-7014)
       the task (MM:7016-7045):
@@ -20,7 +21,7 @@ import numpy as np
 
 from modelmesh_b200 import _lib as L
 from oracle import binding as ob
-from rate_run_oracle import jlong, refused
+from rate_run_oracle import jlong, refused, saturated
 
 
 def shutdown_run(o: ob.OracleFleet, fl, ts, pod: int, entries, params, seed: int, fresh_self=None):
@@ -44,6 +45,9 @@ def shutdown_run(o: ob.OracleFleet, fl, ts, pod: int, entries, params, seed: int
     tasks = []   # (r, model, lruTime) of each triggerNewModelCopyElsewhere
     for r, ent in enumerate(entries):
         m = int(ent["model"])
+        if saturated(fl, m):
+            out["what"][r] = L.SD_UNDECIDED
+            continue
         a, k = int(fl.edge_off[m]), int(fl.n_loaded[m])
         if pod not in set(int(i) for i in fl.edge_inst[a:a + k]):
             out["what"][r] = L.SD_NOT_REGISTERED

@@ -10,6 +10,7 @@ import janitor_run_oracle as jro
 from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import make_fleet
+from pod_task_edges import janitor_hand_fleet as hand_fleet
 from test_oracle_properties import brute_janitor_entry
 
 EXPIRY = 900_000          # LOAD_FAILURE_EXPIRY_MS
@@ -32,24 +33,6 @@ def entry(model, last_used, weight=10, load_ts=0, failed=False, last_heavy=0, co
     e["model"], e["weight"], e["last_used"], e["load_ts"], e["flags"] = model, weight, last_used, load_ts, L.JANITOR_FAILED if failed else 0
     e["last_heavy"], e["count"] = last_heavy, count
     return e
-
-
-def hand_fleet(regs, seed=3, ni=24):
-    """a C3 fleet 2 % from full whose models hold exactly regs[m] = (loaded [(instance, ts)], failed [(instance, ts)])"""
-    fl = make_fleet("C3", len(regs), ni, seed)
-    fl.inst_rows["used"] = fl.inst_rows["capacity"] - fl.inst_rows["capacity"] // 50
-    inst, ts, off, nl, nf = [], [], [0], [], []
-    for loaded, failed in regs:
-        for i, t in loaded + failed:
-            inst.append(i)
-            ts.append(t)
-        off.append(len(inst))
-        nl.append(len(loaded))
-        nf.append(len(failed))
-    fl.edge_inst, fl.edge_off = np.array(inst, dtype=np.int32), np.array(off, dtype=np.int64)
-    fl.n_loaded, fl.n_failed = np.array(nl, dtype=np.int32), np.array(nf, dtype=np.int32)
-    fl.model_last_used[:] = fl.now_ms - HOUR
-    return fl, np.array(ts, dtype=np.int64)
 
 
 def known_case():

@@ -7,9 +7,9 @@ ms after it."""
 import numpy as np
 
 import rate_run_oracle as rro
-from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import make_fleet
+from pod_task_edges import hand_fleet
 
 HOUR = 3_600_000
 EXPIRY = 900_000
@@ -34,34 +34,6 @@ def entry(pod, model, rpm=0, second=False, delta=10_000):
     e["last_used"] = 1
     e["i1"], e["i2"] = (IT - 100, IT - 100) if second else (IT - 1000, IT - 1000)
     return e
-
-
-def hand_fleet(regs, ni, seed=3, rpm=None, inactive=()):
-    """a C3 fleet half full with no type constraints whose models hold exactly regs[m] = (loaded [(instance, ts)], failed
-    [(instance, ts)]); rpm: per instance published rpm; inactive: instances out of the service-instance map (they count, but
-    no decision can pick them)"""
-    fl = make_fleet("C3", len(regs), ni, seed)
-    fl.type_config = None
-    fl.type_names = fl.type_names[:1]
-    fl.model_type[:] = 0
-    fl.inst_rows["rpm"] = 0 if rpm is None else rpm
-    fl.inst_rows["used"] = fl.inst_rows["capacity"] // 2
-    fl.inst_rows["shutting_down"] = 0
-    fl.inst_rows["active"] = 1
-    for i in inactive:
-        fl.inst_rows["active"][i] = 0
-    inst, ts, off, nl, nf = [], [], [0], [], []
-    for loaded, failed in regs:
-        for i, t in loaded + failed:
-            inst.append(i)
-            ts.append(t)
-        off.append(len(inst))
-        nl.append(len(loaded))
-        nf.append(len(failed))
-    fl.edge_inst, fl.edge_off = np.array(inst, dtype=np.int32), np.array(off, dtype=np.int64)
-    fl.n_loaded, fl.n_failed = np.array(nl, dtype=np.int32), np.array(nf, dtype=np.int32)
-    fl.model_last_used[:] = fl.now_ms - HOUR
-    return fl, np.array(ts, dtype=np.int64), oracle_from_synth(fl)
 
 
 def by_entry(loads):
