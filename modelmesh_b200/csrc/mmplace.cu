@@ -5,6 +5,8 @@
 //                                         the instance under PLACEMENT_ORDER; row stride is a multiple of 128 B
 //   excl_ranks [n_models] int4            the ranks of a model's <= 4 inline edges (-1: none), r[0] = -2: overflow ids,
 //                                         read the row (unsharded fleets)
+//   split_key [n_models] SplitKey 16 B    what k_place_split reads of a model: last_used, lowest live inline rank, type
+//                                         slot | overflow bit (unsharded fleets; built beside excl_ranks)
 //   zero_row  [row_words]           u32   all zero, one per fleet: the row of every MMP_DF_REQUEST_MODEL decision (unsharded fleets)
 //   cand/pref [n_slots][row_words]  u32   per type-constraint slot: allowed ∧ active / preferred instances (TCM:242-251)
 //   candx     [n_slots][row_words]  u32   cand minus likely-replaced replicaset members (MM:4769-4770)
@@ -18,8 +20,9 @@
 //   k_place_direct<4, 5>     the scoring kernel (default): one decision per lane, the row rebuilt from the model's excl_ranks,
 //                            longer walks through the word lists; optional slot-sorted batches (k_slot_keys + cub radix sort)
 //   k_slot_summary, k_place_split, k_place_tail<4, 5>   large batches in two passes (launch_split): per-slot summaries
-//                            answer the decisions clear of their slot's reach, k_place_direct's body walks the rest and a
-//                            warp resolves each decision of a model with overflow ids
+//                            answer the decisions clear of their slot's reach (k_place_split reads the record, the model's
+//                            split_key, rank_of[self] and self's row: 56 B streamed per decision), k_place_direct's body
+//                            walks the rest and a warp resolves each decision of a model with overflow ids
 //   k_place_lanes            round 1's streaming kernel (whole rows through TMA landing stages): MMP_KERNEL=lanes and the
 //                            collective instance-shard path
 //   k_place_small            tiny batches as a stream launch / replayed CUDA graph;  k_place_server: the resident B = 1 server
@@ -75,9 +78,11 @@ static thread_local std::string g_err;
 // One thread per model scatters its (<= 4) inline edges into its own bitmap row: no atomics needed.
 // (instance-sharded: a stored row holds row words [word_lo, word_hi) at a stride of `stride` words)
 // ranks (optional, SnapshotView::excl_ranks): the rank of every bit set here, -1 for an edge that sets none.
+// keys (optional, SnapshotView::split_key, with ranks): each model's SplitKey from the snapshot's model rows and type slots.
 __global__ void k_build_bitmap(uint32_t *__restrict__ excl, const int4 *__restrict__ edge_inl,
                                const int32_t *__restrict__ rank_of, int n_models, int stride, int word_lo, int word_hi,
-                               int4 *__restrict__ ranks) {
+                               int4 *__restrict__ ranks, const mmp_model_row *__restrict__ models,
+                               const uint16_t *__restrict__ type_slot, int n_type_ids, SplitKey *__restrict__ keys) {
   int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= n_models) return;
   int4 e = edge_inl[m];
@@ -92,16 +97,20 @@ __global__ void k_build_bitmap(uint32_t *__restrict__ excl, const int4 *__restri
     }
   }
   if (ranks) ranks[m] = make_int4(rs[0], rs[1], rs[2], rs[3]);
+  if (keys) keys[m] = make_split_key(models[m], rs, type_slot, n_type_ids);
 }
-// (launched after k_build_bitmap: a model with overflow edges gets the EXCL_RANKS_OVF marker in its rank entry)
+// (launched after k_build_bitmap: a model with overflow edges gets the EXCL_RANKS_OVF marker in its rank entry and
+// SPLIT_KEY_OVF in its SplitKey)
 __global__ void k_build_bitmap_ovf(uint32_t *__restrict__ excl, const OvfEdge *__restrict__ ovf, int n_ovf,
-                                   const int32_t *__restrict__ rank_of, int stride, int word_lo, int word_hi, int4 *__restrict__ ranks) {
+                                   const int32_t *__restrict__ rank_of, int stride, int word_lo, int word_hi, int4 *__restrict__ ranks,
+                                   SplitKey *__restrict__ keys) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_ovf) return;
   const int m = ovf[i].model, r = rank_of[ovf[i].inst];
   if (r >= 0 && (r >> 5) >= word_lo && (r >> 5) < word_hi)
     atomicOr(&excl[(size_t)m * stride + ((r >> 5) - word_lo)], 1u << (r & 31));
   if (ranks) ranks[m].x = EXCL_RANKS_OVF;
+  if (keys) atomicOr(&keys[m].slot, SPLIT_KEY_OVF);  // (a model's overflow edges are many threads)
 }
 
 // ---- TMA 1-D bulk copy + mbarrier helpers (cp.async.bulk: SASS UBLKCP) ----
@@ -774,24 +783,25 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
   const bool valid = i < n;
   mmp_decision_in d = no_decision();
   if (valid) d = load_decision_stream(in, i);
-  const int m = excl_row_id(s, d.model, d.flags);
-  RowRanks row;  // (read as k_place_direct reads it: its overflow mark routes the decision the same way)
-  row.r[0] = row.r[1] = row.r[2] = row.r[3] = -1;
-  if (valid && m != ZERO_ROW) row = load_ranks(s.excl_ranks + (size_t)m * 4);
-  CtxA a;
-  a.ok = 0; a.self_rank = -1; a.mr.type_id = 0;
-  if (valid) prepare_ctx_a(s, d, a);
+  // a malformed decision loads nothing more: it is walked, and answered MMP_TARGET_INVALID there
+  const int32_t ok = valid ? decision_ok(s, d) : 0;
+  const bool req = request_model(d);  // (its model is a type id: it has no entry, and is never answered here)
+  int32_t self_rank = -1;
+  SplitKey k;
+  k.last_used = 0; k.min_rank = INT32_MAX; k.slot = 0;
+  if (ok) self_rank = __ldg(s.rank_of + d.self);
+  if (ok && !req) k = load_split_key(s.split_key + d.model);
   mmp_decision_out r;
-  const bool fast = valid && split_answer(s, d, a, row, fresh, n_fresh, sums, members, now, seed, pick_id(d, id_base + (uint64_t)i), r);
+  const bool fast = ok && split_answer(s, d, ok, self_rank, k, fresh, n_fresh, sums, members, now, seed, pick_id(d, id_base + (uint64_t)i), r);
   if (fast) out[i] = r;
-  const bool ovf = valid && !fast && row.overflow();
+  const bool ovf = ok && !req && !fast && (k.slot & SPLIT_KEY_OVF);
   const bool walk = valid && !fast && !ovf;
   warp_append(walk, i, walk_list, counts);
   warp_append(ovf, i, ovf_list, counts + 1);
   if (keys && valid) {
-    uint32_t k = 0xffffu;
-    if (walk) k = a.ok ? slot_key(s, a.mr.type_id) : 0xfffeu;
-    keys[i] = (uint16_t)k;
+    uint32_t key = 0xffffu;
+    if (walk) key = !ok ? 0xfffeu : req ? slot_key(s, d.model) : k.slot;
+    keys[i] = (uint16_t)key;
     key_idx[i] = i;
   }
 }
@@ -1249,7 +1259,7 @@ using IpcMapping = Owned<void *, cudaIpcCloseMemHandle>;   // cudaIpcOpenMemHand
 #include "commit_kernels.cuh"
 
 struct DeviceSnapshot {
-  DevBuf excl, excl_ranks, cand, candx, pref, has_pref, type_slot, full, rows, rank_of, csum, lsum, models;
+  DevBuf excl, excl_ranks, split_key, cand, candx, pref, has_pref, type_slot, full, rows, rank_of, csum, lsum, models;
   DevBuf cap_col, lthreads_col, linprog_col, part_of_rank, count_col, cand_before, nzw, nz_n;
   DevBuf front, nzw_full, nz_n_full;  // instance-sharded fleets: replicated first words of every row; word lists over the whole row
   SnapshotView view{};
@@ -2284,8 +2294,11 @@ static int32_t commit_locked(mmp_fleet *f, bool rows_on_device) {
                                               : (size_t)std::max(nm, 1) * ST * 4));
   // the excluded ranks of every model beside its row (k_place_direct reads them instead of the row): whole rows only
   const bool whole_rows = h.word_lo == 0 && h.word_hi == RW;
-  if (whole_rows) CK(ds.excl_ranks.ensure((size_t)std::max(nm, 1) * 16));
+  // ... and the SplitKey of every model (k_place_split reads it instead of the ranks and the model row), built from the
+  // model rows copied above and this snapshot's type slots
+  if (whole_rows) { CK(ds.excl_ranks.ensure((size_t)std::max(nm, 1) * 16)); CK(ds.split_key.ensure((size_t)std::max(nm, 1) * sizeof(SplitKey))); }
   int4 *ranks = whole_rows ? ds.excl_ranks.as<int4>() : nullptr;
+  SplitKey *keys = whole_rows ? ds.split_key.as<SplitKey>() : nullptr;
   // the row of every request-model decision (MMP_DF_REQUEST_MODEL): the stride is fixed for the fleet, so it is zeroed once
   // (cudaMalloc: 256-byte aligned, as the TMA copies of k_place_lanes and k_place need)
   if (whole_rows && !f->zero_row.p) {
@@ -2295,12 +2308,13 @@ static int32_t commit_locked(mmp_fleet *f, bool rows_on_device) {
   if (nm) {
     CK(cudaMemsetAsync(ds.excl.p, 0, (size_t)nm * ST * 4, st));
     k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, ST,
-                                                     h.word_lo, h.word_hi, ranks);
+                                                     h.word_lo, h.word_hi, ranks, ds.models.as<mmp_model_row>(),
+                                                     ds.type_slot.as<uint16_t>(), (int)h.type_slot.size(), keys);
     f->launches++;
     CK(cudaGetLastError());
     if (lv.n_ovf) {
       k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf,
-                                                                 ds.rank_of.as<int32_t>(), ST, h.word_lo, h.word_hi, ranks);
+                                                                 ds.rank_of.as<int32_t>(), ST, h.word_lo, h.word_hi, ranks, keys);
       f->launches++;
       CK(cudaGetLastError());
     }
@@ -2309,8 +2323,9 @@ static int32_t commit_locked(mmp_fleet *f, bool rows_on_device) {
     const int F = std::min(SHARD_FRONT_WORDS, RW);
     CK(ds.front.ensure((size_t)nm * F * 4));
     CK(cudaMemsetAsync(ds.front.p, 0, (size_t)nm * F * 4, st));
-    k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, F, 0, F, nullptr);
-    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F, nullptr);
+    k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, F, 0, F, nullptr,
+                                                     nullptr, nullptr, 0, nullptr);
+    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F, nullptr, nullptr);
     f->launches += 2;
     CK(cudaGetLastError());
   }
@@ -2330,7 +2345,7 @@ static int32_t commit_locked(mmp_fleet *f, bool rows_on_device) {
   v.word_lo = h.word_lo; v.word_hi = h.word_hi; v.excl_stride = ST; v.n_slots = h.n_slots; v.n_extra = 0;
   v.count_col = ds.count_col.as<int32_t>(); v.cand_before = ds.cand_before.as<int32_t>();
   v.nzw = ds.nzw.as<uint16_t>(); v.nz_n = ds.nz_n.as<int32_t>();
-  v.excl = ds.excl.as<uint32_t>(); v.excl_ranks = ranks ? ds.excl_ranks.as<int32_t>() : nullptr;
+  v.excl = ds.excl.as<uint32_t>(); v.excl_ranks = ranks ? ds.excl_ranks.as<int32_t>() : nullptr; v.split_key = keys;
   v.cand = ds.cand.as<uint32_t>(); v.pref = ds.pref.as<uint32_t>();
   v.has_pref = ds.has_pref.as<uint8_t>(); v.type_slot = ds.type_slot.as<uint16_t>(); v.candx = ds.candx.as<uint32_t>();
   v.full = ds.full.as<uint32_t>(); v.rows = ds.rows.as<RankRow>(); v.rank_of = ds.rank_of.as<int32_t>();

@@ -70,6 +70,11 @@ MMP_HD RankRow load_row_any(const RankRow *p) {  // generic address space (share
 struct WordSumI { int32_t lo, hi; };  // min/max count over the 32 ranks of a bitmap word
 struct WordSumL { int64_t lo, hi; };  // min/max lruTime
 struct FreshRow { int64_t lru, rem; int32_t count, rpm; };  // getFreshInstanceRecord() (MM:5369-5386), what the walk reads of it
+// What k_place_split reads of a decision's model: one 16-byte entry per model, built at commit beside excl_ranks
+// (make_split_key) and fixed for the epoch.  last_used: the snapshot's model row's; min_rank: the lowest live rank among
+// its inline edges, INT32_MAX for none; slot: slot_key of its type id, SPLIT_KEY_OVF set for a model with overflow ids.
+struct alignas(16) SplitKey { int64_t last_used; int32_t min_rank; uint32_t slot; };
+static constexpr uint32_t SPLIT_KEY_OVF = 0x80000000u;
 
 struct SnapshotView {  // pointers into HBM (or host vectors in the CPU harness)
   int32_t n_ranks, row_words, n_models, max_instances;
@@ -98,6 +103,7 @@ struct SnapshotView {  // pointers into HBM (or host vectors in the CPU harness)
   const mmp_model_row *models; // [n_models]
   const uint32_t *zero_row;    // [excl_stride] all zero: the exclusion row of an MMP_DF_REQUEST_MODEL decision; null on
                                // instance-sharded fleets, where such a decision is malformed
+  const SplitKey *split_key;   // [n_models] what k_place_split reads of a model; unsharded fleets only (as excl_ranks), else null
 };
 
 // ---- where a decision's model comes from.  Unflagged: the committed registry (models[d.model], its exclusion row).
@@ -560,15 +566,21 @@ MMP_HD bool ctx_has_pref(const DecisionCtx &c) { return (c.slot >> 16) & 1; }
 // The context is gathered in two steps so that a kernel can issue the first (two independent gathers that depend only on
 // the decision record: the model row from HBM, rank_of[self]) a whole step ahead of the second (what depends on them).
 struct CtxA { mmp_model_row mr; int32_t self_rank; int32_t ok; };
-MMP_HD void prepare_ctx_a(const SnapshotView &s, const mmp_decision_in &d, CtxA &a) {
+// whether a decision is well formed, from its record alone (no load): everything else is answered MMP_TARGET_INVALID
+MMP_HD int32_t decision_ok(const SnapshotView &s, const mmp_decision_in &d) {
   // a request-model decision names a type id (mmp_type_id: [0, 65535)); its last_used can only come from the decision, and
   // only a fleet with the zero row (unsharded) takes it
   const bool req = request_model(d);
-  a.ok = !(d.self < 0 || d.self >= s.max_instances);
-  if (req ? (d.model < 0 || d.model >= 65535 || (d.flags & MMP_DF_MODEL_LAST_USED) || !s.zero_row) : (d.model < 0 || d.model >= s.n_models)) a.ok = 0;
+  int32_t ok = !(d.self < 0 || d.self >= s.max_instances);
+  if (req ? (d.model < 0 || d.model >= 65535 || (d.flags & MMP_DF_MODEL_LAST_USED) || !s.zero_row) : (d.model < 0 || d.model >= s.n_models)) ok = 0;
   // the decision's slice of extra[] must lie inside the table the caller passed (at most 16 entries, MMP_MAX_EXTRA):
   // anything else is a malformed decision (MMP_TARGET_INVALID), never an out-of-bounds read
-  if (d.extra_n < 0 || d.extra_n > 16 || (d.extra_n > 0 && (d.extra_off < 0 || (int64_t)d.extra_off + d.extra_n > (int64_t)s.n_extra))) a.ok = 0;
+  if (d.extra_n < 0 || d.extra_n > 16 || (d.extra_n > 0 && (d.extra_off < 0 || (int64_t)d.extra_off + d.extra_n > (int64_t)s.n_extra))) ok = 0;
+  return ok;
+}
+MMP_HD void prepare_ctx_a(const SnapshotView &s, const mmp_decision_in &d, CtxA &a) {
+  const bool req = request_model(d);
+  a.ok = decision_ok(s, d);
   a.self_rank = -1;
   a.mr.last_used = 0; a.mr.size_units = 0; a.mr.rpm = 0; a.mr.type_id = 0; a.mr.copy_count = 0; a.mr.fail_count = 0; a.mr.reserved = 0;
   if (a.ok && req) {
@@ -598,8 +610,31 @@ MMP_HD void prepare_ctx_a(const SnapshotView &s, const mmp_decision_in &d, CtxA 
 }
 // the mask slot of a type id, resolved as prepare_ctx_b resolves it (an id the snapshot does not know is type 0): the key a
 // slot-ordered batch is sorted by (prepare_ctx_b reads the whole type_slot entry, has_pref included)
-MMP_HD uint32_t slot_key(const SnapshotView &s, int32_t type_id) {
-  return (uint32_t)s.type_slot[(type_id >= 0 && type_id < s.n_type_ids) ? type_id : 0] & 0x7fffu;
+MMP_HD uint32_t slot_key_of(const uint16_t *type_slot, int32_t n_type_ids, int32_t type_id) {
+  return (uint32_t)type_slot[(type_id >= 0 && type_id < n_type_ids) ? type_id : 0] & 0x7fffu;
+}
+MMP_HD uint32_t slot_key(const SnapshotView &s, int32_t type_id) { return slot_key_of(s.type_slot, s.n_type_ids, type_id); }
+// a model's SplitKey from its snapshot row and the epoch ranks of its inline edges (-1: none, or not live), overflow bit
+// clear (k_build_bitmap; k_build_bitmap_ovf sets it)
+MMP_HD SplitKey make_split_key(const mmp_model_row &mr, const int32_t rs[4], const uint16_t *type_slot, int32_t n_type_ids) {
+  SplitKey k;
+  k.last_used = mr.last_used;
+  k.min_rank = INT32_MAX;
+  for (int j = 0; j < 4; j++) if (rs[j] >= 0 && rs[j] < k.min_rank) k.min_rank = rs[j];
+  k.slot = slot_key_of(type_slot, n_type_ids, mr.type_id);
+  return k;
+}
+MMP_HD SplitKey load_split_key(const SplitKey *p) {  // read once per decision: kept out of L1 like the decision record
+#if defined(__CUDA_ARCH__)
+  int4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  SplitKey k;
+  k.last_used = (int64_t)(((uint64_t)(uint32_t)v.y << 32) | (uint32_t)v.x);
+  k.min_rank = v.z; k.slot = (uint32_t)v.w;
+  return k;
+#else
+  return *p;
+#endif
 }
 MMP_HD void prepare_ctx_b(const SnapshotView &s, const mmp_decision_in &d, const CtxA &a, const FreshRow *fresh_tab, int32_t n_fresh,
                           const int32_t *extra, DecisionCtx &c) {
@@ -1699,17 +1734,18 @@ MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, b
 }
 
 // The fast answer of k_place_split: a valid, unflagged decision without extra excludes whose model has no overflow ids
-// and whose exclusions and self all lie at or past its slot's reach for its c_self.  a: prepare_ctx_a of d; row: its
-// model's excluded ranks.  Returns false, with nothing written, for every other decision.
-MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, const CtxA &a, const RowRanks &row, const FreshRow *fresh,
-                         int32_t n_fresh, const SlotSummary *sums, const int32_t *members, int64_t now, uint64_t seed,
-                         uint64_t decision_id, mmp_decision_out &out) {
-  if (!a.ok || request_model(d) || d.extra_n != 0 || row.overflow()) return false;
+// and whose exclusions and self all lie at or past its slot's reach for its c_self.  ok: decision_ok of d; self_rank:
+// rank_of[d.self]; k: its model's SplitKey (read only when ok and not a request-model decision).  Returns false, with
+// nothing written, for every other decision.
+MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, int32_t ok, int32_t self_rank, const SplitKey &k,
+                         const FreshRow *fresh, int32_t n_fresh, const SlotSummary *sums, const int32_t *members, int64_t now,
+                         uint64_t seed, uint64_t decision_id, mmp_decision_out &out) {
+  if (!ok || request_model(d) || d.extra_n != 0 || (k.slot & SPLIT_KEY_OVF)) return false;
   FreshRow fr;  // (as prepare_ctx_b)
   if (d.fresh >= 0 && d.fresh < n_fresh) fr = fresh[d.fresh];
-  else if (a.self_rank >= 0) { const RankRow sr = load_row(s.rows + a.self_rank); fr.lru = sr.lru; fr.rem = sr.rem; fr.count = sr.count; fr.rpm = 0; }
+  else if (self_rank >= 0) { const RankRow sr = load_row(s.rows + self_rank); fr.lru = sr.lru; fr.rem = sr.rem; fr.count = sr.count; fr.rpm = 0; }
   else return false;
-  const int slot = (int)slot_key(s, a.mr.type_id);
+  const int slot = (int)k.slot;
   const SlotSummary &sm = sums[slot];
   int cs;
   if (sm.best_full) {  // (decide_stream's c_self)
@@ -1717,16 +1753,25 @@ MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, const 
     cs = df > 45000 && df > a10;
   } else cs = fr.rem < s.min_space || fr.rem < (sm.best_rem >> 2);
   const int32_t reach = sm.reach[cs];
-  if (reach < 0 || (a.self_rank >= 0 && a.self_rank < reach)) return false;
-  for (int j = 0; j < 4; j++) if (row.r[j] >= 0 && row.r[j] < reach) return false;
+  if (reach < 0 || (self_rank >= 0 && self_rank < reach) || k.min_rank < reach) return false;
   const int32_t n_in = sm.n_in[cs];
-  const int64_t last_used = (d.flags & MMP_DF_MODEL_LAST_USED) ? a.mr.last_used : d.last_used;
+  const int64_t last_used = (d.flags & MMP_DF_MODEL_LAST_USED) ? k.last_used : d.last_used;
   const PickOut pk = pick_survivor(n_in, false, sm.best_rpm, fr.rpm, sm.best_rpm, last_used, now, seed, decision_id);
   if (pk.kind == PICK_SELF) return false;
   const int32_t cidx = pk.kind == PICK_BEST ? sm.best_idx : members[((size_t)slot * 2 + (size_t)cs) * SPLIT_CAP + pk.kth];
   out.target = target_of(cidx, d);
   out.n_candidates = 1 + n_in;
   return true;
+}
+// The same answer for a caller that holds the decision's model row and excluded ranks instead of its SplitKey (the CPU
+// harness): a: prepare_ctx_a of d; row: its model's excl_ranks entry.  The key is made from them as the commit makes it.
+MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, const CtxA &a, const RowRanks &row, const FreshRow *fresh,
+                         int32_t n_fresh, const SlotSummary *sums, const int32_t *members, int64_t now, uint64_t seed,
+                         uint64_t decision_id, mmp_decision_out &out) {
+  if (!a.ok || request_model(d)) return false;
+  SplitKey k = make_split_key(a.mr, row.r, s.type_slot, s.n_type_ids);
+  if (row.overflow()) k.slot |= SPLIT_KEY_OVF;
+  return split_answer(s, d, a.ok, a.self_rank, k, fresh, n_fresh, sums, members, now, seed, decision_id, out);
 }
 
 }  // namespace mmp

@@ -1,8 +1,8 @@
 """Kernel times of the two-pass placement path against the one-pass one (mmp_tune "split" 1 / 0), for the bench
 workloads C2 / C3 / C5: the bench's sweep batch placed through mmp_place_batch_device under torch.profiler, each kernel's
 mean device time per call by name (k_slot_summary, k_place_split, k_place_tail, k_place_direct, the slot sort), and the
-call's CUDA-event time; for k_place_split also the rate at which it streams a plain sweep's 80 B per decision (32 B record,
-16 B excl_ranks, 24 B model row, 8 B result).  GPU only.
+call's CUDA-event time; for k_place_split also the rate at which it streams a plain sweep's 56 B per decision (32 B record,
+16 B SplitKey, 8 B result).  GPU only.
 
     python tools/split_timing.py [--configs C2,C3,C5] [--calls 20]
 """
@@ -17,6 +17,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 SIZES = {"C2": (100_000, 1_000, 2), "C3": (1_000_000, 10_000, 3), "C5": (1_000_000, 10_000, 5)}
+SPLIT_BYTES = 32 + 16 + 8  # what k_place_split streams per plain decision: record, the model's SplitKey, result
 
 
 def main():
@@ -34,6 +35,12 @@ def main():
     lib = _lib.load_product()
     torch.cuda.init()
     print(torch.cuda.get_device_name(0))
+    try:
+        import subprocess
+        print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True).stdout.strip())
+    except OSError:
+        pass
     for cfg in args.configs.split(","):
         nm, ni, seed = SIZES[cfg]
         fl = make_fleet(cfg, nm, ni, seed)
@@ -64,7 +71,7 @@ def main():
                     per[name] += e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
             print(f"{cfg} split={split}: call median {np.median(ev) * 1000:.1f} us (min {np.min(ev) * 1000:.1f})")
             for k, v in sorted(per.items(), key=lambda kv: -kv[1]):
-                rate = f"  {80 * nm / (v / args.calls) / 1e6:6.2f} TB/s" if k == "k_place_split" else ""
+                rate = f"  {SPLIT_BYTES * nm / (v / args.calls) / 1e6:6.2f} TB/s" if k == "k_place_split" else ""
                 print(f"    {k[:60]:60s} {v / args.calls:9.1f} us/call{rate}")
         s._ck(lib.mmp_tune(s.h, b"split", 2))
         s.close()
