@@ -51,6 +51,7 @@
 #include <cstring>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <shared_mutex>
 #include <string>
 #include <thread>
@@ -1295,11 +1296,9 @@ struct PlaceCtx {
   // (k_exclude_slots, k_slot_lists) that the call's view points at
   DevBuf d_xids, d_xcand, d_xcandx, d_xpref, d_xnzw, d_xnz_n, d_xbefore;
   RpScratch rp;  // mmp_reaper_select's pass (scan_kernels.cuh)
-  DevBuf d_view, d_pruned, d_repaired, d_loads;  // mmp_reaper_run (registry_kernels.cuh): the pruned and repaired model rows, its lists
-  DevBuf d_jslot, d_jent, d_jcand, d_jout;        // mmp_janitor_run (registry_kernels.cuh): entry by model, entries, candidates, results
-  DevBuf d_rate, d_rate_rpm;                      // mmp_rate_run (registry_kernels.cuh): its tables up to round 0, the rpm column
-  DevBuf d_sd;                                    // mmp_shutdown_run (registry_kernels.cuh): entries, decisions, results, report, actions
-  DevBuf d_ev;                                    // mmp_evict_run (registry_kernels.cuh): entries, decisions, results, report, actions
+  // the pod-task calls (registry_kernels.cuh): one call's own tables, laid out by carve(); the entry of each model
+  // (max_models ints, -1 = none), filled with -1 when it is allocated and left so by every call; mmp_rate_run's rpm column
+  DevBuf d_task, d_model_slot, d_rate_rpm;
 };
 
 // The scoring kernel of untraced batches (MMP_KERNEL = direct | lanes | tile; launch_place): k_place_direct (rows rebuilt
@@ -1438,6 +1437,9 @@ class CtxLease {
   mmp_fleet *f_;
   PlaceCtx *c_;
 };
+
+// The CUDA-event time from c->e0 to c->e1 into t, which keeps its value where the events cannot be read
+static void event_ms(const PlaceCtx *c, float &t) { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) t = ms; }
 
 // ---------------------------------------------------------------------------------------------------------------
 // kernel dispatch on the row width

@@ -285,7 +285,7 @@ static int32_t registry_prune(mmp_fleet *f, int32_t self, int64_t now_ms, int64_
   CK(cudaMemcpyAsync(&n_out, c->d_n_open.p, 4, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(missing_since, c->d_in.p, (size_t)NI * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_prune_ms = ms; }
+  event_ms(c.get(), f->t_prune_ms);
   return read(c.get(), n_out);
 }
 
@@ -330,9 +330,23 @@ static ScaleTables scale_tables(mmp_fleet *f, const DeviceSnapshot &ds, LiveStat
   return T;
 }
 
+// The pod-task calls index their entries by model in the context's per-model slot array (max_models ints, -1 = no entry):
+// k_slot_claim takes entry k's model slot (atomicCAS -1 -> k) and raises *dup where another entry holds it; k_slot_release
+// gives the same slots back, so the array is filled with -1 only when it is allocated.  mmp_janitor_run and mmp_rate_run
+// launch the pair; k_shutdown_plan / k_evict_plan claim and k_shutdown_pack / k_evict_pack release in their own launches.
+template <class Entry>
+__global__ void k_slot_claim(const Entry *entries, int n, int *slot, int *dup) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n && atomicCAS(&slot[entries[k].model], -1, k) != -1) *dup = 1;
+}
+template <class Entry>
+__global__ void k_slot_release(const Entry *entries, int n, int *slot) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) slot[entries[k].model] = -1;
+}
+
 // mmp_janitor_run: the registry loop of one pod's janitor task (MM:6013-6145).  The pod's entries are indexed by model in
-// slot[] (max_models ints, -1 = no entry): k_janitor_index sets the call's, k_janitor_clear resets the same ones afterwards, so
-// the scratch is filled with -1 only when it is allocated.  A second entry of one model is reported through cnt[JC_DUP].
+// slot[] (k_slot_claim); a second entry of one model is reported through cnt[JC_DUP].
 enum { JC_EDITS = 0, JC_CANDS = 1, JC_REFS = 2, JC_DUP = 3 };
 struct JanitorCand { int model, entry, edit, removes; long long reg_ts; };  // reg_ts: the time of self's loaded registration
 struct JanitorBufs {
@@ -343,14 +357,6 @@ struct JanitorBufs {
   int *cnt;                            // JC_*
   mmp_janitor_report *report;
 };
-__global__ void k_janitor_index(JanitorBufs J, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n && atomicCAS(&J.slot[J.entries[k].model], -1, k) != -1) J.cnt[JC_DUP] = 1;
-}
-__global__ void k_janitor_clear(JanitorBufs J, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n) J.slot[J.entries[k].model] = -1;
-}
 // a deregistration's record changes (the janitor's MM:6059-6073, deregisterModel's MM:2955-2957): updateLastUnloadTime where
 // self's loaded copy left the record's cc loaded copies (MR:260-262), and updateLastUsed(lu) where use_lu (MR:239-246; the
 // callers decide what lu is and when it applies).  k_janitor_sweep, k_janitor_walk and k_evict_plan all make it
@@ -459,17 +465,31 @@ __global__ void k_janitor_walk(JanitorBufs J, const mmp_model_row *__restrict__ 
   *J.report = mmp_janitor_report{J.cnt[JC_REFS], n_edits, kept, removed, weight_removed};
 }
 
+// Lays a call's scratch out in one device buffer: take<T>(n) hands out room for n T's, each 16-byte aligned after the one
+// before.  carve() runs a layout twice: once to size the buffer, which it ensures at that total, then to hand out the
+// pointers, so no pointer is taken into a buffer that ensure() may still move.
+struct Carve {
+  uintptr_t base;
+  size_t off = 0;
+  template <class T> T *take(size_t n) { const size_t o = off; off += (n * sizeof(T) + 15) / 16 * 16; return reinterpret_cast<T *>(base + o); }
+};
+template <class Layout> static int32_t carve(DevBuf &buf, Layout layout) {
+  Carve size{0};
+  layout(size);
+  CK(buf.ensure(size.off));
+  Carve k{reinterpret_cast<uintptr_t>(buf.p)};
+  layout(k);
+  return MMP_OK;
+}
+
 // the epoch's type-set stats, queued on st: k_stats (the per-partition accumulators and the global LRU, into c->d_trace) and
 // k_type_stats per type id.  queue_scale_eval and mmp_evict_run read them
 struct TypeSetStats { StatsAcc *acc; long long *d_min; TypeStat *types; };
 static int32_t queue_type_stats(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, LiveState &lv, TypeSetStats &S, cudaStream_t st) {
   const int np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks, nt = lv.n_type_ids;
-  const size_t acc_bytes = (size_t)(np + 1) * sizeof(StatsAcc) + 8;
-  CK(c->d_trace.ensure(acc_bytes + (size_t)std::max(nt, 1) * sizeof(TypeStat) + 64));
-  S.acc = c->d_trace.as<StatsAcc>();
-  S.d_min = reinterpret_cast<long long *>(c->d_trace.as<char>() + (size_t)(np + 1) * sizeof(StatsAcc));
-  S.types = reinterpret_cast<TypeStat *>(c->d_trace.as<char>() + ((acc_bytes + 15) / 16) * 16);
-  CK(cudaMemsetAsync(c->d_trace.p, 0, acc_bytes, st));
+  const int32_t rc = carve(c->d_trace, [&](Carve &k) { S.acc = k.take<StatsAcc>(np + 1); S.d_min = k.take<long long>(1); S.types = k.take<TypeStat>(std::max(nt, 1)); });
+  if (rc < 0) return rc;
+  CK(cudaMemsetAsync(S.acc, 0, (size_t)(np + 1) * sizeof(StatsAcc), st));
   static const long long init = 0x7fffffffffffffffLL;
   CK(cudaMemcpyAsync(S.d_min, &init, 8, cudaMemcpyHostToDevice, st));
   if (nr > 0) {
@@ -513,8 +533,8 @@ static int32_t queue_scale_eval(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot 
 // inactive record where there is none) and decision 0 of each scale-up chain (compacted in entry order).  The host reads the
 // counts back once, then places the second copies under the epoch's tables and the chains round by round under the tables
 // derived for the heavy set; k_rate_step builds round j from round j - 1.  An inactive decision has model -1: a malformed
-// record, answered MMP_TARGET_INVALID without a walk.  The pod's entries are indexed by model in the janitor's slot[] only to
-// find two entries of one model.
+// record, answered MMP_TARGET_INVALID without a walk.  The pod's entries are indexed by model in slot[] (k_slot_claim) only
+// to find two entries of one model.
 struct RateHdr { int n_heavy, dup, n_second, n_scale_up, n_refused, n_sec_place, n_chain, longest; long long n_ids; };
 struct RateChain { int entry, copies, id0, len; };  // len: the decisions the chain places at most (min(copies, MMP_RATE_CHAIN_MAX))
 struct RateBufs {
@@ -527,14 +547,6 @@ struct RateBufs {
   RateHdr *hdr;
 };
 __device__ __forceinline__ mmp_decision_in rate_inactive(int pod) { return mmp_decision_in{-1, pod, 0, 0u, -1, 0, 0}; }
-__global__ void k_rate_index(RateBufs B, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n && atomicCAS(&B.slot[B.entries[k].model], -1, k) != -1) B.hdr->dup = 1;
-}
-__global__ void k_rate_clear(RateBufs B, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n) B.slot[B.entries[k].model] = -1;
-}
 // getExcludeSet (MM:5835-5856): the instances of the snapshot other than the pod whose published rpm is above the bound, in
 // no order (the derived tables do not depend on it)
 __global__ void k_rate_heavy(const int32_t *__restrict__ rank_of, const RankRow *__restrict__ rows, int max_instances, int pod, int thr,
@@ -641,13 +653,16 @@ __global__ void k_rate_step(const mmp_decision_in *__restrict__ prev, const mmp_
 
 // mmp_shutdown_run: one pod's pre-shutdown migration (MM:6990-7047).  k_shutdown_plan classifies every entry and writes its
 // decision, or rate_inactive's record where there is none; launch_place answers all n; k_shutdown_pack adds the answers and
-// the wait test.  The entries take their model's slot of the janitor's slot[] in k_shutdown_plan and give it back in
-// k_shutdown_pack, a later launch on the same stream: two entries of one model are found without a launch of their own.
-struct SdHdr { mmp_shutdown_report rep; int dup, pad[3]; };  // (48 B: the actions follow it in one copy back)
+// the wait test.  The entries take their model's slot of slot[] in k_shutdown_plan and give it back in k_shutdown_pack, a
+// later launch on the same stream: two entries of one model are found without a launch of their own.
+// mmp_shutdown_run's and mmp_evict_run's header: the report and the duplicate flag (48 B: the actions follow it in one copy
+// back, pack_copy_back)
+template <class Report> struct PackHdr { Report rep; int dup, pad[3]; };
+static_assert(sizeof(PackHdr<mmp_shutdown_report>) == 48 && sizeof(PackHdr<mmp_evict_report>) == 48, "the actions follow the header");
 struct SdBufs {
   const mmp_shutdown_entry *entries; int *slot;
   mmp_decision_in *dec; const mmp_decision_out *res;
-  SdHdr *hdr; mmp_shutdown_action *out;
+  PackHdr<mmp_shutdown_report> *hdr; mmp_shutdown_action *out;
   int32_t *extra;  // [the pod]
 };
 // one thread per entry: foundOther (MM:6968-6976), the registry test over every registration (MM:7007-7010), willBeSkipped
@@ -710,12 +725,11 @@ __global__ void k_shutdown_pack(SdBufs B, int n, long long cutoff) {
 // mmp_evict_run: one pod's eviction listener (MM:2867-2933) for a burst of evictions.  The type-set stats come from
 // queue_type_stats; k_evict_plan makes every entry's deregistration edit and decides its reload, writing the decision or
 // rate_inactive's record; launch_place answers all n; k_evict_pack adds the answers and the report.  The entries take their
-// model's slot of the janitor's slot[] in k_evict_plan and give it back in k_evict_pack, as mmp_shutdown_run's do.
-struct EvHdr { mmp_evict_report rep; int dup, pad[3]; };  // (48 B: the actions follow it in one copy back)
+// model's slot of slot[] in k_evict_plan and give it back in k_evict_pack, as mmp_shutdown_run's do.
 struct EvBufs {
   const mmp_evict_entry *entries; int *slot;
   mmp_decision_in *dec; const mmp_decision_out *res;
-  EvHdr *hdr; mmp_evict_action *out;
+  PackHdr<mmp_evict_report> *hdr; mmp_evict_action *out;
   int32_t *extra;  // [the pod]
 };
 // one thread per entry: the pod's registrations over every registration of the model, deregisterModel's edit (MM:2948-2957,
@@ -789,6 +803,102 @@ __global__ void k_evict_pack(EvBufs B, int n) {
   B.out[r] = a;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// the host steps the pod-task calls share: mmp_reaper_run, mmp_janitor_run, mmp_rate_run, mmp_shutdown_run, mmp_evict_run
+// ---------------------------------------------------------------------------------------------------------------
+// MMP_E_ARG for the first entry whose model index is out of range or that `also` refuses (a message, else null)
+template <class Entry, class Also>
+static int32_t check_entries(const mmp_fleet *f, const Entry *entries, int32_t n, Also also) {
+  for (int32_t k = 0; k < n; k++) {
+    if (entries[k].model < 0 || entries[k].model >= f->hs.cfg.max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
+    if (const char *m = also(entries[k])) { g_err = m; return MMP_E_ARG; }
+  }
+  return MMP_OK;
+}
+template <class Entry> static int32_t check_entries(const mmp_fleet *f, const Entry *entries, int32_t n) {
+  return check_entries(f, entries, n, [](const Entry &) -> const char * { return nullptr; });
+}
+
+static int32_t parse_fresh_self(const mmp_instance_row *fresh_self, FreshRow &fr) {
+  if (fresh_self)
+    if (const char *m = HostState::fresh_row(*fresh_self, fr)) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
+  return MMP_OK;
+}
+
+// How a pod-task call opens, after its own argument checks.  It reads the registry as of the last commit and the epoch built
+// from it: ingest_mu, then snap_mu shared (a commit's order: it flips the epoch under snap_mu while it holds ingest_mu), both
+// held until the call returns.  Then the refusals: no committed snapshot; no registration times (TIMES); a fleet on which
+// placing elsewhere is a collective call (PLACES).  Then the context lease and, for SLOTS, the per-model slot array.
+class PodCall {
+ public:
+  enum : unsigned { TIMES = 1, PLACES = 2, SLOTS = 4 };
+  PlaceCtx *c = nullptr;
+  const DeviceSnapshot *ds = nullptr;
+  LiveState *lv = nullptr;
+
+  int32_t open(mmp_fleet *f, const char *name, unsigned need) {
+    const int32_t rc = set_device(f);
+    if (rc < 0) return rc;
+    ingest_ = std::unique_lock<std::mutex>(f->ingest_mu);
+    snap_ = std::shared_lock<std::shared_mutex>(f->snap_mu);
+    if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+    if ((need & TIMES) && !f->live.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
+    if ((need & PLACES) && places_sharded(f, false)) {
+      g_err = std::string(name) + " places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
+      return MMP_E_STATE;
+    }
+    lease_.emplace(f);
+    if (!*lease_) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+    c = lease_->get(); ds = &f->snaps[f->cur]; lv = &f->live;
+    const size_t slot_b = (size_t)f->hs.cfg.max_models * 4;
+    if ((need & SLOTS) && c->d_model_slot.cap < slot_b) {  // filled with -1 once; every call leaves it so
+      CK(c->d_model_slot.ensure(slot_b));
+      CK(cudaMemsetAsync(c->d_model_slot.p, 0xff, c->d_model_slot.cap, c->stream));
+    }
+    return MMP_OK;
+  }
+
+ private:
+  std::unique_lock<std::mutex> ingest_;
+  std::shared_lock<std::shared_mutex> snap_;
+  std::optional<CtxLease> lease_;  // (after the locks: given back before they are released)
+};
+
+// The call's fresh row for the pod (none where fr is null) into d_fresh, and d_extra sized for n_extra excludes
+static int32_t stage_fresh_self(PlaceCtx *c, const FreshRow *fr, size_t n_extra) {
+  c->fresh_host.assign(fr ? 1 : 0, fr ? *fr : FreshRow{});
+  const int32_t rc = stage_side_tables(c, c->fresh_host.data(), (int32_t)c->fresh_host.size(), nullptr, 0, c->stream);
+  if (rc < 0) return rc;
+  CK(c->d_extra.ensure(n_extra * 4));
+  return MMP_OK;
+}
+
+// Places in[0, n) under the view v into out on the call's stream, with the fresh row and the extras stage_fresh_self staged
+static cudaError_t place_staged(mmp_fleet *f, PlaceCtx *c, const SnapshotView &v, const mmp_decision_in *in, int n,
+                                mmp_decision_out *out, int64_t now, uint64_t seed) {
+  PlaceArgs a{v, in, n, c->d_fresh.as<FreshRow>(), (int)c->fresh_host.size(), c->d_extra.as<int32_t>(), out, nullptr, nullptr, now, seed,
+              f->id_base.load()};
+  a.ctx = c;
+  return launch_place(f, a, c->stream);
+}
+
+// The end of mmp_shutdown_run and mmp_evict_run: e1, one copy back of [header | actions], the synchronise and the timer; then
+// two entries of one model are refused, or the actions and the report are written
+template <class Report, class Action>
+static int32_t pack_copy_back(PlaceCtx *c, const PackHdr<Report> *hdr, int32_t n, float &t_ms, Action *out, Report *report) {
+  CK(cudaEventRecord(c->e1, c->stream));
+  std::vector<char> back(sizeof(PackHdr<Report>) + (size_t)n * sizeof(Action));
+  CK(cudaMemcpyAsync(back.data(), hdr, back.size(), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  event_ms(c, t_ms);
+  PackHdr<Report> H;
+  memcpy(&H, back.data(), sizeof(H));
+  if (H.dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
+  if (n) memcpy(out, back.data() + sizeof(H), (size_t)n * sizeof(Action));
+  *report = H.rep;
+  return n;
+}
+
 extern "C" {
 
 int32_t mmp_scale_eval(mmp_fleet *f, const mmp_scale_in *in, int32_t n, const mmp_scale_params *params, mmp_scale_out *out) {
@@ -855,52 +965,44 @@ int32_t mmp_reaper_run(mmp_fleet *f, int32_t leader, int64_t now_ms, int64_t ass
       (repaired_cap > 0 && !repaired_models) || (loads_cap > 0 && !loads)) {
     g_err = "bad argument"; return MMP_E_ARG;
   }
-  int32_t rc = set_device(f);
-  if (rc < 0) return rc;
   // The prune reads the live registry (as registry_prune does), the selection and the placement the epoch (as mmp_reaper_select
-  // and mmp_place_batch do): ingest_mu, then snap_mu shared -- the order of a commit, which flips the epoch under snap_mu while
-  // it holds ingest_mu.  Holding both, the registry read is the one the epoch was built from.
-  std::lock_guard<std::mutex> g(f->ingest_mu);
-  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
-  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  if (places_sharded(f, false)) {
-    g_err = "mmp_reaper_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
-    return MMP_E_STATE;
-  }
-  const DeviceSnapshot &ds = f->snaps[f->cur];
+  // and mmp_place_batch do): holding both locks, the registry read is the one the epoch was built from.
+  PodCall pc;
+  int32_t rc = pc.open(f, "mmp_reaper_run", PodCall::PLACES);
+  if (rc < 0) return rc;
+  PlaceCtx *c = pc.c; const DeviceSnapshot &ds = *pc.ds; LiveState &lv = *pc.lv;
   const HostSnapshot &h = ds.host;
-  LiveState &lv = f->live;
   const int32_t NM = ds.n_models, NI = f->hs.cfg.max_instances, np = (int)h.part_types.size();
   const int tc = h.tc_enabled ? 1 : 0, ns = tc ? np : 1;
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
   cudaStream_t st = c->stream;
   RpScratch &rs = c->rp;
   const size_t nmx = (size_t)std::max(NM, 1);
   const int32_t reg_cap = NM * HostState::EDGE_INL + lv.n_ovf;  // every registration
-  CK(c->d_view.ensure(nmx * sizeof(mmp_model_row)));
-  CK(c->d_pruned.ensure((size_t)std::max(reg_cap, 1) * sizeof(PrunedReg)));
-  CK(c->d_repaired.ensure(nmx * 4));
+  // [the pruned and repaired model rows | pruned registrations | repaired models | loads (a run selects a model at most once)]
+  mmp_model_row *view; PrunedReg *d_pruned; int *d_repaired; mmp_reaper_load *d_loads;
+  rc = carve(c->d_task, [&](Carve &k) {
+    view = k.take<mmp_model_row>(nmx); d_pruned = k.take<PrunedReg>(std::max(reg_cap, 1));
+    d_repaired = k.take<int>(nmx); d_loads = k.take<mmp_reaper_load>(std::min(nmx, (size_t)loads_cap));
+  });
+  if (rc < 0) return rc;
   CK(c->d_n_open.ensure(16));
   // [missing_since (NI) | stats (np + 1) | the cluster's LRU, from Long.MAX_VALUE (ISST)]
-  const size_t acc_b = (size_t)(np + 1) * sizeof(StatsAcc);
-  CK(c->d_trace.ensure((size_t)NI * 8 + acc_b + 8));
-  long long *d_miss = c->d_trace.as<long long>();
-  StatsAcc *acc = reinterpret_cast<StatsAcc *>(d_miss + NI);
-  long long *d_min = reinterpret_cast<long long *>(reinterpret_cast<char *>(acc) + acc_b);
+  long long *d_miss, *d_min;
+  StatsAcc *acc;
+  rc = carve(c->d_trace, [&](Carve &k) { d_miss = k.take<long long>(NI); acc = k.take<StatsAcc>(np + 1); d_min = k.take<long long>(1); });
+  if (rc < 0) return rc;
   int *d_cnt = c->d_n_open.as<int>();                         // [0] pruned registrations, [1] repaired models
   int *h_cnt = reinterpret_cast<int *>(c->mapped.get());      // ... read back with the selection count (pinned)
-  mmp_model_row *view = c->d_view.as<mmp_model_row>();
   static const long long lru_init = 0x7fffffffffffffffLL;
   CK(cudaMemcpyAsync(d_miss, missing_since, (size_t)NI * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(d_cnt, 0, 8, st));
-  CK(cudaMemsetAsync(acc, 0, acc_b, st));
+  CK(cudaMemsetAsync(acc, 0, (size_t)(np + 1) * sizeof(StatsAcc), st));
   CK(cudaMemcpyAsync(d_min, &lru_init, 8, cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(c->e0, st));
   if (NM) {
     k_registry_prune<<<(NM + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.inst_meta.as<int2>(), NM, NI, leader,
-                                                      now_ms, assume_gone_ms, d_miss, 1, nullptr, nullptr, c->d_pruned.as<PrunedReg>(), reg_cap,
-                                                      d_cnt, PruneView{view, c->d_repaired.as<int>(), d_cnt + 1});
+                                                      now_ms, assume_gone_ms, d_miss, 1, nullptr, nullptr, d_pruned, reg_cap, d_cnt,
+                                                      PruneView{view, d_repaired, d_cnt + 1});
     f->launches++;
     CK(cudaGetLastError());
   }
@@ -927,22 +1029,17 @@ int32_t mmp_reaper_run(mmp_fleet *f, int32_t leader, int64_t now_ms, int64_t ass
   // the decisions, built on the device from the selections, placed as mmp_place_batch_device places a batch
   const int n_loads = std::min(n_sel, loads_cap);
   if (n_sel) {
-    if ((rc = stage_side_tables(c.get(), nullptr, 0, nullptr, 0, st)) < 0) return rc;
+    if ((rc = stage_fresh_self(c, nullptr, 1)) < 0) return rc;
     CK(c->d_in.ensure((size_t)n_sel * sizeof(mmp_decision_in)));
     CK(c->d_out.ensure((size_t)n_sel * sizeof(mmp_decision_out)));
-    CK(c->d_loads.ensure((size_t)n_sel * sizeof(mmp_reaper_load)));
     k_reaper_decisions<<<(n_sel + 255) / 256, 256, 0, st>>>(rs.sel.as<int2>(), n_sel, view, leader, c->d_in.as<mmp_decision_in>());
     f->launches++;
     CK(cudaGetLastError());
-    PlaceArgs a{ds.view, c->d_in.as<mmp_decision_in>(), n_sel, c->d_fresh.as<FreshRow>(), 0, c->d_extra.as<int32_t>(),
-                c->d_out.as<mmp_decision_out>(), nullptr, nullptr, now_ms, seed, f->id_base.load()};
-    a.ctx = c.get();
-    CK(launch_place(f, a, st));
+    CK(place_staged(f, c, ds.view, c->d_in.as<mmp_decision_in>(), n_sel, c->d_out.as<mmp_decision_out>(), now_ms, seed));
   }
   CK(cudaEventRecord(c->e1, st));
   if (n_loads) {
-    k_reaper_loads<<<(n_loads + 255) / 256, 256, 0, st>>>(c->d_in.as<mmp_decision_in>(), c->d_out.as<mmp_decision_out>(), n_loads,
-                                                         c->d_loads.as<mmp_reaper_load>());
+    k_reaper_loads<<<(n_loads + 255) / 256, 256, 0, st>>>(c->d_in.as<mmp_decision_in>(), c->d_out.as<mmp_decision_out>(), n_loads, d_loads);
     f->launches++;
     CK(cudaGetLastError());
   }
@@ -955,16 +1052,16 @@ int32_t mmp_reaper_run(mmp_fleet *f, int32_t leader, int64_t now_ms, int64_t ass
   const size_t parts_b = (size_t)ns * sizeof(RpPart), space_b = (size_t)ns * 8;
   std::vector<char> hb(parts_b + space_b + sizeof(RpPlan) + (size_t)ns * 4);
   int ncand = 0;
-  if (n_pruned) CK(cudaMemcpyAsync(regs.data(), c->d_pruned.p, regs.size() * sizeof(PrunedReg), cudaMemcpyDeviceToHost, st));
-  if (n_repaired) CK(cudaMemcpyAsync(rep.data(), c->d_repaired.p, rep.size() * 4, cudaMemcpyDeviceToHost, st));
-  if (n_loads) CK(cudaMemcpyAsync(ld.data(), c->d_loads.p, ld.size() * sizeof(mmp_reaper_load), cudaMemcpyDeviceToHost, st));
+  if (n_pruned) CK(cudaMemcpyAsync(regs.data(), d_pruned, regs.size() * sizeof(PrunedReg), cudaMemcpyDeviceToHost, st));
+  if (n_repaired) CK(cudaMemcpyAsync(rep.data(), d_repaired, rep.size() * 4, cudaMemcpyDeviceToHost, st));
+  if (n_loads) CK(cudaMemcpyAsync(ld.data(), d_loads, ld.size() * sizeof(mmp_reaper_load), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(miss.data(), d_miss, (size_t)NI * 8, cudaMemcpyDeviceToHost, st));
   if (NM) {
     CK(cudaMemcpyAsync(hb.data(), rs.plan.p, hb.size(), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(&ncand, rs.idx.as<int>() + 2 * nmx, 4, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_reaper_run_ms = ms; }
+  event_ms(c, f->t_reaper_run_ms);
   int stopped = -1;
   if (NM) {  // k_rp_walk's loop over the partitions: the first whose counts throw
     RpPlan plan;
@@ -1000,50 +1097,39 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
   if (p->scale.now - p->scale.last_check_time <= 0 || p->scale.scale_up_rpm_threshold <= 0) {
     g_err = "now must be after last_check_time and the threshold positive"; return MMP_E_ARG;
   }
-  const int32_t max_models = f->hs.cfg.max_models;
-  for (int32_t k = 0; k < n; k++)
-    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
-  int32_t rc = set_device(f);
+  int32_t rc = check_entries(f, entries, n);
   if (rc < 0) return rc;
-  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_reaper_run)
-  std::lock_guard<std::mutex> g(f->ingest_mu);
-  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
-  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  LiveState &lv = f->live;
-  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
-  const DeviceSnapshot &ds = f->snaps[f->cur];
+  PodCall pc;
+  if ((rc = pc.open(f, "mmp_janitor_run", PodCall::TIMES | PodCall::SLOTS)) < 0) return rc;
+  PlaceCtx *c = pc.c; const DeviceSnapshot &ds = *pc.ds; LiveState &lv = *pc.lv;
   const int32_t NM = ds.n_models, np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks;
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
   cudaStream_t st = c->stream;
-  const size_t slot_b = (size_t)max_models * 4;
-  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
-    CK(c->d_jslot.ensure(slot_b));
-    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
-  }
-  const size_t nx = (size_t)std::max(n, 1), hdr_b = sizeof(mmp_janitor_report) + 8 + 16;  // [report | pad | cnt[4] | edits]
-  CK(c->d_jent.ensure(nx * sizeof(mmp_janitor_entry)));
-  CK(c->d_jcand.ensure(nx * (16 + 8 + sizeof(JanitorCand))));
-  CK(c->d_jout.ensure(hdr_b + (size_t)std::max(NM, 1) * sizeof(mmp_janitor_edit)));
-  const size_t acc_b = (size_t)(np + 1) * sizeof(StatsAcc);
-  CK(c->d_trace.ensure(acc_b + 8));
-  StatsAcc *acc = c->d_trace.as<StatsAcc>();
-  long long *d_min = reinterpret_cast<long long *>(c->d_trace.as<char>() + acc_b);
-  char *out = c->d_jout.as<char>();
-  unsigned long long *keys = c->d_jcand.as<unsigned long long>();
-  int *vals = reinterpret_cast<int *>(keys + 2 * nx);
-  JanitorBufs J{c->d_jent.as<mmp_janitor_entry>(), c->d_jslot.as<int>(), reinterpret_cast<mmp_janitor_edit *>(out + hdr_b), keys, vals,
-                reinterpret_cast<JanitorCand *>(vals + 2 * nx), reinterpret_cast<int *>(out + sizeof(mmp_janitor_report) + 8),
-                reinterpret_cast<mmp_janitor_report *>(out)};
+  // [entries | keys | sorted keys | values | sorted values | candidates | report | cnt[4] | edits]: the report, the counters
+  // and the edits come back in one copy
+  const size_t nx = (size_t)std::max(n, 1);
+  JanitorBufs J{};
+  mmp_janitor_entry *d_ent; unsigned long long *skeys; int *svals;
+  rc = carve(c->d_task, [&](Carve &k) {
+    J.entries = d_ent = k.take<mmp_janitor_entry>(nx); J.keys = k.take<unsigned long long>(nx); skeys = k.take<unsigned long long>(nx);
+    J.vals = k.take<int>(nx); svals = k.take<int>(nx); J.cand = k.take<JanitorCand>(nx);
+    J.report = k.take<mmp_janitor_report>(1); J.cnt = k.take<int>(4); J.edits = k.take<mmp_janitor_edit>(std::max(NM, 1));
+  });
+  if (rc < 0) return rc;
+  J.slot = c->d_model_slot.as<int>();
   JanitorBufs Js = J;  // the same with the sorted keys and values
-  Js.keys = keys + nx; Js.vals = vals + nx;
+  Js.keys = skeys; Js.vals = svals;
+  char *out = reinterpret_cast<char *>(J.report);
+  const size_t o_cnt = reinterpret_cast<char *>(J.cnt) - out, hdr_b = reinterpret_cast<char *>(J.edits) - out;
+  StatsAcc *acc;
+  long long *d_min;
+  if ((rc = carve(c->d_trace, [&](Carve &k) { acc = k.take<StatsAcc>(np + 1); d_min = k.take<long long>(1); })) < 0) return rc;
   static const long long lru_init = 0x7fffffffffffffffLL;
-  CK(cudaMemsetAsync(acc, 0, acc_b, st));
+  CK(cudaMemsetAsync(acc, 0, (size_t)(np + 1) * sizeof(StatsAcc), st));
   CK(cudaMemcpyAsync(d_min, &lru_init, 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(J.cnt, 0, 16, st));
   if (n) {
-    CK(cudaMemcpyAsync(c->d_jent.p, entries, (size_t)n * sizeof(mmp_janitor_entry), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(keys, 0xff, (size_t)n * 8, st));
+    CK(cudaMemcpyAsync(d_ent, entries, (size_t)n * sizeof(mmp_janitor_entry), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(J.keys, 0xff, (size_t)n * 8, st));
   }
   CK(cudaEventRecord(c->e0, st));
   if (nr > 0) {  // instanceSetStats / globalLru for the scale-down
@@ -1051,7 +1137,7 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
                                                                      f->hs.cfg.min_space_units, acc, d_min, np);
     f->launches++;
   }
-  if (n) { k_janitor_index<<<(n + 255) / 256, 256, 0, st>>>(J, n); f->launches++; }
+  if (n) { k_slot_claim<<<(n + 255) / 256, 256, 0, st>>>(J.entries, n, J.slot, J.cnt + JC_DUP); f->launches++; }
   if (NM) {
     k_janitor_sweep<<<(NM + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.model_lul.as<long long>(), NM, self,
                                                       p->scale.now, p->load_failure_expiry_ms, J);
@@ -1063,14 +1149,14 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
     sp.can_remove = 1;
     k_janitor_eval<<<(n + 127) / 128, 128, 0, st>>>(scale_tables(f, ds, lv, acc, d_min, nullptr, nullptr), sp, self, (int)p->flags, J, n);
     size_t tmp = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, Js.keys, vals, Js.vals, n, 0, 64, st));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, J.keys, Js.keys, J.vals, Js.vals, n, 0, 64, st));
     CK(c->d_cub.ensure(tmp + 16));
-    CK(cub::DeviceRadixSort::SortPairs(c->d_cub.p, tmp, keys, Js.keys, vals, Js.vals, n, 0, 64, st));
+    CK(cub::DeviceRadixSort::SortPairs(c->d_cub.p, tmp, J.keys, Js.keys, J.vals, Js.vals, n, 0, 64, st));
     f->launches += 2;
   }
   k_janitor_walk<<<1, 1, 0, st>>>(Js, lv.models.as<mmp_model_row>(), p->adjusted_capacity / 20, p->scale.now);
   CK(cudaEventRecord(c->e1, st));
-  if (n) k_janitor_clear<<<(n + 255) / 256, 256, 0, st>>>(J, n);
+  if (n) k_slot_release<<<(n + 255) / 256, 256, 0, st>>>(J.entries, n, J.slot);
   f->launches += n ? 2 : 1;
   CK(cudaGetLastError());
   // one copy back: the report, the counters and the edits, as many as a pod is likely to have (twice its entries + 1024: most
@@ -1079,17 +1165,16 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
   std::vector<char> hb(hdr_b + first * sizeof(mmp_janitor_edit));
   CK(cudaMemcpyAsync(hb.data(), out, hb.size(), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_janitor_ms = ms; }
+  event_ms(c, f->t_janitor_ms);
   mmp_janitor_report r;
   int cnt[4];
   memcpy(&r, hb.data(), sizeof(r));
-  memcpy(cnt, hb.data() + sizeof(r) + 8, 16);
+  memcpy(cnt, hb.data() + o_cnt, 16);
   if (cnt[JC_DUP]) { g_err = "two entries of one model"; return MMP_E_ARG; }
   std::vector<mmp_janitor_edit> ed((size_t)r.n_edits);
   memcpy(ed.data(), hb.data() + hdr_b, std::min(ed.size(), first) * sizeof(mmp_janitor_edit));
   if (ed.size() > first)
-    CK(cudaMemcpy(ed.data() + first, out + hdr_b + first * sizeof(mmp_janitor_edit), (ed.size() - first) * sizeof(mmp_janitor_edit),
-                  cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(ed.data() + first, J.edits + first, (ed.size() - first) * sizeof(mmp_janitor_edit), cudaMemcpyDeviceToHost));
   std::sort(ed.begin(), ed.end(), [](const mmp_janitor_edit &a, const mmp_janitor_edit &b) { return a.model < b.model; });
   if (cap > 0 && r.n_edits) memcpy(edits, ed.data(), (size_t)std::min(r.n_edits, cap) * sizeof(mmp_janitor_edit));
   *report = r;
@@ -1110,61 +1195,39 @@ int32_t mmp_rate_run(mmp_fleet *f, int32_t self, const mmp_scale_in *entries, in
     g_err = "now must be after last_check_time and the threshold positive"; return MMP_E_ARG;
   }
   sp.can_remove = 0;
-  const int32_t max_models = f->hs.cfg.max_models;
-  for (int32_t k = 0; k < n; k++) {
-    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
-    if (entries[k].instance != self) { g_err = "an entry of another instance than self"; return MMP_E_ARG; }
-  }
-  FreshRow fr{};
-  if (fresh_self)
-    if (const char *m = HostState::fresh_row(*fresh_self, fr)) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
-  int32_t rc = set_device(f);
+  int32_t rc = check_entries(f, entries, n, [self](const mmp_scale_in &e) -> const char * {
+    return e.instance != self ? "an entry of another instance than self" : nullptr;
+  });
   if (rc < 0) return rc;
-  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_reaper_run)
-  std::lock_guard<std::mutex> g(f->ingest_mu);
-  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
-  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  LiveState &lv = f->live;
-  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
-  if (places_sharded(f, false)) {
-    g_err = "mmp_rate_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
-    return MMP_E_STATE;
-  }
-  const DeviceSnapshot &ds = f->snaps[f->cur];
+  FreshRow fr{};
+  if ((rc = parse_fresh_self(fresh_self, fr)) < 0) return rc;
+  PodCall pc;
+  if ((rc = pc.open(f, "mmp_rate_run", PodCall::TIMES | PodCall::PLACES | PodCall::SLOTS)) < 0) return rc;
+  PlaceCtx *c = pc.c; const DeviceSnapshot &ds = *pc.ds; LiveState &lv = *pc.lv;
+  cudaStream_t st = c->stream;
   const int32_t NI = f->hs.cfg.max_instances, fresh_idx = fresh_self ? 0 : -1;
   // the gates of MM:5646-5670, in Java long arithmetic
   const int64_t delta = (int64_t)((uint64_t)sp.now - (uint64_t)sp.last_check_time);
   const bool too_soon = (int64_t)((uint64_t)delta * 5u) < (int64_t)((uint64_t)sp.rate_check_interval_ms * 3u);
   const int gate = too_soon ? MMP_RATE_TOO_SOON : ds.host.n_ranks < 2 ? MMP_RATE_FEW_INSTANCES : n == 0 ? MMP_RATE_NO_ENTRIES : MMP_RATE_RAN;
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
-  cudaStream_t st = c->stream;
-  const size_t slot_b = (size_t)max_models * 4;
-  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
-    CK(c->d_jslot.ensure(slot_b));
-    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
-  }
   // [header | entries | k_scale_eval's results | second copies | chains' decision 0 | chains | second copies' results | heavy set]
   const size_t nx = (size_t)std::max(n, 1);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
-  const size_t o_hdr = take(sizeof(RateHdr)), o_ent = take(nx * sizeof(mmp_scale_in)), o_sout = take(nx * sizeof(mmp_scale_out));
-  const size_t o_sec = take(nx * sizeof(mmp_decision_in)), o_c0 = take(nx * sizeof(mmp_decision_in)), o_ch = take(nx * sizeof(RateChain));
-  const size_t o_sres = take(nx * sizeof(mmp_decision_out)), o_heavy = take((size_t)NI * 4);
-  CK(c->d_rate.ensure(off));
-  char *base = c->d_rate.as<char>();
-  RateBufs B{reinterpret_cast<mmp_scale_in *>(base + o_ent), reinterpret_cast<mmp_scale_out *>(base + o_sout), c->d_jslot.as<int>(),
-             reinterpret_cast<mmp_decision_in *>(base + o_sec), reinterpret_cast<mmp_decision_in *>(base + o_c0),
-             reinterpret_cast<RateChain *>(base + o_ch), nullptr, reinterpret_cast<int32_t *>(base + o_heavy),
-             reinterpret_cast<RateHdr *>(base + o_hdr)};
-  mmp_decision_out *sres = reinterpret_cast<mmp_decision_out *>(base + o_sres);
+  RateBufs B{};
+  mmp_decision_out *sres;
+  rc = carve(c->d_task, [&](Carve &k) {
+    B.hdr = k.take<RateHdr>(1); B.entries = k.take<mmp_scale_in>(nx); B.sout = k.take<mmp_scale_out>(nx);
+    B.sec = k.take<mmp_decision_in>(nx); B.c0 = k.take<mmp_decision_in>(nx); B.chains = k.take<RateChain>(nx);
+    sres = k.take<mmp_decision_out>(nx); B.heavy = k.take<int32_t>(NI);
+  });
+  if (rc < 0) return rc;
+  B.slot = c->d_model_slot.as<int>();
   RateHdr *h_hdr = reinterpret_cast<RateHdr *>(c->mapped.get());  // the one read-back before the placement (pinned)
   CK(cudaMemsetAsync(B.hdr, 0, sizeof(RateHdr), st));
   if (n) CK(cudaMemcpyAsync(const_cast<mmp_scale_in *>(B.entries), entries, (size_t)n * sizeof(mmp_scale_in), cudaMemcpyHostToDevice, st));
   if (gate != MMP_RATE_RAN) {  // nothing is evaluated; two entries of one model are still refused
     if (n) {
-      k_rate_index<<<(n + 255) / 256, 256, 0, st>>>(B, n);
-      k_rate_clear<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+      k_slot_claim<<<(n + 255) / 256, 256, 0, st>>>(B.entries, n, B.slot, &B.hdr->dup);
+      k_slot_release<<<(n + 255) / 256, 256, 0, st>>>(B.entries, n, B.slot);
       f->launches += 2;
       CK(cudaGetLastError());
       CK(cudaMemcpyAsync(h_hdr, B.hdr, sizeof(RateHdr), cudaMemcpyDeviceToHost, st));
@@ -1175,15 +1238,13 @@ int32_t mmp_rate_run(mmp_fleet *f, int32_t self, const mmp_scale_in *entries, in
     *report = mmp_rate_report{gate, 0, 0, 0, 0, 0, 0, 0};
     return 0;
   }
-  c->fresh_host.assign(fresh_self ? 1 : 0, fr);
-  if ((rc = stage_side_tables(c.get(), c->fresh_host.data(), fresh_self ? 1 : 0, nullptr, 0, st)) < 0) return rc;
-  CK(c->d_extra.ensure(((size_t)n * MMP_MAX_EXTRA + 1) * 4));
+  if ((rc = stage_fresh_self(c, fresh_self ? &fr : nullptr, (size_t)n * MMP_MAX_EXTRA + 1)) < 0) return rc;
   B.extra = c->d_extra.as<int32_t>();
   CK(cudaEventRecord(c->e0, st));
-  k_rate_index<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+  k_slot_claim<<<(n + 255) / 256, 256, 0, st>>>(B.entries, n, B.slot, &B.hdr->dup);
   f->launches++;
-  if ((rc = queue_scale_eval(f, c.get(), ds, lv, B.entries, n, sp, c->d_rate_rpm, const_cast<mmp_scale_out *>(B.sout), st)) < 0) return rc;
-  k_rate_clear<<<(n + 255) / 256, 256, 0, st>>>(B, n);
+  if ((rc = queue_scale_eval(f, c, ds, lv, B.entries, n, sp, c->d_rate_rpm, const_cast<mmp_scale_out *>(B.sout), st)) < 0) return rc;
+  k_slot_release<<<(n + 255) / 256, 256, 0, st>>>(B.entries, n, B.slot);
   k_rate_heavy<<<(NI + 255) / 256, 256, 0, st>>>(ds.rank_of.as<int32_t>(), ds.rows.as<RankRow>(), NI, self, sp.scale_up_rpm_threshold, B);
   const long long fail_since = (long long)((uint64_t)sp.now - (uint64_t)(p->load_failure_expiry_ms / 2));
   k_rate_plan<<<1, RATE_PLAN_THREADS, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), B, n, self, fail_since, fresh_idx);
@@ -1199,17 +1260,12 @@ int32_t mmp_rate_run(mmp_fleet *f, int32_t self, const mmp_scale_in *entries, in
   SnapshotView vw = ds.view;
   vw.n_extra = 1 + MMP_MAX_EXTRA * nq;
   const int64_t now = sp.now;
-  auto place = [&](const SnapshotView &v, const mmp_decision_in *in, int cnt, mmp_decision_out *res) -> cudaError_t {
-    PlaceArgs a{v, in, cnt, c->d_fresh.as<FreshRow>(), fresh_self ? 1 : 0, B.extra, res, nullptr, nullptr, now, seed, f->id_base.load()};
-    a.ctx = c.get();
-    return launch_place(f, a, st);
-  };
-  if (H.n_sec_place) CK(place(vw, B.sec, n, sres));
+  if (H.n_sec_place) CK(place_staged(f, c, vw, B.sec, n, sres, now, seed));
   if (nq) {
     CK(c->d_out.ensure((size_t)L * nq * sizeof(mmp_decision_out)));
     if (L > 1) CK(c->d_in.ensure((size_t)(L - 1) * nq * sizeof(mmp_decision_in)));
     SnapshotView xv = vw;
-    if (H.n_heavy && (rc = derive_exclude_tables_dev(f, c.get(), B.heavy, H.n_heavy, xv, st)) < 0) return rc;
+    if (H.n_heavy && (rc = derive_exclude_tables_dev(f, c, B.heavy, H.n_heavy, xv, st)) < 0) return rc;
     for (int j = 0; j < L; j++) {
       const mmp_decision_in *dj = j ? c->d_in.as<mmp_decision_in>() + (size_t)(j - 1) * nq : B.c0;
       if (j) {
@@ -1219,7 +1275,7 @@ int32_t mmp_rate_run(mmp_fleet *f, int32_t self, const mmp_scale_in *entries, in
         f->launches++;
         CK(cudaGetLastError());
       }
-      CK(place(xv, dj, nq, c->d_out.as<mmp_decision_out>() + (size_t)j * nq));
+      CK(place_staged(f, c, xv, dj, nq, c->d_out.as<mmp_decision_out>() + (size_t)j * nq, now, seed));
     }
   }
   CK(cudaEventRecord(c->e1, st));
@@ -1237,7 +1293,7 @@ int32_t mmp_rate_run(mmp_fleet *f, int32_t self, const mmp_scale_in *entries, in
     CK(cudaMemcpyAsync(res.data(), c->d_out.p, (size_t)L * nq * sizeof(mmp_decision_out), cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_rate_ms = ms; }
+  event_ms(c, f->t_rate_ms);
   // the loads in (entry, chain_pos) order; a chain whose last decision would continue and that has copies left is cut there
   std::vector<mmp_rate_load> ld;
   int n_cut = 0;
@@ -1273,54 +1329,32 @@ int32_t mmp_shutdown_run(mmp_fleet *f, int32_t self, const mmp_shutdown_entry *e
   if (self < 0 || self >= f->hs.cfg.max_instances || n < 0 || n > (1 << 24) || (n > 0 && (!entries || !out)) || !p || !report) {
     g_err = "bad argument"; return MMP_E_ARG;  // (n <= 2^24: entry r draws with id r, MMP_DF_OWN_ID's 24 bits)
   }
-  const int32_t max_models = f->hs.cfg.max_models;
-  for (int32_t k = 0; k < n; k++)
-    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
-  FreshRow fr{};
-  if (fresh_self)
-    if (const char *m = HostState::fresh_row(*fresh_self, fr)) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
-  int32_t rc = set_device(f);
+  int32_t rc = check_entries(f, entries, n);
   if (rc < 0) return rc;
-  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_rate_run)
-  std::lock_guard<std::mutex> g(f->ingest_mu);
-  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
-  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  LiveState &lv = f->live;
-  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
-  if (places_sharded(f, false)) {
-    g_err = "mmp_shutdown_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
-    return MMP_E_STATE;
-  }
-  const DeviceSnapshot &ds = f->snaps[f->cur];
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  FreshRow fr{};
+  if ((rc = parse_fresh_self(fresh_self, fr)) < 0) return rc;
+  PodCall pc;
+  if ((rc = pc.open(f, "mmp_shutdown_run", PodCall::TIMES | PodCall::PLACES | PodCall::SLOTS)) < 0) return rc;
+  PlaceCtx *c = pc.c; const DeviceSnapshot &ds = *pc.ds; LiveState &lv = *pc.lv;
   cudaStream_t st = c->stream;
-  const size_t slot_b = (size_t)max_models * 4;
-  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
-    CK(c->d_jslot.ensure(slot_b));
-    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
-  }
   // [entries | decisions | results | header | actions]: the header and the actions come back in one copy
   const size_t nx = (size_t)std::max(n, 1);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
-  const size_t o_ent = take(nx * sizeof(mmp_shutdown_entry)), o_dec = take(nx * sizeof(mmp_decision_in));
-  const size_t o_res = take(nx * sizeof(mmp_decision_out)), o_hdr = take(sizeof(SdHdr)), o_out = take(nx * sizeof(mmp_shutdown_action));
-  static_assert(sizeof(SdHdr) % 16 == 0, "the actions follow the header");
-  CK(c->d_sd.ensure(off));
-  char *base = c->d_sd.as<char>();
-  SdBufs B{reinterpret_cast<mmp_shutdown_entry *>(base + o_ent), c->d_jslot.as<int>(), reinterpret_cast<mmp_decision_in *>(base + o_dec),
-           reinterpret_cast<mmp_decision_out *>(base + o_res), reinterpret_cast<SdHdr *>(base + o_hdr),
-           reinterpret_cast<mmp_shutdown_action *>(base + o_out), nullptr};
-  c->fresh_host.assign(fresh_self ? 1 : 0, fr);
-  if ((rc = stage_side_tables(c.get(), c->fresh_host.data(), fresh_self ? 1 : 0, nullptr, 0, st)) < 0) return rc;
+  SdBufs B{};
+  rc = carve(c->d_task, [&](Carve &k) {
+    B.entries = k.take<mmp_shutdown_entry>(nx); B.dec = k.take<mmp_decision_in>(nx); B.res = k.take<mmp_decision_out>(nx);
+    B.hdr = k.take<PackHdr<mmp_shutdown_report>>(1); B.out = k.take<mmp_shutdown_action>(nx);
+  });
+  if (rc < 0) return rc;
+  B.slot = c->d_model_slot.as<int>();
+  if ((rc = stage_fresh_self(c, fresh_self ? &fr : nullptr, 1)) < 0) return rc;
   B.extra = c->d_extra.as<int32_t>();
-  CK(cudaMemsetAsync(B.hdr, 0, sizeof(SdHdr), st));
+  CK(cudaMemsetAsync(B.hdr, 0, sizeof(*B.hdr), st));
   if (n) CK(cudaMemcpyAsync(const_cast<mmp_shutdown_entry *>(B.entries), entries, (size_t)n * sizeof(mmp_shutdown_entry), cudaMemcpyHostToDevice, st));
   const int64_t now = p->now;
   const long long cutoff = (long long)((uint64_t)now - (uint64_t)p->cutoff_age_ms);
   const long long fail_since = (long long)((uint64_t)now - (uint64_t)(p->load_failure_expiry_ms / 2));
   CK(cudaEventRecord(c->e0, st));
+  // (launched at n == 0 too: block 0 writes found_other and extra[0])
   k_shutdown_plan<<<std::max((n + 255) / 256, 1), 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), ds.rank_of.as<int32_t>(),
                                                                 ds.host.n_ranks, B, n, self, cutoff, fail_since, fresh_self ? 0 : -1);
   f->launches++;
@@ -1328,25 +1362,12 @@ int32_t mmp_shutdown_run(mmp_fleet *f, int32_t self, const mmp_shutdown_entry *e
   if (n) {
     SnapshotView vw = ds.view;
     vw.n_extra = 1;
-    PlaceArgs a{vw, B.dec, n, c->d_fresh.as<FreshRow>(), fresh_self ? 1 : 0, B.extra, const_cast<mmp_decision_out *>(B.res), nullptr,
-                nullptr, now, seed, f->id_base.load()};
-    a.ctx = c.get();
-    CK(launch_place(f, a, st));
+    CK(place_staged(f, c, vw, B.dec, n, const_cast<mmp_decision_out *>(B.res), now, seed));
     k_shutdown_pack<<<(n + 255) / 256, 256, 0, st>>>(B, n, cutoff);
     f->launches++;
     CK(cudaGetLastError());
   }
-  CK(cudaEventRecord(c->e1, st));
-  std::vector<char> back(sizeof(SdHdr) + (size_t)n * sizeof(mmp_shutdown_action));
-  CK(cudaMemcpyAsync(back.data(), B.hdr, back.size(), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_shutdown_ms = ms; }
-  SdHdr H;
-  memcpy(&H, back.data(), sizeof(SdHdr));
-  if (H.dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
-  if (n) memcpy(out, back.data() + sizeof(SdHdr), (size_t)n * sizeof(mmp_shutdown_action));
-  *report = H.rep;
-  return n;
+  return pack_copy_back(c, B.hdr, n, f->t_shutdown_ms, out, report);
 }
 
 int32_t mmp_evict_run(mmp_fleet *f, int32_t self, const mmp_evict_entry *entries, int32_t n, const mmp_evict_params *p,
@@ -1355,81 +1376,45 @@ int32_t mmp_evict_run(mmp_fleet *f, int32_t self, const mmp_evict_entry *entries
   if (self < 0 || self >= f->hs.cfg.max_instances || n < 0 || n > (1 << 24) || (n > 0 && (!entries || !out)) || !p || !report) {
     g_err = "bad argument"; return MMP_E_ARG;  // (n <= 2^24: entry r draws with id r, MMP_DF_OWN_ID's 24 bits)
   }
-  const int32_t max_models = f->hs.cfg.max_models;
-  for (int32_t k = 0; k < n; k++)
-    if (entries[k].model < 0 || entries[k].model >= max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
-  FreshRow fr{};
-  if (fresh_self)
-    if (const char *m = HostState::fresh_row(*fresh_self, fr)) { g_err = std::string("fresh row: ") + m; return MMP_E_ARG; }
-  int32_t rc = set_device(f);
+  int32_t rc = check_entries(f, entries, n);
   if (rc < 0) return rc;
-  // the registry as of the last commit and the epoch it was built into: ingest_mu, then snap_mu shared (as mmp_shutdown_run)
-  std::lock_guard<std::mutex> g(f->ingest_mu);
-  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
-  if (f->epoch == 0 || !f->live.valid) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
-  LiveState &lv = f->live;
-  if (!lv.have_times) { g_err = "the committed registry has no registration times (mmp_model_times)"; return MMP_E_STATE; }
-  if (places_sharded(f, false)) {
-    g_err = "mmp_evict_run places on an unsharded fleet without a communicator (elsewhere placement is a collective call)";
-    return MMP_E_STATE;
-  }
-  const DeviceSnapshot &ds = f->snaps[f->cur];
-  CtxLease c(f);
-  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  FreshRow fr{};
+  if ((rc = parse_fresh_self(fresh_self, fr)) < 0) return rc;
+  PodCall pc;
+  if ((rc = pc.open(f, "mmp_evict_run", PodCall::TIMES | PodCall::PLACES | PodCall::SLOTS)) < 0) return rc;
+  PlaceCtx *c = pc.c; const DeviceSnapshot &ds = *pc.ds; LiveState &lv = *pc.lv;
   cudaStream_t st = c->stream;
-  const size_t slot_b = (size_t)max_models * 4;
-  if (c->d_jslot.cap < slot_b) {  // filled with -1 once; every call leaves it so
-    CK(c->d_jslot.ensure(slot_b));
-    CK(cudaMemsetAsync(c->d_jslot.p, 0xff, c->d_jslot.cap, st));
-  }
   // [entries | decisions | results | header | actions]: the header and the actions come back in one copy
   const size_t nx = (size_t)std::max(n, 1);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
-  const size_t o_ent = take(nx * sizeof(mmp_evict_entry)), o_dec = take(nx * sizeof(mmp_decision_in));
-  const size_t o_res = take(nx * sizeof(mmp_decision_out)), o_hdr = take(sizeof(EvHdr)), o_out = take(nx * sizeof(mmp_evict_action));
-  static_assert(sizeof(EvHdr) % 16 == 0, "the actions follow the header");
-  CK(c->d_ev.ensure(off));
-  char *base = c->d_ev.as<char>();
-  EvBufs B{reinterpret_cast<mmp_evict_entry *>(base + o_ent), c->d_jslot.as<int>(), reinterpret_cast<mmp_decision_in *>(base + o_dec),
-           reinterpret_cast<mmp_decision_out *>(base + o_res), reinterpret_cast<EvHdr *>(base + o_hdr),
-           reinterpret_cast<mmp_evict_action *>(base + o_out), nullptr};
-  c->fresh_host.assign(fresh_self ? 1 : 0, fr);
-  if ((rc = stage_side_tables(c.get(), c->fresh_host.data(), fresh_self ? 1 : 0, nullptr, 0, st)) < 0) return rc;
+  EvBufs B{};
+  rc = carve(c->d_task, [&](Carve &k) {
+    B.entries = k.take<mmp_evict_entry>(nx); B.dec = k.take<mmp_decision_in>(nx); B.res = k.take<mmp_decision_out>(nx);
+    B.hdr = k.take<PackHdr<mmp_evict_report>>(1); B.out = k.take<mmp_evict_action>(nx);
+  });
+  if (rc < 0) return rc;
+  B.slot = c->d_model_slot.as<int>();
+  if ((rc = stage_fresh_self(c, fresh_self ? &fr : nullptr, 1)) < 0) return rc;
   B.extra = c->d_extra.as<int32_t>();
-  CK(cudaMemsetAsync(B.hdr, 0, sizeof(EvHdr), st));
+  CK(cudaMemsetAsync(B.hdr, 0, sizeof(*B.hdr), st));
   if (n) CK(cudaMemcpyAsync(const_cast<mmp_evict_entry *>(B.entries), entries, (size_t)n * sizeof(mmp_evict_entry), cudaMemcpyHostToDevice, st));
   const int64_t now = p->now;
   const long long reload_age = (long long)(2u * (uint64_t)p->load_timeout_ms);
   const long long fail_since = (long long)((uint64_t)now - (uint64_t)(p->load_failure_expiry_ms / 2));
   CK(cudaEventRecord(c->e0, st));
-  if (n) {
+  if (n) {  // (nothing at n == 0, the type-set stats included)
     TypeSetStats S;
-    if ((rc = queue_type_stats(f, c.get(), ds, lv, S, st)) < 0) return rc;
+    if ((rc = queue_type_stats(f, c, ds, lv, S, st)) < 0) return rc;
     k_evict_plan<<<(n + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.model_lul.as<long long>(),
                                                   ds.rank_of.as<int32_t>(), S.types, lv.n_type_ids, B, n, self, now, reload_age, fail_since,
                                                   fresh_self ? 0 : -1);
     SnapshotView vw = ds.view;
     vw.n_extra = 1;
-    PlaceArgs a{vw, B.dec, n, c->d_fresh.as<FreshRow>(), fresh_self ? 1 : 0, B.extra, const_cast<mmp_decision_out *>(B.res), nullptr,
-                nullptr, now, seed, f->id_base.load()};
-    a.ctx = c.get();
-    CK(launch_place(f, a, st));
+    CK(place_staged(f, c, vw, B.dec, n, const_cast<mmp_decision_out *>(B.res), now, seed));
     k_evict_pack<<<(n + 255) / 256, 256, 0, st>>>(B, n);
     f->launches += 2;
     CK(cudaGetLastError());
   }
-  CK(cudaEventRecord(c->e1, st));
-  std::vector<char> back(sizeof(EvHdr) + (size_t)n * sizeof(mmp_evict_action));
-  CK(cudaMemcpyAsync(back.data(), B.hdr, back.size(), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_evict_ms = ms; }
-  EvHdr H;
-  memcpy(&H, back.data(), sizeof(EvHdr));
-  if (H.dup) { g_err = "two entries of one model"; return MMP_E_ARG; }
-  if (n) memcpy(out, back.data() + sizeof(EvHdr), (size_t)n * sizeof(mmp_evict_action));
-  *report = H.rep;
-  return n;
+  return pack_copy_back(c, B.hdr, n, f->t_evict_ms, out, report);
 }
 
 }  // extern "C"

@@ -76,7 +76,7 @@ static int32_t run_stats(mmp_fleet *f, const DeviceSnapshot &ds, StatsResult &re
   CK(cudaMemcpyAsync(acc.data(), c->d_trace.p, (size_t)(np + 1) * sizeof(StatsAcc), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaMemcpyAsync(&mn, d_min, 8, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_stats_ms = ms; }
+  event_ms(c.get(), f->t_stats_ms);
   res.parts.resize(np + 1);
   for (int i = 0; i <= np; i++) {
     mmp_cluster_stats &s = res.parts[i];
@@ -968,8 +968,7 @@ int32_t mmp_reaper_select(mmp_fleet *f, int32_t partition, int64_t now_ms, uint8
   const bool counted = rp_counts(part, space, now_ms, free_count, total, cutoff);
   if (counted && total <= 0) return 0;
   auto timed = [&](int32_t r) {  // t_reaper_ms: from the candidate sweep to the last stage run
-    float ms = 0;
-    if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_reaper_ms = ms;
+    event_ms(c.get(), f->t_reaper_ms);
     return r;
   };
   // the candidates: those of the base rule alone when the size estimate is 0 (the reference throws only when there is one,
@@ -1104,7 +1103,7 @@ static int32_t lru_apply_impl(mmp_fleet *f, const mmp_lru_event *ev, int32_t n, 
   CK(cudaMemcpyAsync(hdr, c->d_trace.p, 8, cudaMemcpyDeviceToHost, s));
   if (status) CK(cudaMemcpyAsync(status, c->d_trace.as<char>() + 16, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) f->t_lru_ms = ms; }
+  event_ms(c.get(), f->t_lru_ms);
   if (hdr[1]) { g_err = "LRU slot capacity exceeded for some instance (raise slots_per_instance)"; return MMP_E_NOMEM; }
   int got = std::min(hdr[0], cap);
   std::vector<EvictRec> tmp((size_t)got);
@@ -1184,7 +1183,7 @@ int32_t mmp_lru_read(mmp_fleet *f, const int32_t *instances, int32_t n, int64_t 
   CK(cudaMemcpyAsync(off.data(), d_off, n1 * 8, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   float ms_count = 0;
-  if (cudaEventElapsedTime(&ms_count, c->e0, c->e1) != cudaSuccess) ms_count = 0;
+  event_ms(c.get(), ms_count);
   const int64_t total = off[n], written = std::min(total, cap);
   // the walks longer than the shared-memory path holds, among those that start before cap: one segment each
   std::vector<int32_t> big;
@@ -1226,7 +1225,8 @@ int32_t mmp_lru_read(mmp_fleet *f, const int32_t *instances, int32_t n, int64_t 
     CK(cudaMemcpyAsync(out, d_out, (size_t)written * sizeof(mmp_lru_entry), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     float ms = 0;
-    if (cudaEventElapsedTime(&ms, c->e0, c->e1) == cudaSuccess) ms_count += ms;
+    event_ms(c.get(), ms);
+    ms_count += ms;
   }
   f->t_lru_read_ms = ms_count;
   std::memcpy(offsets, off.data(), n1 * 8);
