@@ -578,6 +578,87 @@ typedef struct {
 typedef struct { int32_t n_referencing, n_edits, n_candidates, n_removed; int64_t weight_removed; } mmp_janitor_report;
 int32_t mmp_janitor_run(mmp_fleet *, int32_t self, const mmp_janitor_entry *entries, int32_t n, const mmp_janitor_params *p,
                         mmp_janitor_edit *edits, int32_t cap, mmp_janitor_report *report);
+/* One run of one pod's whole janitor task (janitorTask MM:5876-6145) against the committed epoch and the registry as of the
+ * last commit, in one call: the cache pass over the pod's cache (MM:5892-6008), then mmp_janitor_run's registry pass on the
+ * records the cache pass left.  entries[] is runtimeCache.descendingMap() (MM:5892) after removeUnloadBufferEntry, IN THAT
+ * ORDER (most recently used first), at most one entry per model.  In Java long arithmetic, now = p->janitor.scale.now,
+ * window = janitor_freq_secs * 2000 + load_timeout_ms (MM:5933-5934); a "record" is the committed one (no record: the model
+ * index is at or past the committed model count, a model never upserted).  Per entry, in order:
+ *   skips       MMP_JANITOR_NOT_DONE: MMP_JC_NOT_DONE.  last_used <= 0: MMP_JC_NOT_CACHED.  Nothing else (MM:5905-5912).
+ *   order       the entries past the skips "qualify": one whose last_used > the previous qualifying one's (Long.MAX_VALUE
+ *               before the first) gets MMP_JC_OUT_OF_ORDER, the log line of MM:5913-5917.
+ *   stop        the first qualifying entry with last_used == Long.MAX_VALUE (quirk N16): MMP_JC_STOP, the pod force-sets its
+ *               cache entry's lastUsed to out[r].last_used = now - 3 x 3 600 000 (LASTUSED_AGE_ON_ADD_MS); MMP_JC_REPAIR where
+ *               the record's lastUsed is Long.MAX_VALUE (repairLastUsedTimeIfNeeded MM:6837-6850: the record gets the same
+ *               value).  The task ends there (`return`, MM:5929): every later entry is MMP_JC_NOT_REACHED alone, no registry
+ *               pass runs (report.registry_ran = 0, its report zero, no edits).
+ *   recent      now - last_used < window: the stale update where there is a record (MM:5933-5939).
+ *   stale       updateLastUsedTimeInRegistryIfStale (MM:6165-6183): last_used - rec.lastUsed >= min_stale_age_ms writes the
+ *               record's lastUsed, raised to last_used as updateLastUsed does (MR:239-246): MMP_JC_STALE_UPDATE.
+ *   check       otherwise (MM:5941-5997), over every registration of the model (the overflow ones included):
+ *                 undecided   a copy_count saturated at 255 over more than 255 registrations (as MMP_JE_UNDECIDED):
+ *                             MMP_JC_UNDECIDED, nothing written; the pod runs the loop body for that entry itself
+ *                 matched     the pod's first failed registration's time == load_complete_ts (an MMP_JANITOR_FAILED
+ *                             entry), else its first loaded registration's time == load_ts: the stale update
+ *                 remove      no record, MMP_JANITOR_NOT_LIVE or MMP_JANITOR_UNLOAD_RECENT: MMP_JC_REMOVE, ce.remove()
+ *                 re-register otherwise MMP_JC_REREGISTER: instanceIds.put(self, load_ts), removeLoadFailure(self),
+ *                             updateLastUsed(last_used) (MM:5980-5982); out[r].replaced_ts is the pod's loaded registration
+ *                             time it replaced (not for a failed entry, as regLoadTimestamp), -1 where there was none.
+ * out[r] is entries[r]'s action in entry order: the OR of its MMP_JC_* bits and last_used, the record's lastUsed after the
+ * cache pass (its own where nothing was written, 0 without a record), or for MMP_JC_STOP the forced cache value.
+ * The registry pass is mmp_janitor_run's on the same entries, with two differences: a record the cache pass wrote is read as
+ * written (a re-registered model has the pod among its loaded copies at load_ts, one more loaded copy where the pod was not
+ * loaded, and no failure record of the pod; a raised lastUsed), and an entry the cache pass removed reads last_used = -1
+ * (getLastUsedTime of a key no longer in the cache, MM:6045, 6068, 6094) while its MMP_JANITOR_FAILED stays as given.
+ * Edits come back in model order, as mmp_janitor_run's.
+ * Epoch batching: one now for both loops (the reference reads the clock at MM:5899 and MM:6018); registry.get and getStrong
+ * both read the committed record; every conditional write, forceSetLastUsedTime and ce.remove() of the cache pass succeeds,
+ * and the registry pass sees them.  Not modelled (stays in the pod): shuttingDown, verifyKvStoreConnection, the unload-buffer
+ * step, the KV writes and their retry, publishInstanceRecordAsync (report.cache_changed) and the log lines (INTEGRATION.md §8).
+ * Returns the number of edits.  Errors (nothing written): MMP_E_ARG for self outside [0, max_instances), an entry's model out of
+ * range or two entries of one model, n < 0 or n > 2^24, p or report NULL, out NULL with n > 0, edits NULL with cap > 0, or a
+ * p->janitor mmp_janitor_run refuses; MMP_E_EPOCH without a commit; MMP_E_STATE when the committed registry holds no
+ * registration times.  Sets the "janitor_task" timing. */
+#define MMP_JANITOR_NOT_DONE 2u            /* !ce.isDone(): still loading (MM:5905) */
+#define MMP_JANITOR_NOT_LIVE 4u            /* ce.state < CacheEntry.LOADING || ce.state > CacheEntry.ACTIVE (MM:5968) */
+#define MMP_JANITOR_UNLOAD_RECENT 8u       /* ce.unloadAttemptedRecently() (MM:5969) */
+typedef struct {
+  mmp_janitor_entry e;                     /* as mmp_janitor_run reads it; flags MMP_JANITOR_FAILED | the bits above */
+  int64_t load_complete_ts;                /* ce.loadCompleteTimestamp (a failed entry's registration time, MM:5952) */
+} mmp_janitor_task_entry;                  /* 56 B */
+typedef struct {
+  mmp_janitor_params janitor;              /* as mmp_janitor_run reads them */
+  int64_t min_stale_age_ms;                /* minStaleAge (MM:6162): the pod draws it once, 6 h + a random hour */
+  int64_t janitor_freq_secs;               /* LOCAL_JANITOR_FREQ_SECS (MM:235) */
+  int64_t load_timeout_ms;                 /* loadTimeoutMs */
+} mmp_janitor_task_params;                 /* 120 B */
+#define MMP_JC_NOT_DONE      1u   /* skipped: still loading */
+#define MMP_JC_NOT_CACHED    2u   /* skipped: last_used <= 0 */
+#define MMP_JC_OUT_OF_ORDER  4u   /* last_used above the previous qualifying entry's: log it */
+#define MMP_JC_STOP          8u   /* Long.MAX_VALUE last_used: forceSetLastUsedTime(out.last_used); the task ends here */
+#define MMP_JC_REPAIR       16u   /* with MMP_JC_STOP: the record's lastUsed was Long.MAX_VALUE, set it to out.last_used */
+#define MMP_JC_NOT_REACHED  32u   /* after the stop: alone, nothing done */
+#define MMP_JC_STALE_UPDATE 64u   /* conditionalSet of the record with lastUsed = out.last_used */
+#define MMP_JC_REMOVE      128u   /* ce.remove() */
+#define MMP_JC_REREGISTER  256u   /* put self at load_ts, removeLoadFailure(self), lastUsed = out.last_used; conditionalSetAndGet */
+#define MMP_JC_UNDECIDED   512u   /* copy_count saturated at 255 over > 255 registrations: nothing decided */
+typedef struct {
+  int32_t model; uint32_t what;            /* model; the OR of MMP_JC_* */
+  int64_t last_used;                       /* the record's lastUsed after the cache pass, or the forced cache value (MMP_JC_STOP) */
+  int64_t replaced_ts;                     /* MMP_JC_REREGISTER: the registration time it replaced, -1 for none; else -1 */
+} mmp_janitor_cache_action;                /* 24 B */
+typedef struct {
+  int32_t n_not_done, n_not_cached, n_out_of_order, n_stop, n_repair;  /* entries with each MMP_JC_* bit, in bit order */
+  int32_t n_not_reached, n_stale_update, n_remove, n_reregister, n_undecided;
+  int32_t stopped_at;                      /* the MMP_JC_STOP entry, -1 for none */
+  int32_t registry_ran;                    /* 1: the registry pass ran (no stop) */
+  int32_t cache_changed;                   /* some ce.remove(): the pod calls publishInstanceRecordAsync (MM:6002-6004) */
+  int32_t reserved;
+  mmp_janitor_report registry;             /* the registry pass's, zero where it did not run */
+} mmp_janitor_task_report;                 /* 80 B */
+int32_t mmp_janitor_task(mmp_fleet *, int32_t self, const mmp_janitor_task_entry *entries, int32_t n,
+                         const mmp_janitor_task_params *p, mmp_janitor_cache_action *out, mmp_janitor_edit *edits, int32_t cap,
+                         mmp_janitor_task_report *report);
 /* One run of one pod's rate-tracking task (rateTrackingTask MM:5619-5858) against the committed epoch and the registry as of
  * the last commit, in one call: the loop body of every cache entry and the loads it triggers, placed.  entries[] is the
  * pod's runtimeCache as the loop reads it, every entry's instance == self, at most one entry per model, in any order.
@@ -827,7 +908,7 @@ int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
  * sweep through the selection, k_rp_flag to k_rp_pick, without the stats and plan), mmp_lru_apply ("lru_apply": the event kernel), mmp_lru_read ("lru_read": count, scan and emit kernels) on
  * this fleet; "commit": host-clock ms of the last commit; "prune": mmp_registry_prune / mmp_registry_prune_ids;
  * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel; "janitor_run": mmp_janitor_run from its stats
- * kernel to its budget walk; "rate_run": mmp_rate_run from its stats kernel to its last placement round; "shutdown_run":
+ * kernel to its budget walk; "janitor_task": mmp_janitor_task from its cache-pass plan kernel to its budget walk; "rate_run": mmp_rate_run from its stats kernel to its last placement round; "shutdown_run":
  * mmp_shutdown_run from its index kernel to its pack kernel; "evict_run": mmp_evict_run from its stats kernel to its pack kernel;
  * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);

@@ -154,6 +154,13 @@ public final class GpuPlacement implements AutoCloseable {
         return check(MmPlace.janitorRun(h, self, entries, n, params, edits, cap, report));
     }
 
+    // one run of this pod's whole janitor task (ModelMesh.java:5876-6145): the cache pass over entries (most recently used
+    // first), an action per entry in out, then the registry loop on the records it left; returns the number of edits
+    public int janitorTask(int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer out, ByteBuffer edits, int cap,
+                           ByteBuffer report) {
+        return check(MmPlace.janitorTask(h, self, entries, n, params, out, edits, cap, report));
+    }
+
     // one run of this pod's rate-tracking task (ModelMesh.java:5619-5858): returns the number of loads; report gets the gate
     // and the totals.  freshSelf may be null
     public int rateRun(int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, ByteBuffer out, ByteBuffer loads,

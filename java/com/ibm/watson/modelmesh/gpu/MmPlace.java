@@ -52,6 +52,9 @@ final class MmPlace {
     // the registry loop of one pod's janitor task (MM:6013-6145): stale registrations, expired failures, budgeted scale-down
     static native int janitorRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer edits, int cap,
                                  ByteBuffer report);
+    // one run of one pod's whole janitor task (MM:5876-6145): the cache pass, then the registry loop on the records it left
+    static native int janitorTask(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer out, ByteBuffer edits,
+                                  int cap, ByteBuffer report);
     // one run of one pod's rate-tracking task (MM:5619-5858): second copies, scale-up chains under the heavy-instance set (mmp_rate_run)
     static native int rateRun(long h, int self, ByteBuffer entries, int n, ByteBuffer params, ByteBuffer freshSelf, long seed,
                               ByteBuffer out, ByteBuffer loads, int loadsCap, ByteBuffer report);

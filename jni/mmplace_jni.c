@@ -157,6 +157,15 @@ jint FN(janitorRun)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, 
   return mmp_janitor_run(H(h), self, (const mmp_janitor_entry *)BUF(entries), n, (const mmp_janitor_params *)BUF(params),
                          (mmp_janitor_edit *)BUF(edits), cap, (mmp_janitor_report *)BUF(report));
 }
+/* one run of one pod's whole janitor task.  entries: n x mmp_janitor_task_entry (56 B) most recently used first, params: one
+ * mmp_janitor_task_params (120 B), out: n x mmp_janitor_cache_action (24 B), edits: cap x mmp_janitor_edit (24 B), report: one
+ * mmp_janitor_task_report (80 B) -- direct buffers */
+jint FN(janitorTask)(JNIEnv *env, jclass c, jlong h, jint self, jobject entries, jint n, jobject params, jobject out, jobject edits,
+                     jint cap, jobject report) {
+  (void)c;
+  return mmp_janitor_task(H(h), self, (const mmp_janitor_task_entry *)BUF(entries), n, (const mmp_janitor_task_params *)BUF(params),
+                          (mmp_janitor_cache_action *)BUF(out), (mmp_janitor_edit *)BUF(edits), cap, (mmp_janitor_task_report *)BUF(report));
+}
 /* one run of one pod's rate-tracking task.  entries: n x mmp_scale_in (48 B), params: one mmp_rate_params (80 B), freshSelf:
  * one mmp_instance_row (64 B) or null, out: n x mmp_scale_out (40 B), loads: loadsCap x mmp_rate_load (40 B), report: one
  * mmp_rate_report (32 B) -- direct buffers */

@@ -66,6 +66,14 @@ JANITOR_PARAMS = np.dtype([("scale", SCALE_PARAMS), ("load_failure_expiry_ms", "
                            ("reserved", "<u4")], align=True)
 JANITOR_EDIT = np.dtype([("model", "<i4"), ("what", "<u4"), ("last_used", "<i8"), ("last_unload_time", "<i8")], align=True)
 assert JANITOR_ENTRY.itemsize == 48 and JANITOR_PARAMS.itemsize == 96 and JANITOR_EDIT.itemsize == 24
+JANITOR_NOT_DONE, JANITOR_NOT_LIVE, JANITOR_UNLOAD_RECENT = 2, 4, 8
+JANITOR_TASK_ENTRY = np.dtype([("e", JANITOR_ENTRY), ("load_complete_ts", "<i8")], align=True)
+JANITOR_TASK_PARAMS = np.dtype([("janitor", JANITOR_PARAMS), ("min_stale_age_ms", "<i8"), ("janitor_freq_secs", "<i8"),
+                                ("load_timeout_ms", "<i8")], align=True)
+JANITOR_CACHE_ACTION = np.dtype([("model", "<i4"), ("what", "<u4"), ("last_used", "<i8"), ("replaced_ts", "<i8")], align=True)
+assert JANITOR_TASK_ENTRY.itemsize == 56 and JANITOR_TASK_PARAMS.itemsize == 120 and JANITOR_CACHE_ACTION.itemsize == 24
+JC_NOT_DONE, JC_NOT_CACHED, JC_OUT_OF_ORDER, JC_STOP, JC_REPAIR = 1, 2, 4, 8, 16
+JC_NOT_REACHED, JC_STALE_UPDATE, JC_REMOVE, JC_REREGISTER, JC_UNDECIDED = 32, 64, 128, 256, 512
 RATE_PARAMS = np.dtype([("scale", SCALE_PARAMS), ("load_failure_expiry_ms", "<i8")], align=True)
 RATE_LOAD = np.dtype([("entry", "<i4"), ("model", "<i4"), ("chain_pos", "<i4"), ("self", "<i4"), ("target", "<i4"), ("n_candidates", "<i4"),
                       ("last_used", "<i8"), ("flags", "<u4"), ("remaining", "<u4")], align=True)
@@ -109,6 +117,16 @@ class ReaperReport(C.Structure):
 class JanitorReport(C.Structure):
     _fields_ = [("n_referencing", C.c_int32), ("n_edits", C.c_int32), ("n_candidates", C.c_int32), ("n_removed", C.c_int32),
                 ("weight_removed", C.c_int64)]
+
+
+class JanitorTaskReport(C.Structure):
+    _fields_ = [("n_not_done", C.c_int32), ("n_not_cached", C.c_int32), ("n_out_of_order", C.c_int32), ("n_stop", C.c_int32),
+                ("n_repair", C.c_int32), ("n_not_reached", C.c_int32), ("n_stale_update", C.c_int32), ("n_remove", C.c_int32),
+                ("n_reregister", C.c_int32), ("n_undecided", C.c_int32), ("stopped_at", C.c_int32), ("registry_ran", C.c_int32),
+                ("cache_changed", C.c_int32), ("reserved", C.c_int32), ("registry", JanitorReport)]
+
+
+assert C.sizeof(JanitorTaskReport) == 80
 
 
 class RateReport(C.Structure):
@@ -190,6 +208,7 @@ SYMBOLS = [
     ("mmp_reaper_select", _I32, [_P, _I32, _I64, _P, _P, _I32]),
     ("mmp_reaper_run", _I32, [_P, _I32, _I64, _I64, _P, _U64, _P, _P, _I32, _P, _I32, _P, _I32, C.c_void_p]),
     ("mmp_janitor_run", _I32, [_P, _I32, _P, _I32, _P, _P, _I32, C.c_void_p]),
+    ("mmp_janitor_task", _I32, [_P, _I32, _P, _I32, _P, _P, _P, _I32, C.c_void_p]),
     ("mmp_rate_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, _P, _I32, C.c_void_p]),
     ("mmp_shutdown_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, C.c_void_p]),
     ("mmp_evict_run", _I32, [_P, _I32, _P, _I32, _P, _P, _U64, _P, C.c_void_p]),

@@ -1327,6 +1327,7 @@ struct mmp_fleet {
   float t_lru_read_ms = 0;      // ... and of the last mmp_lru_read (its count + scan part plus its emit part)
   float t_reaper_run_ms = 0;    // ... and of the last mmp_reaper_run (its prune sweep to its last placement kernel)
   float t_janitor_ms = 0;       // ... and of the last mmp_janitor_run (its stats kernel to its budget walk)
+  float t_janitor_task_ms = 0;  // ... and of the last mmp_janitor_task (its cache-pass plan kernel to its budget walk)
   float t_rate_ms = 0;          // ... and of the last mmp_rate_run that ran the task (its stats kernel to its last placement round)
   float t_shutdown_ms = 0;      // ... and of the last mmp_shutdown_run (its index kernel to its pack kernel)
   float t_evict_ms = 0;         // ... and of the last mmp_evict_run (its stats kernel to its pack kernel)
@@ -2391,6 +2392,7 @@ int32_t mmp_last_timing(mmp_fleet *f, const char *key, double *ms) {
   else if (!strcmp(key, "prune")) *ms = f->t_prune_ms;
   else if (!strcmp(key, "reaper_run")) *ms = f->t_reaper_run_ms;
   else if (!strcmp(key, "janitor_run")) *ms = f->t_janitor_ms;
+  else if (!strcmp(key, "janitor_task")) *ms = f->t_janitor_task_ms;
   else if (!strcmp(key, "rate_run")) *ms = f->t_rate_ms;
   else if (!strcmp(key, "shutdown_run")) *ms = f->t_shutdown_ms;
   else if (!strcmp(key, "evict_run")) *ms = f->t_evict_ms;

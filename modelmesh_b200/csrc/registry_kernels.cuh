@@ -62,10 +62,12 @@ __device__ __forceinline__ int exclude_set_max_rpm(int thr, int our_rpm) {
 
 // removeModelCopies (MM:6197-6335) with canRemove = true for `instance`'s copy of `model` (who-drops-the-copy by PLACEMENT_ORDER
 // MM:6314-6335 included): k_scale_eval's scale-down and the janitor's registry pass (k_janitor_eval) both run it.  g / loaded:
-// the model's registrations and how many of them are loaded copies; self_rank: `instance`'s rank in the snapshot (-1: none)
+// the model's registrations and how many of them are loaded copies; self_rank: `instance`'s rank in the snapshot (-1: none).
+// rereg (mmp_janitor_task's registry pass): the cache pass re-registered `instance` at rereg_ts; `added` of the loaded copies
+// are that registration, past the committed ones (0 where it replaced the time of `instance`'s committed copy)
 __device__ __forceinline__ bool scale_down_removes(const ScaleTables &T, const mmp_scale_params &p, int instance, int model, long long last_used,
                                                    long long last_heavy, long long count, int flags, const ModelRegs &g, int loaded,
-                                                   int self_rank) {
+                                                   int self_rank, bool rereg = false, long long rereg_ts = 0, int added = 0) {
   long long ts;
   if (last_used == 0 || loaded < 2) return false;
   // instanceSetStats(): the local instance's partition with type constraints, else the cluster (MM:1440-1446, TCM:236-239)
@@ -80,7 +82,7 @@ __device__ __forceinline__ bool scale_down_removes(const ScaleTables &T, const m
   // the first other copy in instance-ID order that is in the table and not shutting down (MM:6236-6245)
   int other = -1;
   unsigned best_id = 0xffffffffu;
-  for (int j = 0; j < loaded; j++) {
+  for (int j = 0; j < loaded - added; j++) {
     const int i = reg_at(T.R, g, j, ts);
     if (i < 0 || i == instance || T.rank_of[i] < 0) continue;
     const unsigned idr = T.inst_tie[i].x;
@@ -103,9 +105,9 @@ __device__ __forceinline__ bool scale_down_removes(const ScaleTables &T, const m
   }
   const long long lul = T.model_lul ? T.model_lul[model] : 0;
   if (lul > 0 && jsub(p.now, lul) < jmul64(8, p.rate_check_interval_ms)) return false;
-  bool recent = false;
-  for (int j = 0; j < loaded; j++) {
-    reg_at(T.R, g, j, ts);
+  bool recent = rereg && added && rereg_ts > jsub(p.now, 1800000LL);
+  for (int j = 0; j < loaded - added; j++) {
+    if (reg_at(T.R, g, j, ts) == instance && rereg) ts = rereg_ts;
     if (ts > jsub(p.now, 1800000LL)) recent = true;
   }
   if (recent) return false;
@@ -349,8 +351,13 @@ __global__ void k_slot_release(const Entry *entries, int n, int *slot) {
 // slot[] (k_slot_claim); a second entry of one model is reported through cnt[JC_DUP].
 enum { JC_EDITS = 0, JC_CANDS = 1, JC_REFS = 2, JC_DUP = 3 };
 struct JanitorCand { int model, entry, edit, removes; long long reg_ts; };  // reg_ts: the time of self's loaded registration
+// mmp_janitor_task: a model's record as the cache pass left it, per entry beside the entry's slot -- its lastUsed, and where
+// the pass re-registered the pod, self's loaded registration time and whether it added a loaded copy
+struct JanitorOv { long long last_used, reg_ts; int rereg, added; };
 struct JanitorBufs {
   const mmp_janitor_entry *entries; int *slot;
+  const JanitorOv *ov;                 // mmp_janitor_task: per entry (NULL for mmp_janitor_run: the committed records)
+  const int *halt;                     // mmp_janitor_task: nonzero when the cache pass stopped (no registry pass)
   mmp_janitor_edit *edits;             // one per model at most, in no order
   unsigned long long *keys; int *vals; // candidate keys (last_used; ~0 past the candidates) and their JanitorCand index
   JanitorCand *cand;
@@ -365,16 +372,23 @@ __device__ __forceinline__ void dereg_record_edit(bool unregistered, bool use_lu
   if (unregistered) lul = cc - 1 <= 2 ? 0 : now;
   if (use_lu && lu > lu_rec) lu_rec = lu;
 }
+// the record of entry k's model as the registry pass reads it: the cache pass's (J.ov) where there is one, else the committed
+__device__ __forceinline__ JanitorOv janitor_record(const JanitorBufs &J, const mmp_model_row &mr, int k) {
+  return J.ov && k >= 0 ? J.ov[k] : JanitorOv{mr.last_used, 0, 0, 0};
+}
 // one thread per model record, in the shape of k_registry_prune: self's loaded and failed registrations, remLoaded / remFailed
 // (MM:6028-6053), the record changes of the edit (MM:6059-6073), REMOVE_LOCAL (MM:6089-6091) and the scale-down candidates
 // (MM:6092-6100) with their last_used as the key
 __global__ void k_janitor_sweep(RegTables R, const mmp_model_row *__restrict__ models, const long long *__restrict__ model_lul, int n_models,
                                 int self, long long now, long long expiry_ms, JanitorBufs J) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= n_models) return;
+  if (m >= n_models || (J.halt && *J.halt)) return;
   const mmp_model_row mr = models[m];
-  const int n_regs = (int)mr.reserved, cc = mr.copy_count;
-  if (n_regs == 0) return;
+  const int n_regs = (int)mr.reserved;
+  const int k_ov = J.ov ? J.slot[m] : -1;
+  const JanitorOv rec = janitor_record(J, mr, k_ov);  // (a re-registration may give a model its first registration)
+  if (n_regs == 0 && !rec.rereg) return;
+  const int cc = mr.copy_count + rec.added;
   const ModelRegs g = model_regs(R, m, mr.reserved);
   int loaded_pos = -1;
   bool failed = false;
@@ -382,17 +396,18 @@ __global__ void k_janitor_sweep(RegTables R, const mmp_model_row *__restrict__ m
   for (int j = 0; j < n_regs; j++) {
     long long ts;
     if (reg_at(R, g, j, ts) != self) continue;
-    if (j < cc) { if (loaded_pos < 0) { loaded_pos = j; loaded_ts = ts; } }
+    if (j < mr.copy_count) { if (loaded_pos < 0) { loaded_pos = j; loaded_ts = ts; } }
     else if (!failed) { failed = true; failed_ts = ts; }
   }
+  if (rec.rereg) { loaded_pos = max(loaded_pos, 0); loaded_ts = rec.reg_ts; failed = false; }  // (put, removeLoadFailure)
   if (loaded_pos < 0 && !failed) return;
   atomicAdd(&J.cnt[JC_REFS], 1);
   const long long lul0 = model_lul[m];
   if (loaded_copies(mr) < 0) {  // where the loaded copies end is unknown (mmp_scale_eval's -1)
-    J.edits[atomicAdd(&J.cnt[JC_EDITS], 1)] = mmp_janitor_edit{m, MMP_JE_UNDECIDED, mr.last_used, lul0};
+    J.edits[atomicAdd(&J.cnt[JC_EDITS], 1)] = mmp_janitor_edit{m, MMP_JE_UNDECIDED, rec.last_used, lul0};
     return;
   }
-  const int k = J.slot[m];
+  const int k = J.ov ? k_ov : J.slot[m];
   mmp_janitor_entry ce{};
   if (k >= 0) ce = J.entries[k];
   const bool has = k >= 0, ce_failed = has && (ce.flags & MMP_JANITOR_FAILED), loaded = loaded_pos >= 0;
@@ -408,7 +423,7 @@ __global__ void k_janitor_sweep(RegTables R, const mmp_model_row *__restrict__ m
     }
   }
   unsigned what = 0;
-  int64_t lu_rec = mr.last_used, lul = lul0;
+  int64_t lu_rec = rec.last_used, lul = lul0;
   if (rem_loaded || rem_failed) {
     if (rem_loaded) what |= MMP_JE_UNREGISTER;
     if (rem_failed) what |= MMP_JE_DROP_FAILURE;
@@ -433,8 +448,10 @@ __global__ void k_janitor_eval(ScaleTables T, mmp_scale_params p, int self, int 
   const mmp_janitor_entry ce = J.entries[x.entry];
   const mmp_model_row mr = T.models[x.model];
   const ModelRegs g = model_regs(T.R, x.model, mr.reserved);
-  const int loaded = loaded_copies(mr);  // (>= 0: k_janitor_sweep makes no candidate of a saturated record)
-  J.cand[c].removes = scale_down_removes(T, p, self, x.model, ce.last_used, ce.last_heavy, ce.count, flags, g, loaded, T.rank_of[self]) &&
+  const JanitorOv rec = janitor_record(J, mr, x.entry);
+  const int loaded = loaded_copies(mr) + rec.added;  // (>= 0: k_janitor_sweep makes no candidate of a saturated record)
+  J.cand[c].removes = scale_down_removes(T, p, self, x.model, ce.last_used, ce.last_heavy, ce.count, flags, g, loaded, T.rank_of[self],
+                                         rec.rereg, rec.reg_ts, rec.added) &&
                       x.reg_ts == ce.load_ts;
 }
 // one thread: the TreeSet(VALUE_COMP) over the sorted candidates (of an equal-last_used run the first model in index order,
@@ -456,13 +473,138 @@ __global__ void k_janitor_walk(JanitorBufs J, const mmp_model_row *__restrict__ 
     budget -= ce.weight;
     weight_removed += ce.weight;
     // the async removal's record changes (MM:6363-6365) on the record after this run's edit of it
-    const int cc = models[x.model].copy_count;
+    const mmp_model_row mr = models[x.model];
+    const JanitorOv rec = janitor_record(J, mr, x.entry);
+    const int cc = mr.copy_count + rec.added;
     mmp_janitor_edit &e = x.edit >= 0 ? J.edits[x.edit] : J.edits[n_edits++];
-    if (x.edit < 0) e = mmp_janitor_edit{x.model, 0u, models[x.model].last_used, 0};
+    if (x.edit < 0) e = mmp_janitor_edit{x.model, 0u, rec.last_used, 0};
     e.what |= MMP_JE_SCALE_DOWN;
     dereg_record_edit(true, true, ce.last_used, cc, now, e.last_used, e.last_unload_time);
   }
   *J.report = mmp_janitor_report{J.cnt[JC_REFS], n_edits, kept, removed, weight_removed};
+}
+
+// mmp_janitor_task's cache pass (MM:5892-6008).  k_jt_plan gives every entry the action the loop would take if it reached
+// the entry, the registry pass's copy of it (last_used -1 where it is removed) and its record after the action (JanitorOv,
+// read beside the entry's slot); k_jt_order (one block, in entry order) adds the out-of-order scan and cuts the entries
+// past the stop.  JtHdr.stop: the first qualifying Long.MAX_VALUE entry (atomicMin from 0x7f7f7f7f, > 2^24: none);
+// halt: the registry pass does not run.  The header, the counters and the actions come back in one copy.
+struct JtHdr { mmp_janitor_task_report rep; int stop, halt, pad[2]; };
+static_assert(sizeof(JtHdr) == 96, "the counters follow the header");
+constexpr long long JT_LONG_MAX = 0x7fffffffffffffffLL;
+// updateLastUsedTimeInRegistryIfStale (MM:6165-6183; last_used is never Long.MAX_VALUE here) on the record rec
+__device__ __forceinline__ void jt_stale_update(long long lu, long long min_stale, JanitorOv &rec, unsigned &what) {
+  if (jsub(lu, rec.last_used) < min_stale) return;
+  what |= MMP_JC_STALE_UPDATE;
+  if (lu > rec.last_used) rec.last_used = lu;  // updateLastUsed (MR:239-246)
+}
+// one thread per entry: the loop body of MM:5904-5997 past the out-of-order log line
+__global__ void k_jt_plan(RegTables R, const mmp_model_row *__restrict__ models, int n_models, const mmp_janitor_task_entry *__restrict__ te,
+                          int n, int self, long long now, long long window, long long min_stale, mmp_janitor_entry *__restrict__ ent,
+                          JanitorOv *__restrict__ ov, mmp_janitor_cache_action *__restrict__ out, JtHdr *__restrict__ hdr) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  mmp_janitor_entry e = te[r].e;
+  const long long lu = e.last_used;
+  const bool has_rec = e.model < n_models;  // registry.get / getStrong: the committed record, none for a model never upserted
+  const mmp_model_row mr = has_rec ? models[e.model] : mmp_model_row{};
+  JanitorOv rec{mr.last_used, 0, 0, 0};
+  unsigned what = 0;
+  long long shown = 0, replaced = -1;
+  if (e.flags & MMP_JANITOR_NOT_DONE) {
+    what = MMP_JC_NOT_DONE;
+  } else if (lu <= 0) {
+    what = MMP_JC_NOT_CACHED;
+  } else if (lu == JT_LONG_MAX) {  // forceSetLastUsedTime, repairLastUsedTimeIfNeeded and the task's return (quirk N16)
+    what = MMP_JC_STOP;
+    shown = jsub(now, 3LL * 3600000LL);
+    if (has_rec && mr.last_used == JT_LONG_MAX) { what |= MMP_JC_REPAIR; rec.last_used = shown; }
+    atomicMin(&hdr->stop, r);
+  } else if (jsub(now, lu) < window) {  // new or recently used
+    if (has_rec) jt_stale_update(lu, min_stale, rec, what);
+  } else if (has_rec && loaded_copies(mr) < 0) {
+    what = MMP_JC_UNDECIDED;
+  } else {
+    // the pod's first loaded and first failed registration, as k_janitor_sweep finds them
+    bool loaded_at = false, failed_at = false;
+    long long loaded_ts = 0, failed_ts = 0;
+    if (has_rec) {
+      const ModelRegs g = model_regs(R, e.model, mr.reserved);
+      for (int j = 0; j < (int)mr.reserved; j++) {
+        long long ts;
+        if (reg_at(R, g, j, ts) != self) continue;
+        if (j < mr.copy_count) { if (!loaded_at) { loaded_at = true; loaded_ts = ts; } }
+        else if (!failed_at) { failed_at = true; failed_ts = ts; }
+      }
+    }
+    const bool failed = e.flags & MMP_JANITOR_FAILED;
+    if (has_rec && (failed ? failed_at && failed_ts == te[r].load_complete_ts : loaded_at && loaded_ts == e.load_ts)) {
+      jt_stale_update(lu, min_stale, rec, what);
+    } else if (!has_rec || (e.flags & (MMP_JANITOR_NOT_LIVE | MMP_JANITOR_UNLOAD_RECENT))) {
+      what = MMP_JC_REMOVE;
+      e.last_used = -1;  // getLastUsedTime of a key no longer in the cache (MM:6045, 6068, 6094)
+    } else {  // instanceIds.put(self, loadTimestamp), removeLoadFailure(self), updateLastUsed(lastUsed)
+      what = MMP_JC_REREGISTER;
+      if (!failed && loaded_at) replaced = loaded_ts;
+      rec = JanitorOv{max(rec.last_used, lu), e.load_ts, 1, loaded_at ? 0 : 1};
+    }
+  }
+  ent[r] = e;
+  ov[r] = rec;
+  out[r] = mmp_janitor_cache_action{e.model, what, (what & MMP_JC_STOP) ? shown : rec.last_used, replaced};
+}
+// One block over the entries in order, a tile of JT_ORDER_THREADS at a time: lastLastUsed (MM:5900, 5913-5917) is the
+// last_used of the previous qualifying entry, found by an exclusive max-scan of the qualifying indices; the entries past the
+// stop are not reached (their record's own lastUsed); the counts per bit and the report's flags
+constexpr int JT_ORDER_THREADS = 512;
+struct JtMax { __device__ __forceinline__ int operator()(int a, int b) const { return a > b ? a : b; } };
+__global__ void __launch_bounds__(JT_ORDER_THREADS) k_jt_order(const mmp_janitor_task_entry *__restrict__ te, int n,
+                                                               const mmp_model_row *__restrict__ models, int n_models,
+                                                               mmp_janitor_cache_action *__restrict__ out, JtHdr *__restrict__ hdr) {
+  using Scan = cub::BlockScan<int, JT_ORDER_THREADS>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ int carry, cnt[10];
+  if (threadIdx.x < 10) cnt[threadIdx.x] = 0;
+  if (threadIdx.x == 0) carry = -1;
+  __syncthreads();
+  const int stop = hdr->stop;
+  for (int base = 0; base < n; base += JT_ORDER_THREADS) {
+    const int r = base + threadIdx.x;
+    int q = -1;
+    long long lu = 0;
+    if (r < n) {
+      const mmp_janitor_entry e = te[r].e;
+      lu = e.last_used;
+      if (!(e.flags & MMP_JANITOR_NOT_DONE) && lu > 0) q = r;
+    }
+    const int before = carry;
+    int prev, tile_max;
+    Scan(tmp).ExclusiveScan(q, prev, before, JtMax(), tile_max);
+    if (r < n) {
+      mmp_janitor_cache_action a = out[r];
+      if (r > stop) {
+        a = mmp_janitor_cache_action{a.model, MMP_JC_NOT_REACHED, a.model < n_models ? models[a.model].last_used : 0, -1};
+        out[r] = a;
+      } else if (q >= 0 && prev >= 0 && lu > te[prev].e.last_used) {
+        a.what |= MMP_JC_OUT_OF_ORDER;
+        out[r].what = a.what;
+      }
+#pragma unroll
+      for (int b = 0; b < 10; b++)
+        if (a.what & (1u << b)) atomicAdd(&cnt[b], 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) carry = max(before, tile_max);
+    __syncthreads();
+  }
+  if (threadIdx.x < 10) (&hdr->rep.n_not_done)[threadIdx.x] = cnt[threadIdx.x];
+  if (threadIdx.x == 0) {
+    const bool stopped = stop < n;
+    hdr->rep.stopped_at = stopped ? stop : -1;
+    hdr->rep.registry_ran = !stopped;
+    hdr->rep.cache_changed = cnt[7] > 0;  // MMP_JC_REMOVE
+    hdr->halt = stopped;
+  }
 }
 
 // Lays a call's scratch out in one device buffer: take<T>(n) hands out room for n T's, each 16-byte aligned after the one
@@ -807,10 +949,13 @@ __global__ void k_evict_pack(EvBufs B, int n) {
 // the host steps the pod-task calls share: mmp_reaper_run, mmp_janitor_run, mmp_rate_run, mmp_shutdown_run, mmp_evict_run
 // ---------------------------------------------------------------------------------------------------------------
 // MMP_E_ARG for the first entry whose model index is out of range or that `also` refuses (a message, else null)
+template <class Entry> static int32_t entry_model(const Entry &e) { return e.model; }
+static int32_t entry_model(const mmp_janitor_task_entry &e) { return e.e.model; }
 template <class Entry, class Also>
 static int32_t check_entries(const mmp_fleet *f, const Entry *entries, int32_t n, Also also) {
   for (int32_t k = 0; k < n; k++) {
-    if (entries[k].model < 0 || entries[k].model >= f->hs.cfg.max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
+    const int32_t m = entry_model(entries[k]);
+    if (m < 0 || m >= f->hs.cfg.max_models) { g_err = "entry model index out of range"; return MMP_E_ARG; }
     if (const char *m = also(entries[k])) { g_err = m; return MMP_E_ARG; }
   }
   return MMP_OK;
@@ -897,6 +1042,56 @@ static int32_t pack_copy_back(PlaceCtx *c, const PackHdr<Report> *hdr, int32_t n
   if (n) memcpy(out, back.data() + sizeof(H), (size_t)n * sizeof(Action));
   *report = H.rep;
   return n;
+}
+
+// mmp_janitor_run's and mmp_janitor_task's registry pass, queued on the call's stream once the pod's entries are on the
+// device: the stats (into acc / d_min, cleared by the caller), the slot claim, the sweep, the candidates' eval and sort, the
+// budget walk (e1 is recorded after it) and the slot release
+static int32_t queue_janitor_pass(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, LiveState &lv, const JanitorBufs &J, const JanitorBufs &Js,
+                                  int32_t n, int32_t self, const mmp_janitor_params &p, StatsAcc *acc, long long *d_min) {
+  const int32_t NM = ds.n_models, np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks;
+  cudaStream_t st = c->stream;
+  if (nr > 0) {  // instanceSetStats / globalLru for the scale-down
+    k_stats<<<std::min(f->sm_count, (nr + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(), ds.part_of_rank.as<int32_t>(), nr,
+                                                                     f->hs.cfg.min_space_units, acc, d_min, np);
+    f->launches++;
+  }
+  if (n) { k_slot_claim<<<(n + 255) / 256, 256, 0, st>>>(J.entries, n, J.slot, J.cnt + JC_DUP); f->launches++; }
+  if (NM) {
+    k_janitor_sweep<<<(NM + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.model_lul.as<long long>(), NM, self,
+                                                      p.scale.now, p.load_failure_expiry_ms, J);
+    f->launches++;
+  }
+  CK(cudaGetLastError());
+  if (n) {  // the candidates (at most one per entry) by ascending last_used; eval before the sort reads them by JanitorCand index
+    mmp_scale_params sp = p.scale;
+    sp.can_remove = 1;
+    k_janitor_eval<<<(n + 127) / 128, 128, 0, st>>>(scale_tables(f, ds, lv, acc, d_min, nullptr, nullptr), sp, self, (int)p.flags, J, n);
+    size_t tmp = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, J.keys, Js.keys, J.vals, Js.vals, n, 0, 64, st));
+    CK(c->d_cub.ensure(tmp + 16));
+    CK(cub::DeviceRadixSort::SortPairs(c->d_cub.p, tmp, J.keys, Js.keys, J.vals, Js.vals, n, 0, 64, st));
+    f->launches += 2;
+  }
+  k_janitor_walk<<<1, 1, 0, st>>>(Js, lv.models.as<mmp_model_row>(), p.adjusted_capacity / 20, p.scale.now);
+  CK(cudaEventRecord(c->e1, st));
+  if (n) k_slot_release<<<(n + 255) / 256, 256, 0, st>>>(J.entries, n, J.slot);
+  f->launches += n ? 2 : 1;
+  CK(cudaGetLastError());
+  return MMP_OK;
+}
+// the edits the first copy back brings: as many as a pod is likely to have (twice its entries + 1024: most edits are of
+// models the pod holds); more take a second copy (janitor_edits_out)
+static size_t janitor_first_edits(int32_t NM, int32_t n) { return (size_t)std::min<int64_t>(std::max(NM, 1), 2 * (int64_t)n + 1024); }
+// the n_edits edits in model order into edits[0, cap): the first `first` from the copy back at hb, the rest from the device
+static int32_t janitor_edits_out(const JanitorBufs &J, const char *hb, size_t first, int32_t n_edits, mmp_janitor_edit *edits, int32_t cap) {
+  std::vector<mmp_janitor_edit> ed((size_t)n_edits);
+  memcpy(ed.data(), hb, std::min(ed.size(), first) * sizeof(mmp_janitor_edit));
+  if (ed.size() > first)
+    CK(cudaMemcpy(ed.data() + first, J.edits + first, (ed.size() - first) * sizeof(mmp_janitor_edit), cudaMemcpyDeviceToHost));
+  std::sort(ed.begin(), ed.end(), [](const mmp_janitor_edit &a, const mmp_janitor_edit &b) { return a.model < b.model; });
+  if (cap > 0 && n_edits) memcpy(edits, ed.data(), (size_t)std::min(n_edits, cap) * sizeof(mmp_janitor_edit));
+  return MMP_OK;
 }
 
 extern "C" {
@@ -1102,7 +1297,7 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
   PodCall pc;
   if ((rc = pc.open(f, "mmp_janitor_run", PodCall::TIMES | PodCall::SLOTS)) < 0) return rc;
   PlaceCtx *c = pc.c; const DeviceSnapshot &ds = *pc.ds; LiveState &lv = *pc.lv;
-  const int32_t NM = ds.n_models, np = (int)ds.host.part_types.size(), nr = ds.host.n_ranks;
+  const int32_t NM = ds.n_models, np = (int)ds.host.part_types.size();
   cudaStream_t st = c->stream;
   // [entries | keys | sorted keys | values | sorted values | candidates | report | cnt[4] | edits]: the report, the counters
   // and the edits come back in one copy
@@ -1132,36 +1327,9 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
     CK(cudaMemsetAsync(J.keys, 0xff, (size_t)n * 8, st));
   }
   CK(cudaEventRecord(c->e0, st));
-  if (nr > 0) {  // instanceSetStats / globalLru for the scale-down
-    k_stats<<<std::min(f->sm_count, (nr + 255) / 256), 256, 0, st>>>(ds.rows.as<RankRow>(), ds.cap_col.as<int64_t>(), ds.part_of_rank.as<int32_t>(), nr,
-                                                                     f->hs.cfg.min_space_units, acc, d_min, np);
-    f->launches++;
-  }
-  if (n) { k_slot_claim<<<(n + 255) / 256, 256, 0, st>>>(J.entries, n, J.slot, J.cnt + JC_DUP); f->launches++; }
-  if (NM) {
-    k_janitor_sweep<<<(NM + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), lv.model_lul.as<long long>(), NM, self,
-                                                      p->scale.now, p->load_failure_expiry_ms, J);
-    f->launches++;
-  }
-  CK(cudaGetLastError());
-  if (n) {  // the candidates (at most one per entry) by ascending last_used; eval before the sort reads them by JanitorCand index
-    mmp_scale_params sp = p->scale;
-    sp.can_remove = 1;
-    k_janitor_eval<<<(n + 127) / 128, 128, 0, st>>>(scale_tables(f, ds, lv, acc, d_min, nullptr, nullptr), sp, self, (int)p->flags, J, n);
-    size_t tmp = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, J.keys, Js.keys, J.vals, Js.vals, n, 0, 64, st));
-    CK(c->d_cub.ensure(tmp + 16));
-    CK(cub::DeviceRadixSort::SortPairs(c->d_cub.p, tmp, J.keys, Js.keys, J.vals, Js.vals, n, 0, 64, st));
-    f->launches += 2;
-  }
-  k_janitor_walk<<<1, 1, 0, st>>>(Js, lv.models.as<mmp_model_row>(), p->adjusted_capacity / 20, p->scale.now);
-  CK(cudaEventRecord(c->e1, st));
-  if (n) k_slot_release<<<(n + 255) / 256, 256, 0, st>>>(J.entries, n, J.slot);
-  f->launches += n ? 2 : 1;
-  CK(cudaGetLastError());
-  // one copy back: the report, the counters and the edits, as many as a pod is likely to have (twice its entries + 1024: most
-  // edits are of models the pod holds); more take a second copy
-  const size_t first = (size_t)std::min<int64_t>(std::max(NM, 1), 2 * (int64_t)n + 1024);
+  if ((rc = queue_janitor_pass(f, c, ds, lv, J, Js, n, self, *p, acc, d_min)) < 0) return rc;
+  // one copy back: the report, the counters and the first edits
+  const size_t first = janitor_first_edits(NM, n);
   std::vector<char> hb(hdr_b + first * sizeof(mmp_janitor_edit));
   CK(cudaMemcpyAsync(hb.data(), out, hb.size(), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -1171,14 +1339,89 @@ int32_t mmp_janitor_run(mmp_fleet *f, int32_t self, const mmp_janitor_entry *ent
   memcpy(&r, hb.data(), sizeof(r));
   memcpy(cnt, hb.data() + o_cnt, 16);
   if (cnt[JC_DUP]) { g_err = "two entries of one model"; return MMP_E_ARG; }
-  std::vector<mmp_janitor_edit> ed((size_t)r.n_edits);
-  memcpy(ed.data(), hb.data() + hdr_b, std::min(ed.size(), first) * sizeof(mmp_janitor_edit));
-  if (ed.size() > first)
-    CK(cudaMemcpy(ed.data() + first, J.edits + first, (ed.size() - first) * sizeof(mmp_janitor_edit), cudaMemcpyDeviceToHost));
-  std::sort(ed.begin(), ed.end(), [](const mmp_janitor_edit &a, const mmp_janitor_edit &b) { return a.model < b.model; });
-  if (cap > 0 && r.n_edits) memcpy(edits, ed.data(), (size_t)std::min(r.n_edits, cap) * sizeof(mmp_janitor_edit));
+  if ((rc = janitor_edits_out(J, hb.data() + hdr_b, first, r.n_edits, edits, cap)) < 0) return rc;
   *report = r;
   return r.n_edits;
+}
+
+int32_t mmp_janitor_task(mmp_fleet *f, int32_t self, const mmp_janitor_task_entry *entries, int32_t n, const mmp_janitor_task_params *p,
+                         mmp_janitor_cache_action *out, mmp_janitor_edit *edits, int32_t cap, mmp_janitor_task_report *report) {
+  NEED(f);
+  if (self < 0 || self >= f->hs.cfg.max_instances || n < 0 || n > (1 << 24) || (n > 0 && (!entries || !out)) || !p || !report || cap < 0 ||
+      (cap > 0 && !edits)) {
+    g_err = "bad argument"; return MMP_E_ARG;
+  }
+  const mmp_janitor_params &jp = p->janitor;
+  if (jp.scale.now - jp.scale.last_check_time <= 0 || jp.scale.scale_up_rpm_threshold <= 0) {
+    g_err = "now must be after last_check_time and the threshold positive"; return MMP_E_ARG;
+  }
+  int32_t rc = check_entries(f, entries, n);
+  if (rc < 0) return rc;
+  PodCall pc;
+  if ((rc = pc.open(f, "mmp_janitor_task", PodCall::TIMES | PodCall::SLOTS)) < 0) return rc;
+  PlaceCtx *c = pc.c; const DeviceSnapshot &ds = *pc.ds; LiveState &lv = *pc.lv;
+  const int32_t NM = ds.n_models, np = (int)ds.host.part_types.size();
+  cudaStream_t st = c->stream;
+  // [task entries | the registry pass's entries | their records | keys | sorted keys | values | sorted values | candidates |
+  //  header | cnt[4] | actions | edits]: the header, the counters, the actions and the edits come back in one copy
+  const size_t nx = (size_t)std::max(n, 1);
+  JanitorBufs J{};
+  mmp_janitor_task_entry *d_te; mmp_janitor_entry *d_ent; JanitorOv *d_ov; unsigned long long *skeys; int *svals;
+  JtHdr *hdr; mmp_janitor_cache_action *d_out;
+  rc = carve(c->d_task, [&](Carve &k) {
+    d_te = k.take<mmp_janitor_task_entry>(nx); J.entries = d_ent = k.take<mmp_janitor_entry>(nx); J.ov = d_ov = k.take<JanitorOv>(nx);
+    J.keys = k.take<unsigned long long>(nx); skeys = k.take<unsigned long long>(nx);
+    J.vals = k.take<int>(nx); svals = k.take<int>(nx); J.cand = k.take<JanitorCand>(nx);
+    hdr = k.take<JtHdr>(1); J.cnt = k.take<int>(4); d_out = k.take<mmp_janitor_cache_action>(nx); J.edits = k.take<mmp_janitor_edit>(std::max(NM, 1));
+  });
+  if (rc < 0) return rc;
+  J.slot = c->d_model_slot.as<int>();
+  J.report = &hdr->rep.registry;
+  J.halt = &hdr->halt;
+  JanitorBufs Js = J;  // the same with the sorted keys and values
+  Js.keys = skeys; Js.vals = svals;
+  char *back = reinterpret_cast<char *>(hdr);
+  const size_t o_cnt = reinterpret_cast<char *>(J.cnt) - back, o_out = reinterpret_cast<char *>(d_out) - back,
+               hdr_b = reinterpret_cast<char *>(J.edits) - back;
+  StatsAcc *acc;
+  long long *d_min;
+  if ((rc = carve(c->d_trace, [&](Carve &k) { acc = k.take<StatsAcc>(np + 1); d_min = k.take<long long>(1); })) < 0) return rc;
+  static const long long lru_init = 0x7fffffffffffffffLL;
+  CK(cudaMemsetAsync(acc, 0, (size_t)(np + 1) * sizeof(StatsAcc), st));
+  CK(cudaMemcpyAsync(d_min, &lru_init, 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(hdr, 0, sizeof(JtHdr) + 16, st));  // (and cnt)
+  CK(cudaMemsetAsync(&hdr->stop, 0x7f, 4, st));
+  if (n) {
+    CK(cudaMemcpyAsync(d_te, entries, (size_t)n * sizeof(mmp_janitor_task_entry), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(J.keys, 0xff, (size_t)n * 8, st));
+  }
+  // the window of MM:5933-5934 in Java long arithmetic
+  const long long window = (long long)((uint64_t)p->janitor_freq_secs * 2000u + (uint64_t)p->load_timeout_ms);
+  CK(cudaEventRecord(c->e0, st));
+  if (n) {
+    k_jt_plan<<<(n + 255) / 256, 256, 0, st>>>(reg_tables(lv), lv.models.as<mmp_model_row>(), NM, d_te, n, self, jp.scale.now, window,
+                                               p->min_stale_age_ms, d_ent, d_ov, d_out, hdr);
+    f->launches++;
+  }
+  k_jt_order<<<1, JT_ORDER_THREADS, 0, st>>>(d_te, n, lv.models.as<mmp_model_row>(), NM, d_out, hdr);
+  f->launches++;
+  CK(cudaGetLastError());
+  if ((rc = queue_janitor_pass(f, c, ds, lv, J, Js, n, self, jp, acc, d_min)) < 0) return rc;
+  const size_t first = janitor_first_edits(NM, n);
+  std::vector<char> hb(hdr_b + first * sizeof(mmp_janitor_edit));
+  CK(cudaMemcpyAsync(hb.data(), back, hb.size(), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  event_ms(c, f->t_janitor_task_ms);
+  JtHdr H;
+  int cnt[4];
+  memcpy(&H, hb.data(), sizeof(H));
+  memcpy(cnt, hb.data() + o_cnt, 16);
+  if (cnt[JC_DUP]) { g_err = "two entries of one model"; return MMP_E_ARG; }
+  const int32_t n_edits = H.rep.registry.n_edits;
+  if ((rc = janitor_edits_out(J, hb.data() + hdr_b, first, n_edits, edits, cap)) < 0) return rc;
+  if (n) memcpy(out, hb.data() + o_out, (size_t)n * sizeof(mmp_janitor_cache_action));
+  *report = H.rep;
+  return n_edits;
 }
 
 

@@ -13,10 +13,10 @@ import numpy as np
 
 from . import _lib
 from ._lib import (CHURN_DECISION, CHURN_EVENT, CHURN_EVICTION, CHURN_REAPER, CLUSTER_STATS, DECISION_IN, DECISION_OUT,
-                   DECISION_TRACE, EVICT_ACTION, EVICT_ENTRY, EVICT_PARAMS, EVICTION, INSTANCE_ROW, JANITOR_EDIT, JANITOR_ENTRY,
-                   JANITOR_PARAMS, LRU_ENTRY, LRU_EVENT, MODEL_ROW, RATE_LOAD, RATE_PARAMS, REAPER_LOAD, SCALE_IN, SCALE_OUT,
-                   SHUTDOWN_ACTION, SHUTDOWN_ENTRY, SHUTDOWN_PARAMS, ChurnConfig, ChurnReport, EvictReport, JanitorReport, MmpConfig,
-                   RateReport, ReaperReport, ShutdownReport)
+                   DECISION_TRACE, EVICT_ACTION, EVICT_ENTRY, EVICT_PARAMS, EVICTION, INSTANCE_ROW, JANITOR_CACHE_ACTION, JANITOR_EDIT,
+                   JANITOR_ENTRY, JANITOR_PARAMS, JANITOR_TASK_ENTRY, JANITOR_TASK_PARAMS, LRU_ENTRY, LRU_EVENT, MODEL_ROW, RATE_LOAD,
+                   RATE_PARAMS, REAPER_LOAD, SCALE_IN, SCALE_OUT, SHUTDOWN_ACTION, SHUTDOWN_ENTRY, SHUTDOWN_PARAMS, ChurnConfig,
+                   ChurnReport, EvictReport, JanitorReport, JanitorTaskReport, MmpConfig, RateReport, ReaperReport, ShutdownReport)
 
 
 class MmpError(RuntimeError):
@@ -374,6 +374,22 @@ class Fleet:
             if cap is not None or r.n_edits <= room:
                 return edits[:min(r.n_edits, room)].copy(), r
             room = r.n_edits
+
+    def janitor_task(self, self_idx: int, entries: np.ndarray, params: np.ndarray, cap: Optional[int] = None):
+        """mmp_janitor_task, one run of one pod's whole janitor task: (out (JANITOR_CACHE_ACTION per entry), edits
+        (JANITOR_EDIT records, model order), report).  entries: JANITOR_TASK_ENTRY records of the pod's cache, most recently used
+        first; params: one JANITOR_TASK_PARAMS record.  The edits hold the first min(n_edits, cap); without a cap every edit."""
+        assert entries.dtype == JANITOR_TASK_ENTRY and params.dtype == JANITOR_TASK_PARAMS and entries.flags.c_contiguous
+        room = 2 * len(entries) + 1024 if cap is None else cap
+        while True:
+            out = np.zeros(len(entries), dtype=JANITOR_CACHE_ACTION)
+            edits = np.zeros(max(room, 1), dtype=JANITOR_EDIT)
+            r = JanitorTaskReport()
+            self._ck(self.lib.mmp_janitor_task(self.h, self_idx, _ptr(entries), len(entries), _ptr(params), _ptr(out), _ptr(edits), room,
+                                               C.byref(r)))
+            if cap is not None or r.registry.n_edits <= room:
+                return out, edits[:min(r.registry.n_edits, room)].copy(), r
+            room = r.registry.n_edits
 
     def rate_run(self, self_idx: int, entries: np.ndarray, params: np.ndarray, seed: int, fresh_self: Optional[np.ndarray] = None,
                  loads_cap: Optional[int] = None):
