@@ -25,7 +25,8 @@ import numpy as np
 
 from modelmesh_b200 import _lib as L
 from oracle import binding as ob
-from rate_run_oracle import jdiv, jlong, refused, saturated
+from common import jdiv, jlong
+from rate_run_oracle import refused, saturated
 
 REPORT_KEYS = ("n_unregister", "n_drop_failure", "n_reload", "n_cluster_full", "n_loaded_elsewhere", "n_refused", "n_placed")
 BITS = (L.EV_UNREGISTER, L.EV_DROP_FAILURE, L.EV_RELOAD, L.EV_CLUSTER_FULL, L.EV_LOADED_ELSEWHERE, L.EV_REFUSED, L.EV_PLACED)

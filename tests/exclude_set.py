@@ -4,7 +4,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from modelmesh_b200.synth import SplitMix
+from modelmesh_b200.synth import SplitMix, SynthDecisions
 
 from helpers import oracle_inputs_fast
 from request_model import oracle_inputs_request
@@ -83,3 +83,16 @@ def rs_retry_type(s, fl):
             return t, free, flagged
     raise AssertionError("no type with flagged and unflagged candidates")
 
+
+def compact(sd, n):
+    """the first n decisions with only the fresh rows and extras they use (a small call's own side tables)"""
+    dec = sd.dec[:n].copy()
+    fr = dec["fresh"] >= 0
+    fresh = sd.fresh[dec["fresh"][fr]] if len(sd.fresh) else sd.fresh[:0]
+    dec["fresh"][fr] = np.arange(int(fr.sum()))
+    slices = [sd.extra[a:a + b] for a, b in zip(dec["extra_off"], dec["extra_n"])]
+    off = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum([len(x) for x in slices], out=off[1:])
+    dec["extra_off"] = off[:-1]
+    extra = np.concatenate(slices).astype(np.int32) if n else np.zeros(0, dtype=np.int32)
+    return SynthDecisions(dec, fresh, extra)

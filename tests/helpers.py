@@ -1,24 +1,31 @@
 """Shared test plumbing: feed one SynthFleet to the oracle and to a solver, then compare decision by decision."""
 from __future__ import annotations
 
+import socket
+
 import numpy as np
 
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet, candidates_from_masks
-from modelmesh_b200.synth import SynthDecisions, SynthFleet, load_into_fleet
+from modelmesh_b200.synth import SynthDecisions, SynthFleet, load_into_fleet, make_fleet
 from oracle import binding as ob
 
 
-def oracle_from_synth(fl: SynthFleet, bulk=None) -> ob.OracleFleet:
-    """Config first (as a pod does at start-up, MM:777), instances as ADDED events, then one converged refresh."""
+def oracle_from_synth(fl: SynthFleet, bulk=None, gone=()) -> ob.OracleFleet:
+    """Config first (as a pod does at start-up, MM:777), instances as ADDED events, then one converged refresh.  gone: the
+    instances left out (they left the table and a commit dropped them; one event at a time only)."""
     o = ob.OracleFleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units)
     o.types_set(fl.type_config)
     if bulk is None:
         bulk = fl.n_instances > 3000
+    gone = set(int(i) for i in gone)
+    assert not (bulk and gone), "bulk_add adds every instance"
     if bulk:  # same final state (checked in test_host_logic.py) without the per-event O(N) work
         o.bulk_add(fl.inst_rows, fl.inst_ids, fl.inst_locs, fl.inst_zones, fl.inst_labels)
     else:
         for i in range(fl.n_instances):
+            if i in gone:
+                continue
             o.instance_event(ob.ADDED, i, fl.inst_rows[i], fl.inst_ids[i], fl.inst_locs[i], fl.inst_zones[i],
                              fl.inst_labels[i], fl.now_ms)
         if fl.type_config is not None:
@@ -137,3 +144,44 @@ def _first_diff(a, b, sd, ores, out, tr):
     d = np.nonzero(a != b)[0]
     i = int(d[0])
     return f"{len(d)} mismatches; first at {i}: got {a[i]} want {b[i]} dec={sd.dec[i]} oracle={ores[i]} out={out[i]} trace={tr[i]}"
+
+
+def place_kw(sd: SynthDecisions) -> dict:
+    """place_batch's fresh and extra arguments for sd"""
+    return dict(fresh=sd.fresh if len(sd.fresh) else None, extra=sd.extra if len(sd.extra) else None)
+
+
+def same_answers(got, want, what):
+    bad = np.nonzero((got["target"] != want["target"]) | (got["n_candidates"] != want["n_candidates"]))[0]
+    assert len(bad) == 0, (what, len(bad), bad[:5], got[bad[:5]], want[bad[:5]])
+
+
+def word_edge_fleet(ni: int, nm: int, seed: int):
+    """C3 with about a quarter of the models holding 5-12 instances; the first (inline) edges of every model are the
+    instances at ranks 0, 31, 32 (word edge), 383, 384, 385 (edge of the 12-word window) and n_ranks-1."""
+    fl = make_fleet("C3", nm, ni, seed)
+    # the placement order depends on the instance rows only: take it from the oracle
+    order = oracle_from_synth(fl).cluster_order()
+    nr = len(order)
+    special = order[[0, 31, 32, 383, 384, 385, nr - 1]]
+    rng = np.random.default_rng(seed)
+    deg = np.where(rng.uniform(size=nm) < 0.25, rng.integers(5, 13, size=nm), rng.integers(0, 5, size=nm))
+    edges = []
+    for m in range(nm):
+        inl = list(rng.choice(special, size=min(4, deg[m]), replace=False))
+        rest = [int(x) for x in rng.choice(ni, size=deg[m] + 8, replace=False) if x not in inl][:max(0, deg[m] - 4)]
+        edges.append([int(x) for x in inl] + rest)
+    fl.edge_off = np.zeros(nm + 1, dtype=np.int64)
+    np.cumsum([len(e) for e in edges], out=fl.edge_off[1:])
+    fl.edge_inst = np.asarray([x for e in edges for x in e], dtype=np.int32)
+    fl.n_loaded = np.asarray([len(e) for e in edges], dtype=np.int32)
+    fl.n_failed = np.zeros(nm, dtype=np.int32)
+    return fl, order, edges
+
+
+def free_port():
+    s = socket.socket()
+    s.bind(("127.0.0.1", 0))
+    p = s.getsockname()[1]
+    s.close()
+    return p

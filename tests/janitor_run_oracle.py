@@ -8,21 +8,14 @@ Quirk N15 (the janitor's TreeSet): scaleCopiesCandidates is a TreeSet ordered by
 lastUsed value only, so of candidates with equal lastUsed the set keeps the first one added and drops the others.  The
 reference adds them in registry iteration order; model index order stands in for it, as it does for the reaper's bounded set
 (N12)."""
-import ctypes as C
-
 import numpy as np
 
+from common import jsub, vp
 from modelmesh_b200 import _lib as L
 from oracle import binding as ob
 from rate_run_oracle import saturated
 
 SHORT_EXPIRY_RECENT_USE_TIME_MS = 180_000
-vp = lambda a: a.ctypes.data_as(C.c_void_p)
-
-
-def jsub(a: int, b: int) -> int:
-    """Java long a - b"""
-    return ((int(a) - int(b) + (1 << 63)) % (1 << 64)) - (1 << 63)
 
 
 def remove_model_copies(o: ob.OracleFleet, fl, ts, lul, self_idx: int, m: int, ce, params, can_remove: int) -> int:

@@ -13,17 +13,11 @@ import copy
 import numpy as np
 
 import janitor_run_oracle as jro
-from janitor_run_oracle import jsub
+from common import LONG_MAX, jlong, jsub
 from modelmesh_b200 import _lib as L
 from rate_run_oracle import saturated
 
-LONG_MAX = (1 << 63) - 1
 LASTUSED_AGE_ON_ADD_MS = 3_600_000
-
-
-def jlong(x: int) -> int:
-    return ((int(x) + (1 << 63)) % (1 << 64)) - (1 << 63)
-
 
 def _self_regs(fl, ts, S, m):
     """(loaded time or None, failed time or None): the pod's first loaded and first failed registration of model m"""

@@ -21,15 +21,13 @@ import evict_run_oracle as ero
 import janitor_run_oracle as jro
 import rate_run_oracle as rro
 import shutdown_run_oracle as sro
+from common import HOUR, LONG_MAX
 from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
-from modelmesh_b200.synth import LONG_MAX, NOW_MS, make_fleet
+from modelmesh_b200.synth import NOW_MS, make_fleet
+from pod_tasks import HAND_TIMEOUT, IT, evict_params, janitor_params, rate_params, shutdown_params
 
-HOUR = 3_600_000
-EXPIRY = 900_000
 LONG_MIN = -(1 << 63)
-IT = 5000
-TIMEOUT = 60_000
 TASKS = ("janitor", "rate", "shutdown", "evict")
 
 
@@ -187,24 +185,12 @@ def hand_cases(oracle_lib):
 
 # ------------------------------------------------------------------------------------------------------- the edge pairs
 
-def evict_params(now=NOW_MS, timeout=TIMEOUT, expiry=EXPIRY):
-    p = np.zeros(1, dtype=L.EVICT_PARAMS)
-    p["now"], p["load_timeout_ms"], p["load_failure_expiry_ms"] = now, timeout, expiry
-    return p
-
-
 def evict_entries(*rows):
     """rows of (model, last_used, load_ts, load_complete_ts, flags)"""
     e = np.zeros(len(rows), dtype=L.EVICT_ENTRY)
     for r, (m, lu, lt, lct, f) in enumerate(rows):
         e[r] = (m, f, lu, lt, lct)
     return e
-
-
-def shutdown_params(now=NOW_MS, cutoff_age=HOUR, expiry=EXPIRY):
-    p = np.zeros(1, dtype=L.SHUTDOWN_PARAMS)
-    p["now"], p["cutoff_age_ms"], p["load_failure_expiry_ms"] = now, cutoff_age, expiry
-    return p
 
 
 def shutdown_entries(*rows):
@@ -215,17 +201,6 @@ def shutdown_entries(*rows):
     return e
 
 
-def rate_params(now, thr, delta=10_000, expiry=EXPIRY):
-    p = np.zeros(1, dtype=L.RATE_PARAMS)
-    s = p["scale"]
-    s["now"], s["last_check_time"], s["iteration"], s["scale_up_rpm_threshold"] = now, now - delta, IT, thr
-    s["second_copy_min_age_iters"], s["second_copy_max_age_iters"], s["second_copy_lru_threshold_ms"] = 42, 240, -1
-    s["rate_check_interval_ms"], s["assume_completed_ms"], s["second_copy_remove_max_age_ms"] = 10_000, 30_000, HOUR
-    p["scale"] = s
-    p["load_failure_expiry_ms"] = expiry
-    return p
-
-
 def rate_entry(pod, model, rpm=0, second=False, delta=10_000):
     """an entry measuring at least rpm over delta ms; second: its usage iterations trigger the second-copy check"""
     e = np.zeros(1, dtype=L.SCALE_IN)
@@ -233,16 +208,6 @@ def rate_entry(pod, model, rpm=0, second=False, delta=10_000):
     e["last_used"] = 1
     e["i1"], e["i2"] = (IT - 100, IT - 100) if second else (IT - 1000, IT - 1000)
     return e
-
-
-def janitor_params(now, adjusted_capacity, flags=0):
-    p = np.zeros(1, dtype=L.JANITOR_PARAMS)
-    s = p["scale"]
-    s["now"], s["last_check_time"], s["iteration"], s["scale_up_rpm_threshold"] = now, now - 10_000, 5000, 2000
-    s["rate_check_interval_ms"], s["assume_completed_ms"], s["second_copy_remove_max_age_ms"] = 10_000, 30_000, 1000
-    p["scale"] = s
-    p["load_failure_expiry_ms"], p["adjusted_capacity"], p["flags"] = EXPIRY, adjusted_capacity, flags
-    return p
 
 
 def janitor_entry(model, last_used, weight=10, load_ts=0, failed=False):
@@ -286,7 +251,7 @@ def _what(res):
 
 
 def evict_pairs():
-    now, old = NOW_MS, NOW_MS - 2 * TIMEOUT - 1
+    now, old = NOW_MS, NOW_MS - 2 * HAND_TIMEOUT - 1
     P = 0
     one = [([(P, old)], [])]
     row = evict_entries((0, now - 10, old, 0, 0))

@@ -15,21 +15,11 @@ import ctypes as C
 
 import numpy as np
 
+from common import jdiv, jlong, vp
 from modelmesh_b200 import _lib as L
 from oracle import binding as ob
 
-vp = lambda a: a.ctypes.data_as(C.c_void_p)
 FAILURE_LIMIT = 3   # checkLoadFailureCount's MAX_LOAD_FAILURES
-
-
-def jlong(x: int) -> int:
-    return ((int(x) + (1 << 63)) % (1 << 64)) - (1 << 63)
-
-
-def jdiv(a: int, b: int) -> int:
-    """Java long a / b (truncates toward zero)"""
-    q = abs(a) // abs(b)
-    return q if (a >= 0) == (b >= 0) else -q
 
 
 def saturated(fl, m: int) -> bool:

@@ -3,7 +3,8 @@ orc_sim_step plus the reaper's proactive loads as a third event type.
 
 `reaper_oracle` (a module fixture) builds that library -- the whole oracle plus the one step function -- and makes it the
 library oracle/binding.py hands out while the module runs, so every OracleFleet / OracleSim the module creates lives in it.
-`with_reaper(sim)` then makes sim.step run orc_sim_step_reaper."""
+`with_reaper(sim)` then makes sim.step run orc_sim_step_reaper; reaper_sim(w) builds a churn workload's oracle and loop that
+way, and reaper_event() is one REAPER event of it."""
 import ctypes as C
 import os
 import subprocess
@@ -11,6 +12,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from helpers import oracle_from_synth
+from modelmesh_b200._lib import CHURN_REAPER
 from oracle import binding as ob
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -61,3 +64,26 @@ def with_reaper(sim: ob.OracleSim, n_models: int) -> ob.OracleSim:
     sim.reaper_models = n_models
     sim.step = lambda ev, now0, now1, seed: step(sim, ev, now0, now1, seed)
     return sim
+
+
+def reaper_sim(w):
+    """(the oracle fleet of w, its closed loop seeded with w's caches and stepping with REAPER events)"""
+    fl = w.fleet
+    o = oracle_from_synth(fl, bulk=False)
+    models = np.zeros(fl.n_models, dtype=ob.SIM_MODEL)
+    models["last_used"], models["type_idx"], models["size_units"] = fl.model_last_used, fl.model_type, fl.model_size
+    sim = with_reaper(ob.OracleSim(o, models, fl.type_names, fl.edge_off, fl.edge_inst, fl.n_loaded, w.capacity, w.load_timeout_ms,
+                                   fl.now_ms - 60_000), fl.n_models)
+    order = np.argsort(w.seed_instance, kind="stable")
+    bounds = np.searchsorted(w.seed_instance[order], np.arange(fl.n_instances + 1))
+    for i in range(fl.n_instances):
+        sel = order[bounds[i]:bounds[i + 1]]
+        if len(sel):
+            sim.seed(i, w.seed_model[sel], w.seed_last_used[sel], w.seed_weight[sel], w.seed_load_ts[sel], fl.now_ms)
+    return o, sim
+
+
+def reaper_event(caller: int, t: int) -> np.ndarray:
+    e = np.zeros(1, dtype=ob.SIM_EVENT)
+    e["type"], e["caller"], e["t"] = CHURN_REAPER, caller, t
+    return e

@@ -12,12 +12,10 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from common import HOUR, LONG_MAX, vp
 from oracle import binding as ob
 
-HOUR = 3_600_000
 REPAIR_AGE_MS = 3 * HOUR   # LASTUSED_AGE_ON_ADD_MS x 3
-LONG_MAX = np.iinfo(np.int64).max
-vp = lambda a: a.ctypes.data_as(C.c_void_p)
 
 
 @dataclass

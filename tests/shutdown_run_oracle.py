@@ -21,7 +21,8 @@ import numpy as np
 
 from modelmesh_b200 import _lib as L
 from oracle import binding as ob
-from rate_run_oracle import jlong, refused, saturated
+from common import jlong
+from rate_run_oracle import refused, saturated
 
 
 def shutdown_run(o: ob.OracleFleet, fl, ts, pod: int, entries, params, seed: int, fresh_self=None):

@@ -8,10 +8,10 @@ import dataclasses
 import numpy as np
 import pytest
 
+from churn_harness import build, compare_window
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet
 from modelmesh_b200.synth import load_into_fleet, make_churn, make_churn_overflow
-from test_churn_gpu import _build, _compare_window
 
 pytestmark = pytest.mark.gpu
 
@@ -45,13 +45,13 @@ class _Registry:
 
 def _run(product_lib, w, windows, seed, slots=256, events=None):
     fl = w.fleet
-    o, sim, s = _build(product_lib, w, slots=slots)
+    o, sim, s = build(product_lib, w, slots=slots)
     reg = _Registry(fl)
     reg.check(-1, sim, s)
     for ep in range(windows):
         ev = events(ep) if events else w.events(ep, 2000, seed)
         now0 = fl.now_ms + ep * w.window_ms
-        _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
+        compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
         reg.check(ep, sim, s)
     return o, sim, s, reg
 
@@ -129,12 +129,12 @@ def test_overflow_edges_by_hand(product_lib, oracle_lib):
             return w.events(ep, 3000, 11)
         return np.sort(np.concatenate([out, w.events(ep, 600, 11)]), order="t", kind="stable")
 
-    o, sim, s = _build(product_lib, w, slots=256)
+    o, sim, s = build(product_lib, w, slots=256)
     reg = _Registry(fl)
     for ep in range(8):
         ev = events(ep)
         now0 = fl.now_ms + ep * w.window_ms
-        dec, evi, _ = _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 1100 + ep)
+        dec, evi, _ = compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 1100 + ep)
         crossed = reg.check(ep, sim, s)
         if ep == 0:
             assert crossed == 0, crossed  # nothing left past four: the overflow table is empty
@@ -230,10 +230,10 @@ def test_overflow_closed_loop_c4_full_size(product_lib, oracle_lib):
     w = make_churn_overflow(make_churn(500_000, 2_500, 4), 0.002, 4, regs=(6, 6))
     fl = w.fleet
     assert (np.diff(fl.edge_off) > 4).sum() > 500
-    o, sim, s = _build(product_lib, w, slots=512)
+    o, sim, s = build(product_lib, w, slots=512)
     reg = _Registry(fl)
     for ep in range(3):
         ev = w.events(ep, 20_000, 4)
         now0 = fl.now_ms + ep * w.window_ms
-        _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep)
+        compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep)
         reg.check(ep, sim, s)

@@ -10,23 +10,20 @@
   * a window without REAPER events reports the same bytes and launches the same kernels after a REAPER window as on a fleet
     that never saw one;
   * C4 at full size (500k models x 2 500 instances) with one REAPER event per window."""
-import dataclasses
-
 import numpy as np
 import pytest
 
+from churn_harness import build as _build_churn, compare_window, device_selection, recent_unloaded, reaper_workload, with_failed
 from modelmesh_b200 import _lib as L
-from modelmesh_b200.fleet import MmpError
 from modelmesh_b200.synth import make_churn, make_churn_overflow
 from oracle import binding as ob
 from reaper_oracle import _reaper_oracle_so, reaper_oracle, with_reaper  # noqa: F401
-from test_churn_gpu import _build as _build_churn, _compare_window
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("reaper_oracle")]
 
 
 def _build(product_lib, w, slots):
-    """test_churn_gpu's fleet, oracle and device loop, the oracle's loop stepping with REAPER events (reaper_oracle.py)"""
+    """churn_harness.build's fleet, oracle and device loop, the oracle's loop stepping with REAPER events (reaper_oracle.py)"""
     o, sim, s = _build_churn(product_lib, w, slots)
     return o, with_reaper(sim, w.fleet.n_models), s
 
@@ -43,75 +40,16 @@ def request_event(model: int, caller: int, t: int) -> np.ndarray:
     return e
 
 
-def device_selection(s, t: int):
-    """mmp_reaper_select over the partitions in mmp_stats order with one `taken` array; a size estimate of 0 ends the run"""
-    _, ids = s.stats()
-    parts = [int(p) for p in ids[1:]] if len(ids) > 1 else [-1]
-    taken = np.zeros(s.max_models, dtype=np.uint8)
-    sel = []
-    for p in parts:
-        try:
-            sel += [int(x) for x in s.reaper_select(p, t, taken)]
-        except MmpError as e:
-            assert e.code == -1 and "size estimate is zero" in str(e), e
-            break
-    return sel
-
-
-def _with_failed(w, fails: dict):
-    """w with model m registering fails[m] failed loads (on instances 0, 1, ...) after its loaded copies"""
-    fl = w.fleet
-    nf = fl.n_failed.copy()
-    for m, k in fails.items():
-        nf[m] = k
-    cnt = (fl.n_loaded + nf).astype(np.int64)
-    off = np.zeros(fl.n_models + 1, dtype=np.int64)
-    np.cumsum(cnt, out=off[1:])
-    inst = np.zeros(int(off[-1]), dtype=np.int32)
-    for m in range(fl.n_models):
-        a, nl = int(fl.edge_off[m]), int(fl.n_loaded[m])
-        inst[off[m]:off[m] + nl] = fl.edge_inst[a:a + nl]
-        held = set(int(x) for x in fl.edge_inst[a:a + nl])
-        inst[off[m] + nl:off[m + 1]] = [i for i in range(fl.n_instances) if i not in held][:int(nf[m])]
-    return dataclasses.replace(w, fleet=dataclasses.replace(fl, edge_off=off, edge_inst=inst, n_failed=nf.astype(np.int32)))
-
-
-def _recent_unloaded(w, k):
-    fl = w.fleet
-    u = w.unloaded_models
-    return u[np.argsort(-fl.model_last_used[u], kind="stable")[:k]]
-
-
-def _workload(case, seed):
-    with_types = case.endswith("_tc")
-    base = case.removesuffix("_tc")
-    fill = {"free": 0.5, "cutoff": 0.9, "full": 0.97, "ties": 0.5, "none": 0.5, "zero": 0.5, "part0": 0.5}[base]
-    w = make_churn(20_000, 200, seed, fill=fill, with_types=with_types)
-    fl = w.fleet
-    if base == "ties":  # equal-lastUsed runs among the most recent candidates, and 0 / 1 / 2 failed loads on them
-        top = _recent_unloaded(w, 60)
-        for g in range(0, 60, 3):
-            fl.model_last_used[top[g:g + 3]] = fl.model_last_used[top[g]]
-        w = _with_failed(w, {int(m): j % 3 for j, m in enumerate(top[:45])})
-    elif base == "none":  # two failed loads on every unloaded model: no candidate at all
-        w = _with_failed(w, {int(m): 2 for m in w.unloaded_models})
-    elif base == "zero":  # published records with copies but nothing used: the size estimate is 0 (MM:6626-6628)
-        fl.inst_rows["used"] = 0
-    elif base == "part0":  # one half of the fleet published full: its partition has no free space, counts 0
-        fl.inst_rows["used"][1::2] = fl.inst_rows["capacity"][1::2]
-    return w
-
-
 @pytest.mark.parametrize("case,seed", [("free", 3), ("free_tc", 4), ("cutoff", 5), ("cutoff_tc", 6), ("full", 7), ("ties", 8),
                                        ("none", 9), ("zero", 10), ("part0_tc", 11)])
 def test_reaper_window_decides_the_selection(product_lib, oracle_lib, case, seed):
-    w = _workload(case, seed)
+    w = reaper_workload(case, seed)
     fl = w.fleet
     o, sim, s = _build(product_lib, w, slots=256)
     t = fl.now_ms + 500
     want = device_selection(s, t)
     ev = reaper_event(17, t)
-    dec, _, _ = _compare_window(0, o, sim, s, ev, fl.now_ms, fl.now_ms + w.window_ms, seed)
+    dec, _, _ = compare_window(0, o, sim, s, ev, fl.now_ms, fl.now_ms + w.window_ms, seed)
     assert [int(m) for m in dec["model"]] == want, (case, len(dec), len(want))
     assert np.all(dec["event"] == 0) and np.all(dec["self"] == 17)
     if case in ("free", "free_tc", "cutoff", "cutoff_tc", "ties", "part0_tc"):
@@ -124,10 +62,8 @@ def test_reaper_window_decides_the_selection(product_lib, oracle_lib, case, seed
         lu = fl.model_last_used[want]
         assert len(set(lu.tolist())) == len(lu)  # one model per lastUsed
         assert not set(want) & set(int(m) for m in w.unloaded_models if fl.n_failed[m] >= 2)
-
-
 def _compare_malformed_window(ep, o, sim, s, ev, now0, now1, seed):
-    """_compare_window for a window whose REAPER caller is no instance: its malformed decisions name no target on either side
+    """compare_window for a window whose REAPER caller is no instance: its malformed decisions name no target on either side
     (the oracle answers getNext's null, the device MMP_TARGET_INVALID, as for a REQUEST of that caller)"""
     dec_o, evi_o, rows_o, npub_o, carry_o = sim.step(ev, now0, now1, seed)
     dec_p, evi_p, rows_p, rep = s.churn_step(ev, now0, now1, seed)
@@ -157,7 +93,7 @@ def _run_trace(product_lib, w, windows, seed, build_events):
         ev = build_events(ep, now0)
         co0 = sim.coalesced()
         bad = np.any((ev["type"] == L.CHURN_REAPER) & ((ev["caller"] < 0) | (ev["caller"] >= fl.n_instances)))
-        dec, evi, rep = (_compare_malformed_window if bad else _compare_window)(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
+        dec, evi, rep = (_compare_malformed_window if bad else compare_window)(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
         assert rep.n_coalesced == sim.coalesced() - co0, (ep, rep.n_coalesced, sim.coalesced() - co0)
         reaper = np.isin(dec["event"], np.nonzero(ev["type"] == L.CHURN_REAPER)[0])
         out.append((ev, dec, reaper, rep))
@@ -171,7 +107,7 @@ def _run_trace(product_lib, w, windows, seed, build_events):
 def test_reaper_trace_coalescing_and_malformed_caller(product_lib, oracle_lib):
     w = make_churn(20_000, 200, 21, fill=0.5)
     fl = w.fleet
-    top = [int(m) for m in _recent_unloaded(w, 4)]  # surely selected by the first REAPER (free space: the most recent first)
+    top = [int(m) for m in recent_unloaded(w, 4)]  # surely selected by the first REAPER (free space: the most recent first)
 
     def events(ep, now0):
         base = w.events(ep, 2000, 21)
@@ -219,7 +155,7 @@ def test_window_without_reaper_unchanged(product_lib, oracle_lib):
     """Fleets a and b from one workload without reaper candidates; b's first window carries a REAPER event at its end (which
     selects nothing).  Every window's reports are the same bytes, and every later window launches the same kernels."""
     w = make_churn(20_000, 200, 27, fill=0.9)
-    w = _with_failed(w, {int(m): 2 for m in w.unloaded_models})
+    w = with_failed(w, {int(m): 2 for m in w.unloaded_models})
     fl = w.fleet
     _, _, a = _build(product_lib, w, slots=256)
     _, _, b = _build(product_lib, w, slots=256)
@@ -255,6 +191,6 @@ def test_reaper_c4_full_size(product_lib, oracle_lib):
         now0 = fl.now_ms + ep * w.window_ms
         base = w.events(ep, 20_000, 4)
         ev = np.concatenate([base[:10_000], reaper_event(ep * 7, now0 + 1000), base[10_000:]])
-        dec, _, rep = _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep)
+        dec, _, rep = compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep)
         picked += int(np.count_nonzero(dec["event"] == 10_000))
     assert picked > 1000, picked

@@ -10,31 +10,9 @@ from helpers import oracle_from_synth
 from modelmesh_b200._lib import CHURN_REAPER
 from modelmesh_b200.synth import make_churn
 from oracle import binding as ob
-from reaper_oracle import _reaper_oracle_so, reaper_oracle, with_reaper  # noqa: F401
+from reaper_oracle import _reaper_oracle_so, reaper_event, reaper_oracle, reaper_sim  # noqa: F401
 
 pytestmark = pytest.mark.usefixtures("reaper_oracle")
-
-
-def _sim(w):
-    fl = w.fleet
-    o = oracle_from_synth(fl, bulk=False)
-    models = np.zeros(fl.n_models, dtype=ob.SIM_MODEL)
-    models["last_used"], models["type_idx"], models["size_units"] = fl.model_last_used, fl.model_type, fl.model_size
-    sim = with_reaper(ob.OracleSim(o, models, fl.type_names, fl.edge_off, fl.edge_inst, fl.n_loaded, w.capacity, w.load_timeout_ms,
-                                   fl.now_ms - 60_000), fl.n_models)
-    order = np.argsort(w.seed_instance, kind="stable")
-    bounds = np.searchsorted(w.seed_instance[order], np.arange(fl.n_instances + 1))
-    for i in range(fl.n_instances):
-        sel = order[bounds[i]:bounds[i + 1]]
-        if len(sel):
-            sim.seed(i, w.seed_model[sel], w.seed_last_used[sel], w.seed_weight[sel], w.seed_load_ts[sel], fl.now_ms)
-    return o, sim
-
-
-def reaper_event(caller: int, t: int) -> np.ndarray:
-    e = np.zeros(1, dtype=ob.SIM_EVENT)
-    e["type"], e["caller"], e["t"] = CHURN_REAPER, caller, t
-    return e
 
 
 def expected_selection(o, sim, fl, t):
@@ -56,7 +34,7 @@ def expected_selection(o, sim, fl, t):
 def test_sim_reaper_decisions_are_the_partition_selections(oracle_lib, with_types, fill, seed):
     w = make_churn(6000, 48, seed, fill=fill, with_types=with_types)
     fl = w.fleet
-    o, sim = _sim(w)
+    o, sim = reaper_sim(w)
     picked = 0
     for ep in range(3):
         now0 = fl.now_ms + ep * w.window_ms
@@ -80,7 +58,7 @@ def test_sim_reaper_decisions_are_the_partition_selections(oracle_lib, with_type
 def test_closed_loop_with_reaper_conserves_copies_and_capacity(oracle_lib, with_types, fill, seed):
     w = make_churn(8000, 60, seed, fill=fill, with_types=with_types)
     fl = w.fleet
-    o, sim = _sim(w)
+    o, sim = reaper_sim(w)
     accepted = 0
     for ep in range(6):
         now0 = fl.now_ms + ep * w.window_ms
@@ -107,7 +85,7 @@ def test_reaper_step_without_reaper_events_is_the_oracle_step(oracle_lib):
     """orc_sim_step_reaper restates orc_sim_step: on a trace without REAPER events the two sims report the same"""
     w = make_churn(6000, 48, 7, fill=0.9, with_types=True)
     fl = w.fleet
-    _, a = _sim(w)
+    _, a = reaper_sim(w)
     o = oracle_from_synth(fl, bulk=False)
     models = np.zeros(fl.n_models, dtype=ob.SIM_MODEL)
     models["last_used"], models["type_idx"], models["size_units"] = fl.model_last_used, fl.model_type, fl.model_size

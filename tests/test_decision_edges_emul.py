@@ -12,7 +12,7 @@ from modelmesh_b200 import _lib as L
 
 from decision_edges import _jdiv, all_cases, check_built
 from helpers import compare_decisions, oracle_from_synth, oracle_inputs, solver_from_synth
-from test_split_place_emul import place_split, split_lib  # noqa: F401  (module fixture)
+from split_place import place_split, split_lib  # noqa: F401  (module fixture)
 
 CASES = all_cases()
 FAMILIES = sorted({c.family for c in CASES})

@@ -17,30 +17,17 @@ import numpy as np
 import pytest
 
 import evict_run_oracle as ero
-from helpers import oracle_from_synth, solver_from_synth
+from common import EXPIRY, HOUR, vp
+from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet, MmpError
 from modelmesh_b200.synth import load_into_fleet, make_fleet
+from pod_tasks import (TASK_FLEETS, TimedReplay, busiest_pod, composed_evict, evict_params, held_models, report_dict, set_regs,
+                       task_fleet, timed_solver)
 from replay import run_window
-from test_janitor_run_gpu import _set_regs
-from test_registry_overflow_gpu import _TimedReplay
-from test_shutdown_run_gpu import FLEETS, _fleet
 
 pytestmark = pytest.mark.gpu
-vp = lambda a: a.ctypes.data_as(C.c_void_p)
-HOUR = 3_600_000
-EXPIRY = 900_000
-TIMEOUT = 120_000
-
-
-def params(now):
-    p = np.zeros(1, dtype=L.EVICT_PARAMS)
-    p["now"], p["load_timeout_ms"], p["load_failure_expiry_ms"] = now, TIMEOUT, EXPIRY
-    return p
-
-
-def _held(fl, S):
-    return sorted(set(int(m) for m in np.searchsorted(fl.edge_off, np.nonzero(fl.edge_inst == S)[0], side="right") - 1))
+WORKLOAD_TIMEOUT = 120_000   # load_timeout_ms of these workloads (the hand-built cases take pod_tasks.HAND_TIMEOUT, 60 000)
 
 
 def _workload(config, nm, ni, seed):
@@ -48,10 +35,10 @@ def _workload(config, nm, ni, seed):
     copy; the pod added as one more loaded copy of 40 other models, as a failed load of 20 and as the only copy of 12; three
     recent failure records on every fourth model of which the pod is the only copy; the pod's own registrations at the reload
     edges"""
-    fl = _fleet(config, nm, ni, seed)
+    fl = task_fleet(config, nm, ni, seed)
     rng = np.random.default_rng(seed)
-    S = int(np.argmax(np.bincount(fl.edge_inst, minlength=ni)))
-    held = _held(fl, S)
+    S = busiest_pod(fl)
+    held = held_models(fl, S)
     loaded = [m for m in held if S in set(int(i) for i in fl.edge_inst[fl.edge_off[m]:fl.edge_off[m] + fl.n_loaded[m]])]
     free = rng.permutation([m for m in range(nm) if m not in set(held)])
     others = [i for i in range(ni) if i != S]
@@ -71,15 +58,15 @@ def _workload(config, nm, ni, seed):
         if m in failing:
             y += [int(i) for i in rng.choice(others, 8, replace=False) if i not in y][:3]
         changes[m] = ([S], y)
-    _set_regs(fl, changes)
+    set_regs(fl, changes)
     n, now = len(fl.edge_inst), fl.now_ms
     ts = np.where(rng.uniform(size=n) < 0.3, now - rng.integers(0, EXPIRY, size=n), now - rng.integers(EXPIRY, 4 * HOUR, size=n)).astype(np.int64)
     for m in failing:
         ts[int(fl.edge_off[m + 1]) - 3:int(fl.edge_off[m + 1])] = now - rng.integers(0, EXPIRY // 2, size=3)
     mine = np.nonzero(fl.edge_inst == S)[0]
     edge = rng.choice(mine, min(len(mine), 12), replace=False)
-    ts[edge[0::2]] = now - 2 * TIMEOUT
-    ts[edge[1::2]] = now - 2 * TIMEOUT - 1
+    ts[edge[0::2]] = now - 2 * WORKLOAD_TIMEOUT
+    ts[edge[1::2]] = now - 2 * WORKLOAD_TIMEOUT - 1
     lul = np.where(rng.uniform(size=nm) < 0.3, now - rng.integers(0, 200_000, size=nm), 0).astype(np.int64)
     return fl, ts, lul, S
 
@@ -87,7 +74,7 @@ def _workload(config, nm, ni, seed):
 def _entries(fl, ts, S, rng, n_unreg=30):
     """the evictions of a burst in listener order: every model the pod is registered on, and models it does not hold"""
     now = fl.now_ms
-    models = _held(fl, S)
+    models = held_models(fl, S)
     rest = [m for m in range(fl.n_models) if m not in set(models)]
     models += [int(m) for m in rng.choice(rest, n_unreg, replace=False)]
     e = np.zeros(len(models), dtype=L.EVICT_ENTRY)
@@ -105,55 +92,28 @@ def _entries(fl, ts, S, rng, n_unreg=30):
     return e[rng.permutation(len(e))]
 
 
-def _build(lib, fl, ts, lul):
-    s = solver_from_synth(fl, lib)
-    for m in range(fl.n_models):
-        s.model_times(m, ts[fl.edge_off[m]:fl.edge_off[m + 1]], int(lul[m]))
-    s.commit()
-    return s
-
-
-def _rep(r):
-    return {k: getattr(r, k) for k, _ in L.EvictReport._fields_}
-
-
 def _check(s, o, fl, ts, lul, S, ents, p, seed, fresh=None):
     out, r = s.evict_run(S, ents, p, seed, fresh_self=fresh)
     want, wr = ero.evict_run(o, fl, ts, lul, S, ents, p, seed, fresh_self=fresh)
     bad = np.nonzero(out != want)[0]
     assert len(bad) == 0, (len(bad), out[bad[:3]], want[bad[:3]])
-    assert _rep(r) == wr
+    assert report_dict(r) == wr
     return out, wr
 
 
-def _composed(s, S, ents, out, p, seed, fresh):
-    """the placed entries as mmp_place_batch records with the same ids: the answers must be out's, byte for byte"""
-    rows = np.nonzero(out["what"] & L.EV_PLACED)[0]
-    if not len(rows):
-        return 0
-    d = np.zeros(len(rows), dtype=L.DECISION_IN)
-    d["model"], d["self"], d["last_used"] = ents["model"][rows], S, ents["last_used"][rows]
-    d["flags"] = L.DF_FAVOUR_SELF | L.DF_OWN_ID | (rows.astype(np.uint32) << 8)
-    d["fresh"], d["extra_off"], d["extra_n"] = -1 if fresh is None else 0, 0, 1
-    kw = dict(fresh=None if fresh is None else np.asarray(fresh, dtype=L.INSTANCE_ROW).reshape(1))
-    res = s.place_batch(d, int(p["now"][0]), seed, extra=np.array([S], dtype=np.int32), **kw)
-    assert res.tobytes() == out[["target", "n_candidates"]][rows].astype(res.dtype).tobytes()
-    return len(rows)
-
-
-@pytest.mark.parametrize("config,nm,ni,seed", FLEETS)
+@pytest.mark.parametrize("config,nm,ni,seed", TASK_FLEETS)
 def test_evict_run_matches_the_restatement(product_lib, oracle_lib, config, nm, ni, seed):
     fl, ts, lul, S = _workload(config, nm, ni, seed)
     ents = _entries(fl, ts, S, np.random.default_rng(seed))
-    s, o = _build(product_lib, fl, ts, lul), oracle_from_synth(fl)
+    s, o = timed_solver(product_lib, fl, ts, lul), oracle_from_synth(fl)
     fresh = fl.inst_rows[S].copy()
     fresh["used"] = fresh["used"] + fresh["capacity"] // 100
-    p = params(fl.now_ms)
+    p = evict_params(fl.now_ms, WORKLOAD_TIMEOUT)
     seen = {k: 0 for k in ero.REPORT_KEYS}
     out = np.zeros(len(ents), dtype=L.EVICT_ACTION)
     for fr in (None, fresh):
         got, wr = _check(s, o, fl, ts, lul, S, ents, p, 100 + seed, fresh=fr)
-        assert _composed(s, S, ents, got, p, 100 + seed, fr) == wr["n_placed"]
+        assert composed_evict(s, S, ents, got, p, 100 + seed, fr) == wr["n_placed"]
         for k in seen:
             seen[k] += wr[k]
         t = C.c_double()
@@ -179,26 +139,16 @@ def test_evict_run_matches_the_restatement(product_lib, oracle_lib, config, nm, 
 
 def test_evict_run_replayed_stream(product_lib, oracle_lib):
     """after device-path and host-path commits of a replayed ingest stream whose upserts come with registration times"""
-    rp = _TimedReplay(make_fleet("C3", 3000, 600, 3), product_lib, 3)
+    rp = TimedReplay(make_fleet("C3", 3000, 600, 3), product_lib, 3)
     paths = set()
     for w in range(8):
         run_window(rp, w)
         paths.add(rp.windows[-1][1])
         v, o = rp.view(), rp.oracle()
-        ts = np.zeros(len(v.edge_inst), dtype=np.int64)
-        lul = np.zeros(v.n_models, dtype=np.int64)
-        for m, (t, u) in rp.times.items():
-            a, b = int(v.edge_off[m]), int(v.edge_off[m + 1])
-            k = min(len(t), b - a)
-            ts[a:a + k] = t[:k]
-            lul[m] = u
-        co = o.cluster_order()
-        cnt = np.bincount(v.edge_inst, minlength=max(v.n_instances, int(co.max()) + 1))
-        ranked = np.zeros(len(cnt), dtype=bool)
-        ranked[co] = True
-        S = int(np.argmax(np.where(ranked, cnt, -1)))   # (the stream takes pods out: the pod places from its published row)
+        ts, lul = rp.view_times(v)
+        S = busiest_pod(v, ranked=o.cluster_order())   # (the stream takes pods out: the pod places from its published row)
         ents = _entries(v, ts, S, np.random.default_rng(w), n_unreg=10)
-        _, wr = _check(rp.f, o, v, ts, lul, S, ents, params(rp.now), 7)
+        _, wr = _check(rp.f, o, v, ts, lul, S, ents, evict_params(rp.now, WORKLOAD_TIMEOUT), 7)
         assert wr["n_unregister"] > 0 and wr["n_reload"] > 0
         o.close()
     assert paths == {1, 2}, paths
@@ -209,7 +159,7 @@ def test_evict_run_pod_out_of_the_table(product_lib, oracle_lib):
     one are answered MMP_TARGET_INVALID"""
     fl, ts, lul, S = _workload("C3", 4000, 600, 3)
     ents = _entries(fl, ts, S, np.random.default_rng(4))
-    s = _build(product_lib, fl, ts, lul)
+    s = timed_solver(product_lib, fl, ts, lul)
     fl.inst_rows["shutting_down"][S] = 1
     s.instance_update(S, fl.inst_rows[S])
     s.commit()
@@ -217,7 +167,7 @@ def test_evict_run_pod_out_of_the_table(product_lib, oracle_lib):
     assert S not in set(int(i) for i in o.cluster_order())
     fresh = fl.inst_rows[S].copy()
     fresh["shutting_down"] = 0
-    p = params(fl.now_ms)
+    p = evict_params(fl.now_ms, WORKLOAD_TIMEOUT)
     with_row, wr = _check(s, o, fl, ts, lul, S, ents, p, 9, fresh=fresh)
     without, wr2 = _check(s, o, fl, ts, lul, S, ents, p, 9)
     placed = (without["what"] & L.EV_PLACED) != 0
@@ -232,7 +182,7 @@ def test_evict_run_pod_out_of_the_table(product_lib, oracle_lib):
 def test_evict_run_errors(product_lib):
     fl = make_fleet("C3", 200, 40, 5)
     s = Fleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, fl.n_instances, fl.n_models, lib=product_lib)
-    p = params(fl.now_ms)
+    p = evict_params(fl.now_ms, WORKLOAD_TIMEOUT)
     ents = np.zeros(2, dtype=L.EVICT_ENTRY)
     ents["model"], ents["last_used"] = [3, 4], fl.now_ms - 1
     with pytest.raises(MmpError) as e:

@@ -10,20 +10,14 @@ import evict_run_oracle as ero
 from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import NOW_MS
-from test_rate_run_oracle import EXPIRY, HOUR, hand_fleet
+from common import EXPIRY, HOUR
+from pod_task_edges import hand_fleet
+from pod_tasks import HAND_TIMEOUT, evict_params
 
 POD = 0
-TIMEOUT = 60_000
-OLD = NOW_MS - 2 * TIMEOUT - 1   # a registration time that reloads
+OLD = NOW_MS - 2 * HAND_TIMEOUT - 1   # a registration time that reloads
 RECENT_FAIL = NOW_MS - EXPIRY // 2 + 1
 UR = L.EV_UNREGISTER | L.EV_RELOAD
-
-
-def params(now):
-    p = np.zeros(1, dtype=L.EVICT_PARAMS)
-    p["now"], p["load_timeout_ms"], p["load_failure_expiry_ms"] = now, TIMEOUT, EXPIRY
-    return p
-
 
 def ents(*rows):
     """rows of (model, last_used, load_ts, load_complete_ts, flags)"""
@@ -42,7 +36,7 @@ def run(regs, ni, rows, seed=5, lul=None, edit=None, **kw):
         edit(fl)
         o = oracle_from_synth(fl)
     lul = np.zeros(len(regs), dtype=np.int64) if lul is None else np.asarray(lul, dtype=np.int64)
-    out, rep = ero.evict_run(o, fl, ts, lul, POD, ents(*rows), params(fl.now_ms), seed)
+    out, rep = ero.evict_run(o, fl, ts, lul, POD, ents(*rows), evict_params(fl.now_ms, HAND_TIMEOUT), seed)
     stats = o.type_stats(fl.type_names[0])
     o.close()
     return fl, out, rep, stats
@@ -54,7 +48,7 @@ def report(**nonzero):
 
 def test_reload_needs_an_age_past_twice_the_timeout(oracle_lib):
     now = NOW_MS
-    t0, t1 = now - 2 * TIMEOUT, now - 2 * TIMEOUT - 1
+    t0, t1 = now - 2 * HAND_TIMEOUT, now - 2 * HAND_TIMEOUT - 1
     fl, out, rep, _ = run([([(POD, t0)], []), ([(POD, t1)], [])], 12, [(0, now - 5000, t0, 0, 0), (1, now - 5000, t1, 0, 0)])
     assert list(out["what"]) == [L.EV_UNREGISTER, UR | L.EV_PLACED]
     assert out["target"][0] == L.TARGET_INVALID and out["n_candidates"][0] == 0
@@ -83,7 +77,7 @@ def test_load_ts_that_does_not_match_writes_nothing_but_still_reloads(oracle_lib
 
 def test_pod_only_in_failed_in_reloads_from_the_failure_time(oracle_lib):
     """model 0: an old failure record; model 1: a failure 2 x timeout ago, too young to reload"""
-    young = NOW_MS - 2 * TIMEOUT
+    young = NOW_MS - 2 * HAND_TIMEOUT
     fl, out, rep, _ = run([([], [(POD, OLD)]), ([], [(POD, young)])], 12, [(0, 0, 5, OLD, 0), (1, 0, 5, young, 0)])
     assert list(out["what"]) == [L.EV_DROP_FAILURE | L.EV_RELOAD | L.EV_PLACED, L.EV_DROP_FAILURE]
     assert list(out["last_used"]) == [NOW_MS] * 2   # updateLastUsed(0) is now

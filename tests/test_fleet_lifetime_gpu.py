@@ -8,12 +8,10 @@ import os
 import numpy as np
 import pytest
 
-from exclude_set import oracle_excluding, random_set
-from helpers import compare_decisions, oracle_from_synth
+from churn_harness import build, compare_window
+from exclude_set import compact, oracle_excluding, random_set
+from helpers import compare_decisions, free_port, oracle_from_synth, place_kw, same_answers
 from modelmesh_b200.synth import SynthDecisions, load_into_fleet, make_churn, make_decisions, make_fleet
-from test_churn_gpu import _build, _compare_window
-from test_exclude_set_gpu import _compact, _kw, _same
-from test_instance_shards_gpu import _free_port
 
 pytestmark = pytest.mark.gpu
 
@@ -27,7 +25,7 @@ def test_fresh_fleets_after_destroy_match_the_oracle(product_lib, oracle_lib):
         seed = 4 + rnd
         w = make_churn(20_000, 200, seed, fill=0.9, with_types=True)
         fl = w.fleet
-        o, sim, s = _build(product_lib, w, slots=256)
+        o, sim, s = build(product_lib, w, slots=256)
         sd = make_decisions(fl, 9000, seed)
         # a batch large enough for the slot sort, in slot order, against the oracle
         s._ck(lib.mmp_tune(s.h, b"sort_slots", 1))
@@ -36,18 +34,18 @@ def test_fresh_fleets_after_destroy_match_the_oracle(product_lib, oracle_lib):
         want = oracle_excluding(o, fl, sd, NONE, seed)
         # a call-wide exclude set: the call's own slot tables
         xs = random_set(fl.n_instances, 24, seed)
-        _same(s.place_batch(sd.dec, fl.now_ms, seed, exclude=xs, **_kw(sd)), oracle_excluding(o, fl, sd, xs, seed), (rnd, "exclude"))
+        same_answers(s.place_batch(sd.dec, fl.now_ms, seed, exclude=xs, **place_kw(sd)), oracle_excluding(o, fl, sd, xs, seed), (rnd, "exclude"))
         # B <= 32 through the captured graph (one_mode 2) and the resident server (3)
-        part = _compact(sd, 32)
+        part = compact(sd, 32)
         for mode in (2, 3):
             s._ck(lib.mmp_tune(s.h, b"one_mode", mode))
             for n in (1, 32):
                 small = SynthDecisions(part.dec[:n], part.fresh, part.extra)
-                _same(s.place_batch(small.dec, fl.now_ms, seed, **_kw(small)), want[:n], (rnd, "one_mode", mode, n))
+                same_answers(s.place_batch(small.dec, fl.now_ms, seed, **place_kw(small)), want[:n], (rnd, "one_mode", mode, n))
         # the closed loop: two windows, each ending in a device-path commit
         for ep in range(2):
             now0 = fl.now_ms + ep * w.window_ms
-            _compare_window((rnd, ep), o, sim, s, w.events(ep, 2000, seed), now0, now0 + w.window_ms, seed * 100 + ep)
+            compare_window((rnd, ep), o, sim, s, w.events(ep, 2000, seed), now0, now0 + w.window_ms, seed * 100 + ep)
         s.close()
 
 
@@ -75,7 +73,7 @@ def _peer_worker(rank, world, port, q):
             dist.all_gather_object(blobs, f.shard_ipc_export(8192))
             f.shard_ipc_import(blobs)
             dist.barrier()
-            results.append(f.place_batch(sd.dec, fl.now_ms, 77, **_kw(sd)).copy())
+            results.append(f.place_batch(sd.dec, fl.now_ms, 77, **place_kw(sd)).copy())
             results.append(int(f.shard_peer_stats()["batches"]))
             dist.barrier()
             f.close()
@@ -96,7 +94,7 @@ def test_fresh_sharded_fleets_after_destroy_match_the_oracle(product_lib, oracle
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_peer_worker, args=(r, world, port, q)) for r in range(world)]
     for p in procs:
         p.start()
@@ -116,5 +114,5 @@ def test_fresh_sharded_fleets_after_destroy_match_the_oracle(product_lib, oracle
     want = oracle_excluding(oracle_from_synth(fl), fl, sd, NONE, 77)
     for r in range(world):
         for k in range(ROUNDS):
-            _same(got[r][2 * k], want, ("rank", r, "round", k))
+            same_answers(got[r][2 * k], want, ("rank", r, "round", k))
             assert got[r][2 * k + 1] == 1, (r, k)  # the batch went through the peer path

@@ -15,23 +15,19 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from churn_harness import build, compare_window
+from common import LONG_MAX, vp
 from helpers import oracle_from_synth, solver_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import MmpError
 from modelmesh_b200.synth import SplitMix, make_churn, make_fleet
 from oracle import binding as ob
-from test_churn_gpu import _build, _compare_window
-from test_scans_gpu import _partition_maps
+from scan_checks import converged_oracle, partition_maps
 
 pytestmark = pytest.mark.gpu
 
-LONG_MAX = (1 << 63) - 1
 FIELDS = ("total_capacity", "total_free", "global_lru", "instance_count", "model_copy_count")
 SMEM_PARTS = 511  # STATS_SMEM_PARTS (scan_kernels.cuh): past it k_stats accumulates in global memory
-
-
-def _vp(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def _partition_heavy(fl, seed):
@@ -54,21 +50,6 @@ def _partition_heavy(fl, seed):
     return fl
 
 
-def _converged_oracle(fl):
-    """The oracle with every subset's LRU recomputed over the final fleet (N10): bulk_add above 3 000 instances, else the
-    ADDED events and then one UPDATED event per instance (as test_stats_match_oracle)."""
-    o = oracle_from_synth(fl)
-    if fl.n_instances <= 3000:
-        for i in range(fl.n_instances):
-            if not fl.inst_rows["shutting_down"][i]:
-                r = fl.inst_rows[i].copy()
-                r["l_in_prog"] += 1
-                o.instance_event(ob.UPDATED, i, r, fl.inst_ids[i], fl.inst_locs[i], fl.inst_zones[i], fl.inst_labels[i], fl.now_ms)
-                o.instance_event(ob.UPDATED, i, fl.inst_rows[i], fl.inst_ids[i], fl.inst_locs[i], fl.inst_zones[i],
-                                 fl.inst_labels[i], fl.now_ms)
-    return o
-
-
 def _check_stats(fl, o, s):
     """mmp_stats against orc_cluster_stats / orc_partition_stats: every field of every partition (ids mapped through instance
     membership), the number of entries, and the PARTITION_STATS_COMP order (TCM:264-271).  Partitions that tie exactly keep
@@ -84,7 +65,7 @@ def _check_stats(fl, o, s):
     live = ost["instance_count"] > 0
     by_o = {int(i): x for i, x in zip(oids[live], ost[live])}
     assert len(st) - 1 == len(by_o), (len(st) - 1, len(by_o))
-    pmap = _partition_maps(fl, o, s)
+    pmap = partition_maps(fl, o, s)
     assert len(set(int(p) for p in ids[1:])) == len(ids) - 1
     for x, pid in zip(st[1:], ids[1:]):
         y = by_o[pmap[int(pid)]]
@@ -117,7 +98,7 @@ def _reaper_partitions(fl, o, s, ids):
     """every partition in the product's stats order, `taken` carried from one to the next (MM:6473-6489);
     returns the selection of each call"""
     om = _om(fl)
-    pmap = _partition_maps(fl, o, s)
+    pmap = partition_maps(fl, o, s)
     taken_o, taken_s = np.zeros(fl.n_models, np.uint8), np.zeros(fl.n_models, np.uint8)
     sel = []
     for pid in ids[1:]:
@@ -158,7 +139,7 @@ def heavy(product_lib, oracle_lib):
     s = solver_from_synth(fl, product_lib)
     for m in range(fl.n_models):
         e = np.ascontiguousarray(ts[fl.edge_off[m]:fl.edge_off[m + 1]])
-        s._ck(product_lib.mmp_model_times(s.h, m, _vp(e), len(e), int(lul[m])))
+        s._ck(product_lib.mmp_model_times(s.h, m, vp(e), len(e), int(lul[m])))
     s.commit()
     o = oracle_from_synth(fl, bulk=True)  # bulk_add is the converged state (N10)
     return fl, o, s, ts, lul
@@ -182,7 +163,7 @@ def test_partition_heavy_stats_cap_contract(heavy):
         out = np.zeros(cap + 4, dtype=L.CLUSTER_STATS)
         out["total_capacity"] = -7
         ids = np.full(cap + 4, -7, dtype=np.int32)
-        n = s._ck(s.lib.mmp_stats(s.h, _vp(out), _vp(ids), cap))
+        n = s._ck(s.lib.mmp_stats(s.h, vp(out), vp(ids), cap))
         assert n == len(full)
         assert np.array_equal(out[:cap], full[:cap]) and np.array_equal(ids[:cap], fids[:cap])
         assert (out["total_capacity"][cap:] == -7).all() and (ids[cap:] == -7).all()
@@ -252,16 +233,16 @@ def test_partition_heavy_scale_eval_matches_oracle(heavy, product_lib, oracle_li
         p["second_copy_min_age_iters"], p["second_copy_max_age_iters"], p["second_copy_lru_threshold_ms"] = 42, 240, lru_thr
         p["rate_check_interval_ms"], p["assume_completed_ms"], p["second_copy_remove_max_age_ms"], p["can_remove"] = 10_000, 30_000, 36_000_000, can_remove
         out = np.zeros(n, dtype=L.SCALE_OUT)
-        s._ck(lib.mmp_scale_eval(s.h, _vp(rec), n, _vp(p), _vp(out)))
+        s._ck(lib.mmp_scale_eval(s.h, vp(rec), n, vp(p), vp(out)))
         op = np.zeros(1, dtype=ob.SCALE_PARAMS)
         for k in op.dtype.names:
             if k != "pad":
                 op[k] = p[k]
         up = np.zeros(n, dtype=ob.SCALE_OUT)
         down = np.zeros(n, dtype=ob.SCALE_OUT)
-        assert oracle_lib.orc_rate_task_eval(o.h, n, _vp(orec), _vp(op), names, len(fl.type_names), _vp(tidx), _vp(eoff), _vp(einst),
-                                             _vp(ets), _vp(nl), _vp(up)) == 0
-        assert oracle_lib.orc_janitor_eval(o.h, n, _vp(orec), _vp(op), _vp(eoff), _vp(einst), _vp(ets), _vp(nl), _vp(lulr), _vp(down)) == 0
+        assert oracle_lib.orc_rate_task_eval(o.h, n, vp(orec), vp(op), names, len(fl.type_names), vp(tidx), vp(eoff), vp(einst),
+                                             vp(ets), vp(nl), vp(up)) == 0
+        assert oracle_lib.orc_janitor_eval(o.h, n, vp(orec), vp(op), vp(eoff), vp(einst), vp(ets), vp(nl), vp(lulr), vp(down)) == 0
         for k in ("action", "copies_to_load", "load_last_used", "rpm", "i1", "i2", "set_heavy"):
             bad = np.nonzero(out[k] != up[k])[0]
             assert len(bad) == 0, (thr, k, len(bad), bad[:5], out[bad[:5]], up[bad[:5]], rec[bad[:5]])
@@ -278,7 +259,7 @@ def test_partition_heavy_closed_loop_matches_oracle(product_lib, oracle_lib):
     w = make_churn(30_000, 1_500, seed, fill=0.90)
     _partition_heavy(w.fleet, seed)
     fl = w.fleet
-    o, sim, s = _build(product_lib, w, slots=256)
+    o, sim, s = build(product_lib, w, slots=256)
     n_p = len(s.stats(cap=fl.n_instances + 2)[0]) - 1
     ost, _ = o.partition_stats(cap=fl.n_instances + 2)
     n_o = int(np.count_nonzero(ost["instance_count"] > 0))
@@ -288,7 +269,7 @@ def test_partition_heavy_closed_loop_matches_oracle(product_lib, oracle_lib):
     for ep in range(6):
         ev = w.events(ep, 3000, seed)
         now0 = fl.now_ms + ep * w.window_ms
-        dec, evi, rep = _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
+        dec, evi, rep = compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
         totals["dec"] += len(dec); totals["acc"] += int(np.count_nonzero(dec["status"] == ob.SIM_ACCEPTED))
         totals["evict"] += len(evi); totals["reload"] += int(evi["reload"].sum())
     print(totals)
@@ -331,7 +312,7 @@ def _boundary_fleet(case, seed=31):
 @pytest.mark.parametrize("case", ["lru_max", "lru_mix", "is_full_edge", "count_wrap", "capacity_wrap", "all_down"])
 def test_boundary_stats_match_oracle(product_lib, oracle_lib, case):
     fl = _boundary_fleet(case)
-    o = _converged_oracle(fl)
+    o = converged_oracle(fl)
     s = solver_from_synth(fl, product_lib)
     st, ids, n_o = _check_stats(fl, o, s)
     g = st[0]
@@ -387,7 +368,7 @@ def _edge_fleet(regime):
             rows["used"][:3] = 1 << 61
             for i in range(3):
                 fl.inst_labels[i] = ["lbl-00", "lbl-01", "lbl-02", "lbl-03"]
-        _EDGE_FLEETS[regime] = (fl, _converged_oracle(fl))
+        _EDGE_FLEETS[regime] = (fl, converged_oracle(fl))
     return _EDGE_FLEETS[regime]
 
 
@@ -442,7 +423,7 @@ def test_reaper_selection_edges(product_lib, oracle_lib, regime, n):
     total = len(sel_c) + sum(len(a) for a in sel_p)
     assert total > 0
     # a cap below the selection: the full count comes back, the first `cap` ids are written, every selected model is taken
-    pmap = _partition_maps(fl, o, s)
+    pmap = partition_maps(fl, o, s)
     om = _om(fl)
     for pid in [-1] + [int(p) for p in ids[1:]]:
         taken_o = np.zeros(n, np.uint8)
@@ -452,7 +433,7 @@ def test_reaper_selection_edges(product_lib, oracle_lib, regime, n):
         cap = len(a) // 2
         out = np.full(cap + 4, -7, dtype=np.int32)
         taken_s = np.zeros(n, np.uint8)
-        k = s._ck(product_lib.mmp_reaper_select(s.h, pid, now, _vp(taken_s), _vp(out), cap))
+        k = s._ck(product_lib.mmp_reaper_select(s.h, pid, now, vp(taken_s), vp(out), cap))
         assert k == len(a) and np.array_equal(out[:cap], a[:cap]) and (out[cap:] == -7).all(), (pid, k, len(a))
         assert np.array_equal(taken_s, taken_o) and int(taken_s.sum()) == len(a)
         break
@@ -472,7 +453,7 @@ def test_reaper_total_count_edges(product_lib, oracle_lib, regime):
     probe = _with_registry(fl0, cutoff + 1 + np.arange(n_probe), np.zeros(n_probe), np.zeros(n_probe), np.full(n_probe, untyped))
     s = solver_from_synth(probe, product_lib)
     st, ids = s.stats(cap=fl0.n_instances + 2)
-    pmap = _partition_maps(probe, o, s)
+    pmap = partition_maps(probe, o, s)
     target = None
     for pid in [-1] + [int(p) for p in ids[1:]]:
         a = o.reaper_select(_om(probe), probe.type_names, pid if pid < 0 else pmap[pid], now)
@@ -495,7 +476,7 @@ def test_reaper_total_count_edges(product_lib, oracle_lib, regime):
         pid = target
         if pid >= 0:  # the same partition in this fleet's numbering
             want = pmap[pid]
-            pid = next(int(p) for p, q in _partition_maps(f, o, s2).items() if q == want)
+            pid = next(int(p) for p, q in partition_maps(f, o, s2).items() if q == want)
         taken_o, taken_s = np.zeros(len(lu), np.uint8), np.zeros(len(lu), np.uint8)
         a = o.reaper_select(_om(f), f.type_names, target if target < 0 else pmap[target], now, taken=taken_o)
         b = s2.reaper_select(pid, now, taken=taken_s)
@@ -521,14 +502,14 @@ def _zero_estimate_fleet(with_candidates):
 @pytest.mark.parametrize("with_candidates", [True, False])
 def test_reaper_zero_size_estimate(product_lib, oracle_lib, with_candidates):
     fl = _zero_estimate_fleet(with_candidates)
-    o = _converged_oracle(fl)
+    o = converged_oracle(fl)
     s = solver_from_synth(fl, product_lib)
     g = o.cluster_stats()
     assert int(g["total_capacity"]) == int(g["total_free"]) > 0 and int(g["model_copy_count"]) > 10
     om = _om(fl)
     out = np.zeros(fl.n_models, dtype=np.int32)
     names = (C.c_char_p * len(fl.type_names))(*[t.encode() for t in fl.type_names])
-    rc = oracle_lib.orc_reaper_select(o.h, fl.n_models, _vp(om), names, len(fl.type_names), -1, fl.now_ms, None, _vp(out), len(out))
+    rc = oracle_lib.orc_reaper_select(o.h, fl.n_models, vp(om), names, len(fl.type_names), -1, fl.now_ms, None, vp(out), len(out))
     if with_candidates:
         assert rc == -4  # the reference's ArithmeticException (MM:6651)
         with pytest.raises(MmpError) as e:

@@ -5,11 +5,11 @@ Checked against the unsharded solver (which the other parity tests pin to the or
 CUDA library; the gloo test runs the same exchange with torch.distributed all_reduce(MIN) on two processes."""
 import ctypes as C
 import os
-import socket
 
 import numpy as np
 import pytest
 
+from helpers import free_port
 from modelmesh_b200 import _lib
 from modelmesh_b200.fleet import Fleet
 from modelmesh_b200.sharding import combine_shard_keys, decode_shard_keys
@@ -64,14 +64,6 @@ def test_min_loc_combine_matches_unsharded(emul_lib, config, nm, ni, seed, world
     assert not o1.any() and np.array_equal(t1, ref["target"]) and np.array_equal(c1, ref["n_candidates"])
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _worker(rank, world, port, so_path, q):
     import torch
     import torch.distributed as dist
@@ -98,7 +90,7 @@ def test_two_process_gloo_exchange(emul_lib):
     so = emul_lib._name
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, so, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -4,11 +4,11 @@ from / results stored to peers' memory through CUDA IPC mappings, k_place_dealt)
 unsharded solver returns.  Needs >= 2 GPUs; skipped on
 a single-GPU box.  The protocol itself is covered on CPU by test_instance_shards_cpu.py."""
 import os
-import socket
 
 import numpy as np
 import pytest
 
+from helpers import free_port
 from modelmesh_b200.synth import load_into_fleet, make_decisions, make_fleet
 
 CASES = [("C3", 3000, 10000, 3), ("C5", 2000, 5000, 5), ("MIX", 500, 700, 8), ("MIX", 500, 300, 14), ("C2", 3000, 1000, 2)]
@@ -69,14 +69,6 @@ def _worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("world", [2, 4, 8])
 def test_sharded_matches_unsharded(product_lib, world):
@@ -87,7 +79,7 @@ def test_sharded_matches_unsharded(product_lib, world):
     from modelmesh_b200.fleet import Fleet
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
     for p in procs:
         p.start()

@@ -3,30 +3,17 @@
     179 999 and 180 000, a failure without an entry, a failed entry on a loaded registration, equal-lastUsed candidates (N15),
     the budget (a first removal over it allowed, a later heavy one refused, a later light one allowed), a registration time
     that is not the entry's loadTimestamp, and Long.MAX_VALUE as an entry's lastUsed;
-  * its removeModelCopies part (orc_janitor_eval) against brute_janitor_entry of tests/test_oracle_properties.py."""
+  * its removeModelCopies part (orc_janitor_eval) against brute_janitor_entry of tests/brute.py."""
 import numpy as np
 
 import janitor_run_oracle as jro
+from common import EXPIRY, HOUR, LONG_MAX
 from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import make_fleet
 from pod_task_edges import janitor_hand_fleet as hand_fleet
-from test_oracle_properties import brute_janitor_entry
-
-EXPIRY = 900_000          # LOAD_FAILURE_EXPIRY_MS
-LONG_MAX = np.iinfo(np.int64).max
-HOUR = 3_600_000
-
-
-def params(now, adjusted_capacity, flags=0):
-    p = np.zeros(1, dtype=L.JANITOR_PARAMS)
-    s = p["scale"]
-    s["now"], s["last_check_time"], s["iteration"], s["scale_up_rpm_threshold"] = now, now - 10_000, 5000, 2000
-    s["rate_check_interval_ms"], s["assume_completed_ms"], s["second_copy_remove_max_age_ms"] = 10_000, 30_000, 1000
-    p["scale"] = s
-    p["load_failure_expiry_ms"], p["adjusted_capacity"], p["flags"] = EXPIRY, adjusted_capacity, flags
-    return p
-
+from pod_tasks import janitor_params
+from brute import brute_janitor_entry
 
 def entry(model, last_used, weight=10, load_ts=0, failed=False, last_heavy=0, count=0):
     e = np.zeros(1, dtype=L.JANITOR_ENTRY)
@@ -78,7 +65,7 @@ def test_known_answers(oracle_lib):
     now = fl.now_ms
     rec_lu = now - HOUR
     # budget 100: model 6 (5, first removal), 9 (60), 10 refused (50 > 35), 11 (30)
-    edits, rep = jro.janitor_run(o, fl, ts, lul, S, ents, params(now, 2000))
+    edits, rep = jro.janitor_run(o, fl, ts, lul, S, ents, janitor_params(now, 2000))
     got = {m: (w, lu, ul) for m, w, lu, ul in edits}
     assert got[1] == (L.JE_DROP_FAILURE, rec_lu, 0)
     assert got[2] == (L.JE_DROP_FAILURE | L.JE_REMOVE_LOCAL, now - 179_999, 0)
@@ -91,15 +78,15 @@ def test_known_answers(oracle_lib):
     assert set(got) == {1, 2, 4, 5, 6, 9, 11, 12, 13}   # 0, 3 kept; 7 dropped by N15; 8 load_ts; 10 over the budget
     assert rep == dict(n_referencing=14, n_edits=9, n_candidates=6, n_removed=3, weight_removed=95)
     # budget 50: model 6 (5), then 9 (60 > 45) refused, 10 (50) refused, 11 (30) allowed
-    edits, rep = jro.janitor_run(o, fl, ts, lul, S, ents, params(now, 1000))
+    edits, rep = jro.janitor_run(o, fl, ts, lul, S, ents, janitor_params(now, 1000))
     assert [m for m, w, _, _ in edits if w & L.JE_SCALE_DOWN] == [6, 11] and rep["weight_removed"] == 35
     # without models 6 and 7 the first removal (60) exceeds the budget of 50 and is allowed; nothing fits after it
-    edits, rep = jro.janitor_run(o, fl, ts, lul, S, ents[~np.isin(ents["model"], [6, 7])], params(now, 1000))
+    edits, rep = jro.janitor_run(o, fl, ts, lul, S, ents[~np.isin(ents["model"], [6, 7])], janitor_params(now, 1000))
     assert [m for m, w, _, _ in edits if w & L.JE_SCALE_DOWN] == [9] and rep["n_removed"] == 1
     # every candidate removable but the mismatched load_ts with the budget out of the way
-    assert jro.remove_model_copies(o, fl, ts, lul, S, 8, ents[ents["model"] == 8][0], params(now, 1000)[0], 1) == 1
-    assert jro.remove_model_copies(o, fl, ts, lul, S, 7, ents[ents["model"] == 7][0], params(now, 1000)[0], 1) == 1
-    assert jro.remove_model_copies(o, fl, ts, lul, S, 12, ents[ents["model"] == 12][0], params(now, 1000)[0], 1) == 0
+    assert jro.remove_model_copies(o, fl, ts, lul, S, 8, ents[ents["model"] == 8][0], janitor_params(now, 1000)[0], 1) == 1
+    assert jro.remove_model_copies(o, fl, ts, lul, S, 7, ents[ents["model"] == 7][0], janitor_params(now, 1000)[0], 1) == 1
+    assert jro.remove_model_copies(o, fl, ts, lul, S, 12, ents[ents["model"] == 12][0], janitor_params(now, 1000)[0], 1) == 0
     o.close()
 
 
@@ -125,7 +112,7 @@ def test_remove_model_copies_matches_brute_force(oracle_lib):
     for S in range(fl.n_instances):
         S = int(S)
         local = pst.get(o.instance_partition(S)) if have_tc else gst   # instanceSetStats() of the pod
-        p = params(fl.now_ms, 10_000)[0]
+        p = janitor_params(fl.now_ms, 10_000)[0]
         p["scale"]["second_copy_remove_max_age_ms"] = 36 * HOUR
         for m in range(fl.n_models):
             a, k = int(fl.edge_off[m]), int(fl.n_loaded[m])

@@ -14,27 +14,17 @@ import numpy as np
 import pytest
 
 import janitor_task_oracle as jto
-from helpers import oracle_from_synth, solver_from_synth
+from common import HOUR, LONG_MAX, vp
+from helpers import oracle_from_synth
+from janitor_task_cases import CASES
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet, MmpError
 from modelmesh_b200.synth import load_into_fleet, make_fleet
+from pod_tasks import (MIN_STALE, WINDOW, TimedReplay, busiest_pod, janitor_entries, janitor_task_params, janitor_workload, report_dict,
+                       timed_solver)
 from replay import run_window
-from test_janitor_run_gpu import _build, _entries, _workload
-from test_janitor_run_oracle import HOUR, LONG_MAX
-from test_janitor_task_oracle import CASES, MIN_STALE, WINDOW, params
-from test_registry_overflow_gpu import _TimedReplay
 
 pytestmark = pytest.mark.gpu
-vp = lambda a: a.ctypes.data_as(C.c_void_p)
-REPORT_FIELDS = ["n_not_done", "n_not_cached", "n_out_of_order", "n_stop", "n_repair", "n_not_reached", "n_stale_update", "n_remove",
-                 "n_reregister", "n_undecided", "stopped_at", "registry_ran", "cache_changed"]
-REGISTRY_FIELDS = ["n_referencing", "n_edits", "n_candidates", "n_removed", "weight_removed"]
-
-
-def _report(r):
-    d = {k: getattr(r, k) for k in REPORT_FIELDS}
-    d["registry"] = {k: getattr(r.registry, k) for k in REGISTRY_FIELDS}
-    return d
 
 
 def _check(s, o, fl, ts, lul, S, ents, p, cap=None):
@@ -45,7 +35,7 @@ def _check(s, o, fl, ts, lul, S, ents, p, cap=None):
     got = [(int(e["model"]), int(e["what"]), int(e["last_used"]), int(e["last_unload_time"])) for e in edits]
     n = len(want_edits) if cap is None else min(cap, len(want_edits))
     assert got == want_edits[:n], next(((a, b) for a, b in zip(got, want_edits) if a != b), (len(got), len(want_edits)))
-    assert _report(r) == want_rep
+    assert report_dict(r) == want_rep
     t = C.c_double()
     s._ck(s.lib.mmp_last_timing(s.h, b"janitor_task", C.byref(t)))
     assert t.value > 0
@@ -53,10 +43,10 @@ def _check(s, o, fl, ts, lul, S, ents, p, cap=None):
 
 
 def _task_entries(fl, ts, S, rng, with_stop, n_unreg=40):
-    """test_janitor_run_gpu's cache, in most-recently-used order with a few neighbours swapped (out of order), as task entries:
+    """janitor_entries' cache, in most-recently-used order with a few neighbours swapped (out of order), as task entries:
     some undone, some out of LOADING..ACTIVE or unloaded recently, some recent; failed ones carry their failure time or not;
     Long.MAX_VALUE entries only with_stop"""
-    base = _entries(fl, ts, S, rng, n_unreg)
+    base = janitor_entries(fl, ts, S, rng, n_unreg)
     te = np.zeros(len(base), dtype=L.JANITOR_TASK_ENTRY)
     te["e"] = base
     e = te["e"]
@@ -95,13 +85,13 @@ def _task_entries(fl, ts, S, rng, with_stop, n_unreg=40):
 
 
 def _tparams(now, cap_units=2_000, flags=0, min_stale=MIN_STALE):
-    return params(now, cap_units, flags, min_stale=min_stale)
+    return janitor_task_params(now, cap_units, flags, min_stale=min_stale)
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [("C2", 3000, 400, 2), ("C3", 6000, 400, 3), ("MIX", 1500, 320, 14), ("MIX", 1500, 400, 41)])
 def test_janitor_task_matches_the_restatement(product_lib, oracle_lib, config, nm, ni, seed):
-    fl, ts, lul, S = _workload(config, nm, ni, seed, wide=True, saturated=True)
-    s, o = _build(product_lib, fl, ts, lul), oracle_from_synth(fl)
+    fl, ts, lul, S = janitor_workload(config, nm, ni, seed, wide=True, saturated=True)
+    s, o = timed_solver(product_lib, fl, ts, lul), oracle_from_synth(fl)
     seen = 0
     for with_stop in (False, True):
         ents = _task_entries(fl, ts, S, np.random.default_rng(seed + with_stop), with_stop)
@@ -119,7 +109,7 @@ def test_janitor_task_matches_the_restatement(product_lib, oracle_lib, config, n
 
 
 def test_janitor_task_replayed_stream(product_lib, oracle_lib):
-    rp = _TimedReplay(make_fleet("C3", 3000, 600, 3), product_lib, 3)
+    rp = TimedReplay(make_fleet("C3", 3000, 600, 3), product_lib, 3)
     seen = set()
     for w in range(12):
         run_window(rp, w)
@@ -128,14 +118,8 @@ def test_janitor_task_replayed_stream(product_lib, oracle_lib):
             continue
         seen.add(path)
         v, o = rp.view(), rp.oracle()
-        ts = np.zeros(len(v.edge_inst), dtype=np.int64)
-        lul = np.zeros(v.n_models, dtype=np.int64)
-        for m, (t, u) in rp.times.items():
-            a, b = int(v.edge_off[m]), int(v.edge_off[m + 1])
-            k = min(len(t), b - a)
-            ts[a:a + k] = t[:k]
-            lul[m] = u
-        S = int(np.argmax(np.bincount(v.edge_inst, minlength=v.n_instances)))
+        ts, lul = rp.view_times(v)
+        S = busiest_pod(v)
         ents = _task_entries(v, ts, S, np.random.default_rng(w), False, n_unreg=10)
         _, edits, _ = _check(rp.f, o, v, ts, lul, S, ents, _tparams(rp.now, 1 << 40))
         assert edits
@@ -148,10 +132,7 @@ def test_janitor_task_replayed_stream(product_lib, oracle_lib):
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_janitor_task_hand_cases(product_lib, oracle_lib, name):
     c = CASES[name]()
-    s = solver_from_synth(c.fl, product_lib, max_models=c.max_models)
-    for m in range(c.fl.n_models):
-        s.model_times(m, c.ts[c.fl.edge_off[m]:c.fl.edge_off[m + 1]], int(c.lul[m]))
-    s.commit()
+    s = timed_solver(product_lib, c.fl, c.ts, c.lul, max_models=c.max_models)
     o = oracle_from_synth(c.fl)
     _check(s, o, c.fl, c.ts, c.lul, c.S, c.entries, c.params)
     s.close()
@@ -160,8 +141,8 @@ def test_janitor_task_hand_cases(product_lib, oracle_lib, name):
 
 @pytest.fixture(scope="module")
 def edge_fleet(product_lib):
-    fl, ts, lul, S = _workload("C3", 3200, 400, 9)
-    return fl, ts, lul, S, _build(product_lib, fl, ts, lul)
+    fl, ts, lul, S = janitor_workload("C3", 3200, 400, 9)
+    return fl, ts, lul, S, timed_solver(product_lib, fl, ts, lul)
 
 
 @pytest.mark.parametrize("n", [1, 255, 256, 257, 511, 512, 513, 1023, 1024, 1025])
@@ -200,9 +181,9 @@ def test_janitor_task_block_edges(edge_fleet, oracle_lib, n):
 def test_janitor_task_without_writes_is_janitor_run(product_lib, oracle_lib):
     """entries the cache pass writes nothing for (recent, with records that are not stale; undone ones) give mmp_janitor_run's
     edits and registry report on the same entries, byte for byte"""
-    fl, ts, lul, S = _workload("C3", 6000, 400, 3, wide=True, saturated=True)
-    s = _build(product_lib, fl, ts, lul)
-    base = _entries(fl, ts, S, np.random.default_rng(3))
+    fl, ts, lul, S = janitor_workload("C3", 6000, 400, 3, wide=True, saturated=True)
+    s = timed_solver(product_lib, fl, ts, lul)
+    base = janitor_entries(fl, ts, S, np.random.default_rng(3))
     base["last_used"] = np.where(base["last_used"] == LONG_MAX, fl.now_ms - 1000, base["last_used"])
     te = np.zeros(len(base), dtype=L.JANITOR_TASK_ENTRY)
     te["e"] = base

@@ -10,10 +10,11 @@ import time
 import numpy as np
 import pytest
 
+from churn_harness import build, compare_window
 from modelmesh_b200 import _lib as L
 from lru_read_oracle import _read_oracle_so, lru_last_used, lru_read, lru_weight, read_oracle, sim_lru_read  # noqa: F401
 from modelmesh_b200.fleet import MmpError, _ptr
-from test_lru_edges_gpu import INSERT, NOW0, SETCAP, TOUCH, Gen, Ref, check, events, fleet
+from lru_ref import INSERT, NOW0, SETCAP, TOUCH, Gen, Ref, check, events, fleet
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("read_oracle")]
 
@@ -264,18 +265,17 @@ def _check_loop_caches(ep, sim, s, fl, pairs):
 @pytest.mark.parametrize("with_types", [False, True])
 def test_closed_loop_reads_match_oracle(product_lib, oracle_lib, overflow, with_types):
     from modelmesh_b200.synth import make_churn, make_churn_overflow
-    from test_churn_gpu import _build, _compare_window
     seed = 4 + with_types
     w = make_churn(20_000, 200, seed, fill=0.90, with_types=with_types)
     if overflow:
         w = make_churn_overflow(w, 0.05, seed)
     fl = w.fleet
-    o, sim, s = _build(product_lib, w, slots=256)
+    o, sim, s = build(product_lib, w, slots=256)
     _check_loop_caches(-1, sim, s, fl, True)
     for ep in range(8):
         ev = w.events(ep, 2000, seed)
         now0 = fl.now_ms + ep * w.window_ms
-        _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
+        compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, seed * 100 + ep)
         _check_loop_caches(ep, sim, s, fl, ep in (3, 7))
 
 

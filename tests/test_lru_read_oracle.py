@@ -11,7 +11,7 @@ import pytest
 
 from lru_read_oracle import _read_oracle_so, lru_last_used, lru_read, lru_weight, read_oracle  # noqa: F401 (fixtures)
 from oracle import binding as ob
-from test_oracle_properties import BruteLru
+from brute import BruteLru
 
 pytestmark = pytest.mark.usefixtures("read_oracle")
 

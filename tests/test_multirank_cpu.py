@@ -1,7 +1,6 @@
 """world_size-2 (and 3) gloo tests of the N>1 host logic: registry sharding, gather of per-shard results, max-over-ranks
 timing reduction — on CPU, with the tests/emul harness standing in for the CUDA library."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -9,6 +8,7 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from helpers import free_port
 from modelmesh_b200.sharding import localize_decisions, owner_of, shard_range
 
 
@@ -26,14 +26,6 @@ def test_shard_range_and_owner():
             for i, o in zip(idx, own):
                 lo, hi = shard_range(int(o), w, n)
                 assert lo <= i < hi
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _worker(rank, world, port, so_path, q):
@@ -92,7 +84,7 @@ def test_registry_sharded_placement_matches_unsharded(emul_lib, world):
     so = emul_lib._name
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, world, port, so, q)) for r in range(world)]
     for p in procs:
         p.start()

@@ -18,6 +18,8 @@ shortlist as a sorted-prefix enumeration), must give the same ordered shortlist,
 import numpy as np
 import pytest
 
+from brute import BruteLru, brute_compare, brute_janitor_entry, free_space, trunc_div
+from common import vp
 from helpers import oracle_from_synth, oracle_inputs
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import LONG_MAX, make_decisions, make_fleet
@@ -48,10 +50,6 @@ def _java_int(d):  # (int) double: truncation toward zero, saturating
     return max(-(1 << 31), min((1 << 31) - 1, int(d)))
 
 
-def _rem(r):
-    return max(0, int(r["capacity"]) - int(r["used"]))
-
-
 def brute_get_next(order, rows, ids, active, replaced, min_space, self_idx, fresh, favour_self, last_used, excluded, now, rnd):
     """getNext for a type WITHOUT constraints or preferences (constrainTo == null, prefer == null), naive form."""
     def in_filter(i, use_rs):
@@ -69,7 +67,7 @@ def brute_get_next(order, rows, ids, active, replaced, min_space, self_idx, fres
     exclude_self = self_idx in excluded
     us = best == self_idx and not exclude_self                          # MM:4808
     best_rec = fresh if us else rows[best]
-    best_full = _rem(best_rec) < min_space
+    best_full = free_space(best_rec) < min_space
     if us and favour_self:
         return dict(target=ob.SELF, cands=[], keep=[], n_remaining=0, pick=0)
     cands, loads = [best], [int(best_rec["rpm"])]
@@ -84,8 +82,8 @@ def brute_get_next(order, rows, ids, active, replaced, min_space, self_idx, fres
             if diff > 45_000 and diff > a10:
                 break
         else:
-            rem = _rem(cur)
-            if rem < min_space or rem < (_rem(best_rec) >> 2):
+            rem = free_space(cur)
+            if rem < min_space or rem < (free_space(best_rec) >> 2):
                 break
             cnt, first = int(rows[i]["count"]), int(best_rec["count"])
             if cnt >= 10 and cnt > first + (first >> 2):
@@ -271,7 +269,7 @@ def brute_get_next_tc(order, rows, ids, active, replaced, min_space, self_idx, f
     best_iid = best_entry
     us = (not exclude_self) and best_iid == self_idx
     best_inst = fresh if us else rows[best_iid]
-    best_is_full = _rem(best_inst) < min_space                          # final: keeps the FIRST entry's verdict
+    best_is_full = free_space(best_inst) < min_space                     # final: keeps the FIRST entry's verdict
     cands, loads = [], []
     case = "simple"
     simple = prefer is None or best_iid in prefer
@@ -286,7 +284,7 @@ def brute_get_next_tc(order, rows, ids, active, replaced, min_space, self_idx, f
                     best_inst = rows[ent]                               # ent.getValue(): the published record, even for self
                     us = (not us) and (not exclude_self) and ent == self_idx
                     break
-                if _rem(rows[ent]) < min_space:
+                if free_space(rows[ent]) < min_space:
                     break
                 replay.append(ent)
             case = "a_found" if found else "a_rewind"
@@ -330,8 +328,8 @@ def brute_get_next_tc(order, rows, ids, active, replaced, min_space, self_idx, f
                 if diff > 45_000 and diff > int(_age(oldest, now) / 10):
                     break
             else:
-                rem = _rem(cur)
-                if rem < min_space or rem < (_rem(best_inst) >> 2):
+                rem = free_space(cur)
+                if rem < min_space or rem < (free_space(best_inst) >> 2):
                     break
                 cnt, first = int(rows[ent]["count"]), int(best_inst["count"])
                 if cnt >= 10 and cnt > first + (first >> 2):
@@ -409,11 +407,6 @@ def test_constrained_brute_force_reached_every_case():
 # only: two candidates with the same lastUsed are ONE element -- N12), partitions visited in getPartitionStats() order with
 # the selected models nulled out of the shared candidate list.
 # ---------------------------------------------------------------------------------------------------------------
-def _trunc_div(a, b):  # Java integer division truncates toward zero
-    q = abs(a) // abs(b)
-    return q if (a >= 0) == (b >= 0) else -q
-
-
 def brute_reaper(stats, global_stats, insts_of_subset, rows, models, type_prohibited, default_size, now, taken):
     """stats / global_stats: ClusterStats dicts; insts_of_subset: instance indices the subset's loop visits (cluster order);
     models: list of (last_used, type_idx, n_loaded, n_failed); type_prohibited(type_idx) -> bool for this subset."""
@@ -428,21 +421,21 @@ def brute_reaper(stats, global_stats, insts_of_subset, rows, models, type_prohib
         else:
             used = stats["total_capacity"] - stats["total_free"]
             used32 = ((used + (1 << 31)) % (1 << 32)) - (1 << 31)       # (int) of a long
-            avg = _trunc_div(used32, stats["model_copy_count"])
-            size_est = avg if stats["model_copy_count"] > 10 else _trunc_div(avg + default_size, 2)
+            avg = trunc_div(used32, stats["model_copy_count"])
+            size_est = avg if stats["model_copy_count"] > 10 else trunc_div(avg + default_size, 2)
         space = 0
         for i in insts_of_subset:
             r = rows[i]
             max_loads = int(r["l_threads"]) * 50 - int(r["l_in_prog"])
             if max_loads <= 0:
                 continue
-            avail = _rem(r) - int(r["capacity"]) // 8
+            avail = free_space(r) - int(r["capacity"]) // 8
             if avail > 0:
                 space += min(avail, max_loads * size_est)
-        space = _trunc_div(space, 2)
-        free_count = _trunc_div(space, size_est)
-        total_count = max(free_count, _trunc_div(stats["total_capacity"], 20 * size_est))
-    cutoff = 0 if stats["global_lru"] == LONG_MAX else stats["global_lru"] + max(_trunc_div(_age(stats["global_lru"], now), 3), 1_200_000)
+        space = trunc_div(space, 2)
+        free_count = trunc_div(space, size_est)
+        total_count = max(free_count, trunc_div(stats["total_capacity"], 20 * size_est))
+    cutoff = 0 if stats["global_lru"] == LONG_MAX else stats["global_lru"] + max(trunc_div(_age(stats["global_lru"], now), 3), 1_200_000)
     to_load = []                                                        # [(lastUsed, model)], lastUsed descending, unique lastUsed
     for m in cands:
         if taken[m]:
@@ -526,7 +519,7 @@ def test_cluster_and_partition_stats_are_plain_sums(oracle_lib, config, nm, ni, 
     live = [int(x) for x in o.cluster_order()]                          # the instances in the cluster state (shutting-down ones are not)
     def sums(members):
         cap = sum(int(rows["capacity"][i]) for i in members)
-        free = sum(_rem(rows[i]) for i in members if _rem(rows[i]) >= fl.min_space_units)
+        free = sum(free_space(rows[i]) for i in members if free_space(rows[i]) >= fl.min_space_units)
         copies = sum(int(rows["count"][i]) for i in members)
         return cap, free, len(members), copies
     lrus = [int(rows["lru_time"][i]) for i in live if int(rows["lru_time"][i]) > 0]
@@ -570,8 +563,8 @@ def brute_rate_entry(e, p, inst_count, have_tc, tstats, loaded, failed, rows, or
         if suitable < 2:
             return o
     thr = p["scale_up_rpm_threshold"]
-    heavy = _trunc_div(thr * 3, 4)
-    rpm = _trunc_div(e["count"] * 60_000, time_delta)
+    heavy = trunc_div(thr * 3, 4)
+    rpm = trunc_div(e["count"] * 60_000, time_delta)
     o["rpm"] = rpm
     if rpm > heavy:
         o["set_heavy"] = 1
@@ -591,7 +584,7 @@ def brute_rate_entry(e, p, inst_count, have_tc, tstats, loaded, failed, rows, or
         if in1 or in2:
             if tstats["total_capacity"] == 0:
                 return o                                                # ArithmeticException, caught at MM:5797
-            if _trunc_div(10 * tstats["total_free"], tstats["total_capacity"]) >= 1 or \
+            if trunc_div(10 * tstats["total_free"], tstats["total_capacity"]) >= 1 or \
                     (p["now"] - tstats["global_lru"]) > p["second_copy_lru_threshold_ms"]:
                 o.update(action=1, copies_to_load=1, load_last_used=p["last_check_time"])
                 return o
@@ -611,52 +604,11 @@ def brute_rate_entry(e, p, inst_count, have_tc, tstats, loaded, failed, rows, or
         cand -= len(exclude)                                            # (sic: subtracted again, MM:5767)
         if cand <= 0:
             return o
-    copies = min(_trunc_div(rpm, thr), cand)
+    copies = min(trunc_div(rpm, thr), cand)
     if copies > 2:
         copies = min(copies, suitable // 3)
     o.update(action=2, copies_to_load=copies, load_last_used=p["now"] + 20_000)
     return o
-
-
-def brute_janitor_entry(e, p, have_tc, local_stats, loaded, lul, ids, shutting_down, pos):
-    """removeModelCopies for the entry's pod; local_stats: instanceSetStats() of that pod (None: EMPTY_STATS, quirk N13)."""
-    if not p["can_remove"] or e["last_used"] == 0 or len(loaded) < 2:
-        return 0
-    st = local_stats if local_stats is not None else dict(total_capacity=0, total_free=0, global_lru=LONG_MAX)
-    if st["total_capacity"] == 0 or _trunc_div(st["total_free"] * 100, st["total_capacity"]) > 5:
-        return 0
-    other = None
-    for i, _ in sorted(loaded, key=lambda x: ids[x[0]]):                # TreeMap key order
-        if i != e["instance"] and not shutting_down[i]:
-            other = i
-            break
-    if other is None:
-        return 0
-    now = p["now"]
-    if len(loaded) == 2:
-        cache_age = now - st["global_lru"]
-        down_age = _trunc_div(cache_age, 10)
-        if e["last_heavy"] == 0 or (now - e["last_heavy"]) < _trunc_div(cache_age, 5):
-            down_age = min(p["second_copy_remove_max_age_ms"], down_age)
-        if (now - e["last_used"]) > down_age:
-            if shutting_down[e["instance"]]:
-                return 0
-            return 0 if pos[other] > pos[e["instance"]] else 1         # PLACEMENT_ORDER.compare(other, this) > 0: the other pod flushes
-        return 0
-    if lul > 0 and now - lul < 8 * p["rate_check_interval_ms"]:
-        return 0
-    if any(ts > now - 1_800_000 for _, ts in loaded):
-        return 0
-    min_age = _trunc_div(3 * st["global_lru"] + 10_400_000, 100)
-    min_age = 600_000 if min_age < 600_000 else (18_000_000 if min_age > 18_000_000 else min_age)
-    if now - e["last_heavy"] < min_age:
-        return 0
-    since = now - p["last_check_time"]
-    if since < p["rate_check_interval_ms"] // 10:
-        return 0
-    if _trunc_div(e["count"] * 60_000, since) > _trunc_div(p["scale_up_rpm_threshold"] * 2, 3):
-        return 0
-    return 1
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [("C2", 3000, 300, 2), ("C3", 3000, 400, 3), ("C5", 3000, 400, 5), ("MIX", 1500, 160, 14),
@@ -697,7 +649,6 @@ def test_scale_arithmetic_parity_unpinned_by_reference_tests(oracle_lib, config,
     nl = n_loaded[m64].astype(np.int32)
     tidx = fl.model_type[m64].astype(np.int32)
     lulr = lul[m64].astype(np.int64)
-    vp = lambda a: a.ctypes.data_as(C.c_void_p)
     names = (C.c_char_p * len(fl.type_names))(*[t.encode() for t in fl.type_names])
     # what the brute force reads
     stat_names = ("total_capacity", "total_free", "global_lru", "instance_count", "model_copy_count")
@@ -860,55 +811,6 @@ def test_type_sets_parity_unpinned_by_reference_tests(oracle_lib, config, nm, ni
     assert checked == len(fl.type_names)
 
 
-def brute_compare(r1, id1, loc1, zone1, lab1, r2, id2, loc2, zone2, lab2, min_space, min_churn_age):
-    """PLACEMENT_ORDER.compare (MM:4646-4703) for two DIFFERENT records, from the Java text; returns the sign."""
-    sgn = lambda a, b: (a > b) - (a < b)
-    def nulls_last(a, b):
-        if a is None or b is None:
-            return 0 if a is b else (1 if a is None else -1)
-        return sgn(a, b)
-    sd1, sd2 = bool(r1["shutting_down"]), bool(r2["shutting_down"])
-    if sd1 != sd2:
-        return 1 if sd1 else -1
-    v1, v2 = int(r1["vers"]), int(r2["vers"])
-    rem1, rem2 = _rem(r1), _rem(r2)
-    full1, full2 = rem1 < min_space, rem2 < min_space
-    if v1 != v2:                                                         # N1: "prefer newer version unless it's saturated"
-        if v1 > v2:
-            if not full1 or int(r1["lru_time"]) > min_churn_age * 2:
-                return -1
-        elif not full2 or int(r2["lru_time"]) > min_churn_age * 2:
-            return 1
-    if full1 != full2:
-        return 1 if full1 else -1
-    if full1:
-        d = sgn(int(r1["lru_time"]), int(r2["lru_time"]))
-        if d:
-            return d
-    d = sgn(int(r1["count"]) - int(r2["count"]), 0)
-    if d:
-        return d
-    d = sgn(rem2, rem1)
-    if d:
-        return d
-    if not full1:
-        d = sgn(int(r1["lru_time"]), int(r2["lru_time"]))
-        if d:
-            return d
-    lip1, lip2 = int(r1["l_in_prog"]), int(r2["l_in_prog"])
-    for d in (sgn(int(r2["l_threads"]) - lip2, int(r1["l_threads"]) - lip1), sgn(lip1, lip2), sgn(int(r2["capacity"]), int(r1["capacity"])),
-              sgn(int(r1["rpm"]), int(r2["rpm"])), sgn(id1, id2), nulls_last(loc1, loc2), nulls_last(zone1, zone2)):
-        if d:
-            return d
-    l1, l2 = list(lab1 or []), list(lab2 or [])
-    if len(l1) != len(l2):
-        return sgn(len(l1), len(l2))
-    for a, b in zip(l1, l2):
-        if a != b:
-            return sgn(a, b)
-    return 0
-
-
 @pytest.mark.parametrize("mixed_vers", [False, True])
 @pytest.mark.parametrize("config,ni,seed", [("C2", 300, 2), ("C3", 400, 3), ("C5", 400, 5), ("MIX", 200, 8), ("MIX", 160, 14), ("MIX", 120, 21)])
 def test_placement_order_comparator_parity_unpinned_by_reference_tests(oracle_lib, config, ni, seed, mixed_vers):
@@ -938,94 +840,6 @@ def test_placement_order_comparator_parity_unpinned_by_reference_tests(oracle_li
             assert brute_compare(rows[a], fl.inst_ids[a], fl.inst_locs[a], fl.inst_zones[a], fl.inst_labels[a],
                                  rows[b], fl.inst_ids[b], fl.inst_locs[b], fl.inst_zones[b], fl.inst_labels[b],
                                  fl.min_space_units, fl.min_churn_age_ms) < 0
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# a10: the time-ordered weighted LRU (clhm/ConcurrentLinkedHashMap + LinkedDeque, single-threaded reading: every read is
-# drained at once) as a plain Python list, from the Java text: put / putIfAbsent (CLHM:821-858, AddTask 590-610), get
-# (731-738 -> touch 1357-1360 -> LinkedDeque.reposition / insert LD:243-288), replaceQuietly (963-984, UpdateTask 631-652),
-# remove (860-871), setCapacity (305-316: evict, notify, oldestTime NOT refreshed), forceSetLastUsedTime (756-768: no
-# reposition), evict from the head while weightedSize > capacity with |weight| on makeDead (329-352), oldestTime (1129-1133).
-# ---------------------------------------------------------------------------------------------------------------
-class BruteLru:
-    def __init__(self, capacity):
-        self.cap, self.wsize, self.oldest = capacity, 0, -1
-        self.deque = []          # [key, weight, lastUsed], oldest first
-        self.pending = []
-
-    def _find(self, key):
-        for n in self.deque:
-            if n[0] == key:
-                return n
-        return None
-
-    def _insert(self, node):    # LD:258-288: after the last element whose lastUsed <= ts, scanning from the tail
-        pos = len(self.deque)
-        while pos > 0 and self.deque[pos - 1][2] > node[2]:
-            pos -= 1
-        self.deque.insert(pos, node)
-
-    def _reposition(self, node):  # LD:243-255
-        i = next(k for k, n in enumerate(self.deque) if n is node)
-        lu = node[2]
-        if i == 0 or self.deque[i - 1][2] <= lu:
-            if i == len(self.deque) - 1 or self.deque[i + 1][2] >= lu:
-                return
-        del self.deque[i]
-        self._insert(node)
-
-    def _evict(self, ev_index):
-        while self.wsize > self.cap and self.deque:
-            k, w, lu = self.deque.pop(0)
-            self.wsize -= abs(w)
-            self.pending.append((k, ev_index, lu, w))
-
-    def _oldest(self):
-        self.oldest = self.deque[0][2] if self.deque else -1
-
-    def _after_read(self, node, last_used, now):
-        t = last_used if last_used > 0 else 0
-        node[2] = now if t == 0 else max(node[2], t)
-        self._reposition(node)
-        self._oldest()
-
-    def apply(self, op, key, weight, last_used, ev_index, now, out):
-        node = self._find(key)
-        if op == 0:
-            if node is None:
-                n = [key, weight, now if last_used == 0 else max(0, last_used)]
-                self.wsize += weight
-                self._insert(n)
-                self._evict(ev_index)
-                self._oldest()
-                out.extend(self.pending); self.pending = []
-            else:
-                self._after_read(node, last_used, now)
-        elif op == 1:
-            if node is not None:
-                self._after_read(node, last_used, now)
-        elif op == 2:
-            if node is not None:
-                diff = weight - node[1]
-                node[1] = weight
-                if diff != 0:
-                    self.wsize += diff
-                    self._evict(ev_index)
-                    self._oldest()
-                    if diff > 0:
-                        out.extend(self.pending); self.pending = []
-        elif op == 3:
-            if node is not None:
-                self.wsize -= abs(node[1])
-                self.deque.remove(node)
-                self._oldest()
-        elif op == 4:
-            self.cap = weight
-            self._evict(ev_index)
-            out.extend(self.pending); self.pending = []
-        elif op == 5:
-            if node is not None:
-                node[2] = last_used
 
 
 @pytest.mark.parametrize("seed", range(8))

@@ -9,7 +9,7 @@ import pytest
 from modelmesh_b200.synth import make_decisions, make_fleet
 
 from helpers import compare_decisions, oracle_from_synth, solver_from_synth
-from test_rolling_upgrade_gpu import fleet_for
+from upgrade import fleet_for
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [

@@ -20,41 +20,31 @@ import pytest
 
 import pod_task_edges as pe
 import rate_run_oracle as rro
-from helpers import oracle_from_synth, solver_from_synth
+from common import EXPIRY, HOUR
+from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import MmpError
 from modelmesh_b200.synth import make_fleet
-from test_evict_run_gpu import _composed as evict_composed, _rep as evict_rep
-from test_rate_run_gpu import _cross_check, _ids, _same_out
-from test_shutdown_run_gpu import _composed as shutdown_composed, _rep as shutdown_rep
+from pod_tasks import (IT, busiest_pod, composed_evict, composed_shutdown, cross_check_rate, evict_params, ids, janitor_params, rate_params,
+                       report_dict, same_out, shutdown_params, timed_solver)
 
 pytestmark = pytest.mark.gpu
 SIZES = (255, 256, 257, 511, 512, 513, 1025, 3000)
-
-
-def _build(lib, c):
-    s = solver_from_synth(c.fl, lib)
-    for m in range(c.fl.n_models):
-        s.model_times(m, c.ts[c.fl.edge_off[m]:c.fl.edge_off[m + 1]], int(c.lul[m]))
-    s.commit()
-    return s
 
 
 def _device(s, c):
     """c on the device, in the restatement's shape"""
     if c.task == "janitor":
         edits, r = s.janitor_run(c.pod, c.entries, c.params)
-        return ([(int(e["model"]), int(e["what"]), int(e["last_used"]), int(e["last_unload_time"])) for e in edits],
-                dict(n_referencing=r.n_referencing, n_edits=r.n_edits, n_candidates=r.n_candidates, n_removed=r.n_removed,
-                     weight_removed=r.weight_removed))
+        return [(int(e["model"]), int(e["what"]), int(e["last_used"]), int(e["last_unload_time"])) for e in edits], report_dict(r)
     if c.task == "rate":
         out, loads, r = s.rate_run(c.pod, c.entries, c.params, c.seed, fresh_self=c.fresh)
         return out, [tuple(int(x) for x in ld) for ld in loads], {k: getattr(r, k) for k in c.want[2]}
     if c.task == "shutdown":
         out, r = s.shutdown_run(c.pod, c.entries, c.params, c.seed, fresh_self=c.fresh)
-        return out, shutdown_rep(r)
+        return out, report_dict(r)
     out, r = s.evict_run(c.pod, c.entries, c.params, c.seed, fresh_self=c.fresh)
-    return out, evict_rep(r)
+    return out, report_dict(r)
 
 
 def _same(c, got):
@@ -62,7 +52,7 @@ def _same(c, got):
     if c.task == "janitor":
         return got[0] == w[0] and got[1] == w[1]
     if c.task == "rate":
-        return _same_out(got[0], w[0]) and got[1] == w[1] and got[2] == w[2]
+        return same_out(got[0], w[0]) and got[1] == w[1] and got[2] == w[2]
     return got[0].tobytes() == w[0].tobytes() and got[1] == w[1]
 
 
@@ -71,16 +61,16 @@ def _check(s, c, o=None):
     got = _device(s, c)
     assert _same(c, got), (c.name, got, c.want)
     if c.task == "shutdown":
-        assert shutdown_composed(s, c.pod, c.entries, got[0], c.params, c.seed, c.fresh) == got[1]["n_placed"]
+        assert composed_shutdown(s, c.pod, c.entries, got[0], c.params, c.seed, c.fresh) == got[1]["n_placed"]
     elif c.task == "evict":
-        assert evict_composed(s, c.pod, c.entries, got[0], c.params, c.seed, c.fresh) == got[1]["n_placed"]
+        assert composed_evict(s, c.pod, c.entries, got[0], c.params, c.seed, c.fresh) == got[1]["n_placed"]
     elif c.task == "rate" and got[2]["gate"] == L.RATE_RAN:
         own = o is None
         o = oracle_from_synth(c.fl) if own else o
         heavy = rro.heavy_set(o, c.fl, c.pod, int(c.params["scale"]["scale_up_rpm_threshold"][0]))
         if own:
             o.close()
-        _cross_check(s, c.fl, c.ts, c.pod, c.entries, c.params, c.seed, got[0], got[1], heavy, c.fresh)
+        cross_check_rate(s, c.fl, c.ts, c.pod, c.entries, c.params, c.seed, got[0], got[1], heavy, c.fresh)
     return got
 
 
@@ -90,7 +80,7 @@ def _run_all(lib, cases):
         for c in cases:
             k = c.fleet_key()
             if k not in fleets:
-                fleets[k] = _build(lib, c)
+                fleets[k] = timed_solver(lib, c.fl, c.ts, c.lul)
             _check(fleets[k], c)
     finally:
         for s in fleets.values():
@@ -125,10 +115,10 @@ def _shape_fleet():
     fl = make_fleet("C3", 3200, 400, 11)
     rng = np.random.default_rng(11)
     n, now = len(fl.edge_inst), fl.now_ms
-    ts = np.where(rng.uniform(size=n) < 0.3, now - rng.integers(0, pe.EXPIRY, size=n),
-                  now - rng.integers(pe.EXPIRY, 4 * pe.HOUR, size=n)).astype(np.int64)
+    ts = np.where(rng.uniform(size=n) < 0.3, now - rng.integers(0, EXPIRY, size=n),
+                  now - rng.integers(EXPIRY, 4 * HOUR, size=n)).astype(np.int64)
     lul = np.where(rng.uniform(size=fl.n_models) < 0.3, now - rng.integers(0, 200_000, size=fl.n_models), 0).astype(np.int64)
-    S = int(np.argmax(np.bincount(fl.edge_inst, minlength=fl.n_instances)))
+    S = busiest_pod(fl)
     return fl, ts, lul, S
 
 
@@ -147,28 +137,28 @@ def _shape_entries(fl, ts, S, n_max):
     u = rng.uniform(size=n)
     ev = np.zeros(n, dtype=L.EVICT_ENTRY)
     ev["model"], ev["load_ts"], ev["load_complete_ts"] = models, first_ts, first_ts
-    ev["last_used"] = np.where(u < 0.1, 0, now - rng.integers(1, pe.HOUR, size=n))
+    ev["last_used"] = np.where(u < 0.1, 0, now - rng.integers(1, HOUR, size=n))
     sd = np.zeros(n, dtype=L.SHUTDOWN_ENTRY)
     sd["model"] = models
-    sd["lru_t"] = np.where(u < 0.6, now - rng.integers(0, pe.HOUR, size=n), now - rng.integers(pe.HOUR, 6 * pe.HOUR, size=n))
-    sd["last_used"] = now - rng.integers(1, 3 * pe.HOUR, size=n)
+    sd["lru_t"] = np.where(u < 0.6, now - rng.integers(0, HOUR, size=n), now - rng.integers(HOUR, 6 * HOUR, size=n))
+    sd["last_used"] = now - rng.integers(1, 3 * HOUR, size=n)
     ra = np.zeros(n, dtype=L.SCALE_IN)
     ra["instance"], ra["model"] = S, models
     ra["count"] = np.where(u < 0.25, rng.integers(2000, 20_000, size=n), rng.integers(0, 200, size=n))
-    ra["last_used"] = now - rng.integers(0, pe.HOUR, size=n)
-    ra["i1"] = pe.IT - rng.integers(0, 400, size=n)
-    ra["i2"] = np.minimum(pe.IT, ra["i1"] + rng.integers(0, 300, size=n))
+    ra["last_used"] = now - rng.integers(0, HOUR, size=n)
+    ra["i1"] = IT - rng.integers(0, 400, size=n)
+    ra["i2"] = np.minimum(IT, ra["i1"] + rng.integers(0, 300, size=n))
     ja = np.zeros(n, dtype=L.JANITOR_ENTRY)
     ja["model"], ja["weight"], ja["load_ts"] = models, rng.integers(1, 400, size=n), first_ts
-    ja["last_used"] = now - rng.integers(1, 40 * pe.HOUR, size=n)
+    ja["last_used"] = now - rng.integers(1, 40 * HOUR, size=n)
     ja["flags"] = np.where(rng.uniform(size=n) < 0.1, L.JANITOR_FAILED, 0)
     return dict(evict=ev, shutdown=sd, rate=ra, janitor=ja)
 
 
 def _shape_case(fl, ts, lul, S, task, entries):
     now = fl.now_ms
-    params = dict(evict=pe.evict_params(now), shutdown=pe.shutdown_params(now), rate=pe.rate_params(now, 1000),
-                  janitor=pe.janitor_params(now, 1 << 40))[task]
+    params = dict(evict=evict_params(now), shutdown=shutdown_params(now), rate=rate_params(now, 1000),
+                  janitor=janitor_params(now, 1 << 40))[task]
     return pe.solved(pe.Case(task, fl, ts, lul, S, np.ascontiguousarray(entries), params, 23, None, f"shape/{task}/{len(entries)}"))
 
 
@@ -176,10 +166,7 @@ def test_shapes_duplicates_and_interleaving(product_lib, oracle_lib):
     fl, ts, lul, S = _shape_fleet()
     ents = _shape_entries(fl, ts, S, max(SIZES))
     o = oracle_from_synth(fl)
-    s = solver_from_synth(fl, product_lib)
-    for m in range(fl.n_models):
-        s.model_times(m, ts[fl.edge_off[m]:fl.edge_off[m + 1]], int(lul[m]))
-    s.commit()
+    s = timed_solver(product_lib, fl, ts, lul)
     alone = {}
     for n in SIZES:
         for task in pe.TASKS:
@@ -187,9 +174,9 @@ def test_shapes_duplicates_and_interleaving(product_lib, oracle_lib):
             alone[(task, n)] = (c, _check(s, c, o))
     # the rate runs draw past one tile: chains in at least two 512-entry tiles, decision ids of 512 and more
     c, (out, loads, _) = alone[("rate", max(SIZES))]
-    ids = _ids(fl, ts, c.entries, out, c.params)
-    chain_rows = np.nonzero((ids >= 0) & (out["action"] == 2))[0]
-    assert len(set(chain_rows // 512)) >= 2 and ids.max() >= 512 and any(ld[2] > 0 for ld in loads)
+    first = ids(fl, ts, c.entries, out, c.params)
+    chain_rows = np.nonzero((first >= 0) & (out["action"] == 2))[0]
+    assert len(set(chain_rows // 512)) >= 2 and first.max() >= 512 and any(ld[2] > 0 for ld in loads)
     # the shutdown and evict plans decide and place entries in their first block and in later ones (256 threads each)
     for task, bit in (("shutdown", L.SD_PLACED), ("evict", L.EV_PLACED)):
         placed = np.nonzero(alone[(task, max(SIZES))][1][0]["what"] & bit)[0]

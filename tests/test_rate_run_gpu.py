@@ -6,25 +6,24 @@
   * with heavy sets that are empty (C2: every published rpm 0), of at most 16, and of more than 1 000 members;
   * with caps below the load count, and on a replayed ingest stream after a device-path and after a host-path commit;
   * every argument error, MMP_E_EPOCH and MMP_E_STATE.
-Cross-checks: out is mmp_scale_eval's (can_remove = 0) field by field; round-0 scale-up loads are mmp_place_batch_excluding's
-under the heavy set with the same MMP_DF_OWN_ID ids; second copies are mmp_place_batch's with extra {self}."""
+Cross-checks (pod_tasks.cross_check_rate): out is mmp_scale_eval's (can_remove = 0) field by field; round-0 scale-up loads are
+mmp_place_batch_excluding's under the heavy set with the same MMP_DF_OWN_ID ids; second copies are mmp_place_batch's with extra
+{self}."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
 import rate_run_oracle as rro
-from helpers import oracle_from_synth, solver_from_synth
+from common import EXPIRY, HOUR, vp
+from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet, MmpError
 from modelmesh_b200.synth import load_into_fleet, make_fleet
+from pod_tasks import IT, TimedReplay, busiest_pod, cross_check_rate, held_models, rate_params, same_out, set_regs, timed_solver
 from replay import run_window
-from test_janitor_run_gpu import _set_regs
-from test_rate_run_oracle import EXPIRY, HOUR, IT, params
-from test_registry_overflow_gpu import _TimedReplay
 
 pytestmark = pytest.mark.gpu
-vp = lambda a: a.ctypes.data_as(C.c_void_p)
 # each fleet with what it is there to cover over its three thresholds (checked, so that a changed fleet does not stop covering it)
 FLEETS = [("C2", 3000, 400, 2, "no-heavy cut refused"), ("C3", 4000, 600, 3, "small-heavy cut refused"), ("C5", 3000, 500, 5, "second"),
           ("MIX", 1500, 320, 14, "small-heavy cut refused"), ("C3", 3000, 4000, 31, "large-heavy refused")]
@@ -38,17 +37,17 @@ def _workload(config, nm, ni, seed):
     u = rng.uniform(size=ni)
     rpm = np.where(u < 0.7, rng.integers(0, 21, size=ni), np.where(u < 0.9, rng.integers(21, 1500, size=ni), rng.integers(1500, 10_000, size=ni)))
     fl.inst_rows["rpm"] = 0 if config == "C2" else rpm
-    S = int(np.argmax(np.bincount(fl.edge_inst, minlength=ni)))
+    S = busiest_pod(fl)
     fl.inst_rows["rpm"][S] = min(int(fl.inst_rows["rpm"][S]), 20)
-    held = [int(m) for m in np.searchsorted(fl.edge_off, np.nonzero(fl.edge_inst == S)[0], side="right") - 1]
+    held = held_models(fl, S)
     changes = {}
     others = [i for i in range(ni) if i != S]
-    for m in rng.choice(sorted(set(held)), min(10, len(set(held))), replace=False):
+    for m in rng.choice(held, min(10, len(held)), replace=False):
         a, k, b = int(fl.edge_off[m]), int(fl.n_loaded[m]), int(fl.edge_off[m + 1])
         regs = list(fl.edge_inst[a:b])
         extra = [i for i in rng.choice(others, 8, replace=False) if i not in regs][:3]
         changes[int(m)] = (list(fl.edge_inst[a:a + k]), list(fl.edge_inst[a + k:b]) + extra)
-    _set_regs(fl, changes)
+    set_regs(fl, changes)
     n = len(fl.edge_inst)
     ts = np.where(rng.uniform(size=n) < 0.3, fl.now_ms - rng.integers(0, EXPIRY, size=n),
                   fl.now_ms - rng.integers(EXPIRY, 4 * HOUR, size=n)).astype(np.int64)
@@ -60,7 +59,7 @@ def _workload(config, nm, ni, seed):
 def _entries(fl, S, rng, n_unreg=30):
     """the pod's cache: every model it holds or has failed on, and models it does not hold, counts from idle to far past
     the threshold, usage iterations in and out of the second-copy window"""
-    mine = sorted(set(int(m) for m in np.searchsorted(fl.edge_off, np.nonzero(fl.edge_inst == S)[0], side="right") - 1))
+    mine = held_models(fl, S)
     rest = [m for m in range(fl.n_models) if m not in set(mine)]
     models = mine + [int(m) for m in rng.choice(rest, n_unreg, replace=False)]
     e = np.zeros(len(models), dtype=L.SCALE_IN)
@@ -74,22 +73,10 @@ def _entries(fl, S, rng, n_unreg=30):
     return e[rng.permutation(len(e))]
 
 
-def _build(lib, fl, ts):
-    s = solver_from_synth(fl, lib)
-    for m in range(fl.n_models):
-        s.model_times(m, ts[fl.edge_off[m]:fl.edge_off[m + 1]], 0)
-    s.commit()
-    return s
-
-
-def _same_out(x, y):
-    return all(np.array_equal(x[k], y[k]) for k in x.dtype.names)
-
-
 def _check(s, o, fl, ts, S, ents, p, seed, fresh=None, cap=None):
     out, loads, r = s.rate_run(S, ents, p, seed, fresh_self=fresh, loads_cap=cap)
     wout, wloads, wr = rro.rate_run(o, fl, ts, S, ents, p, seed, fresh_self=fresh)
-    assert _same_out(out, wout), next((k for k in out.dtype.names if not np.array_equal(out[k], wout[k])))
+    assert same_out(out, wout), next((k for k in out.dtype.names if not np.array_equal(out[k], wout[k])))
     got = [tuple(int(x) for x in ld) for ld in loads]
     assert got == wloads[:len(got)] and len(got) == (len(wloads) if cap is None else min(cap, len(wloads))), \
         next(((a, b) for a, b in zip(got, wloads) if a != b), (len(got), len(wloads)))
@@ -97,61 +84,21 @@ def _check(s, o, fl, ts, S, ents, p, seed, fresh=None, cap=None):
     return out, wloads, wr
 
 
-def _ids(fl, ts, ents, out, p):
-    """each entry's first decision id (the exclusive prefix sum of its decisions), -1 where it places none"""
-    now, expiry = int(p["scale"]["now"][0]), int(p["load_failure_expiry_ms"][0])
-    ids, off = np.full(len(ents), -1), 0
-    for r, (e, x) in enumerate(zip(ents, out)):
-        if int(x["action"]) in (1, 2) and not rro.refused(fl, ts, int(e["model"]), now, expiry):
-            ids[r] = off
-            off += 1 if int(x["action"]) == 1 else min(int(x["copies_to_load"]), L.RATE_CHAIN_MAX)
-    return ids
-
-
-def _cross_check(s, fl, ts, S, ents, p, seed, out, loads, heavy, fresh):
-    sp = p["scale"].copy()
-    sp["can_remove"] = 0
-    se = np.zeros(len(ents), dtype=L.SCALE_OUT)
-    s._ck(s.lib.mmp_scale_eval(s.h, vp(ents), len(ents), vp(sp), vp(se)))
-    assert _same_out(out, se)
-    ids = _ids(fl, ts, ents, out, p)
-    now = int(p["scale"]["now"][0])
-    kw = dict(fresh=None if fresh is None else np.asarray(fresh, dtype=L.INSTANCE_ROW).reshape(1))
-    for second in (True, False):
-        sel = [ld for ld in loads if ld[2] == 0 and bool(ld[7] & L.RL_SECOND_COPY) == second]
-        if not sel:
-            continue
-        d = np.zeros(len(sel), dtype=L.DECISION_IN)
-        for q, ld in enumerate(sel):
-            r, m = ld[0], ld[1]
-            a, k = int(fl.edge_off[m]), int(fl.n_loaded[m])
-            fav = second or S in set(int(i) for i in fl.edge_inst[a:a + k])
-            d["model"][q], d["self"][q], d["last_used"][q] = m, S, ld[6]
-            d["flags"][q] = (L.DF_FAVOUR_SELF if fav else 0) | L.DF_OWN_ID | (int(ids[r]) << 8)
-            d["fresh"][q] = -1 if fresh is None else 0
-            d["extra_off"][q], d["extra_n"][q] = 0, 1 if second else 0
-        if second:
-            res = s.place_batch(d, now, seed, extra=np.array([S], dtype=np.int32), **kw)
-        else:
-            res = s.place_batch(d, now, seed, exclude=np.asarray(heavy, dtype=np.int32), **kw)
-        assert [(int(x["target"]), int(x["n_candidates"])) for x in res] == [(ld[4], ld[5]) for ld in sel], second
-
-
 @pytest.mark.parametrize("config,nm,ni,seed,covers", FLEETS)
 def test_rate_run_matches_the_composition(product_lib, oracle_lib, config, nm, ni, seed, covers):
     fl, ts, S = _workload(config, nm, ni, seed)
     rng = np.random.default_rng(seed)
     ents = _entries(fl, S, rng)
-    s, o = _build(product_lib, fl, ts), oracle_from_synth(fl)
+    s, o = timed_solver(product_lib, fl, ts), oracle_from_synth(fl)
     fresh = fl.inst_rows[S].copy()
     fresh["used"] = fresh["used"] + fresh["capacity"] // 100
     seen = dict(second=0, up=0, cut=0, refused=0, heavy=set())
     for thr in (2000, 300, 5):
-        p = params(fl.now_ms, thr)
+        p = rate_params(fl.now_ms, thr)
         for fr in (None, fresh):
             out, loads, rep = _check(s, o, fl, ts, S, ents, p, 100 + thr, fresh=fr)
             heavy = rro.heavy_set(o, fl, S, thr)
-            _cross_check(s, fl, ts, S, ents, p, 100 + thr, out, loads, heavy, fr)
+            cross_check_rate(s, fl, ts, S, ents, p, 100 + thr, out, loads, heavy, fr)
             seen["second"] += rep["n_second"]
             seen["up"] += rep["n_scale_up"]
             seen["cut"] += rep["n_chains_cut"]
@@ -172,7 +119,7 @@ def test_rate_run_matches_the_composition(product_lib, oracle_lib, config, nm, n
 def test_rate_run_replayed_stream(product_lib, oracle_lib):
     """after a device-path commit and after a host-path commit of a replayed ingest stream whose upserts come with
     registration times"""
-    rp = _TimedReplay(make_fleet("C3", 3000, 600, 3), product_lib, 3)
+    rp = TimedReplay(make_fleet("C3", 3000, 600, 3), product_lib, 3)
     seen = set()
     for w in range(12):
         run_window(rp, w)
@@ -181,15 +128,11 @@ def test_rate_run_replayed_stream(product_lib, oracle_lib):
             continue
         seen.add(path)
         v, o = rp.view(), rp.oracle()
-        ts = np.zeros(len(v.edge_inst), dtype=np.int64)
-        for m, (t, _) in rp.times.items():
-            a, b = int(v.edge_off[m]), int(v.edge_off[m + 1])
-            k = min(len(t), b - a)
-            ts[a:a + k] = t[:k]
-        S = int(np.argmax(np.bincount(v.edge_inst, minlength=v.n_instances)))
+        ts, _ = rp.view_times(v)
+        S = busiest_pod(v)
         ents = _entries(v, S, np.random.default_rng(w), n_unreg=10)
         ents["count"] = np.maximum(ents["count"], 200)
-        _, loads, _ = _check(rp.f, o, v, ts, S, ents, params(rp.now, 300), 7)
+        _, loads, _ = _check(rp.f, o, v, ts, S, ents, rate_params(rp.now, 300), 7)
         assert loads
         o.close()
         if seen == {1, 2}:
@@ -200,16 +143,16 @@ def test_rate_run_replayed_stream(product_lib, oracle_lib):
 def test_rate_run_gates(product_lib, oracle_lib):
     fl, ts, S = _workload("C3", 1000, 200, 4)
     ents = _entries(fl, S, np.random.default_rng(4), n_unreg=5)
-    s, o = _build(product_lib, fl, ts), oracle_from_synth(fl)
+    s, o = timed_solver(product_lib, fl, ts), oracle_from_synth(fl)
     for delta, gate in ((5999, L.RATE_TOO_SOON), (6000, L.RATE_RAN)):
-        _, _, r = _check(s, o, fl, ts, S, ents, params(fl.now_ms, 300, delta=delta), 1)
+        _, _, r = _check(s, o, fl, ts, S, ents, rate_params(fl.now_ms, 300, delta=delta), 1)
         assert r["gate"] == gate
-    _, _, r = _check(s, o, fl, ts, S, ents[:0], params(fl.now_ms, 300), 1)
+    _, _, r = _check(s, o, fl, ts, S, ents[:0], rate_params(fl.now_ms, 300), 1)
     assert r["gate"] == L.RATE_NO_ENTRIES
     # a gated call still refuses two entries of one model
     dup = np.concatenate([ents[:2], ents[:1]])
     with pytest.raises(MmpError) as e:
-        s.rate_run(S, dup, params(fl.now_ms, 300, delta=10), 1)
+        s.rate_run(S, dup, rate_params(fl.now_ms, 300, delta=10), 1)
     assert e.value.code == L.E_ARG
     s.close()
     o.close()
@@ -221,7 +164,7 @@ def test_rate_run_gates(product_lib, oracle_lib):
     s.commit()
     e1 = np.zeros(1, dtype=L.SCALE_IN)
     e1["instance"], e1["model"], e1["count"], e1["i1"], e1["i2"] = 0, 0, 5000, 7, 9
-    out, loads, r = s.rate_run(0, e1, params(one.now_ms, 300), 1)
+    out, loads, r = s.rate_run(0, e1, rate_params(one.now_ms, 300), 1)
     assert r.gate == L.RATE_FEW_INSTANCES and len(loads) == 0 and out["action"][0] == 0 and (out["i1"][0], out["i2"][0]) == (7, 9)
     s.close()
 
@@ -229,7 +172,7 @@ def test_rate_run_gates(product_lib, oracle_lib):
 def test_rate_run_errors(product_lib):
     fl = make_fleet("C3", 200, 40, 5)
     s = Fleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, fl.n_instances, fl.n_models, lib=product_lib)
-    p = params(fl.now_ms, 1000)
+    p = rate_params(fl.now_ms, 1000)
     ents = np.zeros(2, dtype=L.SCALE_IN)
     ents["instance"], ents["model"] = 0, [3, 4]
     with pytest.raises(MmpError) as e:
@@ -256,7 +199,7 @@ def test_rate_run_errors(product_lib):
         b[field] = bad
         before = out.copy()
         assert call(**args(e=vp(b))) == L.E_ARG
-        assert _same_out(out, before)
+        assert same_out(out, before)
     assert call(**args(n=-1)) == L.E_ARG
     assert call(**args(pp=None)) == L.E_ARG
     assert call(**args(r_=None)) == L.E_ARG

@@ -7,25 +7,11 @@ ms after it."""
 import numpy as np
 
 import rate_run_oracle as rro
+from common import EXPIRY, HOUR
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import make_fleet
 from pod_task_edges import hand_fleet
-
-HOUR = 3_600_000
-EXPIRY = 900_000
-IT = 5000
-
-
-def params(now, thr, delta=10_000):
-    p = np.zeros(1, dtype=L.RATE_PARAMS)
-    s = p["scale"]
-    s["now"], s["last_check_time"], s["iteration"], s["scale_up_rpm_threshold"] = now, now - delta, IT, thr
-    s["second_copy_min_age_iters"], s["second_copy_max_age_iters"], s["second_copy_lru_threshold_ms"] = 42, 240, -1
-    s["rate_check_interval_ms"], s["assume_completed_ms"], s["second_copy_remove_max_age_ms"] = 10_000, 30_000, HOUR
-    p["scale"] = s
-    p["load_failure_expiry_ms"] = EXPIRY
-    return p
-
+from pod_tasks import IT, rate_params
 
 def entry(pod, model, rpm=0, second=False, delta=10_000):
     """an entry measuring rpm over delta ms; second: its usage iterations trigger the second-copy check"""
@@ -47,15 +33,15 @@ def test_gates_at_their_edges(oracle_lib):
     fl, ts, o = hand_fleet([([(0, 0)], [])], 4)
     now = fl.now_ms
     ents = entry(0, 0, rpm=5000, delta=6000)
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, params(now, 1000, delta=5999), 1)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, rate_params(now, 1000, delta=5999), 1)
     assert rep["gate"] == L.RATE_TOO_SOON and loads == [] and out["action"][0] == 0 and out["i1"][0] == ents["i1"][0]
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, params(now, 1000, delta=6000), 1)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, rate_params(now, 1000, delta=6000), 1)
     assert rep["gate"] == L.RATE_RAN and out["action"][0] == 2 and rep["n_scale_up"] == 1 and len(loads) > 0
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents[:0], params(now, 1000), 1)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents[:0], rate_params(now, 1000), 1)
     assert rep["gate"] == L.RATE_NO_ENTRIES and loads == []
     o.close()
     fl, ts, o = hand_fleet([([(0, 0)], [])], 1)
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, entry(0, 0, rpm=5000), params(fl.now_ms, 1000), 1)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, entry(0, 0, rpm=5000), rate_params(fl.now_ms, 1000), 1)
     assert rep["gate"] == L.RATE_FEW_INSTANCES and loads == [] and out["rpm"][0] == 0
     o.close()
 
@@ -85,7 +71,7 @@ def test_heavy_instance_second_copy_takes_it_scale_up_does_not(oracle_lib):
     fl, ts, o = hand_fleet([([(0, old)], [(x, old) for x in range(1, ni) if x != H]), reg1], ni, rpm=rpm)
     assert H in picks(o, fl, 1, 0, now, [], 11)
     ents = np.concatenate([entry(0, 0, rpm=10, second=True), entry(0, 1, rpm=3000)])
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, params(now, 1000), 11)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, rate_params(now, 1000), 11)
     assert list(out["action"]) == [1, 2] and rep["n_heavy"] == 1 and rep["n_second"] == 1 and rep["n_scale_up"] == 1
     got = by_entry(loads)
     assert got[0] == [(0, 0, 0, 0, H, got[0][0][5], out["load_last_used"][0], L.RL_SECOND_COPY, 0)]
@@ -104,7 +90,7 @@ def test_chain_ended_by_none(oracle_lib):
     ni = 12
     now = make_fleet("C3", 1, ni, 3).now_ms
     fl, ts, o = hand_fleet([([(0, now - HOUR), (1, now - HOUR)], [])], ni, inactive=range(4, 12))
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, entry(0, 0, rpm=4000), params(now, 1000), 5)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, entry(0, 0, rpm=4000), rate_params(now, 1000), 5)
     assert out["action"][0] == 2 and out["copies_to_load"][0] == 4
     assert [ld[2] for ld in loads] == [0, 1, 2] and loads[2][4] == L.TARGET_NONE
     assert sorted(ld[4] for ld in loads[:2]) == [2, 3] and rep["n_loads"] == 3 and rep["n_chains_cut"] == 0
@@ -116,7 +102,7 @@ def test_chain_cut_at_17(oracle_lib):
     ni = 60
     now = make_fleet("C3", 1, ni, 3).now_ms
     fl, ts, o = hand_fleet([([(0, now - HOUR), (1, now - HOUR)], [])], ni)
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, entry(0, 0, rpm=100_000), params(now, 5), 7)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, entry(0, 0, rpm=100_000), rate_params(now, 5), 7)
     assert out["copies_to_load"][0] == 20
     assert [ld[2] for ld in loads] == list(range(17)) and rep["n_chains_cut"] == 1
     assert loads[-1][7] == L.RL_CHAIN_CUT and loads[-1][8] == 3 and all(ld[7] == 0 for ld in loads[:-1])
@@ -135,8 +121,8 @@ def test_self_answer_continues_from_the_pod(oracle_lib):
     P = min(picks(o, fl, 0, 1, now, [], 3) - {1, 2, -1, -2})
     ents = entry(P, 0, rpm=3000)
     # (the pick among the best candidates is a hash of the seed and the id: the first seed whose draw is the pod)
-    seed = next(k for k in range(500) if rro.rate_run(o, fl, ts, P, ents, params(now, 1000), k)[1][0][4] == L.TARGET_SELF)
-    out, loads, rep = rro.rate_run(o, fl, ts, P, ents, params(now, 1000), seed)
+    seed = next(k for k in range(500) if rro.rate_run(o, fl, ts, P, ents, rate_params(now, 1000), k)[1][0][4] == L.TARGET_SELF)
+    out, loads, rep = rro.rate_run(o, fl, ts, P, ents, rate_params(now, 1000), seed)
     assert out["action"][0] == 2 and len(loads) >= 2
     assert loads[0][3] == P and loads[0][4] == L.TARGET_SELF
     assert loads[1][3] == P and loads[1][4] not in (P, L.TARGET_SELF, L.TARGET_NONE)
@@ -151,7 +137,7 @@ def test_failure_count_gate_edges(oracle_lib):
             ([(0, now - HOUR)], [(2, edge + 1), (3, edge + 1), (4, edge + 1)])]   # ... a scale-up too
     fl, ts, o = hand_fleet(regs, 20)
     ents = np.concatenate([entry(0, 0, second=True), entry(0, 1, second=True), entry(0, 2, rpm=3000)])
-    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, params(now, 1000), 9)
+    out, loads, rep = rro.rate_run(o, fl, ts, 0, ents, rate_params(now, 1000), 9)
     assert list(out["action"]) == [1, 1, 2]
     assert [ld[0] for ld in loads] == [0] and rep["n_refused_failures"] == 2 and rep["n_second"] == 2 and rep["n_scale_up"] == 1
     o.close()

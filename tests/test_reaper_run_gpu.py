@@ -17,17 +17,16 @@ import numpy as np
 import pytest
 
 import reaper_run_oracle as rro
-from helpers import oracle_from_synth, solver_from_synth
+from churn_harness import device_selection, reaper_workload, with_failed
+from common import GONE_MS, vp
+from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet, MmpError
 from modelmesh_b200.synth import load_into_fleet, make_churn, make_churn_overflow, make_fleet
-from oracle import binding as ob
+from pod_tasks import timed_solver
 from replay import Replay, run_window
-from test_churn_reaper_gpu import _with_failed, _workload, device_selection
 
 pytestmark = pytest.mark.gpu
-
-GONE_MS = 600_000   # ASSUME_INSTANCE_GONE_AFTER_MS
 
 
 def _times(fl, rng, recent=0.3):
@@ -38,24 +37,9 @@ def _times(fl, rng, recent=0.3):
 
 
 def _build(product_lib, fl, ts, gone=()):
-    s = solver_from_synth(fl, product_lib)
-    for m in range(fl.n_models):
-        a, b = int(fl.edge_off[m]), int(fl.edge_off[m + 1])
-        if a < b:
-            s.model_times(m, ts[a:b])
-    for i in gone:
-        s.instance_remove(int(i))
-    s.commit()
+    s = timed_solver(product_lib, fl, ts, gone=gone, skip_empty=True)
     # the oracle's table as the commit holds it: every instance but the gone ones, as ADDED events, one converged refresh
-    o = ob.OracleFleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units)
-    o.types_set(fl.type_config)
-    out = set(int(i) for i in gone)
-    for i in range(fl.n_instances):
-        if i not in out:
-            o.instance_event(ob.ADDED, i, fl.inst_rows[i], fl.inst_ids[i], fl.inst_locs[i], fl.inst_zones[i], fl.inst_labels[i], fl.now_ms)
-    if fl.type_config is not None:
-        o.tc_converge()
-    o.set_replaced_replicasets(fl.replaced_replicasets)
+    o = oracle_from_synth(fl, bulk=False, gone=gone)
     # a pruned registration names an instance outside the table: no rank, so the committed exclusion rows are those of the
     # pruned records.  That needs every ranked instance to be in the table.
     assert not set(int(i) for i in s.cluster_order()) & set(int(i) for i in gone)
@@ -104,7 +88,7 @@ def _late_zero(seed):
 @pytest.mark.parametrize("case,seed", [("free", 3), ("free_tc", 4), ("cutoff", 5), ("cutoff_tc", 6), ("full", 7), ("ties", 8),
                                        ("none", 9), ("zero", 10), ("part0_tc", 11), ("late0_tc", 12)])
 def test_reaper_run_without_prune(product_lib, oracle_lib, case, seed):
-    w = _late_zero(seed) if case == "late0_tc" else _workload(case, seed)
+    w = _late_zero(seed) if case == "late0_tc" else reaper_workload(case, seed)
     fl = w.fleet
     ts = np.full(len(fl.edge_inst), fl.now_ms - rro.HOUR, dtype=np.int64)
     s, o = _build(product_lib, fl, ts)
@@ -134,7 +118,7 @@ def test_reaper_run_without_prune(product_lib, oracle_lib, case, seed):
 def test_reaper_run_with_pods_gone(product_lib, oracle_lib, with_types, leader_gone, seed):
     w = make_churn(20_000, 200, seed, fill=0.5, with_types=with_types)
     twice = [int(m) for m in w.unloaded_models[:300]]
-    w = _with_failed(w, {m: 2 for m in twice})   # two failed loads, on instances 0 and 1
+    w = with_failed(w, {m: 2 for m in twice})   # two failed loads, on instances 0 and 1
     fl = w.fleet
     rng = np.random.default_rng(seed)
     fl.model_last_used[twice] = fl.now_ms - rng.integers(0, 1000, size=len(twice))  # the most recent: selected once candidates
@@ -232,7 +216,6 @@ def test_reaper_run_errors(product_lib):
         s.reaper_run(0, fl.now_ms, -1, missing, 1)
     assert e.value.code == L.E_ARG
     rep = L.ReaperReport()
-    vp = lambda a: a.ctypes.data_as(C.c_void_p)
     buf = np.zeros(16, dtype=np.int32)
     loads = np.zeros(4, dtype=L.REAPER_LOAD)
     for args in ((vp(buf), vp(buf), -1, vp(buf), 4, vp(loads), 4), (None, vp(buf), 4, vp(buf), 4, vp(loads), 4),

@@ -9,12 +9,10 @@ import pytest
 import reaper_run_oracle as rro
 from helpers import oracle_from_synth
 from oracle import binding as ob
-from reaper_oracle import _reaper_oracle_so, reaper_oracle  # noqa: F401
-from test_churn_reaper_gpu import _with_failed
-from test_churn_reaper_oracle import _sim, reaper_event
+from churn_harness import with_failed
+from common import GONE_MS
 from modelmesh_b200.synth import make_churn
-
-GONE_MS = 600_000
+from reaper_oracle import _reaper_oracle_so, reaper_event, reaper_oracle, reaper_sim  # noqa: F401
 
 
 @pytest.mark.usefixtures("reaper_oracle")
@@ -22,7 +20,7 @@ GONE_MS = 600_000
 def test_composition_selects_what_the_reaper_event_decides(oracle_lib, with_types, fill, seed):
     w = make_churn(6000, 48, seed, fill=fill, with_types=with_types)
     fl = w.fleet
-    o, sim = _sim(w)
+    o, sim = reaper_sim(w)
     t = fl.now_ms + 500
     missing = np.zeros(fl.n_instances, dtype=np.int64)
     got = rro.reaper_run(o, fl, np.full(len(fl.edge_inst), fl.now_ms - rro.HOUR, dtype=np.int64), 5, t, GONE_MS, missing,
@@ -69,7 +67,7 @@ def _restated(fl, ts, present, leader, now, gone_ms, missings: dict, last_used, 
 @pytest.mark.parametrize("seed", [41, 42, 43])
 def test_composition_prunes_as_the_reference_loop(oracle_lib, seed):
     w = make_churn(3000, 40, seed, fill=0.5)
-    w = _with_failed(w, {int(m): 2 for m in w.unloaded_models[:200]})  # failed loads on instances 0 and 1
+    w = with_failed(w, {int(m): 2 for m in w.unloaded_models[:200]})  # failed loads on instances 0 and 1
     fl = w.fleet
     rng = np.random.default_rng(seed)
     fl.model_last_used[rng.choice(fl.n_models, size=30, replace=False)] = rro.LONG_MAX

@@ -9,9 +9,7 @@ import pytest
 from modelmesh_b200 import _lib as L
 from modelmesh_b200._lib import MODEL_ROW
 from modelmesh_b200.fleet import Fleet, MmpError
-from modelmesh_b200.synth import load_into_fleet, make_decisions, make_fleet
-
-LONG_MAX = 9223372036854775807
+from modelmesh_b200.synth import LONG_MAX, load_into_fleet, make_decisions, make_fleet
 
 
 def instance_json(fl, i, extra=None):

@@ -5,25 +5,24 @@
   mmp_registry_prune      the four-registration view, against the oracle run on each model's first four registrations
 Times reach positions past the fourth through mmp_model_times and through mmp_model_upsert_json alike, and survive the
 incremental commits of a replayed ingest stream (tests/replay.py) as a fleet rebuilt from scratch holds them."""
-import ctypes as C
 import json
 
 import numpy as np
 import pytest
 
+from common import GONE_MS, HOUR, vp
 from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet
 from modelmesh_b200.synth import load_into_fleet, make_fleet
 from oracle import binding as ob
-from replay import Replay, run_window
+from pod_tasks import TimedReplay
+from replay import run_window
+from scan_checks import oracle_prune, oracle_scale, scale_eval, scale_params
 
 pytestmark = pytest.mark.gpu
 
-HOUR = 3_600_000
-GONE_MS = 600_000   # ASSUME_INSTANCE_GONE_AFTER_MS
 PARAM_SETS = ((2000, 1, 6 * HOUR), (300, 1, 1000), (5, 0, 6 * HOUR))
-vp = lambda a: a.ctypes.data_as(C.c_void_p)
 
 
 def _overflow_heavy(nm: int, ni: int, seed: int):
@@ -88,50 +87,9 @@ def _records(fl, rng, n, models):
     return rec
 
 
-def _params(now, thr, can_remove, lru_thr):
-    p = np.zeros(1, dtype=L.SCALE_PARAMS)
-    p["now"], p["last_check_time"], p["iteration"], p["scale_up_rpm_threshold"] = now, now - 10_000, 5000, thr
-    p["second_copy_min_age_iters"], p["second_copy_max_age_iters"], p["second_copy_lru_threshold_ms"] = 42, 240, lru_thr
-    p["rate_check_interval_ms"], p["assume_completed_ms"], p["second_copy_remove_max_age_ms"], p["can_remove"] = 10_000, 30_000, 36 * HOUR, can_remove
-    return p
-
-
-def _scale(lib, s, rec, p):
-    out = np.zeros(len(rec), dtype=L.SCALE_OUT)
-    s._ck(lib.mmp_scale_eval(s.h, vp(rec), len(rec), vp(p), vp(out)))
-    return out
-
-
 def _same_scale(x, y) -> bool:
     """Field by field: mmp_scale_out ends in 4 bytes of padding that the library does not write."""
     return all(np.array_equal(x[k], y[k]) for k in x.dtype.names)
-
-
-def _oracle_scale(oracle_lib, o, fl, ts, lul, rec, p):
-    """orc_rate_task_eval / orc_janitor_eval with each record's model as CSR edge lists: every registration, loaded first."""
-    n = len(rec)
-    m64 = rec["model"].astype(np.int64)
-    deg = (fl.edge_off[m64 + 1] - fl.edge_off[m64]).astype(np.int64)
-    eoff = np.zeros(n + 1, dtype=np.int64)
-    np.cumsum(deg, out=eoff[1:])
-    einst = np.concatenate([fl.edge_inst[fl.edge_off[m]:fl.edge_off[m + 1]] for m in m64]).astype(np.int32)
-    ets = np.concatenate([ts[fl.edge_off[m]:fl.edge_off[m + 1]] for m in m64]).astype(np.int64)
-    nl = fl.n_loaded[m64].astype(np.int32)
-    tidx = fl.model_type[m64].astype(np.int32)
-    orec = np.zeros(n, dtype=ob.SCALE_IN)
-    for k in ("instance", "model", "count", "last_used", "last_heavy", "i1", "i2", "flags"):
-        orec[k] = rec[k]
-    op = np.zeros(1, dtype=ob.SCALE_PARAMS)
-    for k in op.dtype.names:
-        if k != "pad":
-            op[k] = p[k]
-    up = np.zeros(n, dtype=ob.SCALE_OUT)
-    down = np.zeros(n, dtype=ob.SCALE_OUT)
-    names = (C.c_char_p * len(fl.type_names))(*[t.encode() for t in fl.type_names])
-    assert oracle_lib.orc_rate_task_eval(o.h, n, vp(orec), vp(op), names, len(fl.type_names), vp(tidx), vp(eoff), vp(einst), vp(ets), vp(nl), vp(up)) == 0
-    lulr = lul[m64].astype(np.int64)
-    assert oracle_lib.orc_janitor_eval(o.h, n, vp(orec), vp(op), vp(eoff), vp(einst), vp(ets), vp(nl), vp(lulr), vp(down)) == 0
-    return up, down
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [("C3", 4000, 500, 3), ("C5", 3000, 400, 5), ("MIX", 1500, 160, 14), ("HEAVY", 3000, 500, 41)])
@@ -161,9 +119,9 @@ def test_scale_eval_over_every_registration(product_lib, oracle_lib, config, nm,
     ovf = deg[models] > 4
     seen = np.zeros(3, dtype=np.int64)
     for thr, can_remove, lru_thr in PARAM_SETS:
-        p = _params(fl.now_ms, thr, can_remove, lru_thr)
-        out = _scale(product_lib, s, rec, p)
-        up, down = _oracle_scale(oracle_lib, o, fl, ts, lul, rec, p)
+        p = scale_params(fl.now_ms, thr, can_remove, lru_thr)
+        out = scale_eval(product_lib, s, rec, p)
+        up, down = oracle_scale(oracle_lib, o, fl, ts, lul, rec, p)
         for k in ("action", "copies_to_load", "load_last_used", "rpm", "i1", "i2", "set_heavy"):
             bad = np.nonzero(out[k] != up[k])[0]
             assert len(bad) == 0, (thr, k, len(bad), bad[:5], out[bad[:5]], up[bad[:5]], rec[bad[:5]], deg[models[bad[:5]]])
@@ -173,29 +131,12 @@ def test_scale_eval_over_every_registration(product_lib, oracle_lib, config, nm,
         seen += [np.count_nonzero(ovf & (out["action"] == 1)), np.count_nonzero(ovf & (out["action"] == 2)), np.count_nonzero(ovf & (out["remove"] == 1))]
         if len(saturated):  # copy_count 255 over 300 registrations: loaded and failed cannot be told apart
             srec = _records(fl, rng, 64, np.full(64, saturated[0]))
-            sout = _scale(product_lib, s, srec, p)
+            sout = scale_eval(product_lib, s, srec, p)
             assert (sout["action"] == -1).all() and not sout["remove"].any()
     if config == "HEAVY":
         assert (seen > 0).all(), seen
     o.close()
     s.close()
-
-
-def _oracle_prune(oracle_lib, o, fl, ts, self_idx, now, missing, first=None):
-    """orc_prune_missing over every model (or its first `first` registrations): (model, instance) pairs and per-model masks."""
-    pairs, masks = [], {}
-    pruned = np.zeros(max(1, int(np.diff(fl.edge_off).max())), dtype=np.uint8)
-    for m in range(fl.n_models):
-        a, b = int(fl.edge_off[m]), int(fl.edge_off[m + 1])
-        if first is not None:
-            b = min(b, a + first)
-        if a == b:
-            continue
-        k = oracle_lib.orc_prune_missing(o.h, self_idx, vp(fl.edge_inst[a:b]), vp(ts[a:b]), b - a, now, GONE_MS, vp(missing), vp(pruned))
-        if k:
-            pairs += [(m, int(fl.edge_inst[a + j])) for j in range(b - a) if pruned[j]]
-            masks[m] = sum(int(pruned[j]) << j for j in range(b - a))
-    return pairs, masks
 
 
 def test_registry_prune_over_every_registration(product_lib, oracle_lib):
@@ -221,7 +162,7 @@ def test_registry_prune_over_every_registration(product_lib, oracle_lib):
     for rnd, now in enumerate((fl.now_ms, fl.now_ms + 360_000, fl.now_ms + 720_000)):
         before = miss_p.copy()
         n, pm, pi = s.registry_prune_ids(self_idx, now, GONE_MS, miss_p, 1 << 20)
-        want, _ = _oracle_prune(oracle_lib, o, fl, ts, self_idx, now, miss_o)
+        want, _ = oracle_prune(oracle_lib, o, fl, ts, self_idx, now, miss_o)
         assert n == len(want) and list(zip(pm.tolist(), pi.tolist())) == want, (rnd, n, len(want))
         assert np.array_equal(miss_p, miss_o), rnd
         assert not np.array_equal(before, miss_p) or rnd > 0
@@ -238,7 +179,7 @@ def test_registry_prune_over_every_registration(product_lib, oracle_lib):
         outm = np.zeros(nm, dtype=np.int32)
         outk = np.zeros(nm, dtype=np.uint8)
         k = s._ck(product_lib.mmp_registry_prune(s.h, self_idx, now, GONE_MS, vp(miss_pi), vp(outm), vp(outk), nm))
-        _, masks = _oracle_prune(oracle_lib, o, fl, ts, self_idx, now, miss_oi, first=4)
+        _, masks = oracle_prune(oracle_lib, o, fl, ts, self_idx, now, miss_oi, first=4)
         assert {int(outm[i]): int(outk[i]) for i in range(k)} == masks, rnd
         assert np.array_equal(miss_pi, miss_oi), rnd
     deg = np.diff(fl.edge_off)
@@ -279,8 +220,8 @@ def test_json_and_index_ingest_agree(product_lib):
 
     def same_scale(what):
         for thr, can_remove, lru_thr in PARAM_SETS:
-            p = _params(fl.now_ms, thr, can_remove, lru_thr)
-            assert _same_scale(_scale(product_lib, a, rec, p), _scale(product_lib, b, rec, p)), (what, thr)
+            p = scale_params(fl.now_ms, thr, can_remove, lru_thr)
+            assert _same_scale(scale_eval(product_lib, a, rec, p), scale_eval(product_lib, b, rec, p)), (what, thr)
 
     same_scale("ingest")
     # 40 pods leave, most of them named past the fourth position of JSON records
@@ -310,46 +251,9 @@ def test_json_and_index_ingest_agree(product_lib):
     b.close()
 
 
-class _TimedReplay(Replay):
-    """A replayed stream whose index upserts come with a time for every registration (mmp_model_times before the commit, so
-    that the window's own commit carries them).  JSON records carry none: their times read 0."""
-
-    def __init__(self, fl, lib, seed):
-        super().__init__(fl, lib, seed)
-        self.trng = np.random.default_rng(seed + 1000)
-        self.times = {}
-        self.touched = set(range(self.n_used))
-        self._give()
-        self.touched = set()
-        self.f.commit()
-
-    def _give(self):
-        edges = self.current_edges()
-        for m in self.touched:
-            if m in self.json_ids:
-                self.times[m] = (np.zeros(0, dtype=np.int64), 0)
-                continue
-            k = len(edges[m])
-            ts = np.where(self.trng.uniform(size=k) < 0.3, self.now - self.trng.integers(0, 900_000, size=k),
-                          self.now - self.trng.integers(0, 4 * HOUR, size=k)).astype(np.int64)
-            self.times[m] = (ts, int(self.now - self.trng.integers(0, 200_000)) if self.trng.uniform() < 0.3 else 0)
-            self.f.model_times(m, *self.times[m])
-
-    def commit(self, kind, n_model_edits, events=()):
-        self._give()
-        return super().commit(kind, n_model_edits, events)
-
-    def timed_scratch(self):
-        g = self.scratch()
-        for m, (ts, lul) in self.times.items():
-            g.model_times(m, ts, lul)
-        g.commit()
-        return g
-
-
 @pytest.mark.parametrize("config,nm,ni,seed,n_windows", [("C3", 3000, 600, 3, 8), ("MIX", 2000, 400, 14, 8)])
 def test_replayed_commits_match_scratch(product_lib, config, nm, ni, seed, n_windows):
-    rp = _TimedReplay(make_fleet(config, nm, ni, seed), product_lib, seed)
+    rp = TimedReplay(make_fleet(config, nm, ni, seed), product_lib, seed)
     crossed = 0
     for w in range(n_windows):
         before = [len(e) > 4 for e in rp.current_edges()]
@@ -377,7 +281,7 @@ def test_replayed_commits_match_scratch(product_lib, config, nm, ni, seed, n_win
         rec["i1"] = 5000 - rng.integers(0, 400, size=n)
         rec["i2"] = np.minimum(5000, rec["i1"] + rng.integers(0, 300, size=n))
         for thr, can_remove, lru_thr in PARAM_SETS:
-            p = _params(rp.now, thr, can_remove, lru_thr)
-            assert _same_scale(_scale(product_lib, f, rec, p), _scale(product_lib, g, rec, p)), ("scale", w, thr)
+            p = scale_params(rp.now, thr, can_remove, lru_thr)
+            assert _same_scale(scale_eval(product_lib, f, rec, p), scale_eval(product_lib, g, rec, p)), ("scale", w, thr)
         g.close()
     assert crossed > 0

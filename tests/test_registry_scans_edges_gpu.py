@@ -18,9 +18,9 @@ from helpers import oracle_from_synth, solver_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import LONG_MAX, NOW_MS, SynthFleet
 from oracle import binding as ob
-from test_fleet_scans_edges_gpu import _converged_oracle
-from test_oracle_properties import brute_compare
-from test_registry_overflow_gpu import GONE_MS, HOUR, _oracle_prune, _oracle_scale, _params, _scale
+from brute import brute_compare
+from common import GONE_MS, HOUR, vp
+from scan_checks import converged_oracle, oracle_prune, oracle_scale, scale_eval, scale_params
 
 NOW = NOW_MS
 INT_MAX, INT_MIN = (1 << 31) - 1, -(1 << 31)
@@ -243,7 +243,7 @@ def _fleet(name, pts):
 
 
 def _oracle(fl):
-    o = _converged_oracle(fl) if fl.type_config is not None else oracle_from_synth(fl)
+    o = converged_oracle(fl) if fl.type_config is not None else oracle_from_synth(fl)
     o.instance_event(ob.DELETED, GONE, None, fl.inst_ids[GONE], now_ms=NOW)
     return o
 
@@ -271,7 +271,7 @@ def _batch(pts, p_over, model0=0):
         for k, v in x["rec"].items():
             rec[k][r] = v
         rec["model"][r] = model0 + r
-    p = _params(NOW, 1000, 1, 0)
+    p = scale_params(NOW, 1000, 1, 0)
     for k, v in dict(DEFAULT_P, **dict(p_over)).items():
         p[k] = v
     return rec, p
@@ -291,8 +291,8 @@ def _run(oracle_lib, product_lib=None):
         m0 = 0
         for p_over, pts in groups:
             rec, p = _batch(pts, p_over, m0)
-            up, down = _oracle_scale(oracle_lib, o, fl, ts, lul, rec, p)
-            out = _scale(product_lib, s, rec, p) if s is not None else None
+            up, down = oracle_scale(oracle_lib, o, fl, ts, lul, rec, p)
+            out = scale_eval(product_lib, s, rec, p) if s is not None else None
             for r, (name, _) in enumerate(pts):
                 want = tuple(int(up[k][r]) for k in ("action", "copies_to_load", "load_last_used", "rpm", "i1", "i2", "set_heavy")) + (int(down["remove"][r]),)
                 got = None if out is None else tuple(int(out[k][r]) for k in ("action", "copies_to_load", "load_last_used", "rpm", "i1", "i2", "set_heavy", "remove"))
@@ -406,7 +406,6 @@ def test_registry_prune_boundaries_match_oracle(product_lib, oracle_lib):
         s.instance_remove(i)
         o.instance_event(ob.DELETED, i, None, fl.inst_ids[i], now_ms=NOW)
     s.commit()
-    vp = lambda a: a.ctypes.data_as(C.c_void_p)
     views = {"ids": (_missing(), _missing()), "four": (_missing(), _missing())}
     deg = np.diff(fl.edge_off)
     on = lambda i: {m for m in range(NM) if i in fl.edge_inst[fl.edge_off[m]:fl.edge_off[m + 1]]}
@@ -418,7 +417,7 @@ def test_registry_prune_boundaries_match_oracle(product_lib, oracle_lib):
         mp, mo = views["ids"]
         before = mp.copy()
         n, pm, pi = s.registry_prune_ids(0, now, GONE_MS, mp, 1 << 20)
-        want, _ = _oracle_prune(oracle_lib, o, fl, ts, 0, now, mo)
+        want, _ = oracle_prune(oracle_lib, o, fl, ts, 0, now, mo)
         got = list(zip(pm.tolist(), pi.tolist()))
         assert n == len(want) and got == want, (rnd, n, len(want))
         assert np.array_equal(mp, mo), rnd
@@ -429,7 +428,7 @@ def test_registry_prune_boundaries_match_oracle(product_lib, oracle_lib):
         before4 = fp.copy()
         outm, outk = np.zeros(NM, dtype=np.int32), np.zeros(NM, dtype=np.uint8)
         k4 = s._ck(product_lib.mmp_registry_prune(s.h, 0, now, GONE_MS, vp(fp), vp(outm), vp(outk), NM))
-        _, masks = _oracle_prune(oracle_lib, o, fl, ts, 0, now, fo, first=4)
+        _, masks = oracle_prune(oracle_lib, o, fl, ts, 0, now, fo, first=4)
         assert k4 == len(masks) and list(zip(outm[:k4].tolist(), outk[:k4].tolist())) == sorted(masks.items()), rnd
         assert np.array_equal(fp, fo), rnd
         # a cap below the count: the first cap models in model order (the pruned models spread over every block)
@@ -457,7 +456,7 @@ def test_registry_prune_boundaries_match_oracle(product_lib, oracle_lib):
     m2 = _missing()
     mo2 = _missing()
     n, pm, pi = s.registry_prune_ids(SELF2, NOW, GONE_MS, m2, 1 << 20)
-    want, _ = _oracle_prune(oracle_lib, o, fl, ts, SELF2, NOW, mo2)
+    want, _ = oracle_prune(oracle_lib, o, fl, ts, SELF2, NOW, mo2)
     assert list(zip(pm.tolist(), pi.tolist())) == want and np.array_equal(m2, mo2) and SELF2 not in set(pi.tolist())
     o.close()
     s.close()

@@ -9,6 +9,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from common import vp
 from helpers import oracle_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.fleet import Fleet
@@ -88,7 +89,6 @@ def test_scale_eval_matches_oracle(product_lib, oracle_lib, config, nm, ni, seed
         up = np.zeros(n, dtype=ob.SCALE_OUT)
         down = np.zeros(n, dtype=ob.SCALE_OUT)
         names = (C.c_char_p * len(fl.type_names))(*[t.encode() for t in fl.type_names])
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)
         assert oracle_lib.orc_rate_task_eval(o.h, n, vp(orec), vp(op), names, len(fl.type_names), vp(tidx), vp(eoff), vp(einst), vp(ets), vp(nl), vp(up)) == 0
         lulr = lul[m64].astype(np.int64)
         assert oracle_lib.orc_janitor_eval(o.h, n, vp(orec), vp(op), vp(eoff), vp(einst), vp(ets), vp(nl), vp(lulr), vp(down)) == 0

@@ -7,8 +7,8 @@ from helpers import compare_decisions, oracle_from_synth, solver_from_synth
 from modelmesh_b200 import _lib as L
 from modelmesh_b200._lib import DF_FAVOUR_SELF
 from modelmesh_b200.synth import make_decisions, make_fleet
-from test_rolling_upgrade_gpu import PATTERNS, check_total_order, full_best_then_room, upgrade, versions
-from test_split_place_emul import _oracle_same, place_split, split_lib  # noqa: F401 (split_lib: fixture)
+from split_place import oracle_same, place_split, split_lib  # noqa: F401 (split_lib: fixture)
+from upgrade import PATTERNS, check_total_order, full_best_then_room, upgrade, versions
 
 # fleets whose slot summaries reach past the newer pods (long shortlists: C5's near-full fleet, MIX's low counts, a saturated
 # front); elsewhere a summary's best and shortlist lie among the newer pods
@@ -51,7 +51,7 @@ def test_upgrade_split_summaries(split_lib, oracle_lib, config, nm, ni, seed, pa
     for k, sd in enumerate((sweep, fav, make_decisions(fl, 2000, seed + 1))):
         out, counts = place_split(split_lib, s, sd, fl.now_ms, seed + k)
         assert counts[1] == 0, (config, pattern, k, counts)
-        _oracle_same(o, fl, sd, out, seed + k)
+        oracle_same(o, fl, sd, out, seed + k)
         total += counts
     assert total[0] > 0
     if (config, pattern) in CROSSING:

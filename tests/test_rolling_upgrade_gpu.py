@@ -6,124 +6,27 @@ shape: the full instances no longer form one suffix, counts and lruTimes restart
 can be followed by non-full candidates.  A commit whose live set holds more than one version leaves the device path for
 the host's merge sort (path 1); the closed loop must then build that commit from the device's instance rows and registry.
 
-upgrade() and fleet_for() build the fleets; the CPU side of these tests is test_rolling_upgrade_emul.py."""
+tests/upgrade.py builds the fleets; the CPU side of these tests is test_rolling_upgrade_emul.py."""
 import dataclasses
 
 import numpy as np
 import pytest
 
+from churn_harness import build, compare_window, run_small_closed_loop
 from exclude_set import oracle_excluding
-from helpers import compare_decisions, oracle_from_synth, oracle_inputs_fast, solver_from_synth
+from helpers import compare_decisions, oracle_from_synth, oracle_inputs_fast, place_kw, same_answers, solver_from_synth
 from modelmesh_b200 import _lib as L
-from modelmesh_b200.synth import LONG_MAX, SynthFleet, make_churn, make_decisions, make_fleet
-from oracle import binding as ob
+from modelmesh_b200.synth import LONG_MAX, make_churn, make_decisions, make_fleet
 from replay import STRUCTURAL, Replay, check_against_oracle, check_against_scratch, check_sorted_batch, describe
+from upgrade import NEW_RS, PATTERNS, bump, check_total_order, full_best_then_room, upgrade, versions
 
 pytestmark = pytest.mark.gpu
-
-PATTERNS = ("canary", "half", "rsroll", "saturated", "three")
-NEW_RS = "mmupgr"  # the replicaset prefix of the pods an rsroll upgrade brings up
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# upgrade fleets
-# ---------------------------------------------------------------------------------------------------------------
-def upgrade(fl: SynthFleet, pattern: str, seed: int) -> SynthFleet:
-    """fl with some of its pods moved to newer versions:
-      canary     one to three live pods on vers + 1
-      half       about half of the pods, drawn at random
-      rsroll     up to a tenth of the pods, drawn among those without labels, on vers + 1 under the new replicaset
-                 prefix NEW_RS; every old prefix is listed as likely-replaced (UpgradeTracker, MM:4769-4770): a type that
-                 requires a label has every candidate flagged, and the candx filter is retried across the boundary
-      saturated  about a third of the pods on vers + 1, every one of them full with an lruTime hours old: the best is
-                 full and non-full older pods follow it
-      three      three versions (about 50 / 30 / 20 %)
-    Every full instance keeps an lruTime above 2 * minChurnAgeMs, so the comparator stays a strict total order."""
-    rng = np.random.default_rng(seed ^ 0x5EED)
-    rows = fl.inst_rows.copy()
-    ni = len(rows)
-    v0 = int(rows["vers"][0])
-    assert (rows["vers"] == v0).all()
-    ids, replaced = list(fl.inst_ids), list(fl.replaced_replicasets)
-    live = np.nonzero(rows["shutting_down"] == 0)[0]
-    if pattern == "canary":
-        rows["vers"][rng.choice(live, size=int(rng.integers(1, 4)), replace=False)] = v0 + 1
-    elif pattern == "half":
-        rows["vers"][rng.uniform(size=ni) < 0.5] = v0 + 1
-    elif pattern == "rsroll":
-        pool = [int(i) for i in live if not fl.inst_labels[i]] or list(live)
-        new = rng.choice(pool, size=max(1, min(len(pool), ni // 10)), replace=False)
-        rows["vers"][new] = v0 + 1
-        for i in new:
-            ids[i] = f"{NEW_RS}-{i:05x}"
-        replaced = sorted({ids[i][:6] for i in range(ni) if len(ids[i]) >= 7 and not ids[i].startswith(NEW_RS)})
-    elif pattern == "saturated":
-        new = np.nonzero(rng.uniform(size=ni) < 0.33)[0]
-        rows["vers"][new] = v0 + 1
-        rows["used"][new] = rows["capacity"][new] - rng.integers(0, fl.min_space_units, size=len(new))
-        rows["lru_time"][new] = fl.now_ms - rng.integers(3_600_000, 12 * 3_600_000, size=len(new))
-    elif pattern == "three":
-        u = rng.uniform(size=ni)
-        rows["vers"] = v0 + (u < 0.5) + (u < 0.2)
-    else:
-        raise ValueError(pattern)
-    return dataclasses.replace(fl, inst_rows=rows, inst_ids=ids, replaced_replicasets=replaced)
-
-
-def fleet_for(config: str, nm: int, ni: int, seed: int) -> SynthFleet:
-    """make_fleet(config) or, for "BASE/pattern", make_fleet(BASE) in that rolling upgrade"""
-    base, _, pattern = config.partition("/")
-    fl = make_fleet(base, nm, ni, seed)
-    return upgrade(fl, pattern, seed) if pattern else fl
-
-
-def check_total_order(fl: SynthFleet, o: ob.OracleFleet, seed: int, n: int = 3000):
-    """No full live instance at or below 2 * minChurnAgeMs (N1's non-transitive corner), and the oracle's comparator
-    is antisymmetric and transitive on sampled triples of live instances."""
-    r = fl.inst_rows
-    live = np.nonzero(r["shutting_down"] == 0)[0]
-    full = (np.maximum(0, r["capacity"] - r["used"]) < fl.min_space_units)[live]
-    assert not (full & (r["lru_time"][live] <= 2 * fl.min_churn_age_ms)).any()
-    rng = np.random.default_rng(seed)
-    for a, b, c in live[rng.integers(0, len(live), size=(n, 3))]:
-        a, b, c = int(a), int(b), int(c)
-        if len({a, b, c}) < 3:
-            continue
-        ab, bc, ac = o.compare(a, b), o.compare(b, c), o.compare(a, c)
-        assert np.sign(ab) == -np.sign(o.compare(b, a)) != 0, (a, b)
-        if ab < 0 and bc < 0:
-            assert ac < 0, (a, b, c)
-        if ab > 0 and bc > 0:
-            assert ac > 0, (a, b, c)
-
-
-def versions(fl: SynthFleet) -> np.ndarray:
-    return np.unique(fl.inst_rows["vers"][fl.inst_rows["shutting_down"] == 0])
-
-
-def full_best_then_room(fl: SynthFleet, tr: np.ndarray, out: np.ndarray) -> int:
-    """decisions whose best is full and whose answer is an instance with room: non-full candidates after a full best"""
-    r = fl.inst_rows
-    t = out["target"]
-    ok = (t >= 0) & ((tr["flags"] & L.TF_BEST_FULL) != 0)
-    room = np.zeros(len(t), dtype=bool)
-    room[ok] = (r["capacity"][t[ok]] - r["used"][t[ok]]) >= fl.min_space_units
-    return int(np.count_nonzero(room))
-
-
-def _kw(sd):
-    return dict(fresh=sd.fresh if len(sd.fresh) else None, extra=sd.extra if len(sd.extra) else None)
 
 
 def _oracle(fl, sd, o, seed, candidates=False):
     od, off, idx = oracle_inputs_fast(fl, sd)
     return o.get_next_batch(od, fl.type_names, off, idx, fl.now_ms, seed, fresh=sd.fresh if len(sd.fresh) else None,
                             want_candidates=candidates)
-
-
-def _same(got, want, what):
-    bad = np.nonzero((got["target"] != want["target"]) | (got["n_candidates"] != want["n_candidates"]))[0]
-    assert len(bad) == 0, (what, len(bad), bad[:5], got[bad[:5]], want[bad[:5]])
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -173,11 +76,11 @@ def test_upgrade_batches_split_sorted_sweep_and_latency(product_lib, oracle_lib,
         got = {}
         for split in (1, 0):
             s._ck(lib.mmp_tune(s.h, b"split", split))
-            got[split] = s.place_batch(sd.dec, fl.now_ms, 7 + k, **_kw(sd))
+            got[split] = s.place_batch(sd.dec, fl.now_ms, 7 + k, **place_kw(sd))
         s._ck(lib.mmp_tune(s.h, b"split", 2))
         assert got[1].tobytes() == got[0].tobytes(), (pattern, k, int(np.sum(got[1] != got[0])))
         want, coff, cidx, _, _ = _oracle(fl, sd, o, 7 + k, candidates=True)
-        _same(got[1], want, (pattern, "split", k))
+        same_answers(got[1], want, (pattern, "split", k))
         # decisions whose best and shortlist hold more than one version
         owner = np.repeat(np.arange(len(sd.dec)), np.diff(coff))
         lo, hi = np.full(len(sd.dec), LONG_MAX), np.full(len(sd.dec), -1)
@@ -191,20 +94,20 @@ def test_upgrade_batches_split_sorted_sweep_and_latency(product_lib, oracle_lib,
         want = _oracle(fl, sd, o, 5)
         for sort in (0, 1):
             s._ck(lib.mmp_tune(s.h, b"sort_slots", sort))
-            _same(s.place_batch(sd.dec, fl.now_ms, 5, **_kw(sd)), want, (pattern, "sort_slots", sort, n))
+            same_answers(s.place_batch(sd.dec, fl.now_ms, 5, **place_kw(sd)), want, (pattern, "sort_slots", sort, n))
         s._ck(lib.mmp_tune(s.h, b"sort_slots", 2))
     sd = make_decisions(fl, 20_000, 12, sweep=True, plain=True)
     whole = s.place_batch(sd.dec, fl.now_ms, 5)
     fav = (sd.dec["flags"] & L.DF_FAVOUR_SELF) != 0
     assert np.array_equal(s.place_sweep(0, 20_000, sd.dec["self"], fl.now_ms, 5, favour=fav), whole)
-    _same(whole, _oracle(fl, sd, o, 5), (pattern, "sweep"))
+    same_answers(whole, _oracle(fl, sd, o, 5), (pattern, "sweep"))
     sd = make_decisions(fl, 400, 13)
-    whole = s.place_batch(sd.dec, fl.now_ms, 11, **_kw(sd))
+    whole = s.place_batch(sd.dec, fl.now_ms, 11, **place_kw(sd))
     for mode in (3, 2, 1, 0):
         s._ck(lib.mmp_tune(s.h, b"one_mode", mode))
         for lo, cnt in ((0, 1), (5, 7), (40, 32), (100, 33)):
             s._ck(lib.mmp_fleet_set_id_base(s.h, lo))
-            assert np.array_equal(s.place_batch(sd.dec[lo:lo + cnt], fl.now_ms, 11, **_kw(sd)), whole[lo:lo + cnt]), (pattern, mode, lo)
+            assert np.array_equal(s.place_batch(sd.dec[lo:lo + cnt], fl.now_ms, 11, **place_kw(sd)), whole[lo:lo + cnt]), (pattern, mode, lo)
         s._ck(lib.mmp_fleet_set_id_base(s.h, 0))
     s._ck(lib.mmp_tune(s.h, b"one_mode", 3))
     s.close()
@@ -222,10 +125,10 @@ def test_exclude_set_moves_best_across_the_boundary(product_lib, oracle_lib, pat
     for split in (1, 0):
         for sd in (make_decisions(fl, 8192 + 77, 9, sweep=True, plain=True), make_decisions(fl, 3000, 10)):
             s._ck(product_lib.mmp_tune(s.h, b"split", split))
-            plain = s.place_batch(sd.dec, fl.now_ms, 5, **_kw(sd))
-            got = s.place_batch(sd.dec, fl.now_ms, 5, exclude=newest, **_kw(sd))
+            plain = s.place_batch(sd.dec, fl.now_ms, 5, **place_kw(sd))
+            got = s.place_batch(sd.dec, fl.now_ms, 5, exclude=newest, **place_kw(sd))
             s._ck(product_lib.mmp_tune(s.h, b"split", 2))
-            _same(got, oracle_excluding(o, fl, sd, newest, 5), (pattern, split, "exclude"))
+            same_answers(got, oracle_excluding(o, fl, sd, newest, 5), (pattern, split, "exclude"))
             t, t0 = got["target"], plain["target"]
             assert (vers[t[t >= 0]] < vers.max()).all()
             assert np.count_nonzero((t0 >= 0) & (vers[np.maximum(t0, 0)] == vers.max())) > 10  # without the set, best was newer
@@ -235,15 +138,6 @@ def test_exclude_set_moves_best_across_the_boundary(product_lib, oracle_lib, pat
 # ---------------------------------------------------------------------------------------------------------------
 # commit paths across an upgrade
 # ---------------------------------------------------------------------------------------------------------------
-def _bump(rp: Replay, idx, vers: int):
-    """mmp_instance_update with a new version and nothing else changed (the same pod, restarted on a new image)"""
-    for i in np.atleast_1d(idx):
-        r = rp.rows[int(i)].copy()
-        r["vers"] = vers
-        rp.f.instance_update(int(i), r)
-        rp.rows[int(i)] = r
-
-
 def _check(rp: Replay, seed: int):
     check_against_oracle(rp, seed, 400, 3000)
     check_sorted_batch(rp, seed)
@@ -260,7 +154,7 @@ def test_commit_paths_across_an_upgrade(product_lib, oracle_lib):
     # 1. a uniform fleet: numeric windows on the device
     paths.append(rp.numeric_window(n_inst=40, n_models=80)); _check(rp, 1)
     # 2. one pod restarts on the new version (same id, numeric update): the device path finds two versions, falls back
-    _bump(rp, rp._live()[7], v0 + 1)
+    bump(rp, rp._live()[7], v0 + 1)
     paths.append(rp.numeric_window(n_inst=40, n_models=80)); _check(rp, 2)
     # 3. new-version pods of a new replicaset join at new indices, the old replicasets are marked likely-replaced
     for k in range(3):
@@ -275,14 +169,14 @@ def test_commit_paths_across_an_upgrade(product_lib, oracle_lib):
         paths.append(rp.numeric_window(n_inst=40, n_models=80, n_json=3)); _check(rp, 4 + w)
     # 5. the last old pods are bumped: back on the device path
     live = rp._live()
-    _bump(rp, live[rp.rows["vers"][live] == v0], v0 + 1)
+    bump(rp, live[rp.rows["vers"][live] == v0], v0 + 1)
     paths.append(rp.numeric_window(n_inst=20, n_models=40)); _check(rp, 6)
     paths.append(rp.numeric_window(n_inst=20, n_models=40)); _check(rp, 7)
     # an odd version held only by a shutting-down pod does not force the host path
     i = int(rp._live()[11])
     rp.toggle(i, "shutting_down")
     paths.append(rp.commit(STRUCTURAL, 0, ["toggle"])); _check(rp, 8)
-    _bump(rp, i, v0 + 5)
+    bump(rp, i, v0 + 5)
     paths.append(rp.numeric_window(n_inst=20, n_models=40)); _check(rp, 9)
     assert paths == [2, 1, 1, 1, 1, 2, 2, 1, 2], describe(rp)
 
@@ -294,7 +188,6 @@ def test_commit_paths_across_an_upgrade(product_lib, oracle_lib):
 def test_closed_loop_on_an_upgrade_fleet(product_lib, oracle_lib, with_types, fill, seed):
     """12 windows of the closed loop with about half of the pods on vers + 1, event for event against the oracle's loop;
     every window's commit takes the host path (the live set holds two versions)."""
-    from test_churn_gpu import run_small_closed_loop
     w = make_churn(20_000, 200, seed, fill=fill, with_types=with_types)
     w = dataclasses.replace(w, fleet=upgrade(w.fleet, "half", seed))
     assert len(versions(w.fleet)) == 2
@@ -304,11 +197,10 @@ def test_closed_loop_on_an_upgrade_fleet(product_lib, oracle_lib, with_types, fi
 def test_closed_loop_commit_host_only(product_lib, oracle_lib):
     """The closed loop on a uniform fleet with every commit on the host path (mmp_tune "commit_host_only"): equal to
     the oracle window by window, and byte for byte to a twin fleet whose commits take the device path."""
-    from test_churn_gpu import _build, _compare_window
     w = make_churn(20_000, 200, 4, fill=0.90)
     fl = w.fleet
-    o, sim, s = _build(product_lib, w, slots=256)
-    _, _, twin = _build(product_lib, w, slots=256)
+    o, sim, s = build(product_lib, w, slots=256)
+    _, _, twin = build(product_lib, w, slots=256)
     s._ck(product_lib.mmp_tune(s.h, b"commit_host_only", 1))
     steps = []  # what s.churn_step returned, window by window
     step = s.churn_step
@@ -317,7 +209,7 @@ def test_closed_loop_commit_host_only(product_lib, oracle_lib):
     for ep in range(12):
         ev = w.events(ep, 2000, 4)
         now0 = fl.now_ms + ep * w.window_ms
-        _, _, rep = _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep, path=1)
+        _, _, rep = compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep, path=1)
         got, want = steps[-1], twin.churn_step(ev, now0, now0 + w.window_ms, 400 + ep)
         assert twin.commit_info()[0] == 2
         for k in range(3):  # decisions, evictions, published rows, field by field (an eviction record has 4 bytes of padding)

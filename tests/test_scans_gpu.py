@@ -7,21 +7,9 @@ from modelmesh_b200.synth import SplitMix, make_fleet
 from oracle import binding as ob
 
 from helpers import oracle_from_synth, solver_from_synth
+from scan_checks import partition_maps
 
 pytestmark = pytest.mark.gpu
-
-
-def _partition_maps(fl, o, s):
-    """partition id correspondence through instance membership (numbering differs between the two)."""
-    m = {}
-    for i in range(fl.n_instances):
-        po, ps = o.instance_partition(i), s.instance_partition(i)
-        if fl.inst_rows["shutting_down"][i]:
-            continue
-        assert (po < 0) == (ps < 0)
-        if po >= 0:
-            assert m.setdefault(ps, po) == po
-    return m
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [("C2", 2000, 500, 2), ("C3", 3000, 3000, 3), ("C5", 3000, 2500, 5),
@@ -44,7 +32,7 @@ def test_stats_match_oracle(product_lib, oracle_lib, config, nm, ni, seed):
     if fl.type_config is None:
         assert len(st) == 1
         return
-    pmap = _partition_maps(fl, o, s)
+    pmap = partition_maps(fl, o, s)
     ost, oids = o.partition_stats()
     by_o = {int(i): x for i, x in zip(oids, ost) if x["instance_count"] > 0}
     assert len(st) - 1 == len(by_o)
@@ -72,7 +60,7 @@ def test_reaper_select_matches_oracle(product_lib, oracle_lib, config, nm, ni, s
         b = s.reaper_select(-1, fl.now_ms)
         assert len(a) > 0 and np.array_equal(a, b)
         return
-    pmap = _partition_maps(fl, o, s)
+    pmap = partition_maps(fl, o, s)
     st, ids = s.stats()
     taken_o = np.zeros(nm, dtype=np.uint8)
     taken_s = np.zeros(nm, dtype=np.uint8)

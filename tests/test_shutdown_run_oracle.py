@@ -8,16 +8,11 @@ import numpy as np
 import shutdown_run_oracle as sro
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import NOW_MS
-from test_rate_run_oracle import EXPIRY, HOUR, hand_fleet
+from common import EXPIRY, HOUR
+from pod_task_edges import hand_fleet
+from pod_tasks import shutdown_params
 
 POD = 0
-
-
-def params(now):
-    p = np.zeros(1, dtype=L.SHUTDOWN_PARAMS)
-    p["now"], p["cutoff_age_ms"], p["load_failure_expiry_ms"] = now, HOUR, EXPIRY
-    return p
-
 
 def ents(*rows):
     """rows of (model, lru_t, last_used, flags)"""
@@ -29,7 +24,7 @@ def ents(*rows):
 
 def run(regs, ni, rows, seed=5, **kw):
     fl, ts, o = hand_fleet(regs, ni, **kw)
-    out, rep = sro.shutdown_run(o, fl, ts, POD, ents(*rows), params(fl.now_ms), seed)
+    out, rep = sro.shutdown_run(o, fl, ts, POD, ents(*rows), shutdown_params(fl.now_ms), seed)
     o.close()
     return fl, out, rep
 

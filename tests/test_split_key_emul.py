@@ -14,7 +14,7 @@ from modelmesh_b200._lib import DF_FAVOUR_SELF, DF_MODEL_LAST_USED, DF_REQUEST_M
 from modelmesh_b200.synth import make_decisions, make_fleet
 
 from helpers import oracle_from_synth, solver_from_synth
-from test_rolling_upgrade_gpu import upgrade
+from upgrade import upgrade
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 

@@ -10,12 +10,12 @@ import threading
 import numpy as np
 import pytest
 
+from churn_harness import build, compare_window
 from modelmesh_b200 import _lib as L
 from modelmesh_b200.synth import SynthDecisions, make_churn, make_fleet
 from oracle import binding as ob
 from replay import GAP_TYPE, NUMERIC, STRUCTURAL, Replay, assert_same_results, oracle_batch
-from test_churn_gpu import _build, _compare_window
-from test_rolling_upgrade_gpu import _bump
+from upgrade import bump
 
 pytestmark = pytest.mark.gpu
 
@@ -125,10 +125,10 @@ def test_split_key_through_a_commit_sequence(product_lib, oracle_lib):
     # a rolling upgrade: a third of the pods on the next version (host path), then all of them (device path again)
     live = rp._live()
     v0 = int(rp.rows["vers"][live[0]])
-    _bump(rp, live[::3], v0 + 1)
+    bump(rp, live[::3], v0 + 1)
     assert rp.numeric_window(n_inst=20, n_models=60) == 1
     _check(rp, 14, "upgrade, mixed versions")
-    _bump(rp, rp._live(), v0 + 1)
+    bump(rp, rp._live(), v0 + 1)
     assert rp.numeric_window(n_inst=20, n_models=60) == 2
     _check(rp, 15, "upgrade done")
     rp.f.close()
@@ -171,12 +171,12 @@ def test_split_key_after_churn_windows(product_lib, oracle_lib):
     byte for byte."""
     w = make_churn(20_000, 200, 4, fill=0.9)
     fl = w.fleet
-    o, sim, s = _build(product_lib, w, slots=256)
+    o, sim, s = build(product_lib, w, slots=256)
     rng = np.random.default_rng(4)
     for ep in range(3):
         ev = w.events(ep, 2000, 4)
         now0 = fl.now_ms + ep * w.window_ms
-        _compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep)
+        compare_window(ep, o, sim, s, ev, now0, now0 + w.window_ms, 400 + ep)
         dec = np.zeros(fl.n_models, dtype=L.DECISION_IN)
         dec["model"] = np.arange(fl.n_models)
         dec["self"] = rng.integers(0, fl.n_instances, size=fl.n_models)

@@ -3,53 +3,14 @@ answer they give a decision clear of its slot's reach (split_answer), compiled b
 
 The tests/emul/split_place.cpp harness resolves a batch as k_place_direct does, then answers from the summaries every
 decision k_place_split would answer, and counts the answers that differ from the walk."""
-import ctypes as C
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
-from modelmesh_b200 import _lib
 from modelmesh_b200._lib import DF_FAVOUR_SELF
 from modelmesh_b200.synth import make_decisions, make_fleet
 
-from helpers import oracle_from_synth, oracle_inputs, solver_from_synth
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-@pytest.fixture(scope="module")
-def split_lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("split_place") / "libmmplace_emul_split.so")
-    subprocess.check_call(["g++", "-O2", "-g", "-std=c++17", "-fPIC", "-Wall", "-Wl,-Bsymbolic", "-shared", "-o", so,
-                           os.path.join(HERE, "emul", "split_place.cpp")])
-    lib = _lib.load(so, require_all=False)
-    lib.mmp_emul_place_split.restype = C.c_int32
-    lib.mmp_emul_place_split.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
-                                         C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p]
-    return lib
-
-
-def _ptr(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
-def place_split(lib, s, sd, now_ms, seed):
-    dec = np.ascontiguousarray(sd.dec, dtype=_lib.DECISION_IN)
-    fresh = np.ascontiguousarray(sd.fresh, dtype=_lib.INSTANCE_ROW) if len(sd.fresh) else None
-    extra = np.ascontiguousarray(sd.extra, dtype=np.int32) if len(sd.extra) else None
-    out = np.zeros(len(dec), dtype=_lib.DECISION_OUT)
-    counts = np.zeros(6, dtype=np.int64)
-    s._ck(lib.mmp_emul_place_split(s.h, _ptr(dec), len(dec), _ptr(fresh), 0 if fresh is None else len(fresh), _ptr(extra),
-                                   0 if extra is None else len(extra), _ptr(out), now_ms, seed, _ptr(counts)))
-    return out, counts
-
-
-def _oracle_same(o, fl, sd, out, seed):
-    od, off, idx = oracle_inputs(fl, sd)
-    want = o.get_next_batch(od, fl.type_names, off, idx, fl.now_ms, seed, fresh=sd.fresh if len(sd.fresh) else None)
-    assert np.array_equal(out["target"], want["target"]) and np.array_equal(out["n_candidates"], want["n_candidates"])
+from helpers import oracle_from_synth, solver_from_synth
+from split_place import oracle_same, place_split, split_lib  # noqa: F401  (split_lib: module fixture)
 
 
 @pytest.mark.parametrize("config,nm,ni,seed", [("C3", 3000, 1300, 33), ("C5", 1500, 500, 5), ("MIX", 800, 300, 14),
@@ -67,7 +28,7 @@ def test_summary_answers_equal_the_walk(split_lib, oracle_lib, config, nm, ni, s
     for k, sd in enumerate((sweep, fav, make_decisions(fl, 2000, seed + 1))):
         out, counts = place_split(split_lib, s, sd, fl.now_ms, seed + k)
         assert counts[1] == 0, (config, k, counts)
-        _oracle_same(o, fl, sd, out, seed + k)
+        oracle_same(o, fl, sd, out, seed + k)
         answered += counts[0]
     assert answered > 0
     s.close()
@@ -94,6 +55,6 @@ def test_reach_edges_on_a_front_loaded_fleet(split_lib, oracle_lib):
     for k in range(2):
         out, counts = place_split(split_lib, s, sd, fl.now_ms, 21 + k)
         assert counts[1] == 0, counts
-        _oracle_same(o, fl, sd, out, 21 + k)
+        oracle_same(o, fl, sd, out, 21 + k)
         sd.dec["flags"] |= DF_FAVOUR_SELF
     s.close()
