@@ -12,29 +12,37 @@ from modelmesh_b200.synth import load_into_fleet, make_churn
 from oracle import binding as ob
 
 
-def build(product_lib, w, slots):
+def build_oracle(w, last_published_ms=None):
+    """(the oracle fleet of w, its closed loop seeded with w's caches); every pod last published at last_published_ms
+    (default: a minute before the fleet's clock)"""
     fl = w.fleet
     o = oracle_from_synth(fl, bulk=False if fl.n_instances <= 300 else None)
     models = np.zeros(fl.n_models, dtype=ob.SIM_MODEL)
     models["last_used"], models["type_idx"], models["size_units"] = fl.model_last_used, fl.model_type, fl.model_size
     sim = ob.OracleSim(o, models, fl.type_names, fl.edge_off, fl.edge_inst, fl.n_loaded, w.capacity, w.load_timeout_ms,
-                       fl.now_ms - 60_000)
+                       fl.now_ms - 60_000 if last_published_ms is None else last_published_ms)
     order = np.argsort(w.seed_instance, kind="stable")
     bounds = np.searchsorted(w.seed_instance[order], np.arange(fl.n_instances + 1))
     for i in range(fl.n_instances):
         sel = order[bounds[i]:bounds[i + 1]]
         if len(sel):
             sim.seed(i, w.seed_model[sel], w.seed_last_used[sel], w.seed_weight[sel], w.seed_load_ts[sel], fl.now_ms)
+    return o, sim
+
+
+def build(product_lib, w, slots, last_published_ms=None):
+    fl = w.fleet
+    o, sim = build_oracle(w, last_published_ms)
     s = Fleet(fl.min_space_units, fl.min_churn_age_ms, fl.default_model_size_units, fl.n_instances, fl.n_models, lib=product_lib)
     load_into_fleet(fl, s)
-    s.churn_init(w.load_timeout_ms, fl.now_ms - 60_000, slots)
+    s.churn_init(w.load_timeout_ms, fl.now_ms - 60_000 if last_published_ms is None else last_published_ms, slots)
     s.churn_seed(w.seed_instance, w.seed_model, w.seed_last_used, w.seed_weight, w.seed_load_ts, fl.now_ms)
     return o, sim, s
 
 
-def compare_window(ep, o, sim, s, ev, now0, now1, seed, path=2):
+def compare_window(ep, o, sim, s, ev, now0, now1, seed, path=2, out=None):
     """path: the commit path the window must end with (mmp_commit_info): 2, the device path; 1, the host path (a live set
-    of more than one instance version, or commit_host_only)"""
+    of more than one instance version, or commit_host_only); out: a dict that receives both sides' instance rows"""
     dec_o, evi_o, rows_o, npub_o, carry_o = sim.step(ev, now0, now1, seed)
     dec_p, evi_p, rows_p, rep = s.churn_step(ev, now0, now1, seed)
     assert len(dec_p) == len(dec_o), (ep, len(dec_p), len(dec_o))
@@ -54,6 +62,8 @@ def compare_window(ep, o, sim, s, ev, now0, now1, seed, path=2):
     assert rep.n_published == npub_o and rep.n_carry == carry_o, (ep, rep.n_published, npub_o, rep.n_carry, carry_o)
     assert np.array_equal(s.cluster_order(), o.cluster_order()), ep
     assert s.commit_info()[0] == path, (ep, s.commit_info()[0], path)
+    if out is not None:
+        out.update(rows_o=rows_o, rows_p=rows_p)
     return dec_o, evi_o, rep
 
 
