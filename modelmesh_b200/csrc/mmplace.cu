@@ -127,6 +127,16 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// cp.async (SASS LDGSTS): BYTES (4, 8 or 16) from global to shared memory without passing through registers, so a thread
+// has its whole share of a copy in flight at once (cp_async_wait_all ends it); in = false writes BYTES zero bytes and
+// reads nothing
+template <int BYTES>
+__device__ __forceinline__ void cp_async_or_zero(void *dst, const void *src, bool in) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2, %3;" ::"r"(smem_u32(dst)), "l"(__cvta_generic_to_global(src)), "n"(BYTES),
+               "r"(in ? BYTES : 0)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -406,15 +416,18 @@ static constexpr int LANE_SLOTS = 64;    // type-constraint mask slots whose win
 static constexpr int LANE_WARPS = 12;    // warps per block of k_place_lanes
 static constexpr int LANE_STAGES = 4;    // landing stages per SM at most: a fifth takes the shared-memory carve-out from 196 to
                                          // 228 KB and leaves too little L1 for the lane tables to stay resident
-// The window part of the lane tables in shared memory (k_place_lanes, k_place_server): the masks of the first LANE_SLOTS
-// slots and full / csum / count_col / rows over the first LANE_WIN words of this process's rows, zero past their end.
+// The window part of the lane tables in shared memory (k_place_lanes, k_place_server, k_slot_summary): the masks of the
+// first LANE_SLOTS slots and full / csum / count_col / rows over the first LANE_WIN words of this process's rows, zero past
+// their end.
 struct WinTabs {
   uint32_t cx[LANE_SLOTS * LANE_WIN], p[LANE_SLOTS * LANE_WIN], full[LANE_WIN];
   WordSumI csum[LANE_WIN];
   __align__(16) int32_t count[LANE_WIN * 32];
   __align__(16) RankRow rows[LANE_WIN * 32];
   // thread tid of nthreads copies its share of the tables (the caller synchronises).  N: the type of the stride, blockDim.x
-  // or a constant int, as each kernel steps its loops (it decides how far the compiler unrolls them)
+  // or a constant int, as each kernel steps its loops (it decides how far the compiler unrolls them).  Every element is
+  // one cp.async and the thread waits once at the end: its share costs one round trip to memory, not one per element
+  // (k_slot_summary waits for the copy with every other SM idle).
   template <class N>
   __device__ __forceinline__ void fill(const SnapshotView &s, int tid, N nthreads) {
     const int WS = s.word_lo;
@@ -424,21 +437,30 @@ struct WinTabs {
     for (int i = tid; i < nsl * LANE_WIN; i += nthreads) {
       const int sl = i / LANE_WIN, w = i - sl * LANE_WIN;
       const bool in = (uint32_t)w < win_words;
-      cx[i] = in ? gcx[(size_t)sl * s.row_words + WS + w] : 0u;
-      p[i] = in ? s.pref[(size_t)sl * s.row_words + WS + w] : 0u;
+      const size_t g = in ? (size_t)sl * s.row_words + WS + w : 0;
+      cp_async_or_zero<4>(cx + i, gcx + g, in);
+      cp_async_or_zero<4>(p + i, s.pref + g, in);
     }
     for (int w = tid; w < LANE_WIN; w += nthreads) {
       const bool in = (uint32_t)w < win_words;
-      full[w] = in ? s.full[WS + w] : 0u;
-      csum[w] = in ? s.csum[WS + w] : WordSumI{0, 0};
+      cp_async_or_zero<4>(full + w, s.full + (in ? WS + w : 0), in);
+      const WordSumI *gs = s.csum + (in ? WS + w : 0);
+      cp_async_or_zero<4>(&csum[w].lo, &gs->lo, in);
+      cp_async_or_zero<4>(&csum[w].hi, &gs->hi, in);
     }
     for (int i = tid; i < LANE_WIN * 32; i += nthreads) {
       const int r = WS * 32 + i;
       const bool in = (uint32_t)(i >> 5) < win_words && r < s.n_ranks;
-      count[i] = in ? s.count_col[r] : 0;
-      RankRow z; z.lru = 0; z.rem = 0; z.count = 0; z.rpm = 0; z.idx = -1; z.flags = 0;
-      rows[i] = in ? s.rows[r] : z;
+      cp_async_or_zero<4>(count + i, s.count_col + (in ? r : 0), in);
+      if (in) {
+        cp_async_or_zero<16>(&rows[i], &s.rows[r], true);
+        cp_async_or_zero<16>(reinterpret_cast<char *>(&rows[i]) + 16, reinterpret_cast<const char *>(&s.rows[r]) + 16, true);
+      } else {
+        RankRow z; z.lru = 0; z.rem = 0; z.count = 0; z.rpm = 0; z.idx = -1; z.flags = 0;
+        rows[i] = z;
+      }
     }
+    cp_async_wait_all();
   }
   // T (the slot's global tables) with its window part pointed here: indexed by absolute row word / rank, so biased by the
   // window's first word
@@ -742,24 +764,26 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
 
 // ---- the two-pass path of a large batch (launch_place, DESIGN.md §5.2) ----
 // one lane per (type slot, c_self): the slot summaries of this call's view (slot_summary); also zeroes the worklist counters
-// and k_place_tail's work counter
+// and k_place_tail's work counter.  The walks and the member listing read the window part of the tables from shared memory
+// (a block copies it in one parallel pass): each of their steps waits on the one before, and from global memory each would
+// be a round trip to L2 or DRAM.  Every lane's exclusion window is the same all-zero one.
 __global__ void __launch_bounds__(128) k_slot_summary(const SnapshotView s, int64_t now, SlotSummary *__restrict__ sums,
                                                       int32_t *__restrict__ members, int32_t *__restrict__ counts) {
-  __shared__ uint32_t win_s[4][32 * LANE_STRIDE];
+  __shared__ WinTabs tabs;
+  __shared__ uint32_t zwin[LANE_WIN];
   __shared__ uint32_t chunk_s[4][32 * MMP_CHUNK_WORDS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int t = blockIdx.x * 128 + threadIdx.x, sl = t >> 1, cs = t & 1;
   if (t < 3) counts[t] = 0;
+  if (threadIdx.x < LANE_WIN) zwin[threadIdx.x] = 0u;
+  tabs.fill(s, threadIdx.x, 128);
+  __syncthreads();
   const bool active = sl < s.n_slots;
-  uint32_t *w = win_s[warp] + lane * LANE_STRIDE;
-#pragma unroll
-  for (int j = 0; j < LANE_WIN; j++) w[j] = 0u;
-  __syncwarp();
   const int slot = active ? sl : 0;
   const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
   const LaneTables T = lane_tables_global(s, slot);
-  slot_summary(s, T, slot, active, cs, w, win_words, now, WarpVote(), chunk_s[warp] + lane * MMP_CHUNK_WORDS, sums[slot],
-               members + ((size_t)slot * 2 + cs) * SPLIT_CAP);
+  slot_summary<TabWin>(s, tabs.view(T, slot, s.word_lo), T, slot, active, cs, zwin, win_words, now, WarpVote(),
+                       chunk_s[warp] + lane * MMP_CHUNK_WORDS, sums[slot], members + ((size_t)slot * 2 + cs) * SPLIT_CAP);
 }
 // appends v to list (length in *count) for the lanes where p holds: one atomic per warp
 __device__ __forceinline__ void warp_append(bool p, int32_t v, int32_t *list, int32_t *count) {

@@ -876,7 +876,8 @@ MMP_HD WordSumI ldro_sum(const WordSumI *p) {
 
 // how the lane routine reads its tables: beyond the window through the read-only path from the snapshot's own arrays
 // (TabGlob); inside the window through plain loads (TabWin) where the caller points them at shared-memory copies of the
-// tables' window part (k_place_lanes, k_place_server), or through TabGlob too where its window tables are the global ones
+// tables' window part (k_place_lanes, k_place_server, k_slot_summary), or through TabGlob too where its window tables are
+// the global ones
 struct TabWin {
   const LaneTables &t;
   MMP_HD uint32_t cx(uint32_t wi) const { return t.cx[wi]; }
@@ -927,6 +928,16 @@ struct TabGlob {
 #endif
     return vm;
   }
+};
+// a lookup by rank or row word that may land on either side of the window's end: row word wi < win_end (rank r: word
+// r >> 5) from the window tables w, every later one from the global tables g
+template <class AWT>
+struct TabEither {
+  const AWT &w; const TabGlob &g; uint32_t win_end;
+  MMP_HD uint32_t cx(uint32_t wi) const { return wi < win_end ? w.cx(wi) : g.cx(wi); }
+  MMP_HD uint32_t p(uint32_t wi) const { return wi < win_end ? w.p(wi) : g.p(wi); }
+  MMP_HD RankRow row(uint32_t r) const { return (r >> 5) < win_end ? w.row(r) : g.row(r); }
+  MMP_HD int32_t idx(uint32_t r) const { return (r >> 5) < win_end ? w.idx(r) : g.idx(r); }
 };
 // a step beyond the window: its filtered word (candidates & ~exclusions), preferred word and count class were gathered
 // when the chunk of 8 steps was (re)filled -- one round of independent loads per 8 steps instead of three dependent ones
@@ -1054,8 +1065,8 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
     for (int e = 0; e < LANE_MAX_EXTRA; e++) { const int32_t r = c.xr[e]; if (r >= 0 && ((uint32_t)r >> 5) == wi) m |= 1u << (r & 31); }
     return m;
   };
-  auto pbit = [&](uint32_t r) -> bool { const uint32_t w = r >> 5; return ((w < win_end ? AW.p(w) : AG.p(w)) >> (r & 31)) & 1u; };
-  auto row_of = [&](uint32_t r) -> RankRow { return (r >> 5) < win_end ? AW.row(r) : AG.row(r); };
+  const TabEither<AWT> AE{AW, AG, win_end};
+  auto pbit = [&](uint32_t r) -> bool { return (AE.p(r >> 5) >> (r & 31)) & 1u; };
   // ---- beyond the window: a chunk of 8 consecutive steps [base, base + 8) in registers ----
   uint32_t base = 0xfffffff0u;  // no chunk loaded
   // chunk storage, MMP_CHUNK_WORDS words per lane: [0,4) the list entries (u16 pairs), [4,12) filtered words cx & ~row,
@@ -1160,7 +1171,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   // take entries out of F, so it would find nothing with them either.
   uint32_t dep = b;
   if (live) {
-    rb = row_of(b);
+    rb = AE.row(b);
     us = rb.idx == d.self;
     best_rem = us ? fr.rem : rb.rem; best_count = us ? fr.count : rb.count; best_rpm = us ? fr.rpm : rb.rpm; best_idx = rb.idx;
     best_lru = us ? fr.lru : rb.lru;
@@ -1227,7 +1238,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   if (live && !simple && !best_full) {
     if (r1 == NONE_RANK) open = open_end;  // else: neither kind follows, "no preference" logic over the whole remainder
     else if (pbit(r1)) {
-      const RankRow rp = row_of(r1);
+      const RankRow rp = AE.row(r1);
       best_rank = r1; best_idx = rp.idx; best_rem = rp.rem; best_count = rp.count; best_rpm = rp.rpm;
       us = rp.idx == d.self;
       lo = r1; k_lo = k1; use_pref = true;
@@ -1388,7 +1399,7 @@ MMP_HD bool decide_stream(const SnapshotView &s, const LaneTables &Tw, const Lan
   o.best = best_idx; o.best_rank = (int32_t)best_rank;
   if (open) { o.flags = MMP_TF_OPEN; return true; }
   if (!done) {
-    const int32_t cidx = chosen_rank == best_rank ? best_idx : ((int32_t)chosen_rank == self_rank ? d.self : ((chosen_rank >> 5) < win_end ? AW.idx(chosen_rank) : AG.idx(chosen_rank)));
+    const int32_t cidx = chosen_rank == best_rank ? best_idx : ((int32_t)chosen_rank == self_rank ? d.self : AE.idx(chosen_rank));
     o.target = target_of(cidx, d);
     o.n_candidates = ccount;
     o.n_remaining = remaining; o.pick_index = (int32_t)index;
@@ -1675,10 +1686,12 @@ struct SlotSummary {
 // The summary of type slot `slot` for c_self = cs, and its shortlist members (instance indices, rank order) into
 // members[0, SPLIT_CAP): decide_stream on a decision without exclusions, with a self that is not live and a record
 // that makes c_self come out as cs.  Called by every lane of the vote group (active = false for lanes without a slot);
-// ewin: win_words zero words.
-template <class V>
-MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, bool active, int cs, const uint32_t *ewin,
-                         uint32_t win_words, int64_t now, const V &vote, uint32_t *chunk, SlotSummary &sum, int32_t *members) {
+// ewin: win_words zero words.  Tw, AWT: the window's tables and how they are read, as for decide_stream; every rank or
+// word read after the walks comes from them inside the window and from T beyond it.
+template <class AWT = TabWin, class V>
+MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &Tw, const LaneTables &T, int slot, bool active, int cs,
+                         const uint32_t *ewin, uint32_t win_words, int64_t now, const V &vote, uint32_t *chunk, SlotSummary &sum,
+                         int32_t *members) {
   DecisionCtx c;
   c.d.model = 0; c.d.self = -1; c.d.last_used = 0; c.d.flags = 0; c.d.fresh = -1; c.d.extra_off = 0; c.d.extra_n = 0;
   c.last_used = 0; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
@@ -1691,14 +1704,17 @@ MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, b
   // first pass: the best (phases A, A', A'' do not read the caller's record of a self that is not live), and the
   // shortlist when the best has room
   DecideOut o;
-  bool ok = decide_stream<TabGlob>(s, T, T, c, active, ewin, win_words, none, 0u, now, 0, 0, vote, o, 0x3fffffff, chunk) && active &&
+  bool ok = decide_stream<AWT>(s, Tw, T, c, active, ewin, win_words, none, 0u, now, 0, 0, vote, o, 0x3fffffff, chunk) && active &&
             o.best_rank >= 0 && !(o.flags & MMP_TF_OPEN);
+  const AWT AW{Tw};
+  const TabGlob AG{T};
+  const TabEither<AWT> AE{AW, AG, (uint32_t)s.word_lo + win_words};
   RankRow r0, rb;
   r0.lru = r0.rem = 0; r0.rpm = 0; rb = r0; rb.idx = -1;
   bool full = false;
   if (ok) {
-    r0 = load_row(s.rows + o.first_rank);
-    rb = load_row(s.rows + o.best_rank);
+    r0 = AE.row((uint32_t)o.first_rank);
+    rb = AE.row((uint32_t)o.best_rank);
     full = r0.rem < s.min_space;  // (a full first entry is never replaced as best: A' runs for a best with room only)
     if (full) {
       const int64_t a10 = age_of(r0.lru, now) / 10;
@@ -1706,9 +1722,12 @@ MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, b
     }
   }
   // second pass, for a full best: c_self tests lruTime against the best's, which the record now forces to come out as cs
+  // (skipped by the whole vote group when none of its lanes has a full best: with every lane idle it still takes ~0.9 µs
+  // on an H100)
   const bool again = ok && full;
   DecideOut ox;
-  const bool ok2 = decide_stream<TabGlob>(s, T, T, c, again, ewin, win_words, none, 0u, now, 0, 0, vote, ox, 0x3fffffff, chunk);
+  bool ok2 = false;
+  if (vote.any(again)) ok2 = decide_stream<AWT>(s, Tw, T, c, again, ewin, win_words, none, 0u, now, 0, 0, vote, ox, 0x3fffffff, chunk);
   const DecideOut &o2 = again ? ox : o;
   ok = ok && (!again || ok2) && o2.best_rank == o.best_rank && !(o2.flags & (MMP_TF_OPEN | MMP_TF_FAVOUR_EXIT)) && o2.n_candidates >= 1 &&
        o2.n_candidates - 1 <= SPLIT_CAP;
@@ -1716,12 +1735,12 @@ MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, b
   if (ok) {  // the members: S' strictly between best and the cut (no cut: the end of S, one below the reach)
     const uint32_t lo = (uint32_t)o2.best_rank;
     const uint32_t lim = o2.cut_rank != (int32_t)NONE_RANK ? (uint32_t)o2.cut_rank : (o2.reach == (int32_t)NONE_RANK ? NONE_RANK : (uint32_t)o2.reach - 1u);
-    const bool use_pref = (c.slot >> 16) && ((T.p[lo >> 5] >> (lo & 31)) & 1u);
+    const bool use_pref = (c.slot >> 16) && ((AE.p(lo >> 5) >> (lo & 31)) & 1u);
     int32_t k = 0;
     for (uint32_t w = lo >> 5; w < (uint32_t)s.row_words && w * 32u < lim && k <= n_in; w++) {
-      uint32_t x = T.cx[w] & (use_pref ? T.p[w] : 0xffffffffu) & mask_above(w * 32u, lo) & mask_below(w * 32u, lim);
+      uint32_t x = AE.cx(w) & (use_pref ? AE.p(w) : 0xffffffffu) & mask_above(w * 32u, lo) & mask_below(w * 32u, lim);
       for (; x; x &= x - 1u) {
-        if (k < SPLIT_CAP) members[k] = s.rows[w * 32u + (uint32_t)ffs32(x)].idx;
+        if (k < SPLIT_CAP) members[k] = AE.idx(w * 32u + (uint32_t)ffs32(x));
         k++;
       }
     }
@@ -1731,6 +1750,13 @@ MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, b
   if (cs == 0) { sum.best_rem = rb.rem; sum.best_lru = r0.lru; sum.best_idx = rb.idx; sum.best_rpm = rb.rpm; sum.best_full = full ? 1 : 0; sum.pad_ = 0; }
   sum.reach[cs] = ok ? o2.reach : -1;
   sum.n_in[cs] = n_in;
+}
+
+// The same summary for a caller whose window tables are the global ones (the CPU harness)
+template <class V>
+MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, bool active, int cs, const uint32_t *ewin,
+                         uint32_t win_words, int64_t now, const V &vote, uint32_t *chunk, SlotSummary &sum, int32_t *members) {
+  slot_summary<TabGlob>(s, T, T, slot, active, cs, ewin, win_words, now, vote, chunk, sum, members);
 }
 
 // The fast answer of k_place_split: a valid, unflagged decision without extra excludes whose model has no overflow ids
