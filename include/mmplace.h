@@ -266,9 +266,12 @@ int64_t mmp_shard_open_decisions(mmp_fleet *);                  /* decisions tha
  * DEALT across the shards -- each decides 1/shard_count of it, reading row words beyond the replicated front from the owning
  * shard's memory, and stores its results into every shard's result buffer.  No NCCL call and no host synchronisation on
  * that path (mmp_shard_connect is then optional).  Each shard: export (after its first commit or before), exchange the
- * blobs by any means, import all shard_count blobs ordered by rank.  Works across processes (CUDA IPC) and between fleets
- * of one process (peer access).  Same contract as the collective path: every shard commits the same epochs and is given
- * the same batches in the same order; every shard ends with the whole batch's results.  Batches of up to max_batch. */
+ * blobs by any means, import all shard_count blobs ordered by rank.  Works across processes (CUDA IPC), between fleets
+ * of one process on different devices (peer access), and between up to 16 fleets of one process on the same device (their
+ * memory is used directly; each shard's call then needs a thread of its own, and no shard may synchronise the device -- a
+ * buffer that grows, a commit, mmp_fleet_destroy -- while a peer is inside a call, since the peer waits for it).  Same
+ * contract as the collective path: every shard commits the same epochs and is given the same batches in the same order;
+ * every shard ends with the whole batch's results.  Batches of up to max_batch. */
 #define MMP_SHARD_IPC_BYTES 512
 int32_t mmp_shard_ipc_export(mmp_fleet *, int32_t max_batch, void *blob /* MMP_SHARD_IPC_BYTES */);
 int32_t mmp_shard_ipc_import(mmp_fleet *, const void *blobs /* shard_count x MMP_SHARD_IPC_BYTES, by shard rank */);
@@ -910,7 +913,8 @@ int32_t mmp_tune(mmp_fleet *, const char *key, int64_t value);
  * "reaper_run": mmp_reaper_run from its prune sweep to its last placement kernel; "janitor_run": mmp_janitor_run from its stats
  * kernel to its budget walk; "janitor_task": mmp_janitor_task from its cache-pass plan kernel to its budget walk; "rate_run": mmp_rate_run from its stats kernel to its last placement round; "shutdown_run":
  * mmp_shutdown_run from its index kernel to its pack kernel; "evict_run": mmp_evict_run from its stats kernel to its pack kernel;
- * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait of the last peer-access step of an instance-sharded fleet */
+ * "dealt_kernel" / "dealt_wait": k_place_dealt and the arrival wait (up to the host's wake-up) of the last peer-access step
+ * of an instance-sharded fleet */
 int32_t mmp_last_timing(mmp_fleet *, const char *key, double *ms);
 /* which path the last mmp_fleet_commit took: 1 = structural (host: string ranks, type-constraint sets, sort), 2 = device
  * (numeric instance updates / model-record deltas only: scattered into the device-resident tables, re-ranked and rebuilt

@@ -1061,7 +1061,9 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_dealt(const Snapshot
   RowDealt row{front, P.blocks, (uint32_t)front_words, (uint32_t)s.excl_stride, (uint32_t)s.excl_stride, (uint64_t)m, (uint32_t)me, 0u};
   uint32_t self_eword = 0;
   if (valid && c.self_rank >= 0) self_eword = row.word((uint32_t)(c.self_rank >> 5));
-  // the window: the first MMP_LANE_WIN words of the row, from the replicated front (local memory on every shard)
+  // the window: the first MMP_LANE_WIN words of the row, from the replicated front (local memory on every shard).
+  // Rows are whole 32-word units (HostState::row_words), so front_words is always SHARD_FRONT_WORDS = 16: the scalar
+  // loads and the no-window case below are never taken, and no test reaches them.
   const uint32_t win_words = (uint32_t)min(min(LANE_WIN, front_words), RW);
   uint32_t *w = win_d[warp] + lane * LANE_STRIDE;
   if ((front_words & 3) == 0) {  // (front rows are 16-byte aligned then: three vector loads)
@@ -1671,6 +1673,11 @@ static int32_t place_dealt(mmp_fleet *f, PlaceCtx *c, const DeviceSnapshot &ds, 
   CK(cudaEventRecord(pr.ev[1], st));
   k_dealt_wait<<<1, 32, 0, st>>>(P, G, me, step, 4000000000ull, pr.err.as<int>());
   CK(cudaGetLastError());
+  // Nothing goes onto the stream behind k_dealt_wait until it has completed.  Shard fleets of one device share its
+  // hardware work queues, and a stream maps onto one of them: work queued behind the wait (an event, the result copy)
+  // would stand at the head of that queue until the wait ends, and a peer's k_place_dealt queued behind it could then not
+  // start -- the wait would wait for itself until the timeout.  (ev[2] therefore also counts the host's wake-up.)
+  CK(cudaStreamSynchronize(st));
   CK(cudaEventRecord(pr.ev[2], st));
   CK(cudaMemcpyAsync(d_out, pr.out_buf() + (size_t)(step & 1) * pr.max_batch, (size_t)n * sizeof(mmp_decision_out),
                      cudaMemcpyDeviceToDevice, st));
@@ -1935,7 +1942,9 @@ int32_t mmp_shard_ipc_import(mmp_fleet *f, const void *blobs) {
     if (bl.magic != 0x4d4d5049u || (int)bl.rank != q || (int)bl.count != G) { g_err = "blob of the wrong shard / fleet"; return MMP_E_ARG; }
     if ((int32_t)bl.max_batch != pr.max_batch) { g_err = "shards exported different max_batch"; return MMP_E_ARG; }
     if (q == me) continue;
-    if (bl.pid == (uint64_t)getpid()) {  // the peer fleet lives in this process: its pointers are valid here once peer access is on
+    if (bl.pid == (uint64_t)getpid() && bl.device == f->device) {  // a peer fleet of this process on this device: its pointers as they are
+      for (int k = 0; k < 3; k++) pr.peer_base[q][k] = (void *)(uintptr_t)bl.ptr[k];
+    } else if (bl.pid == (uint64_t)getpid()) {  // ... on another device: its pointers are valid here once peer access is on
       int can = 0;
       CK(cudaDeviceCanAccessPeer(&can, f->device, bl.device));
       if (!can) { g_err = "no peer access between the shards' devices"; return MMP_E_CUDA; }
