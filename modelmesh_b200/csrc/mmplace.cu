@@ -5,7 +5,7 @@
 //                                         the instance under PLACEMENT_ORDER; row stride is a multiple of 128 B
 //   excl_ranks [n_models] int4            the ranks of a model's <= 4 inline edges (-1: none), r[0] = -2: overflow ids,
 //                                         read the row (unsharded fleets)
-//   split_key [n_models] SplitKey 16 B    what k_place_split reads of a model: last_used, lowest live inline rank, type
+//   split_key [n_models] SplitKey 16 B    what k_place_split reads of a model: last_used, lowest live candidate rank, type
 //                                         slot | overflow bit (unsharded fleets; built beside excl_ranks)
 //   zero_row  [row_words]           u32   all zero, one per fleet: the row of every MMP_DF_REQUEST_MODEL decision (unsharded fleets)
 //   cand/pref [n_slots][row_words]  u32   per type-constraint slot: allowed ∧ active / preferred instances (TCM:242-251)
@@ -79,11 +79,13 @@ static thread_local std::string g_err;
 // One thread per model scatters its (<= 4) inline edges into its own bitmap row: no atomics needed.
 // (instance-sharded: a stored row holds row words [word_lo, word_hi) at a stride of `stride` words)
 // ranks (optional, SnapshotView::excl_ranks): the rank of every bit set here, -1 for an edge that sets none.
-// keys (optional, SnapshotView::split_key, with ranks): each model's SplitKey from the snapshot's model rows and type slots.
+// keys (optional, SnapshotView::split_key, with ranks): each model's SplitKey from the snapshot's model rows, type slots
+// and cand masks (row_words words per slot).
 __global__ void k_build_bitmap(uint32_t *__restrict__ excl, const int4 *__restrict__ edge_inl,
                                const int32_t *__restrict__ rank_of, int n_models, int stride, int word_lo, int word_hi,
                                int4 *__restrict__ ranks, const mmp_model_row *__restrict__ models,
-                               const uint16_t *__restrict__ type_slot, int n_type_ids, SplitKey *__restrict__ keys) {
+                               const uint16_t *__restrict__ type_slot, int n_type_ids, const uint32_t *__restrict__ cand,
+                               int row_words, SplitKey *__restrict__ keys) {
   int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= n_models) return;
   int4 e = edge_inl[m];
@@ -98,20 +100,23 @@ __global__ void k_build_bitmap(uint32_t *__restrict__ excl, const int4 *__restri
     }
   }
   if (ranks) ranks[m] = make_int4(rs[0], rs[1], rs[2], rs[3]);
-  if (keys) keys[m] = make_split_key(models[m], rs, type_slot, n_type_ids);
+  if (keys) keys[m] = make_split_key(models[m], rs, type_slot, n_type_ids, cand, row_words);
 }
-// (launched after k_build_bitmap: a model with overflow edges gets the EXCL_RANKS_OVF marker in its rank entry and
-// SPLIT_KEY_OVF in its SplitKey)
+// (launched after k_build_bitmap: a model with overflow edges gets the EXCL_RANKS_OVF marker in its rank entry, and
+// SPLIT_KEY_OVF and the candidate ranks of its overflow edges in its SplitKey, which keeps SPLIT_KEY_ALL_EDGES)
 __global__ void k_build_bitmap_ovf(uint32_t *__restrict__ excl, const OvfEdge *__restrict__ ovf, int n_ovf,
                                    const int32_t *__restrict__ rank_of, int stride, int word_lo, int word_hi, int4 *__restrict__ ranks,
-                                   SplitKey *__restrict__ keys) {
+                                   const uint32_t *__restrict__ cand, int row_words, SplitKey *__restrict__ keys) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_ovf) return;
   const int m = ovf[i].model, r = rank_of[ovf[i].inst];
   if (r >= 0 && (r >> 5) >= word_lo && (r >> 5) < word_hi)
     atomicOr(&excl[(size_t)m * stride + ((r >> 5) - word_lo)], 1u << (r & 31));
   if (ranks) ranks[m].x = EXCL_RANKS_OVF;
-  if (keys) atomicOr(&keys[m].slot, SPLIT_KEY_OVF);  // (a model's overflow edges are many threads)
+  if (keys) {  // (a model's overflow edges are many threads; the slot bits are k_build_bitmap's, which no thread changes)
+    const uint32_t sl = atomicOr(&keys[m].slot, SPLIT_KEY_OVF) & SPLIT_KEY_SLOT;
+    if (r >= 0 && mask_bit(cand + (size_t)sl * (size_t)row_words, r)) atomicMin(&keys[m].min_rank, r);
+  }
 }
 
 // ---- TMA 1-D bulk copy + mbarrier helpers (cp.async.bulk: SASS UBLKCP) ----
@@ -816,8 +821,15 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
   k.last_used = 0; k.min_rank = INT32_MAX; k.slot = 0;
   if (ok) self_rank = __ldg(s.rank_of + d.self);
   if (ok && !req) k = load_split_key(s.split_key + d.model);
+  // whether self is a member of its slot's mask (split_answer: a self that is not cannot change the answer), gathered
+  // beside self's rank row
+  bool self_cand = true;
+  if (ok && !req && self_rank >= 0)
+    self_cand = (__ldg((s.any_rs ? s.candx : s.cand) + (size_t)(k.slot & SPLIT_KEY_SLOT) * (size_t)s.row_words + ((uint32_t)self_rank >> 5)) >>
+                 (self_rank & 31)) & 1u;
   mmp_decision_out r;
-  const bool fast = ok && split_answer(s, d, ok, self_rank, k, fresh, n_fresh, sums, members, now, seed, pick_id(d, id_base + (uint64_t)i), r);
+  const bool fast = ok && split_answer(s, d, ok, self_rank, k, fresh, n_fresh, sums, members, now, seed, pick_id(d, id_base + (uint64_t)i), r,
+                                       self_cand);
   if (fast) out[i] = r;
   const bool ovf = ok && !req && !fast && (k.slot & SPLIT_KEY_OVF);
   const bool walk = valid && !fast && !ovf;
@@ -825,7 +837,7 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
   warp_append(ovf, i, ovf_list, counts + 1);
   if (keys && valid) {
     uint32_t key = 0xffffu;
-    if (walk) key = !ok ? 0xfffeu : req ? slot_key(s, d.model) : k.slot;
+    if (walk) key = !ok ? 0xfffeu : req ? slot_key(s, d.model) : k.slot & SPLIT_KEY_SLOT;
     keys[i] = (uint16_t)key;
     key_idx[i] = i;
   }
@@ -2345,12 +2357,13 @@ static int32_t commit_locked(mmp_fleet *f, bool rows_on_device) {
     CK(cudaMemsetAsync(ds.excl.p, 0, (size_t)nm * ST * 4, st));
     k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, ST,
                                                      h.word_lo, h.word_hi, ranks, ds.models.as<mmp_model_row>(),
-                                                     ds.type_slot.as<uint16_t>(), (int)h.type_slot.size(), keys);
+                                                     ds.type_slot.as<uint16_t>(), (int)h.type_slot.size(), ds.cand.as<uint32_t>(), RW, keys);
     f->launches++;
     CK(cudaGetLastError());
     if (lv.n_ovf) {
       k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.excl.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf,
-                                                                 ds.rank_of.as<int32_t>(), ST, h.word_lo, h.word_hi, ranks, keys);
+                                                                 ds.rank_of.as<int32_t>(), ST, h.word_lo, h.word_hi, ranks,
+                                                                 ds.cand.as<uint32_t>(), RW, keys);
       f->launches++;
       CK(cudaGetLastError());
     }
@@ -2360,8 +2373,9 @@ static int32_t commit_locked(mmp_fleet *f, bool rows_on_device) {
     CK(ds.front.ensure((size_t)nm * F * 4));
     CK(cudaMemsetAsync(ds.front.p, 0, (size_t)nm * F * 4, st));
     k_build_bitmap<<<(nm + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.edges.as<int4>(), ds.rank_of.as<int32_t>(), nm, F, 0, F, nullptr,
-                                                     nullptr, nullptr, 0, nullptr);
-    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F, nullptr, nullptr);
+                                                     nullptr, nullptr, 0, nullptr, 0, nullptr);
+    if (lv.n_ovf) k_build_bitmap_ovf<<<(lv.n_ovf + 255) / 256, 256, 0, st>>>(ds.front.as<uint32_t>(), lv.ovf.as<OvfEdge>(), lv.n_ovf, ds.rank_of.as<int32_t>(), F, 0, F, nullptr,
+                                                                              nullptr, 0, nullptr);
     f->launches += 2;
     CK(cudaGetLastError());
   }

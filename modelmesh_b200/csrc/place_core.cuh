@@ -71,10 +71,12 @@ struct WordSumI { int32_t lo, hi; };  // min/max count over the 32 ranks of a bi
 struct WordSumL { int64_t lo, hi; };  // min/max lruTime
 struct FreshRow { int64_t lru, rem; int32_t count, rpm; };  // getFreshInstanceRecord() (MM:5369-5386), what the walk reads of it
 // What k_place_split reads of a decision's model: one 16-byte entry per model, built at commit beside excl_ranks
-// (make_split_key) and fixed for the epoch.  last_used: the snapshot's model row's; min_rank: the lowest live rank among
-// its inline edges, INT32_MAX for none; slot: slot_key of its type id, SPLIT_KEY_OVF set for a model with overflow ids.
+// (make_split_key) and fixed for the epoch.  last_used: the snapshot's model row's; min_rank: the lowest live rank of its
+// exclusion row that is a member of its slot's cand, INT32_MAX for none (SPLIT_KEY_ALL_EDGES: every edge, inline and
+// overflow, counted; without it: the inline edges only, candidates or not); slot: slot_key of its type id (SPLIT_KEY_SLOT),
+// SPLIT_KEY_OVF set for a model with overflow ids.
 struct alignas(16) SplitKey { int64_t last_used; int32_t min_rank; uint32_t slot; };
-static constexpr uint32_t SPLIT_KEY_OVF = 0x80000000u;
+static constexpr uint32_t SPLIT_KEY_OVF = 0x80000000u, SPLIT_KEY_ALL_EDGES = 0x40000000u, SPLIT_KEY_SLOT = 0x7fffu;
 
 struct SnapshotView {  // pointers into HBM (or host vectors in the CPU harness)
   int32_t n_ranks, row_words, n_models, max_instances;
@@ -614,14 +616,22 @@ MMP_HD uint32_t slot_key_of(const uint16_t *type_slot, int32_t n_type_ids, int32
   return (uint32_t)type_slot[(type_id >= 0 && type_id < n_type_ids) ? type_id : 0] & 0x7fffu;
 }
 MMP_HD uint32_t slot_key(const SnapshotView &s, int32_t type_id) { return slot_key_of(s.type_slot, s.n_type_ids, type_id); }
+// whether rank r is a member of the mask row m (one slot's row_words words)
+MMP_HD bool mask_bit(const uint32_t *m, int32_t r) { return (m[(uint32_t)r >> 5] >> (r & 31)) & 1u; }
 // a model's SplitKey from its snapshot row and the epoch ranks of its inline edges (-1: none, or not live), overflow bit
-// clear (k_build_bitmap; k_build_bitmap_ovf sets it)
-MMP_HD SplitKey make_split_key(const mmp_model_row &mr, const int32_t rs[4], const uint16_t *type_slot, int32_t n_type_ids) {
+// clear (k_build_bitmap; k_build_bitmap_ovf sets it).  cand: the snapshot's cand masks ([n_slots][row_words]); given, only
+// the ranks in the model's slot count and the key is marked SPLIT_KEY_ALL_EDGES (k_build_bitmap_ovf folds the overflow
+// edges in); null, every inline rank counts.
+MMP_HD SplitKey make_split_key(const mmp_model_row &mr, const int32_t rs[4], const uint16_t *type_slot, int32_t n_type_ids,
+                               const uint32_t *cand = nullptr, int32_t row_words = 0) {
   SplitKey k;
   k.last_used = mr.last_used;
   k.min_rank = INT32_MAX;
-  for (int j = 0; j < 4; j++) if (rs[j] >= 0 && rs[j] < k.min_rank) k.min_rank = rs[j];
   k.slot = slot_key_of(type_slot, n_type_ids, mr.type_id);
+  const uint32_t *cm = cand ? cand + (size_t)k.slot * (size_t)row_words : nullptr;
+  for (int j = 0; j < 4; j++)
+    if (rs[j] >= 0 && rs[j] < k.min_rank && (!cm || mask_bit(cm, rs[j]))) k.min_rank = rs[j];
+  if (cand) k.slot |= SPLIT_KEY_ALL_EDGES;
   return k;
 }
 MMP_HD SplitKey load_split_key(const SplitKey *p) {  // read once per decision: kept out of L1 like the decision record
@@ -1759,19 +1769,21 @@ MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, b
   slot_summary<TabGlob>(s, T, T, slot, active, cs, ewin, win_words, now, vote, chunk, sum, members);
 }
 
-// The fast answer of k_place_split: a valid, unflagged decision without extra excludes whose model has no overflow ids
-// and whose exclusions and self all lie at or past its slot's reach for its c_self.  ok: decision_ok of d; self_rank:
-// rank_of[d.self]; k: its model's SplitKey (read only when ok and not a request-model decision).  Returns false, with
-// nothing written, for every other decision.
+// The fast answer of k_place_split: a valid, unflagged decision without extra excludes whose key covers all of its
+// model's exclusions (no overflow ids, or SPLIT_KEY_ALL_EDGES), and whose candidate exclusions and self, when self is a
+// candidate, all lie at or past its slot's reach for its c_self (DESIGN.md §5.2.1).  ok: decision_ok of d; self_rank:
+// rank_of[d.self]; k: its model's SplitKey (read only when ok and not a request-model decision); self_cand: whether self's
+// bit is set in its slot's mask of the call's view (true for a caller that does not know).  Returns false, with nothing
+// written, for every other decision.
 MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, int32_t ok, int32_t self_rank, const SplitKey &k,
                          const FreshRow *fresh, int32_t n_fresh, const SlotSummary *sums, const int32_t *members, int64_t now,
-                         uint64_t seed, uint64_t decision_id, mmp_decision_out &out) {
-  if (!ok || request_model(d) || d.extra_n != 0 || (k.slot & SPLIT_KEY_OVF)) return false;
+                         uint64_t seed, uint64_t decision_id, mmp_decision_out &out, bool self_cand = true) {
+  if (!ok || request_model(d) || d.extra_n != 0 || (k.slot & (SPLIT_KEY_OVF | SPLIT_KEY_ALL_EDGES)) == SPLIT_KEY_OVF) return false;
   FreshRow fr;  // (as prepare_ctx_b)
   if (d.fresh >= 0 && d.fresh < n_fresh) fr = fresh[d.fresh];
   else if (self_rank >= 0) { const RankRow sr = load_row(s.rows + self_rank); fr.lru = sr.lru; fr.rem = sr.rem; fr.count = sr.count; fr.rpm = 0; }
   else return false;
-  const int slot = (int)k.slot;
+  const int slot = (int)(k.slot & SPLIT_KEY_SLOT);
   const SlotSummary &sm = sums[slot];
   int cs;
   if (sm.best_full) {  // (decide_stream's c_self)
@@ -1779,7 +1791,7 @@ MMP_HD bool split_answer(const SnapshotView &s, const mmp_decision_in &d, int32_
     cs = df > 45000 && df > a10;
   } else cs = fr.rem < s.min_space || fr.rem < (sm.best_rem >> 2);
   const int32_t reach = sm.reach[cs];
-  if (reach < 0 || (self_rank >= 0 && self_rank < reach) || k.min_rank < reach) return false;
+  if (reach < 0 || (self_cand && self_rank >= 0 && self_rank < reach) || k.min_rank < reach) return false;
   const int32_t n_in = sm.n_in[cs];
   const int64_t last_used = (d.flags & MMP_DF_MODEL_LAST_USED) ? k.last_used : d.last_used;
   const PickOut pk = pick_survivor(n_in, false, sm.best_rpm, fr.rpm, sm.best_rpm, last_used, now, seed, decision_id);
