@@ -240,6 +240,11 @@ int32_t mmp_place_one(mmp_fleet *, const mmp_decision_in *in, const mmp_instance
  * CUDA-event duration of the scoring kernel on its launch stream. */
 int32_t mmp_place_batch_device(mmp_fleet *, const void *d_in, int32_t n, void *d_out, int64_t now_ms, uint64_t seed,
                                float *kernel_ms);
+/* The per-slot summaries of the two-pass placement path (k_slot_summary, DESIGN.md §5.2) on the committed snapshot at
+ * now_ms, read back for tests: sums receives up to cap 48-byte records {int64 best_rem, best_lru; int32 best_idx, best_rpm,
+ * best_full, reach[2], n_in[2], pad}, members [cap][2][256] shortlist members (instance indices; entries past n_in[c_self]
+ * are undefined).  Whole-row (unsharded) fleets only.  Returns the number of type slots. */
+int32_t mmp_slot_summaries(mmp_fleet *, int64_t now_ms, void *sums, int32_t *members, int32_t cap);
 int32_t mmp_device_alloc(mmp_fleet *, int64_t bytes, void **out);
 int32_t mmp_device_free(mmp_fleet *, void *p);
 int32_t mmp_device_upload(mmp_fleet *, void *dst, const void *src, int64_t bytes);

@@ -90,6 +90,7 @@ final class MmPlace {
     static native ByteBuffer allocPinned(long h, long bytes);
     static native int freePinned(long h, ByteBuffer buf);
     static native int flushL2(long h);
+    static native int slotSummaries(long h, long nowMs, ByteBuffer sums, ByteBuffer members, int cap);
     // instance-sharded fleets
     static native int shardUniqueId(byte[] out128);
     static native int shardConnect(long h, byte[] id128);

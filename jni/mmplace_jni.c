@@ -324,6 +324,11 @@ jobject FN(allocPinned)(JNIEnv *env, jclass c, jlong h, jlong bytes) {
 }
 jint FN(freePinned)(JNIEnv *env, jclass c, jlong h, jobject buf) { (void)c; return mmp_host_free(H(h), BUF(buf)); }
 jint FN(flushL2)(JNIEnv *env, jclass c, jlong h) { (void)env; (void)c; return mmp_flush_l2(H(h)); }
+/* the two-pass path's per-slot summaries, read back (tests) */
+jint FN(slotSummaries)(JNIEnv *env, jclass c, jlong h, jlong nowMs, jobject sums, jobject members, jint cap) {
+  (void)c;
+  return mmp_slot_summaries(H(h), nowMs, BUF(sums), (int32_t *)BUF(members), cap);
+}
 
 /* ---- instance-sharded fleets ---- */
 jint FN(shardUniqueId)(JNIEnv *env, jclass c, jbyteArray out) {

@@ -191,6 +191,7 @@ SYMBOLS = [
     ("mmp_place_one", _I32, [_P, _P, _P, _P, _P, _I64, _U64]),
     ("mmp_place_sweep", _I32, [_P, _I32, _I32, _P, _I32, _P, _P, _I64, _U64]),
     ("mmp_place_batch_device", _I32, [_P, _P, _I32, _P, _I64, _U64, C.POINTER(C.c_float)]),
+    ("mmp_slot_summaries", _I32, [_P, _I64, _P, _P, _I32]),
     ("mmp_device_alloc", _I32, [_P, _I64, C.POINTER(_P)]),
     ("mmp_device_free", _I32, [_P, _P]),
     ("mmp_device_upload", _I32, [_P, _P, _P, _I64]),

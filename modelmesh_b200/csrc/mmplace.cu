@@ -421,7 +421,7 @@ static constexpr int LANE_SLOTS = 64;    // type-constraint mask slots whose win
 static constexpr int LANE_WARPS = 12;    // warps per block of k_place_lanes
 static constexpr int LANE_STAGES = 4;    // landing stages per SM at most: a fifth takes the shared-memory carve-out from 196 to
                                          // 228 KB and leaves too little L1 for the lane tables to stay resident
-// The window part of the lane tables in shared memory (k_place_lanes, k_place_server, k_slot_summary): the masks of the
+// The window part of the lane tables in shared memory (k_place_lanes, k_place_server): the masks of the
 // first LANE_SLOTS slots and full / csum / count_col / rows over the first LANE_WIN words of this process's rows, zero past
 // their end.
 struct WinTabs {
@@ -431,8 +431,7 @@ struct WinTabs {
   __align__(16) RankRow rows[LANE_WIN * 32];
   // thread tid of nthreads copies its share of the tables (the caller synchronises).  N: the type of the stride, blockDim.x
   // or a constant int, as each kernel steps its loops (it decides how far the compiler unrolls them).  Every element is
-  // one cp.async and the thread waits once at the end: its share costs one round trip to memory, not one per element
-  // (k_slot_summary waits for the copy with every other SM idle).
+  // one cp.async and the thread waits once at the end: its share costs one round trip to memory, not one per element.
   template <class N>
   __device__ __forceinline__ void fill(const SnapshotView &s, int tid, N nthreads) {
     const int WS = s.word_lo;
@@ -768,27 +767,15 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
 }
 
 // ---- the two-pass path of a large batch (launch_place, DESIGN.md §5.2) ----
-// one lane per (type slot, c_self): the slot summaries of this call's view (slot_summary); also zeroes the worklist counters
-// and k_place_tail's work counter.  The walks and the member listing read the window part of the tables from shared memory
-// (a block copies it in one parallel pass): each of their steps waits on the one before, and from global memory each would
-// be a round trip to L2 or DRAM.  Every lane's exclusion window is the same all-zero one.
-__global__ void __launch_bounds__(128) k_slot_summary(const SnapshotView s, int64_t now, SlotSummary *__restrict__ sums,
-                                                      int32_t *__restrict__ members, int32_t *__restrict__ counts) {
-  __shared__ WinTabs tabs;
-  __shared__ uint32_t zwin[LANE_WIN];
-  __shared__ uint32_t chunk_s[4][32 * MMP_CHUNK_WORDS];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int t = blockIdx.x * 128 + threadIdx.x, sl = t >> 1, cs = t & 1;
-  if (t < 3) counts[t] = 0;
-  if (threadIdx.x < LANE_WIN) zwin[threadIdx.x] = 0u;
-  tabs.fill(s, threadIdx.x, 128);
-  __syncthreads();
-  const bool active = sl < s.n_slots;
-  const int slot = active ? sl : 0;
-  const uint32_t win_words = (uint32_t)min(LANE_WIN, s.word_hi - s.word_lo);
-  const LaneTables T = lane_tables_global(s, slot);
-  slot_summary<TabWin>(s, tabs.view(T, slot, s.word_lo), T, slot, active, cs, zwin, win_words, now, WarpVote(),
-                       chunk_s[warp] + lane * MMP_CHUNK_WORDS, sums[slot], members + ((size_t)slot * 2 + cs) * SPLIT_CAP);
+// one warp per (type slot, c_self), SUMMARY_WARPS to a block: the slot summaries of this call's view (slot_summary on
+// the cooperative shape, 32 row words per step); also zeroes the worklist counters and k_place_tail's work counter
+static constexpr int SUMMARY_WARPS = 4;
+__global__ void __launch_bounds__(SUMMARY_WARPS * 32) k_slot_summary(const SnapshotView s, int64_t now, SlotSummary *__restrict__ sums,
+                                                                     int32_t *__restrict__ members, int32_t *__restrict__ counts) {
+  const int t = blockIdx.x * SUMMARY_WARPS + (threadIdx.x >> 5), sl = t >> 1, cs = t & 1;
+  if (blockIdx.x == 0 && threadIdx.x < 3) counts[threadIdx.x] = 0;
+  if (sl >= s.n_slots) return;
+  slot_summary(s, sl, cs, now, Coop32(), sums[sl], members + ((size_t)sl * 2 + cs) * SPLIT_CAP);
 }
 // appends v to list (length in *count) for the lanes where p holds: one atomic per warp
 __device__ __forceinline__ void warp_append(bool p, int32_t v, int32_t *list, int32_t *count) {
@@ -1417,8 +1404,8 @@ struct mmp_fleet {
                                 // resolves a large batch in type-slot order
   PlaceKernel kernel = PlaceKernel::direct;  // MMP_KERNEL, mmp_tune("direct"): which kernel resolves untraced unsharded batches
   int lane_budget = LANE_BUDGET;  // MMP_LANE_BUDGET: walk steps per lane before a decision is handed to the whole warp
-  int split = 2;                // mmp_tune("split"): 0 never | 1 always | 2 (default) from SPLIT_MIN_BATCH decisions on snapshots whose
-                                // candidate sets are not sparse: k_place_direct batches go through the two-pass path (launch_split)
+  int split = 2;                // mmp_tune("split"): 0 never | 1 always | 2 (default) from SPLIT_MIN_BATCH decisions: k_place_direct
+                                // batches go through the two-pass path (launch_split)
   // LRU store (plug point 3)
   DevBuf lru_ts, lru_seq, lru_weight, lru_model, lru_cap, lru_wsize, lru_count, lru_seqctr, lru_loadts, lru_pin;
   int32_t lru_n = 0, lru_slots = 0;
@@ -1600,7 +1587,7 @@ static cudaError_t launch_split(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
       (e = c->d_counts[ss].ensure(16)) != cudaSuccess) return e;
   if (sorted && (e = slot_key_buffers(a)) != cudaSuccess) return e;
   int32_t *counts = c->d_counts[ss].as<int32_t>();
-  k_slot_summary<<<(2 * n_slots + 127) / 128, 128, 0, st>>>(a.s, a.now, c->d_sums[ss].as<SlotSummary>(), c->d_members[ss].as<int32_t>(), counts);
+  k_slot_summary<<<(2 * n_slots + SUMMARY_WARPS - 1) / SUMMARY_WARPS, SUMMARY_WARPS * 32, 0, st>>>(a.s, a.now, c->d_sums[ss].as<SlotSummary>(), c->d_members[ss].as<int32_t>(), counts);
   k_place_split<<<(a.n + 255) / 256, 256, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.out, a.now, a.seed, a.id_base,
                                                    c->d_sums[ss].as<SlotSummary>(), c->d_members[ss].as<int32_t>(), c->d_walk[ss].as<int32_t>(),
                                                    c->d_ovf[ss].as<int32_t>(), counts, sorted ? c->d_skey[ss].as<uint16_t>() : nullptr,
@@ -1626,7 +1613,7 @@ static cudaError_t launch_place(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
   if (a.emit_keys || a.orig_id) return lanes_geometry(a.s.excl_stride, ns) ? launch_place_lanes(f, a, st, ns) : cudaErrorInvalidValue;
   // the direct kernel: rows rebuilt from the snapshot's excl_ranks (whole-row fleets), no landing stages
   if (f->kernel == PlaceKernel::direct && a.s.word_lo == 0 && a.s.word_hi == a.s.row_words && a.s.excl_ranks) {
-    if (a.ctx && a.s.n_slots > 0 && (f->split == 1 || (f->split == 2 && a.n >= SPLIT_MIN_BATCH && !f->snaps[f->cur].sparse_slots)))
+    if (a.ctx && a.s.n_slots > 0 && (f->split == 1 || (f->split == 2 && a.n >= SPLIT_MIN_BATCH)))
       return launch_split(f, a, st);
     const int32_t *perm = nullptr;  // k_place_direct: position j of the launch resolves decision perm[j]
     if (a.ctx && a.n >= 8192 && sorts_slots(f)) {
@@ -2815,6 +2802,35 @@ int32_t mmp_place_batch_device(mmp_fleet *f, const void *d_in, int32_t n, void *
   CK(cudaEventSynchronize(c->e1));
   if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, c->e0, c->e1));
   return MMP_OK;
+}
+
+int32_t mmp_slot_summaries(mmp_fleet *f, int64_t now_ms, void *sums, int32_t *members, int32_t cap) {
+  NEED(f);
+  if (cap < 0 || (cap > 0 && (!sums || !members))) { g_err = "bad argument"; return MMP_E_ARG; }
+  int32_t rc = set_device(f);
+  if (rc < 0) return rc;
+  std::shared_lock<std::shared_mutex> rd(f->snap_mu);
+  if (f->epoch == 0) { g_err = "no committed snapshot"; return MMP_E_EPOCH; }
+  const SnapshotView &v = f->snaps[f->cur].view;
+  if (v.word_lo != 0 || v.word_hi != v.row_words || !v.zero_row) { g_err = "slot summaries need a whole-row fleet"; return MMP_E_ARG; }
+  if (v.n_slots <= 0) return 0;
+  CtxLease c(f);
+  if (!c) { g_err = "cannot create CUDA stream"; return MMP_E_CUDA; }
+  cudaStream_t st = c->stream;
+  CK(c->d_sums[0].ensure((size_t)v.n_slots * sizeof(SlotSummary)));
+  CK(c->d_members[0].ensure((size_t)v.n_slots * 2 * SPLIT_CAP * 4));
+  CK(c->d_counts[0].ensure(16));
+  k_slot_summary<<<(2 * v.n_slots + SUMMARY_WARPS - 1) / SUMMARY_WARPS, SUMMARY_WARPS * 32, 0, st>>>(
+      v, now_ms, c->d_sums[0].as<SlotSummary>(), c->d_members[0].as<int32_t>(), c->d_counts[0].as<int32_t>());
+  f->launches++;
+  CK(cudaGetLastError());
+  const size_t n = (size_t)std::min(cap, v.n_slots);
+  if (n) {
+    CK(cudaMemcpyAsync(sums, c->d_sums[0].p, n * sizeof(SlotSummary), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(members, c->d_members[0].p, n * 2 * SPLIT_CAP * 4, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  return v.n_slots;
 }
 
 int32_t mmp_device_alloc(mmp_fleet *f, int64_t bytes, void **out) {

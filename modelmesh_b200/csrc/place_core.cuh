@@ -19,6 +19,9 @@
 // in the filtered set?") are answered in O(1) from the staged row.  No per-lane copy of the row is kept in registers.
 #pragma once
 #include <stdint.h>
+#if !defined(__CUDACC__)
+#include <vector>
+#endif
 
 #include "../../include/mmplace.h"
 
@@ -462,8 +465,8 @@ struct DecideOut {
   int32_t target, n_candidates;
   int32_t best, n_remaining, pick_index, flags, cut_rank, best_rank;
   int32_t first_rank;  // rank of the first filtered entry (before preferred handling): the min-loc key of a shard
-  // decide_stream: every rank its answer depends on lies below reach (NONE_RANK: any rank may), so an exclusion or a self
-  // at or beyond it leaves the answer as it is (k_slot_summary)
+  // decide_stream, decide_ctx: every rank its answer depends on lies below reach (NONE_RANK: any rank may), so an
+  // exclusion or a self at or beyond it leaves the answer as it is (k_slot_summary)
   int32_t reach;
 };
 
@@ -886,7 +889,7 @@ MMP_HD WordSumI ldro_sum(const WordSumI *p) {
 
 // how the lane routine reads its tables: beyond the window through the read-only path from the snapshot's own arrays
 // (TabGlob); inside the window through plain loads (TabWin) where the caller points them at shared-memory copies of the
-// tables' window part (k_place_lanes, k_place_server, k_slot_summary), or through TabGlob too where its window tables are
+// tables' window part (k_place_lanes, k_place_server), or through TabGlob too where its window tables are
 // the global ones
 struct TabWin {
   const LaneTables &t;
@@ -1428,7 +1431,7 @@ template <class C>
 MMP_HD void decide_ctx(const SnapshotView &s, const DecisionCtx &c, const uint32_t *erow, const int32_t *extra, int64_t now,
                        uint64_t seed, uint64_t decision_id, const C &co, DecideOut &o, uint32_t *cand_rows) {
   o.target = MMP_TARGET_NONE; o.n_candidates = 0; o.best = -1; o.n_remaining = 0; o.pick_index = 0; o.flags = 0;
-  o.cut_rank = (int32_t)NONE_RANK; o.best_rank = -1; o.first_rank = -1;
+  o.cut_rank = (int32_t)NONE_RANK; o.best_rank = -1; o.first_rank = -1; o.reach = (int32_t)NONE_RANK;
   const uint32_t NW = (uint32_t)s.row_words;
   // this process's part of the row: words [WS, WE); erow[0] is row word WS.  Not sharded: [0, NW).
   const uint32_t WS = (uint32_t)s.word_lo, WE = (uint32_t)s.word_hi;
@@ -1492,6 +1495,8 @@ MMP_HD void decide_ctx(const SnapshotView &s, const DecisionCtx &c, const uint32
   uint32_t lo = b, hi = NONE_RANK;
   bool use_pref = has_pref && simple;  // best is preferred: preference is treated as required (MM:4905-4907)
   o.best = best_idx; o.best_rank = (int32_t)b; o.first_rank = (int32_t)b;
+  // the highest rank the answer rests on (o.reach, as decide_stream's): a phase that finds nothing adds nothing
+  uint32_t dep = b;
 #define MMP_OPEN_EXIT do { o.flags |= MMP_TF_OPEN; o.target = MMP_TARGET_NONE; o.n_candidates = 0; return; } while (0)
 
   if (!simple) {
@@ -1513,6 +1518,7 @@ MMP_HD void decide_ctx(const SnapshotView &s, const DecisionCtx &c, const uint32
       }
       MMP_BAIL_CHECK;
       if (open_end && p1 == NONE_RANK && f1 == NONE_RANK) MMP_OPEN_EXIT;  // the deciding entry is in a later shard
+      if (p1 != NONE_RANK || f1 != NONE_RANK) dep = p1 < f1 ? p1 : f1;
       if (p1 < f1) {
         const RankRow rp = s.rows[p1];
         best_rank = p1; best_idx = rp.idx; best_rem = rp.rem; best_lru = rp.lru; best_count = rp.count; best_rpm = rp.rpm;
@@ -1585,6 +1591,7 @@ MMP_HD void decide_ctx(const SnapshotView &s, const DecisionCtx &c, const uint32
         return;
       }
       hi = kb; simple = true;  // no preferred in range: rewind, "no preference" logic over the replayed prefix
+      if (kb != NONE_RANK) dep = kb;
     }
   }
   // ---- simple case MM:4889-4938 ----
@@ -1632,6 +1639,9 @@ MMP_HD void decide_ctx(const SnapshotView &s, const DecisionCtx &c, const uint32
   const uint32_t cut = cut_others < cut_self ? cut_others : cut_self;
   o.cut_rank = (int32_t)cut;
   if (open_end && cut == NONE_RANK && hi == NONE_RANK) MMP_OPEN_EXIT;  // the shortlist runs on into the next shard
+  // no cut: every member of S counted, the answer rests on the end of S (hi; none: the row's end)
+  if (cut != NONE_RANK ? cut > dep : (hi == NONE_RANK || hi > dep)) dep = cut != NONE_RANK ? cut : hi;
+  o.reach = (int32_t)(dep == NONE_RANK ? NONE_RANK : dep + 1u);
   const bool self_in_sl = self_in_s && (uint32_t)self_rank < cut;
   if (favour_self && self_in_sl) { o.flags |= MMP_TF_FAVOUR_EXIT; o.target = MMP_TARGET_SELF; return; }
   const uint32_t endc = cut == NONE_RANK ? end : (end_for(cut) < end ? end_for(cut) : end);
@@ -1694,80 +1704,86 @@ struct SlotSummary {
 };
 
 // The summary of type slot `slot` for c_self = cs, and its shortlist members (instance indices, rank order) into
-// members[0, SPLIT_CAP): decide_stream on a decision without exclusions, with a self that is not live and a record
-// that makes c_self come out as cs.  Called by every lane of the vote group (active = false for lanes without a slot);
-// ewin: win_words zero words.  Tw, AWT: the window's tables and how they are read, as for decide_stream; every rank or
-// word read after the walks comes from them inside the window and from T beyond it.
-template <class AWT = TabWin, class V>
-MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &Tw, const LaneTables &T, int slot, bool active, int cs,
-                         const uint32_t *ewin, uint32_t win_words, int64_t now, const V &vote, uint32_t *chunk, SlotSummary &sum,
-                         int32_t *members) {
+// members[0, SPLIT_CAP): decide_ctx on the snapshot's zero row, for a decision without exclusions, with a self that is
+// not live and a record that makes c_self come out as cs.  Every lane of the shape calls it; lane 0 writes sum.
+template <class C>
+MMP_HD void slot_summary(const SnapshotView &s, int slot, int cs, int64_t now, const C &co, SlotSummary &sum, int32_t *members) {
   DecisionCtx c;
   c.d.model = 0; c.d.self = -1; c.d.last_used = 0; c.d.flags = 0; c.d.fresh = -1; c.d.extra_off = 0; c.d.extra_n = 0;
   c.last_used = 0; c.self_rank = -1; c.self_bits = 0; c.self_count = 0;
   c.xr[0] = c.xr[1] = c.xr[2] = c.xr[3] = -1;
-  c.slot = active ? (slot | ((s.has_pref[slot] ? 1 : 0) << 16)) : -1;
+  c.slot = slot | ((s.has_pref[slot] ? 1 : 0) << 16);
   // c_self against a best with room tests remaining: this record makes it come out as cs
   c.fr.lru = 0; c.fr.rem = cs ? INT64_MIN : INT64_MAX; c.fr.count = 0; c.fr.rpm = 0;
-  RowRanks none;
-  none.r[0] = none.r[1] = none.r[2] = none.r[3] = -1;
-  // first pass: the best (phases A, A', A'' do not read the caller's record of a self that is not live), and the
-  // shortlist when the best has room
+  const uint32_t *zero = excl_row(s, ZERO_ROW);
+  // what pick_survivor cannot answer (the preferred candidates of non-simple (b)) or what a decision's own filter would
+  // change (the replicaset retry) is walked
+  const int32_t declined = MMP_TF_OPEN | MMP_TF_FAVOUR_EXIT | MMP_TF_RS_RETRY | MMP_TF_PREF_B;
+  // first pass: the best (the phases before the shortlist do not read the caller's record of a self that is not live),
+  // and the shortlist when the best has room
   DecideOut o;
-  bool ok = decide_stream<AWT>(s, Tw, T, c, active, ewin, win_words, none, 0u, now, 0, 0, vote, o, 0x3fffffff, chunk) && active &&
-            o.best_rank >= 0 && !(o.flags & MMP_TF_OPEN);
-  const AWT AW{Tw};
-  const TabGlob AG{T};
-  const TabEither<AWT> AE{AW, AG, (uint32_t)s.word_lo + win_words};
+  decide_ctx(s, c, zero, nullptr, now, 0, 0, co, o, nullptr);
+  bool ok = o.best_rank >= 0 && !(o.flags & declined);
   RankRow r0, rb;
   r0.lru = r0.rem = 0; r0.rpm = 0; rb = r0; rb.idx = -1;
   bool full = false;
   if (ok) {
-    r0 = AE.row((uint32_t)o.first_rank);
-    rb = AE.row((uint32_t)o.best_rank);
-    full = r0.rem < s.min_space;  // (a full first entry is never replaced as best: A' runs for a best with room only)
+    r0 = load_row(s.rows + o.first_rank);
+    rb = load_row(s.rows + o.best_rank);
+    full = r0.rem < s.min_space;  // (a full first entry is never replaced as best: non-simple (a) runs for a best with room only)
     if (full) {
       const int64_t a10 = age_of(r0.lru, now) / 10;
       c.fr.lru = cs ? (int64_t)((uint64_t)r0.lru + (uint64_t)((a10 > 45000 ? a10 : 45000) + 1)) : r0.lru;
     }
   }
   // second pass, for a full best: c_self tests lruTime against the best's, which the record now forces to come out as cs
-  // (skipped by the whole vote group when none of its lanes has a full best: with every lane idle it still takes ~0.9 µs
-  // on an H100)
-  const bool again = ok && full;
-  DecideOut ox;
-  bool ok2 = false;
-  if (vote.any(again)) ok2 = decide_stream<AWT>(s, Tw, T, c, again, ewin, win_words, none, 0u, now, 0, 0, vote, ox, 0x3fffffff, chunk);
-  const DecideOut &o2 = again ? ox : o;
-  ok = ok && (!again || ok2) && o2.best_rank == o.best_rank && !(o2.flags & (MMP_TF_OPEN | MMP_TF_FAVOUR_EXIT)) && o2.n_candidates >= 1 &&
-       o2.n_candidates - 1 <= SPLIT_CAP;
+  DecideOut o2 = o;
+  if (ok && full) decide_ctx(s, c, zero, nullptr, now, 0, 0, co, o2, nullptr);
+  ok = ok && o2.best_rank == o.best_rank && !(o2.flags & declined) && o2.n_candidates >= 1 && o2.n_candidates - 1 <= SPLIT_CAP;
   const int32_t n_in = ok ? o2.n_candidates - 1 : 0;
-  if (ok) {  // the members: S' strictly between best and the cut (no cut: the end of S, one below the reach)
+  if (ok) {  // the members: S strictly between best and the cut (no cut: the end of S, one below the reach)
+    const uint32_t NW = (uint32_t)s.row_words;
+    const uint32_t *CX = (s.any_rs ? s.candx : s.cand) + (size_t)slot * NW, *P = s.pref + (size_t)slot * NW;
     const uint32_t lo = (uint32_t)o2.best_rank;
     const uint32_t lim = o2.cut_rank != (int32_t)NONE_RANK ? (uint32_t)o2.cut_rank : (o2.reach == (int32_t)NONE_RANK ? NONE_RANK : (uint32_t)o2.reach - 1u);
-    const bool use_pref = (c.slot >> 16) && ((AE.p(lo >> 5) >> (lo & 31)) & 1u);
-    int32_t k = 0;
-    for (uint32_t w = lo >> 5; w < (uint32_t)s.row_words && w * 32u < lim && k <= n_in; w++) {
-      uint32_t x = AE.cx(w) & (use_pref ? AE.p(w) : 0xffffffffu) & mask_above(w * 32u, lo) & mask_below(w * 32u, lim);
-      for (; x; x &= x - 1u) {
-        if (k < SPLIT_CAP) members[k] = AE.idx(w * 32u + (uint32_t)ffs32(x));
-        k++;
+    const bool use_pref = (c.slot >> 16) && ((P[lo >> 5] >> (lo & 31)) & 1u);
+    const uint32_t end = lim == NONE_RANK ? NW : ((lim + 31u) >> 5 < NW ? (lim + 31u) >> 5 : NW);
+    // a window at a time: each lane lists its word's members from the exclusive prefix of the window's counts
+    uint32_t k = 0;
+    for (uint32_t wb = lo >> 5; wb < end && k <= (uint32_t)n_in; wb += C::L) {
+      const uint32_t wi = wb + co.lane();
+      uint32_t x = 0;
+      if (wi < end) {
+        x = CX[wi] & mask_above(wi * 32u, lo) & mask_below(wi * 32u, lim);
+        if (use_pref) x &= P[wi];
       }
+      const uint32_t cnt = (uint32_t)popc32(x);
+      uint32_t j = k + co.exscan(cnt);
+      for (; x; x &= x - 1u, j++)
+        if (j < (uint32_t)SPLIT_CAP) members[j] = ldro(&s.rows[wi * 32u + (uint32_t)ffs32(x)].idx);
+      k += co.rsum(cnt);
     }
-    ok = k == n_in;
+    ok = k == (uint32_t)n_in;
   }
-  if (!active) return;
+  if (co.lane() != 0) return;
   if (cs == 0) { sum.best_rem = rb.rem; sum.best_lru = r0.lru; sum.best_idx = rb.idx; sum.best_rpm = rb.rpm; sum.best_full = full ? 1 : 0; sum.pad_ = 0; }
   sum.reach[cs] = ok ? o2.reach : -1;
   sum.n_in[cs] = n_in;
 }
 
-// The same summary for a caller whose window tables are the global ones (the CPU harness)
+#if !defined(__CUDACC__)
+// The same summary in the CPU harness's calling convention (the lane routine's: its tables, window and vote are not
+// read; a view without a zero row is given one)
 template <class V>
-MMP_HD void slot_summary(const SnapshotView &s, const LaneTables &T, int slot, bool active, int cs, const uint32_t *ewin,
-                         uint32_t win_words, int64_t now, const V &vote, uint32_t *chunk, SlotSummary &sum, int32_t *members) {
-  slot_summary<TabGlob>(s, T, T, slot, active, cs, ewin, win_words, now, vote, chunk, sum, members);
+inline void slot_summary(const SnapshotView &s, const LaneTables &, int slot, bool active, int cs, const uint32_t *, uint32_t,
+                         int64_t now, const V &, uint32_t *, SlotSummary &sum, int32_t *members) {
+  if (!active) return;
+  SnapshotView v = s;
+  std::vector<uint32_t> zero;
+  if (!v.zero_row) { zero.assign((size_t)(v.excl_stride > 0 ? v.excl_stride : v.row_words), 0u); v.zero_row = zero.data(); }
+  slot_summary(v, slot, cs, now, Coop1(), sum, members);
 }
+#endif
 
 // The fast answer of k_place_split: a valid, unflagged decision without extra excludes whose key covers all of its
 // model's exclusions (no overflow ids, or SPLIT_KEY_ALL_EDGES), and whose candidate exclusions and self, when self is a
