@@ -770,32 +770,56 @@ __global__ void __launch_bounds__(WARPS * 32, MINB) k_place_direct(const Snapsho
 // one warp per (type slot, c_self), SUMMARY_WARPS to a block: the slot summaries of this call's view (slot_summary on
 // the cooperative shape, 32 row words per step); also zeroes the worklist counters and k_place_tail's work counter
 static constexpr int SUMMARY_WARPS = 4;
+// The worklists of k_place_split: block b appends to sub-list b % SPLIT_LISTS of each list, with one atomic per block on
+// that sub-list's counter, so the blocks of a wave do not all queue on one address.  counts[] holds, 32 words (one
+// 128-byte line) apart, the walk sub-lists' lengths, then the overflow sub-lists' lengths, then k_place_tail's work
+// counter.  Sub-list r holds at most the decisions of its blocks: split_list_cap entries, from r * split_list_cap.
+static constexpr int SPLIT_LISTS = 32;  // (at most 32: k_place_tail scans the lengths with one lane per sub-list)
+static constexpr int SPLIT_COUNT_STRIDE = 32;
+static constexpr int SPLIT_COUNTERS = 2 * SPLIT_LISTS + 1;
+static constexpr size_t SPLIT_COUNTS_BYTES = (size_t)SPLIT_COUNTERS * SPLIT_COUNT_STRIDE * 4;
+static_assert(SPLIT_LISTS <= 32 && SPLIT_COUNTERS <= SUMMARY_WARPS * 32, "one lane per sub-list, one thread per counter");
+__host__ __device__ inline int split_list_cap(int n) { return (n + 256 * SPLIT_LISTS - 1) / (256 * SPLIT_LISTS) * 256; }
 __global__ void __launch_bounds__(SUMMARY_WARPS * 32) k_slot_summary(const SnapshotView s, int64_t now, SlotSummary *__restrict__ sums,
                                                                      int32_t *__restrict__ members, int32_t *__restrict__ counts) {
   const int t = blockIdx.x * SUMMARY_WARPS + (threadIdx.x >> 5), sl = t >> 1, cs = t & 1;
-  if (blockIdx.x == 0 && threadIdx.x < 3) counts[threadIdx.x] = 0;
+  if (blockIdx.x == 0 && threadIdx.x < SPLIT_COUNTERS) counts[threadIdx.x * SPLIT_COUNT_STRIDE] = 0;
   if (sl >= s.n_slots) return;
   slot_summary(s, sl, cs, now, Coop32(), sums[sl], members + ((size_t)sl * 2 + cs) * SPLIT_CAP);
 }
-// appends v to list (length in *count) for the lanes where p holds: one atomic per warp
-__device__ __forceinline__ void warp_append(bool p, int32_t v, int32_t *list, int32_t *count) {
-  const uint32_t m = __ballot_sync(0xffffffffu, p);
-  if (!m) return;
-  const int lane = threadIdx.x & 31, leader = __ffs((int)m) - 1;
-  int base = 0;
-  if (lane == leader) base = atomicAdd(count, __popc(m));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  if (p) list[base + __popc(m & ((1u << lane) - 1u))] = v;
+// appends v to the walk list for the threads of the block where walk holds, and to the overflow list where ovf does
+// (lists and counts: the block's sub-lists and their counters): one atomic per list per block, positions from the
+// block's exclusive prefix of its warps' ballots.  Every thread of the block calls.
+template <int WARPS>
+__device__ __forceinline__ void block_append(bool walk, bool ovf, int32_t v, int32_t *walk_list, int32_t *ovf_list, int32_t *walk_count,
+                                             int32_t *ovf_count) {
+  __shared__ int32_t n_s[2][WARPS];  // each warp's count; then its first position
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t mw = __ballot_sync(0xffffffffu, walk), mo = __ballot_sync(0xffffffffu, ovf);
+  if (lane == 0) { n_s[0][warp] = __popc(mw); n_s[1][warp] = __popc(mo); }
+  __syncthreads();
+  if (threadIdx.x < 2) {  // thread l: list l
+    int sum = 0;
+#pragma unroll
+    for (int w = 0; w < WARPS; w++) { const int c = n_s[threadIdx.x][w]; n_s[threadIdx.x][w] = sum; sum += c; }
+    const int base = sum ? atomicAdd(threadIdx.x ? ovf_count : walk_count, sum) : 0;
+#pragma unroll
+    for (int w = 0; w < WARPS; w++) n_s[threadIdx.x][w] += base;
+  }
+  __syncthreads();
+  const uint32_t below = (1u << lane) - 1u;
+  if (walk) walk_list[n_s[0][warp] + __popc(mw & below)] = v;
+  if (ovf) ovf_list[n_s[1][warp] + __popc(mo & below)] = v;
 }
 // one thread per decision: answered from its slot's summary (split_answer), or put on a worklist -- a model with overflow
-// ids on ovf_list, everything else on walk_list (k_place_tail takes both).  keys / key_idx (sparse snapshots): the
-// slot-order sort of the batch, the walked decisions' keys below everyone else's.
+// ids on ovf_list, everything else on walk_list (k_place_tail takes both; cap: split_list_cap(n)).  keys / key_idx
+// (sparse snapshots): the slot-order sort of the batch, the walked decisions' keys below everyone else's.
 __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
                                                      const FreshRow *__restrict__ fresh, int n_fresh, mmp_decision_out *__restrict__ out,
                                                      int64_t now, uint64_t seed, uint64_t id_base, const SlotSummary *__restrict__ sums,
                                                      const int32_t *__restrict__ members, int32_t *__restrict__ walk_list,
-                                                     int32_t *__restrict__ ovf_list, int32_t *__restrict__ counts, uint16_t *__restrict__ keys,
-                                                     int32_t *__restrict__ key_idx) {
+                                                     int32_t *__restrict__ ovf_list, int cap, int32_t *__restrict__ counts,
+                                                     uint16_t *__restrict__ keys, int32_t *__restrict__ key_idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const bool valid = i < n;
   mmp_decision_in d = no_decision();
@@ -820,8 +844,9 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
   if (fast) out[i] = r;
   const bool ovf = ok && !req && !fast && (k.slot & SPLIT_KEY_OVF);
   const bool walk = valid && !fast && !ovf;
-  warp_append(walk, i, walk_list, counts);
-  warp_append(ovf, i, ovf_list, counts + 1);
+  const int sub = blockIdx.x % SPLIT_LISTS;
+  block_append<256 / 32>(walk, ovf, i, walk_list + (size_t)sub * cap, ovf_list + (size_t)sub * cap, counts + sub * SPLIT_COUNT_STRIDE,
+                         counts + (SPLIT_LISTS + sub) * SPLIT_COUNT_STRIDE);
   if (keys && valid) {
     uint32_t key = 0xffffu;
     if (walk) key = !ok ? 0xfffeu : req ? slot_key(s, d.model) : k.slot & SPLIT_KEY_SLOT;
@@ -830,30 +855,57 @@ __global__ void __launch_bounds__(256) k_place_split(const SnapshotView s, const
   }
 }
 // The decisions k_place_split could not answer, in one persistent launch (resident blocks of 4 warps): each warp takes
-// work items from counts[2] until none is left.  Items 0 .. ceil(counts[0] / 32) - 1 are tiles of 32 positions of perm
-// (the walk list, or its slot-order sort), resolved by k_place_direct's body; the next counts[1] are the decisions of
-// ovf_list, one each, resolved from the model's bitmap row as the warp redo resolves them.  Walk tiles go first: on C3
-// that measured 20.7 us per call against 22.8 with the overflow decisions first (DESIGN.md §5.2.1).
+// work items from k_place_tail's counter until none is left.  The first items are tiles of 32 positions of the walk
+// sub-lists, sub-list by sub-list (a tile never spans two), or of perm, the slot-order sort of every walked decision,
+// when there is one; each is resolved by k_place_direct's body.  The rest are the decisions of the overflow sub-lists,
+// one each, resolved from the model's bitmap row as the warp redo resolves them.  Walk tiles go first: on C3 that
+// measured 20.7 us per call against 22.8 with the overflow decisions first (DESIGN.md §5.2.1).
 template <int WARPS, int MINB>
-__global__ void __launch_bounds__(WARPS * 32, MINB) k_place_tail(const SnapshotView s, const mmp_decision_in *__restrict__ in, int n,
+__global__ void __launch_bounds__(WARPS * 32, MINB) k_place_tail(const SnapshotView s, const mmp_decision_in *__restrict__ in,
                                                                 const FreshRow *__restrict__ fresh, int n_fresh,
                                                                 const int32_t *__restrict__ extra, mmp_decision_out *__restrict__ out,
                                                                 int64_t now, uint64_t seed, uint64_t id_base, int budget,
-                                                                const int32_t *__restrict__ perm, const int32_t *__restrict__ ovf_list,
-                                                                int32_t *__restrict__ counts) {
+                                                                const int32_t *__restrict__ perm, const int32_t *__restrict__ walk_list,
+                                                                const int32_t *__restrict__ ovf_list, int cap, int32_t *__restrict__ counts) {
   __shared__ DirectSmem<WARPS> sm;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int n_walk = min(n, __ldg(counts)), n_ovf = __ldg(counts + 1);
-  const int walk_items = (n_walk + 31) >> 5;
+  // per sub-list r: its walk length, the inclusive prefix of the walk tiles, its overflow length, the inclusive prefix of
+  // the overflow lengths (warp 0, lane r)
+  __shared__ int32_t lists_s[4][SPLIT_LISTS];
+  if (warp == 0) {
+    int n_w = 0, n_o = 0;
+    if (lane < SPLIT_LISTS) {
+      n_w = __ldg(counts + lane * SPLIT_COUNT_STRIDE);
+      n_o = __ldg(counts + (SPLIT_LISTS + lane) * SPLIT_COUNT_STRIDE);
+    }
+    if (perm) {  // one list of every walked decision
+      n_w = (int)__reduce_add_sync(0xffffffffu, (uint32_t)n_w);
+      if (lane) n_w = 0;
+    }
+    int t_w = (n_w + 31) >> 5, e_o = n_o;
+#pragma unroll
+    for (int o = 1; o < SPLIT_LISTS; o <<= 1) {
+      const int a = __shfl_up_sync(0xffffffffu, t_w, o), b = __shfl_up_sync(0xffffffffu, e_o, o);
+      if (lane >= o) { t_w += a; e_o += b; }
+    }
+    if (lane < SPLIT_LISTS) { lists_s[0][lane] = n_w; lists_s[1][lane] = t_w; lists_s[2][lane] = n_o; lists_s[3][lane] = e_o; }
+  }
+  __syncthreads();
+  const int walk_items = lists_s[1][SPLIT_LISTS - 1], n_ovf = lists_s[3][SPLIT_LISTS - 1];
   for (;;) {
     int item = 0;
-    if (lane == 0) item = atomicAdd(counts + 2, 1);
+    if (lane == 0) item = atomicAdd(counts + 2 * SPLIT_LISTS * SPLIT_COUNT_STRIDE, 1);
     item = __shfl_sync(0xffffffffu, item, 0);
     if (item >= walk_items + n_ovf) break;
     if (item < walk_items) {
-      place_direct<WARPS>(sm, item * 32, s, in, n_walk, fresh, n_fresh, extra, out, now, seed, id_base, budget, perm);
+      const int r = __popc(__ballot_sync(0xffffffffu, lane < SPLIT_LISTS && lists_s[1][lane] <= item));  // the tile's sub-list
+      const int len = lists_s[0][r], t0 = lists_s[1][r] - ((len + 31) >> 5);
+      place_direct<WARPS>(sm, (item - t0) * 32, s, in, len, fresh, n_fresh, extra, out, now, seed, id_base, budget,
+                          perm ? perm : walk_list + (size_t)r * cap);
     } else {
-      const int i = ovf_list[item - walk_items];
+      const int e = item - walk_items;
+      const int r = __popc(__ballot_sync(0xffffffffu, lane < SPLIT_LISTS && lists_s[3][lane] <= e));
+      const int i = ovf_list[(size_t)r * cap + e - (lists_s[3][r] - lists_s[2][r])];
       const mmp_decision_in d = in[i];
       if (lane == 0) prepare_ctx(s, d, fresh, n_fresh, extra, sm.ctx_w[warp]);
       __syncwarp();
@@ -1580,23 +1632,26 @@ static cudaError_t launch_split(mmp_fleet *f, const PlaceArgs &a, cudaStream_t s
   const int ss = sort_set(a);
   const int n_slots = std::max(a.s.n_slots, 1);
   const bool sorted = sorts_slots(f);
+  const int cap = split_list_cap(a.n);
   cudaError_t e;
   if ((e = c->d_sums[ss].ensure((size_t)n_slots * sizeof(SlotSummary))) != cudaSuccess ||
       (e = c->d_members[ss].ensure((size_t)n_slots * 2 * SPLIT_CAP * 4)) != cudaSuccess ||
-      (e = c->d_walk[ss].ensure((size_t)a.n * 4)) != cudaSuccess || (e = c->d_ovf[ss].ensure((size_t)a.n * 4)) != cudaSuccess ||
-      (e = c->d_counts[ss].ensure(16)) != cudaSuccess) return e;
+      (e = c->d_walk[ss].ensure((size_t)SPLIT_LISTS * cap * 4)) != cudaSuccess ||
+      (e = c->d_ovf[ss].ensure((size_t)SPLIT_LISTS * cap * 4)) != cudaSuccess || (e = c->d_counts[ss].ensure(SPLIT_COUNTS_BYTES)) != cudaSuccess)
+    return e;
   if (sorted && (e = slot_key_buffers(a)) != cudaSuccess) return e;
   int32_t *counts = c->d_counts[ss].as<int32_t>();
   k_slot_summary<<<(2 * n_slots + SUMMARY_WARPS - 1) / SUMMARY_WARPS, SUMMARY_WARPS * 32, 0, st>>>(a.s, a.now, c->d_sums[ss].as<SlotSummary>(), c->d_members[ss].as<int32_t>(), counts);
   k_place_split<<<(a.n + 255) / 256, 256, 0, st>>>(a.s, a.in, a.n, a.fresh, a.n_fresh, a.out, a.now, a.seed, a.id_base,
                                                    c->d_sums[ss].as<SlotSummary>(), c->d_members[ss].as<int32_t>(), c->d_walk[ss].as<int32_t>(),
-                                                   c->d_ovf[ss].as<int32_t>(), counts, sorted ? c->d_skey[ss].as<uint16_t>() : nullptr,
+                                                   c->d_ovf[ss].as<int32_t>(), cap, counts, sorted ? c->d_skey[ss].as<uint16_t>() : nullptr,
                                                    sorted ? c->d_sidx[ss].as<int32_t>() : nullptr);
   f->launches += 2;
-  const int32_t *perm = c->d_walk[ss].as<int32_t>();
+  const int32_t *perm = nullptr;
   if (sorted && (e = sort_slot_keys(f, a, st, &perm)) != cudaSuccess) return e;
   k_place_tail<4, 5><<<std::max(1, std::min((a.n + 127) / 128, f->sm_count * 5)), 128, 0, st>>>(
-      a.s, a.in, a.n, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, f->lane_budget, perm, c->d_ovf[ss].as<int32_t>(), counts);
+      a.s, a.in, a.fresh, a.n_fresh, a.extra, a.out, a.now, a.seed, a.id_base, f->lane_budget, perm, c->d_walk[ss].as<int32_t>(),
+      c->d_ovf[ss].as<int32_t>(), cap, counts);
   f->launches++;
   return cudaGetLastError();
 }
@@ -2819,7 +2874,7 @@ int32_t mmp_slot_summaries(mmp_fleet *f, int64_t now_ms, void *sums, int32_t *me
   cudaStream_t st = c->stream;
   CK(c->d_sums[0].ensure((size_t)v.n_slots * sizeof(SlotSummary)));
   CK(c->d_members[0].ensure((size_t)v.n_slots * 2 * SPLIT_CAP * 4));
-  CK(c->d_counts[0].ensure(16));
+  CK(c->d_counts[0].ensure(SPLIT_COUNTS_BYTES));
   k_slot_summary<<<(2 * v.n_slots + SUMMARY_WARPS - 1) / SUMMARY_WARPS, SUMMARY_WARPS * 32, 0, st>>>(
       v, now_ms, c->d_sums[0].as<SlotSummary>(), c->d_members[0].as<int32_t>(), c->d_counts[0].as<int32_t>());
   f->launches++;
